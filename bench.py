@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """bench.py -- MAC reasoning steps/sec on synthetic CLEVR-shaped batches (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--prec bf16|fp32] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--prec bf16|fp32] [--impl ours|reference] [--dump-outputs DIR]
 
 A bench "step" is one full pass of the hot path over one batch: the netLength-step unroll of the MAC cell
 (model.py:447-458) on B=64 questions -- 12 reasoning steps at the headline configuration (BASELINE.json
 configs[2]: B=64, S=40, 14x14 KB, d=512, netLength=12).  `value` = reasoning steps/s = K * netLength * N / t.
 
   value   inputs resident in HBM when the timed region starts; the K timed passes rotate over 8 resident
-          batches (8 x 31 MB > 126 MB L2) so the knowledge base comes from HBM every pass.
+          batches (8 x 31 MB > 50 MB L2) so the knowledge base comes from HBM every pass.
   e2e     the same metric through the public API with HOST (pinned) buffers: per pass the H2D copy of the batch
           (KB, words, question vector, lengths) and the D2H read of the final state + attention maps are inside the
           timed region (double-buffered against compute on a copy stream).
@@ -16,6 +16,7 @@ configs[2]: B=64, S=40, 14x14 KB, d=512, netLength=12).  `value` = reasoning ste
   cpu_baseline   the oracle's fp32 PyTorch-CPU port (oracle/mac_torch_cpu.py) timed on this box's host cores.
 
 `--impl reference` times that CPU port alone (TensorFlow-1 cannot be installed offline; see DESIGN.md).
+`--dump-outputs DIR` writes what the last timed pass computed (final control / memory, both attention maps) as DIR/<name>.npy.
 """
 import argparse
 import json
@@ -77,7 +78,8 @@ def peaks():
         p = json.load(open(path))
         return {"hbm": p["hbm_gbs"], "tensor_burst": p["bf16_tflops"], "tensor_sustained": p["bf16_tflops_sustained"],
                 "src": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm": 6650.0, "tensor_burst": 1590.0, "tensor_sustained": 1400.0, "src": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- bounds, not reached rates
+    return {"hbm": 3350.0, "tensor_burst": 989.0, "tensor_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 def local_device():
@@ -89,7 +91,7 @@ def local_device():
 
 
 class ClockSampler(object):
-    """nvidia-smi sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi sampled DURING the timed region (read-only queries: clocks, power, throttle reasons)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -239,18 +241,17 @@ class Slot(object):
         c = self.cell
         return [c._hc[self.L], c._hm[self.L], c._att_kb, c._att_q]
 
-
-def ncu_traffic(key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))[key]["dram_bytes_per_launch"]
-    except Exception:
-        return None
+    def dump(self, out_dir):
+        """The arrays a caller of the pass receives -- final control and memory, attention over the knowledge base and over
+        the question words -- as <out_dir>/<name>.npy (float32)."""
+        os.makedirs(out_dir, exist_ok=True)
+        for name, t in zip(("control", "memory", "att_kb", "att_q"), self.outputs()):
+            np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def time_kernel(fns, iters=24, flush=None):
     """Average device time (s) per launch.  `fns` is a list of closures launching the SAME kernel on DIFFERENT
-    buffers whose total footprint exceeds the 126 MB L2 (so every launch reads HBM); the launches are issued back
+    buffers whose total footprint exceeds the 50 MB L2 (so every launch reads HBM); the launches are issued back
     to back and bracketed by one pair of CUDA events on the launching stream.  With `flush` given, each launch is
     instead timed alone after a cold-L2 flush (a 256 MB write)."""
     for f in fns:
@@ -282,7 +283,7 @@ def kernel_rooflines(shape, prec, pk):
     B, S, N, d, _ = shape
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")
     out = {}
-    NB = 12        # rotating input sets: 12 x 25.7 MB (fp32) / 12 x 12.8 MB (bf16) > 126 MB L2
+    NB = 12        # rotating input sets: 12 x 25.7 MB (fp32) / 12 x 12.8 MB (bf16) > 50 MB L2
     # ---- K3: softmax over the KB + weighted sum.  Algorithmic bytes (SURVEY 8(d)): KB once + logits in + att out + info out
     for name, bf16 in (("fp32_kb", 0), ("bf16_kb", 1)):
         kbs = [torch.randn(B, N, d, device="cuda") for _ in range(NB)]
@@ -302,10 +303,10 @@ def kernel_rooflines(shape, prec, pk):
         t_cold = time_kernel(fns, iters=12, flush=flush)
         nbytes = B * N * d * (2 if bf16 else 4) + B * N * 4 * 4 + B * N * 4 + B * d * 4
         out["kb_attend_" + name] = {"bound": "hbm", "achieved": nbytes / t / 1e9, "peak": pk["hbm"], "unit": "GB/s",
-                                    "frac": nbytes / t / 1e9 / pk["hbm"], "traffic": ncu_traffic("kb_attend_" + name),
+                                    "frac": nbytes / t / 1e9 / pk["hbm"], "traffic": None,
                                     "us": t * 1e6,
                                     "algorithmic_bytes": nbytes,
-                                    "l2": "launches rotate over %d knowledge bases (%.0f MB > 126 MB L2), back to back"
+                                    "l2": "launches rotate over %d knowledge bases (%.0f MB > 50 MB L2), back to back"
                                           % (NB, NB * B * N * d * (2 if bf16 else 4) / 1e6),
                                     "us_single_launch_after_256MB_write_flush": t_cold * 1e6}
         if not bf16:
@@ -358,7 +359,7 @@ def kernel_rooflines(shape, prec, pk):
                                   "unit": "TFLOP/s", "frac": flops / t / 1e12 / pk["tensor_burst"], "traffic": None,
                                   "us": t * 1e6, "note": "fp32 FMA-pipe kernel (parity path) against the bf16 tensor peak"}
     del xs
-    # ---- the same projection on tensor cores (tcgen05.mma, bf16 operands, fp32 accumulate in TMEM)
+    # ---- the same projection on tensor cores (wgmma, bf16 operands, fp32 accumulate in registers)
     xb = [torch.randn(M, K, device="cuda").to(torch.bfloat16) for _ in range(6)]      # 6 x 25.7 MB > L2
     Wt = torch.empty(d, K, dtype=torch.bfloat16, device="cuda")
     L.check(lib.mac_pack_weight_bf16(L.ptr(W), L.ptr(Wt), K, d, L.stream_ptr()))
@@ -372,9 +373,9 @@ def kernel_rooflines(shape, prec, pk):
     t = time_kernel([mkt(x) for x in xb], iters=30)
     out["memKbProj_gemm_tc"] = {"bound": "tensor", "achieved": flops / t / 1e12, "peak": pk["tensor_burst"],
                                 "unit": "TFLOP/s", "frac": flops / t / 1e12 / pk["tensor_burst"],
-                                "traffic": ncu_traffic("tc_gemm_memKbProj"), "us": t * 1e6, "algorithmic_flops": flops,
-                                "note": "tcgen05 UMMA, H = ELU([12544,1024] @ [1024,512] + b) bf16 in / bf16 out, "
-                                        "fp32 accumulate in TMEM; A rotates over 6 buffers (154 MB > L2); burst peak"}
+                                "traffic": None, "us": t * 1e6, "algorithmic_flops": flops,
+                                "note": "wgmma, H = ELU([12544,1024] @ [1024,512] + b) bf16 in / bf16 out, "
+                                        "fp32 accumulate; A rotates over 6 buffers (154 MB > L2)"}
     # ---- the per-step form of the same projection in inference: P and Q = P @ Wm[d:2d] + bm are hoisted out of the
     #      netLength loop (mac_read_invariant), each step runs H = ELU((P*y) @ Wm[0:d] + Q): K = d.  With bf16 in/out this
     #      GEMM is below the ridge point (AI = 2MKN / 2(MK + 2MN) = K/3 ... 171 FLOP/B < peak_tensor / peak_hbm), i.e.
@@ -391,13 +392,13 @@ def kernel_rooflines(shape, prec, pk):
         "bound": "hbm" if t_hbm >= t_tc else "tensor",
         "achieved": hbytes / t / 1e9 if t_hbm >= t_tc else hflops / t / 1e12,
         "peak": pk["hbm"] if t_hbm >= t_tc else pk["tensor_burst"], "unit": "GB/s" if t_hbm >= t_tc else "TFLOP/s",
-        "frac": max(t_hbm, t_tc) / t, "traffic": ncu_traffic("tc_gemm_memKbProj_step"), "us": t * 1e6,
+        "frac": max(t_hbm, t_tc) / t, "traffic": None, "us": t * 1e6,
         "algorithmic_bytes": hbytes, "algorithmic_flops": hflops, "tflops": hflops / t / 1e12,
-        "note": "tcgen05 UMMA, ELU([12544,512] @ [512,512] (+ Q)) bf16 in / bf16 out; timed through mac_linear_tc_fwd "
+        "note": "wgmma, ELU([12544,512] @ [512,512] (+ Q)) bf16 in / bf16 out; timed through mac_linear_tc_fwd "
                 "(same kernel template, bias instead of the Q addend); A rotates over 6 buffers"}
     del xb, xh
-    # ---- the inference read step as ONE kernel (csrc/read_step.cuh): scale + both projections + logits + softmax + KB
-    #      weighted sum.  The REAL kernel, on rotating inputs: NR sets of (P, Q, KB) bf16 = NR x 38.5 MB > L2, and rotating
+    # ---- the inference read step (csrc/read_step.cuh): scale + both projections + logits + softmax + KB weighted sum.
+    #      The real launches, on rotating inputs: NR sets of (P, Q, KB) bf16 = NR x 38.5 MB > L2, and rotating
     #      y / control / outputs.  Algorithmic work per launch (SURVEY 8(d), hoisted inference form): 4*B*N*d^2 flops
     #      (two [B*N,d]x[d,d] products); bytes = P + Q + KB (bf16) + both weights + y, control in + att, info out.
     try:
@@ -433,16 +434,8 @@ def kernel_rooflines(shape, prec, pk):
                                                     L.ptr(info_o), L.ptr(att_o), B, N, d, L.stream_ptr()))
                 return rs
             fns = [mkr(sx) for sx in sets]
-            # the dominant kernel alone: profiling flag 8 skips the ~2 us combine launch that follows it in the packed form
-            # (its outputs are then unmerged partials; nothing reads them here); the pair is timed too and reported beside it
-            raw_lib = ctypes.CDLL(L.LIB_PATH)
-            t_pair = time_kernel(fns, iters=60)
-            raw_lib.mac_dbg_read_step_flags(8)
-            try:
-                t = time_kernel(fns, iters=60)
-                t_cold = time_kernel(fns, iters=12, flush=flush)
-            finally:
-                raw_lib.mac_dbg_read_step_flags(0)
+            t = time_kernel(fns, iters=60)
+            t_cold = time_kernel(fns, iters=12, flush=flush)
             Mr = B * N
             rflops = 4.0 * Mr * d * d
             rbytes = 3.0 * Mr * d * 2 + 2.0 * d * d * 2 + 2.0 * B * d * 4 + B * N * 4 + B * d * 4
@@ -451,23 +444,17 @@ def kernel_rooflines(shape, prec, pk):
                 "bound": "tensor" if t_tc >= t_hbm else "hbm",
                 "achieved": rflops / t / 1e12 if t_tc >= t_hbm else rbytes / t / 1e9,
                 "peak": pk["tensor_burst"] if t_tc >= t_hbm else pk["hbm"], "unit": "TFLOP/s" if t_tc >= t_hbm else "GB/s",
-                "frac": max(t_hbm, t_tc) / t, "traffic": ncu_traffic("read_step_fused"), "us": t * 1e6,
+                "frac": max(t_hbm, t_tc) / t, "traffic": None, "us": t * 1e6,
                 "us_single_launch_after_256MB_write_flush": t_cold * 1e6,
-                "us_with_combine_kernel": t_pair * 1e6, "ctas": (Mr + 127) // 128 if N > 128 else None,
-                # the packed kernel launches ceil(B*N/128) CTAs (1 per SM) and leaves the other SMs to the next pass's kernels:
-                # the same fraction against the roof of the SMs it occupies (informational; `frac` is against the whole GPU)
-                "frac_of_occupied_sms": (max(t_hbm, t_tc) / t) * (148.0 / max(1, min(148, (Mr + 127) // 128))) if N > 128 else None,
                 "algorithmic_flops": rflops, "algorithmic_bytes": rbytes, "hbm_gbs": rbytes / t / 1e9,
                 "hbm_frac": rbytes / t / 1e9 / pk["hbm"], "tflops": rflops / t / 1e12,
-                "l2": "launches rotate over %d input sets (%.0f MB of bf16 P, Q, KB > 126 MB L2), back to back" % (NR, NR * 3 * Mr * d * 2 / 1e6),
-                "note": "ONE launch per reasoning step: (P*y) @ Wm[0:d] + Q -> ELU -> @ Wm2 -> logits -> softmax -> sum att*KB; "
-                        "tcgen05 cta_group::2 pairs over PACKED 128-row tiles (ceil(B*N/128) CTAs, no padded rows for N > 128), "
-                        "fp32 accumulators fill TMEM (128 x 512), H stays in shared memory, per-sample softmax partials merged by "
-                        "a B-CTA combine kernel (inside the timed launch pair); flops are the ALGORITHMIC 4*B*N*d^2"}
+                "l2": "launches rotate over %d input sets (%.0f MB of bf16 P, Q, KB > 50 MB L2), back to back" % (NR, NR * 3 * Mr * d * 2 / 1e6),
+                "note": "per reasoning step: read_step_kernel (P*y -> (P*y) @ Wm[0:d] + Q -> ELU -> @ Wm2 -> logits, on the SM) + "
+                        "kb_attend (softmax + sum att*KB); flops are the ALGORITHMIC 4*B*N*d^2"}
             del sets
     except Exception as exc:
         out["read_step_fused"] = {"error": repr(exc)[:300]}
-    # ---- "next" row: the image stem that produces the knowledge base (2 x conv3x3 as im2col + tcgen05 GEMM)
+    # ---- "next" row: the image stem that produces the knowledge base (2 x conv3x3 as im2col + wgmma GEMM)
     try:
         from mac_network_b200.stem import Stem, stem_specs, init_stem_params
         sp = {k: torch.from_numpy(v).cuda() for k, v in init_stem_params(stem_specs(1024, d), seed=3).items()}
@@ -478,7 +465,7 @@ def kernel_rooflines(shape, prec, pk):
         out["stem_forward_tc"] = {"bound": "tensor", "achieved": sflops / t / 1e12, "peak": pk["tensor_burst"],
                                   "unit": "TFLOP/s", "frac": sflops / t / 1e12 / pk["tensor_burst"], "traffic": None,
                                   "us": t * 1e6, "algorithmic_flops": sflops,
-                                  "note": "stem (model.py:165-204): 2 x [fused im2col -> tcgen05 GEMM + ELU], bf16 operands"}
+                                  "note": "stem (model.py:165-204): 2 x [fused im2col -> wgmma GEMM + ELU], bf16 operands"}
     except Exception as exc:                      # the stem is a 'next' row: never let it break the headline line
         out["stem_forward_tc"] = {"error": repr(exc)[:200]}
     return out
@@ -601,9 +588,12 @@ def run_ours(args):
         sampler.start()
     # K = --steps passes per block, blocks repeated until >= 0.5 s of device time: the reported time is the MEDIAN block
     t_dev, dev_blocks = timed_blocks(run_passes, args.steps, barrier, dist, min_total_s=args.min_time)
-    # the sampler stops HERE: polling nvidia-smi through the host-driven end-to-end region below costs it ~15 % (19.8k vs
-    # 23.5k reasoning-steps/s on the B200 box, profiles/r1/NOTES.md) -- the queries contend with the copy / launch calls
+    # the sampler stops HERE: polling nvidia-smi through the host-driven end-to-end region below slows it -- the queries
+    # contend with the copy / launch calls
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        torch.cuda.synchronize()
+        slots[(args.steps - 1) % nslots].dump(args.dump_outputs)        # the slot the last timed pass ran on
 
     # ---- end-to-end arm: host (pinned) buffers; every pass does H2D of its batch, the netLength unroll, and D2H of the
     #      final state + attention maps.  ND device slots, each on its own stream, so the copies of one pass overlap the
@@ -649,7 +639,7 @@ def run_ours(args):
             train_full = {"skipped": "measured at N=1 only; the N>1 lines carry the cell's DP-training arm (`train`)"}
         if world == 1:
             # sub-lines (VERDICT r1 'missing' #1, #6): the two paths inside the 1e-4 parity bar at the headline shape -- tc32 =
-            # split-bf16 products on tcgen05 (6e-7 measured), fp32 = the SIMT FMA path (7e-7) -- and the GQA-shaped variant
+            # split-bf16 products on wgmma, fp32 = the SIMT FMA path -- and the GQA-shaped variant
             # (BASELINE configs[4]: 7x7 grid, self-attention + gate, netLength 6), resident inputs, measured in child processes
             sub_lines = {"tc32_headline": child_measure(["--mode", "quick", "--prec", "tc32", "--streams", "4", "--steps", "12",
                                                          "--warmup", "3"], timeout_s=120),
@@ -659,8 +649,8 @@ def run_ours(args):
                                                     "--warmup", "6"], timeout_s=120),
                          "fp32_gqa": child_measure(["--mode", "quick", "--workload", "gqa", "--prec", "fp32", "--streams", "4",
                                                     "--steps", "12", "--warmup", "3"], timeout_s=120)}
-            train_tc = {"note": "since round 2 the `train` entry above IS the tensor-core form (bf16 forward, tcgen05 backward products); "
-                                "MAC_TRAIN_FP32=1 measures the all-fp32 SIMT form (38.8 ms per step: forward 12.3 + backward 26.5)"}
+            train_tc = {"note": "the `train` entry above IS the tensor-core form (bf16 forward, wgmma backward products); "
+                                "MAC_TRAIN_FP32=1 measures the all-fp32 SIMT form"}
             # informational (NOT the headline configuration): six B=64 requests concatenated into one B=384 pass -- what
             # dynamic batching across requests would buy over independent passes in flight; measured in a child process
             batched = {"requests_x6_one_stream": child_measure(["--mode", "quick", "--batch-mult", "6", "--streams", "1",
@@ -687,12 +677,12 @@ def run_ours(args):
                        "step": "one netLength-step unroll over one batch (%d reasoning steps)" % L,
                        "timing": "blocks of exactly --steps passes (barrier + synchronize on both sides, CUDA events, max over "
                                  "ranks), repeated until >= %.2f s; ms_per_step / value are the MEDIAN block" % args.min_time,
-                       "l2": "timed passes rotate over %d resident batches (%.0f MB > 126 MB L2)"
+                       "l2": "timed passes rotate over %d resident batches (%.0f MB > 50 MB L2)"
                              % (nslots, nslots * (B * N * d + B * S * d) * 4 / 1e6),
                        "cuda_graph": use_graph, "projections": args.prec, "concurrent_passes": nstreams,
                        "write_unit_folded_with_next_projY": bool(fold_y or small_tc),
-                       "batch_sized_projections": "tcgen05, 3-pass split bf16 (fp32-class accuracy)" if small_tc else "fp32 cluster kernel",
-                       "read_step": "one fused launch per reasoning step (csrc/read_step.cuh)", "parallelism": "dp%d (replicas, no "
+                       "batch_sized_projections": "wgmma, 3-pass split bf16 (fp32-class accuracy)" if small_tc else "fp32 cluster kernel",
+                       "read_step": "one wgmma kernel per 64 KB rows (P*y, both projections, logits on the SM) + softmax / weighted sum (csrc/read_step.cuh)", "parallelism": "dp%d (replicas, no "
                        "data-path collective in inference)" % world},
             "sample_steps_per_sec": value * B,
             "timed_blocks": {"resident": {"blocks": len(dev_blocks), "total_s": float(np.sum(dev_blocks)),
@@ -735,9 +725,9 @@ def train_arm(steps, warmup, rank, world, dist):
     B, S, N, d, L = shape
     cfg = MACConfig.args("args", netLength=L)
     pv = perturb_biases(init_params(cfg, L, seed=100), seed=101)
-    # read unit's forward and backward products on tcgen05 tensor cores (bf16 operands, fp32 accumulation / master weights /
-    # optimizer state): the DP default since round 2 (gated by tests/test_zzz_tensor_core_training.py); MAC_TRAIN_FP32=1
-    # measures the all-fp32 SIMT form instead (38.9 ms per step in round 1)
+    # read unit's forward and backward products on wgmma tensor cores (bf16 operands, fp32 accumulation / master weights /
+    # optimizer state): the DP default (gated by tests/test_zzz_tensor_core_training.py); MAC_TRAIN_FP32=1 measures the
+    # all-fp32 SIMT form instead
     tc = os.environ.get("MAC_TRAIN_FP32", "0") != "1"
     tr = DPTrainer(cfg, L, param_values=pv, seed=7, rank=rank, world=world, classifier=(28, [512]),   # CLEVR: 28 answers
                    prec="bf16" if tc else "fp32", bwd_tc=tc)
@@ -770,7 +760,7 @@ def train_arm(steps, warmup, rank, world, dist):
     out = {"value": steps * L * world / t, "unit": UNIT, "ms_per_step": t / steps * 1e3, "steps": steps,
            "what": "DP training step: train-mode cell forward + output unit + mean softmax-CE over the global batch + hand-written "
                    "backward + all-reduce of the flat gradient bucket (%.1f MB, NCCL) + fused clip/Adam/EMA; B=%d per GPU, %s"
-                   % (tr.params.numel * 4 / 1e6, B, "read-unit forward + backward products on tcgen05 (bf16 operands, fp32 "
+                   % (tr.params.numel * 4 / 1e6, B, "read-unit forward + backward products on wgmma (bf16 operands, fp32 "
                       "accumulate, fp32 master weights)" if tc else "fp32 path"),
            "replicas_in_sync": sync}
     del tr
@@ -792,7 +782,7 @@ def train_tc_arm(timeout_s=90):
         return {"value": line["value"], "unit": line["unit"], "ms_per_step": line["ms_per_step"], "steps": line["steps"],
                 "gpu_launches": line["gpu_launches"], "replicas_in_sync": line["config"]["replicas_in_sync_after_run"],
                 "what": "bench.py --mode train --train-prec bf16 --bwd-tc 1 in a child process: DP training step of the cell with "
-                        "the read unit's forward and backward products on tcgen05 tensor cores (linear-probe loss)"}
+                        "the read unit's forward and backward products on wgmma tensor cores (linear-probe loss)"}
     except Exception as exc:
         return {"error": repr(exc)[:300]}
 
@@ -943,7 +933,7 @@ def run_quick(args):
     params = MACParams(cfg, L, values=perturb_biases(init_params(cfg, L, seed=100), seed=101))
     nstreams = max(1, args.streams)
     fold_y = (nstreams < 4) if args.fold_y < 0 else bool(args.fold_y)
-    nslots = max(2, min(NSLOTS, 2 * nstreams)) if mult > 1 else max(NSLOTS, nstreams)   # keep > 126 MB of inputs in rotation
+    nslots = max(2, min(NSLOTS, 2 * nstreams)) if mult > 1 else max(NSLOTS, nstreams)   # keep > 50 MB of inputs in rotation
     slots = [Slot(cfg, params, shape, 1234 + s, args.prec, not args.no_graph, fold_y=fold_y, small_tc=(nstreams >= 2))
              for s in range(nslots)]
     side = [torch.cuda.Stream() for _ in range(nstreams - 1)]
@@ -1034,11 +1024,12 @@ def main():
     ap.add_argument("--skip-train", action="store_true", help="skip the short DP-training arm of the default run")
     ap.add_argument("--mode", default="infer", choices=["infer", "train", "quick"])
     ap.add_argument("--batch-mult", type=int, default=1, help="--mode quick: requests of B=64 concatenated per pass")
-    ap.add_argument("--streams", type=int, default=12, help="independent passes in flight (each on its own stream); "
-                    "measured on the B200 (packed read step): 1: 19.9k, 4: 32.4k, 8: 34.4k, 12: 35.1k, 16: 35.1k reasoning-steps/s")
+    ap.add_argument("--streams", type=int, default=12, help="independent passes in flight (each on its own stream)")
     ap.add_argument("--fold-y", type=int, default=-1, help="write unit folded with the next step's projY: 1/0, -1 = by --streams")
-    ap.add_argument("--rooflines-only", action="store_true", help="only the per-kernel measurements (for ncu)")
-    ap.add_argument("--min-time", type=float, default=0.5, help="repeat the --steps block until this many seconds are timed")
+    ap.add_argument("--rooflines-only", action="store_true", help="only the per-kernel measurements")
+    ap.add_argument("--min-time", type=float, default=0.0, help="repeat the --steps block until this many seconds are timed "
+                    "(default: one block, i.e. exactly --steps timed passes)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed pass's outputs as DIR/<name>.npy")
     ap.add_argument("--workload", default="headline", choices=["headline", "gqa", "cpu_ref"], help="--mode quick: shape + flag file")
     ap.add_argument("--train-prec", default="fp32", choices=["fp32", "bf16"], help="--mode train: read-unit forward GEMMs")
     ap.add_argument("--bwd-tc", type=int, default=0, help="--mode train: read-unit backward GEMMs on tensor cores (1/0)")

@@ -1,5 +1,5 @@
 /*
- * mac_b200.h -- C ABI of the B200-native MAC reasoning cell (libmac_b200.so).
+ * mac_b200.h -- C ABI of the GPU-native MAC reasoning cell (libmac_b200.so, sm_90a).
  *
  * Drop-in boundary for the hot path of stanfordnlp/mac-network: the three units of
  * `MACCell` (reference `mac_cell.py`) plus the slice of `ops.py` they call.  The reference
@@ -41,7 +41,7 @@ enum {
   MAC_ERR_ALIGN = -2,       /* pointer or leading dimension not 16-byte aligned */
   MAC_ERR_UNSUPPORTED = -3, /* flag combination outside the fused path */
   MAC_ERR_WORKSPACE = -4,   /* workspace too small */
-  MAC_ERR_ARCH = -5         /* not an sm_100 device / tensor-map driver entry point missing */
+  MAC_ERR_ARCH = -5         /* not an sm_90 device / tensor-map driver entry point missing */
 };
 
 /* ops.activations (ops.py:181-187) with the config.relu switch (ops.py:161-179) resolved by the caller */
@@ -50,15 +50,15 @@ enum { MAC_ACT_NON = 0, MAC_ACT_TANH = 1, MAC_ACT_SIGMOID = 2, MAC_ACT_ELU = 3, 
 /* arithmetic of the d x d projections */
 enum {
   MAC_PREC_FP32 = 0, /* fp32 FMA pipe, fp32 accumulate: the <=1e-4 parity configuration */
-  MAC_PREC_BF16 = 1, /* bf16 operands on tcgen05 tensor cores, fp32 accumulate in TMEM: the headline configuration */
-  MAC_PREC_TC32 = 2  /* split-bf16 on tcgen05 (x = hi + lo, three of the four partial products, fp32 accumulate): a tensor-core
+  MAC_PREC_BF16 = 1, /* bf16 operands on wgmma tensor cores, fp32 accumulate: the headline configuration */
+  MAC_PREC_TC32 = 2  /* split-bf16 on wgmma (x = hi + lo, three of the four partial products, fp32 accumulate): a tensor-core
                         path inside the 1e-4 parity bar.  Inference form only (mac_read_invariant / mac_read_fwd_inv); fp32
                         knowledge base; everything outside the three [B*N, .] projections as in MAC_PREC_FP32 */
 };
 
 int mac_b200_abi_version(void);
 const char* mac_b200_strerror(int status);
-/* 1 if the current device is compute capability 10.x (tcgen05/TMEM/TMA available) */
+/* 1 if the current device is compute capability 9.0 (wgmma/TMA available) */
 int mac_b200_device_ok(void);
 /* number of kernels this library has launched (or recorded into a stream capture) in this process */
 long long mac_b200_launch_count(void);
@@ -145,13 +145,12 @@ int mac_read_fwd_inv(const float* kb, const void* kb_bf16, const void* inv, cons
                      mac_stream_t stream);
 /* y_pre (may be NULL): y = memory_in @ Wy + by [B, d] when the caller already has it, see mac_write_fwd_next_y. */
 
-/* One inference read step as ONE kernel (csrc/read_step.cuh): given inv = [P | Q] from mac_read_invariant (bf16), the bf16
- * knowledge base, y = memory @ Wy + by [B, d] (ops.py:689) and the control state [B, d], computes
+/* One inference read step (csrc/read_step.cuh): given inv = [P | Q] from mac_read_invariant (bf16), the bf16 knowledge base,
+ * y = memory @ Wy + by [B, d] (ops.py:689) and the control state [B, d], computes
  *   H = ELU((P*y) @ Wm[0:d] + Q);  logits = ELU((H @ Wm2 + bm2) * control) . wr + br;  att = softmax_n(logits);
  *   info = sum_n att * KB                                     (mac_cell.py:230-275 at readDropout == 1)
- * with P*y, H, I1, I2 and the logits kept on the SM (shared / tensor memory).  For N > 128 the kernel walks the [B*N, d]
- * matrices in packed 128-row tiles across sample boundaries (ceil(B*N/128) CTAs), leaves per-tile softmax partials in the scratch
- * that mac_read_invariant_bytes reserves behind [P | Q] in `inv`, and a second, B-CTA launch merges them into att / info (so
+ * as four launches (row scaling, two wgmma GEMMs with the element-wise work in their epilogues, softmax + weighted sum).
+ * P*y, H and the logit partial sums go to the scratch that mac_read_invariant_bytes reserves behind [P | Q] in `inv` (so
  * `inv` is read AND written by this call: one call at a time per `inv`).  mac_read_fwd_inv dispatches to it when
  * mac_read_step_fused_supported(B, N, d) (d == 512, N <= 256) unless the environment sets MAC_READ_FUSED=0.
  * Returns MAC_ERR_UNSUPPORTED for other shapes. */
@@ -159,15 +158,15 @@ int mac_read_step_fused(const void* inv, const void* kb_bf16, const float* y, co
                         const mac_read_weights* w, float* info, float* att, int B, int N, int d, mac_stream_t stream);
 int mac_read_step_fused_supported(int B, int N, int d);
 
-/* One whole inference reasoning step as ONE kernel (plain write unit: writeInputs=BOTH, writeMemProj, no self-attention,
- * no gate; control chain hoisted; dropouts = 1).  mac_read_step_fused with the recurrent glue moved into its prologue:
+/* One whole inference reasoning step (plain write unit: writeInputs=BOTH, writeMemProj, no self-attention,
+ * no gate; control chain hoisted; dropouts = 1).  mac_read_step_fused after a per-sample prologue kernel:
  *   memory = info_prev ? [mem_prev, info_prev] @ Ww + bw : mem_prev      (write unit of the PREVIOUS step, mac_cell.py:339-352)
  *   y      = memory @ Wy + by                                            (ops.py:689)
  *   info, att = read step (as mac_read_step_fused) with this y and `control`
  * `memory` is written to mem_out when info_prev != NULL.  The two products are per-sample matrix-vector products against bf16
  * [out, in] copies of the weights (mac_pack_weight_bf16; fp32 activations and accumulation), computed while the kernel's
  * first TMA requests wait for their tensor-map descriptors.  The caller runs mac_write_fwd once after the last step for the
- * final memory.  mac_step_fused_supported: d == 512 and 128 < N <= 256 (a CTA pair per sample). */
+ * final memory.  mac_step_fused_supported: d == 512 and 128 < N <= 256. */
 int mac_step_fused(const void* inv, const void* kb_bf16, const float* mem_prev, const float* info_prev, const float* control,
                    const mac_read_weights* w, const void* Ww_t_bf16, const float* bw, const void* Wy_t_bf16, float* mem_out,
                    float* info, float* att, int B, int N, int d, mac_stream_t stream);
@@ -248,9 +247,9 @@ uint32_t mac_host_crc32c(const void* data, long long n, uint32_t crc);
 /* ------------------------------------------------------------------------------------------------
  * Tensor-core (MAC_PREC_BF16) helpers.
  * mac_pack_weight_bf16: fp32 W[K, n_out] (the reference's [in, out] layout, ops.py:304) -> bf16 Wt[n_out, K], the
- *   K-major B operand tcgen05.mma consumes; call once per weight update.
+ *   K-major B operand wgmma consumes; call once per weight update.
  * mac_linear_tc_fwd: y[M,n_out] = act(x[M,K] @ W + b) with x bf16 row-major and W given as the packed Wt;
- *   fp32 accumulation in TMEM; output fp32, or bf16 when y_is_bf16 (the form the read-unit chain uses; act in
+ *   fp32 accumulation; output fp32, or bf16 when y_is_bf16 (the form the read-unit chain uses; act in
  *   {NON, ELU}, b required).  Requires K % 64 == 0 and n_out % 128 == 0.
  * --------------------------------------------------------------------------------------------- */
 int mac_pack_weight_bf16(const float* W, void* Wt_bf16, int K, int n_out, mac_stream_t stream);
@@ -264,7 +263,7 @@ int mac_linear_tc_fwd(const void* x_bf16, const void* wt_bf16, const float* b, i
  * qInput{i}), 322 (ctrlProj), 352 (newMemory), 363 (gate) and ops.py:689 (projY), the calls whose M is the batch:
  *   y[M, n_out] = epilogue( concat_k(x_0 .. x_{nseg-1})[M, K] @ W + b + bias_const ),  M <= 128, fp32 in / fp32 out.
  * mac_pack_weight_bf16_split: fp32 W[K, n_out] -> bf16 hi and lo halves, both [n_out, K] (K-major), W ~= hi + lo.
- * With wt_lo != NULL the product is three tcgen05 passes (x_hi W_hi + x_lo W_hi + x_hi W_lo, the activations split in the
+ * With wt_lo != NULL the product is three wgmma passes (x_hi W_hi + x_lo W_hi + x_hi W_lo, the activations split in the
  * kernel) accumulated in fp32 in tensor memory: fp32-class accuracy (~1e-5) on the tensor pipe, so the recurrent state
  * does not pass through bf16.  wt_lo == NULL: one plain bf16 pass.
  * Epilogue: act in MAC_ACT_*; y2 != NULL sends columns >= n_split to y2[m, n - n_split] (the folded write unit, see
@@ -305,7 +304,7 @@ int mac_read_bwd(const float* kb, const float* memory_in, const float* control, 
                  float* dWm, float* dbm_part, float* dWm2, float* dbm2_part, float* dwr_part, float* dbr_part,
                  void* workspace, size_t workspace_bytes, int B, int N, int d, mac_stream_t stream);
 size_t mac_read_bwd_workspace_bytes(int B, int N, int d);
-/* mac_read_bwd with its six [B*N, .] products on tcgen05 tensor cores (bf16 operands, fp32 accumulation; all element-wise
+/* mac_read_bwd with its six [B*N, .] products on wgmma tensor cores (bf16 operands, fp32 accumulation; all element-wise
  * work in fp32): dgrad = mac_linear_tc_fwd(bf16(dY), bf16(W) in its own [in,out] layout), wgrad = mac_linear_tc_fwd(bf16(X)^T,
  * bf16(dY)^T) with K = B*N, fed by mac_cast_bf16 / mac_pack_weight_bf16.  Same arguments and accumulation conventions as
  * mac_read_bwd (the transposed fp32 weights are not needed except Wy_t); dWx, dWm, dWm2 are required.

@@ -131,7 +131,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise MacB200Error("%s not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                           "(nvcc, sm_100a).  mac_network_b200 has no CPU/PyTorch fallback." % LIB_PATH)
+                           "(nvcc, sm_90a).  mac_network_b200 has no CPU/PyTorch fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in PROTOTYPES.items():
         fn = getattr(lib, name)          # AttributeError if the .so does not export a declared symbol

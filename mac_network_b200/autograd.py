@@ -29,7 +29,7 @@ def _t(params, W, key):
 class _Bwd(object):
     def __init__(self, cell, bucket=None, zero_bucket=True, tc=False):
         self.cell, self.lib = cell, cell.lib
-        # tc: the read unit's six big products on tcgen05 tensor cores (mac_read_bwd_tc) instead of the fp32 FMA GEMMs
+        # tc: the read unit's six big products on wgmma tensor cores (mac_read_bwd_tc) instead of the fp32 FMA GEMMs
         self.tc = bool(tc)
         if self.tc and (cell.d % 128 or (cell.B * cell.N) % 64):
             raise NotImplementedError("tensor-core backward needs d % 128 == 0 and (B*N) % 64 == 0")

@@ -175,7 +175,7 @@ class MACConfig:
 
     @property
     def is_fast_path(self):
-        """True when the flag set is one the fused sm_100a kernels cover (the shipped args*.txt family)."""
+        """True when the flag set is one the fused sm_90a kernels cover (the shipped args*.txt family)."""
         return (self.readProjInputs and not self.readProjShared and self.readMemConcatKB and self.readMemConcatProj
                 and self.readMemProj and self.readCtrl and self.readMemAttType == "MUL"
                 and self.readCtrlAttType == "MUL" and self.readMemAct == "RELU" and self.readCtrlAct == "RELU"

@@ -287,10 +287,10 @@ extern "C" int mac_control_attend_fwd(const float* cc, long long cc_tstride, lon
   if (smem > 220 * 1024) return MAC_ERR_UNSUPPORTED;   // S*d beyond one SM's shared memory (not a MAC shape)
   if ((size_t)S * d * sizeof(float) * 2 >= (1u << 20)) return MAC_ERR_UNSUPPORTED;  // mbarrier tx-count range
   MAC_CUDA_TRY(cudaFuncSetAttribute(control_attend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  // B CTAs cannot fill 148 SMs at B=64: split the steps over gridDim.y so that ~2 CTAs/SM are resident
+  // B CTAs cannot fill the SMs at B=64: split the steps over gridDim.y so that ~2 CTAs/SM are resident
   int groups = 1;
   if (nsteps > 1) {
-    groups = (296 + B - 1) / B;
+    groups = (2 * mac_num_sms() + B - 1) / B;
     if (groups > nsteps) groups = nsteps;
   }
   const int per = (nsteps + groups - 1) / groups;

@@ -906,8 +906,8 @@ extern "C" int mac_read_bwd(const float* kb, const float* memory_in, const float
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Backward of the read unit with the six [B*N, .] x [., .] products on tcgen05 tensor cores (bf16 operands, fp32
-// accumulation in TMEM; everything element-wise stays fp32).  Same inputs, outputs and accumulation conventions as
+// Backward of the read unit with the six [B*N, .] x [., .] products on wgmma tensor cores (bf16 operands, fp32
+// accumulation; everything element-wise stays fp32).  Same inputs, outputs and accumulation conventions as
 // mac_read_bwd; the GEMMs go through the entry points the forward uses (mac_linear_tc_fwd), fed by the cast / transposing
 // cast kernels (mac_cast_bf16, mac_pack_weight_bf16):
 //   dgrad  dX[M, in]   = dY[M, out] @ W^T        x = bf16(dY) [M, out],  Wt operand = bf16(W) in its own [in, out] layout

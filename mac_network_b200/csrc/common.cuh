@@ -1,4 +1,4 @@
-// Shared device/host helpers for libmac_b200.so (sm_100a only).
+// Shared device/host helpers for libmac_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -20,6 +20,16 @@ extern "C" void mac_b200_count_launch_(void);
   } while (0)
 
 static inline bool mac_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// SM count of the current device (cached per device ordinal): the grid-sizing heuristics aim at ~2 CTAs per SM
+static inline int mac_num_sms() {
+  static int sms[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) dev = 0;
+  if (!sms[dev]) cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
+  return sms[dev];
+}
 
 namespace mac {
 
@@ -122,6 +132,11 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, in
           smem_u32(smem_dst)),
       "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
+}
+__device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
+  uint4 v;
+  asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+  return v;
 }
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");

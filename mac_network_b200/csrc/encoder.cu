@@ -2,7 +2,7 @@
 // (model.py:208-220, ops.py:877) and the bidirectional BasicLSTMCell encoder run under
 // tf.nn.bidirectional_dynamic_rnn(sequence_length = questionLengths) (ops.py:859-905, model.py:279-307).
 //
-// B200 formulation.  The input half of the LSTM kernel does not depend on the recurrence, so
+// GPU formulation.  The input half of the LSTM kernel does not depend on the recurrence, so
 //     gx[dir] = dropout(X)[B*S, E] @ kernel[dir][0:E, :] + bias[dir]
 // is ONE GEMM per direction over all time steps (mac_linear_fwd).  What is left per step is the recurrent half
 //     gates(b, :) = gx[dir][b, t, :] + h_prev[dir][b, :] @ kernel[dir][E:E+h, :]

@@ -1,1225 +1,283 @@
-// One reasoning step of the read unit as ONE kernel (inference form, mac_cell.py:209-277 with readDropout == 1):
+// One reasoning step of the read unit in inference form (mac_cell.py:209-277 with readDropout == 1), P and Q hoisted:
 //
 //   H      = ELU((P * y_b) @ Wm[0:d, :] + Q)            (ops.py:694-703 MUL, mac_cell.py:236-238; P, Q step-invariant)
 //   I2     = ELU((H @ Wm2 + bm2) * control_b)           (ops.py:325-328, mac_cell.py:248-250, 262)
 //   logit  = I2 . wr + br                               (mac_cell.py:266, ops.py:316-317)
 //   att    = softmax_n(logit);  info = sum_n att * KB   (ops.py:143, 149-150; original KB, mac_cell.py:271-275)
 //
-// replacing scale_rows_bf16 + tc_gemm<ADDACT> + tc_gemm<LOGITS> + kb_attend (4 launches, ~64 MB of L2/HBM traffic for the
-// P*y and H round trips) by one launch in which P*y, H, I1, I2 and the logits never leave the SM.
+// read_step_kernel computes the logits of 64 knowledge-base rows per CTA (rows packed across sample boundaries, so
+// ceil(B*N / 64) CTAs) with P*y, H and I2 never leaving the SM; kb_attend (attend.cu) then does the per-sample softmax and
+// weighted sum.  Two launches per step instead of the four of scale_rows_bf16 + tc_gemm<ADDACT> + tc_gemm<LOGITS> + kb_attend,
+// and none of the P*y / H round trips through L2 and HBM (4 x B*N*d bf16).
 //
-// Tiling: a CTA owns 128 knowledge-base rows and the FULL d = 512 output width, so the fp32 accumulator fills the SM's
-// whole tensor memory (128 lanes x 512 columns) and every logit is finished inside one CTA.  Rows are aligned to samples:
-//   PAIR  (128 < N <= 256, CLEVR's 14x14 grid): a 2-CTA cluster per sample; rank r takes rows [128 r, min(N, 128 r + 128)).
-//         The softmax statistics and the two partial weighted sums are exchanged through distributed shared memory.
-//   !PAIR (N <= 128, e.g. the 7x7 GQA grid): a CTA takes spc = min(128 / N, 2) whole samples; no exchange.
+// CTA = 288 threads: warp 8 is the TMA producer; warpgroups 0 and 1 each own one 256-column half of the d = 512 outputs
+// (wgmma m64n256k16, a 64 x 256 fp32 accumulator in 128 registers per thread).  Shared memory:
+//   A   [64 x 512] bf16 as 8 K-major 128-byte-swizzled [64 x 64] blocks (64 KB): the P tile (one TMA wave), scaled by y in
+//       place into P*y, then overwritten by H = GEMM 1's epilogue, the A operand of GEMM 2
+//   B   2 stages x [512 x 64] bf16 (128 KB): the k-blocks of Wm[0:d] and then of Wm2, streamed through one mbarrier ring
+// The logits are summed over both halves in shared memory and written as one partial per row.
 //
-// Warp roles (576 threads):
-//   warp 0       TMA producer: P tile k-blocks (A ring), Wm[0:d] and then Wm2 k-blocks in [256 x 64] halves (B ring)
-//   warp 1       TMEM allocator + tcgen05.mma issuer (UMMA 128 x 256 x 16, two N halves per k-step)
-//   warps 2..17  workers (512 threads).  GEMM 1: scale each landed P k-block by y_b IN PLACE in shared memory (the
-//                operand never exists in HBM), fence it to the async proxy and hand it to the MMA warp.  Then epilogue 1:
-//                TMEM -> registers, + Q, ELU, bf16 -> shared memory in the 128-byte-swizzled K-major layout tcgen05
-//                reads as the A operand of GEMM 2.  Then epilogue 2 (bias, control product, ELU, dot with wr) and the
-//                attention tail (softmax, weighted sum over the bf16 knowledge base).
-//
-// Shared memory (13 units of 16 KB + 14 KB of parameters / exchange): GEMM 1 uses 3 A slots (units 0-2) and 5 B slots
-// (units 3-12); H (128 KB) then overlays units 0-7 and GEMM 2 streams Wm2 through B slots 3 and 4 (units 9-12).
+// Whole-step form (mac_step_fused, N > 128 so that a tile touches at most two samples): the CTA first computes, for each
+// sample it touches, the previous step's plain write unit m = [m_prev, info_prev] @ Ww + bw (mac_cell.py:339-352) and this
+// step's memory projection y = m @ Wy + by (ops.py:689) as matrix-vector products against the bf16 weights (fp32
+// activations and accumulation) while the TMA loads are in flight; the CTA that owns a sample's first row writes its m.
+// That removes the separate write / projY launch, at the price of every CTA re-reading those weights (opt-in form).
 #pragma once
 #include "tc_gemm.cuh"
 
 namespace mac {
 
-constexpr int RS_D = 512;                       // d (TMEM columns of the accumulator)
-constexpr int RS_KB = RS_D / TC_BK;             // 8 k-blocks of 64
-constexpr int RS_WORKER_WARPS = 16;
-constexpr int RS_WORKERS = 32 * RS_WORKER_WARPS;
-constexpr int RS_THREADS = 64 + RS_WORKERS;     // 576
-constexpr int RS_UNIT = 16384;                  // one [128 x 64] bf16 tile
-constexpr int RS_A_SLOTS = 3;
-constexpr int RS_B_SLOTS = 5;
-constexpr int RS_UNITS = RS_A_SLOTS + 2 * RS_B_SLOTS;      // 13
-constexpr int RS_MAX_SPC = 2;                   // samples per CTA on the N <= 128 path
-constexpr int RS_PAR_FLOATS = (2 + RS_MAX_SPC) * RS_D;     // bm2, wr, control rows
-constexpr int RS_RED_GROUPS = 8;                // row groups of the weighted sum
-constexpr int RS_SMEM_BYTES = RS_UNITS * RS_UNIT + 1024 /*align*/ + 256 /*barriers*/ + RS_PAR_FLOATS * 4 +
-                              4 * 128 * 4 /*logit partials*/ + 128 * 4 /*att*/ + 64 /*exchange*/ + RS_D * 4 /*peer info*/;
+constexpr int RS_D = 512;                       // d of the shipped configurations
+constexpr int RS_BM = 64;                       // knowledge-base rows per CTA
+constexpr int RS_KB = RS_D / TC_BK;             // 8 k-blocks
+constexpr int RS_BLK = RS_BM * TC_BK * 2;       // one [64 x 64] bf16 A block: 8 KB
+constexpr int RS_A_BYTES = RS_KB * RS_BLK;      // 64 KB
+constexpr int RS_B_HALF = 256 * TC_BK * 2;      // [256 x 64] bf16: 32 KB
+constexpr int RS_STAGE = 2 * RS_B_HALF;         // 64 KB
+constexpr int RS_STAGES = 2;
+constexpr int RS_CONSUMERS = 256;
+constexpr int RS_THREADS = RS_CONSUMERS + 32;
+constexpr int RS_SMEM_BYTES = RS_A_BYTES + RS_STAGES * RS_STAGE + 1024 /*align*/ + 64 /*barriers*/ +
+                              2 * RS_BM * 4 /*logit halves*/ + 2 * RS_D * 4 /*y of <= 2 samples*/ + 2 * RS_D * 4 /*m*/;
 
-struct ReadStepParams {
-  int B, N;
-  int spc;                          // samples per CTA (!PAIR); 1 for PAIR
-  const float* y;                   // [B, d]   memory projection (ops.py:689)
-  const float* ctrl;                // [B, d]
-  const float* bm2;                 // [d]
-  const float* wr;                  // [d]
-  float br;
-  const __nv_bfloat16* Q;           // [B*N, d]  P @ Wm[d:2d] + bm
-  const __nv_bfloat16* kb;          // [B*N, d]  bf16 knowledge base
-  float* att;                       // [B, N]
-  float* info;                      // [B, d]
-  // whole-step form (pair kernel only; Wy_t != NULL): the memory projection -- and, from the second step on, the previous
-  // step's write unit -- are computed in the kernel's prologue (see read_step2_kernel); `y` is then unused
-  const float* mem_prev;            // [B, d]   memory the previous step read with (or the initial memory when info_prev == NULL)
-  const float* info_prev;           // [B, d]   previous step's retrieved information, or NULL (first step: memory = mem_prev)
-  const __nv_bfloat16* Ww_t;        // [d, 2d]  write/linearLayernewMemory weight, bf16 [out, in]
-  const float* bw;                  // [d]
-  const __nv_bfloat16* Wy_t;        // [d, d]   read/.../linearLayerprojY weight, bf16 [out, in]
-  const float* by;                  // [d]
-  float* mem_out;                   // [B, d]   memory of THIS step (written when info_prev != NULL)
-  // packed form (pair kernel, N > 128, no whole-step prologue): CTA i takes knowledge-base rows [128 i, 128 i + 128) of the
-  // [B*N, d] matrices whatever samples they belong to (at most two when N > 128) -- no padded rows: ceil(B*N / 128) CTAs
-  // instead of 2 B (98 instead of 128 at B = 64, N = 196).  Each CTA leaves, per sample it touches, an un-normalised softmax
-  // partial (local max, sum of exponentials, sum of exp * KB rows) in `part`, and exp values in `att`; read_step_combine_kernel
-  // merges the 2-3 partials of every sample.  part = [B][3][d] partial sums, then [B][3][2] (max, sum).
-  int packed;
-  float* part;
-  int dbg_flags;                    // profiling only (mac_dbg_read_step_flags; results are WRONG when set): 1 skip the P*y
-                                    // smem pass, 2 skip the GEMM-1/2 MMAs, 4 skip the Wm loads of GEMM 1 (pair kernel),
-                                    // 8 skip the combine launch of the packed form
-  long long* dbg;                   // profiling only (mac_dbg_read_step_timestamps): [gridDim.x][64] SM-clock stamps, or NULL
-};
-
-__device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
-  uint4 v;
-  asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-  return v;
-}
-__device__ __forceinline__ void l2_prefetch_bulk(const void* p, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void st_cluster_f32(const float* local_addr, uint32_t cta, float v) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "st.shared::cluster.f32 [ra], %2;\n\t}"
-      ::"r"(smem_u32(local_addr)), "r"(cta), "f"(v)
-      : "memory");
-}
 __device__ __forceinline__ float bf16lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf16hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
-__device__ __forceinline__ void rs_stamp(const ReadStepParams& p, int slot) {
-  if (p.dbg) p.dbg[(size_t)blockIdx.x * 64 + slot] = clock64();
-}
-__device__ __forceinline__ void rs_worker_bar() { asm volatile("bar.sync 1, %0;" ::"n"(RS_WORKERS) : "memory"); }
 
-template <bool PAIR>
-__global__ void __launch_bounds__(RS_THREADS, 1)
-read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constant__ CUtensorMap map_w1,
-                 const __grid_constant__ CUtensorMap map_w2, const ReadStepParams p) {
-  extern __shared__ unsigned char smem_dyn[];
-  const uint32_t base_u32 = smem_u32(smem_dyn);
-  const uint32_t pad = (1024u - (base_u32 & 1023u)) & 1023u;
-  unsigned char* tiles = smem_dyn + pad;                         // 13 units, 1024-byte aligned
-  unsigned char* a_slots = tiles;                                // units 0..2
-  unsigned char* b_slots = tiles + RS_A_SLOTS * RS_UNIT;         // units 3..12, 32 KB each
-  unsigned char* h_tile = tiles;                                 // units 0..7 (after GEMM 1)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + RS_UNITS * RS_UNIT);
-  uint64_t* a_full = bars;                         // [3] TMA -> workers
-  uint64_t* a_ready = bars + 3;                    // [3] workers -> MMA   (16 warp arrivals)
-  uint64_t* a_empty = bars + 6;                    // [3] MMA -> TMA
-  uint64_t* b_full = bars + 9;                     // [5] TMA -> MMA
-  uint64_t* b_empty = bars + 14;                   // [5] MMA -> TMA
-  uint64_t* g1_done = bars + 19;                   // MMA -> workers (accumulator of GEMM 1 complete)
-  uint64_t* hk_ready = bars + 20;                  // [8] workers -> MMA (H k-block in shared memory, its accumulator columns drained)
-  uint64_t* g2_done = bars + 28;                   // [2] MMA -> workers (N half of GEMM 2 complete)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 30);
-  float* par = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(bars) + 256);   // bm2 | wr | ctrl rows
-  float* s_part = par + RS_PAR_FLOATS;             // [4][128] logit partial sums
-  float* s_att = s_part + 4 * 128;                 // [128] logits, then attention weights
-  float* s_xch = s_att + 128;                      // [2 ranks][max, sum] (+ padding to 64 B)
-  float* s_peer = s_xch + 16;                      // [512] partner's partial weighted sum (rank 0 only reads it)
-  float* s_red = reinterpret_cast<float*>(b_slots + 3 * 2 * RS_UNIT);   // [8][512] over B slots 3, 4 (after GEMM 2)
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int N = p.N;
-  uint32_t rank = 0;
-  int s0, nsamp, row0, valid;            // first sample, samples of this CTA, first flat KB row, valid tile rows
-  if constexpr (PAIR) {
-    rank = cluster_rank();
-    s0 = blockIdx.x >> 1;
-    nsamp = 1;
-    row0 = s0 * N + (int)rank * 128;
-    valid = min(128, N - (int)rank * 128);
-  } else {
-    s0 = blockIdx.x * p.spc;
-    nsamp = min(p.spc, p.B - s0);
-    row0 = s0 * N;
-    valid = nsamp * N;
-  }
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_p);
-    tma_prefetch_desc(&map_w1);
-    tma_prefetch_desc(&map_w2);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-      mbar_init(&a_full[i], 1);
-      mbar_init(&a_ready[i], RS_WORKER_WARPS);
-      mbar_init(&a_empty[i], 1);
-    }
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      mbar_init(&b_full[i], 1);
-      mbar_init(&b_empty[i], 1);
-    }
-    mbar_init(g1_done, 1);
-#pragma unroll
-    for (int i = 0; i < RS_KB; ++i) mbar_init(&hk_ready[i], RS_WORKER_WARPS);
-    mbar_init(&g2_done[0], 1);
-    mbar_init(&g2_done[1], 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ===================================================== TMA producer
-    if (elect_one()) {
-      // the tiles the tail of this CTA will read with plain loads: start them towards L2 now
-      {
-        const size_t bytes = (size_t)valid * RS_D * 2;
-        const char* q0 = reinterpret_cast<const char*>(p.Q + (size_t)row0 * RS_D);
-        const char* k0 = reinterpret_cast<const char*>(p.kb + (size_t)row0 * RS_D);
-        for (size_t o = 0; o < bytes; o += 16384) {
-          const uint32_t n = (uint32_t)min((size_t)16384, bytes - o);
-          l2_prefetch_bulk(q0 + o, n);
-          l2_prefetch_bulk(k0 + o, n);
-        }
-      }
-      // GEMM 1: A = P rows of this tile, B = Wm[0:d] in two [256 x 64] halves per k-block
-      for (int kb = 0; kb < RS_KB; ++kb) {
-        const int sa = kb % RS_A_SLOTS, na = kb / RS_A_SLOTS;
-        mbar_wait(&a_empty[sa], (na & 1) ^ 1);
-        mbar_expect_tx(&a_full[sa], RS_UNIT);
-        tma_load_2d(a_slots + sa * RS_UNIT, &map_p, kb * TC_BK, row0, &a_full[sa]);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int j = kb * 2 + h, sb = j % RS_B_SLOTS, nb = j / RS_B_SLOTS;
-          mbar_wait(&b_empty[sb], (nb & 1) ^ 1);
-          mbar_expect_tx(&b_full[sb], 2 * RS_UNIT);
-          tma_load_2d(b_slots + sb * 2 * RS_UNIT, &map_w1, kb * TC_BK, h * 256, &b_full[sb]);
-        }
-      }
-      // GEMM 2: B = Wm2 through slots 3 and 4 only (0..2 are under H); use index continues the per-slot count
-      //         order: all k-blocks of output half 0, then half 1 (epilogue 2 of half 0 overlaps the MMAs of half 1)
-      for (int i = 0; i < 2 * RS_KB; ++i) {
-        const int sb = 3 + (i & 1), nb = 3 + (i >> 1);
-        mbar_wait(&b_empty[sb], (nb & 1) ^ 1);
-        mbar_expect_tx(&b_full[sb], 2 * RS_UNIT);
-        tma_load_2d(b_slots + sb * 2 * RS_UNIT, &map_w2, (i & 7) * TC_BK, (i >> 3) * 256, &b_full[sb]);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    constexpr uint32_t idesc = make_idesc_bf16(128, 256);
-    for (int kb = 0; kb < RS_KB; ++kb) {
-      const int sa = kb % RS_A_SLOTS, na = kb / RS_A_SLOTS;
-      mbar_wait(&a_ready[sa], na & 1);                         // scaled by the workers, visible to the async proxy
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int j = kb * 2 + h, sb = j % RS_B_SLOTS, nb = j / RS_B_SLOTS;
-        mbar_wait(&b_full[sb], nb & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(a_slots + sa * RS_UNIT));
-          const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(b_slots + sb * 2 * RS_UNIT));
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)
-            umma_bf16(tmem_base + h * 256, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          umma_commit(&b_empty[sb]);
-          if (h == 1) {
-            umma_commit(&a_empty[sa]);
-            if (kb == RS_KB - 1) umma_commit(g1_done);
-          }
-        }
-        __syncwarp();
-      }
-    }
-    // GEMM 2, output half h = columns [256 h, 256 h + 256): k-block kb needs H k-block kb (hk_ready[kb]); the first MMA of
-    // half 0 overwrites accumulator columns 0..255 = the GEMM-1 columns of H k-blocks 0..3, so it waits for those four;
-    // half 1 (columns 256..511) starts after all eight.  Epilogue 1 of k-blocks 4..7 thus overlaps half 0's first MMAs.
-    for (int i = 0; i < 2 * RS_KB; ++i) {
-      const int h = i >> 3, kb = i & 7;
-      const int sb = 3 + (i & 1), nb = 3 + (i >> 1);
-      if (h == 0) {
-        if (kb == 0) {
-          mbar_wait(&hk_ready[0], 0);
-          mbar_wait(&hk_ready[1], 0);
-          mbar_wait(&hk_ready[2], 0);
-          mbar_wait(&hk_ready[3], 0);
-        } else if (kb >= 4) {
-          mbar_wait(&hk_ready[kb], 0);
-        }
-      }
-      mbar_wait(&b_full[sb], nb & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(h_tile + kb * RS_UNIT));
-        const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(b_slots + sb * 2 * RS_UNIT));
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k)
-          umma_bf16(tmem_base + h * 256, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-        umma_commit(&b_empty[sb]);
-        if (kb == RS_KB - 1) umma_commit(&g2_done[h]);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===================================================== workers
-    const int wt = threadIdx.x - 64;                 // 0..511
-    const int q = warp & 3;                          // TMEM lane quarter this warp may touch
-    const int cg = (warp - 2) >> 2;                  // column group: 16 columns of every 64-column k-block
-    const int row = q * 32 + lane;                   // tile row == TMEM lane of this thread in the epilogues
-    if (wt == 0) rs_stamp(p, 0);
-    // ---- parameters of epilogue 2 into shared memory (overlaps the first TMA round trips)
-    for (int i = wt; i < RS_D; i += RS_WORKERS) {
-      par[i] = __ldg(p.bm2 + i);
-      par[RS_D + i] = __ldg(p.wr + i);
-    }
-    for (int i = wt; i < nsamp * RS_D; i += RS_WORKERS) par[2 * RS_D + i] = __ldg(p.ctrl + (size_t)s0 * RS_D + i);
-    // ---- Q addend of this thread's row: its 16 columns of k-blocks 0..3 now (8 x 16 B), k-blocks 4..7 while consuming
-    const bool row_ok = row < valid;
-    const __nv_bfloat16* qrow = p.Q + (size_t)(row0 + (row_ok ? row : 0)) * RS_D + cg * 16;
-    uint4 qv[8];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      qv[2 * i] = ldg_nc_v4(qrow + 64 * i);
-      qv[2 * i + 1] = ldg_nc_v4(qrow + 64 * i + 8);
-    }
-
-    // ---- GEMM 1 operand path: P k-block -> (P * y_b) in place.  Thread handles 16-byte chunks c = wt and wt + 512 of
-    //      the 1024 in a [128 x 64] tile: row c >> 3, physical chunk c & 7 == logical chunk (c & 7) ^ (row & 7)
-    //      (the 128-byte swizzle TMA wrote and tcgen05 expects).
-    {
-      const int r_a = wt >> 3, r_b = r_a + 64;
-      const int pc = wt & 7;
-      const int lc_a = pc ^ (r_a & 7), lc_b = pc ^ (r_b & 7);
-      const bool ok_a = r_a < valid, ok_b = r_b < valid;
-      const int b_a = s0 + (PAIR ? 0 : (ok_a ? r_a / N : 0));
-      const int b_b = s0 + (PAIR ? 0 : (ok_b ? r_b / N : 0));
-      const float* y_a = p.y + (size_t)b_a * RS_D + lc_a * 8;
-      const float* y_b = p.y + (size_t)b_b * RS_D + lc_b * 8;
-      auto scale16 = [](uint4 v, const float4 f0, const float4 f1) {
-        uint4 o;
-        o.x = pack_bf16(bf16lo(v.x) * f0.x, bf16hi(v.x) * f0.y);
-        o.y = pack_bf16(bf16lo(v.y) * f0.z, bf16hi(v.y) * f0.w);
-        o.z = pack_bf16(bf16lo(v.z) * f1.x, bf16hi(v.z) * f1.y);
-        o.w = pack_bf16(bf16lo(v.w) * f1.z, bf16hi(v.w) * f1.w);
-        return o;
-      };
-      for (int kb = 0; kb < RS_KB; ++kb) {
-        const int sa = kb % RS_A_SLOTS, na = kb / RS_A_SLOTS;
-        // this k-block's y values (L1-resident after the first touch) before the wait on the tile
-        const float4 ya0 = __ldg(reinterpret_cast<const float4*>(y_a + kb * TC_BK));
-        const float4 ya1 = __ldg(reinterpret_cast<const float4*>(y_a + kb * TC_BK + 4));
-        const float4 yb0 = __ldg(reinterpret_cast<const float4*>(y_b + kb * TC_BK));
-        const float4 yb1 = __ldg(reinterpret_cast<const float4*>(y_b + kb * TC_BK + 4));
-        mbar_wait(&a_full[sa], na & 1);
-        uint4* t = reinterpret_cast<uint4*>(a_slots + sa * RS_UNIT);
-        if (ok_a) t[wt] = scale16(t[wt], ya0, ya1);
-        if (ok_b) t[wt + 512] = scale16(t[wt + 512], yb0, yb1);
-        fence_proxy_async();                       // generic-proxy writes -> visible to tcgen05's async-proxy reads
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a_ready[sa]);
-      }
-    }
-
-    // ---- epilogue 1: H = ELU(acc + Q) -> bf16, K-major 128-byte-swizzled tiles over units 0..7.  One H k-block (64
-    //      columns) at a time across all 16 warps, so that GEMM 2 can start on the k-blocks that are done.
-    const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16);
-    if (wt == 0) rs_stamp(p, 1);                   // last P k-block scaled
-    mbar_wait(g1_done, 0);
-    tc_fence_after();
-    if (wt == 0) rs_stamp(p, 2);                   // GEMM 1 complete
-#pragma unroll
-    for (int kb2 = 0; kb2 < RS_KB; ++kb2) {
-      uint32_t r[16];
-      tmem_ld16(tlane + kb2 * 64 + cg * 16, r);
-      tmem_ld_wait();
-      const uint4 qa = qv[(2 * kb2) & 7], qb = qv[(2 * kb2 + 1) & 7];
-      if (kb2 < 4) {                               // refill the two slots just consumed with k-block kb2 + 4
-        qv[(2 * kb2) & 7] = ldg_nc_v4(qrow + 64 * (kb2 + 4));
-        qv[(2 * kb2 + 1) & 7] = ldg_nc_v4(qrow + 64 * (kb2 + 4) + 8);
-      }
-      const uint32_t qw[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
-      uint32_t w[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        w[j] = pack_bf16(elu_fast(__uint_as_float(r[2 * j]) + bf16lo(qw[j])),
-                         elu_fast(__uint_as_float(r[2 * j + 1]) + bf16hi(qw[j])));
-      const int lc = cg * 2;                       // 16-byte chunk of w[0..3] inside the k-block's 128-byte row
-      unsigned char* hrow = h_tile + kb2 * RS_UNIT + row * 128;
-      *reinterpret_cast<uint4*>(hrow + ((lc ^ (row & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-      *reinterpret_cast<uint4*>(hrow + (((lc + 1) ^ (row & 7)) << 4)) = make_uint4(w[4], w[5], w[6], w[7]);
-      fence_proxy_async();                         // H k-block visible to tcgen05's async-proxy reads
-      tc_fence_before();                           // ... and this warp's reads of the accumulator columns are done
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&hk_ready[kb2]);
-    }
-    if (wt == 0) rs_stamp(p, 3);                   // H written
-
-    // ---- epilogue 2: logit partial of this thread's row; output half h as soon as its MMAs are done
-    rs_worker_bar();                               // parameters staged by all workers are visible
-    const int ls = PAIR ? 0 : (row_ok ? row / N : 0);
-    const float* crow = par + (2 + ls) * RS_D;
-    float part = 0.f;
-#pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
-      mbar_wait(&g2_done[h], 0);
-      tc_fence_after();
-      if (wt == 0 && h == 1) rs_stamp(p, 4);       // GEMM 2 complete
-#pragma unroll 2
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t r[16];
-        const int c0 = h * 256 + cg * 64 + 16 * ch;
-        tmem_ld16(tlane + c0, r);
-        tmem_ld_wait();
-        const float4* b4 = reinterpret_cast<const float4*>(par + c0);
-        const float4* w4 = reinterpret_cast<const float4*>(par + RS_D + c0);
-        const float4* c4 = reinterpret_cast<const float4*>(crow + c0);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 bb = b4[j], ww = w4[j], cc = c4[j];
-          part = fmaf(elu_fast((__uint_as_float(r[4 * j]) + bb.x) * cc.x), ww.x, part);
-          part = fmaf(elu_fast((__uint_as_float(r[4 * j + 1]) + bb.y) * cc.y), ww.y, part);
-          part = fmaf(elu_fast((__uint_as_float(r[4 * j + 2]) + bb.z) * cc.z), ww.z, part);
-          part = fmaf(elu_fast((__uint_as_float(r[4 * j + 3]) + bb.w) * cc.w), ww.w, part);
-        }
-      }
-    }
-    tc_fence_before();
-    s_part[cg * 128 + row] = part;
-    rs_worker_bar();
-    if (wt < 128) s_att[wt] = s_part[wt] + s_part[128 + wt] + s_part[256 + wt] + s_part[384 + wt] + p.br;
-    rs_worker_bar();
-    if (wt == 0) rs_stamp(p, 5);                   // logits
-
-    // ---- knowledge-base rows of the weighted sum: thread = (row group rg of 8, 8-column chunk cq of 64); nrows <= 128 ->
-    //      at most 16 rows per thread.  The 16-byte loads do not depend on the attention weights: all of them are issued
-    //      here, before the softmax (and the pair's cluster barrier), and consumed after it.
-    const int nrows = PAIR ? valid : N;
-    const int rg = wt >> 6, cq = wt & 63;
-    uint4 v[16];
-    auto load_kb_rows = [&](int s) {
-      const __nv_bfloat16* kbase = p.kb + (size_t)(row0 + s * N) * RS_D + cq * 8;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int n = rg + RS_RED_GROUPS * i;
-        v[i] = n < nrows ? ldg_nc_v4(kbase + (size_t)n * RS_D) : make_uint4(0u, 0u, 0u, 0u);
-      }
-    };
-    load_kb_rows(0);
-
-    // ---- softmax statistics: worker warp w < nsamp owns local sample w (rows [w N, w N + nrows))
-    const int wi = warp - 2;
-    float e_lane[4] = {0.f, 0.f, 0.f, 0.f};
-    float mx = -INFINITY, sum = 0.f;
-    if (wi < nsamp) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int n = lane + 32 * i;
-        if (n < nrows) mx = fmaxf(mx, s_att[wi * N + n]);
-      }
-      mx = warp_max(mx);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int n = lane + 32 * i;
-        if (n < nrows) {
-          e_lane[i] = __expf(s_att[wi * N + n] - mx);
-          sum += e_lane[i];
-        }
-      }
-      sum = warp_sum(sum);
-      if constexpr (PAIR) {
-        if (lane == 0) {
-          s_xch[2 * rank] = mx;
-          s_xch[2 * rank + 1] = sum;
-          st_cluster_f32(&s_xch[2 * rank], rank ^ 1u, mx);
-          st_cluster_f32(&s_xch[2 * rank + 1], rank ^ 1u, sum);
-        }
-      }
-    }
-    if constexpr (PAIR) cluster_barrier();         // #1 (all 576 threads of both CTAs; warps 0/1 join below)
-    if (wi < nsamp) {
-      float scale;
-      if constexpr (PAIR) {
-        const float m0 = s_xch[0], z0 = s_xch[1], m1 = s_xch[2], z1 = s_xch[3];
-        const float M = fmaxf(m0, m1);
-        const float Z = z0 * __expf(m0 - M) + z1 * __expf(m1 - M);
-        scale = __expf(mx - M) / Z;
-      } else {
-        scale = 1.f / sum;
-      }
-      const int b = s0 + wi;
-      const int n_off = PAIR ? (int)rank * 128 : 0;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int n = lane + 32 * i;
-        if (n < nrows) {
-          const float a = e_lane[i] * scale;
-          s_att[wi * N + n] = a;
-          p.att[(size_t)b * N + n_off + n] = a;
-        }
-      }
-    }
-    rs_worker_bar();
-
-    if (wt == 0) rs_stamp(p, 6);                   // attention weights
-    // ---- info = sum_n att[n] * KB[n, :]
-    for (int s = 0; s < nsamp; ++s) {
-      float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      const float* a_s = s_att + s * N;
-      if (s > 0) load_kb_rows(s);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int n = rg + RS_RED_GROUPS * i;
-        const float a = n < nrows ? a_s[n] : 0.f;
-        acc[0] = fmaf(a, bf16lo(v[i].x), acc[0]); acc[1] = fmaf(a, bf16hi(v[i].x), acc[1]);
-        acc[2] = fmaf(a, bf16lo(v[i].y), acc[2]); acc[3] = fmaf(a, bf16hi(v[i].y), acc[3]);
-        acc[4] = fmaf(a, bf16lo(v[i].z), acc[4]); acc[5] = fmaf(a, bf16hi(v[i].z), acc[5]);
-        acc[6] = fmaf(a, bf16lo(v[i].w), acc[6]); acc[7] = fmaf(a, bf16hi(v[i].w), acc[7]);
-      }
-      if (s > 0) rs_worker_bar();                  // previous sample's reduction has been read
-      float4* dst = reinterpret_cast<float4*>(s_red + rg * RS_D + cq * 8);
-      dst[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
-      dst[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
-      rs_worker_bar();
-      float t = 0.f;
-#pragma unroll
-      for (int g = 0; g < RS_RED_GROUPS; ++g) t += s_red[g * RS_D + wt];
-      if constexpr (PAIR) {
-        if (rank == 1) st_cluster_f32(&s_peer[wt], 0u, t);        // partner's half of the rows -> leader's smem
-        cluster_barrier();                         // #2
-        if (rank == 0) p.info[(size_t)s0 * RS_D + wt] = t + s_peer[wt];
-      } else {
-        p.info[(size_t)(s0 + s) * RS_D + wt] = t;
-      }
-    }
-    if (wt == 0) rs_stamp(p, 7);
-  }
-  if constexpr (PAIR) {
-    if (warp < 2) {                                // the producer / MMA warps take part in the two cluster barriers
-      __syncwarp();
-      cluster_barrier();
-      cluster_barrier();
-    }
-  }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// =====================================================================================================================
-// cta_group::2 form of the PAIR case: the two CTAs of a sample's cluster issue ONE tcgen05.mma per k-step (M = 256: rank r
-// contributes its 128 rows, N = 256 per output half), so each CTA stages only HALF of every weight tile -- 512 KB instead
-// of 1 MB of L2 -> SM traffic per CTA and step (the chip-wide L2 read rate, ~6300 B/clk, is what bounds the 1-CTA form:
-// 128 CTAs x 1.4 MB per step), and each SM's shared memory feeds 8 KB instead of 12 KB per MMA (SS-mode operand limit).
-//   * A tiles (own 128 rows of P) land on the CTA's OWN a_full barrier, are scaled by its own workers, and every worker
-//     warp of BOTH CTAs arrives on the LEADER's a_ready (32 arrivals, release/acquire at cluster scope).
-//   * B half tiles ([128 x 64] of the [256 x 64] block: rows 256 h + 128 rank) complete on the LEADER's b_full
-//     (cp.async.bulk.tensor ... .cta_group::2); the leader's tcgen05.commit multicasts to both CTAs' empty barriers.
-//   * H stays local (each CTA's 128 rows); hk_ready on the leader counts both CTAs' warps.
-// Shared memory: GEMM 1 = 4 stages x (A | B half 0 | B half 1) over units 0..11; H over units 0..7; GEMM 2 streams Wm2
-// through 5 single-unit slots (units 8..12).  Unit 12 is outside the GEMM-1 ring, so the FIRST Wm2 tile is requested at
-// kernel start: a tensor map's first use costs a ~4.5k-clock descriptor fetch (measured: GEMM 2's first MMA was issued
-// 5.9k clocks after GEMM 1 completed), which this hides; the other slots are filled once GEMM 1 is complete.
-// Whole-step form (p.Wy_t != NULL): while the first TMA requests wait ~6k clocks for their tensor-map descriptors, the
-// workers compute, per sample, the previous step's write unit m = [m_prev, info_prev] @ Ww + bw (mac_cell.py:339-352,
-// plain form) and this step's memory projection y = m @ Wy + by (ops.py:689) as two matrix-vector products against bf16
-// weights (fp32 activations and accumulation), each CTA half of the outputs, exchanged through distributed shared
-// memory.  A reasoning step is then ONE launch: no separate write / projY kernels, and y never exists in HBM.
-// Tail: ONE cluster barrier -- rank 1 ships its local softmax statistics, its un-normalised exp values and its
-// un-normalised partial weighted sum to rank 0, which combines and writes att / info for the whole sample.
-// =====================================================================================================================
-constexpr int RS2_STAGES = 4;
-constexpr int RS2_B2_SLOTS = 5;
-constexpr int RS2_SMEM_BYTES = RS_UNITS * RS_UNIT + 1024 /*align*/ + 512 /*barriers*/ + RS_PAR_FLOATS * 4 + 4 * 128 * 4 +
-                               128 * 4 + 64 + RS_D * 4 + 128 * 4 /*partner's exp values*/;
-
-// arrive on the barrier at the same offset in CTA `cta` of the cluster.  Default semantics (release at CTA scope), as
-// CUTLASS's ClusterBarrier::arrive(cta_id): the data the barrier guards is this CTA's OWN shared memory, published to the
-// async proxy by fence.proxy.async before the arrive and read by the pair's tcgen05.mma -- an explicit .release.cluster
-// costs a cluster-scope fence (L1 invalidate) per arrive and made the 2-CTA form slower than the 1-CTA one (52k vs 44k clk).
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+__device__ __forceinline__ void wgmma_bf16_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
   asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
 }
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
-
-__global__ void __launch_bounds__(RS_THREADS, 1)
-read_step2_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constant__ CUtensorMap map_w1,
-                  const __grid_constant__ CUtensorMap map_w2, const ReadStepParams p) {
-  extern __shared__ unsigned char smem_dyn[];
-  const uint32_t base_u32 = smem_u32(smem_dyn);
-  const uint32_t pad = (1024u - (base_u32 & 1023u)) & 1023u;
-  unsigned char* tiles = smem_dyn + pad;
-  unsigned char* h_tile = tiles;                                 // units 0..7 (after GEMM 1)
-  unsigned char* b2_slots = tiles + 8 * RS_UNIT;                 // units 8..12
-  uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + RS_UNITS * RS_UNIT);
-  uint64_t* a_full = bars;                         // [4] own:    TMA A -> own workers
-  uint64_t* a_ready = bars + 4;                    // [4] leader: workers of both CTAs -> MMA (32 arrivals)
-  uint64_t* b_full = bars + 8;                     // [4] leader: B halves of both CTAs -> MMA
-  uint64_t* s_empty = bars + 12;                   // [4] own:    MMA (multicast commit) -> TMA
-  uint64_t* b2_full = bars + 16;                   // [5] leader
-  uint64_t* b2_empty = bars + 21;                  // [5] own
-  uint64_t* g1_done = bars + 26;                   // own (multicast commit)
-  uint64_t* hk_ready = bars + 27;                  // [8] leader (32 arrivals)
-  uint64_t* g2_done = bars + 35;                   // [2] own (multicast commit)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 37);
-  uint64_t* xm_ready = bars + 40;                  // own: both CTAs' halves of the new memory are in s_m (32 warp arrivals)
-  uint64_t* xy_ready = bars + 41;                  // own: both halves of y are in s_y
-  float* par = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(bars) + 512);
-  float* s_part = par + RS_PAR_FLOATS;
-  float* s_att = s_part + 4 * 128;
-  float* s_xch = s_att + 128;
-  float* s_peer = s_xch + 16;                      // [512] rank 1's un-normalised partial weighted sum (read by rank 0)
-  float* s_peer_e = s_peer + RS_D;                 // [128] rank 1's un-normalised exp values (read by rank 0)
-  float* s_red = reinterpret_cast<float*>(tiles + 9 * RS_UNIT);          // [8][512] over units 9..12 (after GEMM 2)
-  float* s_m = s_peer;                             // [512] prologue only: this step's memory (s_peer is used by the tail)
-  float* s_y = s_part;                             // [512] prologue + GEMM 1: y (s_part is used from epilogue 2 on)
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int N = p.N;
-  const uint32_t rank = cluster_rank();
-  const bool packed = p.packed != 0;
-  // per-sample form: pair = sample, rank = its row half.  packed form: CTA = 128 consecutive rows of [B*N, d]
-  const int row0 = packed ? (int)blockIdx.x * 128 : (int)(blockIdx.x >> 1) * N + (int)rank * 128;
-  const int valid = packed ? max(0, min(128, p.B * N - row0)) : min(128, N - (int)rank * 128);
-  const int s0 = packed ? min(row0 / N, p.B - 1) : (int)(blockIdx.x >> 1);      // sample of the tile's first row
-  const int s1 = min(s0 + 1, p.B - 1);                                          // packed: sample of the rows from `bnd` on
-  const int bnd = packed ? max(0, min(valid, (s0 + 1) * N - row0)) : valid;     // rows [0, bnd): s0, [bnd, valid): s1
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_p);
-    tma_prefetch_desc(&map_w1);
-    tma_prefetch_desc(&map_w2);
-#pragma unroll
-    for (int i = 0; i < RS2_STAGES; ++i) {
-      mbar_init(&a_full[i], 1);
-      mbar_init(&a_ready[i], 2 * RS_WORKER_WARPS);
-      mbar_init(&b_full[i], 1);
-      mbar_init(&s_empty[i], 1);
-    }
-#pragma unroll
-    for (int i = 0; i < RS2_B2_SLOTS; ++i) {
-      mbar_init(&b2_full[i], 1);
-      mbar_init(&b2_empty[i], 1);
-    }
-    mbar_init(g1_done, 1);
-#pragma unroll
-    for (int i = 0; i < RS_KB; ++i) mbar_init(&hk_ready[i], 2 * RS_WORKER_WARPS);
-    mbar_init(&g2_done[0], 1);
-    mbar_init(&g2_done[1], 1);
-    mbar_init(xm_ready, 2 * RS_WORKER_WARPS);
-    mbar_init(xy_ready, 2 * RS_WORKER_WARPS);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc2(tmem_ptr, 512);
-  tc_fence_before();
-  __syncthreads();
-  cluster_barrier();                               // #0: both CTAs' barriers and tensor memory exist
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ===================================================== TMA producer (both CTAs)
-    if (elect_one()) {
-      auto issue_stage = [&](int kb) {
-        const int s = kb % RS2_STAGES, n = kb / RS2_STAGES;
-        unsigned char* st = tiles + s * 3 * RS_UNIT;
-        mbar_wait(&s_empty[s], (n & 1) ^ 1);
-        rs_stamp(p, 16 + kb);                      // stage free: loads of k-block kb issued
-        mbar_expect_tx(&a_full[s], RS_UNIT);
-        tma_load_2d(st, &map_p, kb * TC_BK, row0, &a_full[s]);
-        if (p.dbg_flags & 4) {
-          if (rank == 0) mbar_arrive(&b_full[s]);
-        } else {
-          if (rank == 0) mbar_expect_tx(&b_full[s], 4 * RS_UNIT);      // two halves from each of the two CTAs
-          tma2_load_2d(st + RS_UNIT, &map_w1, kb * TC_BK, (int)rank * 128, &b_full[s]);
-          tma2_load_2d(st + 2 * RS_UNIT, &map_w1, kb * TC_BK, 256 + (int)rank * 128, &b_full[s]);
-        }
-      };
-      // GEMM-2 tile i = (half h = i / 8, k-block i % 8) goes to slot (i + 4) % 5, i.e. tile 0 to unit 12
-      auto issue_w2 = [&](int i) {
-        const int h = i >> 3, kb = i & 7;
-        const int sl = (i + 4) % RS2_B2_SLOTS, n = i / RS2_B2_SLOTS;
-        mbar_wait(&b2_empty[sl], (n & 1) ^ 1);
-        if (rank == 0) mbar_expect_tx(&b2_full[sl], 2 * RS_UNIT);
-        tma2_load_2d(b2_slots + sl * RS_UNIT, &map_w2, kb * TC_BK, h * 256 + (int)rank * 128, &b2_full[sl]);
-      };
-      for (int kb = 0; kb < RS2_STAGES; ++kb) issue_stage(kb);          // the whole ring first: nothing else delays it
-      issue_w2(0);                                                       // unit 12; also warms the Wm2 descriptor
-      for (int kb = RS2_STAGES; kb < RS_KB; ++kb) issue_stage(kb);
-      mbar_wait(g1_done, 0);                       // the rest of the GEMM-2 ring overlays stages 2 and 3
-      rs_stamp(p, 56);
-      for (int i = 1; i < 2 * RS_KB; ++i) issue_w2(i);
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer (leader CTA only)
-    if (rank == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(256, 256);
-      for (int kb = 0; kb < RS_KB; ++kb) {
-        const int s = kb % RS2_STAGES, n = kb / RS2_STAGES;
-        mbar_wait_cluster(&a_ready[s], n & 1);
-        if (lane == 0) rs_stamp(p, 48 + kb);       // both CTAs' P k-block scaled
-        mbar_wait(&b_full[s], n & 1);
-        tc_fence_after();
-        if (lane == 0) rs_stamp(p, 8 + kb);        // MMAs of k-block kb issued
-        if (elect_one()) {
-          const uint32_t st = smem_u32(tiles + s * 3 * RS_UNIT);
-          const uint64_t adesc = make_sw128_kmajor_desc(st);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint64_t bdesc = make_sw128_kmajor_desc(st + (1 + h) * RS_UNIT);
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k)
-              if (!(p.dbg_flags & 2)) umma2_bf16(tmem_base + h * 256, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          }
-          umma2_commit_mc(&s_empty[s], 0x3);
-          if (kb == RS_KB - 1) umma2_commit_mc(g1_done, 0x3);
-        }
-        __syncwarp();
-      }
-      for (int i = 0; i < 2 * RS_KB; ++i) {
-        const int h = i >> 3, kb = i & 7;
-        const int sl = (i + 4) % RS2_B2_SLOTS, n = i / RS2_B2_SLOTS;
-        if (h == 0) {                              // H hand-over groups {0..3}, {4, 5}, {6, 7}
-          if (kb == 0) mbar_wait_cluster(&hk_ready[0], 0);
-          else if (kb == 4) mbar_wait_cluster(&hk_ready[1], 0);
-          else if (kb == 6) mbar_wait_cluster(&hk_ready[2], 0);
-        }
-        mbar_wait(&b2_full[sl], n & 1);
-        tc_fence_after();
-        if (lane == 0) rs_stamp(p, 32 + i);        // GEMM-2 MMAs of (half, k-block) i issued
-        if (elect_one()) {
-          const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(h_tile + kb * RS_UNIT));
-          const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(b2_slots + sl * RS_UNIT));
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)
-            if (!(p.dbg_flags & 2)) umma2_bf16(tmem_base + h * 256, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          umma2_commit_mc(&b2_empty[sl], 0x3);
-          if (kb == RS_KB - 1) umma2_commit_mc(&g2_done[h], 0x3);
-        }
-        __syncwarp();
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================================================== workers (both CTAs; own 128 rows)
-    const int wt = threadIdx.x - 64;
-    const int q = warp & 3;
-    const int cg = (warp - 2) >> 2;
-    const int row = q * 32 + lane;
-    if (wt == 0) rs_stamp(p, 0);
-    for (int i = wt; i < RS_D; i += RS_WORKERS) {
-      par[i] = __ldg(p.bm2 + i);
-      par[RS_D + i] = __ldg(p.wr + i);
-      par[2 * RS_D + i] = __ldg(p.ctrl + (size_t)s0 * RS_D + i);
-      par[3 * RS_D + i] = __ldg(p.ctrl + (size_t)s1 * RS_D + i);
-    }
-    const bool row_ok = row < valid;
-    const int wi = warp - 2;
-    // ---- whole-step prologue: write unit of the previous step + memory projection of this one (see the header comment)
-    if (p.Wy_t) {
-      const int nbase = (int)rank * 256 + wi * 16;                 // this warp's 16 output columns
-      // dot of a bf16 weight row segment with fp32 x held in registers: NV = uint4 loads per lane (8 elements each)
-      auto dot8 = [](const uint4 w, const float* x) {
-        float a = bf16lo(w.x) * x[0];
-        a = fmaf(bf16hi(w.x), x[1], a);
-        a = fmaf(bf16lo(w.y), x[2], a); a = fmaf(bf16hi(w.y), x[3], a);
-        a = fmaf(bf16lo(w.z), x[4], a); a = fmaf(bf16hi(w.z), x[5], a);
-        a = fmaf(bf16lo(w.w), x[6], a); a = fmaf(bf16hi(w.w), x[7], a);
-        return a;
-      };
-      if (p.info_prev) {
-        // m[n] = sum_k [m_prev, info_prev][k] * Ww[k, n] + bw[n]; lane l holds x[32 l, 32 l + 32) (lanes 0..15: m_prev)
-        float x[32];
-        {
-          const float* src = (lane < 16 ? p.mem_prev : p.info_prev) + (size_t)s0 * RS_D + (lane & 15) * 32;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 f = __ldg(reinterpret_cast<const float4*>(src) + i);
-            x[4 * i] = f.x; x[4 * i + 1] = f.y; x[4 * i + 2] = f.z; x[4 * i + 3] = f.w;
-          }
-        }
-        float mine = 0.f;
-#pragma unroll 1
-        for (int j = 0; j < 16; j += 2) {
-          const __nv_bfloat16* r0 = p.Ww_t + (size_t)(nbase + j) * (2 * RS_D) + lane * 32;
-          const __nv_bfloat16* r1 = r0 + 2 * RS_D;
-          uint4 w0[4], w1[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) { w0[i] = ldg_nc_v4(r0 + 8 * i); w1[i] = ldg_nc_v4(r1 + 8 * i); }
-          float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) { a0 += dot8(w0[i], x + 8 * i); a1 += dot8(w1[i], x + 8 * i); }
-          a0 = warp_sum(a0);
-          a1 = warp_sum(a1);
-          if (lane == j) mine = a0;
-          if (lane == j + 1) mine = a1;
-        }
-        if (lane < 16) {
-          const float v_ = mine + __ldg(p.bw + nbase + lane);
-          s_m[nbase + lane] = v_;
-          st_cluster_f32(&s_m[nbase + lane], rank ^ 1u, v_);
-          p.mem_out[(size_t)s0 * RS_D + nbase + lane] = v_;
-        }
-      } else {
-        s_m[wt] = __ldg(p.mem_prev + (size_t)s0 * RS_D + wt);       // first step: the memory is given; both CTAs load all of it
-      }
-      if (p.info_prev) {
-        __syncwarp();
-        if (lane == 0) {
-          asm volatile("mbarrier.arrive.release.cluster.shared::cta.b64 _, [%0];" ::"r"(smem_u32(xm_ready)) : "memory");
-          asm volatile(
-              "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-              "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(xm_ready)), "r"(rank ^ 1u) : "memory");
-        }
-        uint32_t ok;
-        do {
-          asm volatile(
-              "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-              "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(smem_u32(xm_ready)), "r"(0u) : "memory");
-        } while (!ok);
-      } else {
-        rs_worker_bar();
-      }
-      {
-        // y[n] = sum_k m[k] * Wy[k, n] + by[n]; lane l holds m[16 l, 16 l + 16)
-        float x[16];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 f = *reinterpret_cast<const float4*>(s_m + lane * 16 + 4 * i);
-          x[4 * i] = f.x; x[4 * i + 1] = f.y; x[4 * i + 2] = f.z; x[4 * i + 3] = f.w;
-        }
-        float mine = 0.f;
-#pragma unroll 1
-        for (int j = 0; j < 16; j += 4) {
-          uint4 w_[4][2];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const __nv_bfloat16* r = p.Wy_t + (size_t)(nbase + j + u) * RS_D + lane * 16;
-            w_[u][0] = ldg_nc_v4(r);
-            w_[u][1] = ldg_nc_v4(r + 8);
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const float a = warp_sum(dot8(w_[u][0], x) + dot8(w_[u][1], x + 8));
-            if (lane == j + u) mine = a;
-          }
-        }
-        if (lane < 16) {
-          const float v_ = mine + __ldg(p.by + nbase + lane);
-          s_y[nbase + lane] = v_;
-          st_cluster_f32(&s_y[nbase + lane], rank ^ 1u, v_);
-        }
-        __syncwarp();
-        if (lane == 0) {
-          asm volatile("mbarrier.arrive.release.cluster.shared::cta.b64 _, [%0];" ::"r"(smem_u32(xy_ready)) : "memory");
-          asm volatile(
-              "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-              "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(xy_ready)), "r"(rank ^ 1u) : "memory");
-        }
-        uint32_t ok;
-        do {
-          asm volatile(
-              "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-              "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(smem_u32(xy_ready)), "r"(0u) : "memory");
-        } while (!ok);
-      }
-      if (wt == 0) rs_stamp(p, 57);                // y ready
-    }
-    const __nv_bfloat16* qrow = p.Q + (size_t)(row_ok ? row0 + row : 0) * RS_D + cg * 16;
-    uint4 qv[8];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      qv[2 * i] = ldg_nc_v4(qrow + 64 * i);
-      qv[2 * i + 1] = ldg_nc_v4(qrow + 64 * i + 8);
-    }
-    // ---- GEMM 1 operand path: own P k-block -> P * y_b in place (see read_step_kernel)
-    {
-      const int r_a = wt >> 3, r_b = r_a + 64;
-      const int pc = wt & 7;
-      const int lc_a = pc ^ (r_a & 7), lc_b = pc ^ (r_b & 7);
-      const bool ok_a = r_a < valid, ok_b = r_b < valid;
-      const float* y_a = (p.Wy_t ? s_y : p.y + (size_t)(r_a < bnd ? s0 : s1) * RS_D) + lc_a * 8;
-      const float* y_b = (p.Wy_t ? s_y : p.y + (size_t)(r_b < bnd ? s0 : s1) * RS_D) + lc_b * 8;
-      auto scale16 = [](uint4 v, const float4 f0, const float4 f1) {
-        uint4 o;
-        o.x = pack_bf16(bf16lo(v.x) * f0.x, bf16hi(v.x) * f0.y);
-        o.y = pack_bf16(bf16lo(v.y) * f0.z, bf16hi(v.y) * f0.w);
-        o.z = pack_bf16(bf16lo(v.z) * f1.x, bf16hi(v.z) * f1.y);
-        o.w = pack_bf16(bf16lo(v.w) * f1.z, bf16hi(v.w) * f1.w);
-        return o;
-      };
-      for (int kb = 0; kb < RS_KB; ++kb) {
-        const int s = kb % RS2_STAGES, n = kb / RS2_STAGES;
-        const float4 ya0 = *reinterpret_cast<const float4*>(y_a + kb * TC_BK);
-        const float4 ya1 = *reinterpret_cast<const float4*>(y_a + kb * TC_BK + 4);
-        const float4 yb0 = *reinterpret_cast<const float4*>(y_b + kb * TC_BK);
-        const float4 yb1 = *reinterpret_cast<const float4*>(y_b + kb * TC_BK + 4);
-        mbar_wait(&a_full[s], n & 1);
-        if (wt == 0) rs_stamp(p, 24 + kb);         // own P k-block landed
-        uint4* t = reinterpret_cast<uint4*>(tiles + s * 3 * RS_UNIT);
-        if (!(p.dbg_flags & 1)) {
-          if (ok_a) t[wt] = scale16(t[wt], ya0, ya1);
-          if (ok_b) t[wt + 512] = scale16(t[wt + 512], yb0, yb1);
-          fence_proxy_async();
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(&a_ready[s], 0u);
-        // The tiles this CTA reads later with plain loads are started towards L2 from here, NOT at kernel start: with the
-        // inputs of 6+ passes in flight nothing is L2-resident, and at kernel start these requests competed with the first
-        // P tiles for HBM (GEMM-1 feed 25k clocks cold vs 13.6k warm).  Q (epilogue 1) after k-block 1, KB (tail) after 5.
-        if ((kb == 1 || kb == 5) && wt < 8) {
-          const size_t bytes = (size_t)valid * RS_D * 2;
-          const char* base = reinterpret_cast<const char*>((kb == 1 ? p.Q : p.kb) + (size_t)row0 * RS_D);
-          const size_t o = (size_t)wt * 16384;
-          if (o < bytes) l2_prefetch_bulk(base + o, (uint32_t)min((size_t)16384, bytes - o));
-        }
-      }
-    }
-
-    // ---- epilogue 1
-    const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16);
-    if (wt == 0) rs_stamp(p, 1);
-    mbar_wait(g1_done, 0);
-    tc_fence_after();
-    if (wt == 0) rs_stamp(p, 2);
-    // H k-blocks are handed to the MMA warp in three groups -- {0..3} (GEMM 2 cannot start earlier: its first MMA overwrites
-    // the accumulator columns of exactly these), {4, 5}, {6, 7} -- so each warp pays 3 proxy fences + arrives, not 8; the
-    // tensor-memory load of k-block i+1 is issued before k-block i is processed.
-    {
-      uint32_t rn[16];
-      tmem_ld16(tlane + cg * 16, rn);
-#pragma unroll
-      for (int kb2 = 0; kb2 < RS_KB; ++kb2) {
-        uint32_t r[16];
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 16; ++j) r[j] = rn[j];
-        if (kb2 + 1 < RS_KB) tmem_ld16(tlane + (kb2 + 1) * 64 + cg * 16, rn);
-        const uint4 qa = qv[(2 * kb2) & 7], qb = qv[(2 * kb2 + 1) & 7];
-        if (kb2 < 4) {
-          qv[(2 * kb2) & 7] = ldg_nc_v4(qrow + 64 * (kb2 + 4));
-          qv[(2 * kb2 + 1) & 7] = ldg_nc_v4(qrow + 64 * (kb2 + 4) + 8);
-        }
-        const uint32_t qw[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
-        uint32_t w[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          w[j] = pack_bf16(elu_fast(__uint_as_float(r[2 * j]) + bf16lo(qw[j])),
-                           elu_fast(__uint_as_float(r[2 * j + 1]) + bf16hi(qw[j])));
-        const int lc = cg * 2;
-        unsigned char* hrow = h_tile + kb2 * RS_UNIT + row * 128;
-        *reinterpret_cast<uint4*>(hrow + ((lc ^ (row & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-        *reinterpret_cast<uint4*>(hrow + (((lc + 1) ^ (row & 7)) << 4)) = make_uint4(w[4], w[5], w[6], w[7]);
-        if (kb2 == 3 || kb2 == 5 || kb2 == 7) {
-          fence_proxy_async();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster(&hk_ready[kb2 == 3 ? 0 : (kb2 == 5 ? 1 : 2)], 0u);
-        }
-      }
-    }
-    if (wt == 0) rs_stamp(p, 3);
-
-    // ---- epilogue 2
-    rs_worker_bar();
-    const float* crow = par + (row < bnd ? 2 : 3) * RS_D;          // this row's sample's control state
-    float part = 0.f;
-#pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
-      mbar_wait(&g2_done[h], 0);
-      tc_fence_after();
-      if (wt == 0 && h == 1) rs_stamp(p, 4);
-      uint32_t rn[16];
-      tmem_ld16(tlane + h * 256 + cg * 64, rn);
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t r[16];
-        const int c0 = h * 256 + cg * 64 + 16 * ch;
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 16; ++j) r[j] = rn[j];
-        if (ch + 1 < 4) tmem_ld16(tlane + c0 + 16, rn);
-        const float4* b4 = reinterpret_cast<const float4*>(par + c0);
-        const float4* w4 = reinterpret_cast<const float4*>(par + RS_D + c0);
-        const float4* c4 = reinterpret_cast<const float4*>(crow + c0);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 bb = b4[j], ww = w4[j], cc = c4[j];
-          part = fmaf(elu_fast((__uint_as_float(r[4 * j]) + bb.x) * cc.x), ww.x, part);
-          part = fmaf(elu_fast((__uint_as_float(r[4 * j + 1]) + bb.y) * cc.y), ww.y, part);
-          part = fmaf(elu_fast((__uint_as_float(r[4 * j + 2]) + bb.z) * cc.z), ww.z, part);
-          part = fmaf(elu_fast((__uint_as_float(r[4 * j + 3]) + bb.w) * cc.w), ww.w, part);
-        }
-      }
-    }
-    tc_fence_before();
-    s_part[cg * 128 + row] = part;
-    rs_worker_bar();
-    if (wt < 128) s_att[wt] = s_part[wt] + s_part[128 + wt] + s_part[256 + wt] + s_part[384 + wt] + p.br;
-    rs_worker_bar();
-    if (wt == 0) rs_stamp(p, 5);
-
-    // ---- knowledge-base rows of the weighted sum (issued before the softmax, consumed after it)
-    const int nrows = valid;
-    const int rg = wt >> 6, cq = wt & 63;
-    uint4 v[16];
-    {
-      const __nv_bfloat16* kbase = p.kb + (size_t)row0 * RS_D + cq * 8;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int n = rg + RS_RED_GROUPS * i;
-        v[i] = n < nrows ? ldg_nc_v4(kbase + (size_t)n * RS_D) : make_uint4(0u, 0u, 0u, 0u);
-      }
-    }
-    if (packed) {
-      // ---- packed tail: up to two row segments (samples s0, s0 + 1); warp 0 / warp 1 form the local maximum, the exp values
-      //      and their sum of segment 0 / 1, then one weighted-sum pass per non-empty segment; no pair exchange at all.
-      if (wi < 2) {
-        const int lo = wi == 0 ? 0 : bnd, hi = wi == 0 ? bnd : valid;
-        float e_lane[4] = {0.f, 0.f, 0.f, 0.f};
-        float mx = -INFINITY, sum = 0.f;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int n = lane + 32 * i;
-          if (n >= lo && n < hi) mx = fmaxf(mx, s_att[n]);
-        }
-        mx = warp_max(mx);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int n = lane + 32 * i;
-          if (n >= lo && n < hi) {
-            e_lane[i] = __expf(s_att[n] - mx);
-            sum += e_lane[i];
-          }
-        }
-        sum = warp_sum(sum);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int n = lane + 32 * i;
-          if (n >= lo && n < hi) s_att[n] = e_lane[i];
-        }
-        if (lane == 0) {
-          s_xch[2 * wi] = mx;
-          s_xch[2 * wi + 1] = sum;
-        }
-      }
-      rs_worker_bar();
-      if (wt == 0) rs_stamp(p, 6);
-      if (wt < valid) p.att[(size_t)row0 + wt] = s_att[wt];        // exp values; the combine kernel scales them by c_r / Z
-      // both segments' weighted sums in ONE pass over the KB rows held in registers (each row's weight goes to the
-      // accumulators of its own segment, the other set gets an exact zero), into two [8][512] reduction slabs (units 9, 10)
-      {
-        float accA[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        float accB[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int n = rg + RS_RED_GROUPS * i;
-          const float a = n < valid ? s_att[n] : 0.f;
-          const float aA = n < bnd ? a : 0.f, aB = n < bnd ? 0.f : a;
-          const float k0 = bf16lo(v[i].x), k1 = bf16hi(v[i].x), k2 = bf16lo(v[i].y), k3 = bf16hi(v[i].y);
-          const float k4 = bf16lo(v[i].z), k5 = bf16hi(v[i].z), k6 = bf16lo(v[i].w), k7 = bf16hi(v[i].w);
-          accA[0] = fmaf(aA, k0, accA[0]); accA[1] = fmaf(aA, k1, accA[1]); accA[2] = fmaf(aA, k2, accA[2]);
-          accA[3] = fmaf(aA, k3, accA[3]); accA[4] = fmaf(aA, k4, accA[4]); accA[5] = fmaf(aA, k5, accA[5]);
-          accA[6] = fmaf(aA, k6, accA[6]); accA[7] = fmaf(aA, k7, accA[7]);
-          accB[0] = fmaf(aB, k0, accB[0]); accB[1] = fmaf(aB, k1, accB[1]); accB[2] = fmaf(aB, k2, accB[2]);
-          accB[3] = fmaf(aB, k3, accB[3]); accB[4] = fmaf(aB, k4, accB[4]); accB[5] = fmaf(aB, k5, accB[5]);
-          accB[6] = fmaf(aB, k6, accB[6]); accB[7] = fmaf(aB, k7, accB[7]);
-        }
-        float4* dst = reinterpret_cast<float4*>(s_red + rg * RS_D + cq * 8);
-        dst[0] = make_float4(accA[0], accA[1], accA[2], accA[3]);
-        dst[1] = make_float4(accA[4], accA[5], accA[6], accA[7]);
-        dst += RS_RED_GROUPS * RS_D / 4;
-        dst[0] = make_float4(accB[0], accB[1], accB[2], accB[3]);
-        dst[1] = make_float4(accB[4], accB[5], accB[6], accB[7]);
-      }
-      rs_worker_bar();
-#pragma unroll 1
-      for (int seg = 0; seg < 2; ++seg) {
-        if ((seg == 0 ? bnd : valid - bnd) <= 0) continue;
-        float t = 0.f;
-#pragma unroll
-        for (int g = 0; g < RS_RED_GROUPS; ++g) t += s_red[(seg * RS_RED_GROUPS + g) * RS_D + wt];
-        const int smp = seg == 0 ? s0 : s1;
-        const int slot = (int)blockIdx.x - (smp * N) / 128;        // 0 .. 2: this tile's position among the sample's tiles
-        p.part[((size_t)smp * 3 + slot) * RS_D + wt] = t;
-        if (wt == 0) {
-          float* mz = p.part + (size_t)p.B * 3 * RS_D + ((size_t)smp * 3 + slot) * 2;
-          mz[0] = s_xch[2 * seg];
-          mz[1] = s_xch[2 * seg + 1];
-        }
-      }
-      if (wt == 0) rs_stamp(p, 7);
-    } else {
-    // ---- softmax over the sample's N rows, split over the pair: each CTA forms its LOCAL maximum m_r, exp values
-    //      e[n] = exp(l[n] - m_r), their sum z_r and the un-normalised partial I_r = sum_n e[n] KB[n, :]; rank 1 ships
-    //      (m_1, z_1, e_1[], I_1[]) into rank 0's shared memory, ONE cluster barrier, and rank 0 writes
-    //      att[n] = e_r[n] c_r / Z,  info = (c_0 I_0 + c_1 I_1) / Z   with c_r = exp(m_r - max(m_0, m_1)), Z = c_0 z_0 + c_1 z_1.
-    if (wi == 0) {
-      float e_lane[4] = {0.f, 0.f, 0.f, 0.f};
-      float mx = -INFINITY, sum = 0.f;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int n = lane + 32 * i;
-        if (n < nrows) mx = fmaxf(mx, s_att[n]);
-      }
-      mx = warp_max(mx);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int n = lane + 32 * i;
-        if (n < nrows) {
-          e_lane[i] = __expf(s_att[n] - mx);
-          sum += e_lane[i];
-        }
-      }
-      sum = warp_sum(sum);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int n = lane + 32 * i;
-        if (n < nrows) s_att[n] = e_lane[i];
-      }
-      if (lane == 0) {
-        s_xch[2 * rank] = mx;
-        s_xch[2 * rank + 1] = sum;
-      }
-    }
-    rs_worker_bar();
-    if (wt == 0) rs_stamp(p, 6);
-    float t = 0.f;
-    {
-      float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int n = rg + RS_RED_GROUPS * i;
-        const float a = n < nrows ? s_att[n] : 0.f;
-        acc[0] = fmaf(a, bf16lo(v[i].x), acc[0]); acc[1] = fmaf(a, bf16hi(v[i].x), acc[1]);
-        acc[2] = fmaf(a, bf16lo(v[i].y), acc[2]); acc[3] = fmaf(a, bf16hi(v[i].y), acc[3]);
-        acc[4] = fmaf(a, bf16lo(v[i].z), acc[4]); acc[5] = fmaf(a, bf16hi(v[i].z), acc[5]);
-        acc[6] = fmaf(a, bf16lo(v[i].w), acc[6]); acc[7] = fmaf(a, bf16hi(v[i].w), acc[7]);
-      }
-      float4* dst = reinterpret_cast<float4*>(s_red + rg * RS_D + cq * 8);
-      dst[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
-      dst[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
-      rs_worker_bar();
-#pragma unroll
-      for (int g = 0; g < RS_RED_GROUPS; ++g) t += s_red[g * RS_D + wt];
-    }
-    if (rank == 1) {
-      st_cluster_f32(&s_peer[wt], 0u, t);
-      if (wt < nrows) st_cluster_f32(&s_peer_e[wt], 0u, s_att[wt]);
-      if (wt == 0) {
-        st_cluster_f32(&s_xch[2], 0u, s_xch[2]);
-        st_cluster_f32(&s_xch[3], 0u, s_xch[3]);
-      }
-    }
-    cluster_barrier();                             // #1 (the only one of the tail)
-    if (rank == 0) {
-      const float m0 = s_xch[0], z0 = s_xch[1], m1 = s_xch[2], z1 = s_xch[3];
-      const float M = fmaxf(m0, m1);
-      const float c0 = __expf(m0 - M), c1 = __expf(m1 - M);
-      const float rZ = 1.f / (c0 * z0 + c1 * z1);
-      p.info[(size_t)s0 * RS_D + wt] = (c0 * t + c1 * s_peer[wt]) * rZ;
-      if (wt < 128) {
-        if (wt < nrows) p.att[(size_t)s0 * N + wt] = s_att[wt] * c0 * rZ;
-      } else if (wt - 128 < N - 128) {
-        p.att[(size_t)s0 * N + wt] = s_peer_e[wt - 128] * c1 * rZ;
-      }
-    }
-    if (wt == 0) rs_stamp(p, 7);
-    }                                              // !packed
-  }
-  if (warp < 2 && !packed) {                       // the producer / MMA warps take part in the tail's cluster barrier
-    __syncwarp();
-    cluster_barrier();
-  }
-
-  // ---- teardown: neither CTA frees its tensor memory while the pair may still use it
-  tc_fence_before();
-  __syncthreads();
-  cluster_barrier();                               // #3
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, 512);
-  }
-}
-
-// profiling hook (not part of the ABI header): device buffer [grid][8] that subsequent launches fill with clock64 stamps
-inline long long*& read_step_dbg_ptr() { static long long* p = nullptr; return p; }
-inline int& read_step_dbg_flags() { static int f = 0; return f; }
-
-// can the fused kernel take this shape?
+// can the read step take this shape?
 inline bool read_step_supported(int B, int N, int d) { return d == RS_D && N >= 1 && N <= 256 && B >= 1; }
 
-// Packed form: merge the per-tile softmax partials of every sample (read_step2_kernel, `packed`).  Sample s owns tiles
-// first = floor(s N / 128) .. last = floor((s N + N - 1) / 128) (2 or 3 of them for 128 < N <= 256); with the local maxima m_r,
-// sums z_r and un-normalised partial sums I_r:  M = max m_r, c_r = exp(m_r - M), Z = sum c_r z_r,
-//   info[s, :] = sum_r c_r I_r / Z ,   att[s, n] = e[n] * c_{r(n)} / Z   (e[n] left in `att` by the tile that owns row n).
-// grid B, RS_D threads.
-__global__ void __launch_bounds__(RS_D) read_step_combine_kernel(const float* __restrict__ part, float* __restrict__ att,
-                                                                float* __restrict__ info, int B, int N) {
-  const int s = blockIdx.x, k = threadIdx.x;
-  const int first = (s * N) / 128, last = (s * N + N - 1) / 128;
-  const int ns = last - first + 1;                                 // <= 3
-  const float* mz = part + (size_t)B * 3 * RS_D + (size_t)s * 3 * 2;
-  float m[3], c[3];
-  float M = -INFINITY;
-#pragma unroll
-  for (int r = 0; r < 3; ++r) {
-    m[r] = r < ns ? mz[2 * r] : -INFINITY;
-    M = fmaxf(M, m[r]);
-  }
-  float Z = 0.f;
-#pragma unroll
-  for (int r = 0; r < 3; ++r) {
-    c[r] = r < ns ? __expf(m[r] - M) : 0.f;
-    if (r < ns) Z = fmaf(c[r], mz[2 * r + 1], Z);
-  }
-  const float rZ = 1.f / Z;
-  float acc = 0.f;
-#pragma unroll
-  for (int r = 0; r < 3; ++r)
-    if (r < ns) acc = fmaf(c[r], part[((size_t)s * 3 + r) * RS_D + k], acc);
-  info[(size_t)s * RS_D + k] = acc * rZ;
-  for (int n = k; n < N; n += RS_D) {
-    const int r = (s * N + n) / 128 - first;
-    att[(size_t)s * N + n] *= c[r] * rZ;
-  }
-}
-
-inline size_t read_step_partial_bytes(int B) { return (size_t)B * 3 * (RS_D + 2) * sizeof(float) + 1024; }
-
-// inv = [P | Q] (tc_read_invariant); y, control [B, d] fp32; att [B, N], info [B, d]
-// whole-step form: the write unit of the previous step and this step's memory projection in the kernel's prologue
+// whole-step form: the write unit of the previous step and this step's memory projection run in the kernel's prologue
 struct WholeStepArgs {
   const float* mem_prev;
-  const float* info_prev;           // NULL on the first step
+  const float* info_prev;           // NULL on the first step (the memory is then mem_prev itself)
   const void* Ww_t_bf16;            // [d, 2d] bf16 (mac_pack_weight_bf16 of write/newMemory)
   const float* bw;
   const void* Wy_t_bf16;            // [d, d] bf16 (mac_pack_weight_bf16 of projY)
   float* mem_out;
 };
-inline bool whole_step_supported(int B, int N, int d) {
-  static const bool pair_mma = !(getenv("MAC_READ_PAIR_MMA") && atoi(getenv("MAC_READ_PAIR_MMA")) == 0);
-  return read_step_supported(B, N, d) && N > 128 && pair_mma;
+inline bool whole_step_supported(int B, int N, int d) { return read_step_supported(B, N, d) && N > 128; }
+
+struct ReadStepParams {
+  int M, N;
+  const float* y;                   // [B, d] memory projection, or NULL in the whole-step form
+  const float* ctrl;                // [B, d]
+  const float* bm2;                 // [d]
+  const float* wr;                  // [d]
+  const __nv_bfloat16* Q;           // [B*N, d]  P @ Wm[d:2d] + bm
+  float* logits;                    // [B*N]  I2 . wr (without br)
+  const float* mem_prev;            // whole-step form (see WholeStepArgs); Wy_t == NULL otherwise
+  const float* info_prev;
+  const __nv_bfloat16* Ww_t;
+  const float* bw;
+  const __nv_bfloat16* Wy_t;
+  const float* by;
+  float* mem_out;
+};
+
+// sum_k x[k] * W_t[n, k] over K (K % 256 == 0), one warp per output column
+__device__ __forceinline__ float bf16_row_dot(const __nv_bfloat16* row, const float* x, int K, int lane) {
+  float a = 0.f;
+  for (int k = lane * 8; k < K; k += 256) {
+    const uint4 w = ldg_nc_v4(row + k);
+    a = fmaf(bf16lo(w.x), x[k], a);     a = fmaf(bf16hi(w.x), x[k + 1], a);
+    a = fmaf(bf16lo(w.y), x[k + 2], a); a = fmaf(bf16hi(w.y), x[k + 3], a);
+    a = fmaf(bf16lo(w.z), x[k + 4], a); a = fmaf(bf16hi(w.z), x[k + 5], a);
+    a = fmaf(bf16lo(w.w), x[k + 6], a); a = fmaf(bf16hi(w.w), x[k + 7], a);
+  }
+  return warp_sum(a);
 }
 
+__device__ __forceinline__ void rs_consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(RS_CONSUMERS) : "memory"); }
+
+__global__ void __launch_bounds__(RS_THREADS, 1)
+read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constant__ CUtensorMap map_w1,
+                 const __grid_constant__ CUtensorMap map_w2, const ReadStepParams p) {
+  extern __shared__ unsigned char smem_dyn[];
+  const uint32_t base_u32 = smem_u32(smem_dyn);
+  unsigned char* a_tile = smem_dyn + ((1024u - (base_u32 & 1023u)) & 1023u);
+  unsigned char* b_ring = a_tile + RS_A_BYTES;
+  uint64_t* a_full = reinterpret_cast<uint64_t*>(b_ring + RS_STAGES * RS_STAGE);
+  uint64_t* full = a_full + 1;                     // [STAGES] TMA -> consumers
+  uint64_t* empty = full + RS_STAGES;              // [STAGES] consumers -> TMA (8 warp arrivals)
+  float* s_lg = reinterpret_cast<float*>(a_full + 8);       // [2][64] logit halves
+  float* s_y = s_lg + 2 * RS_BM;                             // [2][d] y of the samples of the whole-step form
+  float* s_m = s_y + 2 * RS_D;                               // [2][d] m
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int row0 = blockIdx.x * RS_BM;
+  const int s_lo = row0 / p.N;                               // first sample of the tile
+
+  if (threadIdx.x == RS_CONSUMERS) {
+    tma_prefetch_desc(&map_p);
+    tma_prefetch_desc(&map_w1);
+    tma_prefetch_desc(&map_w2);
+    mbar_init(a_full, 1);
+    for (int i = 0; i < RS_STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], RS_CONSUMERS / 32);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp == RS_CONSUMERS / 32) {
+    // ===================================================== TMA producer
+    if (elect_one()) {
+      mbar_expect_tx(a_full, RS_A_BYTES);
+      for (int kb = 0; kb < RS_KB; ++kb) tma_load_2d(a_tile + kb * RS_BLK, &map_p, kb * TC_BK, row0, a_full);
+      for (int j = 0; j < 2 * RS_KB; ++j) {
+        const int s = j % RS_STAGES;
+        mbar_wait(&empty[s], ((j / RS_STAGES) & 1) ^ 1);
+        mbar_expect_tx(&full[s], RS_STAGE);
+        const CUtensorMap* m = j < RS_KB ? &map_w1 : &map_w2;
+        const int k0 = (j % RS_KB) * TC_BK;
+        unsigned char* dst = b_ring + s * RS_STAGE;
+        tma_load_2d(dst, m, k0, 0, &full[s]);
+        tma_load_2d(dst + RS_B_HALF, m, k0, 256, &full[s]);
+      }
+    }
+    return;
+  }
+
+  // ===================================================== consumers
+  const int tid = threadIdx.x;
+  const int last_row = min(p.M, row0 + RS_BM) - 1;
+  const float* y_src = p.y;
+  if (p.Wy_t) {
+    const int nsamp = last_row / p.N - s_lo + 1;
+    for (int q = 0; q < nsamp; ++q) {
+      const int s = s_lo + q;
+      float* m = s_m + q * RS_D;
+      if (p.info_prev) {
+        // m[n] = [m_prev, info_prev] . Ww_t[n, :] + bw[n]: x read straight from global (2d floats, L1-resident)
+        const float* mp = p.mem_prev + (size_t)s * RS_D;
+        const float* ip = p.info_prev + (size_t)s * RS_D;
+        for (int n = warp; n < RS_D; n += RS_CONSUMERS / 32) {
+          const __nv_bfloat16* row = p.Ww_t + (size_t)n * 2 * RS_D;
+          float a = 0.f;
+          for (int k = lane * 8; k < 2 * RS_D; k += 256) {
+            const uint4 w = ldg_nc_v4(row + k);
+            const float* x = k < RS_D ? mp + k : ip + (k - RS_D);
+            const float4 x0 = __ldg(reinterpret_cast<const float4*>(x)), x1 = __ldg(reinterpret_cast<const float4*>(x) + 1);
+            a = fmaf(bf16lo(w.x), x0.x, a); a = fmaf(bf16hi(w.x), x0.y, a);
+            a = fmaf(bf16lo(w.y), x0.z, a); a = fmaf(bf16hi(w.y), x0.w, a);
+            a = fmaf(bf16lo(w.z), x1.x, a); a = fmaf(bf16hi(w.z), x1.y, a);
+            a = fmaf(bf16lo(w.w), x1.z, a); a = fmaf(bf16hi(w.w), x1.w, a);
+          }
+          a = warp_sum(a) + __ldg(p.bw + n);
+          if (lane == 0) {
+            m[n] = a;
+            if (s * p.N >= row0) p.mem_out[(size_t)s * RS_D + n] = a;     // the CTA owning the sample's first row
+          }
+        }
+      } else {
+        for (int i = tid; i < RS_D; i += RS_CONSUMERS) m[i] = p.mem_prev[(size_t)s * RS_D + i];
+      }
+    }
+    rs_consumer_bar();
+    for (int q = 0; q < nsamp; ++q)
+      for (int n = warp; n < RS_D; n += RS_CONSUMERS / 32) {
+        const float v = bf16_row_dot(p.Wy_t + (size_t)n * RS_D, s_m + q * RS_D, RS_D, lane) + __ldg(p.by + n);
+        if (lane == 0) s_y[q * RS_D + n] = v;
+      }
+    rs_consumer_bar();
+  }
+
+  // ---- P -> P*y in place (rows past M are TMA zero fill and stay zero)
+  mbar_wait(a_full, 0);
+  for (int i = tid; i < RS_KB * RS_BM * 8; i += RS_CONSUMERS) {
+    const int kb = i >> 9, r = (i >> 3) & 63, pos = i & 7;
+    const int col = kb * TC_BK + ((pos ^ (r & 7)) << 3);
+    const int s = min(row0 + r, p.M - 1) / p.N;
+    const float* yy = p.Wy_t ? s_y + (s - s_lo) * RS_D + col : y_src + (size_t)s * RS_D + col;
+    uint4* ptr = reinterpret_cast<uint4*>(a_tile + kb * RS_BLK + r * 128 + pos * 16);
+    const uint4 v = *ptr;
+    const float4 y0 = *reinterpret_cast<const float4*>(yy), y1 = *reinterpret_cast<const float4*>(yy + 4);
+    *ptr = make_uint4(pack_bf16(bf16lo(v.x) * y0.x, bf16hi(v.x) * y0.y), pack_bf16(bf16lo(v.y) * y0.z, bf16hi(v.y) * y0.w),
+                      pack_bf16(bf16lo(v.z) * y1.x, bf16hi(v.z) * y1.y), pack_bf16(bf16lo(v.w) * y1.z, bf16hi(v.w) * y1.w));
+  }
+  fence_proxy_async();                                       // generic-proxy stores -> visible to wgmma
+  rs_consumer_bar();
+
+  const int g = warp >> 2;                                   // warpgroup: output columns [256 g, 256 g + 256)
+  float acc[128];
+  const uint32_t a_u = smem_u32(a_tile);
+  auto gemm = [&](int j0) {
+    for (int j = j0; j < j0 + RS_KB; ++j) {
+      const int s = j % RS_STAGES;
+      mbar_wait(&full[s], (j / RS_STAGES) & 1);
+      const uint64_t adesc = make_sw128_kmajor_desc(a_u + (j - j0) * RS_BLK);
+      const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(b_ring + s * RS_STAGE + g * RS_B_HALF));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n256(acc, adesc + 2 * k, bdesc + 2 * k, (j > j0 || k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      wgmma_hold(acc);
+      if (j > j0 && lane == 0) mbar_arrive(&empty[(j - 1) % RS_STAGES]);
+    }
+    wgmma_wait<0>();
+    wgmma_hold(acc);
+    if (lane == 0) mbar_arrive(&empty[(j0 + RS_KB - 1) % RS_STAGES]);
+  };
+  // acc[4 j + 2 h + e] is tile row 16 (warp & 3) + lane / 4 + 8 h, column 256 g + 8 j + 2 (lane & 3) + e
+  const int rl = 16 * (warp & 3) + (lane >> 2);
+  const int cq = 256 * g + 2 * (lane & 3);
+
+  // ---- GEMM 1 and its epilogue: H = ELU(acc + Q) -> bf16 into the A tile (K-major, swizzled) once both halves are done
+  gemm(0);
+  rs_consumer_bar();                                         // the other warpgroup has finished reading P*y
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = rl + 8 * h, row = row0 + r;
+    const __nv_bfloat16* qrow = p.Q + (size_t)min(row, p.M - 1) * RS_D;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int n = cq + 8 * j;
+      const uint32_t q = __ldg(reinterpret_cast<const unsigned int*>(qrow + n));
+      const uint32_t hv = row < p.M ? pack_bf16(elu_fast(acc[4 * j + 2 * h] + bf16lo(q)), elu_fast(acc[4 * j + 2 * h + 1] + bf16hi(q)))
+                                    : 0u;
+      const int kb = n >> 6, c = (n & 63) >> 3;
+      *reinterpret_cast<uint32_t*>(a_tile + kb * RS_BLK + r * 128 + ((c ^ (r & 7)) << 4) + (n & 7) * 2) = hv;
+    }
+  }
+  fence_proxy_async();
+  rs_consumer_bar();
+
+  // ---- GEMM 2 and its epilogue: I2 = ELU((acc + bm2) * control_b); logit half = sum_n I2 * wr
+  gemm(RS_KB);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = rl + 8 * h, row = row0 + r;
+    const float* crow = p.ctrl + (size_t)(min(row, p.M - 1) / p.N) * RS_D;
+    float part = 0.f;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int n = cq + 8 * j;
+      const float2 cc = __ldg(reinterpret_cast<const float2*>(crow + n));
+      const float t0 = elu_fast((acc[4 * j + 2 * h] + __ldg(p.bm2 + n)) * cc.x);
+      const float t1 = elu_fast((acc[4 * j + 2 * h + 1] + __ldg(p.bm2 + n + 1)) * cc.y);
+      part = fmaf(t0, __ldg(p.wr + n), part);
+      part = fmaf(t1, __ldg(p.wr + n + 1), part);
+    }
+    part += __shfl_xor_sync(0xffffffffu, part, 1);
+    part += __shfl_xor_sync(0xffffffffu, part, 2);
+    if ((lane & 3) == 0) s_lg[g * RS_BM + r] = part;
+  }
+  rs_consumer_bar();
+  if (tid < RS_BM && row0 + tid < p.M) p.logits[row0 + tid] = s_lg[tid] + s_lg[RS_BM + tid];
+}
+
+// inv = [P | Q] (tc_read_invariant); y, control [B, d] fp32; att [B, N], info [B, d]
 inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y, const float* control,
                             const mac_read_weights* w, float* att, float* info, int B, int N, int d, cudaStream_t stream,
                             const WholeStepArgs* ws = nullptr) {
@@ -1234,96 +292,26 @@ inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y
       return MAC_ERR_ALIGN;
   }
   const int M = B * N;
-  const size_t slab = (((size_t)M * d * 2 + 1023) & ~(size_t)1023);
-  const char* ibase = tc_align1k(const_cast<void*>(inv));
+  const TcReadScratch s = tc_read_scratch(const_cast<void*>(inv), B, N, d);
   CUtensorMap mp, mw1, mw2;
-  int st = make_tmap_2d(&mp, ibase, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, 128, TC_BK, 1);
+  int st = make_tmap_2d(&mp, s.P, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS_BM, TC_BK, 1);
   if (st != MAC_OK) return st;
   st = make_tmap_2d(&mw1, w->Wm_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)2 * d * 2, 256, TC_BK, 1);   // Wm[0:d] of [d, 2d]
   if (st != MAC_OK) return st;
   st = make_tmap_2d(&mw2, w->Wm2_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)d * 2, 256, TC_BK, 1);
   if (st != MAC_OK) return st;
   ReadStepParams p{};
-  p.B = B; p.N = N; p.y = y; p.ctrl = control; p.bm2 = w->bm2; p.wr = w->wr; p.br = w->br;
-  p.Q = reinterpret_cast<const __nv_bfloat16*>(ibase + slab);
-  p.kb = reinterpret_cast<const __nv_bfloat16*>(kb_bf16);
-  p.att = att; p.info = info; p.dbg = read_step_dbg_ptr(); p.dbg_flags = read_step_dbg_flags();
+  p.M = M; p.N = N; p.y = y; p.ctrl = control; p.bm2 = w->bm2; p.wr = w->wr; p.Q = s.Q; p.logits = s.parts;
   if (ws) {
-    p.mem_prev = ws->mem_prev; p.info_prev = ws->info_prev; p.bw = ws->bw; p.by = w->by; p.mem_out = ws->mem_out;
+    p.y = nullptr; p.mem_prev = ws->mem_prev; p.info_prev = ws->info_prev; p.bw = ws->bw; p.by = w->by; p.mem_out = ws->mem_out;
     p.Ww_t = reinterpret_cast<const __nv_bfloat16*>(ws->Ww_t_bf16);
     p.Wy_t = reinterpret_cast<const __nv_bfloat16*>(ws->Wy_t_bf16);
   }
-  static bool attr_set[3] = {false, false, false};
-  static const bool pair_mma = !(getenv("MAC_READ_PAIR_MMA") && atoi(getenv("MAC_READ_PAIR_MMA")) == 0);
-  if (N > 128 && pair_mma) {
-    // weight boxes are [128 x 64] halves here: separate tensor maps
-    CUtensorMap hw1, hw2;
-    st = make_tmap_2d(&hw1, w->Wm_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)2 * d * 2, 128, TC_BK, 1);
-    if (st != MAC_OK) return st;
-    st = make_tmap_2d(&hw2, w->Wm2_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)d * 2, 128, TC_BK, 1);
-    if (st != MAC_OK) return st;
-    auto kern = read_step2_kernel;
-    if (!attr_set[2]) {
-      MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, RS2_SMEM_BYTES));
-      attr_set[2] = true;
-    }
-    p.spc = 1;
-    // packed tiles (no padded rows) unless the whole-step prologue needs the pair = sample mapping; MAC_READ_PACKED=0 reverts
-    static const bool packed_ok = !(getenv("MAC_READ_PACKED") && atoi(getenv("MAC_READ_PACKED")) == 0);
-    const bool packed = packed_ok && !ws;
-    const int ntiles = (M + 127) / 128;
-    p.packed = packed ? 1 : 0;
-    // the partials live behind [P | Q] in the invariant buffer (tc_read_invariant_bytes reserves read_step_partial_bytes)
-    p.part = packed ? reinterpret_cast<float*>(const_cast<char*>(ibase) + 2 * slab) : nullptr;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(packed ? 2 * ((ntiles + 1) / 2) : 2 * B, 1, 1);
-    cfg.blockDim = dim3(RS_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = RS2_SMEM_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    MAC_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, mp, hw1, hw2, p));
-    if (packed && !(p.dbg_flags & 8)) {            // flag 8 (profiling: time the main kernel alone) leaves att / info unmerged
-      MAC_LAUNCH_CHECK();
-      read_step_combine_kernel<<<B, RS_D, 0, stream>>>(p.part, att, info, B, N);
-    }
-  } else if (N > 128) {
-    auto kern = read_step_kernel<true>;
-    if (!attr_set[0]) {
-      MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM_BYTES));
-      attr_set[0] = true;
-    }
-    p.spc = 1;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2 * B, 1, 1);
-    cfg.blockDim = dim3(RS_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = RS_SMEM_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    MAC_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, mp, mw1, mw2, p));
-  } else {
-    auto kern = read_step_kernel<false>;
-    if (!attr_set[1]) {
-      MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM_BYTES));
-      attr_set[1] = true;
-    }
-    p.spc = min(128 / N, RS_MAX_SPC);
-    const int grid = (B + p.spc - 1) / p.spc;
-    kern<<<grid, RS_THREADS, RS_SMEM_BYTES, stream>>>(mp, mw1, mw2, p);
-  }
+  // the opt-in is per device context: set it on every launch
+  MAC_CUDA_TRY(cudaFuncSetAttribute(read_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM_BYTES));
+  read_step_kernel<<<(M + RS_BM - 1) / RS_BM, RS_THREADS, RS_SMEM_BYTES, stream>>>(mp, mw1, mw2, p);
   MAC_LAUNCH_CHECK();
-  return MAC_OK;
+  return mac_kb_attend_fwd(s.parts, 1, w->br, kb_bf16, 1, att, info, B, N, d, stream);
 }
 
 }  // namespace mac

@@ -407,7 +407,7 @@ __global__ void __launch_bounds__(256, SGEMM_MIN_BLOCKS) sgemm_kernel(const Sgem
   }
 }
 
-// host-side launch: picks the tile shape and a split-K factor that fills the 148 SMs
+// host-side launch: picks the tile shape and a split-K factor that fills the SMs
 inline size_t sgemm_workspace_bytes(int M, int N, int K) {
   // worst case: split so that each split has >= 2 k-iterations of 16; cap at 32 splits
   int splitk = K / 32;
@@ -420,7 +420,7 @@ inline size_t sgemm_workspace_bytes(int M, int N, int K) {
 // 1024 x 512) get 16-32 tiles and at most 2 K slices out of them, 64x64 tiles give 64-128 tiles x 2 slices.
 // (EPI_READ_LOGITS callers size their per-column-tile partial logits with sgemm_tile_n.)
 inline bool sgemm_big_tiles(int M, int N, int K) {
-  return (M >= 512) && (K >= 256 || ((M + 127) / 128) * ((N + 127) / 128) >= 148);
+  return (M >= 512) && (K >= 256 || ((M + 127) / 128) * ((N + 127) / 128) >= mac_num_sms());
 }
 inline int sgemm_tile_n(int M, int N, int K) { return sgemm_big_tiles(M, N, K) ? 128 : 64; }
 
@@ -439,8 +439,8 @@ inline int sgemm_launch(SgemmParams p, unsigned int* counters, float* partial, s
   if (p.epi == EPI_READ_LOGITS || counters == nullptr || partial == nullptr) allow_splitk = false;
   int splitk = 1;
   const int tiles = grid.x * grid.y;
-  if (allow_splitk && tiles < 148 && tiles <= 1024 && p.K >= 64) {
-    splitk = (296 + tiles - 1) / tiles;           // aim at ~2 CTAs per SM
+  if (allow_splitk && tiles < mac_num_sms() && tiles <= 1024 && p.K >= 64) {
+    splitk = (2 * mac_num_sms() + tiles - 1) / tiles;           // aim at ~2 CTAs per SM
     const int maxk = p.K / 32;                    // >= 2 k-iterations per split
     if (splitk > maxk) splitk = maxk;
     if (splitk > 32) splitk = 32;

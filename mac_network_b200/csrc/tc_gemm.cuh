@@ -1,15 +1,15 @@
-// bf16 tensor-core GEMM for sm_100a: tcgen05.mma (UMMA 128 x BN x 16, cta_group::1) with fp32 accumulators in
-// TMEM, operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) through a 4-stage mbarrier ring, and the
-// read unit's elementwise work fused into the TMEM->register epilogue.
+// bf16 tensor-core GEMM for sm_90a: wgmma.mma_async (64 x 128 x 16 per warpgroup, fp32 accumulators in registers), operands
+// staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) through an mbarrier ring, and the read unit's elementwise work
+// fused into the register epilogue.
 //
 //   C[M,N] = epilogue( A[M,K] @ Wt[N,K]^T )      A, Wt bf16 row-major with K contiguous ("K-major" both)
 //
-// Warp roles (192 threads, persistent over output tiles, one CTA per SM):
-//   warp 0      TMA producer          (one elected lane issues the A and B boxes of each k-block)
-//   warp 1      TMEM allocator + MMA issuer (one elected lane issues tcgen05.mma / tcgen05.commit)
-//   warps 2..9  epilogue              (tcgen05.ld 32 lanes x 32 columns per instruction; thread == output row;
-//                                      two warps per TMEM lane quarter, each takes half of the tile's columns)
-// Two accumulator buffers (2 x BN TMEM columns) let the epilogue of tile i overlap the MMAs of tile i+1.
+// One CTA per 128 x 128 output tile (x K slice when split-K), 288 threads:
+//   warpgroups 0, 1   consumers: rows [64 g, 64 g + 64) of the tile against all 128 columns (64 accumulators per thread);
+//                     they issue the wgmma, then run the epilogue straight from the accumulator registers
+//   warp 8            TMA producer (one elected lane issues the A and B boxes of each k-block)
+// The 3-stage ring takes 96 KB of shared memory.  The epilogues with the most live values (P, LOGITS) need 160+ registers,
+// so a CTA of 288 threads has the SM's register file to itself: there is no cross-CTA overlap of epilogue and main loop.
 //
 // Epilogues (the read-unit chain of mac_cell.py:230-266 / ops.py:668-725, see mac_b200.h):
 //   TC_EPI_P       P = acc + bx            -> bf16 P and bf16 P*y[b]            (ops.py:688, 694-703)
@@ -45,20 +45,17 @@ struct TcGemmParams {
   const float* y;          // [B, N] row scale for TC_EPI_P
   const float* ctrl;       // [B, N] for TC_EPI_LOGITS
   const float* wr;         // [N]
-  float* parts;            // [M, gridN]
+  float* parts;            // [M, N / TC_BN]
   int rows_per_batch;
   uint32_t e_thresh;       // dropout on the logits' input (0 = none)
   float e_scale;
   uint64_t seed;
   int e_site, step;
-  int ksplit;              // split-K (TC_EPI_F32 only, single-CTA kernel): the K range is cut into `ksplit` equal slices, each an
-  long long split_stride;  //   extra "tile" writing its fp32 partial to outf + slice * split_stride; 0 / 1 = off
-  int debug;               // MAC_TC_DEBUG (profiling experiments only): 1 skip epilogue math/stores, 2 skip MMA, 4 skip TMA
+  int ksplit;              // split-K (TC_EPI_F32 only): the K range is cut into `ksplit` equal slices (grid z), each writing
+  long long split_stride;  //   its fp32 partial to outf + slice * split_stride; 0 / 1 = off
 };
 
-// ------------------------------------------------------------------ tcgen05 PTX wrappers
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ------------------------------------------------------------------ wgmma PTX wrappers
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -68,100 +65,74 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulators are register operands of the asynchronous MMA: keep the compiler from touching them before the wait
+template <int R>
+__device__ __forceinline__ void wgmma_hold(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; single-thread issue
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-// mbarrier arrive when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor) for a K-major tile stored as rows of 128 bytes with
-// the 128-byte swizzle (what TMA SWIZZLE_128B writes for a [rows x 64 bf16] box):
-//   start address >> 4 | LBO (ignored for swizzled K-major; 1) | SBO = 1024 B between 8-row groups | version 1 |
-//   layout type 2 (SWIZZLE_128B).  The tile base must be 1024-byte aligned (base_offset 0).
+// Shared-memory matrix descriptor of a K-major tile stored as rows of 128 bytes with the 128-byte swizzle (what TMA
+// SWIZZLE_128B writes for a [rows x 64 bf16] box): start address >> 4 | LBO (unused for swizzled K-major; 1) |
+// SBO = 1024 B between 8-row groups | layout type 1 (SWIZZLE_128B) in bits 62-63.  The tile base must be 1024-byte aligned.
+// Advancing 16 bf16 (32 bytes) along K inside the swizzle atom is +2 in the address field.
 __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);   // bits [0,14)
   d |= (uint64_t)1 << 16;                        // leading byte offset (16-B units), bits [16,30)
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                        // version = 1 (Blackwell), bits [46,48)
-  d |= (uint64_t)2 << 61;                        // layout type SWIZZLE_128B, bits [61,64)
+  d |= (uint64_t)1 << 62;                        // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A/B bf16, both K-major, dense, M x N
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// D[64 x N] (+)= A[64 x 16] B[16 x N], both operands from shared memory; accum == 0 overwrites D
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
+}
+
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
+}
+
+__device__ __forceinline__ void wgmma_bf16_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
 }
 
 constexpr int TC_BK = 64;                 // 64 bf16 = 128 B = one swizzle atom row
-constexpr int TC_MAX_VEC = 4;              // a 128-row tile spans at most this many samples on the smem-parameter path
-constexpr int TC_EPI_WARPS = 8;            // cta_group::2 kernel: two per TMEM lane quarter
-constexpr int TC_THREADS = 64 + 32 * TC_EPI_WARPS;
-constexpr int TC_EW = 16;                  // single-CTA kernel: four epilogue warps per TMEM lane quarter
-constexpr int TC_THREADS1 = 64 + 32 * TC_EW;
-
-// Tile shapes.  The measured per-SM TMA fill rate is ~64 B/clk (profiles/r1/NOTES.md): a k-block of a BM x BN tile
-// brings (BM + BN) * 128 B and feeds BM * BN / 64 MMA cycles, so
-//   128 x 128 -> 128 B/clk needed (2x fill-bound), 128 x 256 -> 96 B/clk (1.5x), 256 x 256 -> 64 B/clk (balanced).
-// BM = 256 is two M=128 UMMAs per k-step that share the B tile in shared memory and own one accumulator each
-// (2 x 256 TMEM columns, not double-buffered); BM = 128 keeps two accumulator buffers so the epilogue of tile i
-// overlaps the MMAs of tile i+1.
-template <int BM, int BN>
-struct TcCfg {
-  static constexpr int NMS = BM / 128;                      // M sub-tiles (UMMA M = 128 each)
-  static constexpr int STAGES = BM == 256 ? 3 : (BN == 256 ? 4 : 6);
-  static constexpr int A_BYTES = BM * TC_BK * 2;            // 16 / 32 KB
-  static constexpr int B_BYTES = BN * TC_BK * 2;            // 16 / 32 KB
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int NBUF = BM == 256 ? 1 : 2;            // accumulator buffers
-  static constexpr int BUF_COLS = NMS * BN;
-  static constexpr int TMEM_COLS = 512 / (BM == 128 && BN == 128 ? 2 : 1);   // NBUF * BUF_COLS, a power of two
-  static constexpr int STG_WORDS = 32 * 8;                  // per epilogue warp: 32 rows x 8 words (32 B), XOR-swizzled
-  static constexpr int PAR_ROWS = 2 + TC_MAX_VEC;           // bias, wr, and up to TC_MAX_VEC per-sample rows (y / control)
-  static constexpr int PAR_WORDS = NBUF * PAR_ROWS * BN;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ +
-                                    TC_EW * STG_WORDS * 4 + PAR_WORDS * 4;
-};
+constexpr int TC_BM = 128;
+constexpr int TC_BN = 128;
+constexpr int TC_STAGES = 3;
+constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;             // 16 KB
+constexpr int TC_B_BYTES = TC_BN * TC_BK * 2;             // 16 KB
+constexpr int TC_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;
+constexpr int TC_CONSUMERS = 256;                         // two warpgroups
+constexpr int TC_THREADS = TC_CONSUMERS + 32;
+constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 1024 /*align*/ + 128 /*barriers*/;
 
 // fast ELU for the tensor-core path: x > 0 ? x : exp(x) - 1 with the SFU exponential (abs error ~1e-7 near 0,
 // far below the bf16 rounding of the stored activations)
-// (ex2.approx.ftz directly: without -ftz, __expf expands to a ~10-instruction denormal-safe sequence per element, which
-// made the 128 x 512 epilogues of the fused read step issue-bound)
 __device__ __forceinline__ float ex2_ftz(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -184,821 +155,200 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
-template <int BM, int BN, int EPI, int ACT>
-__global__ void __launch_bounds__(TC_THREADS1, 1)
+template <int EPI, int ACT>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
                const __grid_constant__ CUtensorMap map_b, const TcGemmParams p) {
-  using C = TcCfg<BM, BN>;
-  constexpr int TC_BM = BM;
   extern __shared__ unsigned char smem_dyn[];
-  // 1024-byte aligned operand ring
   const uint32_t base_u32 = smem_u32(smem_dyn);
   const uint32_t pad = (1024u - (base_u32 & 1023u)) & 1023u;
-  unsigned char* tiles = smem_dyn + pad;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + C::STAGES * C::STAGE_BYTES);
-  uint64_t* full = bars;                       // [STAGES]  TMA -> MMA
-  uint64_t* empty = bars + C::STAGES;          // [STAGES]  MMA -> TMA
-  uint64_t* tfull = bars + 2 * C::STAGES;      // [2]       MMA -> epilogue
-  uint64_t* tempty = tfull + 2;                // [2]       epilogue -> MMA
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty + 2);
-  uint32_t* stg_all = reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(bars) + 256);
-  float* par_all = reinterpret_cast<float*>(stg_all + TC_EW * C::STG_WORDS);
+  unsigned char* tiles = smem_dyn + pad;                   // 1024-byte aligned operand ring
+  uint64_t* full = reinterpret_cast<uint64_t*>(tiles + TC_STAGES * TC_STAGE_BYTES);   // [STAGES] TMA -> consumers
+  uint64_t* empty = full + TC_STAGES;                                                 // [STAGES] consumers -> TMA
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (p.M + TC_BM - 1) / TC_BM;
-  const int n_tiles = p.N / BN;
-  const int ksplit = p.ksplit > 1 ? p.ksplit : 1;
-  const int mn_tiles = m_tiles * n_tiles;
-  const int num_tiles = mn_tiles * ksplit;                 // tile t = (K slice t / mn_tiles, output tile t % mn_tiles)
-  const int kblocks = p.K / TC_BK / ksplit;                // k-blocks per slice
+  const int nt = blockIdx.x, mt = blockIdx.y;
+  const int n_tiles = gridDim.x;
+  const int kblocks = p.K / TC_BK / (int)gridDim.z;        // k-blocks of this CTA's K slice
+  const int kb0 = (int)blockIdx.z * kblocks;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == TC_CONSUMERS) {
     tma_prefetch_desc(&map_a0);
     tma_prefetch_desc(&map_a1);
     tma_prefetch_desc(&map_b);
 #pragma unroll
-    for (int i = 0; i < C::STAGES; ++i) {
+    for (int i = 0; i < TC_STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
+      mbar_init(&empty[i], TC_CONSUMERS / 32);
     }
-    mbar_init(&tfull[0], 1);
-    mbar_init(&tfull[1], 1);
-    mbar_init(&tempty[0], TC_EW);
-    mbar_init(&tempty[1], TC_EW);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == TC_CONSUMERS / 32) {
     // ===================================================== TMA producer
     if (elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int tt = t % mn_tiles, kb0 = (t / mn_tiles) * kblocks;
-        const int mt = tt / n_tiles, nt = tt % n_tiles;
-        for (int kb = kb0; kb < kb0 + kblocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          unsigned char* sa = tiles + stage * C::STAGE_BYTES;
-          unsigned char* sb = sa + C::A_BYTES;
-          if (p.debug & 4) {
-            mbar_arrive(&full[stage]);
-            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            continue;
-          }
-          mbar_expect_tx(&full[stage], C::STAGE_BYTES);
-          if (kb < p.kblocks0)
-            tma_load_2d(sa, &map_a0, kb * TC_BK, mt * TC_BM, &full[stage]);
-          else
-            tma_load_2d(sa, &map_a1, (kb - p.kblocks0) * TC_BK, mt * TC_BM, &full[stage]);
-          tma_load_2d(sb, &map_b, kb * TC_BK, nt * BN, &full[stage]);
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
+      for (int kb = kb0; kb < kb0 + kblocks; ++kb) {
+        mbar_wait(&empty[stage], phase ^ 1);
+        unsigned char* sa = tiles + stage * TC_STAGE_BYTES;
+        mbar_expect_tx(&full[stage], TC_STAGE_BYTES);
+        if (kb < p.kblocks0)
+          tma_load_2d(sa, &map_a0, kb * TC_BK, mt * TC_BM, &full[stage]);
+        else
+          tma_load_2d(sa, &map_a1, (kb - p.kblocks0) * TC_BK, mt * TC_BM, &full[stage]);
+        tma_load_2d(sa + TC_A_BYTES, &map_b, kb * TC_BK, nt * TC_BN, &full[stage]);
+        if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    constexpr uint32_t idesc = make_idesc_bf16(128, BN);
-    int stage = 0;
+    return;
+  }
+
+  // ===================================================== consumers: main loop
+  const int g = warp >> 2;                                  // warpgroup: rows [64 g, 64 g + 64) of the tile
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  {
+    int stage = 0, prev = 0;
     uint32_t phase = 0;
-    int it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int acc = it % C::NBUF;
-      const uint32_t acc_phase = (it / C::NBUF) & 1;
-      mbar_wait(&tempty[acc], acc_phase ^ 1);        // epilogue has drained this accumulator buffer
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * C::BUF_COLS;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t sa = smem_u32(tiles + stage * C::STAGE_BYTES);
-          const uint64_t adesc = make_sw128_kmajor_desc(sa);
-          const uint64_t bdesc = make_sw128_kmajor_desc(sa + C::A_BYTES);
+    for (int kb = 0; kb < kblocks; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(tiles + stage * TC_STAGE_BYTES);
+      const uint64_t adesc = make_sw128_kmajor_desc(sa + g * (64 * 128));
+      const uint64_t bdesc = make_sw128_kmajor_desc(sa + TC_A_BYTES);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) {
-            // advance 16 bf16 = 32 bytes along K inside the 128-byte swizzle atom: +2 in the 16-B address field;
-            // the second M sub-tile's rows start 16 KB (= 1024 in 16-B units) further
-#pragma unroll
-            for (int ms = 0; ms < C::NMS; ++ms)
-              if (!(p.debug & 2))
-                umma_bf16(tmem_d + ms * BN, adesc + 2 * k + ms * 1024, bdesc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);                // frees the smem slot when these MMAs retire
-          if (kb == kblocks - 1) umma_commit(&tfull[acc]);
-        }
-        __syncwarp();
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-      }
+      for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n128(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();                                      // the previous k-block's products have retired
+      wgmma_hold(acc);
+      if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
     }
-  } else {
-    // ===================================================== epilogue: TC_EW = 16 warps, four per TMEM lane quarter
-    // thread == one output row of the tile (TMEM lane); the warp walks its share of the tile's columns 16 at a time
-    // (one tcgen05.ld 32x32b.x16).  With two warps per scheduler (the 8-warp version) the ELU/pack/store chain was
-    // issue-latency bound and its ~4 us per 128x256 tile was the largest non-MMA term of the K=512 projections;
-    // four warps per scheduler overlap those chains.
-    const int q = warp & 3;
-    const int ew = warp - 2;
-    uint32_t* stg = stg_all + ew * C::STG_WORDS;    // 1 KB patch: 32 rows x 32 B
-    const int grp = ew >> 2;                        // 0..3
-    const int ms = C::NMS == 2 ? (grp >> 1) : 0;    // BM=256: which M sub-tile
-    constexpr int CW = C::NMS == 2 ? BN / 2 : BN / 4;                 // columns per warp
-    constexpr int NSUB = C::NMS == 2 ? 2 : 4;                         // logit partial sums per (row, n-tile)
-    const int sub = C::NMS == 2 ? (grp & 1) : grp;
-    const int c_begin = sub * CW, c_end = c_begin + CW;
-    // Row-per-thread registers -> coalesced 128-bit global stores through the warp's private patch.  A patch row is
-    // 32 B = two 16-B groups; group g of row r lives at slot (g ^ ((r >> 2) & 1)), which makes both the row-wise
-    // writes (thread == row) and the read-back (lane l -> group l & 1 of row i*16 + l/2) bank-conflict free.  One
-    // store instruction then covers 16 rows x 32 B (whole sectors).
-    uint4* s4 = reinterpret_cast<uint4*>(stg);
-    const int sw = (lane >> 2) & 1;
-    const int rb_g = lane & 1;
-    auto store_bf16_chunk = [&](const uint32_t (&w)[8], __nv_bfloat16* out, int row0, int col0) {
-      __syncwarp();
-      s4[lane * 2 + (0 ^ sw)] = make_uint4(w[0], w[1], w[2], w[3]);
-      s4[lane * 2 + (1 ^ sw)] = make_uint4(w[4], w[5], w[6], w[7]);
-      __syncwarp();
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int rr = i * 16 + (lane >> 1);
-        const uint4 v = s4[rr * 2 + (rb_g ^ ((rr >> 2) & 1))];
-        if (row0 + rr < p.M) *reinterpret_cast<uint4*>(out + (size_t)(row0 + rr) * p.ldo + col0 + 8 * rb_g) = v;
-      }
-    };
-    auto store_f32_chunk = [&](const float (&w)[16], float* out, int row0, int col0) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {            // two 8-column halves through the 1 KB patch
-        __syncwarp();
-        s4[lane * 2 + (0 ^ sw)] = make_uint4(__float_as_uint(w[8 * h]), __float_as_uint(w[8 * h + 1]),
-                                             __float_as_uint(w[8 * h + 2]), __float_as_uint(w[8 * h + 3]));
-        s4[lane * 2 + (1 ^ sw)] = make_uint4(__float_as_uint(w[8 * h + 4]), __float_as_uint(w[8 * h + 5]),
-                                             __float_as_uint(w[8 * h + 6]), __float_as_uint(w[8 * h + 7]));
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int rr = i * 16 + (lane >> 1);
-          const uint4 v = s4[rr * 2 + (rb_g ^ ((rr >> 2) & 1))];
-          if (row0 + rr < p.M)
-            *reinterpret_cast<uint4*>(out + (size_t)(row0 + rr) * p.ldo + col0 + 8 * h + 4 * rb_g) = v;
-        }
-      }
-    };
-    const int etid = threadIdx.x - 64;              // 0..511 among the epilogue threads
-    const float* vec_src = (EPI == TC_EPI_P) ? p.y : (EPI == TC_EPI_LOGITS ? p.ctrl : nullptr);
-    int it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int tt = t % mn_tiles;
-      const int mt = tt / n_tiles, nt = tt % n_tiles;
-      float* const outf_t = p.outf + (size_t)(t / mn_tiles) * (size_t)p.split_stride;      // split-K partial (slice 0: outf)
-      const int acc = it % C::NBUF;
-      const uint32_t acc_phase = (it / C::NBUF) & 1;
-      // ---- stage this tile's parameters in shared memory while the MMAs of the tile are still running:
-      //      row 0 bias[BN], row 1 wr[BN], rows 2.. the y / control vectors of the samples this tile touches
-      float* par = par_all + acc * (C::PAR_ROWS * BN);
-      const int b_lo = (mt * TC_BM) / p.rows_per_batch;
-      const int last_row = min(p.M, (mt + 1) * TC_BM) - 1;
-      const int nvec = vec_src ? (last_row / p.rows_per_batch - b_lo + 1) : 0;
-      const bool vec_smem = nvec <= TC_MAX_VEC;
-      {
-        const int nb = nt * BN;
-        for (int i = etid; i < BN; i += 32 * TC_EW) {
-          par[i] = p.bias ? __ldg(p.bias + nb + i) : 0.f;
-          if constexpr (EPI == TC_EPI_LOGITS) par[BN + i] = __ldg(p.wr + nb + i);
-        }
-        if (vec_src && vec_smem)
-          for (int i = etid; i < nvec * BN; i += 32 * TC_EW)
-            par[2 * BN + i] = __ldg(vec_src + (size_t)(b_lo + i / BN) * p.N + nb + (i % BN));
-        asm volatile("bar.sync 1, %0;" ::"n"(32 * TC_EW) : "memory");
-      }
-      const int row0 = mt * TC_BM + ms * 128 + q * 32;
-      const int row = row0 + lane;
-      const bool row_ok = row < p.M;
-      const int bidx = row_ok ? row / p.rows_per_batch : b_lo;
-      const float* vrow = vec_smem ? par + (2 + bidx - b_lo) * BN : nullptr;   // this row's y / control vector (tile-local)
-      const uint32_t taddr = tmem_base + acc * C::BUF_COLS + ms * BN + ((uint32_t)(q * 32) << 16);
-      // TC_EPI_ADDACT: the bf16 addend of up to ADD_WIN chunks, in the coalesced (read-back) mapping.  It does not
-      // depend on the accumulator, so the loads are issued before the wait on it and overlap this tile's MMAs
-      // (with a one-chunk look-ahead the epilogue paid one DRAM/L2 round trip per chunk: 24.7 -> 21.1 us -> see NOTES).
-      constexpr int NCH = CW / 16;
-      constexpr int ADD_WIN = (EPI == TC_EPI_ADDACT) ? (NCH < 4 ? NCH : 4) : 1;
-      uint4 addq[ADD_WIN][2];
-      auto load_addend = [&](int slot, int c0) {
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int rr = i * 16 + (lane >> 1);
-          addq[slot][i] = (row0 + rr < p.M)
-              ? __ldg(reinterpret_cast<const uint4*>(p.add + (size_t)(row0 + rr) * p.ldo + nt * BN + c0 + 8 * rb_g))
-              : make_uint4(0u, 0u, 0u, 0u);
-        }
-      };
-      if constexpr (EPI == TC_EPI_ADDACT) {
-#pragma unroll
-        for (int k = 0; k < ADD_WIN; ++k) load_addend(k, c_begin + 16 * k);
-      }
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      float part = 0.f;
-      // the ADDACT variant is fully unrolled so that the addend window is indexed statically
-#pragma unroll (EPI == TC_EPI_ADDACT ? NCH : 1)
-      for (int ch = 0; ch < NCH; ++ch) {
-        const int c0 = c_begin + 16 * ch;
-        if (p.debug & 1) break;
-        uint32_t r[16];
-        if (p.debug & 8) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) r[j] = (uint32_t)(c0 + j);
-        } else {
-          tmem_ld16(taddr + c0, r);
-          tmem_ld_wait();
-        }
-        const int n0 = nt * BN + c0;
-        const float4* bias4 = reinterpret_cast<const float4*>(par + c0);
-        if constexpr (EPI == TC_EPI_P) {
-          const float4* y4 = vec_smem ? reinterpret_cast<const float4*>(vrow + c0)
-                                      : reinterpret_cast<const float4*>(p.y + (size_t)bidx * p.N + n0);
-          uint32_t w0[8], w1[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 b0 = bias4[j / 4], y0 = y4[j / 4];
-            const float x0 = __uint_as_float(r[j]) + b0.x, x1 = __uint_as_float(r[j + 1]) + b0.y;
-            const float x2 = __uint_as_float(r[j + 2]) + b0.z, x3 = __uint_as_float(r[j + 3]) + b0.w;
-            w0[j / 2] = pack_bf16(x0, x1);
-            w0[j / 2 + 1] = pack_bf16(x2, x3);
-            w1[j / 2] = pack_bf16(x0 * y0.x, x1 * y0.y);
-            w1[j / 2 + 1] = pack_bf16(x2 * y0.z, x3 * y0.w);
-          }
-          store_bf16_chunk(w0, p.out0, row0, n0);
-          store_bf16_chunk(w1, p.out1, row0, n0);
-        } else if constexpr (EPI == TC_EPI_ACT) {
-          uint32_t w0[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 b0 = bias4[j / 4];
-            w0[j / 2] = pack_bf16(act_ct<ACT>(__uint_as_float(r[j]) + b0.x), act_ct<ACT>(__uint_as_float(r[j + 1]) + b0.y));
-            w0[j / 2 + 1] = pack_bf16(act_ct<ACT>(__uint_as_float(r[j + 2]) + b0.z), act_ct<ACT>(__uint_as_float(r[j + 3]) + b0.w));
-          }
-          store_bf16_chunk(w0, p.out0, row0, n0);
-        } else if constexpr (EPI == TC_EPI_ADDACT) {
-          // addend chunk -> patch (coalesced mapping) -> own row back into registers
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const int rr = i * 16 + (lane >> 1);
-            s4[rr * 2 + (rb_g ^ ((rr >> 2) & 1))] = addq[ch % ADD_WIN][i];
-          }
-          __syncwarp();
-          const uint4 qa = s4[lane * 2 + (0 ^ sw)], qb = s4[lane * 2 + (1 ^ sw)];
-          if (ch + ADD_WIN < NCH) load_addend(ch % ADD_WIN, c0 + 16 * ADD_WIN);   // refill the slot just consumed
-          const uint32_t qw[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
-          uint32_t w0[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 b0 = bias4[j / 4];
-            // bf16 -> fp32 is a 16-bit shift
-            const float q0 = __uint_as_float(qw[j / 2] << 16), q1 = __uint_as_float(qw[j / 2] & 0xffff0000u);
-            const float q2 = __uint_as_float(qw[j / 2 + 1] << 16), q3 = __uint_as_float(qw[j / 2 + 1] & 0xffff0000u);
-            w0[j / 2] = pack_bf16(act_ct<ACT>(__uint_as_float(r[j]) + b0.x + q0), act_ct<ACT>(__uint_as_float(r[j + 1]) + b0.y + q1));
-            w0[j / 2 + 1] = pack_bf16(act_ct<ACT>(__uint_as_float(r[j + 2]) + b0.z + q2), act_ct<ACT>(__uint_as_float(r[j + 3]) + b0.w + q3));
-          }
-          store_bf16_chunk(w0, p.out0, row0, n0);
-        } else if constexpr (EPI == TC_EPI_ACT_SPLIT) {
-          const float* arow = p.addf ? p.addf + (size_t)(row_ok ? row : 0) * p.ldaf + n0 : nullptr;
-          uint32_t wh[8], wl[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 b0 = bias4[j / 4];
-            const float4 a0 = arow ? *reinterpret_cast<const float4*>(arow + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-            const float x0 = act_ct<ACT>(__uint_as_float(r[j]) + b0.x + a0.x), x1 = act_ct<ACT>(__uint_as_float(r[j + 1]) + b0.y + a0.y);
-            const float x2 = act_ct<ACT>(__uint_as_float(r[j + 2]) + b0.z + a0.z), x3 = act_ct<ACT>(__uint_as_float(r[j + 3]) + b0.w + a0.w);
-            const uint32_t h01 = pack_bf16(x0, x1), h23 = pack_bf16(x2, x3);
-            wh[j / 2] = h01;
-            wh[j / 2 + 1] = h23;
-            wl[j / 2] = pack_bf16(x0 - __uint_as_float(h01 << 16), x1 - __uint_as_float(h01 & 0xffff0000u));
-            wl[j / 2 + 1] = pack_bf16(x2 - __uint_as_float(h23 << 16), x3 - __uint_as_float(h23 & 0xffff0000u));
-          }
-          store_bf16_chunk(wh, p.out0, row0, n0);
-          store_bf16_chunk(wl, p.out0, row0, p.N + n0);
-        } else if constexpr (EPI == TC_EPI_F32) {
-          float w0[16];
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 b0 = bias4[j / 4];
-            w0[j] = act_ct<ACT>(__uint_as_float(r[j]) + b0.x);
-            w0[j + 1] = act_ct<ACT>(__uint_as_float(r[j + 1]) + b0.y);
-            w0[j + 2] = act_ct<ACT>(__uint_as_float(r[j + 2]) + b0.z);
-            w0[j + 3] = act_ct<ACT>(__uint_as_float(r[j + 3]) + b0.w);
-          }
-          store_f32_chunk(w0, outf_t, row0, n0);
-        } else {  // TC_EPI_LOGITS
-          const float4* c4 = vec_smem ? reinterpret_cast<const float4*>(vrow + c0)
-                                      : reinterpret_cast<const float4*>(p.ctrl + (size_t)bidx * p.N + n0);
-          const float4* w4 = reinterpret_cast<const float4*>(par + BN + c0);
-          uint32_t w0[8];
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 b0 = bias4[j / 4], cc = c4[j / 4], ww = w4[j / 4];
-            const float i0 = __uint_as_float(r[j]) + b0.x, i1 = __uint_as_float(r[j + 1]) + b0.y;
-            const float i2 = __uint_as_float(r[j + 2]) + b0.z, i3 = __uint_as_float(r[j + 3]) + b0.w;
-            w0[j / 2] = pack_bf16(i0, i1);
-            w0[j / 2 + 1] = pack_bf16(i2, i3);
-            float t0 = elu_fast(i0 * cc.x), t1 = elu_fast(i1 * cc.y), t2 = elu_fast(i2 * cc.z), t3 = elu_fast(i3 * cc.w);
-            if (p.e_thresh) {
-              const uint64_t e = (uint64_t)row * (uint64_t)p.N + (uint64_t)(n0 + j);
-              const Philox4 rr = philox4x32_10(p.seed, e >> 2, (uint32_t)p.e_site, (uint32_t)p.step);
-              t0 = ((rr.x >> 8) >= p.e_thresh) ? t0 * p.e_scale : 0.f;
-              t1 = ((rr.y >> 8) >= p.e_thresh) ? t1 * p.e_scale : 0.f;
-              t2 = ((rr.z >> 8) >= p.e_thresh) ? t2 * p.e_scale : 0.f;
-              t3 = ((rr.w >> 8) >= p.e_thresh) ? t3 * p.e_scale : 0.f;
-            }
-            part = fmaf(t0, ww.x, part);
-            part = fmaf(t1, ww.y, part);
-            part = fmaf(t2, ww.z, part);
-            part = fmaf(t3, ww.w, part);
-          }
-          if (p.out0) store_bf16_chunk(w0, p.out0, row0, n0);       // I1 kept for backward
-        }
-      }
-      if constexpr (EPI == TC_EPI_LOGITS) {
-        // NSUB partial sums per (row, n-tile): one per epilogue warp that shares the row
-        if (row_ok) p.parts[((size_t)row * n_tiles + nt) * NSUB + sub] = part;
-      }
-      // release the accumulator buffer to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-    }
+    wgmma_wait<0>();
+    wgmma_hold(acc);
   }
 
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
-}
-
-// =====================================================================================================
-// cta_group::2 variant: a CTA PAIR (2-CTA cluster, one TPC) computes a 256 x 256 tile with ONE tcgen05.mma issued by
-// the leader CTA.  Each CTA stages its own 128 rows of A and only HALF of the B tile (128 of the 256 W rows) and keeps
-// its 128 x 256 half of the accumulator in its own TMEM, so per MMA each SM's shared memory supplies 8 KB instead of
-// 12 KB -- the measured SS-mode operand-read limit (~64 B/clk/SM) stops throttling the tensor core.
-//   * TMA loads are issued by both CTAs into their own smem but complete on the LEADER's `full` barrier
-//     (cp.async.bulk.tensor ... .cta_group::2, barrier address with the peer bit cleared).
-//   * the leader's tcgen05.commit multicasts to both CTAs' `empty` / `tfull` barriers.
-//   * each CTA's epilogue drains its own TMEM half; every epilogue warp of BOTH CTAs arrives on the leader's `tempty`.
-// =====================================================================================================
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma2_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// TMA load into this CTA's smem, transaction bytes counted on the LEADER CTA's barrier (peer bit 24 cleared)
-__device__ __forceinline__ void tma2_load_2d(void* smem_dst, const void* tmap, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar) & 0xFEFFFFFFu)
-      : "memory");
-}
-// arrive on the barrier at the same offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_barrier() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-struct Tc2Cfg {
-  static constexpr int BN = 256;
-  static constexpr int STAGES = 5;
-  static constexpr int A_BYTES = 128 * TC_BK * 2;            // this CTA's 128 rows of A
-  static constexpr int B_BYTES = (BN / 2) * TC_BK * 2;       // this CTA's half of the B tile
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;      // 32 KB per CTA per k-block
-  static constexpr int TMEM_COLS = 512;                      // two 256-column accumulator buffers
-  static constexpr int STG_WORDS = 32 * 16;
-  static constexpr int PAR_ROWS = 2 + TC_MAX_VEC;
-  static constexpr int PAR_WORDS = 2 * PAR_ROWS * BN;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + TC_EPI_WARPS * STG_WORDS * 4 + PAR_WORDS * 4;
-};
-
-template <int EPI, int ACT>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tc2_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
-                const __grid_constant__ CUtensorMap map_b, const TcGemmParams p) {
-  using C = Tc2Cfg;
-  constexpr int BN = C::BN;
-  extern __shared__ unsigned char smem_dyn[];
-  const uint32_t base_u32 = smem_u32(smem_dyn);
-  const uint32_t pad = (1024u - (base_u32 & 1023u)) & 1023u;
-  unsigned char* tiles = smem_dyn + pad;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + C::STAGES * C::STAGE_BYTES);
-  uint64_t* full = bars;                       // [STAGES]  (leader's are the live ones)
-  uint64_t* empty = bars + C::STAGES;          // [STAGES]  per CTA
-  uint64_t* tfull = bars + 2 * C::STAGES;      // [2]       per CTA
-  uint64_t* tempty = tfull + 2;                // [2]       leader's are the live ones
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty + 2);
-  uint32_t* stg_all = reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(bars) + 256);
-  float* par_all = reinterpret_cast<float*>(stg_all + TC_EPI_WARPS * C::STG_WORDS);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();                     // 0 = leader
-  const int m_pairs = (p.M + 255) / 256;
-  const int n_tiles = p.N / BN;
-  const int num_tiles = m_pairs * n_tiles;
-  const int kblocks = p.K / TC_BK;
-  const int pair0 = blockIdx.x >> 1, pair_stride = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_a0);
-    tma_prefetch_desc(&map_a1);
-    tma_prefetch_desc(&map_b);
+  // ===================================================== epilogue, straight from the accumulator fragment:
+  // acc[4 j + 2 h + e] is row (16 * (warp & 3) + lane / 4 + 8 h) of the warpgroup's 64, column 8 j + 2 (lane & 3) + e
+  float* const outf_t = p.outf + (size_t)blockIdx.z * (size_t)p.split_stride;      // split-K partial (slice 0: outf)
+  const int cq = 2 * (lane & 3);
 #pragma unroll
-    for (int i = 0; i < C::STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    mbar_init(&tfull[0], 1);
-    mbar_init(&tfull[1], 1);
-    mbar_init(&tempty[0], 2 * TC_EPI_WARPS);
-    mbar_init(&tempty[1], 2 * TC_EPI_WARPS);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc2(tmem_ptr, C::TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  cluster_barrier();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ===================================================== TMA producer (both CTAs)
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = pair0; t < num_tiles; t += pair_stride) {
-        const int mp = t / n_tiles, nt = t % n_tiles;
-        const int row_a = mp * 256 + (int)rank * 128;
-        const int row_b = nt * BN + (int)rank * (BN / 2);
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          unsigned char* sa = tiles + stage * C::STAGE_BYTES;
-          unsigned char* sb = sa + C::A_BYTES;
-          if (rank == 0) mbar_expect_tx(&full[stage], 2 * C::STAGE_BYTES);   // both CTAs' bytes land on the leader's barrier
-          if (kb < p.kblocks0)
-            tma2_load_2d(sa, &map_a0, kb * TC_BK, row_a, &full[stage]);
-          else
-            tma2_load_2d(sa, &map_a1, (kb - p.kblocks0) * TC_BK, row_a, &full[stage]);
-          tma2_load_2d(sb, &map_b, kb * TC_BK, row_b, &full[stage]);
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+  for (int h = 0; h < 2; ++h) {
+    const int row = mt * TC_BM + g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    const bool row_ok = row < p.M;
+    const int bidx = (row_ok ? row : 0) / p.rows_per_batch;
+    float part = 0.f;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int n = nt * TC_BN + 8 * j + cq;
+      float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+      if (p.bias) {
+        x0 += __ldg(p.bias + n);
+        x1 += __ldg(p.bias + n + 1);
+      }
+      const size_t o = (size_t)row * p.ldo + n;
+      if constexpr (EPI == TC_EPI_P) {
+        const float2 yv = __ldg(reinterpret_cast<const float2*>(p.y + (size_t)bidx * p.N + n));
+        if (row_ok) {
+          *reinterpret_cast<uint32_t*>(p.out0 + o) = pack_bf16(x0, x1);
+          *reinterpret_cast<uint32_t*>(p.out1 + o) = pack_bf16(x0 * yv.x, x1 * yv.y);
         }
+      } else if constexpr (EPI == TC_EPI_ACT) {
+        if (row_ok) *reinterpret_cast<uint32_t*>(p.out0 + o) = pack_bf16(act_ct<ACT>(x0), act_ct<ACT>(x1));
+      } else if constexpr (EPI == TC_EPI_ADDACT) {
+        if (row_ok) {
+          const uint32_t q = __ldg(reinterpret_cast<const unsigned int*>(p.add + o));      // bf16 -> fp32 is a 16-bit shift
+          *reinterpret_cast<uint32_t*>(p.out0 + o) =
+              pack_bf16(act_ct<ACT>(x0 + __uint_as_float(q << 16)), act_ct<ACT>(x1 + __uint_as_float(q & 0xffff0000u)));
+        }
+      } else if constexpr (EPI == TC_EPI_ACT_SPLIT) {
+        if (row_ok) {
+          if (p.addf) {
+            const float2 a = *reinterpret_cast<const float2*>(p.addf + (size_t)row * p.ldaf + n);
+            x0 += a.x;
+            x1 += a.y;
+          }
+          x0 = act_ct<ACT>(x0);
+          x1 = act_ct<ACT>(x1);
+          const uint32_t hw = pack_bf16(x0, x1);
+          *reinterpret_cast<uint32_t*>(p.out0 + o) = hw;
+          *reinterpret_cast<uint32_t*>(p.out0 + o + p.N) =
+              pack_bf16(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xffff0000u));
+        }
+      } else if constexpr (EPI == TC_EPI_F32) {
+        if (row_ok) *reinterpret_cast<float2*>(outf_t + o) = make_float2(act_ct<ACT>(x0), act_ct<ACT>(x1));
+      } else {  // TC_EPI_LOGITS
+        const float2 cc = __ldg(reinterpret_cast<const float2*>(p.ctrl + (size_t)bidx * p.N + n));
+        const float2 ww = make_float2(__ldg(p.wr + n), __ldg(p.wr + n + 1));
+        if (p.out0 && row_ok) *reinterpret_cast<uint32_t*>(p.out0 + o) = pack_bf16(x0, x1);   // I1 kept for backward
+        float t0 = elu_fast(x0 * cc.x), t1 = elu_fast(x1 * cc.y);
+        if (p.e_thresh) {
+          // one Philox draw per aligned column quad of element index row * N + n (the fp32 path's numbering)
+          const uint64_t e = (uint64_t)row * (uint64_t)p.N + (uint64_t)n;
+          const Philox4 rr = philox4x32_10(p.seed, e >> 2, (uint32_t)p.e_site, (uint32_t)p.step);
+          const uint32_t u0 = (e & 2) ? rr.z : rr.x, u1 = (e & 2) ? rr.w : rr.y;
+          t0 = ((u0 >> 8) >= p.e_thresh) ? t0 * p.e_scale : 0.f;
+          t1 = ((u1 >> 8) >= p.e_thresh) ? t1 * p.e_scale : 0.f;
+        }
+        part = fmaf(t0, ww.x, part);
+        part = fmaf(t1, ww.y, part);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer (leader CTA only)
-    if (rank == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(256, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int t = pair0; t < num_tiles; t += pair_stride, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tempty[acc], acc_phase ^ 1);      // both CTAs' epilogues have drained this buffer
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t sa = smem_u32(tiles + stage * C::STAGE_BYTES);
-            const uint64_t adesc = make_sw128_kmajor_desc(sa);
-            const uint64_t bdesc = make_sw128_kmajor_desc(sa + C::A_BYTES);
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k) umma2_bf16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) ? 1u : 0u);
-            umma2_commit_mc(&empty[stage], 0x3);     // both CTAs may refill this slot
-            if (kb == kblocks - 1) umma2_commit_mc(&tfull[acc], 0x3);
-          }
-          __syncwarp();
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
+    if constexpr (EPI == TC_EPI_LOGITS) {
+      // the four lanes of a row hold disjoint column pairs: one partial sum per (row, n-tile)
+      part += __shfl_xor_sync(0xffffffffu, part, 1);
+      part += __shfl_xor_sync(0xffffffffu, part, 2);
+      if (row_ok && (lane & 3) == 0) p.parts[(size_t)row * n_tiles + nt] = part;
     }
-  } else {
-    // ===================================================== epilogue (both CTAs; own 128 rows)
-    const int q = warp & 3;
-    uint32_t* stg = stg_all + (warp - 2) * C::STG_WORDS;
-    const int grp = (warp - 2) >> 2;
-    const int c_begin = grp * (BN / 2), c_end = (grp + 1) * (BN / 2);
-    auto store_bf16_chunk = [&](const uint32_t (&w)[16], __nv_bfloat16* out, int row0, int col0) {
-      __syncwarp();
-      uint4* s4 = reinterpret_cast<uint4*>(stg);
-#pragma unroll
-      for (int g = 0; g < 4; ++g) s4[lane * 4 + (g ^ (lane & 3))] = make_uint4(w[4 * g], w[4 * g + 1], w[4 * g + 2], w[4 * g + 3]);
-      __syncwarp();
-      const int g = lane & 3;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int rr = i * 8 + (lane >> 2);
-        const uint4 v = s4[rr * 4 + (g ^ (rr & 3))];
-        if (row0 + rr < p.M) *reinterpret_cast<uint4*>(out + (size_t)(row0 + rr) * p.ldo + col0 + 8 * g) = v;
-      }
-    };
-    auto store_f32_chunk = [&](const float (&w)[32], float* out, int row0, int col0) {
-      float4* s4 = reinterpret_cast<float4*>(stg);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        __syncwarp();
-#pragma unroll
-        for (int g = 0; g < 4; ++g)
-          s4[lane * 4 + (g ^ (lane & 3))] = make_float4(w[16 * h + 4 * g], w[16 * h + 4 * g + 1], w[16 * h + 4 * g + 2], w[16 * h + 4 * g + 3]);
-        __syncwarp();
-        const int g = lane & 3;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int rr = i * 8 + (lane >> 2);
-          const float4 v = s4[rr * 4 + (g ^ (rr & 3))];
-          if (row0 + rr < p.M) *reinterpret_cast<float4*>(out + (size_t)(row0 + rr) * p.ldo + col0 + 16 * h + 4 * g) = v;
-        }
-      }
-    };
-    const int etid = threadIdx.x - 64;
-    const float* vec_src = (EPI == TC_EPI_P) ? p.y : (EPI == TC_EPI_LOGITS ? p.ctrl : nullptr);
-    int it = 0;
-    for (int t = pair0; t < num_tiles; t += pair_stride, ++it) {
-      const int mp = t / n_tiles, nt = t % n_tiles;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int tile_row0 = mp * 256 + (int)rank * 128;
-      float* par = par_all + acc * (C::PAR_ROWS * BN);
-      const int b_lo = min(tile_row0, p.M - 1) / p.rows_per_batch;
-      const int last_row = max(min(p.M, tile_row0 + 128) - 1, min(tile_row0, p.M - 1));
-      const int nvec = vec_src ? (last_row / p.rows_per_batch - b_lo + 1) : 0;
-      const bool vec_smem = nvec <= TC_MAX_VEC;
-      {
-        const int nb = nt * BN;
-        for (int i = etid; i < BN; i += 32 * TC_EPI_WARPS) {
-          par[i] = p.bias ? __ldg(p.bias + nb + i) : 0.f;
-          if constexpr (EPI == TC_EPI_LOGITS) par[BN + i] = __ldg(p.wr + nb + i);
-        }
-        if (vec_src && vec_smem)
-          for (int i = etid; i < nvec * BN; i += 32 * TC_EPI_WARPS)
-            par[2 * BN + i] = __ldg(vec_src + (size_t)(b_lo + i / BN) * p.N + nb + (i % BN));
-        asm volatile("bar.sync 1, %0;" ::"n"(32 * TC_EPI_WARPS) : "memory");
-      }
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      const int row0 = tile_row0 + q * 32;
-      const int row = row0 + lane;
-      const bool row_ok = row < p.M;
-      const int bidx = row_ok ? row / p.rows_per_batch : b_lo;
-      const float* vrow = vec_smem ? par + (2 + bidx - b_lo) * BN : nullptr;
-      const uint32_t taddr = tmem_base + acc * BN + ((uint32_t)(q * 32) << 16);
-      float part = 0.f;
-#pragma unroll 1
-      for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(taddr + c0, r);
-        tmem_ld_wait();
-        const int n0 = nt * BN + c0;
-        const float4* bias4 = reinterpret_cast<const float4*>(par + c0);
-        if constexpr (EPI == TC_EPI_P) {
-          const float4* y4 = vec_smem ? reinterpret_cast<const float4*>(vrow + c0)
-                                      : reinterpret_cast<const float4*>(p.y + (size_t)bidx * p.N + n0);
-          uint32_t w0[16], w1[16];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b0 = bias4[j / 4], y0 = y4[j / 4];
-            const float x0 = __uint_as_float(r[j]) + b0.x, x1 = __uint_as_float(r[j + 1]) + b0.y;
-            const float x2 = __uint_as_float(r[j + 2]) + b0.z, x3 = __uint_as_float(r[j + 3]) + b0.w;
-            w0[j / 2] = pack_bf16(x0, x1);
-            w0[j / 2 + 1] = pack_bf16(x2, x3);
-            w1[j / 2] = pack_bf16(x0 * y0.x, x1 * y0.y);
-            w1[j / 2 + 1] = pack_bf16(x2 * y0.z, x3 * y0.w);
-          }
-          store_bf16_chunk(w0, p.out0, row0, n0);
-          store_bf16_chunk(w1, p.out1, row0, n0);
-        } else if constexpr (EPI == TC_EPI_ACT) {
-          uint32_t w0[16];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b0 = bias4[j / 4];
-            w0[j / 2] = pack_bf16(act_ct<ACT>(__uint_as_float(r[j]) + b0.x), act_ct<ACT>(__uint_as_float(r[j + 1]) + b0.y));
-            w0[j / 2 + 1] = pack_bf16(act_ct<ACT>(__uint_as_float(r[j + 2]) + b0.z), act_ct<ACT>(__uint_as_float(r[j + 3]) + b0.w));
-          }
-          store_bf16_chunk(w0, p.out0, row0, n0);
-        } else if constexpr (EPI == TC_EPI_F32) {
-          float w0[32];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b0 = bias4[j / 4];
-            w0[j] = act_ct<ACT>(__uint_as_float(r[j]) + b0.x);
-            w0[j + 1] = act_ct<ACT>(__uint_as_float(r[j + 1]) + b0.y);
-            w0[j + 2] = act_ct<ACT>(__uint_as_float(r[j + 2]) + b0.z);
-            w0[j + 3] = act_ct<ACT>(__uint_as_float(r[j + 3]) + b0.w);
-          }
-          store_f32_chunk(w0, p.outf, row0, n0);
-        } else {
-          const float4* c4 = vec_smem ? reinterpret_cast<const float4*>(vrow + c0)
-                                      : reinterpret_cast<const float4*>(p.ctrl + (size_t)bidx * p.N + n0);
-          const float4* w4 = reinterpret_cast<const float4*>(par + BN + c0);
-          uint32_t w0[16];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b0 = bias4[j / 4], cc = c4[j / 4], ww = w4[j / 4];
-            const float i0 = __uint_as_float(r[j]) + b0.x, i1 = __uint_as_float(r[j + 1]) + b0.y;
-            const float i2 = __uint_as_float(r[j + 2]) + b0.z, i3 = __uint_as_float(r[j + 3]) + b0.w;
-            w0[j / 2] = pack_bf16(i0, i1);
-            w0[j / 2 + 1] = pack_bf16(i2, i3);
-            float t0 = elu_fast(i0 * cc.x), t1 = elu_fast(i1 * cc.y), t2 = elu_fast(i2 * cc.z), t3 = elu_fast(i3 * cc.w);
-            if (p.e_thresh) {
-              const uint64_t e = (uint64_t)row * (uint64_t)p.N + (uint64_t)(n0 + j);
-              const Philox4 rr = philox4x32_10(p.seed, e >> 2, (uint32_t)p.e_site, (uint32_t)p.step);
-              t0 = ((rr.x >> 8) >= p.e_thresh) ? t0 * p.e_scale : 0.f;
-              t1 = ((rr.y >> 8) >= p.e_thresh) ? t1 * p.e_scale : 0.f;
-              t2 = ((rr.z >> 8) >= p.e_thresh) ? t2 * p.e_scale : 0.f;
-              t3 = ((rr.w >> 8) >= p.e_thresh) ? t3 * p.e_scale : 0.f;
-            }
-            part = fmaf(t0, ww.x, part);
-            part = fmaf(t1, ww.y, part);
-            part = fmaf(t2, ww.z, part);
-            part = fmaf(t3, ww.w, part);
-          }
-          if (p.out0) store_bf16_chunk(w0, p.out0, row0, n0);
-        }
-      }
-      if constexpr (EPI == TC_EPI_LOGITS) {
-        if (row_ok) p.parts[((size_t)row * n_tiles + nt) * 2 + grp] = part;
-      }
-      // release the accumulator buffer: every epilogue warp of both CTAs arrives on the LEADER's barrier
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (rank == 0) mbar_arrive(&tempty[acc]);
-        else mbar_arrive_remote(&tempty[acc], 0);
-      }
-    }
-  }
-
-  // ---- teardown: nobody leaves while the partner may still signal it or read its shared memory
-  tc_fence_before();
-  __syncthreads();
-  cluster_barrier();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, C::TMEM_COLS);
   }
 }
 
 // ------------------------------------------------------------------ host side
-inline int tc_num_sms() {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return sms;
-}
+inline int tc_num_sms() { return mac_num_sms(); }
 
-template <int BM, int BN, int EPI, int ACT>
+template <int EPI, int ACT>
 inline int tc_gemm_launch_t(const CUtensorMap& ma0, const CUtensorMap& ma1, const CUtensorMap& mb,
                             const TcGemmParams& p, cudaStream_t stream) {
-  auto kern = tc_gemm_kernel<BM, BN, EPI, ACT>;
-  MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<BM, BN>::SMEM_BYTES));
-  const int tiles = ((p.M + BM - 1) / BM) * (p.N / BN) * (p.ksplit > 1 ? p.ksplit : 1);
-  // persistent grid balanced over the rounds: same makespan as one CTA per SM, but e.g. 196 tiles run as 98 CTAs x 2
-  // tiles (epilogue of the first overlaps the MMAs of the second) and leave 50 SMs to concurrent streams
-  const int rounds = (tiles + tc_num_sms() - 1) / tc_num_sms();
-  const int grid = (tiles + rounds - 1) / rounds;
-  kern<<<grid, TC_THREADS1, TcCfg<BM, BN>::SMEM_BYTES, stream>>>(ma0, ma1, mb, p);
+  auto kern = tc_gemm_kernel<EPI, ACT>;
+  // the shared-memory opt-in belongs to the current device's context: set it on every launch
+  MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
+  const dim3 grid(p.N / TC_BN, (p.M + TC_BM - 1) / TC_BM, p.ksplit > 1 ? p.ksplit : 1);
+  kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(ma0, ma1, mb, p);
   MAC_LAUNCH_CHECK();
   return MAC_OK;
 }
 
-template <int BM, int BN>
 inline int tc_gemm_dispatch(const CUtensorMap& ma0, const CUtensorMap& ma1, const CUtensorMap& mb,
                             const TcGemmParams& p, cudaStream_t stream) {
   switch (p.epi) {
-    case TC_EPI_P: return tc_gemm_launch_t<BM, BN, TC_EPI_P, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
+    case TC_EPI_P: return tc_gemm_launch_t<TC_EPI_P, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
     case TC_EPI_ADDACT:
-      if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<BM, BN, TC_EPI_ADDACT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
+      if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<TC_EPI_ADDACT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
       return MAC_ERR_UNSUPPORTED;
-    case TC_EPI_LOGITS: return tc_gemm_launch_t<BM, BN, TC_EPI_LOGITS, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
+    case TC_EPI_LOGITS: return tc_gemm_launch_t<TC_EPI_LOGITS, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
     case TC_EPI_ACT_SPLIT:
-      if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<BM, BN, TC_EPI_ACT_SPLIT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
-      if (p.act == MAC_ACT_NON) return tc_gemm_launch_t<BM, BN, TC_EPI_ACT_SPLIT, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
+      if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<TC_EPI_ACT_SPLIT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
+      if (p.act == MAC_ACT_NON) return tc_gemm_launch_t<TC_EPI_ACT_SPLIT, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
       return MAC_ERR_UNSUPPORTED;
     case TC_EPI_ACT:
-      if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<BM, BN, TC_EPI_ACT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
-      if (p.act == MAC_ACT_NON) return tc_gemm_launch_t<BM, BN, TC_EPI_ACT, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
+      if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<TC_EPI_ACT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
+      if (p.act == MAC_ACT_NON) return tc_gemm_launch_t<TC_EPI_ACT, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
       return MAC_ERR_UNSUPPORTED;
     case TC_EPI_F32:
       switch (p.act) {
-        case MAC_ACT_NON: return tc_gemm_launch_t<BM, BN, TC_EPI_F32, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
-        case MAC_ACT_TANH: return tc_gemm_launch_t<BM, BN, TC_EPI_F32, MAC_ACT_TANH>(ma0, ma1, mb, p, stream);
-        case MAC_ACT_SIGMOID: return tc_gemm_launch_t<BM, BN, TC_EPI_F32, MAC_ACT_SIGMOID>(ma0, ma1, mb, p, stream);
-        case MAC_ACT_ELU: return tc_gemm_launch_t<BM, BN, TC_EPI_F32, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
-        case MAC_ACT_RELU: return tc_gemm_launch_t<BM, BN, TC_EPI_F32, MAC_ACT_RELU>(ma0, ma1, mb, p, stream);
+        case MAC_ACT_NON: return tc_gemm_launch_t<TC_EPI_F32, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
+        case MAC_ACT_TANH: return tc_gemm_launch_t<TC_EPI_F32, MAC_ACT_TANH>(ma0, ma1, mb, p, stream);
+        case MAC_ACT_SIGMOID: return tc_gemm_launch_t<TC_EPI_F32, MAC_ACT_SIGMOID>(ma0, ma1, mb, p, stream);
+        case MAC_ACT_ELU: return tc_gemm_launch_t<TC_EPI_F32, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
+        case MAC_ACT_RELU: return tc_gemm_launch_t<TC_EPI_F32, MAC_ACT_RELU>(ma0, ma1, mb, p, stream);
       }
       return MAC_ERR_UNSUPPORTED;
   }
   return MAC_ERR_UNSUPPORTED;
-}
-
-template <int EPI, int ACT>
-inline int tc2_gemm_launch_t(const CUtensorMap& ma0, const CUtensorMap& ma1, const CUtensorMap& mb,
-                             const TcGemmParams& p, cudaStream_t stream) {
-  auto kern = tc2_gemm_kernel<EPI, ACT>;
-  MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Tc2Cfg::SMEM_BYTES));
-  const int tiles = ((p.M + 255) / 256) * (p.N / Tc2Cfg::BN);
-  const int max_pairs = tc_num_sms() / 2;
-  const int rounds = (tiles + max_pairs - 1) / max_pairs;
-  const int pairs = (tiles + rounds - 1) / rounds;        // balanced: 98 pair-tiles -> 49 pairs x 2 tiles (98 SMs)
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pairs, 1, 1);
-  cfg.blockDim = dim3(TC_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = Tc2Cfg::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  MAC_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma0, ma1, mb, p));
-  MAC_LAUNCH_CHECK();
-  return MAC_OK;
-}
-
-inline int tc2_gemm_dispatch(const CUtensorMap& ma0, const CUtensorMap& ma1, const CUtensorMap& mb,
-                             const TcGemmParams& p, cudaStream_t stream) {
-  switch (p.epi) {
-    case TC_EPI_P: return tc2_gemm_launch_t<TC_EPI_P, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
-    case TC_EPI_LOGITS: return tc2_gemm_launch_t<TC_EPI_LOGITS, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
-    case TC_EPI_ACT:
-      if (p.act == MAC_ACT_ELU) return tc2_gemm_launch_t<TC_EPI_ACT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
-      if (p.act == MAC_ACT_NON) return tc2_gemm_launch_t<TC_EPI_ACT, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
-      return MAC_ERR_UNSUPPORTED;
-    case TC_EPI_F32:
-      if (p.act == MAC_ACT_NON) return tc2_gemm_launch_t<TC_EPI_F32, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
-      if (p.act == MAC_ACT_ELU) return tc2_gemm_launch_t<TC_EPI_F32, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
-      if (p.act == MAC_ACT_TANH) return tc2_gemm_launch_t<TC_EPI_F32, MAC_ACT_TANH>(ma0, ma1, mb, p, stream);
-      return MAC_ERR_UNSUPPORTED;
-  }
-  return MAC_ERR_UNSUPPORTED;
-}
-
-// Tile shape: minimise rounds-over-the-SMs x measured cycles per k-block of one tile.  SS-mode UMMAs are fed ~55-64 B/clk
-// from shared memory (profiles/r1/NOTES.md): a 128x256x16 UMMA takes ~224 cycles, a 128x128x16 one ~149, so per
-// k-block: 256x256 -> 1792, 128x256 -> 896 (fill needs 768), 128x128 -> ~620.  Ties go to 128x256: with the balanced
-// persistent grid it runs as 2 tiles per CTA and hides the first tile's epilogue under the second tile's MMAs
-// (measured 21.2k vs 20.9k (256x256) vs 19.4k (128x128) reasoning-steps/s at the headline shape).  Returns BM*1000 + BN.
-inline int tc_pick_tile(int M, int N) {
-  const int sms = tc_num_sms();
-  auto cost = [&](int bm, int bn, int per_tile) {
-    if (N % bn) return 1 << 30;
-    const int tiles = ((M + bm - 1) / bm) * (N / bn);
-    return ((tiles + sms - 1) / sms) * per_tile;
-  };
-  int best = 128256, bc = cost(128, 256, 896);
-  const int c3 = cost(256, 256, 1792), c1 = cost(128, 128, 620);
-  if (c3 < bc) { best = 256256; bc = c3; }
-  if (c1 < bc) { best = 128128; bc = c1; }
-  return best;
 }
 
 // A = [a0 (K0 cols) | a1 (K1 cols)] bf16 row-major (ld = own K), Wt bf16 [N, K0+K1]
@@ -1007,54 +357,24 @@ inline int tc_gemm_launch(const void* a0, int K0, const void* a1, int K1, const 
   if (ldw == 0) ldw = K0 + K1;                  // row pitch of Wt in elements (> K: a column block of a wider weight)
   if (lda0 == 0) lda0 = K0;                     // row pitch of the A segments (> K: a column block of a wider matrix)
   if (lda1 == 0) lda1 = K1;
-  if (p.M <= 0 || p.N <= 0 || (p.N % 128) || (K0 % TC_BK) || (K1 % TC_BK) || K0 <= 0) return MAC_ERR_UNSUPPORTED;
+  if (p.M <= 0 || p.N <= 0 || (p.N % TC_BN) || (K0 % TC_BK) || (K1 % TC_BK) || K0 <= 0) return MAC_ERR_UNSUPPORTED;
   if (!mac_aligned16(a0) || !mac_aligned16(wt)) return MAC_ERR_ALIGN;
-  int tile = tc_pick_tile(p.M, p.N);
-  if (const char* e = getenv("MAC_TC_TILE")) {
-    const int v = atoi(e);
-    if ((v == 128128 || v == 128256 || v == 256256) && p.N % (v % 1000) == 0) tile = v;
-  }
-  if (const char* e = getenv("MAC_TC_DEBUG")) p.debug = atoi(e);
-  // cta_group::2 pair kernel (opt-in while it is being qualified): MAC_TC_PAIR=1
-  bool pair = false;
-  if (const char* e = getenv("MAC_TC_PAIR"))
-    pair = atoi(e) != 0 && (p.N % 256 == 0) && p.M > 128 && p.epi != TC_EPI_ADDACT && p.epi != TC_EPI_ACT_SPLIT &&
-           lda0 == K0 && lda1 == K1 && p.ksplit <= 1;
-  if (pair) {
-    if (nparts_per_row) *nparts_per_row = (p.N / 256) * 2;
-    p.K = K0 + K1;
-    p.kblocks0 = K0 / TC_BK;
-    CUtensorMap ma0, ma1, mb;
-    int st = make_tmap_2d(&ma0, a0, 1, (uint64_t)p.M, (uint64_t)K0, (uint64_t)K0 * 2, 128, TC_BK, 1);
-    if (st != MAC_OK) return st;
-    if (K1 > 0) {
-      st = make_tmap_2d(&ma1, a1, 1, (uint64_t)p.M, (uint64_t)K1, (uint64_t)K1 * 2, 128, TC_BK, 1);
-      if (st != MAC_OK) return st;
-    } else {
-      ma1 = ma0;
-    }
-    st = make_tmap_2d(&mb, wt, 1, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)ldw * 2, 128, TC_BK, 1);
-    if (st != MAC_OK) return st;
-    return tc2_gemm_dispatch(ma0, ma1, mb, p, stream);
-  }
-  const int BM = tile / 1000, BN = tile % 1000;
-  if (nparts_per_row) *nparts_per_row = (p.N / BN) * (BM == 256 ? 2 : 4);
+  if (p.ksplit > 1 && ((K0 + K1) / TC_BK) % p.ksplit) return MAC_ERR_UNSUPPORTED;
+  if (nparts_per_row) *nparts_per_row = p.N / TC_BN;
   p.K = K0 + K1;
   p.kblocks0 = K0 / TC_BK;
   CUtensorMap ma0, ma1, mb;
-  int st = make_tmap_2d(&ma0, a0, 1, (uint64_t)p.M, (uint64_t)K0, (uint64_t)lda0 * 2, (uint32_t)BM, TC_BK, 1);
+  int st = make_tmap_2d(&ma0, a0, 1, (uint64_t)p.M, (uint64_t)K0, (uint64_t)lda0 * 2, (uint32_t)TC_BM, TC_BK, 1);
   if (st != MAC_OK) return st;
   if (K1 > 0) {
-    st = make_tmap_2d(&ma1, a1, 1, (uint64_t)p.M, (uint64_t)K1, (uint64_t)lda1 * 2, (uint32_t)BM, TC_BK, 1);
+    st = make_tmap_2d(&ma1, a1, 1, (uint64_t)p.M, (uint64_t)K1, (uint64_t)lda1 * 2, (uint32_t)TC_BM, TC_BK, 1);
     if (st != MAC_OK) return st;
   } else {
     ma1 = ma0;
   }
-  st = make_tmap_2d(&mb, wt, 1, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)ldw * 2, (uint32_t)BN, TC_BK, 1);
+  st = make_tmap_2d(&mb, wt, 1, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)ldw * 2, (uint32_t)TC_BN, TC_BK, 1);
   if (st != MAC_OK) return st;
-  if (tile == 256256) return tc_gemm_dispatch<256, 256>(ma0, ma1, mb, p, stream);
-  if (tile == 128256) return tc_gemm_dispatch<128, 256>(ma0, ma1, mb, p, stream);
-  return tc_gemm_dispatch<128, 128>(ma0, ma1, mb, p, stream);
+  return tc_gemm_dispatch(ma0, ma1, mb, p, stream);
 }
 
 // fp32 [K, N] (in, out) weight -> bf16 [N, K] (out, in): the K-major B operand of the forward GEMMs
@@ -1228,9 +548,12 @@ inline int tc_read_chain(const float* kb_f32, const void* kb_bf16, const float* 
 // do not depend on the step.  They are computed once per forward into `inv` = [P | Q] (bf16), and each step runs
 //   PY = P * y_b ;  H = ELU(PY @ Wm[0:d, :] + Q) ;  logits = ... (unchanged)
 // i.e. 2 x d instead of 4 x d MACs per knowledge-base element and step.
+// [P | Q] bf16 slabs, then the scratch of the fused read step (read_step.cuh): P*y and H slabs, the logit partial sums
+// [B*N, d / TC_BN] and y [B, d]
 inline size_t tc_read_invariant_bytes(int B, int N, int d) {
-  // [P | Q] bf16 slabs + the per-tile softmax partials of the packed fused read step (read_step.cuh: B x 3 x (512 + 2) floats)
-  return (size_t)2 * (((size_t)B * N * d * 2 + 1023) & ~(size_t)1023) + 1024 + (size_t)B * 3 * (512 + 2) * sizeof(float) + 1024;
+  const size_t slab = (((size_t)B * N * d * 2 + 1023) & ~(size_t)1023);
+  const size_t parts = (((size_t)B * N * (d / TC_BN) * 4 + 1023) & ~(size_t)1023);
+  return 4 * slab + parts + (size_t)B * d * 4 + 1024;
 }
 
 // PY[m, :] = P[m, :] * y[m / rows_per_batch, :]   (8 bf16 per thread)
@@ -1252,6 +575,24 @@ __global__ void scale_rows_bf16_kernel(const uint4* __restrict__ P, const float*
 
 inline char* tc_align1k(void* p) {
   return reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~(uintptr_t)1023);
+}
+
+struct TcReadScratch {
+  __nv_bfloat16 *P, *Q, *PY, *H;
+  float *parts, *y;
+};
+inline TcReadScratch tc_read_scratch(void* inv, int B, int N, int d) {
+  const size_t slab = (((size_t)B * N * d * 2 + 1023) & ~(size_t)1023);
+  const size_t parts = (((size_t)B * N * (d / TC_BN) * 4 + 1023) & ~(size_t)1023);
+  char* base = tc_align1k(inv);
+  TcReadScratch s;
+  s.P = reinterpret_cast<__nv_bfloat16*>(base);
+  s.Q = reinterpret_cast<__nv_bfloat16*>(base + slab);
+  s.PY = reinterpret_cast<__nv_bfloat16*>(base + 2 * slab);
+  s.H = reinterpret_cast<__nv_bfloat16*>(base + 3 * slab);
+  s.parts = reinterpret_cast<float*>(base + 4 * slab);
+  s.y = reinterpret_cast<float*>(base + 4 * slab + parts);
+  return s;
 }
 
 inline int tc_read_invariant(const void* kb_bf16, const mac_read_weights* w, void* inv, size_t inv_bytes, int B, int N,
@@ -1327,7 +668,7 @@ __global__ void splitk_accum_kernel(const float4* __restrict__ part, float4* __r
   dst[i] = a;
 }
 
-// largest S <= 28 that divides K / 64, keeps >= 2 k-blocks per slice and at most two waves of tiles
+// largest S <= 28 that divides K / 64, keeps >= 2 k-blocks per slice and at most two CTAs per SM
 inline int tc_pick_ksplit(int K, int out_tiles) {
   const int kblocks = K / TC_BK;
   int best = 1;
@@ -1344,7 +685,7 @@ inline int tc_wgrad_splitk(const void* xT, const void* gT, float* dW, float* par
   TcGemmParams p{};
   p.M = in_dim; p.N = out_dim; p.act = MAC_ACT_NON; p.bias = nullptr; p.ldo = out_dim; p.rows_per_batch = 1;
   p.epi = TC_EPI_F32; p.outf = partial;
-  const int out_tiles = (in_dim / 128) * (out_dim / (out_dim % 256 == 0 ? 256 : 128));
+  const int out_tiles = (in_dim / TC_BM) * (out_dim / TC_BN);
   const int S = tc_pick_ksplit(K, out_tiles);
   p.ksplit = S; p.split_stride = (long long)in_dim * out_dim;
   int st = tc_gemm_launch(xT, K, nullptr, 0, gT, p, stream);

@@ -69,7 +69,7 @@ extern "C" const char* mac_b200_strerror(int status) {
     case MAC_ERR_ALIGN: return "pointer or stride not 16-byte aligned";
     case MAC_ERR_UNSUPPORTED: return "flag/shape combination outside the fused path";
     case MAC_ERR_WORKSPACE: return "workspace too small";
-    case MAC_ERR_ARCH: return "device is not sm_100 or the tensor-map driver entry point is missing";
+    case MAC_ERR_ARCH: return "device is not sm_90 or the tensor-map driver entry point is missing";
     default: return status > 0 ? cudaGetErrorString((cudaError_t)status) : "unknown mac_b200 status";
   }
 }
@@ -77,9 +77,10 @@ extern "C" const char* mac_b200_strerror(int status) {
 extern "C" int mac_b200_device_ok(void) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  int major = 0;
+  int major = 0, minor = 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
+  return major == 9 && minor == 0 ? 1 : 0;
 }
 
 // ------------------------------------------------------------------------------------------------ linear
@@ -205,8 +206,6 @@ extern "C" int mac_step_fused(const void* inv, const void* kb_bf16, const float*
 }
 extern "C" int mac_step_fused_supported(int B, int N, int d) { return whole_step_supported(B, N, d) ? 1 : 0; }
 
-extern "C" void mac_dbg_read_step_timestamps(long long* dev_buf) { read_step_dbg_ptr() = dev_buf; }
-extern "C" void mac_dbg_read_step_flags(int flags) { read_step_dbg_flags() = flags; }
 extern "C" int mac_read_step_fused_supported(int B, int N, int d) { return read_step_supported(B, N, d) ? 1 : 0; }
 
 extern "C" int mac_read_fwd(const float* kb, const void* kb_bf16, const float* memory_in, const float* control,
@@ -510,7 +509,7 @@ extern "C" int mac_widen_bf16(const void* const* src_bf16, float* const* dst, in
     d[i] = reinterpret_cast<float4*>(dst[i]);
   }
   const long long n8 = n / 8;
-  const unsigned gx = (unsigned)std::min<long long>((n8 + 255) / 256, 148 * 16);
+  const unsigned gx = (unsigned)std::min<long long>((n8 + 255) / 256, (long long)mac_num_sms() * 16);
   widen3_bf16_kernel<<<dim3(gx, nslab), 256, 0, stream>>>(s[0], s[1], s[2], d[0], d[1], d[2], n8);
   MAC_LAUNCH_CHECK();
   return MAC_OK;

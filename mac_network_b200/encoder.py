@@ -9,7 +9,7 @@ optional `projCW` / `projQ` linears (`encProj`, or `encDim != ctrlDim`).
     questionCntxWords  [B,S,encDim] = [h_fw(t), h_bw(t)], zero for t >= length
     vecQuestions       [B,encDim]   = dropout([h_fw(len-1), h_bw(0)])
 
-B200 formulation (csrc/encoder.cu): the input half of both LSTM kernels is one GEMM each over all S steps
+GPU formulation (csrc/encoder.cu): the input half of both LSTM kernels is one GEMM each over all S steps
 (`mac_linear_fwd`), the recurrence is one launch per step for both directions with the gate math, the length masking and
 the backward direction's per-row time reversal fused behind the `[B,h] x [h,4h]` product; BPTT mirrors it and turns the
 weight / input gradients of all steps into GEMMs over the `[B*S, 4h]` gate-gradient matrix.  Variable names follow the

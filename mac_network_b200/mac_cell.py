@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's MAC cell over the sm_100a kernels in libmac_b200.so.
+"""Host-side mirror of the reference's MAC cell over the sm_90a kernels in libmac_b200.so.
 
 Same call surface as `/root/reference/mac_cell.py`:
 
@@ -150,7 +150,7 @@ class MACCell(object):
             raise TypeError("config must be a MACConfig")
         self.cfg.validate()
         c = self.cfg
-        # which units run on the fused sm_100a kernels; everything else goes through the general (composed) path
+        # which units run on the fused sm_90a kernels; everything else goes through the general (composed) path
         self._fused_read = c.is_fast_path
         self._fused_write = (c.writeInputs == "BOTH" and c.writeMemProj and not c.writeConcatMul and not c.writeInfoProj
                              and c.writeInfoAct == "NON" and not c.writeMergeCtrl and c.writeMemAct == "NON")
@@ -189,21 +189,19 @@ class MACCell(object):
         self._read_hoist = (self._fused_read and not c.unsharedCells and not save_for_backward
                             and os.environ.get("MAC_NO_READ_HOIST", "0") != "1")
         # plain write unit: its GEMM also produces the next step's memory projection.  It shortens the dependency chain of
-        # ONE pass (17.0k vs fewer reasoning-steps/s with a single pass in flight); with >= 4 independent passes in flight the
-        # two smaller GEMMs pack better (25.4k vs 24.2k at 6 passes, profiles/r1/sweep_r1.jsonl), so throughput callers pass
-        # fold_y=False.  fold_y=None: on unless env MAC_NO_FOLD_Y=1.
+        # ONE pass; with several independent passes in flight the two smaller GEMMs can pack better, so throughput callers
+        # may pass fold_y=False.  fold_y=None: on unless env MAC_NO_FOLD_Y=1.
         want_fold = (os.environ.get("MAC_NO_FOLD_Y", "0") != "1") if fold_y is None else bool(fold_y)
         self._fold_y = (self._read_hoist and self._fused_write and not (c.writeSelfAtt or c.writeGate)
                         and not (c.writeDropout < 1.0 and float(writeDropout) < 1.0) and want_fold)
         self._y_for = -1
         self.kb_bf16 = None
         self.save_for_backward = bool(save_for_backward)
-        # whole-step form (mac_step_fused): the previous step's plain write unit and this step's memory projection run in
-        # the prologue of the fused read-step kernel -> ONE launch per reasoning step.  bf16 inference, shared cells, plain
-        # write unit (no self-attention / gate / write dropout), all dropouts at 1, a CTA pair per sample (d = 512,
-        # 128 < N <= 256).  OPT-IN (MAC_STEP_FUSED=1): measured on the B200 it is slower (22.3k vs 28.3k reasoning-steps/s
-        # at 6 passes in flight) and less accurate (memory 3.8e-3 vs 4.7e-4): per-sample matrix-vector products read the
-        # write / projY weights once per CTA pair -- 98 MB of L2 traffic per step instead of 3 MB for the batched GEMMs.
+        # whole-step form (mac_step_fused): the previous step's plain write unit and this step's memory projection run as
+        # per-sample matrix-vector products in front of the read step.  bf16 inference, shared cells, plain write unit (no
+        # self-attention / gate / write dropout), all dropouts at 1, d = 512, 128 < N <= 256.  OPT-IN (MAC_STEP_FUSED=1):
+        # the per-sample products read the write / projY weights once per sample (bf16 weights: less accurate than the
+        # batched split-bf16 GEMMs).
         self._step_fused = bool(
             self._read_hoist and self.prec == PREC["bf16"] and self._fused_write and not (c.writeSelfAtt or c.writeGate)
             and not (c.writeDropout < 1.0 and float(writeDropout) < 1.0) and float(readDropout) >= 1.0
@@ -212,10 +210,9 @@ class MACCell(object):
             and self.lib.mac_step_fused_supported(B, N, d) == 1)
         # bf16 inference: the batch-sized projections of the step (projY, write unit, gate, ctrlProj) on tensor cores as
         # three-pass split-bf16 products (mac_linear_tc_small_fwd, fp32-class accuracy): 16-32 independent CTAs that can run
-        # beside another pass's 128-CTA read kernel, which the 8-CTA-cluster fp32 kernel cannot.  Measured on the B200
-        # (headline shape): 29.9k vs 28.4k reasoning-steps/s with 6 passes in flight, but 15.9k vs 21.4k with ONE pass (the
-        # kernel's own latency is 2x the cluster kernel's), so it is the THROUGHPUT form: small_tc=True (callers with
-        # several passes in flight: bench.py, serving.HostPipeline), or MAC_SMALL_TC=1; default off.
+        # beside another pass's read kernels, which the 8-CTA-cluster fp32 kernel cannot; its own latency is higher than the
+        # cluster kernel's, so it is the THROUGHPUT form: small_tc=True (callers with several passes in flight: bench.py,
+        # serving.HostPipeline), or MAC_SMALL_TC=1; default off.
         want_tc = (os.environ.get("MAC_SMALL_TC", "0") == "1") if small_tc is None else bool(small_tc)
         self._small_tc = bool(want_tc and self.prec == PREC["bf16"] and not save_for_backward and B <= 128 and d % 64 == 0
                               and self._fused_write and os.environ.get("MAC_SMALL_TC", "1") != "0")
@@ -287,7 +284,7 @@ class MACCell(object):
         return self.params.derived(("split16", key), build)
 
     def _linear_tc(self, xs, key, W, b, out, act="NON", bias_const=0.0, y2=None, n_split=0, gate=None):
-        """ops.linear on [M <= 128, sum k] segments as a three-pass split-bf16 tcgen05 product (mac_linear_tc_small_fwd).
+        """ops.linear on [M <= 128, sum k] segments as a three-pass split-bf16 wgmma product (mac_linear_tc_small_fwd).
         `gate` = (new, old, z_out): the write gate epilogue (mac_cell.py:358-367)."""
         n = len(xs)
         hi, lo = self._split_weight(key, W)
@@ -474,7 +471,7 @@ class MACCell(object):
                          Wm2.data_ptr(), bm2.data_ptr(), p[lsc + "weights/weight"].data_ptr(),
                          p.scalar(lsc + "biases/bias"), None, None, None)
         if self.prec == PREC["bf16"]:
-            def pack(t):       # fp32 [in, out] -> bf16 [out, in] (K-major B operand of tcgen05.mma)
+            def pack(t):       # fp32 [in, out] -> bf16 [out, in] (K-major B operand of wgmma)
                 o = torch.empty((t.shape[1], t.shape[0]), dtype=torch.bfloat16, device=t.device)
                 check(self.lib.mac_pack_weight_bf16(ptr(t), ptr(o), t.shape[0], t.shape[1], stream_ptr()), "pack")
                 return o

@@ -1,4 +1,4 @@
-"""Run surface of the reference's `MACnet` (`/root/reference/model.py`) over the B200 kernels: the one call the reference's
+"""Run surface of the reference's `MACnet` (`/root/reference/model.py`) over the sm_90a kernels: the one call the reference's
 training / evaluation loop makes per batch,
 
     res = model.runBatch(sess, data, images, train, getAtt)          # model.py:732-760

@@ -162,8 +162,7 @@ class HostPipeline(object):
         """`host_cast`: None = decide here (bf16 path: cast the knowledge base to bf16 on the host if that is faster than the
         PCIe time it saves); False = never.  Callers that run several ranks per socket pass False: the cast makes a pass touch
         ~57 MB of host DRAM (fp32 read + bf16 write + DMA read) instead of 31 MB, and the ranks of one socket share its memory
-        bandwidth -- measured on the 2-socket B200 host: 26.4k reasoning-steps/s end to end with one rank, 29.0k TOTAL with two
-        ranks on the same socket, i.e. the cast was bandwidth-bound at ~135 GB/s of host DRAM traffic per socket."""
+        bandwidth."""
         self.lib = _lib.load()
         self.shape = shape
         self.prec = prec

@@ -3,9 +3,9 @@
 dropout on the layer input, 3x3 stride-1 SAME convolution (HWIO kernel) + bias, ELU after every layer; then the
 `[B,H,W,d] -> [B, H*W, d]` reshape.  177.6 GFLOP per B=64 batch (56 % of the twelve cell steps).
 
-B200 formulation: convolution as GEMM.  `mac_im2col3x3` builds the `[B*H*W, 9*C]` patch matrix (tap-major, channel fastest
+GPU formulation: convolution as GEMM.  `mac_im2col3x3` builds the `[B*H*W, 9*C]` patch matrix (tap-major, channel fastest
 -- exactly the row-major reshape of the HWIO kernel to `[9*C, Cout]`) with the input dropout fused (the Philox mask is
-indexed by the SOURCE element, so all nine copies of a pixel share its mask), in bf16 for the tcgen05 GEMM
+indexed by the SOURCE element, so all nine copies of a pixel share its mask), in bf16 for the wgmma GEMM
 (`mac_linear_tc_fwd`, ELU epilogue) or fp32 for the parity GEMM (`mac_linear_fwd`)."""
 import collections
 import ctypes

@@ -1,7 +1,7 @@
 """ONE headline-shaped inference pass (B=64, S=40, N=196, d=512, netLength=12) in the throughput form the bench uses (bf16,
 fused read step, tensor-core write + projY), without CUDA graphs, between cudaProfilerStart/Stop after three warm passes:
     ncu --profile-from-start off --metrics gpu__time_duration.sum,launch__grid_size --clock-control none --csv --log-file X python profiles/one_pass.py
-    ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:read_step2 -c 1 -o Y python profiles/one_pass.py"""
+    ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:read_step_kernel -c 1 -o Y python profiles/one_pass.py"""
 import os
 import sys
 

@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
     # a GPU-marked test on a box without a GPU is an error of invocation, not a skip-and-pass:
-    # the driver runs `-m "not gpu"` here and `-m gpu` on the B200.
+    # run `-m "not gpu"` without a GPU and `-m gpu` on the H100.
     try:
         import torch
         has_gpu = torch.cuda.is_available()

@@ -130,7 +130,7 @@ def test_dropout_rng_matches_independent_philox():
 @pytest.mark.parametrize("M,K,N,act", [(12544, 512, 512, "NON"), (300, 1024, 256, "ELU"), (128, 64, 256, "NON"),
                                        (3136, 512, 512, "TANH")])
 def test_linear_tensor_core(M, K, N, act):
-    """tcgen05/TMEM GEMM (bf16 operands, fp32 accumulate) against an fp64 product of the same bf16-rounded operands."""
+    """wgmma GEMM (bf16 operands, fp32 accumulate) against an fp64 product of the same bf16-rounded operands."""
     L, lib = _lib()
     rng = np.random.RandomState(3)
     x = torch.from_numpy(rng.standard_normal((M, K)).astype(np.float32)).cuda().to(torch.bfloat16)

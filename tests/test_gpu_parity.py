@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a kernels (through the C ABI / MACCell host mirror) against the fp64 oracle and
+"""GPU parity: the sm_90a kernels (through the C ABI / MACCell host mirror) against the fp64 oracle and
 against the golden fixtures produced by the unmodified reference.  Tolerance (BASELINE.json north_star):
 fp32 projections within 1e-4 relative (max |x - ref| / max |ref| per tensor), probabilities with a 1e-6
 absolute floor."""
@@ -168,7 +168,7 @@ def test_inputs_are_not_modified():
 
 @pytest.mark.parametrize("variant,shape", [("args", (8, 12, 196, 512, 4)), ("gqa", (64, 30, 49, 512, 6))])
 def test_bf16_tensor_core_path(variant, shape):
-    """Headline precision (bf16 operands on tcgen05, fp32 accumulate, bf16 knowledge base): error against the fp64
+    """Headline precision (bf16 operands on wgmma, fp32 accumulate, bf16 knowledge base): error against the fp64
     oracle is REPORTED and bounded loosely -- the 1e-4 bar applies to the fp32 path only (DESIGN.md section 5)."""
     B, S, N, d, L = shape
     cfg = MACConfig.args(variant, netLength=L, memDim=d, ctrlDim=d, attDim=d)

@@ -1,5 +1,5 @@
 """Image stem (SURVEY section 8(f) rank 1): oracle vs fixtures from the reference's own ops.CNNLayer (CPU), product
-(fused dropout+im2col kernel + GEMM) vs oracle on the GPU for the fp32 and the tcgen05 bf16 path."""
+(fused dropout+im2col kernel + GEMM) vs oracle on the GPU for the fp32 and the wgmma bf16 path."""
 import json
 import os
 

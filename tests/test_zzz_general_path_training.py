@@ -1,12 +1,12 @@
 """Training-mode forward of the composed (P2) read unit on the GPU: the product draws its Philox masks, the oracle -- pinned
 to the reference's own training run of these flag sets by `tests/golden/p2_read_*_train.npz` -- is fed the same uniforms.
-Written after round 1's GPU budget was spent (then `xfail(strict=False)`); it XPASSed on the B200 and gates since round 2."""
+"""
 import numpy as np
 import pytest
 
 from tests._util import load_golden, rebuild
 
-pytestmark = pytest.mark.gpu       # round 2: gating (all of these XPASSed on the B200 at the end of round 1)
+pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("case", ["p2_read_add_train", "p2_read_plain_train"])

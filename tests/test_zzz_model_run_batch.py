@@ -1,14 +1,12 @@
 """`model.MACnet.runBatch` (the reference's per-batch call, model.py:732-760) on the GPU.  A composition of classes that each
-have their own hardware-validated parity tests (encoder, stem, cell, output unit, trainer); the composition itself was written
-after round 1's GPU budget was spent (then `xfail(strict=False)`; XPASSed on the B200, gating since round 2; see
-tests/test_zzz_tensor_core_training.py)."""
+have their own hardware-validated parity tests (encoder, stem, cell, output unit, trainer)."""
 import numpy as np
 import pytest
 
 from tests._util import max_rel
 from tests.test_full_model import _oracle_loss
 
-pytestmark = pytest.mark.gpu       # round 2: gating (all of these XPASSed on the B200 at the end of round 1)
+pytestmark = pytest.mark.gpu
 
 
 def _batch(B, S, V, C, H, W, A, seed):

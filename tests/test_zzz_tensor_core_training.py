@@ -1,8 +1,7 @@
-"""Mixed-precision TRAINING forms of the cell (DESIGN.md section 9, item 1), written at the end of round 1 after the GPU
-budget of the round was spent: every CUDA entry point they use is validated elsewhere in this suite (mac_linear_tc_fwd,
-mac_pack_weight_bf16, mac_cast_bf16, the fp32 element-wise kernels of the backward), but their COMPOSITION
-(`mac_read_bwd_tc`, the bf16 training forward with widened saved activations) has not yet run on a B200.  The tests are
-were `xfail(strict=False)` in round 1; all of them XPASSed on the driver's B200 (GPUTEST_r01), so since round 2 they GATE.  Tolerances are mixed-precision ones (bf16 operands, fp32
+"""Mixed-precision TRAINING forms of the cell (DESIGN.md section 9, item 1): every CUDA entry point they use is validated
+elsewhere in this suite (mac_linear_tc_fwd, mac_pack_weight_bf16, mac_cast_bf16, the fp32 element-wise kernels of the
+backward); these tests check their COMPOSITION (`mac_read_bwd_tc`, the bf16 training forward with widened saved
+activations).  Tolerances are mixed-precision ones (bf16 operands, fp32
 accumulation), stated per test."""
 import numpy as np
 import pytest
@@ -13,7 +12,7 @@ from mac_network_b200.params import init_params, perturb_biases
 from mac_network_b200.synthetic import make_inputs
 from tests._util import max_rel
 
-pytestmark = pytest.mark.gpu       # round 2: gating (all of these XPASSed on the B200 at the end of round 1)
+pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("prec,tc,tol", [("fp32", True, 3e-2), ("bf16", False, 3e-2), ("bf16", True, 5e-2)])
