@@ -264,7 +264,7 @@ int mac_linear_tc_fwd(const void* x_bf16, const void* wt_bf16, const float* b, i
  *   y[M, n_out] = epilogue( concat_k(x_0 .. x_{nseg-1})[M, K] @ W + b + bias_const ),  M <= 128, fp32 in / fp32 out.
  * mac_pack_weight_bf16_split: fp32 W[K, n_out] -> bf16 hi and lo halves, both [n_out, K] (K-major), W ~= hi + lo.
  * With wt_lo != NULL the product is three wgmma passes (x_hi W_hi + x_lo W_hi + x_hi W_lo, the activations split in the
- * kernel) accumulated in fp32 in tensor memory: fp32-class accuracy (~1e-5) on the tensor pipe, so the recurrent state
+ * kernel) accumulated in fp32 registers: fp32-class accuracy (~1e-5) on the tensor pipe, so the recurrent state
  * does not pass through bf16.  wt_lo == NULL: one plain bf16 pass.
  * Epilogue: act in MAC_ACT_*; y2 != NULL sends columns >= n_split to y2[m, n - n_split] (the folded write unit, see
  * mac_write_fwd_next_y); gate_new != NULL selects the write gate z = sigmoid(t), y = gate_new*z + gate_old*(1-z), z stored

@@ -916,7 +916,7 @@ extern "C" int mac_read_bwd(const float* kb, const float* memory_in, const float
 // mask while it builds the bf16 operand, and writes the row-major bf16 copy of a gradient from the same read); * ELU'(H) with
 // its column sums and the dropout mask on dKB are one fp32 pass each.  The arithmetic of every pass is the forward's, so the
 // masks and saved tensors are shared.
-// Requires d % 128 == 0 and (B*N) % 64 == 0 (the UMMA K block); otherwise MAC_ERR_UNSUPPORTED (use mac_read_bwd).
+// Requires d % 128 == 0 and (B*N) % 64 == 0 (the wgmma k-block of the weight-gradient products, K = B*N); otherwise MAC_ERR_UNSUPPORTED (use mac_read_bwd).
 // ------------------------------------------------------------------------------------------------------------------
 extern "C" int mac_tc_wgrad_splitk_(const void* xT, const void* gT, float* dW, float* partial, int in_dim, int out_dim, int K,
                                     mac_stream_t stream_);

@@ -96,8 +96,10 @@ def test_fused_read_step_equals_unfused_chain(monkeypatch):
     lib = L_.load()
     d = 512
     # 64-row tiles packed across sample boundaries: a partial last tile (3 x 49, 4 x 17, 11 x 131), tiles spanning many
-    # samples (N = 17, 49), samples spread over five tiles (N = 255) and a single-sample launch
-    for (B, N) in ((64, 196), (3, 49), (5, 130), (2, 256), (7, 128), (4, 17), (9, 200), (1, 129), (3, 255), (11, 131)):
+    # samples (N = 17, 49), samples spread over five tiles (N = 255) and a single-sample launch; one tile holding 64, 32 or
+    # a single one-row sample (N = 1, 2), tiles that are exactly one sample (N = 64) or half of one (N = 128, 256)
+    for (B, N) in ((64, 196), (3, 49), (5, 130), (2, 256), (7, 128), (4, 17), (9, 200), (1, 129), (3, 255), (11, 131),
+                   (1, 1), (64, 1), (3, 2), (2, 64), (4, 128), (1, 256)):
         g = torch.Generator(device="cuda").manual_seed(B * 1000 + N)
 
         def rn(*s, scale=1.0):

@@ -1,6 +1,6 @@
-"""Mixed-precision TRAINING forms of the cell (DESIGN.md section 9, item 1): every CUDA entry point they use is validated
-elsewhere in this suite (mac_linear_tc_fwd, mac_pack_weight_bf16, mac_cast_bf16, the fp32 element-wise kernels of the
-backward); these tests check their COMPOSITION (`mac_read_bwd_tc`, the bf16 training forward with widened saved
+"""Mixed-precision TRAINING forms of the cell (DESIGN.md section 9, item 1): the tensor-core kernels they use are checked
+against fp64 references of their own operation in tests/test_gpu_wgmma.py (the split-K weight gradient, the transposing
+bf16 casts, the bf16 read chain with its dropout masks and saved I1); these tests check their COMPOSITION (`mac_read_bwd_tc`, the bf16 training forward with widened saved
 activations).  Tolerances are mixed-precision ones (bf16 operands, fp32
 accumulation), stated per test."""
 import numpy as np
