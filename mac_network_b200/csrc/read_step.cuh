@@ -14,7 +14,9 @@
 // (wgmma m64n256k16, a 64 x 256 fp32 accumulator in 128 registers per thread).  Shared memory:
 //   A   [64 x 512] bf16 as 8 K-major 128-byte-swizzled [64 x 64] blocks (64 KB): the P tile (one TMA wave), scaled by y in
 //       place into P*y, then overwritten by H = GEMM 1's epilogue, the A operand of GEMM 2
-//   B   2 stages x [512 x 64] bf16 (128 KB): the k-blocks of Wm[0:d] and then of Wm2, streamed through one mbarrier ring
+//   B   2 stages x [512 x 64] bf16 (128 KB): one mbarrier ring carrying the k-blocks of Wm[0:d], then this CTA's Q rows
+//       (64 KB, in the A tile's layout), then the k-blocks of Wm2.  GEMM 1's epilogue reads Q from shared memory: loaded
+//       from global memory there, with the 128 accumulator registers live, too few loads fit in flight to hide latency
 // The logits are summed over both halves in shared memory and written as one partial per row.
 //
 // Whole-step form (mac_step_fused, N > 128 so that a tile touches at most two samples): the CTA first computes, for each
@@ -35,6 +37,7 @@ constexpr int RS_A_BYTES = RS_KB * RS_BLK;      // 64 KB
 constexpr int RS_B_HALF = 256 * TC_BK * 2;      // [256 x 64] bf16: 32 KB
 constexpr int RS_STAGE = 2 * RS_B_HALF;         // 64 KB
 constexpr int RS_STAGES = 2;
+constexpr int RS_Q_SLOT = RS_KB;                // ring slot of the Q tile, between the two GEMMs' k-blocks
 constexpr int RS_CONSUMERS = 256;
 constexpr int RS_THREADS = RS_CONSUMERS + 32;
 constexpr int RS_SMEM_BYTES = RS_A_BYTES + RS_STAGES * RS_STAGE + 1024 /*align*/ + 64 /*barriers*/ +
@@ -99,8 +102,9 @@ __device__ __forceinline__ float bf16_row_dot(const __nv_bfloat16* row, const fl
 __device__ __forceinline__ void rs_consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(RS_CONSUMERS) : "memory"); }
 
 __global__ void __launch_bounds__(RS_THREADS, 1)
-read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constant__ CUtensorMap map_w1,
-                 const __grid_constant__ CUtensorMap map_w2, const ReadStepParams p) {
+read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constant__ CUtensorMap map_q,
+                 const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_w2,
+                 const ReadStepParams p) {
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t base_u32 = smem_u32(smem_dyn);
   unsigned char* a_tile = smem_dyn + ((1024u - (base_u32 & 1023u)) & 1023u);
@@ -118,6 +122,7 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
 
   if (threadIdx.x == RS_CONSUMERS) {
     tma_prefetch_desc(&map_p);
+    tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_w1);
     tma_prefetch_desc(&map_w2);
     mbar_init(a_full, 1);
@@ -134,13 +139,18 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
     if (elect_one()) {
       mbar_expect_tx(a_full, RS_A_BYTES);
       for (int kb = 0; kb < RS_KB; ++kb) tma_load_2d(a_tile + kb * RS_BLK, &map_p, kb * TC_BK, row0, a_full);
-      for (int j = 0; j < 2 * RS_KB; ++j) {
+      // ring slots 0..7: Wm[0:d] k-blocks; slot 8: the Q tile (GEMM 1's addend); slots 9..16: Wm2 k-blocks
+      for (int j = 0; j < RS_Q_SLOT + 1 + RS_KB; ++j) {
         const int s = j % RS_STAGES;
         mbar_wait(&empty[s], ((j / RS_STAGES) & 1) ^ 1);
         mbar_expect_tx(&full[s], RS_STAGE);
-        const CUtensorMap* m = j < RS_KB ? &map_w1 : &map_w2;
-        const int k0 = (j % RS_KB) * TC_BK;
         unsigned char* dst = b_ring + s * RS_STAGE;
+        if (j == RS_Q_SLOT) {
+          for (int kb = 0; kb < RS_KB; ++kb) tma_load_2d(dst + kb * RS_BLK, &map_q, kb * TC_BK, row0, &full[s]);
+          continue;
+        }
+        const CUtensorMap* m = j < RS_Q_SLOT ? &map_w1 : &map_w2;
+        const int k0 = (j < RS_Q_SLOT ? j : j - RS_Q_SLOT - 1) * TC_BK;
         tma_load_2d(dst, m, k0, 0, &full[s]);
         tma_load_2d(dst + RS_B_HALF, m, k0, 256, &full[s]);
       }
@@ -194,16 +204,32 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
 
   // ---- P -> P*y in place (rows past M are TMA zero fill and stay zero)
   mbar_wait(a_full, 0);
-  for (int i = tid; i < RS_KB * RS_BM * 8; i += RS_CONSUMERS) {
-    const int kb = i >> 9, r = (i >> 3) & 63, pos = i & 7;
-    const int col = kb * TC_BK + ((pos ^ (r & 7)) << 3);
-    const int s = min(row0 + r, p.M - 1) / p.N;
-    const float* yy = p.Wy_t ? s_y + (s - s_lo) * RS_D + col : y_src + (size_t)s * RS_D + col;
-    uint4* ptr = reinterpret_cast<uint4*>(a_tile + kb * RS_BLK + r * 128 + pos * 16);
-    const uint4 v = *ptr;
-    const float4 y0 = *reinterpret_cast<const float4*>(yy), y1 = *reinterpret_cast<const float4*>(yy + 4);
-    *ptr = make_uint4(pack_bf16(bf16lo(v.x) * y0.x, bf16hi(v.x) * y0.y), pack_bf16(bf16lo(v.y) * y0.z, bf16hi(v.y) * y0.w),
-                      pack_bf16(bf16lo(v.z) * y1.x, bf16hi(v.z) * y1.y), pack_bf16(bf16lo(v.w) * y1.z, bf16hi(v.w) * y1.w));
+  // loads of a batch first, then its stores: y may be read through a generic pointer the stores could alias, so a
+  // load-store loop would wait out one L2 round trip per 16 bytes
+  constexpr int PY_BATCH = 8;
+  static_assert(RS_KB * RS_BM * 8 % (PY_BATCH * RS_CONSUMERS) == 0, "whole batches");
+  for (int i0 = tid; i0 < RS_KB * RS_BM * 8; i0 += PY_BATCH * RS_CONSUMERS) {
+    uint4 v[PY_BATCH];
+    float4 y0[PY_BATCH], y1[PY_BATCH];
+#pragma unroll
+    for (int u = 0; u < PY_BATCH; ++u) {
+      const int i = i0 + u * RS_CONSUMERS;
+      const int kb = i >> 9, r = (i >> 3) & 63, pos = i & 7;
+      const int col = kb * TC_BK + ((pos ^ (r & 7)) << 3);
+      const int s = min(row0 + r, p.M - 1) / p.N;
+      const float* yy = p.Wy_t ? s_y + (s - s_lo) * RS_D + col : y_src + (size_t)s * RS_D + col;
+      v[u] = *reinterpret_cast<const uint4*>(a_tile + kb * RS_BLK + r * 128 + pos * 16);
+      y0[u] = *reinterpret_cast<const float4*>(yy);
+      y1[u] = *reinterpret_cast<const float4*>(yy + 4);
+    }
+#pragma unroll
+    for (int u = 0; u < PY_BATCH; ++u) {
+      const int i = i0 + u * RS_CONSUMERS;
+      const int kb = i >> 9, r = (i >> 3) & 63, pos = i & 7;
+      *reinterpret_cast<uint4*>(a_tile + kb * RS_BLK + r * 128 + pos * 16) =
+          make_uint4(pack_bf16(bf16lo(v[u].x) * y0[u].x, bf16hi(v[u].x) * y0[u].y), pack_bf16(bf16lo(v[u].y) * y0[u].z, bf16hi(v[u].y) * y0[u].w),
+                     pack_bf16(bf16lo(v[u].z) * y1[u].x, bf16hi(v[u].z) * y1[u].y), pack_bf16(bf16lo(v[u].w) * y1[u].z, bf16hi(v[u].w) * y1[u].w));
+    }
   }
   fence_proxy_async();                                       // generic-proxy stores -> visible to wgmma
   rs_consumer_bar();
@@ -233,28 +259,33 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
   const int rl = 16 * (warp & 3) + (lane >> 2);
   const int cq = 256 * g + 2 * (lane & 3);
 
-  // ---- GEMM 1 and its epilogue: H = ELU(acc + Q) -> bf16 into the A tile (K-major, swizzled) once both halves are done
+  // ---- GEMM 1 and its epilogue: H = ELU(acc + Q) -> bf16 into the A tile (K-major, swizzled) once both halves are done.
+  //      Q comes through the ring in the A tile's layout, so it is read at the same conflict-free offsets H is written to.
   gemm(0);
+  constexpr int qs = RS_Q_SLOT % RS_STAGES;
+  const unsigned char* q_tile = b_ring + qs * RS_STAGE;
+  mbar_wait(&full[qs], (RS_Q_SLOT / RS_STAGES) & 1);
   rs_consumer_bar();                                         // the other warpgroup has finished reading P*y
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = rl + 8 * h, row = row0 + r;
-    const __nv_bfloat16* qrow = p.Q + (size_t)min(row, p.M - 1) * RS_D;
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
       const int n = cq + 8 * j;
-      const uint32_t q = __ldg(reinterpret_cast<const unsigned int*>(qrow + n));
+      const int kb = n >> 6, c = (n & 63) >> 3;
+      const int off = kb * RS_BLK + r * 128 + ((c ^ (r & 7)) << 4) + (n & 7) * 2;
+      const uint32_t q = *reinterpret_cast<const uint32_t*>(q_tile + off);
       const uint32_t hv = row < p.M ? pack_bf16(elu_fast(acc[4 * j + 2 * h] + bf16lo(q)), elu_fast(acc[4 * j + 2 * h + 1] + bf16hi(q)))
                                     : 0u;
-      const int kb = n >> 6, c = (n & 63) >> 3;
-      *reinterpret_cast<uint32_t*>(a_tile + kb * RS_BLK + r * 128 + ((c ^ (r & 7)) << 4) + (n & 7) * 2) = hv;
+      *reinterpret_cast<uint32_t*>(a_tile + off) = hv;
     }
   }
   fence_proxy_async();
   rs_consumer_bar();
+  if (lane == 0) mbar_arrive(&empty[qs]);                    // Q read and used by every thread of this warp
 
   // ---- GEMM 2 and its epilogue: I2 = ELU((acc + bm2) * control_b); logit half = sum_n I2 * wr
-  gemm(RS_KB);
+  gemm(RS_Q_SLOT + 1);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = rl + 8 * h, row = row0 + r;
@@ -293,8 +324,10 @@ inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y
   }
   const int M = B * N;
   const TcReadScratch s = tc_read_scratch(const_cast<void*>(inv), B, N, d);
-  CUtensorMap mp, mw1, mw2;
+  CUtensorMap mp, mq, mw1, mw2;
   int st = make_tmap_2d(&mp, s.P, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS_BM, TC_BK, 1);
+  if (st != MAC_OK) return st;
+  st = make_tmap_2d(&mq, s.Q, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS_BM, TC_BK, 1);
   if (st != MAC_OK) return st;
   st = make_tmap_2d(&mw1, w->Wm_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)2 * d * 2, 256, TC_BK, 1);   // Wm[0:d] of [d, 2d]
   if (st != MAC_OK) return st;
@@ -309,7 +342,7 @@ inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y
   }
   // the opt-in is per device context: set it on every launch
   MAC_CUDA_TRY(cudaFuncSetAttribute(read_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM_BYTES));
-  read_step_kernel<<<(M + RS_BM - 1) / RS_BM, RS_THREADS, RS_SMEM_BYTES, stream>>>(mp, mw1, mw2, p);
+  read_step_kernel<<<(M + RS_BM - 1) / RS_BM, RS_THREADS, RS_SMEM_BYTES, stream>>>(mp, mq, mw1, mw2, p);
   MAC_LAUNCH_CHECK();
   return mac_kb_attend_fwd(s.parts, 1, w->br, kb_bf16, 1, att, info, B, N, d, stream);
 }
