@@ -389,7 +389,8 @@ int mac_col2im3x3(const float* dcols, float* dx, float keep, uint64_t seed, int 
  *   (mac_linear_fwd) and Wh_dir = kernel + E*4h (the recurrent rows).  Direction 1 walks t = len-1 .. 0 (reverse_sequence).
  *   out_seq [B,S,ndir*h] = [fw | bw] outputs, zero for t >= len; vecq [B,ndir*h] (may be NULL) = the final h of each
  *   direction (ops.py:893-898).  save_gates [ndir,B*S,4h], save_c / save_hprev [ndir,B*S,h] (all or none NULL) keep what
- *   the backward needs, indexed by time.  Issues S launches (one per step, both directions) on `stream`.
+ *   the backward needs, indexed by time; save_hprev is zero for t >= len.  Issues S launches (one per step, both directions)
+ *   on `stream`.
  * mac_lstm_bwd: BPTT.  dG_dir [B*S, 4h] receives the gradient w.r.t. the pre-activation gates; parameter and input
  *   gradients are then GEMMs over all steps: mac_linear_bwd(x_segs = [dropout(X), save_hprev_dir], dy = dG_dir).
  * --------------------------------------------------------------------------------------------- */

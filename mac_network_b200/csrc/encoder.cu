@@ -421,6 +421,9 @@ extern "C" int mac_lstm_fwd(const float* gx_fw, const float* gx_bw, const float*
   const size_t sb = (lstm_state_bytes(B, h, ndir) + 255) & ~(size_t)255;
   char* ws = reinterpret_cast<char*>(workspace);
   MAC_CUDA_TRY(cudaMemsetAsync(out_seq, 0, (size_t)B * S * ndir * h * sizeof(float), stream));
+  // the backward's weight-gradient GEMM multiplies every row of save_hprev, those of t >= len by zero gate gradients: they
+  // must be finite, and whatever the caller's buffer held (NaN included) would otherwise reach the gradient
+  if (save_hprev) MAC_CUDA_TRY(cudaMemsetAsync(save_hprev, 0, (size_t)ndir * B * S * h * sizeof(float), stream));
   LstmFwdParams p{};
   p.gx[0] = gx_fw; p.gx[1] = gx_bw; p.Wh[0] = Wh_fw; p.Wh[1] = Wh_bw;
   p.lengths = lengths; p.forget_bias = forget_bias; p.out_seq = out_seq; p.vecq = vecq;

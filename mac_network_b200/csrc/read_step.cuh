@@ -5,19 +5,24 @@
 //   logit  = I2 . wr + br                               (mac_cell.py:266, ops.py:316-317)
 //   att    = softmax_n(logit);  info = sum_n att * KB   (ops.py:143, 149-150; original KB, mac_cell.py:271-275)
 //
-// read_step_kernel computes the logits of 64 knowledge-base rows per CTA (rows packed across sample boundaries, so
-// ceil(B*N / 64) CTAs) with P*y, H and I2 never leaving the SM; kb_attend (attend.cu) then does the per-sample softmax and
+// read_step_kernel computes the logits of 64-row tiles of the knowledge base (rows packed across sample boundaries, so
+// ceil(B*N / 64) tiles) with P*y, H and I2 never leaving the SM; kb_attend (attend.cu) then does the per-sample softmax and
 // weighted sum.  Two launches per step instead of the four of scale_rows_bf16 + tc_gemm<ADDACT> + tc_gemm<LOGITS> + kb_attend,
 // and none of the P*y / H round trips through L2 and HBM (4 x B*N*d bf16).
 //
 // CTA = 288 threads: warp 8 is the TMA producer; warpgroups 0 and 1 each own one 256-column half of the d = 512 outputs
 // (wgmma m64n256k16, a 64 x 256 fp32 accumulator in 128 registers per thread).  Shared memory:
-//   A   [64 x 512] bf16 as 8 K-major 128-byte-swizzled [64 x 64] blocks (64 KB): the P tile (one TMA wave), scaled by y in
-//       place into P*y, then overwritten by H = GEMM 1's epilogue, the A operand of GEMM 2
-//   B   2 stages x [512 x 64] bf16 (128 KB): one mbarrier ring carrying the k-blocks of Wm[0:d], then this CTA's Q rows
-//       (64 KB, in the A tile's layout), then the k-blocks of Wm2.  GEMM 1's epilogue reads Q from shared memory: loaded
-//       from global memory there, with the 128 accumulator registers live, too few loads fit in flight to hide latency
-// The logits are summed over both halves in shared memory and written as one partial per row.
+//   A   [64 x 512] bf16 as 8 K-major 128-byte-swizzled [64 x 64] blocks (64 KB): H = GEMM 1's epilogue, the A operand of
+//       GEMM 2
+//   B   2 stages x 72 KB: one mbarrier ring of 17 slots per tile.  Slots 0..7 each carry k-block j of Wm[0:d] ([512 x 64],
+//       64 KB) and k-block j of the P tile ([64 x 64], 8 KB, the A layout), so GEMM 1 starts when its first 72 KB have
+//       landed; slot 8 carries the tile's Q rows (64 KB, the A layout), GEMM 1's addend; slots 9..16 the k-blocks of Wm2.
+//       GEMM 1's epilogue reads Q from shared memory: loaded from global memory there, with the 128 accumulator registers
+//       live, too few loads fit in flight to hide latency
+// GEMM 1 scales P block j by y in place (P*y, rounded to bf16) while the MMAs of block j - 1 run, then issues block j.
+// Epilogue 2 reads bm2, wr and the control rows of the tile's first two samples from shared memory (rows of later samples,
+// only present when N < 64, from global memory).  The logits are summed over both halves in shared memory and written as one
+// partial per row.
 //
 // Whole-step form (mac_step_fused, N > 128 so that a tile touches at most two samples): the CTA first computes, for each
 // sample it touches, the previous step's plain write unit m = [m_prev, info_prev] @ Ww + bw (mac_cell.py:339-352) and this
@@ -30,18 +35,23 @@
 namespace mac {
 
 constexpr int RS_D = 512;                       // d of the shipped configurations
-constexpr int RS_BM = 64;                       // knowledge-base rows per CTA
+constexpr int RS_BM = 64;                       // knowledge-base rows per CTA (one tile)
 constexpr int RS_KB = RS_D / TC_BK;             // 8 k-blocks
 constexpr int RS_BLK = RS_BM * TC_BK * 2;       // one [64 x 64] bf16 A block: 8 KB
 constexpr int RS_A_BYTES = RS_KB * RS_BLK;      // 64 KB
 constexpr int RS_B_HALF = 256 * TC_BK * 2;      // [256 x 64] bf16: 32 KB
-constexpr int RS_STAGE = 2 * RS_B_HALF;         // 64 KB
+constexpr int RS_W_BYTES = 2 * RS_B_HALF;       // one weight k-block: 64 KB
+constexpr int RS_STAGE = RS_W_BYTES + RS_BLK;   // 72 KB: a weight k-block and, in GEMM 1's slots, a P block
 constexpr int RS_STAGES = 2;
 constexpr int RS_Q_SLOT = RS_KB;                // ring slot of the Q tile, between the two GEMMs' k-blocks
+constexpr int RS_SLOTS = RS_Q_SLOT + 1 + RS_KB; // ring slots per tile
 constexpr int RS_CONSUMERS = 256;
 constexpr int RS_THREADS = RS_CONSUMERS + 32;
 constexpr int RS_SMEM_BYTES = RS_A_BYTES + RS_STAGES * RS_STAGE + 1024 /*align*/ + 64 /*barriers*/ +
-                              2 * RS_BM * 4 /*logit halves*/ + 2 * RS_D * 4 /*y of <= 2 samples*/ + 2 * RS_D * 4 /*m*/;
+                              2 * RS_BM * 4 /*logit halves*/ + 2 * RS_D * 4 /*y of <= 2 samples*/ + 2 * RS_D * 4 /*m*/ +
+                              2 * RS_D * 4 /*control of <= 2 samples*/ + 2 * RS_D * 4 /*bm2, wr*/;
+static_assert(RS_SMEM_BYTES <= 232448, "over the sm_90 per-block shared memory opt-in limit");
+static_assert(RS_STAGE % 1024 == 0 && RS_W_BYTES % 1024 == 0, "swizzled operands need 1024-byte alignment");
 
 __device__ __forceinline__ float bf16lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf16hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
@@ -109,12 +119,14 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
   const uint32_t base_u32 = smem_u32(smem_dyn);
   unsigned char* a_tile = smem_dyn + ((1024u - (base_u32 & 1023u)) & 1023u);
   unsigned char* b_ring = a_tile + RS_A_BYTES;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(b_ring + RS_STAGES * RS_STAGE);
-  uint64_t* full = a_full + 1;                     // [STAGES] TMA -> consumers
+  uint64_t* full = reinterpret_cast<uint64_t*>(b_ring + RS_STAGES * RS_STAGE);   // [STAGES] TMA -> consumers
   uint64_t* empty = full + RS_STAGES;              // [STAGES] consumers -> TMA (8 warp arrivals)
-  float* s_lg = reinterpret_cast<float*>(a_full + 8);       // [2][64] logit halves
+  float* s_lg = reinterpret_cast<float*>(full + 8);          // [2][64] logit halves
   float* s_y = s_lg + 2 * RS_BM;                             // [2][d] y of the samples of the whole-step form
   float* s_m = s_y + 2 * RS_D;                               // [2][d] m
+  float* s_ctrl = s_m + 2 * RS_D;                            // [2][d] control of the tile's first two samples
+  float* s_bm2 = s_ctrl + 2 * RS_D;                          // [d]
+  float* s_wr = s_bm2 + RS_D;                                // [d]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row0 = blockIdx.x * RS_BM;
@@ -125,7 +137,6 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_w1);
     tma_prefetch_desc(&map_w2);
-    mbar_init(a_full, 1);
     for (int i = 0; i < RS_STAGES; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], RS_CONSUMERS / 32);
@@ -137,20 +148,21 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
   if (warp == RS_CONSUMERS / 32) {
     // ===================================================== TMA producer
     if (elect_one()) {
-      mbar_expect_tx(a_full, RS_A_BYTES);
-      for (int kb = 0; kb < RS_KB; ++kb) tma_load_2d(a_tile + kb * RS_BLK, &map_p, kb * TC_BK, row0, a_full);
-      // ring slots 0..7: Wm[0:d] k-blocks; slot 8: the Q tile (GEMM 1's addend); slots 9..16: Wm2 k-blocks
-      for (int j = 0; j < RS_Q_SLOT + 1 + RS_KB; ++j) {
+      // ring slots 0..7: Wm[0:d] k-block j + P k-block j; slot 8: the Q tile (GEMM 1's addend); slots 9..16: Wm2 k-blocks
+      for (int j = 0; j < RS_SLOTS; ++j) {
         const int s = j % RS_STAGES;
         mbar_wait(&empty[s], ((j / RS_STAGES) & 1) ^ 1);
-        mbar_expect_tx(&full[s], RS_STAGE);
         unsigned char* dst = b_ring + s * RS_STAGE;
         if (j == RS_Q_SLOT) {
+          mbar_expect_tx(&full[s], RS_A_BYTES);
           for (int kb = 0; kb < RS_KB; ++kb) tma_load_2d(dst + kb * RS_BLK, &map_q, kb * TC_BK, row0, &full[s]);
           continue;
         }
-        const CUtensorMap* m = j < RS_Q_SLOT ? &map_w1 : &map_w2;
-        const int k0 = (j < RS_Q_SLOT ? j : j - RS_Q_SLOT - 1) * TC_BK;
+        const bool g1 = j < RS_Q_SLOT;
+        mbar_expect_tx(&full[s], g1 ? RS_W_BYTES + RS_BLK : RS_W_BYTES);
+        const CUtensorMap* m = g1 ? &map_w1 : &map_w2;
+        const int k0 = (g1 ? j : j - RS_Q_SLOT - 1) * TC_BK;
+        if (g1) tma_load_2d(dst + RS_W_BYTES, &map_p, k0, row0, &full[s]);
         tma_load_2d(dst, m, k0, 0, &full[s]);
         tma_load_2d(dst + RS_B_HALF, m, k0, 256, &full[s]);
       }
@@ -160,10 +172,25 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
 
   // ===================================================== consumers
   const int tid = threadIdx.x;
+  const int g = warp >> 2;                                   // warpgroup: output columns [256 g, 256 g + 256)
+  // acc[4 j + 2 h + e] is tile row 16 (warp & 3) + lane / 4 + 8 h, column 256 g + 8 j + 2 (lane & 3) + e
+  const int rl = 16 * (warp & 3) + (lane >> 2);
+  const int cq = 256 * g + 2 * (lane & 3);
+  // this thread's two 16-byte chunks of each P block: rows tid / 8 and tid / 8 + 32, chunk tid % 8 of the swizzled
+  // 128-byte row, i.e. columns pcol .. pcol + 7 of the k-block (the swizzle only depends on row % 8)
+  const int prow = tid >> 3;
+  const int poff = prow * 128 + (tid & 7) * 16;
+  const int pcol = ((tid & 7) ^ (prow & 7)) << 3;
+  for (int i = tid; i < RS_D; i += RS_CONSUMERS) {
+    s_bm2[i] = __ldg(p.bm2 + i);
+    s_wr[i] = __ldg(p.wr + i);
+  }
+  float acc[128];
   const int last_row = min(p.M, row0 + RS_BM) - 1;
-  const float* y_src = p.y;
+  const int nsamp = last_row / p.N - s_lo + 1;
+  for (int q = 0; q < min(nsamp, 2); ++q)
+    for (int i = tid; i < RS_D; i += RS_CONSUMERS) s_ctrl[q * RS_D + i] = __ldg(p.ctrl + (size_t)(s_lo + q) * RS_D + i);
   if (p.Wy_t) {
-    const int nsamp = last_row / p.N - s_lo + 1;
     for (int q = 0; q < nsamp; ++q) {
       const int s = s_lo + q;
       float* m = s_m + q * RS_D;
@@ -201,71 +228,54 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
       }
     rs_consumer_bar();
   }
-
-  // ---- P -> P*y in place (rows past M are TMA zero fill and stay zero)
-  mbar_wait(a_full, 0);
-  // loads of a batch first, then its stores: y may be read through a generic pointer the stores could alias, so a
-  // load-store loop would wait out one L2 round trip per 16 bytes
-  constexpr int PY_BATCH = 8;
-  static_assert(RS_KB * RS_BM * 8 % (PY_BATCH * RS_CONSUMERS) == 0, "whole batches");
-  for (int i0 = tid; i0 < RS_KB * RS_BM * 8; i0 += PY_BATCH * RS_CONSUMERS) {
-    uint4 v[PY_BATCH];
-    float4 y0[PY_BATCH], y1[PY_BATCH];
+  // y rows of this thread's two P rows (rows past M are TMA zero fill and stay zero)
+  const float* yrow[2];
 #pragma unroll
-    for (int u = 0; u < PY_BATCH; ++u) {
-      const int i = i0 + u * RS_CONSUMERS;
-      const int kb = i >> 9, r = (i >> 3) & 63, pos = i & 7;
-      const int col = kb * TC_BK + ((pos ^ (r & 7)) << 3);
-      const int s = min(row0 + r, p.M - 1) / p.N;
-      const float* yy = p.Wy_t ? s_y + (s - s_lo) * RS_D + col : y_src + (size_t)s * RS_D + col;
-      v[u] = *reinterpret_cast<const uint4*>(a_tile + kb * RS_BLK + r * 128 + pos * 16);
-      y0[u] = *reinterpret_cast<const float4*>(yy);
-      y1[u] = *reinterpret_cast<const float4*>(yy + 4);
-    }
-#pragma unroll
-    for (int u = 0; u < PY_BATCH; ++u) {
-      const int i = i0 + u * RS_CONSUMERS;
-      const int kb = i >> 9, r = (i >> 3) & 63, pos = i & 7;
-      *reinterpret_cast<uint4*>(a_tile + kb * RS_BLK + r * 128 + pos * 16) =
-          make_uint4(pack_bf16(bf16lo(v[u].x) * y0[u].x, bf16hi(v[u].x) * y0[u].y), pack_bf16(bf16lo(v[u].y) * y0[u].z, bf16hi(v[u].y) * y0[u].w),
-                     pack_bf16(bf16lo(v[u].z) * y1[u].x, bf16hi(v[u].z) * y1[u].y), pack_bf16(bf16lo(v[u].w) * y1[u].z, bf16hi(v[u].w) * y1[u].w));
-    }
+  for (int u = 0; u < 2; ++u) {
+    const int s = min(row0 + prow + 32 * u, p.M - 1) / p.N;
+    yrow[u] = (p.Wy_t ? s_y + (s - s_lo) * RS_D : p.y + (size_t)s * RS_D) + pcol;
   }
-  fence_proxy_async();                                       // generic-proxy stores -> visible to wgmma
-  rs_consumer_bar();
 
-  const int g = warp >> 2;                                   // warpgroup: output columns [256 g, 256 g + 256)
-  float acc[128];
-  const uint32_t a_u = smem_u32(a_tile);
-  auto gemm = [&](int j0) {
-    for (int j = j0; j < j0 + RS_KB; ++j) {
-      const int s = j % RS_STAGES;
-      mbar_wait(&full[s], (j / RS_STAGES) & 1);
-      const uint64_t adesc = make_sw128_kmajor_desc(a_u + (j - j0) * RS_BLK);
-      const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(b_ring + s * RS_STAGE + g * RS_B_HALF));
-      wgmma_fence();
+  // ---- GEMM 1: P block j is scaled by y in place (P*y) while the MMAs of block j - 1 run, then block j is issued
+  for (int j = 0; j < RS_KB; ++j) {
+    const int s = j % RS_STAGES;
+    unsigned char* stage = b_ring + s * RS_STAGE;
+    float4 y0[2], y1[2];
 #pragma unroll
-      for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n256(acc, adesc + 2 * k, bdesc + 2 * k, (j > j0 || k) ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<1>();
-      wgmma_hold(acc);
-      if (j > j0 && lane == 0) mbar_arrive(&empty[(j - 1) % RS_STAGES]);
+    for (int u = 0; u < 2; ++u) {
+      y0[u] = *reinterpret_cast<const float4*>(yrow[u] + j * TC_BK);
+      y1[u] = *reinterpret_cast<const float4*>(yrow[u] + j * TC_BK + 4);
     }
-    wgmma_wait<0>();
+    mbar_wait(&full[s], (j / RS_STAGES) & 1);
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      uint4* c = reinterpret_cast<uint4*>(stage + RS_W_BYTES + poff + u * 32 * 128);
+      const uint4 v = *c;
+      *c = make_uint4(pack_bf16(bf16lo(v.x) * y0[u].x, bf16hi(v.x) * y0[u].y), pack_bf16(bf16lo(v.y) * y0[u].z, bf16hi(v.y) * y0[u].w),
+                      pack_bf16(bf16lo(v.z) * y1[u].x, bf16hi(v.z) * y1[u].y), pack_bf16(bf16lo(v.w) * y1[u].z, bf16hi(v.w) * y1[u].w));
+    }
+    fence_proxy_async();                                   // generic-proxy stores -> visible to wgmma
+    rs_consumer_bar();
+    const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(stage + RS_W_BYTES));
+    const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(stage + g * RS_B_HALF));
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n256(acc, adesc + 2 * k, bdesc + 2 * k, (j || k) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
     wgmma_hold(acc);
-    if (lane == 0) mbar_arrive(&empty[(j0 + RS_KB - 1) % RS_STAGES]);
-  };
-  // acc[4 j + 2 h + e] is tile row 16 (warp & 3) + lane / 4 + 8 h, column 256 g + 8 j + 2 (lane & 3) + e
-  const int rl = 16 * (warp & 3) + (lane >> 2);
-  const int cq = 256 * g + 2 * (lane & 3);
+    if (j && lane == 0) mbar_arrive(&empty[(j - 1) % RS_STAGES]);
+  }
+  wgmma_wait<0>();
+  wgmma_hold(acc);
+  if (lane == 0) mbar_arrive(&empty[(RS_KB - 1) % RS_STAGES]);
 
-  // ---- GEMM 1 and its epilogue: H = ELU(acc + Q) -> bf16 into the A tile (K-major, swizzled) once both halves are done.
-  //      Q comes through the ring in the A tile's layout, so it is read at the same conflict-free offsets H is written to.
-  gemm(0);
+  // ---- GEMM 1's epilogue: H = ELU(acc + Q) -> bf16 into the A tile (K-major, swizzled).  Q comes through the ring in
+  //      the A tile's layout, so it is read at the same conflict-free offsets H is written to.  GEMM 1 takes its A operand
+  //      from the ring, so nothing else uses the A tile before this.
   constexpr int qs = RS_Q_SLOT % RS_STAGES;
   const unsigned char* q_tile = b_ring + qs * RS_STAGE;
   mbar_wait(&full[qs], (RS_Q_SLOT / RS_STAGES) & 1);
-  rs_consumer_bar();                                         // the other warpgroup has finished reading P*y
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = rl + 8 * h, row = row0 + r;
@@ -282,23 +292,44 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
   }
   fence_proxy_async();
   rs_consumer_bar();
-  if (lane == 0) mbar_arrive(&empty[qs]);                    // Q read and used by every thread of this warp
+  if (lane == 0) mbar_arrive(&empty[qs]);                  // Q read and used by every thread of this warp
 
-  // ---- GEMM 2 and its epilogue: I2 = ELU((acc + bm2) * control_b); logit half = sum_n I2 * wr
-  gemm(RS_Q_SLOT + 1);
+  // ---- GEMM 2
+  const uint32_t a_u = smem_u32(a_tile);
+  for (int j = 0; j < RS_KB; ++j) {
+    const int jj = RS_Q_SLOT + 1 + j, s = jj % RS_STAGES;
+    mbar_wait(&full[s], (jj / RS_STAGES) & 1);
+    const uint64_t adesc = make_sw128_kmajor_desc(a_u + j * RS_BLK);
+    const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(b_ring + s * RS_STAGE + g * RS_B_HALF));
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n256(acc, adesc + 2 * k, bdesc + 2 * k, (j || k) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    wgmma_hold(acc);
+    if (j && lane == 0) mbar_arrive(&empty[(jj - 1) % RS_STAGES]);
+  }
+  wgmma_wait<0>();
+  wgmma_hold(acc);
+  if (lane == 0) mbar_arrive(&empty[(RS_SLOTS - 1) % RS_STAGES]);
+
+  // ---- GEMM 2's epilogue: I2 = ELU((acc + bm2) * control_b); logit half = sum_n I2 * wr
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = rl + 8 * h, row = row0 + r;
-    const float* crow = p.ctrl + (size_t)(min(row, p.M - 1) / p.N) * RS_D;
+    const int s = min(row, p.M - 1) / p.N;
+    const float* crow = s - s_lo < 2 ? s_ctrl + (s - s_lo) * RS_D : p.ctrl + (size_t)s * RS_D;
     float part = 0.f;
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
       const int n = cq + 8 * j;
-      const float2 cc = __ldg(reinterpret_cast<const float2*>(crow + n));
-      const float t0 = elu_fast((acc[4 * j + 2 * h] + __ldg(p.bm2 + n)) * cc.x);
-      const float t1 = elu_fast((acc[4 * j + 2 * h + 1] + __ldg(p.bm2 + n + 1)) * cc.y);
-      part = fmaf(t0, __ldg(p.wr + n), part);
-      part = fmaf(t1, __ldg(p.wr + n + 1), part);
+      const float2 cc = *reinterpret_cast<const float2*>(crow + n);
+      const float2 bb = *reinterpret_cast<const float2*>(s_bm2 + n);
+      const float2 ww = *reinterpret_cast<const float2*>(s_wr + n);
+      const float t0 = elu_fast((acc[4 * j + 2 * h] + bb.x) * cc.x);
+      const float t1 = elu_fast((acc[4 * j + 2 * h + 1] + bb.y) * cc.y);
+      part = fmaf(t0, ww.x, part);
+      part = fmaf(t1, ww.y, part);
     }
     part += __shfl_xor_sync(0xffffffffu, part, 1);
     part += __shfl_xor_sync(0xffffffffu, part, 2);
