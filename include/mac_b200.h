@@ -149,28 +149,14 @@ int mac_read_fwd_inv(const float* kb, const void* kb_bf16, const void* inv, cons
  * y = memory @ Wy + by [B, d] (ops.py:689) and the control state [B, d], computes
  *   H = ELU((P*y) @ Wm[0:d] + Q);  logits = ELU((H @ Wm2 + bm2) * control) . wr + br;  att = softmax_n(logits);
  *   info = sum_n att * KB                                     (mac_cell.py:230-275 at readDropout == 1)
- * as four launches (row scaling, two wgmma GEMMs with the element-wise work in their epilogues, softmax + weighted sum).
- * P*y, H and the logit partial sums go to the scratch that mac_read_invariant_bytes reserves behind [P | Q] in `inv` (so
- * `inv` is read AND written by this call: one call at a time per `inv`).  mac_read_fwd_inv dispatches to it when
- * mac_read_step_fused_supported(B, N, d) (d == 512, N <= 256) unless the environment sets MAC_READ_FUSED=0.
- * Returns MAC_ERR_UNSUPPORTED for other shapes. */
+ * as one wgmma kernel over 64-row tiles of the knowledge base (P*y, H and I2 stay on the SM; one logit per row) and the
+ * kb_attend launch (softmax + weighted sum).  The logits go to the scratch that mac_read_invariant_bytes reserves behind
+ * [P | Q] in `inv`, one float per row (so `inv` is read AND written by this call: one call at a time per `inv`).
+ * mac_read_fwd_inv dispatches to it when mac_read_step_fused_supported(B, N, d) (d == 512, N <= 256, B < 2^22) unless
+ * the environment sets MAC_READ_FUSED=0.  Returns MAC_ERR_UNSUPPORTED for other shapes. */
 int mac_read_step_fused(const void* inv, const void* kb_bf16, const float* y, const float* control,
                         const mac_read_weights* w, float* info, float* att, int B, int N, int d, mac_stream_t stream);
 int mac_read_step_fused_supported(int B, int N, int d);
-
-/* One whole inference reasoning step (plain write unit: writeInputs=BOTH, writeMemProj, no self-attention,
- * no gate; control chain hoisted; dropouts = 1).  mac_read_step_fused after a per-sample prologue kernel:
- *   memory = info_prev ? [mem_prev, info_prev] @ Ww + bw : mem_prev      (write unit of the PREVIOUS step, mac_cell.py:339-352)
- *   y      = memory @ Wy + by                                            (ops.py:689)
- *   info, att = read step (as mac_read_step_fused) with this y and `control`
- * `memory` is written to mem_out when info_prev != NULL.  The two products are per-sample matrix-vector products against bf16
- * [out, in] copies of the weights (mac_pack_weight_bf16; fp32 activations and accumulation), computed while the kernel's
- * first TMA requests wait for their tensor-map descriptors.  The caller runs mac_write_fwd once after the last step for the
- * final memory.  mac_step_fused_supported: d == 512 and 128 < N <= 256. */
-int mac_step_fused(const void* inv, const void* kb_bf16, const float* mem_prev, const float* info_prev, const float* control,
-                   const mac_read_weights* w, const void* Ww_t_bf16, const float* bw, const void* Wy_t_bf16, float* mem_out,
-                   float* info, float* att, int B, int N, int d, mac_stream_t stream);
-int mac_step_fused_supported(int B, int N, int d);
 
 /* The HBM-bound tail of the read unit on its own (ops.py:143, 149-150):
  *   att[b,:] = softmax_n( sum_p logit_parts[(b*N+n)*nparts + p] + br );  info[b,:] = sum_n att[b,n] * KB[b,n,:]

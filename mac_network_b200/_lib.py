@@ -52,9 +52,6 @@ PROTOTYPES = {
     "mac_read_step_fused": (c_int, [c_fp, c_fp, c_fp, c_fp, ctypes.POINTER(ReadWeights), c_fp, c_fp, c_int, c_int, c_int,
                                     c_fp]),
     "mac_read_step_fused_supported": (c_int, [c_int, c_int, c_int]),
-    "mac_step_fused": (c_int, [c_fp, c_fp, c_fp, c_fp, c_fp, ctypes.POINTER(ReadWeights), c_fp, c_fp, c_fp, c_fp, c_fp, c_fp,
-                               c_int, c_int, c_int, c_fp]),
-    "mac_step_fused_supported": (c_int, [c_int, c_int, c_int]),
     "mac_write_fwd_next_y": (c_int, [c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_sz, c_int, c_int, c_fp]),
     "mac_kb_attend_fwd": (c_int, [c_fp, c_int, c_f, c_fp, c_int, c_fp, c_fp, c_int, c_int, c_int, c_fp]),
     "mac_write_fwd": (c_int, [c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_f, c_fp, c_fp, c_fp, c_sz, c_int,

@@ -23,12 +23,6 @@
 // Epilogue 2 reads bm2, wr and the control rows of the tile's first two samples from shared memory (rows of later samples,
 // only present when N < 64, from global memory).  The logits are summed over both halves in shared memory and written as one
 // partial per row.
-//
-// Whole-step form (mac_step_fused, N > 128 so that a tile touches at most two samples): the CTA first computes, for each
-// sample it touches, the previous step's plain write unit m = [m_prev, info_prev] @ Ww + bw (mac_cell.py:339-352) and this
-// step's memory projection y = m @ Wy + by (ops.py:689) as matrix-vector products against the bf16 weights (fp32
-// activations and accumulation) while the TMA loads are in flight; the CTA that owns a sample's first row writes its m.
-// That removes the separate write / projY launch, at the price of every CTA re-reading those weights (opt-in form).
 #pragma once
 #include "tc_gemm.cuh"
 
@@ -48,8 +42,8 @@ constexpr int RS_SLOTS = RS_Q_SLOT + 1 + RS_KB; // ring slots per tile
 constexpr int RS_CONSUMERS = 256;
 constexpr int RS_THREADS = RS_CONSUMERS + 32;
 constexpr int RS_SMEM_BYTES = RS_A_BYTES + RS_STAGES * RS_STAGE + 1024 /*align*/ + 64 /*barriers*/ +
-                              2 * RS_BM * 4 /*logit halves*/ + 2 * RS_D * 4 /*y of <= 2 samples*/ + 2 * RS_D * 4 /*m*/ +
-                              2 * RS_D * 4 /*control of <= 2 samples*/ + 2 * RS_D * 4 /*bm2, wr*/;
+                              2 * RS_BM * 4 /*logit halves*/ + 2 * RS_D * 4 /*control of <= 2 samples*/ +
+                              2 * RS_D * 4 /*bm2, wr*/;
 static_assert(RS_SMEM_BYTES <= 232448, "over the sm_90 per-block shared memory opt-in limit");
 static_assert(RS_STAGE % 1024 == 0 && RS_W_BYTES % 1024 == 0, "swizzled operands need 1024-byte alignment");
 
@@ -65,49 +59,19 @@ __device__ __forceinline__ void wgmma_bf16_n256(float (&d)[128], uint64_t adesc,
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "l"(adesc), "l"(bdesc), "r"(accum));
 }
-// can the read step take this shape?
-inline bool read_step_supported(int B, int N, int d) { return d == RS_D && N >= 1 && N <= 256 && B >= 1; }
-
-// whole-step form: the write unit of the previous step and this step's memory projection run in the kernel's prologue
-struct WholeStepArgs {
-  const float* mem_prev;
-  const float* info_prev;           // NULL on the first step (the memory is then mem_prev itself)
-  const void* Ww_t_bf16;            // [d, 2d] bf16 (mac_pack_weight_bf16 of write/newMemory)
-  const float* bw;
-  const void* Wy_t_bf16;            // [d, d] bf16 (mac_pack_weight_bf16 of projY)
-  float* mem_out;
-};
-inline bool whole_step_supported(int B, int N, int d) { return read_step_supported(B, N, d) && N > 128; }
+// can the read step take this shape?  (B < 2^22: the kernel indexes y [B, d] with 32-bit offsets)
+inline bool read_step_supported(int B, int N, int d) {
+  return d == RS_D && N >= 1 && N <= 256 && B >= 1 && B < (1 << 22);
+}
 
 struct ReadStepParams {
   int M, N;
-  const float* y;                   // [B, d] memory projection, or NULL in the whole-step form
+  const float* y;                   // [B, d] memory projection
   const float* ctrl;                // [B, d]
   const float* bm2;                 // [d]
   const float* wr;                  // [d]
-  const __nv_bfloat16* Q;           // [B*N, d]  P @ Wm[d:2d] + bm
   float* logits;                    // [B*N]  I2 . wr (without br)
-  const float* mem_prev;            // whole-step form (see WholeStepArgs); Wy_t == NULL otherwise
-  const float* info_prev;
-  const __nv_bfloat16* Ww_t;
-  const float* bw;
-  const __nv_bfloat16* Wy_t;
-  const float* by;
-  float* mem_out;
 };
-
-// sum_k x[k] * W_t[n, k] over K (K % 256 == 0), one warp per output column
-__device__ __forceinline__ float bf16_row_dot(const __nv_bfloat16* row, const float* x, int K, int lane) {
-  float a = 0.f;
-  for (int k = lane * 8; k < K; k += 256) {
-    const uint4 w = ldg_nc_v4(row + k);
-    a = fmaf(bf16lo(w.x), x[k], a);     a = fmaf(bf16hi(w.x), x[k + 1], a);
-    a = fmaf(bf16lo(w.y), x[k + 2], a); a = fmaf(bf16hi(w.y), x[k + 3], a);
-    a = fmaf(bf16lo(w.z), x[k + 4], a); a = fmaf(bf16hi(w.z), x[k + 5], a);
-    a = fmaf(bf16lo(w.w), x[k + 6], a); a = fmaf(bf16hi(w.w), x[k + 7], a);
-  }
-  return warp_sum(a);
-}
 
 __device__ __forceinline__ void rs_consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(RS_CONSUMERS) : "memory"); }
 
@@ -122,9 +86,7 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
   uint64_t* full = reinterpret_cast<uint64_t*>(b_ring + RS_STAGES * RS_STAGE);   // [STAGES] TMA -> consumers
   uint64_t* empty = full + RS_STAGES;              // [STAGES] consumers -> TMA (8 warp arrivals)
   float* s_lg = reinterpret_cast<float*>(full + 8);          // [2][64] logit halves
-  float* s_y = s_lg + 2 * RS_BM;                             // [2][d] y of the samples of the whole-step form
-  float* s_m = s_y + 2 * RS_D;                               // [2][d] m
-  float* s_ctrl = s_m + 2 * RS_D;                            // [2][d] control of the tile's first two samples
+  float* s_ctrl = s_lg + 2 * RS_BM;                          // [2][d] control of the tile's first two samples
   float* s_bm2 = s_ctrl + 2 * RS_D;                          // [d]
   float* s_wr = s_bm2 + RS_D;                                // [d]
 
@@ -190,61 +152,23 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
   const int nsamp = last_row / p.N - s_lo + 1;
   for (int q = 0; q < min(nsamp, 2); ++q)
     for (int i = tid; i < RS_D; i += RS_CONSUMERS) s_ctrl[q * RS_D + i] = __ldg(p.ctrl + (size_t)(s_lo + q) * RS_D + i);
-  if (p.Wy_t) {
-    for (int q = 0; q < nsamp; ++q) {
-      const int s = s_lo + q;
-      float* m = s_m + q * RS_D;
-      if (p.info_prev) {
-        // m[n] = [m_prev, info_prev] . Ww_t[n, :] + bw[n]: x read straight from global (2d floats, L1-resident)
-        const float* mp = p.mem_prev + (size_t)s * RS_D;
-        const float* ip = p.info_prev + (size_t)s * RS_D;
-        for (int n = warp; n < RS_D; n += RS_CONSUMERS / 32) {
-          const __nv_bfloat16* row = p.Ww_t + (size_t)n * 2 * RS_D;
-          float a = 0.f;
-          for (int k = lane * 8; k < 2 * RS_D; k += 256) {
-            const uint4 w = ldg_nc_v4(row + k);
-            const float* x = k < RS_D ? mp + k : ip + (k - RS_D);
-            const float4 x0 = __ldg(reinterpret_cast<const float4*>(x)), x1 = __ldg(reinterpret_cast<const float4*>(x) + 1);
-            a = fmaf(bf16lo(w.x), x0.x, a); a = fmaf(bf16hi(w.x), x0.y, a);
-            a = fmaf(bf16lo(w.y), x0.z, a); a = fmaf(bf16hi(w.y), x0.w, a);
-            a = fmaf(bf16lo(w.z), x1.x, a); a = fmaf(bf16hi(w.z), x1.y, a);
-            a = fmaf(bf16lo(w.w), x1.z, a); a = fmaf(bf16hi(w.w), x1.w, a);
-          }
-          a = warp_sum(a) + __ldg(p.bw + n);
-          if (lane == 0) {
-            m[n] = a;
-            if (s * p.N >= row0) p.mem_out[(size_t)s * RS_D + n] = a;     // the CTA owning the sample's first row
-          }
-        }
-      } else {
-        for (int i = tid; i < RS_D; i += RS_CONSUMERS) m[i] = p.mem_prev[(size_t)s * RS_D + i];
-      }
-    }
-    rs_consumer_bar();
-    for (int q = 0; q < nsamp; ++q)
-      for (int n = warp; n < RS_D; n += RS_CONSUMERS / 32) {
-        const float v = bf16_row_dot(p.Wy_t + (size_t)n * RS_D, s_m + q * RS_D, RS_D, lane) + __ldg(p.by + n);
-        if (lane == 0) s_y[q * RS_D + n] = v;
-      }
-    rs_consumer_bar();
-  }
-  // y rows of this thread's two P rows (rows past M are TMA zero fill and stay zero)
-  const float* yrow[2];
+  // y rows of this thread's two P rows (rows past M are TMA zero fill and stay zero), as 32-bit offsets into y rather than
+  // pointers: the two registers they save keep the kernel free of spills at its 168-register cap
+  int yoff[2];
 #pragma unroll
-  for (int u = 0; u < 2; ++u) {
-    const int s = min(row0 + prow + 32 * u, p.M - 1) / p.N;
-    yrow[u] = (p.Wy_t ? s_y + (s - s_lo) * RS_D : p.y + (size_t)s * RS_D) + pcol;
-  }
+  for (int u = 0; u < 2; ++u) yoff[u] = min(row0 + prow + 32 * u, p.M - 1) / p.N * RS_D + pcol;
 
   // ---- GEMM 1: P block j is scaled by y in place (P*y) while the MMAs of block j - 1 run, then block j is issued
   for (int j = 0; j < RS_KB; ++j) {
     const int s = j % RS_STAGES;
     unsigned char* stage = b_ring + s * RS_STAGE;
+    // y is loaded ahead of the stage's wait so the loads overlap it.  Plain loads: the compiler schedules __ldg
+    // (ld.global.nc) loads of y after the wait, where their latency is exposed
     float4 y0[2], y1[2];
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
-      y0[u] = *reinterpret_cast<const float4*>(yrow[u] + j * TC_BK);
-      y1[u] = *reinterpret_cast<const float4*>(yrow[u] + j * TC_BK + 4);
+      y0[u] = *reinterpret_cast<const float4*>(p.y + yoff[u] + j * TC_BK);
+      y1[u] = *reinterpret_cast<const float4*>(p.y + yoff[u] + j * TC_BK + 4);
     }
     mbar_wait(&full[s], (j / RS_STAGES) & 1);
 #pragma unroll
@@ -341,18 +265,9 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
 
 // inv = [P | Q] (tc_read_invariant); y, control [B, d] fp32; att [B, N], info [B, d]
 inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y, const float* control,
-                            const mac_read_weights* w, float* att, float* info, int B, int N, int d, cudaStream_t stream,
-                            const WholeStepArgs* ws = nullptr) {
+                            const mac_read_weights* w, float* att, float* info, int B, int N, int d, cudaStream_t stream) {
   if (!read_step_supported(B, N, d)) return MAC_ERR_UNSUPPORTED;
-  if (!inv || !kb_bf16 || (!y && !ws) || !control || !w->Wm_bf16 || !w->Wm2_bf16 || !att || !info) return MAC_ERR_INVALID;
-  if (ws) {
-    if (!whole_step_supported(B, N, d)) return MAC_ERR_UNSUPPORTED;
-    if (!ws->mem_prev || !ws->Wy_t_bf16 || !w->by) return MAC_ERR_INVALID;
-    if (ws->info_prev && (!ws->Ww_t_bf16 || !ws->bw || !ws->mem_out)) return MAC_ERR_INVALID;
-    if (!mac_aligned16(ws->mem_prev) || !mac_aligned16(ws->Wy_t_bf16) || (ws->info_prev && !mac_aligned16(ws->info_prev)) ||
-        (ws->Ww_t_bf16 && !mac_aligned16(ws->Ww_t_bf16)))
-      return MAC_ERR_ALIGN;
-  }
+  if (!inv || !kb_bf16 || !y || !control || !w->Wm_bf16 || !w->Wm2_bf16 || !att || !info) return MAC_ERR_INVALID;
   const int M = B * N;
   const TcReadScratch s = tc_read_scratch(const_cast<void*>(inv), B, N, d);
   CUtensorMap mp, mq, mw1, mw2;
@@ -365,12 +280,7 @@ inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y
   st = make_tmap_2d(&mw2, w->Wm2_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)d * 2, 256, TC_BK, 1);
   if (st != MAC_OK) return st;
   ReadStepParams p{};
-  p.M = M; p.N = N; p.y = y; p.ctrl = control; p.bm2 = w->bm2; p.wr = w->wr; p.Q = s.Q; p.logits = s.parts;
-  if (ws) {
-    p.y = nullptr; p.mem_prev = ws->mem_prev; p.info_prev = ws->info_prev; p.bw = ws->bw; p.by = w->by; p.mem_out = ws->mem_out;
-    p.Ww_t = reinterpret_cast<const __nv_bfloat16*>(ws->Ww_t_bf16);
-    p.Wy_t = reinterpret_cast<const __nv_bfloat16*>(ws->Wy_t_bf16);
-  }
+  p.M = M; p.N = N; p.y = y; p.ctrl = control; p.bm2 = w->bm2; p.wr = w->wr; p.logits = s.parts;
   // the opt-in is per device context: set it on every launch
   MAC_CUDA_TRY(cudaFuncSetAttribute(read_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM_BYTES));
   read_step_kernel<<<(M + RS_BM - 1) / RS_BM, RS_THREADS, RS_SMEM_BYTES, stream>>>(mp, mq, mw1, mw2, p);

@@ -548,12 +548,10 @@ inline int tc_read_chain(const float* kb_f32, const void* kb_bf16, const float* 
 // do not depend on the step.  They are computed once per forward into `inv` = [P | Q] (bf16), and each step runs
 //   PY = P * y_b ;  H = ELU(PY @ Wm[0:d, :] + Q) ;  logits = ... (unchanged)
 // i.e. 2 x d instead of 4 x d MACs per knowledge-base element and step.
-// [P | Q] bf16 slabs, then the scratch of the fused read step (read_step.cuh): P*y and H slabs, the logit partial sums
-// [B*N, d / TC_BN] and y [B, d]
+// [P | Q] bf16 slabs, then the fused read step's (read_step.cuh) logits, one per knowledge-base row [B*N]
 inline size_t tc_read_invariant_bytes(int B, int N, int d) {
   const size_t slab = (((size_t)B * N * d * 2 + 1023) & ~(size_t)1023);
-  const size_t parts = (((size_t)B * N * (d / TC_BN) * 4 + 1023) & ~(size_t)1023);
-  return 4 * slab + parts + (size_t)B * d * 4 + 1024;
+  return 2 * slab + (size_t)B * N * 4 + 1024;
 }
 
 // PY[m, :] = P[m, :] * y[m / rows_per_batch, :]   (8 bf16 per thread)
@@ -578,20 +576,16 @@ inline char* tc_align1k(void* p) {
 }
 
 struct TcReadScratch {
-  __nv_bfloat16 *P, *Q, *PY, *H;
-  float *parts, *y;
+  __nv_bfloat16 *P, *Q;
+  float* parts;
 };
 inline TcReadScratch tc_read_scratch(void* inv, int B, int N, int d) {
   const size_t slab = (((size_t)B * N * d * 2 + 1023) & ~(size_t)1023);
-  const size_t parts = (((size_t)B * N * (d / TC_BN) * 4 + 1023) & ~(size_t)1023);
   char* base = tc_align1k(inv);
   TcReadScratch s;
   s.P = reinterpret_cast<__nv_bfloat16*>(base);
   s.Q = reinterpret_cast<__nv_bfloat16*>(base + slab);
-  s.PY = reinterpret_cast<__nv_bfloat16*>(base + 2 * slab);
-  s.H = reinterpret_cast<__nv_bfloat16*>(base + 3 * slab);
-  s.parts = reinterpret_cast<float*>(base + 4 * slab);
-  s.y = reinterpret_cast<float*>(base + 4 * slab + parts);
+  s.parts = reinterpret_cast<float*>(base + 2 * slab);
   return s;
 }
 
@@ -633,17 +627,9 @@ inline int tc_read_chain_inv(const void* inv, const float* y, const float* contr
   MAC_LAUNCH_CHECK();
   TcGemmParams p{};
   p.M = M; p.N = d; p.rows_per_batch = N; p.ldo = d;
-  int st;
-  static const bool q_hoist = !(getenv("MAC_READ_QHOIST") && atoi(getenv("MAC_READ_QHOIST")) == 0);
-  if (q_hoist) {
-    // H = ELU(PY @ Wm[0:d] + Q)      (bm is inside Q)
-    p.epi = TC_EPI_ADDACT; p.act = MAC_ACT_ELU; p.bias = nullptr; p.out0 = H; p.add = Q;
-    st = tc_gemm_launch(PY, d, nullptr, 0, w->Wm_bf16, p, stream, nullptr, 2 * d);
-  } else {
-    // experiment switch: keep the concatenated K = 2d form, H = ELU([PY, P] @ Wm + bm), with only P hoisted
-    p.epi = TC_EPI_ACT; p.act = MAC_ACT_ELU; p.bias = w->bm; p.out0 = H;
-    st = tc_gemm_launch(PY, d, P, d, w->Wm_bf16, p, stream);
-  }
+  // H = ELU(PY @ Wm[0:d] + Q)      (bm is inside Q)
+  p.epi = TC_EPI_ADDACT; p.act = MAC_ACT_ELU; p.bias = nullptr; p.out0 = H; p.add = Q;
+  int st = tc_gemm_launch(PY, d, nullptr, 0, w->Wm_bf16, p, stream, nullptr, 2 * d);
   if (st != MAC_OK) return st;
   p.epi = TC_EPI_LOGITS; p.act = MAC_ACT_NON; p.bias = w->bm2; p.out0 = nullptr; p.add = nullptr;
   p.ctrl = control; p.wr = w->wr; p.parts = parts;

@@ -192,20 +192,6 @@ extern "C" int mac_read_step_fused(const void* inv, const void* kb_bf16, const f
   if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
   return read_step_launch(inv, kb_bf16, y, control, w, att, info, B, N, d, stream);
 }
-extern "C" int mac_step_fused(const void* inv, const void* kb_bf16, const float* mem_prev, const float* info_prev,
-                              const float* control, const mac_read_weights* w, const void* Ww_t_bf16, const float* bw,
-                              const void* Wy_t_bf16, float* mem_out, float* info, float* att, int B, int N, int d,
-                              mac_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!inv || !kb_bf16 || !mem_prev || !control || !w || !Wy_t_bf16 || !info || !att || B <= 0 || N <= 0 || d <= 0)
-    return MAC_ERR_INVALID;
-  if (!mac_aligned16(inv) || !mac_aligned16(kb_bf16) || !mac_aligned16(control)) return MAC_ERR_ALIGN;
-  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
-  WholeStepArgs ws{mem_prev, info_prev, Ww_t_bf16, bw, Wy_t_bf16, mem_out};
-  return read_step_launch(inv, kb_bf16, nullptr, control, w, att, info, B, N, d, stream, &ws);
-}
-extern "C" int mac_step_fused_supported(int B, int N, int d) { return whole_step_supported(B, N, d) ? 1 : 0; }
-
 extern "C" int mac_read_step_fused_supported(int B, int N, int d) { return read_step_supported(B, N, d) ? 1 : 0; }
 
 extern "C" int mac_read_fwd(const float* kb, const void* kb_bf16, const float* memory_in, const float* control,

@@ -197,17 +197,6 @@ class MACCell(object):
         self._y_for = -1
         self.kb_bf16 = None
         self.save_for_backward = bool(save_for_backward)
-        # whole-step form (mac_step_fused): the previous step's plain write unit and this step's memory projection run as
-        # per-sample matrix-vector products in front of the read step.  bf16 inference, shared cells, plain write unit (no
-        # self-attention / gate / write dropout), all dropouts at 1, d = 512, 128 < N <= 256.  OPT-IN (MAC_STEP_FUSED=1):
-        # the per-sample products read the write / projY weights once per sample (bf16 weights: less accurate than the
-        # batched split-bf16 GEMMs).
-        self._step_fused = bool(
-            self._read_hoist and self.prec == PREC["bf16"] and self._fused_write and not (c.writeSelfAtt or c.writeGate)
-            and not (c.writeDropout < 1.0 and float(writeDropout) < 1.0) and float(readDropout) >= 1.0
-            and float(memoryDropout) >= 1.0 and os.environ.get("MAC_STEP_FUSED", "0") == "1"
-            and os.environ.get("MAC_READ_FUSED", "1") != "0"
-            and self.lib.mac_step_fused_supported(B, N, d) == 1)
         # bf16 inference: the batch-sized projections of the step (projY, write unit, gate, ctrlProj) on tensor cores as
         # three-pass split-bf16 products (mac_linear_tc_small_fwd, fp32-class accuracy): 16-32 independent CTAs that can run
         # beside another pass's read kernels, which the 8-CTA-cluster fp32 kernel cannot; its own latency is higher than the
@@ -219,15 +208,13 @@ class MACCell(object):
         if self._small_tc:        # one launch for the write unit + the next projY: the folded form, whatever fold_y says
             self._fold_y = (self._read_hoist and self._fused_write and not (c.writeSelfAtt or c.writeGate)
                             and not (c.writeDropout < 1.0 and float(writeDropout) < 1.0))
-        self._pending_write = None       # step index i whose memory _hm[i] = write(_hm[i-1], _hi[i]) has not been launched yet
         recurrent_ctrl_ok = (c.controlFeedPrev and self._fused_control and not (c.controlWholeQ or c.controlContinuous
                                                                                 or c.unsharedCells))
         # Backward: the hand-scheduled sweep of autograd._Bwd covers the shipped flag files (fused read + write, control
         # either memory-independent or the plain recurrent chain); every other working flag combination records its
         # primitives on a tape (tape.py) and is differentiated node by node.  MAC_TAPE_BWD=1 forces the tape everywhere.
-        if c.memoryBN:                   # the normalised memory is what the next projY sees: no folded write + projY forms
+        if c.memoryBN:                   # the normalised memory is what the next projY sees: no folded write + projY form
             self._fold_y = False
-            self._step_fused = False
         scheduled_bwd_ok = (self._fused_read and self._fused_write and (self._hoist or recurrent_ctrl_ok)
                             and not c.memoryBN
                             and not (c.controlInWordsProj or c.controlOutWordsProj)      # wordsProj is outside _Bwd (ADVICE r1)
@@ -363,7 +350,6 @@ class MACCell(object):
         self._mem_in = self._new(B, d)
         self._y_next = self._new(B, d)
         self._y_for = -1
-        self._pending_write = None
         if self.save_for_backward:
             self._ctrl_saved = {}
             M = B * self.N
@@ -865,10 +851,6 @@ class MACCell(object):
             if self._tape is not None:
                 self._tape.copy(self._hc[i + 1], self.vecQuestions)
             newControl = self._hc[i + 1]
-        if self._step_fused:
-            newMemory = self._whole_step(i, memory, newControl, cellName)
-            self._set_histories(i + 1)
-            return self.none, MACCellTuple(newControl, newMemory)
         info = self.read(self.knowledgeBase, memory, newControl, name=cellName, _att_out=self._att_kb[i],
                          _out=self._hi[i + 1], _y_pre=self._y_next if self._y_for == i else None)
         if c.writeDropout < 1.0 and self.dropouts["write"] < 1.0:                      # mac_cell.py:461-463
@@ -880,73 +862,6 @@ class MACCell(object):
         self._y_for = i + 1 if fold else -1
         self._set_histories(i + 1)                                                     # mac_cell.py:472-474
         return self.none, MACCellTuple(newControl, newMemory)
-
-    # ------------------------------------------------------------------ whole step as one launch (inference)
-    def _ensure_read_inv(self, name):
-        """P = KB @ Wx + bx and Q = P @ Wm[d:2d] + bm, once per forward (mac_read_invariant)."""
-        if name not in self._read_inv:
-            B, N, d = self.B, self.N, self.d
-            rw = self._read_weights(name)
-            kb32 = None if self.knowledgeBase.dtype == torch.bfloat16 else ptr(self.knowledgeBase)
-            nbytes = self.lib.mac_read_invariant_bytes(B, N, d, self.prec)
-            inv = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            check(self.lib.mac_read_invariant(kb32, ptr(self.kb_bf16), ctypes.byref(rw), self.prec, ptr(inv), nbytes, B, N, d,
-                                              stream_ptr()), "mac_read_invariant")
-            self._read_inv[name] = inv
-        return self._read_inv[name]
-
-    def _step_weights_bf16(self, name):
-        """bf16 [out, in] copies of the write unit's newMemory weight and of projY for the in-kernel matrix-vector products."""
-        def build():
-            Ww, _ = self.params.lin("MACCell/write" + name + "/", "newMemory")
-            Wy, _ = self.params.lin("MACCell/read" + name + "/mulmemInter/", "projY")
-            out = []
-            for t in (Ww, Wy):
-                o = torch.empty((t.shape[1], t.shape[0]), dtype=torch.bfloat16, device=t.device)
-                check(self.lib.mac_pack_weight_bf16(ptr(t), ptr(o), t.shape[0], t.shape[1], stream_ptr()), "pack")
-                out.append(o)
-            return tuple(out)
-        return self.params.derived(("stepW16", name), build)
-
-    def _whole_step(self, i, memory, control, name):
-        """Step i as ONE launch: memory_i = write(memory_{i-1}, info_{i-1}) (deferred from the previous call), y_i, read_i.
-        The memory this call returns, `_hm[i+1]`, is produced by the NEXT call's kernel (or by `finish()` / the last step):
-        consumers inside the unroll only hand it back to `__call__`."""
-        B, N, d = self.B, self.N, self.d
-        rw = self._read_weights(name)
-        inv = self._ensure_read_inv(name)
-        Ww16, Wy16 = self._step_weights_bf16(name)
-        _, bw = self.params.lin("MACCell/write" + name + "/", "newMemory")
-        deferred = (self._pending_write == i and i > 0 and memory.data_ptr() == self._hm[i].data_ptr())
-        if not deferred:
-            self.finish()                                   # a pending memory belongs to an earlier, abandoned step chain
-        mem_prev = self._hm[i - 1] if deferred else memory
-        info_prev = self._hi[i] if deferred else None
-        att, info = self._att_kb[i], self._hi[i + 1]
-        check(self.lib.mac_step_fused(ptr(inv), ptr(self.kb_bf16), ptr(mem_prev), ptr(info_prev), ptr(control),
-                                      ctypes.byref(rw), ptr(Ww16), ptr(bw), ptr(Wy16), ptr(self._hm[i]) if deferred else None,
-                                      ptr(info), ptr(att), B, N, d, stream_ptr()), "mac_step_fused")
-        self.attentions["kb"].append(att)
-        if not deferred and memory.data_ptr() != self._hm[i].data_ptr():
-            self._hm[i].copy_(memory)                       # keep the history consistent with a caller-supplied memory
-        self._pending_write = i + 1
-        if i + 1 >= self.L:
-            self.finish()
-        return self._hm[i + 1]
-
-    def finish(self):
-        """Materialise a memory whose write unit was deferred into the next step's kernel (whole-step form)."""
-        j = self._pending_write
-        if j is None:
-            return
-        self._pending_write = None
-        saved, self._step_fused = self._step_fused, False
-        try:
-            self.iteration, it = j - 1, self.iteration
-            self.write(self._hm[j - 1], self._hi[j], self._hc[j], self.contControl, name="", _out=self._hm[j])
-            self.iteration = it
-        finally:
-            self._step_fused = saved
 
     def _read_inter_width(self):
         """Width of the tensor inter2att drops (mac_cell.py:209-266): the fused family ends in memDim columns."""
@@ -995,5 +910,4 @@ def mac_network(cell, netLength):
     for i in range(netLength):
         cell.iteration = i
         _, state = cell(none, state)
-    cell.finish()          # whole-step form: the last write unit, if the unroll stopped before cell.L steps
     return state.control, state.memory

@@ -199,32 +199,6 @@ def test_backward_full_shape_matches_autograd(variant, shape, dp):
     assert not bad, bad
 
 
-def test_whole_step_kernel_matches_separate_launches(monkeypatch):
-    """mac_step_fused (write unit of the previous step + projY in the fused kernel's prologue, ONE launch per reasoning step)
-    against the same cell with read / write / projY as separate launches (MAC_STEP_FUSED=0), headline shape.  The only
-    arithmetic difference is bf16 instead of fp32 weights in the two batch-sized matrix-vector products."""
-    cfg, inputs, params, ref = headline_case()
-    L = SHAPES["headline"][4]
-    from mac_network_b200 import _lib
-    monkeypatch.setenv("MAC_STEP_FUSED", "1")        # opt-in form (slower and less accurate than the default: DESIGN.md)
-    n0 = _lib.load().mac_b200_launch_count()
-    fused, cell = run_gpu(cfg, params, inputs, L, prec="bf16")
-    n_fused = _lib.load().mac_b200_launch_count() - n0
-    assert cell._step_fused, "whole-step form not selected at the headline shape"
-    monkeypatch.setenv("MAC_STEP_FUSED", "0")
-    n0 = _lib.load().mac_b200_launch_count()
-    sep, cell2 = run_gpu(cfg, params, inputs, L, prec="bf16")
-    n_sep = _lib.load().mac_b200_launch_count() - n0
-    assert not cell2._step_fused
-    print("launches per 12-step pass: whole-step %d, separate %d" % (n_fused, n_sep))
-    assert n_fused < n_sep
-    for k in ("memory", "info", "att_kb"):
-        e = max(max_rel(fused[k][i], sep[k][i]) for i in range(L))
-        print("whole-step vs separate launches,", k, e)
-        assert e < 8e-3, (k, e)        # bf16 weights on the state path: memory 3.8e-3 vs the oracle (measured)
-    assert np.array_equal(fused["control"], sep["control"])
-
-
 @pytest.mark.parametrize("variant", ["args", "gqa"])
 def test_bf16_throughput_form_small_projections_on_tensor_cores(monkeypatch, variant):
     """The throughput form of the bf16 cell (MACCell(small_tc=True) / MAC_SMALL_TC=1: projY, write unit, gate and ctrlProj
