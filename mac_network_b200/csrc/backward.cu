@@ -884,6 +884,9 @@ extern "C" int mac_read_bwd(const float* kb, const float* memory_in, const float
     if (st != MAC_OK) return st;
   }
   // (7) y = md @ Wy + by with md = dropout(memory_in):  dWy += md^T dy ; dby += colsum(dy) ; dmem_in = (dy @ Wy^T)*mask/keep
+  // mac_linear_bwd gets no workspace, so these K = B products run without split-K.  Its split-K partials would start at
+  // ws + BW_HEADER = f, and at small N (B*N*4 < splitk*d) they would overwrite its own inputs dy, md and dmd, which live
+  // in f behind the [B*N] buffers.
   const float* mdp = memory_in;
   if (drop) {
     st = mac_dropout_fwd(memory_in, keep_read, seed, MAC_SITE_READ_MEM, step, md, (long long)B * d, stream_);
@@ -895,7 +898,7 @@ extern "C" int mac_read_bwd(const float* kb, const float* memory_in, const float
     const int ks[1] = {d};
     float* dxs[1] = {drop ? dmd : dmem_in};
     const int acc0[1] = {0};
-    st = mac_linear_bwd(xs, ks, ks, 1, Wy_t, dy, d, dxs, ks, acc0, dWy, dby, B, d, ws, BW_HEADER + pbytes / 2, stream_);
+    st = mac_linear_bwd(xs, ks, ks, 1, Wy_t, dy, d, dxs, ks, acc0, dWy, dby, B, d, nullptr, 0, stream_);
     if (st != MAC_OK) return st;
     if (drop) {
       st = mac_dropout_fwd(dmd, keep_read, seed, MAC_SITE_READ_MEM, step, dmem_in, (long long)B * d, stream_);
