@@ -152,8 +152,9 @@ int mac_read_fwd_inv(const float* kb, const void* kb_bf16, const void* inv, cons
  * as one wgmma kernel over 64-row tiles of the knowledge base (P*y, H and I2 stay on the SM; one logit per row) and the
  * kb_attend launch (softmax + weighted sum).  The logits go to the scratch that mac_read_invariant_bytes reserves behind
  * [P | Q] in `inv`, one float per row (so `inv` is read AND written by this call: one call at a time per `inv`).
- * mac_read_fwd_inv dispatches to it when mac_read_step_fused_supported(B, N, d) (d == 512, N <= 256, B < 2^22) unless
- * the environment sets MAC_READ_FUSED=0.  Returns MAC_ERR_UNSUPPORTED for other shapes. */
+ * Returns MAC_ERR_UNSUPPORTED unless mac_read_step_fused_supported(B, N, d) (d == 512, N <= 256, B < 2^22).
+ * mac_read_fwd_inv with MAC_PREC_BF16 and kb_bf16 dispatches to it whenever the shape is supported, and runs other
+ * shapes as four launches (scale, two GEMMs, kb_attend). */
 int mac_read_step_fused(const void* inv, const void* kb_bf16, const float* y, const float* control,
                         const mac_read_weights* w, float* info, float* att, int B, int N, int d, mac_stream_t stream);
 int mac_read_step_fused_supported(int B, int N, int d);

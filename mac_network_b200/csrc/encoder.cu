@@ -17,7 +17,6 @@
 // and the gate derivatives of step s as the epilogue; the parameter and input gradients of all steps are then two GEMMs per
 // direction over the [B*S, 4h] gate-gradient matrix (mac_linear_bwd on the segments [dropout(X), h_prev]).
 #include <cooperative_groups.h>
-#include <stdlib.h>
 #include "common.cuh"
 
 namespace mac {
@@ -430,9 +429,8 @@ extern "C" int mac_lstm_fwd(const float* gx_fw, const float* gx_bw, const float*
   p.save_gates = save_gates; p.save_c = save_c; p.save_hprev = save_hprev;
   p.B = B; p.S = S; p.h = h; p.ndir = ndir;
   // h == 256 (encDim 512, the reference default): the whole recurrence in one cluster launch (703 vs 805 us for the encoder
-  // forward at B=64, S=40, profiles/r1/lstm_bench_r1.jsonl); MAC_LSTM_PERSIST=0 selects the per-step form.  Both parity-tested.
-  const char* env = getenv("MAC_LSTM_PERSIST");
-  if (h == LP_H && !(env && env[0] == '0')) {
+  // forward at B=64, S=40, profiles/r1/lstm_bench_r1.jsonl); every other h runs the per-step kernels below.
+  if (h == LP_H) {
     const size_t psmem = ((size_t)LP_H * LP_HU * 4 + (size_t)2 * LP_RB * (LP_H + 4)) * sizeof(float);
     MAC_CUDA_TRY(cudaFuncSetAttribute(lstm_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
     cudaLaunchConfig_t cfg{};

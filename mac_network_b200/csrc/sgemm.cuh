@@ -7,7 +7,6 @@
 // deterministic.
 #pragma once
 #include "common.cuh"
-#include <stdlib.h>
 
 namespace mac {
 
@@ -431,7 +430,7 @@ inline int sgemm_launch(SgemmParams p, unsigned int* counters, float* partial, s
                         cudaStream_t stream, bool allow_splitk = true) {
   if (p.M <= 0 || p.N <= 0 || p.K <= 0) return MAC_ERR_INVALID;
   if ((p.N & 3) || ((p.K & 3) && p.a_mode < A_TRANS)) return MAC_ERR_INVALID;   // transposed views walk K row by row
-  if (allow_splitk && skinny_ok(p) && !getenv("MAC_NO_SKINNY")) return skinny_launch(p, stream);   // M <= 64: cluster/DSMEM split-K kernel
+  if (allow_splitk && skinny_ok(p)) return skinny_launch(p, stream);   // M <= 64: cluster/DSMEM split-K kernel
   if (p.a_mode >= A_TRANS && (p.M & 3)) return MAC_ERR_INVALID;
   const bool big = sgemm_big_tiles(p.M, p.N, p.K);
   const int BM = big ? 128 : 64, BN = big ? 128 : 64;

@@ -33,7 +33,7 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
 
-static __global__ void __launch_bounds__(SK_THREADS) skinny_gemm_kernel(const SgemmParams p, int ks, int dbg) {
+static __global__ void __launch_bounds__(SK_THREADS) skinny_gemm_kernel(const SgemmParams p, int ks) {
   extern __shared__ __align__(16) float sk_smem[];
   const int XP = ks + 4;                        // row pitch of the A slice (16-byte aligned rows)
   float* ws = sk_smem;                          // [ks][SK_BN]       W slice
@@ -47,25 +47,23 @@ static __global__ void __launch_bounds__(SK_THREADS) skinny_gemm_kernel(const Sg
 
   // ---- operand load: 16-byte cp.async (LDGSTS) straight into shared memory -- every request of the CTA is in flight
   //      at once, no register staging, one L2 round trip
-  if (!(dbg & 1)) {
-    const int xc = ks / 4;
-    for (int f = tid; f < SK_BM * xc; f += SK_THREADS) {
-      const int row = f / xc, c = f % xc;
-      const float* src = sk_ptr_a(p, row, k0 + c * 4);
-      float* dst = xs + (size_t)row * XP + c * 4;
-      if (src) cp_async16(dst, src);
-      else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    for (int f = tid; f < ks * (SK_BN / 4); f += SK_THREADS) {
-      const int kr = f / (SK_BN / 4), c = f % (SK_BN / 4);
-      const int n = n0 + c * 4;
-      float* dst = ws + (size_t)kr * SK_BN + c * 4;
-      if (n < p.N) cp_async16(dst, p.W + (size_t)(k0 + kr) * p.ldw + n);
-      else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
+  const int xc = ks / 4;
+  for (int f = tid; f < SK_BM * xc; f += SK_THREADS) {
+    const int row = f / xc, c = f % xc;
+    const float* src = sk_ptr_a(p, row, k0 + c * 4);
+    float* dst = xs + (size_t)row * XP + c * 4;
+    if (src) cp_async16(dst, src);
+    else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
   }
+  for (int f = tid; f < ks * (SK_BN / 4); f += SK_THREADS) {
+    const int kr = f / (SK_BN / 4), c = f % (SK_BN / 4);
+    const int n = n0 + c * 4;
+    float* dst = ws + (size_t)kr * SK_BN + c * 4;
+    if (n < p.N) cp_async16(dst, p.W + (size_t)(k0 + kr) * p.ldw + n);
+    else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
 
   // ---- 64 x 32 x ks product, 4 x 4 outputs per thread (2 LDS.128 per 16 FMAs: shared-memory bandwidth is the limit)
@@ -75,25 +73,23 @@ static __global__ void __launch_bounds__(SK_THREADS) skinny_gemm_kernel(const Sg
   for (int i = 0; i < 4; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  if (!(dbg & 2)) {
-    const float* xr = xs + (size_t)(rg * 4) * XP;
+  const float* xr = xs + (size_t)(rg * 4) * XP;
 #pragma unroll 2
-    for (int k = 0; k < ks; k += 4) {
-      float4 a[4], w[4];
+  for (int k = 0; k < ks; k += 4) {
+    float4 a[4], w[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(xr + (size_t)i * XP + k);
+    for (int i = 0; i < 4; ++i) a[i] = *reinterpret_cast<const float4*>(xr + (size_t)i * XP + k);
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) w[kk] = *reinterpret_cast<const float4*>(ws + (k + kk) * SK_BN + cgp * 4);
+    for (int kk = 0; kk < 4; ++kk) w[kk] = *reinterpret_cast<const float4*>(ws + (k + kk) * SK_BN + cgp * 4);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float av[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
+    for (int i = 0; i < 4; ++i) {
+      const float av[4] = {a[i].x, a[i].y, a[i].z, a[i].w};
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          acc[i][0] = fmaf(av[kk], w[kk].x, acc[i][0]);
-          acc[i][1] = fmaf(av[kk], w[kk].y, acc[i][1]);
-          acc[i][2] = fmaf(av[kk], w[kk].z, acc[i][2]);
-          acc[i][3] = fmaf(av[kk], w[kk].w, acc[i][3]);
-        }
+      for (int kk = 0; kk < 4; ++kk) {
+        acc[i][0] = fmaf(av[kk], w[kk].x, acc[i][0]);
+        acc[i][1] = fmaf(av[kk], w[kk].y, acc[i][1]);
+        acc[i][2] = fmaf(av[kk], w[kk].z, acc[i][2]);
+        acc[i][3] = fmaf(av[kk], w[kk].w, acc[i][3]);
       }
     }
   }
@@ -109,10 +105,7 @@ static __global__ void __launch_bounds__(SK_THREADS) skinny_gemm_kernel(const Sg
     const int rr = rank * (SK_BM / SK_CLUSTER) + e / SK_BN, c = e % SK_BN;
     float s = 0.f;
 #pragma unroll
-    for (int z = 0; z < SK_CLUSTER; ++z) {
-      const float* remote = (dbg & 4) ? part : cluster.map_shared_rank(part, z);
-      s += remote[rr * SK_BN + c];
-    }
+    for (int z = 0; z < SK_CLUSTER; ++z) s += cluster.map_shared_rank(part, z)[rr * SK_BN + c];
     const int m = rr, n = n0 + c;
     if (m < p.M && n < p.N) {
       float t = s + p.bias_const + (p.bias ? __ldg(p.bias + n) : 0.f);
@@ -156,9 +149,7 @@ inline int skinny_launch(const SgemmParams& p, cudaStream_t stream) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  int dbg = 0;
-  if (const char* e = getenv("MAC_SK_DEBUG")) dbg = atoi(e);
-  MAC_CUDA_TRY(cudaLaunchKernelEx(&cfg, skinny_gemm_kernel, p, ks, dbg));
+  MAC_CUDA_TRY(cudaLaunchKernelEx(&cfg, skinny_gemm_kernel, p, ks));
   MAC_LAUNCH_CHECK();
   return MAC_OK;
 }

@@ -177,12 +177,6 @@ static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, 
                          uint64_t seed, int step, int prec, float* info, float* att, float* save, void* workspace,
                          size_t workspace_bytes, int B, int N, int d, mac_stream_t stream_);
 
-// MAC_READ_FUSED=0 keeps the four-launch form of the inference read step (scale, two GEMMs, attention) for comparison
-static bool read_step_enabled() {
-  static const bool on = !(getenv("MAC_READ_FUSED") && atoi(getenv("MAC_READ_FUSED")) == 0);
-  return on;
-}
-
 extern "C" int mac_read_step_fused(const void* inv, const void* kb_bf16, const float* y, const float* control,
                                    const mac_read_weights* w, float* info, float* att, int B, int N, int d,
                                    mac_stream_t stream_) {
@@ -260,7 +254,7 @@ static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, 
     if (st != MAC_OK) return st;
   }
   int nparts = 0;
-  if (inv && prec == MAC_PREC_BF16 && kb_bf16 && read_step_supported(B, N, d) && read_step_enabled()) {
+  if (inv && prec == MAC_PREC_BF16 && kb_bf16 && read_step_supported(B, N, d)) {
     // the whole step (P*y, both projections, logits, softmax, weighted sum) as ONE kernel: read_step.cuh
     return read_step_launch(inv, kb_bf16, y, control, w, att, info, B, N, d, stream);
   }

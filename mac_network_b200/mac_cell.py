@@ -20,7 +20,6 @@ plus the three units with the reference signatures (`control` 133-187, `read` 20
 """
 import collections
 import ctypes
-import os
 
 import numpy as np
 import torch
@@ -140,7 +139,8 @@ class MACCell(object):
 
     def __init__(self, vecQuestions, questionWords, questionCntxWords, questionLengths, knowledgeBase,
                  memoryDropout, readDropout, writeDropout, batchSize, train, reuse=None, *,
-                 config=None, params=None, prec="fp32", seed=0, save_for_backward=False, fold_y=None, small_tc=None):
+                 config=None, params=None, prec="fp32", seed=0, save_for_backward=False, fold_y=None, small_tc=None,
+                 tape_bwd=False):
         self.lib = _lib.load()
         self.cfg = config if config is not None else _defaults["config"]
         self.params = params if params is not None else _defaults["params"]
@@ -185,15 +185,8 @@ class MACCell(object):
                        and self._fused_control)
         self._rw = {}
         self._read_inv = {}
-        # eval-mode hoist of the step-invariant read projections (shared cells only; env MAC_NO_READ_HOIST=1 disables)
-        self._read_hoist = (self._fused_read and not c.unsharedCells and not save_for_backward
-                            and os.environ.get("MAC_NO_READ_HOIST", "0") != "1")
-        # plain write unit: its GEMM also produces the next step's memory projection.  It shortens the dependency chain of
-        # ONE pass; with several independent passes in flight the two smaller GEMMs can pack better, so throughput callers
-        # may pass fold_y=False.  fold_y=None: on unless env MAC_NO_FOLD_Y=1.
-        want_fold = (os.environ.get("MAC_NO_FOLD_Y", "0") != "1") if fold_y is None else bool(fold_y)
-        self._fold_y = (self._read_hoist and self._fused_write and not (c.writeSelfAtt or c.writeGate)
-                        and not (c.writeDropout < 1.0 and float(writeDropout) < 1.0) and want_fold)
+        # eval-mode hoist of the step-invariant read projections (shared cells only)
+        self._read_hoist = self._fused_read and not c.unsharedCells and not save_for_backward
         self._y_for = -1
         self.kb_bf16 = None
         self.save_for_backward = bool(save_for_backward)
@@ -201,26 +194,28 @@ class MACCell(object):
         # three-pass split-bf16 products (mac_linear_tc_small_fwd, fp32-class accuracy): 16-32 independent CTAs that can run
         # beside another pass's read kernels, which the 8-CTA-cluster fp32 kernel cannot; its own latency is higher than the
         # cluster kernel's, so it is the THROUGHPUT form: small_tc=True (callers with several passes in flight: bench.py,
-        # serving.HostPipeline), or MAC_SMALL_TC=1; default off.
-        want_tc = (os.environ.get("MAC_SMALL_TC", "0") == "1") if small_tc is None else bool(small_tc)
-        self._small_tc = bool(want_tc and self.prec == PREC["bf16"] and not save_for_backward and B <= 128 and d % 64 == 0
-                              and self._fused_write and os.environ.get("MAC_SMALL_TC", "1") != "0")
-        if self._small_tc:        # one launch for the write unit + the next projY: the folded form, whatever fold_y says
-            self._fold_y = (self._read_hoist and self._fused_write and not (c.writeSelfAtt or c.writeGate)
-                            and not (c.writeDropout < 1.0 and float(writeDropout) < 1.0))
+        # serving.HostPipeline); default off.
+        self._small_tc = bool(small_tc and self.prec == PREC["bf16"] and not save_for_backward and B <= 128 and d % 64 == 0
+                              and self._fused_write)
+        # plain write unit: its GEMM also produces the next step's memory projection.  It shortens the dependency chain of
+        # ONE pass; with several independent passes in flight the two smaller GEMMs can pack better, so throughput callers
+        # may pass fold_y=False.  fold_y=None: on.  The throughput form (small_tc) always folds: one launch for the write
+        # unit + the next projY.  With memoryBN the normalised memory is what the next projY sees: no folded form.
+        self._fold_y = (self._read_hoist and self._fused_write and not (c.writeSelfAtt or c.writeGate)
+                        and not (c.writeDropout < 1.0 and float(writeDropout) < 1.0) and not c.memoryBN
+                        and (fold_y is None or bool(fold_y) or self._small_tc))
         recurrent_ctrl_ok = (c.controlFeedPrev and self._fused_control and not (c.controlWholeQ or c.controlContinuous
                                                                                 or c.unsharedCells))
         # Backward: the hand-scheduled sweep of autograd._Bwd covers the shipped flag files (fused read + write, control
         # either memory-independent or the plain recurrent chain); every other working flag combination records its
-        # primitives on a tape (tape.py) and is differentiated node by node.  MAC_TAPE_BWD=1 forces the tape everywhere.
-        if c.memoryBN:                   # the normalised memory is what the next projY sees: no folded write + projY form
-            self._fold_y = False
+        # primitives on a tape (tape.py) and is differentiated node by node.  tape_bwd=True records the tape even where the
+        # scheduled sweep applies (a check of the tape machinery on the shipped flag files).
         scheduled_bwd_ok = (self._fused_read and self._fused_write and (self._hoist or recurrent_ctrl_ok)
                             and not c.memoryBN
                             and not (c.controlInWordsProj or c.controlOutWordsProj)      # wordsProj is outside _Bwd (ADVICE r1)
                             and not (c.controlFeedPrev and not c.controlFeedPrevAtt)
                             and not (c.controlFeedPrev and c.writeSelfAtt and c.writeSelfAttMod == "CONT"))
-        self._use_tape = self.save_for_backward and (not scheduled_bwd_ok or os.environ.get("MAC_TAPE_BWD", "0") == "1")
+        self._use_tape = self.save_for_backward and (not scheduled_bwd_ok or tape_bwd)
         self._tape = None
         if self._use_tape:
             if self.prec != PREC["fp32"]:

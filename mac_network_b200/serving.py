@@ -81,7 +81,7 @@ def device_for_rank(local_rank, local_world):
     """CUDA device index of a local rank: the identity when every visible GPU is used (or the topology is unknown), else the
     NUMA-spread order above.  Deterministic, so every rank computes the same assignment without talking."""
     n = torch.cuda.device_count()
-    if local_world >= n or os.environ.get("MAC_NO_GPU_SPREAD", "0") == "1":
+    if local_world >= n:
         return local_rank
     nodes = gpu_numa_nodes()
     if len(set(nodes)) <= 1 or any(x < 0 for x in nodes):
@@ -159,21 +159,17 @@ class HostPipeline(object):
 
     def __init__(self, cfg, params, shape, prec="bf16", slots=4, use_graph=True, cast_threads=None, fold_y=None,
                  host_cast=None, stage_ring=None):
-        """`host_cast`: None = decide here (bf16 path: cast the knowledge base to bf16 on the host if that is faster than the
-        PCIe time it saves); False = never.  Callers that run several ranks per socket pass False: the cast makes a pass touch
-        ~57 MB of host DRAM (fp32 read + bf16 write + DMA read) instead of 31 MB, and the ranks of one socket share its memory
-        bandwidth."""
+        """`host_cast` (bf16 path only): None = decide here (cast the knowledge base to bf16 on the host if that is faster
+        than the PCIe time it saves); False = never; True = always.  Callers that run several ranks per socket pass False:
+        the cast makes a pass touch ~57 MB of host DRAM (fp32 read + bf16 write + DMA read) instead of 31 MB, and the ranks
+        of one socket share its memory bandwidth."""
         self.lib = _lib.load()
         self.shape = shape
         self.prec = prec
-        self.host_kb_bf16 = (prec == "bf16" and os.environ.get("MAC_NO_HOST_CAST", "0") != "1"
-                             and os.environ.get("MAC_NO_READ_HOIST", "0") != "1" and cfg.is_fast_path
-                             and not cfg.unsharedCells and host_cast is not False)
+        self.host_kb_bf16 = (prec == "bf16" and cfg.is_fast_path and not cfg.unsharedCells and host_cast is not False)
         self.cast_threads = int(cast_threads) if cast_threads else max(1, min(12, usable_cpus() - 2))
-        if os.environ.get("MAC_HOST_CAST_THREADS"):
-            self.cast_threads = max(1, int(os.environ["MAC_HOST_CAST_THREADS"]))
         self.cast_ms = None
-        if self.host_kb_bf16 and os.environ.get("MAC_NO_HOST_CAST", "") != "0":
+        if self.host_kb_bf16 and host_cast is None:
             # the cast pays off only if it is faster than the PCIe time of the bytes it saves (2 B per KB element at a
             # conservative 25 GB/s); with few host threads per rank (torchrun on a small CPU quota) it is not
             self.cast_ms = self._time_cast(shape)
@@ -192,22 +188,16 @@ class HostPipeline(object):
         # what the cast writes and the H2D engine reads stays in the socket's last-level cache -- the cast then costs DRAM only
         # its fp32 read.  Measured with two ranks on one socket (reasoning-steps/s, both ranks): 30.3k with 12 full-size buffers
         # per rank, 36.9k with 3, 43.4k with 2; no cast: 40.0k.  One rank: 28.4k / 28.9k / 25.2k with 2 / 3 / 12.
-        # The batch can also go through the ring in several pieces (MAC_HOST_CAST_CHUNKS), the cast of piece c+1 under the
-        # copy of piece c: measured WORSE (4 pieces: 18.6k with one rank, 18.8-24.3k with two) -- every piece is one more
-        # wake-up of the cast pool and one more blocking wait in the submit loop -- so the default is one piece.
-        self.chunks = max(1, int(os.environ.get("MAC_HOST_CAST_CHUNKS", "1")))
-        n_kb = B * N * d
-        while n_kb % (self.chunks * 64):
-            self.chunks -= 1
-        self.chunk_elems = n_kb // self.chunks
+        # Each buffer takes a whole knowledge base: casting it in several pieces, the cast of piece c+1 under the copy of
+        # piece c, measured WORSE (4 pieces: 18.6k with one rank, 18.8-24.3k with two) -- every piece is one more wake-up of
+        # the cast pool and one more blocking wait in the submit loop.
         # `stage_ring`: 3 full-size buffers when this rank has its socket to itself (one more pass of slack between a buffer's
         # copy and its next cast), 2 when the socket's cache is shared with another rank's ring (callers pass it; default 3)
-        ring = int(os.environ.get("MAC_HOST_STAGE_RING", "0")) or (int(stage_ring) if stage_ring else 3) * self.chunks
-        ring = max(2, ring)
-        self._stages = ([torch.empty(self.chunk_elems, dtype=torch.bfloat16).pin_memory() for _ in range(ring)]
+        ring = max(2, int(stage_ring) if stage_ring else 3)
+        self._stages = ([torch.empty(B * N * d, dtype=torch.bfloat16).pin_memory() for _ in range(ring)]
                         if self.host_kb_bf16 else [])
         self._stage_busy = [None] * len(self._stages)      # event after the copy that last read each buffer
-        self._piece = 0                                     # running index of the next piece to cast (pass * chunks + c)
+        self._casts = 0                                     # casts started so far: the next one's place in the ring
         kb_bytes = B * N * d * (2 if self.host_kb_bf16 else 4)
         self.h2d_bytes = kb_bytes + B * S * d * 4 + B * d * 4 + B * 4
         self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.slots[0].outs_host.values())
@@ -224,24 +214,23 @@ class HostPipeline(object):
             best = min(best, time.perf_counter() - t0)
         return best * 1e3
 
-    # -- host cast of the knowledge base on the library's thread pool, one PIECE ahead of the copies
+    # -- host cast of the knowledge base on the library's thread pool, one batch ahead of the copies
     #    (mac_host_cast_bf16_begin returns at once; no Python threads, so no GIL hand-offs in the submit loop)
-    def _cast_begin(self, kb, c):
-        """Start the cast of piece c of `kb` into the next staging buffer; returns that buffer's ring index."""
-        si = self._piece % len(self._stages)
-        self._piece += 1
+    def _cast_begin(self, kb):
+        """Start the cast of `kb` into the next staging buffer; returns that buffer's ring index."""
+        si = self._casts % len(self._stages)
+        self._casts += 1
         if self._stage_busy[si] is not None:
             self._stage_busy[si].synchronize()         # the previous copy out of this staging buffer has finished
             self._stage_busy[si] = None
-        src = kb.data_ptr() + 4 * c * self.chunk_elems
-        st = self.lib.mac_host_cast_bf16_begin(ctypes.c_void_p(src), ctypes.c_void_p(self._stages[si].data_ptr()),
-                                               self.chunk_elems, self.cast_threads)
+        st = self.lib.mac_host_cast_bf16_begin(ctypes.c_void_p(kb.data_ptr()), ctypes.c_void_p(self._stages[si].data_ptr()),
+                                               self._stages[si].numel(), self.cast_threads)
         if st != 0:
             raise _lib.MacB200Error("mac_host_cast_bf16_begin failed: %d" % st)
         return si
 
     def prefetch(self, batch):
-        """Optional: start the host cast (of the first piece) for the batch that the NEXT submit() will take."""
+        """Optional: start the host cast for the batch that the NEXT submit() will take."""
         if not self.host_kb_bf16:
             return
         kb = batch["knowledgeBase"]
@@ -249,8 +238,8 @@ class HostPipeline(object):
             if self._cast_for[0] == self._next and self._cast_for[1] is kb:
                 return
             self.lib.mac_host_cast_bf16_end()
-            self._piece -= 1                           # that piece is discarded: its staging buffer is taken again
-        si = self._cast_begin(kb, 0)
+            self._casts -= 1                           # that cast is discarded: its staging buffer is taken again
+        si = self._cast_begin(kb)
         self._cast_for = (self._next, kb, si)
 
     def submit(self, batch, next_batch=None):
@@ -266,19 +255,14 @@ class HostPipeline(object):
             slot.x["questionCntxWords"].copy_(batch["questionCntxWords"], non_blocking=True)
             slot.x["questionLengths"].copy_(batch["questionLengths"], non_blocking=True)
             if self.host_kb_bf16:
-                kb, dev = batch["knowledgeBase"], slot.x["knowledgeBase"].view(-1)
-                for c in range(self.chunks):
-                    self.lib.mac_host_cast_bf16_end()                  # piece c is in its staging buffer
-                    cur = si
-                    if c + 1 < self.chunks:
-                        si = self._cast_begin(kb, c + 1)               # cast of the next piece runs under this piece's copy
-                    elif next_batch is not None:
-                        si = self._cast_begin(next_batch["knowledgeBase"], 0)
-                        self._cast_for = (self._next, next_batch["knowledgeBase"], si)
-                    dev[c * self.chunk_elems:(c + 1) * self.chunk_elems].copy_(self._stages[cur], non_blocking=True)
-                    ev = torch.cuda.Event()
-                    ev.record(slot.stream)
-                    self._stage_busy[cur] = ev
+                self.lib.mac_host_cast_bf16_end()                      # the knowledge base is in its staging buffer
+                if next_batch is not None:                             # the next batch's cast runs under this copy
+                    nsi = self._cast_begin(next_batch["knowledgeBase"])
+                    self._cast_for = (self._next, next_batch["knowledgeBase"], nsi)
+                slot.x["knowledgeBase"].view(-1).copy_(self._stages[si], non_blocking=True)
+                ev = torch.cuda.Event()
+                ev.record(slot.stream)
+                self._stage_busy[si] = ev
             else:
                 slot.x["knowledgeBase"].copy_(batch["knowledgeBase"], non_blocking=True)
                 if next_batch is not None:

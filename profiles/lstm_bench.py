@@ -1,5 +1,5 @@
-"""Question input unit timing at the headline question shape (B=64, S=40, E=300, 2 x 256): per-step LSTM launches vs the
-persistent cluster kernel (MAC_LSTM_PERSIST=1), forward only and forward+backward, eager and as a CUDA graph."""
+"""Question input unit timing at the headline question shape (B=64, S=40, E=300, 2 x 256, which runs the persistent
+cluster kernel of the LSTM): forward only and forward+backward, eager and as a CUDA graph."""
 import json
 import os
 import sys
@@ -35,25 +35,25 @@ def timeit(fn, iters=20):
     return e0.elapsed_time(e1) / iters * 1e3
 
 
-for mode in ("0", "1"):
-    os.environ["MAC_LSTM_PERSIST"] = mode
-    enc = QuestionEncoder(dev)
-    out = {"MAC_LSTM_PERSIST": mode}
-    out["forward_eager_us"] = timeit(lambda: enc.forward(qd, ld))
-    g = torch.cuda.CUDAGraph()
-    s = torch.cuda.Stream()
-    with torch.cuda.stream(s):
+enc = QuestionEncoder(dev)
+out = {"forward_eager_us": timeit(lambda: enc.forward(qd, ld))}
+g = torch.cuda.CUDAGraph()
+s = torch.cuda.Stream()
+with torch.cuda.stream(s):
+    enc.forward(qd, ld)
+    s.synchronize()
+    with torch.cuda.graph(g, stream=s):
         enc.forward(qd, ld)
-        s.synchronize()
-        with torch.cuda.graph(g, stream=s):
-            enc.forward(qd, ld)
-    out["forward_graph_us"] = timeit(g.replay)
-    enc_t = QuestionEncoder(dev, keep_input=0.85, keep_question=0.92)
-    grads = {k: torch.zeros_like(v) for k, v in dev.items()}
-    dc, dq = torch.randn(B, S, D, device="cuda"), torch.randn(B, D, device="cuda")
+out["forward_graph_us"] = timeit(g.replay)
+enc_t = QuestionEncoder(dev, keep_input=0.85, keep_question=0.92)
+grads = {k: torch.zeros_like(v) for k, v in dev.items()}
+dc, dq = torch.randn(B, S, D, device="cuda"), torch.randn(B, D, device="cuda")
 
-    def fb():
-        enc_t.forward(qd, ld, save_for_backward=True)
-        enc_t.backward(dc, dq, grads)
-    out["train_forward_backward_eager_us"] = timeit(fb, iters=10)
-    print(json.dumps(out), flush=True)
+
+def fb():
+    enc_t.forward(qd, ld, save_for_backward=True)
+    enc_t.backward(dc, dq, grads)
+
+
+out["train_forward_backward_eager_us"] = timeit(fb, iters=10)
+print(json.dumps(out), flush=True)

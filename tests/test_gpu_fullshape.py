@@ -88,9 +88,10 @@ def test_bf16_gqa_shape_error_is_bounded_tightly():
     assert errs["memory"] < 1.5e-3 and errs["info"] < 4e-3 and errs["att_kb"] < 3e-3, errs    # measured 3.6e-4 / 1.3e-3 / 7.2e-4
 
 
-def test_fused_read_step_equals_unfused_chain(monkeypatch):
-    """The fused read step (csrc/read_step.cuh) against the four-launch chain it replaces, same inputs through the C ABI:
-    attention and retrieved information agree to fp32 summation order (the bf16 roundings are identical)."""
+def test_fused_read_step_equals_unfused_chain():
+    """The fused read step (csrc/read_step.cuh), called through the C ABI, against a float64 restatement of the four-launch
+    chain it replaces (the same bf16 roundings of P*y and H): attention and retrieved information agree up to fp32
+    summation order."""
     import ctypes
     from mac_network_b200 import _lib as L_
     lib = L_.load()
@@ -200,11 +201,10 @@ def test_backward_full_shape_matches_autograd(variant, shape, dp):
 
 
 @pytest.mark.parametrize("variant", ["args", "gqa"])
-def test_bf16_throughput_form_small_projections_on_tensor_cores(monkeypatch, variant):
-    """The throughput form of the bf16 cell (MACCell(small_tc=True) / MAC_SMALL_TC=1: projY, write unit, gate and ctrlProj
+def test_bf16_small_tc_form_matches_oracle(variant):
+    """The throughput form of the bf16 cell (MACCell(small_tc=True): projY, write unit, gate and ctrlProj
     as three-pass split-bf16 wgmma products, write unit folded with the next projY) against the fp64 oracle at the
     headline and GQA shapes: same bounds as the default form (the split keeps these projections at fp32-class accuracy)."""
-    monkeypatch.setenv("MAC_SMALL_TC", "1")
     if variant == "args":
         cfg, inputs, params, ref = headline_case()
         L = SHAPES["headline"][4]
@@ -212,7 +212,7 @@ def test_bf16_throughput_form_small_projections_on_tensor_cores(monkeypatch, var
         shape = SHAPES["gqa"]
         cfg, inputs, params, ref = headline_case("gqa", shape, seeds=(41, 42, 43))
         L = shape[4]
-    got, cell = run_gpu(cfg, params, inputs, L, prec="bf16")
+    got, cell = run_gpu(cfg, params, inputs, L, prec="bf16", small_tc=True)
     assert cell._small_tc
     errs = {k: max(max_rel(got[k][i], ref[k][i]) for i in range(L)) for k in PER_STEP}
     print("bf16 throughput form (%s) worst per-step max-rel:" % variant, errs)

@@ -25,14 +25,16 @@ def _to_dev(inputs):
     return out
 
 
-def run_gpu(cfg, params_np, inputs_np, L, dropouts=(1.0, 1.0, 1.0), train=False, prec="fp32", seed=0):
+def run_gpu(cfg, params_np, inputs_np, L, dropouts=(1.0, 1.0, 1.0), train=False, prec="fp32", seed=0, small_tc=None,
+            save_for_backward=False):
     from mac_network_b200.mac_cell import MACCell, MACParams
     p32 = {k: np.asarray(v, np.float32) for k, v in params_np.items()}
     params = MACParams(cfg, L, values=p32)
     x = _to_dev({k: (np.asarray(v, np.float32) if v.dtype != np.int32 else v) for k, v in inputs_np.items()})
     cell = MACCell(x["vecQuestions"], x["questionWords"], x["questionCntxWords"], x["questionLengths"],
                    x["knowledgeBase"], dropouts[0], dropouts[1], dropouts[2], x["knowledgeBase"].shape[0], train,
-                   config=cfg, params=params, prec=prec, seed=seed)
+                   config=cfg, params=params, prec=prec, seed=seed, small_tc=small_tc,
+                   save_for_backward=save_for_backward)
     state = cell.zero_state(cell.batchSize)
     trace = []
     for i in range(L):
@@ -257,17 +259,18 @@ def test_checkpoint_roundtrip_and_attention_export(tmp_path):
     ("bf16", "args", (8, 12, 196, 512, 4)),
     ("bf16", "gqa", (64, 30, 49, 512, 6)),
 ])
-def test_step_invariant_read_hoist_is_the_same_function(monkeypatch, prec, variant, shape):
+def test_step_invariant_read_hoist_is_the_same_function(prec, variant, shape):
     """Eval mode computes P = KB@Wx+bx and Q = P@Wm[d:2d]+bm once per forward (mac_read_invariant / mac_read_fwd_inv).
-    The per-step form (mac_read_fwd, what training uses) must stay the same function: both against the oracle, and
-    against each other."""
+    The per-step form (mac_read_fwd, what training uses; here selected by save_for_backward with eval dropouts) must stay
+    the same function: both against the oracle, and against each other."""
     B, S, N, d, L = shape
     cfg = MACConfig.args(variant, netLength=L, memDim=d, ctrlDim=d, attDim=d)
     inputs = make_inputs(B, S, N, d, seed=61, dtype=np.float64)
     params = perturb_biases(init_params(cfg, L, seed=62, dtype=np.float64), seed=63)
-    hoisted, _ = run_gpu(cfg, params, inputs, L, prec=prec)
-    monkeypatch.setenv("MAC_NO_READ_HOIST", "1")
-    stepwise, _ = run_gpu(cfg, params, inputs, L, prec=prec)
+    hoisted, cell = run_gpu(cfg, params, inputs, L, prec=prec)
+    assert cell._read_hoist
+    stepwise, cell = run_gpu(cfg, params, inputs, L, prec=prec, save_for_backward=True)
+    assert not cell._read_hoist
     ref = run_oracle(cfg, params, inputs, L)
     tol = 1e-4 if prec == "fp32" else 3e-2
     for k in ("memory", "info", "att_kb"):
@@ -277,23 +280,20 @@ def test_step_invariant_read_hoist_is_the_same_function(monkeypatch, prec, varia
     print(prec, variant, {k: (max_rel(hoisted[k], ref[k]), max_rel(stepwise[k], ref[k])) for k in ("memory", "info")})
 
 
-@pytest.mark.parametrize("prec,force_cast", [("bf16", False), ("bf16", True), ("fp32", False)])
-def test_host_pipeline_matches_direct_cell(prec, force_cast, monkeypatch):
-    """serving.HostPipeline (host fp32 in -> [host bf16 cast in pieces through the staging ring] -> H2D -> graph -> D2H) returns
-    what the cell computes from device-resident inputs; in-flight slots and staging buffers do not mix batches up."""
+@pytest.mark.parametrize("prec,host_cast", [("bf16", None), ("bf16", True), ("fp32", None)])
+def test_host_pipeline_matches_direct_small_tc_cell(prec, host_cast):
+    """serving.HostPipeline (host fp32 in -> [host bf16 cast through the staging ring] -> H2D -> graph -> D2H) returns
+    bit for bit what a small_tc cell computes from device-resident inputs; in-flight slots and staging buffers do not mix
+    batches up.  host_cast=True casts whatever the timing rule would decide (it switches the cast off at this small shape)."""
     from mac_network_b200.mac_cell import MACParams
     from mac_network_b200.serving import HostPipeline
-    monkeypatch.setenv("MAC_SMALL_TC", "1")      # the pipeline's cells use the throughput form (small_tc): same form for the direct cell
-    if force_cast:                               # the timing rule would switch the host cast off at this small shape
-        monkeypatch.setenv("MAC_NO_HOST_CAST", "0")
-        monkeypatch.setenv("MAC_HOST_CAST_CHUNKS", "4")      # the multi-piece form of the ring (default: one piece)
     B, S, N, d, L = 8, 6, 49, 128, 3
     cfg = MACConfig.args("args", netLength=L, memDim=d, ctrlDim=d, attDim=d)
     pv = perturb_biases(init_params(cfg, L, seed=82), seed=83)
     params = MACParams(cfg, L, values=pv)
-    pipe = HostPipeline(cfg, params, (B, S, N, d, L), prec=prec, slots=2, cast_threads=3)
-    if force_cast:
-        assert pipe.host_kb_bf16 and pipe.chunks == 4 and len(pipe._stages) == 12
+    pipe = HostPipeline(cfg, params, (B, S, N, d, L), prec=prec, slots=2, cast_threads=3, host_cast=host_cast)
+    if host_cast:
+        assert pipe.host_kb_bf16 and len(pipe._stages) == 3
     batches = [make_inputs(B, S, N, d, seed=90 + i) for i in range(5)]
     host = [{k: torch.from_numpy(v).pin_memory() for k, v in b.items() if k != "questionWords"} for b in batches]
     got = []
@@ -301,7 +301,8 @@ def test_host_pipeline_matches_direct_cell(prec, force_cast, monkeypatch):
         t = pipe.submit(hb, next_batch=host[(i + 1) % len(host)])
         got.append({k: v.clone() for k, v in pipe.result(t).items()})
     for b, g in zip(batches, got):
-        ref, _ = run_gpu(cfg, pv, b, L, prec=prec)
+        # the pipeline's cells use the throughput form (small_tc): same form for the direct cell
+        ref, _ = run_gpu(cfg, pv, b, L, prec=prec, small_tc=True)
         assert np.array_equal(g["memory"].numpy(), ref["memory"][-1]), prec       # same kernels, same bits
         assert np.array_equal(g["control"].numpy(), ref["control"][-1])
         assert np.array_equal(g["att_kb"].numpy(), ref["att_kb"])

@@ -2,7 +2,7 @@
 control units, wordsProj, controlWholeQ, controlContinuous, unsharedCells): `tape.py` on the CUDA backward kernels.
 
 Two independent checks:
-  * the tape machinery itself, forced onto the shipped flag files (MAC_TAPE_BWD=1), element-wise against torch.autograd
+  * the tape machinery itself, forced onto the shipped flag files (tape_bwd=True), element-wise against torch.autograd
     on the fp64 restatement (`oracle/mac_torch_autograd.py`) -- the same bar as tests/test_gpu_backward.py;
   * every P2 fixture's flag set against central finite differences of the fp64 numpy oracle (`oracle/mac_oracle.py`, the
     restatement pinned to the reference's own outputs by tests/golden/): directional derivatives of
@@ -24,14 +24,14 @@ P2_CASES = ["p2_control", "p2_control_feed", "p2_ablations", "p2_wholeq", "p2_un
             "p2_read_add_train", "p2_read_plain_train", "p2_memory_bn", "p2_memory_bn_train"]
 
 
-def _cell(cfg, pv32, inputs32, L, dp, seed=777, train=True):
+def _cell(cfg, pv32, inputs32, L, dp, seed=777, train=True, tape_bwd=False):
     from mac_network_b200.mac_cell import MACCell, MACParams, mac_network
     B = inputs32["knowledgeBase"].shape[0]
     params = MACParams(cfg, L, values=pv32)
     x = {k: torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in inputs32.items()}
     cell = MACCell(x["vecQuestions"], x["questionWords"], x["questionCntxWords"], x["questionLengths"],
                    x["knowledgeBase"], dp[0], dp[1], dp[2], B, train, config=cfg, params=params, seed=seed,
-                   save_for_backward=True)
+                   save_for_backward=True, tape_bwd=tape_bwd)
     control, memory = mac_network(cell, L)
     return cell, control, memory
 
@@ -42,8 +42,7 @@ def _cell(cfg, pv32, inputs32, L, dp, seed=777, train=True):
     ("args4", (4, 6, 20, 64, 3), (1.0, 0.85, 1.0)),
     ("args1", (5, 7, 20, 64, 4), (0.85, 0.85, 1.0)),
 ])
-def test_tape_matches_autograd_on_the_shipped_flags(monkeypatch, variant, shape, dp):
-    monkeypatch.setenv("MAC_TAPE_BWD", "1")
+def test_tape_bwd_on_the_shipped_flags_matches_autograd(variant, shape, dp):
     from mac_network_b200.autograd import mac_backward
     from oracle import mac_torch_autograd as TA
     B, S, N, d, L = shape
@@ -57,7 +56,7 @@ def test_tape_matches_autograd_on_the_shipped_flags(monkeypatch, variant, shape,
     gc, gm = rng.standard_normal((B, d)), rng.standard_normal((B, d))
     pv32 = {k: v.astype(np.float32) for k, v in pv.items()}
     in32 = {k: (v if v.dtype == np.int32 else v.astype(np.float32)) for k, v in inputs.items()}
-    cell, control, memory = _cell(cfg, pv32, in32, L, dp, seed=4242)
+    cell, control, memory = _cell(cfg, pv32, in32, L, dp, seed=4242, tape_bwd=True)
     assert cell._tape is not None
     grads = mac_backward(cell, torch.from_numpy(gc.astype(np.float32)).cuda(), torch.from_numpy(gm.astype(np.float32)).cuda())
     torch.cuda.synchronize()
