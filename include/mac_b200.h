@@ -364,6 +364,17 @@ int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float keep, uint64_
  * (gather form, fixed order: deterministic).  The weight / bias gradients of the convolution are mac_linear_bwd on cols. */
 int mac_col2im3x3(const float* dcols, float* dx, float keep, uint64_t seed, int site, int step, int B, int H, int W, int C,
                   mac_stream_t stream);
+/* Backward of one stem layer y = act(conv3x3(dropout(x), kernel) + bias) with both GEMMs on wgmma tensor cores (bf16 operands,
+ * fp32 accumulation; the activation derivative, the bias sums and col2im stay fp32).  x [B,H,W,C] is the layer input BEFORE
+ * dropout, y [B*H*W, Cout] the output after the activation (as the forward saved them), dy the gradient w.r.t. y, kernel the
+ * HWIO fp32 variable.  dkernel [3,3,C,Cout] += and dbias [Cout] += (fixed-order reductions: deterministic); dx [B,H,W,C] =
+ * (NULL skips the data gradient and its GEMM).  keep / seed / site / step are the forward's mac_im2col3x3 arguments, so the
+ * keep-mask is the forward's.  Needs C % 128 == 0 and Cout % 128 == 0, else MAC_ERR_UNSUPPORTED; the workspace
+ * (mac_conv3x3_bwd_tc_workspace_bytes with with_dx = (dx != NULL)) need not be zeroed.  All checks precede any launch. */
+int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep, uint64_t seed,
+                       int site, int step, float* dkernel, float* dbias, float* dx, void* workspace, size_t workspace_bytes,
+                       int B, int H, int W, int C, int Cout, mac_stream_t stream);
+size_t mac_conv3x3_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx);
 
 /* ------------------------------------------------------------------------------------------------
  * Question input unit ("next" row, model.py:208-220, 279-307; ops.py:859-905): embedding lookup + bi-LSTM encoder.

@@ -106,6 +106,9 @@ PROTOTYPES = {
     "mac_lstm_bwd": (c_int, [c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_sz, c_int, c_int, c_int, c_int,
                              c_fp]),
     "mac_col2im3x3": (c_int, [c_fp, c_fp, c_f, c_u64, c_int, c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_conv3x3_bwd_tc": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_fp, c_fp, c_sz,
+                                   c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_conv3x3_bwd_tc_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "mac_pack_weight_bf16": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_split3": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_bf16_split": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_fp]),

@@ -71,18 +71,12 @@ __global__ void __launch_bounds__(256) elu_bwd_colsum_kernel(const float* __rest
   }
 }
 
-// dx = dy * act'(.) expressed through the saved OUTPUT y (tanh: 1-y^2; sigmoid: y(1-y); elu: y>0?1:y+1; relu: y>0)
+// dx = dy * act'(.) expressed through the saved OUTPUT y
 __global__ void act_bwd_kernel(const float* __restrict__ y, const float* __restrict__ dy, int act,
                                float* __restrict__ dx, long long n) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float v = y[i];
-  float g = 1.f;
-  if (act == MAC_ACT_TANH) g = 1.f - v * v;
-  else if (act == MAC_ACT_SIGMOID) g = v * (1.f - v);
-  else if (act == MAC_ACT_ELU) g = v > 0.f ? 1.f : v + 1.f;
-  else if (act == MAC_ACT_RELU) g = v > 0.f ? 1.f : 0.f;
-  dx[i] = dy[i] * g;
+  dx[i] = dy[i] * act_grad_from_output(act, y[i]);
 }
 
 // out[b, k] (+)= sum_n x[b, n, k]     grid (ceil(d/128), B), 256 threads = 32 column quads x 8 row groups (fixed-order reduce)

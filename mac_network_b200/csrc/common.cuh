@@ -45,6 +45,14 @@ __device__ __forceinline__ float apply_act(int act, float x) {
     default: return x;
   }
 }
+// act'(.) expressed through the activation OUTPUT y (tanh: 1-y^2; sigmoid: y(1-y); elu: y>0?1:y+1; relu: y>0)
+__device__ __forceinline__ float act_grad_from_output(int act, float y) {
+  if (act == MAC_ACT_TANH) return 1.f - y * y;
+  if (act == MAC_ACT_SIGMOID) return y * (1.f - y);
+  if (act == MAC_ACT_ELU) return y > 0.f ? 1.f : y + 1.f;
+  if (act == MAC_ACT_RELU) return y > 0.f ? 1.f : 0.f;
+  return 1.f;
+}
 
 // ------------------------------------------------------------------ warp / block reductions
 __device__ __forceinline__ float warp_sum(float v) {

@@ -811,3 +811,163 @@ extern "C" int mac_col2im3x3(const float* dcols, float* dx, float keep, uint64_t
   MAC_LAUNCH_CHECK();
   return MAC_OK;
 }
+
+// ------------------------------------------------------------------------------------------------ stem: backward on wgmma
+// One 3x3 convolution layer's backward with its two GEMMs on tensor cores (bf16 operands, fp32 accumulation, fp32
+// element-wise work), M = B*H*W rows, Mp = M rounded up to the 64-row k-block of the weight gradient:
+//   dZ = dy * act'(y)                      -> bf16 dZ [M, Cout] (dgrad A operand), bf16 dZ^T [Cout, Mp], fp32 column partials
+//   colsT = bf16(dropout(x)) patches^T     -> [9C, Mp], the forward's keep-mask (mac_im2col3x3's Philox numbering)
+//   dKernel [9C, Cout] += colsT @ dZ       (tc_wgrad_splitk, K = Mp; the HWIO kernel viewed as [9C, Cout] is its output)
+//   dBias += column sums of dZ             (fixed order: per-64-row-tile partials, then mac_colsum)
+//   dcols [M, 9C] = dZ @ Kernel^T          (mac_linear_tc_fwd with bf16(Kernel) in its own [9C, Cout] layout as the
+//                                           K-major B operand);  dx = col2im(dcols) * mask / keep   (mac_col2im3x3)
+// Columns M..Mp-1 of both transposed operands are written as zeros on every call: the workspace is not assumed zero.
+namespace mac {
+__global__ void __launch_bounds__(256) conv_dz_pack_kernel(const float* __restrict__ y, const float* __restrict__ dy, int act,
+                                                          __nv_bfloat16* __restrict__ dz, __nv_bfloat16* __restrict__ dzT,
+                                                          float* __restrict__ bpart, int M, int Mp, int N) {
+  __shared__ float tile[64][65];                              // [col][row]
+  const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
+  const int tq = threadIdx.x & 15, tr = threadIdx.x >> 4;     // 16 column quads x 16 rows per pass
+#pragma unroll
+  for (int p = 0; p < 4; ++p) {
+    const int mm = tr + 16 * p, m = m0 + mm, n = n0 + tq * 4;
+    float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (m < M) {
+      const size_t o = (size_t)m * N + n;
+      const float4 v = __ldg(reinterpret_cast<const float4*>(y + o));
+      const float4 d = __ldg(reinterpret_cast<const float4*>(dy + o));
+      g.x = d.x * act_grad_from_output(act, v.x);
+      g.y = d.y * act_grad_from_output(act, v.y);
+      g.z = d.z * act_grad_from_output(act, v.z);
+      g.w = d.w * act_grad_from_output(act, v.w);
+      *reinterpret_cast<uint2*>(dz + o) = make_uint2(pack_bf16(g.x, g.y), pack_bf16(g.z, g.w));
+    }
+    tile[tq * 4 + 0][mm] = g.x;
+    tile[tq * 4 + 1][mm] = g.y;
+    tile[tq * 4 + 2][mm] = g.z;
+    tile[tq * 4 + 3][mm] = g.w;
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int r = warp; r < 64; r += 8) {
+    const float a = tile[r][2 * lane], b = tile[r][2 * lane + 1];
+    *reinterpret_cast<uint32_t*>(dzT + (size_t)(n0 + r) * Mp + m0 + 2 * lane) = pack_bf16(a, b);
+    const float s = warp_sum(a + b);
+    if (lane == 0) bpart[(size_t)blockIdx.y * N + n0 + r] = s;
+  }
+}
+
+// colsT[tap*C + c, m] = bf16(dropout(x))[pixel m shifted by tap, c], zero outside the image and for m >= M.  One 64 (k) x
+// 64 (pixel) tile per block; C % 64 == 0, so a tile lies within one tap.  256-byte channel reads, 128-byte row writes.
+__global__ void __launch_bounds__(256) im2col3x3_t_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ colsT,
+                                                         uint32_t thresh, float scale, uint64_t seed, int site, int step,
+                                                         int B, int H, int W, int C, int Mp) {
+  __shared__ float tile[64][65];                              // [channel][pixel]
+  const int k0 = blockIdx.y * 64, m0 = blockIdx.x * 64;
+  const int tap = k0 / C, c0 = k0 - tap * C;
+  const int dh = tap / 3 - 1, dw = tap % 3 - 1;
+  const int M = B * H * W;
+  const int tq = threadIdx.x & 15, tr = threadIdx.x >> 4;     // 16 channel quads x 16 pixels per pass
+#pragma unroll
+  for (int p = 0; p < 4; ++p) {
+    const int mm = tr + 16 * p, m = m0 + mm;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (m < M) {
+      const int w = m % W, r = m / W;
+      const int h = r % H, b = r / H;
+      const int hs = h + dh, wsrc = w + dw;
+      if (hs >= 0 && hs < H && wsrc >= 0 && wsrc < W) {
+        const long long e = (((long long)b * H + hs) * W + wsrc) * C + c0 + tq * 4;
+        v = __ldg(reinterpret_cast<const float4*>(x + e));
+        if (thresh) {
+          const Philox4 q = philox4x32_10(seed, (uint64_t)e >> 2, (uint32_t)site, (uint32_t)step);
+          v.x = ((q.x >> 8) >= thresh) ? v.x * scale : 0.f;
+          v.y = ((q.y >> 8) >= thresh) ? v.y * scale : 0.f;
+          v.z = ((q.z >> 8) >= thresh) ? v.z * scale : 0.f;
+          v.w = ((q.w >> 8) >= thresh) ? v.w * scale : 0.f;
+        }
+      }
+    }
+    tile[tq * 4 + 0][mm] = v.x;
+    tile[tq * 4 + 1][mm] = v.y;
+    tile[tq * 4 + 2][mm] = v.z;
+    tile[tq * 4 + 3][mm] = v.w;
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int r = warp; r < 64; r += 8)
+    *reinterpret_cast<uint32_t*>(colsT + (size_t)(k0 + r) * Mp + m0 + 2 * lane) =
+        pack_bf16(tile[r][2 * lane], tile[r][2 * lane + 1]);
+}
+
+// workspace of mac_conv3x3_bwd_tc: 1 KB-aligned slabs behind a 1 KB alignment slack
+struct ConvBwdLayout {
+  size_t dz, dzT, colsT, bpart, wpart, k16, dcols, total;
+};
+inline ConvBwdLayout conv_bwd_layout(int B, int H, int W, int C, int Cout, bool with_dx) {
+  auto al = [](size_t v) { return (v + 1023) & ~(size_t)1023; };
+  const size_t M = (size_t)B * H * W, Mp = (M + 63) & ~(size_t)63, K = (size_t)9 * C;
+  // the split-K partials for the slice count the weight gradient will use on this device (tc_wgrad_splitk)
+  const int S = tc_pick_ksplit((int)Mp, (int)(K / TC_BM) * (Cout / TC_BN));
+  ConvBwdLayout l;
+  size_t o = 0;
+  l.dz = o;    o += al(M * Cout * 2);
+  l.dzT = o;   o += al((size_t)Cout * Mp * 2);
+  l.colsT = o; o += al(K * Mp * 2);
+  l.bpart = o; o += al(Mp / 64 * Cout * 4);
+  l.wpart = o; o += al((size_t)S * K * Cout * 4);
+  l.k16 = l.dcols = o;
+  if (with_dx) {
+    o += al(K * Cout * 2);
+    l.dcols = o; o += al(M * K * 4);
+  }
+  l.total = o + 1024;
+  return l;
+}
+}  // namespace mac
+
+extern "C" size_t mac_conv3x3_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx) {
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return 0;
+  return conv_bwd_layout(B, H, W, C, Cout, with_dx != 0).total;
+}
+
+extern "C" int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                                  uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
+                                  size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x || !y || !dy || !kernel || !dkernel || !dbias || !workspace) return MAC_ERR_INVALID;
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0 || !(keep > 0.f && keep <= 1.f)) return MAC_ERR_INVALID;
+  if ((long long)B * H * W > (1LL << 30)) return MAC_ERR_INVALID;
+  if ((C % 128) || (Cout % 128)) return MAC_ERR_UNSUPPORTED;     // wgmma tiles: 9C and Cout are GEMM N / M extents
+  if (!mac_aligned16(x) || !mac_aligned16(y) || !mac_aligned16(dy) || !mac_aligned16(kernel) || !mac_aligned16(dkernel) ||
+      (dx && !mac_aligned16(dx)))
+    return MAC_ERR_ALIGN;
+  const ConvBwdLayout l = conv_bwd_layout(B, H, W, C, Cout, dx != nullptr);
+  if (workspace_bytes < l.total) return MAC_ERR_WORKSPACE;
+  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
+  const int M = B * H * W, Mp = (M + 63) & ~63, K = 9 * C;
+  char* base = tc_align1k(workspace);
+  __nv_bfloat16* dz = reinterpret_cast<__nv_bfloat16*>(base + l.dz);
+  __nv_bfloat16* dzT = reinterpret_cast<__nv_bfloat16*>(base + l.dzT);
+  __nv_bfloat16* colsT = reinterpret_cast<__nv_bfloat16*>(base + l.colsT);
+  float* bpart = reinterpret_cast<float*>(base + l.bpart);
+  float* wpart = reinterpret_cast<float*>(base + l.wpart);
+  conv_dz_pack_kernel<<<dim3(Cout / 64, Mp / 64), 256, 0, stream>>>(y, dy, act, dz, dzT, bpart, M, Mp, Cout);
+  MAC_LAUNCH_CHECK();
+  const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
+  const float scale = keep < 1.f ? 1.f / keep : 1.f;
+  im2col3x3_t_kernel<<<dim3(Mp / 64, K / 64), 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, B, H, W, C, Mp);
+  MAC_LAUNCH_CHECK();
+  int st = mac_colsum(bpart, dbias, 1, Mp / 64, Cout, 1, stream_);
+  if (st != MAC_OK) return st;
+  st = tc_wgrad_splitk(colsT, dzT, dkernel, wpart, K, Cout, Mp, stream);
+  if (st != MAC_OK || !dx) return st;
+  void* k16 = base + l.k16;
+  float* dcols = reinterpret_cast<float*>(base + l.dcols);
+  st = mac_cast_bf16(kernel, k16, (long long)K * Cout, stream_);
+  if (st != MAC_OK) return st;
+  st = mac_linear_tc_fwd(dz, k16, nullptr, MAC_ACT_NON, dcols, 0, M, Cout, K, stream_);
+  if (st != MAC_OK) return st;
+  return mac_col2im3x3(dcols, dx, keep, seed, site, step, B, H, W, C, stream_);
+}

@@ -72,6 +72,19 @@ class Stem(object):
             return W, self._packed[i]
         return W, None
 
+    def _check_trainable(self, in_dim):
+        """Training (forward with save_for_backward + backward) runs in fp32, or in bf16 on tensor cores
+        (`mac_conv3x3_bwd_tc`, DESIGN.md section 9 item 2), whose GEMM tiles need every layer's input and output channel
+        counts to be multiples of 128.  Raises before any launch."""
+        if self.prec == "fp32":
+            return
+        if self.prec != "bf16":
+            raise NotImplementedError("stem training runs in fp32 or bf16, not %r (DESIGN.md section 9)" % self.prec)
+        dims = [in_dim] + [int(self.p["stem/cnnLayercnn_%d/kernels/kernel" % i].shape[3]) for i in range(self.nlayers)]
+        if any(c % 128 for c in dims):
+            raise NotImplementedError("bf16 stem training needs channel counts that are multiples of 128 (the wgmma tiles of "
+                                      "mac_conv3x3_bwd_tc), got %s; use prec='fp32' (DESIGN.md section 9)" % dims)
+
     def forward(self, images, keep=1.0, step=0, save_for_backward=False):
         """images: [B,H,W,C] fp32 NHWC (the reference transposes the NCHW h5 features first, model.py:~770).
         Returns the knowledge base [B, H*W, outDim] fp32."""
@@ -79,8 +92,7 @@ class Stem(object):
         B, H, Wd, C = x.shape
         act = ACT["ELU"] if self.relu == "ELU" else ACT["RELU_STD"]
         if save_for_backward:
-            if self.prec != "fp32":
-                raise NotImplementedError("stem backward runs on the fp32 path (DESIGN.md section 9)")
+            self._check_trainable(C)
             self._saved = {"xs": [], "ys": [], "keep": float(keep), "step": int(step), "act": act}
         for i in range(self.nlayers):
             if save_for_backward:
@@ -112,7 +124,8 @@ class Stem(object):
         model.py:626-636).  d_kb [B, H*W, outDim]; accumulates (+=) into `grads` (dict TF-name -> tensor shaped like the
         parameter).  Per layer, last to first:  dZ = dY * act'(Y);  dKernel += cols^T @ dZ, dBias += colsum(dZ)
         (`mac_linear_bwd` on the re-generated patch matrix);  dcols = dZ @ Kernel^T;  dX = col2im(dcols) * dropout mask.
-        The gradient w.r.t. the images (and with it layer 0's largest GEMM) is skipped unless asked for."""
+        The gradient w.r.t. the images (and with it layer 0's largest GEMM) is skipped unless asked for.
+        With prec="bf16" each layer is one `mac_conv3x3_bwd_tc` call: the same steps with both GEMMs on tensor cores."""
         sv = getattr(self, "_saved", None)
         if sv is None:
             raise RuntimeError("forward(save_for_backward=True) must run first")
@@ -125,6 +138,17 @@ class Stem(object):
             C, Nout = x.shape[3], y.shape[1]
             K = 9 * C
             W, _ = self._weights(i)
+            if self.prec == "bf16":
+                dx = torch.empty_like(x) if (need_d_images or i > 0) else None
+                nbytes = int(self.lib.mac_conv3x3_bwd_tc_workspace_bytes(B, H, Wd, C, Nout, int(dx is not None)))
+                ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+                check(self.lib.mac_conv3x3_bwd_tc(ptr(x), ptr(y), ptr(dy), ptr(W), sv["act"], sv["keep"], self.seed,
+                                                  SITE_STEM + i, sv["step"], ptr(grads["stem/cnnLayercnn_%d/kernels/kernel" % i]),
+                                                  ptr(grads["stem/cnnLayercnn_%d/biases/bias" % i]), ptr(dx), ptr(ws), nbytes,
+                                                  B, H, Wd, C, Nout, stream_ptr()), "mac_conv3x3_bwd_tc")
+                if dx is not None:
+                    dy = dx.view(M, C)
+                continue
             dz = torch.empty_like(y)
             check(self.lib.mac_activation_bwd(ptr(y), ptr(dy), sv["act"], ptr(dz), dz.numel(), stream_ptr()), "mac_activation_bwd")
             cols = torch.empty((M, K), dtype=torch.float32, device=self.device)
