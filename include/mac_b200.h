@@ -51,9 +51,13 @@ enum { MAC_ACT_NON = 0, MAC_ACT_TANH = 1, MAC_ACT_SIGMOID = 2, MAC_ACT_ELU = 3, 
 enum {
   MAC_PREC_FP32 = 0, /* fp32 FMA pipe, fp32 accumulate: the <=1e-4 parity configuration */
   MAC_PREC_BF16 = 1, /* bf16 operands on wgmma tensor cores, fp32 accumulate: the headline configuration */
-  MAC_PREC_TC32 = 2  /* split-bf16 on wgmma (x = hi + lo, three of the four partial products, fp32 accumulate): a tensor-core
+  MAC_PREC_TC32 = 2, /* split-bf16 on wgmma (x = hi + lo, three of the four partial products, fp32 accumulate): a tensor-core
                         path inside the 1e-4 parity bar.  Inference form only (mac_read_invariant / mac_read_fwd_inv); fp32
                         knowledge base; everything outside the three [B*N, .] projections as in MAC_PREC_FP32 */
+  MAC_PREC_FP8 = 3   /* e4m3 operands on wgmma for the two per-step products of the read step, fp32 accumulate, per-row /
+                        per-column fp32 scales (csrc/read_step_fp8.cuh).  Inference form only (mac_read_invariant /
+                        mac_read_fwd_inv), the shapes of mac_read_step_fused_supported, bf16 knowledge base; P and Q as in
+                        MAC_PREC_BF16.  About ten times the bf16 error: opt-in, never a default */
 };
 
 int mac_b200_abi_version(void);
@@ -120,6 +124,9 @@ typedef struct mac_read_weights {
   const void* Wx_bf16; const void* Wm_bf16; const void* Wm2_bf16;
   /* MAC_PREC_TC32 only: split-bf16 copies [out, 3*in] = [hi | hi | lo] (mac_pack_weight_split3) of Wx, Wm[0:d], Wm[d:2d], Wm2 */
   const void* Wx_s3; const void* Wma_s3; const void* Wmb_s3; const void* Wm2_s3;
+  /* MAC_PREC_FP8 only (read under no other precision): e4m3 [out, in] copies of Wm[0:d] and Wm2 with their per-output-column
+   * fp32 scales [d] (mac_pack_weight_fp8) */
+  const void* Wm_fp8; const float* Wm_fp8_scale; const void* Wm2_fp8; const float* Wm2_fp8_scale;
 } mac_read_weights;
 
 int mac_read_fwd(const float* kb, const void* kb_bf16, const float* memory_in, const float* control,
@@ -133,9 +140,13 @@ size_t mac_read_workspace_bytes(int B, int N, int d, int prec);
  * netLength steps, so two of the three big projections do not depend on the step:
  *   P = KB @ Wx + bx                 (ops.py:688)
  *   Q = P @ Wm[d:2d, :] + bm         (the un-scaled half of the [P*y, P] concat, mac_cell.py:236-238)
- * mac_read_invariant computes `inv` = [P | Q] once per forward (fp32 for MAC_PREC_FP32, bf16 for MAC_PREC_BF16);
+ * mac_read_invariant computes `inv` = [P | Q] once per forward (fp32 for MAC_PREC_FP32, bf16 for MAC_PREC_BF16; for
+ * MAC_PREC_FP8 `inv` = [P8 | sP | Q | logit scratch | P]: P8 = e4m3(P / sP) with sP = max|P row| / 448 per row, Q and P bf16,
+ * from kb_bf16 and the bf16 packs Wx_bf16 / Wm_bf16);
  * mac_read_fwd_inv is mac_read_fwd(keep_read = 1, save = NULL) with H = ELU((P*y) @ Wm[0:d, :] + Q): the same
- * function with 2d instead of 4d multiply-adds per knowledge-base element and step. */
+ * function with 2d instead of 4d multiply-adds per knowledge-base element and step.  With MAC_PREC_FP8 it runs
+ * read_step_fp8_kernel + kb_attend (see MAC_PREC_FP8); an unsupported shape or a missing kb_bf16 / inv returns
+ * MAC_ERR_UNSUPPORTED before any launch, and so does mac_read_fwd with MAC_PREC_FP8. */
 size_t mac_read_invariant_bytes(int B, int N, int d, int prec);
 int mac_read_invariant(const float* kb, const void* kb_bf16, const mac_read_weights* w, int prec, void* inv,
                        size_t inv_bytes, int B, int N, int d, mac_stream_t stream);
@@ -243,6 +254,10 @@ int mac_pack_weight_bf16(const float* W, void* Wt_bf16, int K, int n_out, mac_st
 /* fp32 W[K, n_out] -> bf16 Wt3[n_out, 3K] = [hi | hi | lo] (hi = bf16(W), lo = bf16(W - hi)): the B operand of the split-bf16
  * products of MAC_PREC_TC32 (see tc3_gemm in csrc/tc_gemm.cuh).  A row block of a taller weight is passed as W + k0*n_out. */
 int mac_pack_weight_split3(const float* W, void* Wt3_bf16, int K, int n_out, mac_stream_t stream);
+/* fp32 W[K, n_out] -> e4m3 Wt[n_out, K] = e4m3(W / s_c) (round to nearest even, saturating) with the per-output-column scale
+ * col_scale[c] = s_c = max_k |W[k, c]| / 448 (0 for an all-zero column, which packs to zeros): the B operand of the
+ * MAC_PREC_FP8 read step.  A row block of a taller weight is passed as W (its first K rows). */
+int mac_pack_weight_fp8(const float* W, void* Wt_e4m3, float* col_scale, int K, int n_out, mac_stream_t stream);
 int mac_linear_tc_fwd(const void* x_bf16, const void* wt_bf16, const float* b, int act, void* y, int y_is_bf16,
                       int M, int K, int n_out, mac_stream_t stream);
 

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libmac_b200.so")
 
 ACT = {"NON": 0, "TANH": 1, "SIGMOID": 2, "ELU": 3, "RELU_STD": 4}
-PREC = {"fp32": 0, "bf16": 1, "tc32": 2}
+PREC = {"fp32": 0, "bf16": 1, "tc32": 2, "fp8": 3}
 SITE_MEM_VAR, SITE_READ_KB, SITE_READ_MEM, SITE_READ_INTER, SITE_WRITE_INFO, SITE_MEM_PLAIN = range(6)
 
 c_fp = ctypes.c_void_p
@@ -27,7 +27,8 @@ class ReadWeights(ctypes.Structure):
     _fields_ = [("Wx", c_fp), ("bx", c_fp), ("Wy", c_fp), ("by", c_fp), ("Wm", c_fp), ("bm", c_fp),
                 ("Wm2", c_fp), ("bm2", c_fp), ("wr", c_fp), ("br", c_f),
                 ("Wx_bf16", c_fp), ("Wm_bf16", c_fp), ("Wm2_bf16", c_fp),
-                ("Wx_s3", c_fp), ("Wma_s3", c_fp), ("Wmb_s3", c_fp), ("Wm2_s3", c_fp)]
+                ("Wx_s3", c_fp), ("Wma_s3", c_fp), ("Wmb_s3", c_fp), ("Wm2_s3", c_fp),
+                ("Wm_fp8", c_fp), ("Wm_fp8_scale", c_fp), ("Wm2_fp8", c_fp), ("Wm2_fp8_scale", c_fp)]
 
 
 # name -> (restype, argtypes); every symbol include/mac_b200.h declares
@@ -111,6 +112,7 @@ PROTOTYPES = {
     "mac_conv3x3_bwd_tc_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "mac_pack_weight_bf16": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_split3": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
+    "mac_pack_weight_fp8": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_bf16_split": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_linear_tc_small_fwd": (c_int, [ctypes.POINTER(c_fp), ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_fp, c_fp,
                                         c_fp, c_f, c_int, c_fp, c_int, c_fp, c_int, c_fp, c_fp, c_fp, c_int, c_int, c_fp]),

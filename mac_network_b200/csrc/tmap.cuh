@@ -34,7 +34,7 @@ struct TmapKey {
   bool operator==(const TmapKey& o) const { return memcmp(this, &o, sizeof(TmapKey)) == 0; }
 };
 
-// 2-D row-major tensor [rows, cols] (cols contiguous), box = [box_rows, box_cols].  dtype: 0 fp32, 1 bf16.
+// 2-D row-major tensor [rows, cols] (cols contiguous), box = [box_rows, box_cols].  dtype: 0 fp32, 1 bf16, 2 one byte (e4m3).
 // swizzle: 0 none, 1 128B.  Returns MAC_OK or MAC_ERR_ARCH / MAC_ERR_INVALID.
 inline int make_tmap_2d(CUtensorMap* out, const void* base, int dtype, uint64_t rows, uint64_t cols,
                         uint64_t row_stride_bytes, uint32_t box_rows, uint32_t box_cols, int swizzle) {
@@ -65,7 +65,9 @@ inline int make_tmap_2d(CUtensorMap* out, const void* base, int dtype, uint64_t 
   const cuuint64_t gstride[1] = {row_stride_bytes};
   const cuuint32_t box[2] = {box_cols, box_rows};
   const cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapDataType dt = dtype == 0 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUtensorMapDataType dt = dtype == 0   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : dtype == 1 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                              : CU_TENSOR_MAP_DATA_TYPE_UINT8;
   const CUtensorMapSwizzle sw = swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE;
   CUresult r = enc(out, dt, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

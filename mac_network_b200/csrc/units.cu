@@ -4,6 +4,7 @@
 #include "skinny.cuh"
 #include "tc_gemm.cuh"
 #include "read_step.cuh"
+#include "read_step_fp8.cuh"
 #include "skinny_tc.cuh"
 
 using namespace mac;
@@ -144,19 +145,22 @@ static size_t read_inv_fp32_bytes(int B, int N, int d) { return (size_t)2 * B * 
 
 extern "C" size_t mac_read_invariant_bytes(int B, int N, int d, int prec) {
   if (prec == MAC_PREC_TC32) return tc3_invariant_bytes(B, N, d);
+  if (prec == MAC_PREC_FP8) return fp8_read_invariant_bytes(B, N, d);
   return prec == MAC_PREC_BF16 ? tc_read_invariant_bytes(B, N, d) : read_inv_fp32_bytes(B, N, d);
 }
 
 extern "C" int mac_read_invariant(const float* kb, const void* kb_bf16, const mac_read_weights* w, int prec, void* inv,
                                   size_t inv_bytes, int B, int N, int d, mac_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  // the bf16 path reads only kb_bf16: the fp32 knowledge base may be absent (host-cast front end)
-  if ((!kb && !(prec == MAC_PREC_BF16 && kb_bf16)) || !w || !inv || B <= 0 || N <= 0 || d <= 0 || (d & 3))
-    return MAC_ERR_INVALID;
+  if (prec == MAC_PREC_FP8 && (!kb_bf16 || !read_step_supported(B, N, d))) return MAC_ERR_UNSUPPORTED;
+  // the bf16 and fp8 paths read only kb_bf16: the fp32 knowledge base may be absent (host-cast front end)
+  const bool kb_opt = (prec == MAC_PREC_BF16 || prec == MAC_PREC_FP8) && kb_bf16;
+  if ((!kb && !kb_opt) || !w || !inv || B <= 0 || N <= 0 || d <= 0 || (d & 3)) return MAC_ERR_INVALID;
   if ((kb && !mac_aligned16(kb)) || !mac_aligned16(inv)) return MAC_ERR_ALIGN;
   if (inv_bytes < mac_read_invariant_bytes(B, N, d, prec)) return MAC_ERR_WORKSPACE;
   if (prec == MAC_PREC_BF16) return tc_read_invariant(kb_bf16, w, inv, inv_bytes, B, N, d, stream);
   if (prec == MAC_PREC_TC32) return tc3_read_invariant(kb, w, inv, inv_bytes, B, N, d, stream);
+  if (prec == MAC_PREC_FP8) return fp8_read_invariant(kb_bf16, w, inv, inv_bytes, B, N, d, stream);
   const int M = B * N;
   float* P = reinterpret_cast<float*>(inv);
   float* Q = P + (size_t)M * d;
@@ -210,7 +214,11 @@ static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, 
                          uint64_t seed, int step, int prec, float* info, float* att, float* save, void* workspace,
                          size_t workspace_bytes, int B, int N, int d, mac_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const bool kb_opt = inv && prec == MAC_PREC_BF16 && kb_bf16;     // eval bf16 path: only the bf16 copy is read
+  // e4m3: the inference read step only, checked before anything is launched
+  if (prec == MAC_PREC_FP8 && (!inv || !kb_bf16 || keep_read < 1.f || save || !read_step_supported(B, N, d)))
+    return MAC_ERR_UNSUPPORTED;
+  // eval bf16 / fp8 path: only the bf16 copy is read
+  const bool kb_opt = inv && (prec == MAC_PREC_BF16 || prec == MAC_PREC_FP8) && kb_bf16;
   if ((!kb && !kb_opt) || !memory_in || !control || !w || !info || !att || !workspace) return MAC_ERR_INVALID;
   if (B <= 0 || N <= 0 || d <= 0 || (d & 3)) return MAC_ERR_INVALID;
   if (!(keep_read > 0.f && keep_read <= 1.f)) return MAC_ERR_INVALID;
@@ -254,6 +262,7 @@ static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, 
     if (st != MAC_OK) return st;
   }
   int nparts = 0;
+  if (prec == MAC_PREC_FP8) return read_step_fp8_launch(inv, kb_bf16, y, control, w, att, info, B, N, d, stream);
   if (inv && prec == MAC_PREC_BF16 && kb_bf16 && read_step_supported(B, N, d)) {
     // the whole step (P*y, both projections, logits, softmax, weighted sum) as ONE kernel: read_step.cuh
     return read_step_launch(inv, kb_bf16, y, control, w, att, info, B, N, d, stream);
@@ -457,6 +466,14 @@ extern "C" int mac_pack_weight_bf16(const float* W, void* Wt_bf16, int K, int N,
   if (!W || !Wt_bf16 || K <= 0 || N <= 0) return MAC_ERR_INVALID;
   dim3 grid((N + 31) / 32, (K + 31) / 32), block(32, 8);
   pack_weight_bf16_kernel<<<grid, block, 0, stream>>>(W, reinterpret_cast<__nv_bfloat16*>(Wt_bf16), K, N);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+extern "C" int mac_pack_weight_fp8(const float* W, void* Wt_e4m3, float* col_scale, int K, int N, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!W || !Wt_e4m3 || !col_scale || K <= 0 || N <= 0) return MAC_ERR_INVALID;
+  pack_weight_fp8_kernel<<<(N + 31) / 32, dim3(32, 8), 0, stream>>>(W, reinterpret_cast<uint8_t*>(Wt_e4m3), col_scale, K, N);
   MAC_LAUNCH_CHECK();
   return MAC_OK;
 }

@@ -194,9 +194,9 @@ class MACCell(object):
         # three-pass split-bf16 products (mac_linear_tc_small_fwd, fp32-class accuracy): 16-32 independent CTAs that can run
         # beside another pass's read kernels, which the 8-CTA-cluster fp32 kernel cannot; its own latency is higher than the
         # cluster kernel's, so it is the THROUGHPUT form: small_tc=True (callers with several passes in flight: bench.py,
-        # serving.HostPipeline); default off.
-        self._small_tc = bool(small_tc and self.prec == PREC["bf16"] and not save_for_backward and B <= 128 and d % 64 == 0
-                              and self._fused_write)
+        # serving.HostPipeline); default off.  The e4m3 read step (prec="fp8") runs these projections exactly as bf16 does.
+        self._small_tc = bool(small_tc and self.prec in (PREC["bf16"], PREC["fp8"]) and not save_for_backward and B <= 128
+                              and d % 64 == 0 and self._fused_write)
         # plain write unit: its GEMM also produces the next step's memory projection.  It shortens the dependency chain of
         # ONE pass; with several independent passes in flight the two smaller GEMMs can pack better, so throughput callers
         # may pass fold_y=False.  fold_y=None: on.  The throughput form (small_tc) always folds: one launch for the write
@@ -228,8 +228,13 @@ class MACCell(object):
         if self.prec == PREC["tc32"] and (save_for_backward or not self._read_hoist or float(readDropout) < 1.0 or d % 128):
             raise NotImplementedError('prec="tc32" (split-bf16 tensor-core projections inside the 1e-4 bar) is the inference '
                                       "form of the fused read unit: shared cells, readDropout = 1, d % 128 == 0")
-        if self._kb_given_bf16 and not (self.prec == PREC["bf16"] and self._read_hoist and float(readDropout) >= 1.0):
-            raise NotImplementedError("a bf16 knowledge base is accepted by the bf16 inference path only")
+        if self.prec == PREC["fp8"] and (save_for_backward or not self._read_hoist or float(readDropout) < 1.0
+                                         or not (d == 512 and 1 <= N <= 256 and B < 2 ** 22)):
+            raise NotImplementedError('prec="fp8" (e4m3 read step, csrc/read_step_fp8.cuh) is the inference form of the fused '
+                                      "read unit: shared cells, readDropout = 1, d = 512, N <= 256")
+        if self._kb_given_bf16 and not (self.prec in (PREC["bf16"], PREC["fp8"]) and self._read_hoist
+                                        and float(readDropout) >= 1.0):
+            raise NotImplementedError("a bf16 knowledge base is accepted by the bf16 and fp8 inference paths only")
 
     # ------------------------------------------------------------------ reference properties
     @property
@@ -338,7 +343,7 @@ class MACCell(object):
         self._gate = self._new(L, B, d) if c.writeGate else None
         if self._kb_given_bf16:
             self.kb_bf16 = self.knowledgeBase
-        elif self.prec == PREC["bf16"]:
+        elif self.prec in (PREC["bf16"], PREC["fp8"]):
             self.kb_bf16 = torch.empty(self.knowledgeBase.shape, dtype=torch.bfloat16, device=self.device)
             check(self.lib.mac_cast_bf16(ptr(self.knowledgeBase), ptr(self.kb_bf16), self.knowledgeBase.numel(),
                                          stream_ptr()), "mac_cast_bf16")
@@ -451,7 +456,7 @@ class MACCell(object):
         rw = ReadWeights(Wx.data_ptr(), bx.data_ptr(), Wy.data_ptr(), by.data_ptr(), Wm.data_ptr(), bm.data_ptr(),
                          Wm2.data_ptr(), bm2.data_ptr(), p[lsc + "weights/weight"].data_ptr(),
                          p.scalar(lsc + "biases/bias"), None, None, None)
-        if self.prec == PREC["bf16"]:
+        if self.prec in (PREC["bf16"], PREC["fp8"]):     # fp8: P and Q are the bf16 path's (mac_read_invariant)
             def pack(t):       # fp32 [in, out] -> bf16 [out, in] (K-major B operand of wgmma)
                 o = torch.empty((t.shape[1], t.shape[0]), dtype=torch.bfloat16, device=t.device)
                 check(self.lib.mac_pack_weight_bf16(ptr(t), ptr(o), t.shape[0], t.shape[1], stream_ptr()), "pack")
@@ -466,6 +471,15 @@ class MACCell(object):
             d_ = self.d
             keep3 = p.derived(("split3", sc), lambda: (pack3(Wx), pack3(Wm[:d_]), pack3(Wm[d_:]), pack3(Wm2)))
             rw.Wx_s3, rw.Wma_s3, rw.Wmb_s3, rw.Wm2_s3 = (t.data_ptr() for t in keep3)
+        if self.prec == PREC["fp8"]:
+            def pack8(t):      # fp32 [in, out] -> e4m3 [out, in] and the fp32 scale of each output column
+                o = torch.empty((t.shape[1], t.shape[0]), dtype=torch.uint8, device=t.device)
+                s_ = torch.empty(t.shape[1], dtype=torch.float32, device=t.device)
+                check(self.lib.mac_pack_weight_fp8(ptr(t), ptr(o), ptr(s_), t.shape[0], t.shape[1], stream_ptr()), "pack8")
+                return o, s_
+            d_ = self.d
+            keep8 = p.derived(("fp8", sc), lambda: pack8(Wm[:d_]) + pack8(Wm2))
+            rw.Wm_fp8, rw.Wm_fp8_scale, rw.Wm2_fp8, rw.Wm2_fp8_scale = (t.data_ptr() for t in keep8)
         self._rw[name] = rw
         return rw
 

@@ -36,7 +36,8 @@ class MACnet(object):
                  stem_layers=2, seed=0, rank=0, world=1, lr=1e-4, prec="bf16", use_ema=False, answer_decoder=None,
                  device="cuda", **trainer_kw):
         """`vocab`: rows of the question-embedding variable (ids 1..vocab; 0 is padding); `answer_decoder`: optional
-        id -> answer string (`answerDict.decodeId`, model.py:699).  `prec`: arithmetic of the evaluation forward."""
+        id -> answer string (`answerDict.decodeId`, model.py:699).  `prec`: arithmetic of the evaluation forward; with
+        "fp8" the cell's read step runs on e4m3 and the image stem in bf16."""
         self.cfg, self.L, self.prec, self.use_ema = cfg, netLength, prec, bool(use_ema)
         self.decode = answer_decoder
         self.trainer = DPTrainer(cfg, netLength, seed=seed, rank=rank, world=world, lr=lr, device=device,
@@ -46,7 +47,8 @@ class MACnet(object):
         t = self.trainer
         # evaluation-mode views of the same variables: every dropout at 1.0 (model.py:118-125)
         self._enc = QuestionEncoder({k: p.t[k] for k in t._enc_specs}, keep_input=1.0, keep_question=1.0)
-        self._stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=prec, version=lambda: p.version)
+        self._stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec="bf16" if prec == "fp8" else prec,
+                          version=lambda: p.version)
         self._out = OutputUnit({k: p.t[k] for k in p.specs if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu,
                                keep=1.0, version=lambda: p.version)
         self.device = p.device

@@ -159,14 +159,14 @@ class HostPipeline(object):
 
     def __init__(self, cfg, params, shape, prec="bf16", slots=4, use_graph=True, cast_threads=None, fold_y=None,
                  host_cast=None, stage_ring=None):
-        """`host_cast` (bf16 path only): None = decide here (cast the knowledge base to bf16 on the host if that is faster
-        than the PCIe time it saves); False = never; True = always.  Callers that run several ranks per socket pass False:
-        the cast makes a pass touch ~57 MB of host DRAM (fp32 read + bf16 write + DMA read) instead of 31 MB, and the ranks
-        of one socket share its memory bandwidth."""
+        """`host_cast` (bf16 and fp8 paths, which read only the bf16 knowledge base): None = decide here (cast the knowledge
+        base to bf16 on the host if that is faster than the PCIe time it saves); False = never; True = always.  Callers that
+        run several ranks per socket pass False: the cast makes a pass touch ~57 MB of host DRAM (fp32 read + bf16 write +
+        DMA read) instead of 31 MB, and the ranks of one socket share its memory bandwidth."""
         self.lib = _lib.load()
         self.shape = shape
         self.prec = prec
-        self.host_kb_bf16 = (prec == "bf16" and cfg.is_fast_path and not cfg.unsharedCells and host_cast is not False)
+        self.host_kb_bf16 = (prec in ("bf16", "fp8") and cfg.is_fast_path and not cfg.unsharedCells and host_cast is not False)
         self.cast_threads = int(cast_threads) if cast_threads else max(1, min(12, usable_cpus() - 2))
         self.cast_ms = None
         if self.host_kb_bf16 and host_cast is None:
