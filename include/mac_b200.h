@@ -375,6 +375,22 @@ int mac_softmax_xent(const float* logits, const int32_t* labels, float* losses, 
  * --------------------------------------------------------------------------------------------- */
 int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float keep, uint64_t seed, int site, int step,
                   int B, int H, int W, int C, mac_stream_t stream);
+/* Inference stem layer in e4m3 (csrc/tc_gemm_fp8.cuh; Stem(prec="fp8")), no dropout.  All scales fp32; e4m3 rounds to nearest
+ * even and saturates at +-448.
+ * mac_im2col3x3_fp8: the patch matrix of mac_im2col3x3 (same tap-major, channel-fastest layout) as e4m3 cols_e4m3 [M, 9C],
+ *   M = B*H*W, with one scale per row: amax_m = max |x| over the in-image pixels of output pixel m's 3x3 window,
+ *   row_scale[m] = amax_m / 448, cols_e4m3[m, k] = e4m3(patch[m, k] * (448 / amax_m)); a window that is all zero gives
+ *   row_scale 0 and zero bytes.  Needs C % 128 == 0 (else MAC_ERR_UNSUPPORTED) and a workspace of
+ *   mac_im2col3x3_fp8_workspace_bytes (one float per input pixel, need not be zeroed).
+ * mac_linear_fp8_fwd: y[M, n_out] = act((x_e4m3[M, K] @ wt_e4m3[n_out, K]^T) * x_scale[m] * w_scale[n] + b[n]), fp32 y; wt /
+ *   w_scale from mac_pack_weight_fp8.  wgmma m64n128k32 e4m3, every 128-element k-block accumulated in its own registers
+ *   and added into an fp32 master accumulator.  act in {NON, ELU, RELU}; b may be NULL; K % 128 == 0 and n_out % 128 == 0,
+ *   else MAC_ERR_UNSUPPORTED.  M need not be a multiple of 128.  All checks precede any launch. */
+int mac_im2col3x3_fp8(const float* x, void* cols_e4m3, float* row_scale, void* workspace, size_t workspace_bytes,
+                      int B, int H, int W, int C, mac_stream_t stream);
+size_t mac_im2col3x3_fp8_workspace_bytes(int B, int H, int W, int C);
+int mac_linear_fp8_fwd(const void* x_e4m3, const float* x_scale, const void* wt_e4m3, const float* w_scale, const float* b,
+                       int act, float* y, int M, int K, int n_out, mac_stream_t stream);
 /* backward of mac_im2col3x3 (fp32): dx[b,h,w,c] = keep-mask/keep * sum of the <= 9 entries of dcols that copied x[b,h,w,c]
  * (gather form, fixed order: deterministic).  The weight / bias gradients of the convolution are mac_linear_bwd on cols. */
 int mac_col2im3x3(const float* dcols, float* dx, float keep, uint64_t seed, int site, int step, int B, int H, int W, int C,

@@ -99,6 +99,9 @@ PROTOTYPES = {
     "mac_bcast_op": (c_int, [c_fp, c_fp, c_int, c_f, c_fp, c_fp, c_int, c_int, c_int, c_fp]),
     "mac_softmax_xent": (c_int, [c_fp, c_fp, c_fp, c_fp, c_f, c_int, c_int, c_fp]),
     "mac_im2col3x3": (c_int, [c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_im2col3x3_fp8": (c_int, [c_fp, c_fp, c_fp, c_fp, c_sz, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_im2col3x3_fp8_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int]),
+    "mac_linear_fp8_fwd": (c_int, [c_fp, c_fp, c_fp, c_fp, c_fp, c_int, c_fp, c_int, c_int, c_int, c_fp]),
     "mac_embed_fwd": (c_int, [c_fp, c_fp, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_int, c_int, c_int, c_int, c_fp]),
     "mac_embed_bwd": (c_int, [c_fp, c_fp, c_f, c_u64, c_int, c_int, c_fp, c_int, c_int, c_int, c_int, c_fp]),
     "mac_lstm_workspace_bytes": (c_sz, [c_int, c_int, c_int]),

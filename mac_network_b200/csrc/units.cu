@@ -5,6 +5,7 @@
 #include "tc_gemm.cuh"
 #include "read_step.cuh"
 #include "read_step_fp8.cuh"
+#include "tc_gemm_fp8.cuh"
 #include "skinny_tc.cuh"
 
 using namespace mac;
@@ -776,6 +777,35 @@ extern "C" int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float ke
                                                      W, C);
   MAC_LAUNCH_CHECK();
   return MAC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ stem: e4m3 inference
+// (tc_gemm_fp8.cuh)
+extern "C" size_t mac_im2col3x3_fp8_workspace_bytes(int B, int H, int W, int C) {
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0) return 0;
+  return im2col3x3_fp8_workspace_bytes((long long)B * H * W);
+}
+
+extern "C" int mac_im2col3x3_fp8(const float* x, void* cols_e4m3, float* row_scale, void* workspace, size_t workspace_bytes,
+                                 int B, int H, int W, int C, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x || !cols_e4m3 || !row_scale || !workspace) return MAC_ERR_INVALID;
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || (long long)B * H * W > (1LL << 30)) return MAC_ERR_INVALID;
+  if (C % 128) return MAC_ERR_UNSUPPORTED;                  // 9C = whole 128-byte k-blocks of mac_linear_fp8_fwd
+  if (!mac_aligned16(x) || !mac_aligned16(cols_e4m3) || !mac_aligned16(workspace)) return MAC_ERR_ALIGN;
+  if (workspace_bytes < mac_im2col3x3_fp8_workspace_bytes(B, H, W, C)) return MAC_ERR_WORKSPACE;
+  return im2col3x3_fp8_launch(x, cols_e4m3, row_scale, workspace, B, H, W, C, stream);
+}
+
+extern "C" int mac_linear_fp8_fwd(const void* x_e4m3, const float* x_scale, const void* wt_e4m3, const float* w_scale,
+                                  const float* b, int act, float* y, int M, int K, int n_out, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x_e4m3 || !x_scale || !wt_e4m3 || !w_scale || !y || M <= 0 || K <= 0 || n_out <= 0) return MAC_ERR_INVALID;
+  if ((K % F8_BK) || (n_out % TC_BN) || !linear_fp8_act_supported(act)) return MAC_ERR_UNSUPPORTED;
+  if ((M + TC_BM - 1) / TC_BM > 65535) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(x_e4m3) || !mac_aligned16(wt_e4m3) || !mac_aligned16(w_scale) || !mac_aligned16(y)) return MAC_ERR_ALIGN;
+  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
+  return linear_fp8_launch(x_e4m3, x_scale, wt_e4m3, w_scale, b, act, y, M, K, n_out, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ stem: col2im (backward)

@@ -6,7 +6,8 @@ dropout on the layer input, 3x3 stride-1 SAME convolution (HWIO kernel) + bias, 
 GPU formulation: convolution as GEMM.  `mac_im2col3x3` builds the `[B*H*W, 9*C]` patch matrix (tap-major, channel fastest
 -- exactly the row-major reshape of the HWIO kernel to `[9*C, Cout]`) with the input dropout fused (the Philox mask is
 indexed by the SOURCE element, so all nine copies of a pixel share its mask), in bf16 for the wgmma GEMM
-(`mac_linear_tc_fwd`, ELU epilogue) or fp32 for the parity GEMM (`mac_linear_fwd`)."""
+(`mac_linear_tc_fwd`, ELU epilogue) or fp32 for the parity GEMM (`mac_linear_fwd`).  `prec="fp8"` is an inference-only
+forward in e4m3: `mac_im2col3x3_fp8` (per-row scales, no dropout) and `mac_linear_fp8_fwd` (csrc/tc_gemm_fp8.cuh)."""
 import collections
 import ctypes
 
@@ -46,7 +47,7 @@ def init_stem_params(specs, seed=0, dtype=np.float32, bias_scale=0.1):
 class Stem(object):
     def __init__(self, params, relu="ELU", prec="fp32", seed=0, version=None):
         """`params`: dict TF-name -> CUDA fp32 tensor (HWIO kernels, biases).  `version`: optional callable returning a counter
-        that changes whenever the parameter values do (`MACParams.version`): the packed bf16 kernels are rebuilt when it moves
+        that changes whenever the parameter values do (`MACParams.version`): the packed bf16 / e4m3 kernels are rebuilt when it moves
         (optimizer step, checkpoint restore, EMA swap -- ADVICE r1), whoever changed the values."""
         self.lib = _lib.load()
         self.p = params
@@ -58,19 +59,56 @@ class Stem(object):
         self.device = dev
 
     def _weights(self, i):
+        """(W, packed): the fp32 [9*Cin, Cout] view and, for bf16, the bf16 [Cout, 9*Cin] pack; for fp8, the e4m3
+        [Cout, 9*Cin] pack and its per-column scales as a pair."""
         K = self.p["stem/cnnLayercnn_%d/kernels/kernel" % i]
         W = K.reshape(-1, K.shape[3])                       # [9*Cin, Cout], row-major view of the HWIO kernel
-        if self.prec == "bf16":
+        if self.prec in ("bf16", "fp8"):
             v = self._version_fn() if self._version_fn is not None else None
             if v != self._packed_version:
                 self._packed.clear()
                 self._packed_version = v
             if i not in self._packed:
-                Wt = torch.empty((W.shape[1], W.shape[0]), dtype=torch.bfloat16, device=W.device)
-                check(self.lib.mac_pack_weight_bf16(ptr(W), ptr(Wt), W.shape[0], W.shape[1], stream_ptr()), "pack")
-                self._packed[i] = Wt
+                if self.prec == "bf16":
+                    Wt = torch.empty((W.shape[1], W.shape[0]), dtype=torch.bfloat16, device=W.device)
+                    check(self.lib.mac_pack_weight_bf16(ptr(W), ptr(Wt), W.shape[0], W.shape[1], stream_ptr()), "pack")
+                    self._packed[i] = Wt
+                else:
+                    Wt = torch.empty((W.shape[1], W.shape[0]), dtype=torch.uint8, device=W.device)
+                    sw = torch.empty(W.shape[1], dtype=torch.float32, device=W.device)
+                    check(self.lib.mac_pack_weight_fp8(ptr(W), ptr(Wt), ptr(sw), W.shape[0], W.shape[1], stream_ptr()),
+                          "mac_pack_weight_fp8")
+                    self._packed[i] = (Wt, sw)
             return W, self._packed[i]
         return W, None
+
+    def _check_fp8(self, in_dim, keep):
+        """The e4m3 stem is the inference forward only (no dropout) with every channel count a multiple of 128 (whole
+        128-byte k-blocks and 128-column tiles of mac_linear_fp8_fwd).  Raises before any launch."""
+        if float(keep) != 1.0:
+            raise NotImplementedError("the fp8 stem is inference only: keep must be 1.0, got %r" % (keep,))
+        dims = [in_dim] + [int(self.p["stem/cnnLayercnn_%d/kernels/kernel" % i].shape[3]) for i in range(self.nlayers)]
+        if any(c % 128 for c in dims):
+            raise NotImplementedError("the fp8 stem needs channel counts that are multiples of 128, got %s" % dims)
+
+    def _forward_fp8(self, x, act):
+        B, H, Wd, _ = x.shape
+        M = B * H * Wd
+        for i in range(self.nlayers):
+            _, (W8, sw) = self._weights(i)
+            b = self.p["stem/cnnLayercnn_%d/biases/bias" % i]
+            C, Nout = x.shape[3], W8.shape[0]
+            cols = torch.empty((M, 9 * C), dtype=torch.uint8, device=self.device)
+            sa = torch.empty(M, dtype=torch.float32, device=self.device)
+            nbytes = int(self.lib.mac_im2col3x3_fp8_workspace_bytes(B, H, Wd, C))
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            check(self.lib.mac_im2col3x3_fp8(ptr(x), ptr(cols), ptr(sa), ptr(ws), nbytes, B, H, Wd, C, stream_ptr()),
+                  "mac_im2col3x3_fp8")
+            y = torch.empty((M, Nout), dtype=torch.float32, device=self.device)
+            check(self.lib.mac_linear_fp8_fwd(ptr(cols), ptr(sa), ptr(W8), ptr(sw), ptr(b), act, ptr(y), M, 9 * C, Nout,
+                                              stream_ptr()), "mac_linear_fp8_fwd")
+            x = y.view(B, H, Wd, Nout)
+        return x.view(B, H * Wd, x.shape[3])
 
     def _check_trainable(self, in_dim):
         """Training (forward with save_for_backward + backward) runs in fp32, or in bf16 on tensor cores
@@ -94,6 +132,9 @@ class Stem(object):
         if save_for_backward:
             self._check_trainable(C)
             self._saved = {"xs": [], "ys": [], "keep": float(keep), "step": int(step), "act": act}
+        if self.prec == "fp8":
+            self._check_fp8(C, keep)
+            return self._forward_fp8(x, act)
         for i in range(self.nlayers):
             if save_for_backward:
                 self._saved["xs"].append(x)
