@@ -5,47 +5,70 @@
 //   logit  = I2 . wr + br                               (mac_cell.py:266, ops.py:316-317)
 //   att    = softmax_n(logit);  info = sum_n att * KB   (ops.py:143, 149-150; original KB, mac_cell.py:271-275)
 //
-// read_step_kernel computes the logits of 64-row tiles of the knowledge base (rows packed across sample boundaries, so
-// ceil(B*N / 64) tiles) with P*y, H and I2 never leaving the SM; kb_attend (attend.cu) then does the per-sample softmax and
+// read_step_kernel computes the logits of 128-row tiles of the knowledge base (rows packed across sample boundaries, so
+// ceil(B*N / 128) tiles) with P*y, H and I2 never leaving the SM; kb_attend (attend.cu) then does the per-sample softmax and
 // weighted sum.  Two launches per step instead of the four of scale_rows_bf16 + tc_gemm<ADDACT> + tc_gemm<LOGITS> + kb_attend,
 // and none of the P*y / H round trips through L2 and HBM (4 x B*N*d bf16).
 //
-// CTA = 288 threads: warp 8 is the TMA producer; warpgroups 0 and 1 each own one 256-column half of the d = 512 outputs
-// (wgmma m64n256k16, a 64 x 256 fp32 accumulator in 128 registers per thread).  Shared memory:
-//   A   [64 x 512] bf16 as 8 K-major 128-byte-swizzled [64 x 64] blocks (64 KB): H = GEMM 1's epilogue, the A operand of
-//       GEMM 2
-//   B   2 stages x 72 KB: one mbarrier ring of 17 slots per tile.  Slots 0..7 each carry k-block j of Wm[0:d] ([512 x 64],
-//       64 KB) and k-block j of the P tile ([64 x 64], 8 KB, the A layout), so GEMM 1 starts when its first 72 KB have
-//       landed; slot 8 carries the tile's Q rows (64 KB, the A layout), GEMM 1's addend; slots 9..16 the k-blocks of Wm2.
-//       GEMM 1's epilogue reads Q from shared memory: loaded from global memory there, with the 128 accumulator registers
-//       live, too few loads fit in flight to hide latency
-// GEMM 1 scales P block j by y in place (P*y, rounded to bf16) while the MMAs of block j - 1 run, then issues block j.
-// Epilogue 2 reads bm2, wr and the control rows of the tile's first two samples from shared memory (rows of later samples,
-// only present when N < 64, from global memory).  The logits are summed over both halves in shared memory and written as one
-// partial per row.
+// The kernel is bound by its weight stream: every tile streams all of Wm[0:d] and Wm2 (1 MB) from L2.  With 128 rows per CTA
+// each [256 x 64] weight half-block feeds both consumer warpgroups, so a knowledge-base row costs half the weight bytes of a
+// 64-row tile.  CTA = 384 threads: warpgroup 2 is the TMA producer (setmaxnreg down to 40 registers, one elected thread
+// issues); consumer warpgroup g in {0, 1} owns tile rows [64 g, 64 g + 64) (setmaxnreg up to 232) and computes all d = 512
+// output columns of them, one 256-column half at a time (wgmma m64n256k16, a 64 x 256 fp32 accumulator in 128 registers).
+// Shared memory:
+//   A   [128 x 512] bf16 as 8 K-major 128-byte-swizzled [128 x 64] blocks (128 KB).  The producer loads the P tile straight
+//       into it (one mbarrier per block); each warpgroup scales its own 64 rows of block j by y in place (P*y, rounded to
+//       bf16) while the MMAs of block j - 1 run.  Once GEMM 1 is done it holds H, GEMM 2's A operand.  A warpgroup only
+//       reads and writes its own rows, so all A-side synchronisation is a 128-thread named barrier of that warpgroup.
+//   B   3 stages x 32 KB, one mbarrier ring of 36 slots per tile, each slot a [256 x 64] weight half-block or two [128 x 64]
+//       Q blocks: GEMM 1 columns [0, 256) (8 slots), their Q (2), GEMM 1 columns [256, 512) (8), their Q (2), GEMM 2 columns
+//       [0, 256) (8), GEMM 2 columns [256, 512) (8).  Both warpgroups consume every slot.
+// GEMM 1's first half ends in H0 = ELU(acc + Q), packed to bf16 and held in registers (64 per thread) while the second half
+// accumulates; after the second half's MMAs P*y is dead, and H0 and H1 = ELU(acc + Q) are written into the A region.
+// Epilogue 2 reduces ELU((acc + bm2) * control) . wr over each 256-column half (bm2, wr and control through L1) and adds the
+// two halves' sums as half0 + half1.  Every output element takes the same operations in the same order as in the 64-row
+// form (wgmma shape and k order, P*y and H roundings, fmaf order, half sums), so the results do not depend on the tiling.
+//
+// read_step_fp8_kernel (read_step_fp8.cuh) keeps the 64-row form and its RS_* constants: 288 threads, one producer warp and
+// two consumer warpgroups that each own one 256-column half of a 64-row tile, at most 168 registers per thread.
 #pragma once
 #include "tc_gemm.cuh"
 
 namespace mac {
 
 constexpr int RS_D = 512;                       // d of the shipped configurations
-constexpr int RS_BM = 64;                       // knowledge-base rows per CTA (one tile)
+constexpr int RS_BM = 64;                       // knowledge-base rows per CTA of the 64-row form
 constexpr int RS_KB = RS_D / TC_BK;             // 8 k-blocks
 constexpr int RS_BLK = RS_BM * TC_BK * 2;       // one [64 x 64] bf16 A block: 8 KB
 constexpr int RS_A_BYTES = RS_KB * RS_BLK;      // 64 KB
 constexpr int RS_B_HALF = 256 * TC_BK * 2;      // [256 x 64] bf16: 32 KB
-constexpr int RS_W_BYTES = 2 * RS_B_HALF;       // one weight k-block: 64 KB
-constexpr int RS_STAGE = RS_W_BYTES + RS_BLK;   // 72 KB: a weight k-block and, in GEMM 1's slots, a P block
-constexpr int RS_STAGES = 2;
-constexpr int RS_Q_SLOT = RS_KB;                // ring slot of the Q tile, between the two GEMMs' k-blocks
-constexpr int RS_SLOTS = RS_Q_SLOT + 1 + RS_KB; // ring slots per tile
 constexpr int RS_CONSUMERS = 256;
 constexpr int RS_THREADS = RS_CONSUMERS + 32;
-constexpr int RS_SMEM_BYTES = RS_A_BYTES + RS_STAGES * RS_STAGE + 1024 /*align*/ + 64 /*barriers*/ +
-                              2 * RS_BM * 4 /*logit halves*/ + 2 * RS_D * 4 /*control of <= 2 samples*/ +
-                              2 * RS_D * 4 /*bm2, wr*/;
-static_assert(RS_SMEM_BYTES <= 232448, "over the sm_90 per-block shared memory opt-in limit");
-static_assert(RS_STAGE % 1024 == 0 && RS_W_BYTES % 1024 == 0, "swizzled operands need 1024-byte alignment");
+
+// read_step_kernel: 128 rows per CTA
+constexpr int RS128_BM = 128;
+constexpr int RS128_BLK = RS128_BM * TC_BK * 2;          // one [128 x 64] bf16 A block: 16 KB
+constexpr int RS128_A_BYTES = RS_KB * RS128_BLK;         // 128 KB
+constexpr int RS128_STAGE = RS_B_HALF;                   // 32 KB: a weight half-block or two Q blocks
+constexpr int RS128_STAGES = 3;
+constexpr int RS128_Q0 = RS_KB;                          // ring slots of the Q blocks of columns [0, 256)
+constexpr int RS128_G1B = RS128_Q0 + 2;                  // GEMM 1, columns [256, 512)
+constexpr int RS128_Q1 = RS128_G1B + RS_KB;              // Q of columns [256, 512)
+constexpr int RS128_G2A = RS128_Q1 + 2;                  // GEMM 2, columns [0, 256)
+constexpr int RS128_G2B = RS128_G2A + RS_KB;             // GEMM 2, columns [256, 512)
+constexpr int RS128_SLOTS = RS128_G2B + RS_KB;           // 36 ring slots per tile
+constexpr int RS128_CONSUMERS = 256;
+constexpr int RS128_THREADS = RS128_CONSUMERS + 128;
+constexpr int RS128_SMEM_BYTES = RS128_A_BYTES + RS128_STAGES * RS128_STAGE + 1024 /*align*/ +
+                                 8 * (RS_KB + 2 * RS128_STAGES) /*barriers*/;
+static_assert(RS128_SMEM_BYTES <= 232448, "over the sm_90 per-block shared memory opt-in limit");
+static_assert(RS128_BLK % 1024 == 0 && RS128_STAGE % 1024 == 0 && (RS128_BM / 2) * 128 % 1024 == 0,
+              "swizzled operands need 1024-byte alignment");
+static_assert(2 * RS128_BLK == RS128_STAGE, "a ring slot holds two Q blocks");
+// registers per thread of the producer and consumer warpgroups: 40 + 2 x 232 = 3 x 168, the launch allocation of 384 threads
+constexpr int RS128_PRODUCER_REGS = 40;
+constexpr int RS128_CONSUMER_REGS = 232;
+static_assert(RS128_PRODUCER_REGS + 2 * RS128_CONSUMER_REGS <= 3 * (65536 / RS128_THREADS / 8 * 8), "register budget");
 
 __device__ __forceinline__ float bf16lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf16hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
@@ -75,192 +98,251 @@ struct ReadStepParams {
 
 __device__ __forceinline__ void rs_consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(RS_CONSUMERS) : "memory"); }
 
-__global__ void __launch_bounds__(RS_THREADS, 1)
+// named barrier of one consumer warpgroup (ids 1 and 2; 0 is __syncthreads)
+__device__ __forceinline__ void rs128_wg_bar(int g) { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); }
+
+// one warpgroup's 256-column half of a GEMM: acc = A[64 x 512] @ (the [256 x 64] half-blocks in ring slots t0 .. t0 + 7)^T,
+// A block j at a_u + j * RS128_BLK.  Releases each slot once its MMAs are done.
+__device__ __forceinline__ void rs128_gemm_half(float (&acc)[128], uint32_t a_u, uint32_t ring_u, uint64_t* full,
+                                                uint64_t* empty, int t0, int lane) {
+  for (int j = 0; j < RS_KB; ++j) {
+    const int t = t0 + j, s = t % RS128_STAGES;
+    mbar_wait(&full[s], (t / RS128_STAGES) & 1);
+    const uint64_t adesc = make_sw128_kmajor_desc(a_u + j * RS128_BLK);
+    const uint64_t bdesc = make_sw128_kmajor_desc(ring_u + s * RS128_STAGE);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n256(acc, adesc + 2 * k, bdesc + 2 * k, (j || k) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    wgmma_hold(acc);
+    if (j && lane == 0) mbar_arrive(&empty[(t - 1) % RS128_STAGES]);
+  }
+  wgmma_wait<0>();
+  wgmma_hold(acc);
+  if (lane == 0) mbar_arrive(&empty[(t0 + RS_KB - 1) % RS128_STAGES]);
+}
+
+// byte offset of (row r, column n) in a K-major 128-byte-swizzled stack of [rows x 64] bf16 blocks of blk bytes each
+__device__ __forceinline__ int rs128_sw_off(int r, int n, int blk) {
+  return (n >> 6) * blk + r * 128 + ((((n & 63) >> 3) ^ (r & 7)) << 4) + (n & 7) * 2;
+}
+
+__global__ void __launch_bounds__(RS128_THREADS, 1)
 read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constant__ CUtensorMap map_q,
                  const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_w2,
                  const ReadStepParams p) {
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t base_u32 = smem_u32(smem_dyn);
   unsigned char* a_tile = smem_dyn + ((1024u - (base_u32 & 1023u)) & 1023u);
-  unsigned char* b_ring = a_tile + RS_A_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(b_ring + RS_STAGES * RS_STAGE);   // [STAGES] TMA -> consumers
-  uint64_t* empty = full + RS_STAGES;              // [STAGES] consumers -> TMA (8 warp arrivals)
-  float* s_lg = reinterpret_cast<float*>(full + 8);          // [2][64] logit halves
-  float* s_ctrl = s_lg + 2 * RS_BM;                          // [2][d] control of the tile's first two samples
-  float* s_bm2 = s_ctrl + 2 * RS_D;                          // [d]
-  float* s_wr = s_bm2 + RS_D;                                // [d]
+  unsigned char* ring = a_tile + RS128_A_BYTES;
+  uint64_t* pfull = reinterpret_cast<uint64_t*>(ring + RS128_STAGES * RS128_STAGE);   // [8] P block j landed
+  uint64_t* full = pfull + RS_KB;                  // [STAGES] TMA -> consumers
+  uint64_t* empty = full + RS128_STAGES;           // [STAGES] consumers -> TMA (8 warp arrivals)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int row0 = blockIdx.x * RS_BM;
-  const int s_lo = row0 / p.N;                               // first sample of the tile
+  const int row0 = blockIdx.x * RS128_BM;
 
-  if (threadIdx.x == RS_CONSUMERS) {
+  if (threadIdx.x == RS128_CONSUMERS) {
     tma_prefetch_desc(&map_p);
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_w1);
     tma_prefetch_desc(&map_w2);
-    for (int i = 0; i < RS_STAGES; ++i) {
+    for (int i = 0; i < RS_KB; ++i) mbar_init(&pfull[i], 1);
+    for (int i = 0; i < RS128_STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], RS_CONSUMERS / 32);
+      mbar_init(&empty[i], RS128_CONSUMERS / 32);
     }
     fence_mbar_init();
   }
   __syncthreads();
 
-  if (warp == RS_CONSUMERS / 32) {
-    // ===================================================== TMA producer
-    if (elect_one()) {
-      // ring slots 0..7: Wm[0:d] k-block j + P k-block j; slot 8: the Q tile (GEMM 1's addend); slots 9..16: Wm2 k-blocks
-      for (int j = 0; j < RS_SLOTS; ++j) {
-        const int s = j % RS_STAGES;
-        mbar_wait(&empty[s], ((j / RS_STAGES) & 1) ^ 1);
-        unsigned char* dst = b_ring + s * RS_STAGE;
-        if (j == RS_Q_SLOT) {
-          mbar_expect_tx(&full[s], RS_A_BYTES);
-          for (int kb = 0; kb < RS_KB; ++kb) tma_load_2d(dst + kb * RS_BLK, &map_q, kb * TC_BK, row0, &full[s]);
-          continue;
+  if (warp >= RS128_CONSUMERS / 32) {
+    // ===================================================== TMA producer warpgroup
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(RS128_PRODUCER_REGS));
+    if (warp == RS128_CONSUMERS / 32 && elect_one()) {
+      // the P tile goes straight into the A region; its first blocks are interleaved with the first weight slots so
+      // GEMM 1 can start once P block 0 and weight slot 0 have landed
+      auto load_p = [&](int j) {
+        mbar_expect_tx(&pfull[j], RS128_BLK);
+        tma_load_2d(a_tile + j * RS128_BLK, &map_p, j * TC_BK, row0, &pfull[j]);
+      };
+      for (int t = 0; t < RS128_SLOTS; ++t) {
+        if (t < RS128_STAGES) load_p(t);
+        else if (t == RS128_STAGES)
+          for (int j = RS128_STAGES; j < RS_KB; ++j) load_p(j);
+        const int s = t % RS128_STAGES;
+        mbar_wait(&empty[s], ((t / RS128_STAGES) & 1) ^ 1);
+        unsigned char* dst = ring + s * RS128_STAGE;
+        mbar_expect_tx(&full[s], RS128_STAGE);
+        if (t < RS128_G2A) {
+          const int half = t >= RS128_G1B, u = t - half * RS128_G1B;
+          if (u < RS_KB) {
+            tma_load_2d(dst, &map_w1, u * TC_BK, 256 * half, &full[s]);
+          } else {                                       // Q blocks 4 half + 2 (u - 8) and the one after it
+            const int kb = 4 * half + 2 * (u - RS_KB);
+            tma_load_2d(dst, &map_q, kb * TC_BK, row0, &full[s]);
+            tma_load_2d(dst + RS128_BLK, &map_q, (kb + 1) * TC_BK, row0, &full[s]);
+          }
+        } else {
+          const int half = t >= RS128_G2B, u = t - (half ? RS128_G2B : RS128_G2A);
+          tma_load_2d(dst, &map_w2, u * TC_BK, 256 * half, &full[s]);
         }
-        const bool g1 = j < RS_Q_SLOT;
-        mbar_expect_tx(&full[s], g1 ? RS_W_BYTES + RS_BLK : RS_W_BYTES);
-        const CUtensorMap* m = g1 ? &map_w1 : &map_w2;
-        const int k0 = (g1 ? j : j - RS_Q_SLOT - 1) * TC_BK;
-        if (g1) tma_load_2d(dst + RS_W_BYTES, &map_p, k0, row0, &full[s]);
-        tma_load_2d(dst, m, k0, 0, &full[s]);
-        tma_load_2d(dst + RS_B_HALF, m, k0, 256, &full[s]);
       }
     }
     return;
   }
 
   // ===================================================== consumers
-  const int tid = threadIdx.x;
-  const int g = warp >> 2;                                   // warpgroup: output columns [256 g, 256 g + 256)
-  // acc[4 j + 2 h + e] is tile row 16 (warp & 3) + lane / 4 + 8 h, column 256 g + 8 j + 2 (lane & 3) + e
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(RS128_CONSUMER_REGS));
+  const int g = warp >> 2;                                   // warpgroup: tile rows [64 g, 64 g + 64)
+  const int wt = threadIdx.x & 127;
+  // acc[4 j + 2 h + e] is warpgroup row rl + 8 h, column 256 half + 8 j + 2 (lane & 3) + e
   const int rl = 16 * (warp & 3) + (lane >> 2);
-  const int cq = 256 * g + 2 * (lane & 3);
-  // this thread's two 16-byte chunks of each P block: rows tid / 8 and tid / 8 + 32, chunk tid % 8 of the swizzled
-  // 128-byte row, i.e. columns pcol .. pcol + 7 of the k-block (the swizzle only depends on row % 8)
-  const int prow = tid >> 3;
-  const int poff = prow * 128 + (tid & 7) * 16;
-  const int pcol = ((tid & 7) ^ (prow & 7)) << 3;
-  for (int i = tid; i < RS_D; i += RS_CONSUMERS) {
-    s_bm2[i] = __ldg(p.bm2 + i);
-    s_wr[i] = __ldg(p.wr + i);
-  }
-  float acc[128];
-  const int last_row = min(p.M, row0 + RS_BM) - 1;
-  const int nsamp = last_row / p.N - s_lo + 1;
-  for (int q = 0; q < min(nsamp, 2); ++q)
-    for (int i = tid; i < RS_D; i += RS_CONSUMERS) s_ctrl[q * RS_D + i] = __ldg(p.ctrl + (size_t)(s_lo + q) * RS_D + i);
-  // y rows of this thread's two P rows (rows past M are TMA zero fill and stay zero), as 32-bit offsets into y rather than
-  // pointers: the two registers they save keep the kernel free of spills at its 168-register cap
-  int yoff[2];
+  const int cq = 2 * (lane & 3);
+  const int rowg = row0 + 64 * g;                           // first row of this warpgroup
+  unsigned char* a_wg = a_tile + g * (RS128_BM / 2) * 128;  // this warpgroup's rows of every A block
+  const uint32_t a_u = smem_u32(a_wg), ring_u = smem_u32(ring);
+  // this thread's four 16-byte chunks of the warpgroup's rows of each P block: rows wt / 8 + 16 u, chunk wt % 8 of the
+  // swizzled 128-byte row, i.e. columns pcol .. pcol + 7 of the k-block (the swizzle only depends on row % 8)
+  const int prow = wt >> 3;
+  const int poff = prow * 128 + (wt & 7) * 16;
+  const int pcol = ((wt & 7) ^ (prow & 7)) << 3;
+  // y rows of this thread's four P rows (rows past M are TMA zero fill and stay zero)
+  int yoff[4];
 #pragma unroll
-  for (int u = 0; u < 2; ++u) yoff[u] = min(row0 + prow + 32 * u, p.M - 1) / p.N * RS_D + pcol;
+  for (int u = 0; u < 4; ++u) yoff[u] = min(rowg + prow + 16 * u, p.M - 1) / p.N * RS_D + pcol;
 
-  // ---- GEMM 1: P block j is scaled by y in place (P*y) while the MMAs of block j - 1 run, then block j is issued
-  for (int j = 0; j < RS_KB; ++j) {
-    const int s = j % RS_STAGES;
-    unsigned char* stage = b_ring + s * RS_STAGE;
-    // y is loaded ahead of the stage's wait so the loads overlap it.  Plain loads: the compiler schedules __ldg
-    // (ld.global.nc) loads of y after the wait, where their latency is exposed
-    float4 y0[2], y1[2];
+  float acc[128];
+  // ---- GEMM 1, columns [0, 256): P block j is scaled by y in place (P*y) while the MMAs of block j - 1 run, then issued.
+  //      The y of block j + 1 is loaded right after block j's MMAs are issued, so its L2 latency hides under them.  Plain
+  //      loads: the compiler schedules __ldg (ld.global.nc) loads of y after the waits, where their latency is exposed
+  float4 y0[4], y1[4];
+  auto load_y = [&](int j) {
 #pragma unroll
-    for (int u = 0; u < 2; ++u) {
+    for (int u = 0; u < 4; ++u) {
       y0[u] = *reinterpret_cast<const float4*>(p.y + yoff[u] + j * TC_BK);
       y1[u] = *reinterpret_cast<const float4*>(p.y + yoff[u] + j * TC_BK + 4);
     }
-    mbar_wait(&full[s], (j / RS_STAGES) & 1);
+  };
+  load_y(0);
+  for (int j = 0; j < RS_KB; ++j) {
+    const int s = j % RS128_STAGES;
+    mbar_wait(&pfull[j], 0);
 #pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      uint4* c = reinterpret_cast<uint4*>(stage + RS_W_BYTES + poff + u * 32 * 128);
+    for (int u = 0; u < 4; ++u) {
+      uint4* c = reinterpret_cast<uint4*>(a_wg + j * RS128_BLK + poff + u * 16 * 128);
       const uint4 v = *c;
       *c = make_uint4(pack_bf16(bf16lo(v.x) * y0[u].x, bf16hi(v.x) * y0[u].y), pack_bf16(bf16lo(v.y) * y0[u].z, bf16hi(v.y) * y0[u].w),
                       pack_bf16(bf16lo(v.z) * y1[u].x, bf16hi(v.z) * y1[u].y), pack_bf16(bf16lo(v.w) * y1[u].z, bf16hi(v.w) * y1[u].w));
     }
     fence_proxy_async();                                   // generic-proxy stores -> visible to wgmma
-    rs_consumer_bar();
-    const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(stage + RS_W_BYTES));
-    const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(stage + g * RS_B_HALF));
+    rs128_wg_bar(g);
+    mbar_wait(&full[s], (j / RS128_STAGES) & 1);
+    const uint64_t adesc = make_sw128_kmajor_desc(a_u + j * RS128_BLK);
+    const uint64_t bdesc = make_sw128_kmajor_desc(ring_u + s * RS128_STAGE);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n256(acc, adesc + 2 * k, bdesc + 2 * k, (j || k) ? 1u : 0u);
     wgmma_commit();
+    if (j + 1 < RS_KB) load_y(j + 1);
     wgmma_wait<1>();
     wgmma_hold(acc);
-    if (j && lane == 0) mbar_arrive(&empty[(j - 1) % RS_STAGES]);
+    if (j && lane == 0) mbar_arrive(&empty[(j - 1) % RS128_STAGES]);
   }
   wgmma_wait<0>();
   wgmma_hold(acc);
-  if (lane == 0) mbar_arrive(&empty[(RS_KB - 1) % RS_STAGES]);
+  if (lane == 0) mbar_arrive(&empty[(RS_KB - 1) % RS128_STAGES]);
 
-  // ---- GEMM 1's epilogue: H = ELU(acc + Q) -> bf16 into the A tile (K-major, swizzled).  Q comes through the ring in
-  //      the A tile's layout, so it is read at the same conflict-free offsets H is written to.  GEMM 1 takes its A operand
-  //      from the ring, so nothing else uses the A tile before this.
-  constexpr int qs = RS_Q_SLOT % RS_STAGES;
-  const unsigned char* q_tile = b_ring + qs * RS_STAGE;
-  mbar_wait(&full[qs], (RS_Q_SLOT / RS_STAGES) & 1);
+  // ---- H0 = ELU(acc + Q) -> bf16, held in registers.  Q comes through the ring as [128 x 64] blocks in the A layout.
+  uint32_t h0[64];
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    const int t = RS128_Q0 + q, s = t % RS128_STAGES;
+    mbar_wait(&full[s], (t / RS128_STAGES) & 1);
+    const unsigned char* q_tile = ring + s * RS128_STAGE + g * (RS128_BM / 2) * 128 - 2 * q * RS128_BLK;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = rl + 8 * h;
+      const bool live = rowg + r < p.M;
+#pragma unroll
+      for (int j = 16 * q; j < 16 * q + 16; ++j) {
+        const uint32_t qv = *reinterpret_cast<const uint32_t*>(q_tile + rs128_sw_off(r, cq + 8 * j, RS128_BLK));
+        h0[2 * j + h] = live ? pack_bf16(elu_fast(acc[4 * j + 2 * h] + bf16lo(qv)), elu_fast(acc[4 * j + 2 * h + 1] + bf16hi(qv)))
+                             : 0u;
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);                 // this warp's Q reads are done
+  }
+
+  // ---- GEMM 1, columns [256, 512), on the same P*y blocks
+  rs128_gemm_half(acc, a_u, ring_u, full, empty, RS128_G1B, lane);
+
+  // ---- P*y is dead once every warp of the warpgroup is past its MMAs: H0, then H1 = ELU(acc + Q), into the A region
+  rs128_wg_bar(g);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int r = rl + 8 * h, row = row0 + r;
+    const int r = rl + 8 * h;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int n = cq + 8 * j;
-      const int kb = n >> 6, c = (n & 63) >> 3;
-      const int off = kb * RS_BLK + r * 128 + ((c ^ (r & 7)) << 4) + (n & 7) * 2;
-      const uint32_t q = *reinterpret_cast<const uint32_t*>(q_tile + off);
-      const uint32_t hv = row < p.M ? pack_bf16(elu_fast(acc[4 * j + 2 * h] + bf16lo(q)), elu_fast(acc[4 * j + 2 * h + 1] + bf16hi(q)))
-                                    : 0u;
-      *reinterpret_cast<uint32_t*>(a_tile + off) = hv;
+    for (int j = 0; j < 32; ++j) *reinterpret_cast<uint32_t*>(a_wg + rs128_sw_off(r, cq + 8 * j, RS128_BLK)) = h0[2 * j + h];
+  }
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    const int t = RS128_Q1 + q, s = t % RS128_STAGES;
+    mbar_wait(&full[s], (t / RS128_STAGES) & 1);
+    const unsigned char* q_tile = ring + s * RS128_STAGE + g * (RS128_BM / 2) * 128 - 2 * q * RS128_BLK;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = rl + 8 * h;
+      const bool live = rowg + r < p.M;
+#pragma unroll
+      for (int j = 16 * q; j < 16 * q + 16; ++j) {
+        const int n = cq + 8 * j;
+        const uint32_t qv = *reinterpret_cast<const uint32_t*>(q_tile + rs128_sw_off(r, n, RS128_BLK));
+        *reinterpret_cast<uint32_t*>(a_wg + rs128_sw_off(r, 256 + n, RS128_BLK)) =
+            live ? pack_bf16(elu_fast(acc[4 * j + 2 * h] + bf16lo(qv)), elu_fast(acc[4 * j + 2 * h + 1] + bf16hi(qv))) : 0u;
+      }
     }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
   }
   fence_proxy_async();
-  rs_consumer_bar();
-  if (lane == 0) mbar_arrive(&empty[qs]);                  // Q read and used by every thread of this warp
+  rs128_wg_bar(g);
 
-  // ---- GEMM 2
-  const uint32_t a_u = smem_u32(a_tile);
-  for (int j = 0; j < RS_KB; ++j) {
-    const int jj = RS_Q_SLOT + 1 + j, s = jj % RS_STAGES;
-    mbar_wait(&full[s], (jj / RS_STAGES) & 1);
-    const uint64_t adesc = make_sw128_kmajor_desc(a_u + j * RS_BLK);
-    const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(b_ring + s * RS_STAGE + g * RS_B_HALF));
-    wgmma_fence();
+  // ---- GEMM 2, one 256-column half at a time; epilogue: I2 = ELU((acc + bm2) * control_b), sum_n I2 * wr over the half
+  float part[2][2];
 #pragma unroll
-    for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n256(acc, adesc + 2 * k, bdesc + 2 * k, (j || k) ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<1>();
-    wgmma_hold(acc);
-    if (j && lane == 0) mbar_arrive(&empty[(jj - 1) % RS_STAGES]);
+  for (int half = 0; half < 2; ++half) {
+    rs128_gemm_half(acc, a_u, ring_u, full, empty, half ? RS128_G2B : RS128_G2A, lane);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rowg + rl + 8 * h;
+      const float* crow = p.ctrl + (size_t)(min(row, p.M - 1) / p.N) * RS_D + 256 * half;
+      const float* bm2 = p.bm2 + 256 * half;
+      const float* wr = p.wr + 256 * half;
+      float s = 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const int n = cq + 8 * j;
+        const float2 cc = __ldg(reinterpret_cast<const float2*>(crow + n));
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bm2 + n));
+        const float2 ww = __ldg(reinterpret_cast<const float2*>(wr + n));
+        const float t0 = elu_fast((acc[4 * j + 2 * h] + bb.x) * cc.x);
+        const float t1 = elu_fast((acc[4 * j + 2 * h + 1] + bb.y) * cc.y);
+        s = fmaf(t0, ww.x, s);
+        s = fmaf(t1, ww.y, s);
+      }
+      s += __shfl_xor_sync(0xffffffffu, s, 1);
+      s += __shfl_xor_sync(0xffffffffu, s, 2);
+      part[half][h] = s;
+    }
   }
-  wgmma_wait<0>();
-  wgmma_hold(acc);
-  if (lane == 0) mbar_arrive(&empty[(RS_SLOTS - 1) % RS_STAGES]);
-
-  // ---- GEMM 2's epilogue: I2 = ELU((acc + bm2) * control_b); logit half = sum_n I2 * wr
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int r = rl + 8 * h, row = row0 + r;
-    const int s = min(row, p.M - 1) / p.N;
-    const float* crow = s - s_lo < 2 ? s_ctrl + (s - s_lo) * RS_D : p.ctrl + (size_t)s * RS_D;
-    float part = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int n = cq + 8 * j;
-      const float2 cc = *reinterpret_cast<const float2*>(crow + n);
-      const float2 bb = *reinterpret_cast<const float2*>(s_bm2 + n);
-      const float2 ww = *reinterpret_cast<const float2*>(s_wr + n);
-      const float t0 = elu_fast((acc[4 * j + 2 * h] + bb.x) * cc.x);
-      const float t1 = elu_fast((acc[4 * j + 2 * h + 1] + bb.y) * cc.y);
-      part = fmaf(t0, ww.x, part);
-      part = fmaf(t1, ww.y, part);
-    }
-    part += __shfl_xor_sync(0xffffffffu, part, 1);
-    part += __shfl_xor_sync(0xffffffffu, part, 2);
-    if ((lane & 3) == 0) s_lg[g * RS_BM + r] = part;
+    const int row = rowg + rl + 8 * h;
+    if ((lane & 3) == 0 && row < p.M) p.logits[row] = part[0][h] + part[1][h];
   }
-  rs_consumer_bar();
-  if (tid < RS_BM && row0 + tid < p.M) p.logits[row0 + tid] = s_lg[tid] + s_lg[RS_BM + tid];
 }
 
 // inv = [P | Q] (tc_read_invariant); y, control [B, d] fp32; att [B, N], info [B, d]
@@ -271,9 +353,9 @@ inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y
   const int M = B * N;
   const TcReadScratch s = tc_read_scratch(const_cast<void*>(inv), B, N, d);
   CUtensorMap mp, mq, mw1, mw2;
-  int st = make_tmap_2d(&mp, s.P, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS_BM, TC_BK, 1);
+  int st = make_tmap_2d(&mp, s.P, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS128_BM, TC_BK, 1);
   if (st != MAC_OK) return st;
-  st = make_tmap_2d(&mq, s.Q, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS_BM, TC_BK, 1);
+  st = make_tmap_2d(&mq, s.Q, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS128_BM, TC_BK, 1);
   if (st != MAC_OK) return st;
   st = make_tmap_2d(&mw1, w->Wm_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)2 * d * 2, 256, TC_BK, 1);   // Wm[0:d] of [d, 2d]
   if (st != MAC_OK) return st;
@@ -282,8 +364,8 @@ inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y
   ReadStepParams p{};
   p.M = M; p.N = N; p.y = y; p.ctrl = control; p.bm2 = w->bm2; p.wr = w->wr; p.logits = s.parts;
   // the opt-in is per device context: set it on every launch
-  MAC_CUDA_TRY(cudaFuncSetAttribute(read_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM_BYTES));
-  read_step_kernel<<<(M + RS_BM - 1) / RS_BM, RS_THREADS, RS_SMEM_BYTES, stream>>>(mp, mq, mw1, mw2, p);
+  MAC_CUDA_TRY(cudaFuncSetAttribute(read_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RS128_SMEM_BYTES));
+  read_step_kernel<<<(M + RS128_BM - 1) / RS128_BM, RS128_THREADS, RS128_SMEM_BYTES, stream>>>(mp, mq, mw1, mw2, p);
   MAC_LAUNCH_CHECK();
   return mac_kb_attend_fwd(s.parts, 1, w->br, kb_bf16, 1, att, info, B, N, d, stream);
 }

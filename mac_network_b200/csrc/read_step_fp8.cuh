@@ -1,5 +1,5 @@
 // One reasoning step of the read unit in inference form with e4m3 (FP8) operands on wgmma: the same function as
-// read_step_kernel (read_step.cuh), the same tiling (64 knowledge-base rows per CTA, packed across sample boundaries; one
+// read_step_kernel (read_step.cuh), in its 64-row form (64 knowledge-base rows per CTA, packed across sample boundaries; one
 // TMA producer warp and two consumer warpgroups that each own 256 output columns; P*y, H and the logits stay on the SM;
 // kb_attend on the bf16 knowledge base is the tail), but both GEMMs are m64n256k32 e4m3 x e4m3 -> fp32.  A weight k-block of
 // 64 KB holds 128 input rows instead of 64, so each GEMM streams half the weight bytes and waits on half as many ring slots.
@@ -15,7 +15,7 @@
 //
 // Shared memory: A [64 x 512] e4m3 as 4 K-major 128-byte-swizzled [64 x 128] blocks (32 KB): H8, the A operand of GEMM 2.
 // B: 2 stages x 72 KB, one mbarrier ring of 9 slots per tile: slots 0..3 each carry k-block j of Wm[0:d] ([512 x 128] e4m3,
-// 64 KB) and k-block j of the P8 tile ([64 x 128], 8 KB); slot 4 the tile's bf16 Q rows (64 KB, read_step_kernel's layout);
+// 64 KB) and k-block j of the P8 tile ([64 x 128], 8 KB); slot 4 the tile's bf16 Q rows (64 KB, 8 [64 x 64] blocks);
 // slots 5..8 the k-blocks of Wm2.  Three 72 KB stages beside the A tile would need 248 KB, over the 227 KB opt-in limit.
 // y / ay_b of the tile's first two samples is staged in shared memory (rows of later samples, only present when N < 64, are
 // read from global memory and scaled by 1 / ay_b): sixteen y values per 16-byte P8 chunk do not fit in registers beside the
