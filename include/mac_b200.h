@@ -434,6 +434,33 @@ int mac_lstm_fwd(const float* gx_fw, const float* gx_bw, const float* Wh_fw, con
 int mac_lstm_bwd(const float* Wh_fw, const float* Wh_bw, const int32_t* lengths, const float* save_gates,
                  const float* save_c, const float* d_out_seq, const float* d_vecq, float* dG_fw, float* dG_bw,
                  void* workspace, size_t workspace_bytes, int B, int S, int h, int ndir, mac_stream_t stream);
+/* The question encoder on wgmma tensor cores (csrc/encoder_tc.cuh; QuestionEncoder(prec="bf16")): bf16 matrix-product
+ * operands, fp32 accumulation; the cell state, gate non-linearities, outputs, saved tensors and element-wise backward steps
+ * are fp32.  Ep = E rounded up to a multiple of 128; the bf16 operands carry zero columns E..Ep-1.  h must be 256
+ * (MAC_ERR_UNSUPPORTED otherwise).  All checks precede any launch.
+ * mac_embed_fwd_tc: mac_embed_fwd's out_raw (required) and x_bf16 [B*S, Ep] = bf16(dropout(words)) with the same keep-mask.
+ * mac_pack_weight_bf16_kpad: fp32 W[K, n_out] -> bf16 Wt[n_out, Kp] with zero columns K..Kp-1 (Kp >= K); with W = kernel[0:E]
+ *   and Kp = Ep it is the B operand of gx_dir = mac_linear_tc_fwd(x_bf16, Wt, bias_dir, NON, gx_dir, 0, B*S, Ep, 4h).
+ * mac_lstm_fwd_tc: mac_lstm_fwd's recurrence and outputs (same saved-tensor layout) in ONE launch: per (direction, 64 batch
+ *   rows) a cluster of 8 CTAs keeps the bf16 recurrent weights in shared memory and runs the recurrent product of every
+ *   step on wgmma with bf16(h) as its operand.  Wh_dir is the fp32 kernel + E*4h.  Rows t >= len of out_seq and of the
+ *   saved tensors are written as zeros.  No workspace.
+ * mac_lstm_bwd_tc: the whole backward of the recurrence and the input projection: BPTT in one cluster launch, then
+ *   dkernel_dir [E+h, 4h] += [X | h_prev]^T dG (x_bf16 as mac_embed_fwd_tc wrote it, h_prev = bf16(save_hprev)),
+ *   dbias_dir [4h] += column sums of the fp32 gate gradients (fixed order), dx [B*S, E] = sum_dir dG_dir kernel_dir[0:E]^T
+ *   (the gradient w.r.t. dropout(X): feed it to mac_embed_bwd).  kernel_dir is the fp32 TF kernel [E+h, 4h].  The
+ *   workspace (mac_lstm_bwd_tc_workspace_bytes; 0 for an unsupported shape) need not be zeroed. */
+int mac_embed_fwd_tc(const float* emb, const int32_t* idx, float keep, uint64_t seed, int site, int step, float* out_raw,
+                     void* x_bf16, int B, int S, int V, int E, mac_stream_t stream);
+int mac_pack_weight_bf16_kpad(const float* W, void* Wt_bf16, int K, int Kp, int n_out, mac_stream_t stream);
+int mac_lstm_fwd_tc(const float* gx_fw, const float* gx_bw, const float* Wh_fw, const float* Wh_bw, const int32_t* lengths,
+                    float forget_bias, float* out_seq, float* vecq, float* save_gates, float* save_c, float* save_hprev,
+                    int B, int S, int h, int ndir, mac_stream_t stream);
+int mac_lstm_bwd_tc(const void* x_bf16, const float* kernel_fw, const float* kernel_bw, const int32_t* lengths,
+                    const float* save_gates, const float* save_c, const float* save_hprev, const float* d_out_seq,
+                    const float* d_vecq, float* dkernel_fw, float* dkernel_bw, float* dbias_fw, float* dbias_bw, float* dx,
+                    void* workspace, size_t workspace_bytes, int B, int S, int E, int h, int ndir, mac_stream_t stream);
+size_t mac_lstm_bwd_tc_workspace_bytes(int B, int S, int E, int h, int ndir);
 
 /* dropout sites (the `site` word of the Philox counter) */
 enum { MAC_SITE_MEM_VAR = 0, MAC_SITE_READ_KB = 1, MAC_SITE_READ_MEM = 2, MAC_SITE_READ_INTER = 3,

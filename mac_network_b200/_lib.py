@@ -109,6 +109,12 @@ PROTOTYPES = {
                              c_int, c_int, c_fp]),
     "mac_lstm_bwd": (c_int, [c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_sz, c_int, c_int, c_int, c_int,
                              c_fp]),
+    "mac_embed_fwd_tc": (c_int, [c_fp, c_fp, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_pack_weight_bf16_kpad": (c_int, [c_fp, c_fp, c_int, c_int, c_int, c_fp]),
+    "mac_lstm_fwd_tc": (c_int, [c_fp, c_fp, c_fp, c_fp, c_fp, c_f, c_fp, c_fp, c_fp, c_fp, c_fp, c_int, c_int, c_int, c_int,
+                                c_fp]),
+    "mac_lstm_bwd_tc": (c_int, [c_fp] * 15 + [c_sz, c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_lstm_bwd_tc_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int, c_int]),
     "mac_col2im3x3": (c_int, [c_fp, c_fp, c_f, c_u64, c_int, c_int, c_int, c_int, c_int, c_int, c_fp]),
     "mac_conv3x3_bwd_tc": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_fp, c_fp, c_sz,
                                    c_int, c_int, c_int, c_int, c_int, c_fp]),

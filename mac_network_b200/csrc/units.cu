@@ -7,6 +7,7 @@
 #include "read_step_fp8.cuh"
 #include "tc_gemm_fp8.cuh"
 #include "skinny_tc.cuh"
+#include "encoder_tc.cuh"
 
 using namespace mac;
 

@@ -36,7 +36,7 @@ class DPTrainer(object):
     def __init__(self, cfg, netLength, param_values=None, seed=0, rank=0, world=1, lr=1e-4, clip=8.0, ema_decay=0.999,
                  beta1=0.9, beta2=0.999, eps=1e-8, dropouts=None, device="cuda", classifier=None, output_dropout=0.85,
                  encoder=None, stem=None, enc_dropouts=(0.85, 0.92), stem_dropout=0.82, prec="fp32", bwd_tc=False,
-                 stem_prec="fp32"):
+                 stem_prec="fp32", enc_prec="fp32"):
         """`classifier=(answerWordsNum, outClassifierDims)` adds the reference's output unit + answer loss
         (model.py:512-528, 547-576, 593-596); `encoder=(vocabulary rows, wrdEmbDim)` the question input unit
         (model.py:208-220, 279-307) and `stem=(imageInDim, stemNumLayers)` the image stem (model.py:165-204), with the
@@ -45,7 +45,8 @@ class DPTrainer(object):
         `prec="bf16"` runs the read unit's forward projections on tensor cores in training too (activations saved in bf16,
         widened for the backward); `bwd_tc=True` runs its six backward products on tensor cores (`mac_read_bwd_tc`).
         `stem_prec="bf16"` trains the image stem on tensor cores too (forward `mac_linear_tc_fwd`, backward
-        `mac_conv3x3_bwd_tc`; every stem channel count must be a multiple of 128).
+        `mac_conv3x3_bwd_tc`; every stem channel count must be a multiple of 128).  `enc_prec="bf16"` trains the question
+        encoder's LSTM on tensor cores (`QuestionEncoder(prec="bf16")`; needs ctrlDim = 512, i.e. h = 256 per direction).
         All are mixed precision: bf16 operands, fp32 accumulation, fp32 master weights / gradients / optimizer state
         (DESIGN.md section 9)."""
         from .mac_cell import MACParams, views_of
@@ -58,8 +59,16 @@ class DPTrainer(object):
             if stem[0] % 128 or cfg.memDim % 128:
                 raise NotImplementedError("stem_prec='bf16' needs the image channels (%d) and memDim (%d) to be multiples of "
                                           "128 (the wgmma tiles of mac_conv3x3_bwd_tc)" % (stem[0], cfg.memDim))
+        if enc_prec not in ("fp32", "bf16"):
+            raise ValueError("enc_prec must be 'fp32' or 'bf16', got %r" % (enc_prec,))
+        if enc_prec != "fp32":
+            if encoder is None:
+                raise ValueError("enc_prec=%r needs encoder=" % (enc_prec,))
+            if cfg.ctrlDim != 512:
+                raise NotImplementedError("enc_prec='bf16' needs ctrlDim = 512 (h = 256 per LSTM direction), got %d"
+                                          % cfg.ctrlDim)
         self.cfg, self.L, self.rank, self.world = cfg, netLength, rank, world
-        self.prec, self.bwd_tc, self.stem_prec = prec, bool(bwd_tc), stem_prec
+        self.prec, self.bwd_tc, self.stem_prec, self.enc_prec = prec, bool(bwd_tc), stem_prec, enc_prec
         self.lib = _lib.load()
         extra_specs = extra_values = None
         if classifier is not None:
@@ -96,7 +105,8 @@ class DPTrainer(object):
             from .encoder import QuestionEncoder
             from .stem import Stem
             self.enc = QuestionEncoder({k: self.params.t[k] for k in self._enc_specs}, keep_input=enc_dropouts[0],
-                                       keep_question=enc_dropouts[1], seed=seed)
+                                       keep_question=enc_dropouts[1], seed=seed, prec=enc_prec,
+                                       version=lambda: self.params.version)
             self.stem = Stem({k: self.params.t[k] for k in self._stem_specs}, relu=cfg.relu, prec=stem_prec, seed=seed,
                              version=lambda: self.params.version)
             self.stem_dropout = float(stem_dropout)
@@ -243,6 +253,7 @@ class DPTrainer(object):
         self.apply()
         self.out.invalidate()
         self.stem._packed.clear()
+        self.enc._packed.clear()
         return logits, losses
 
     def train_step(self, key, batch, t_control, t_memory, global_batch):

@@ -12,7 +12,9 @@ optional `projCW` / `projQ` linears (`encProj`, or `encDim != ctrlDim`).
 GPU formulation (csrc/encoder.cu): the input half of both LSTM kernels is one GEMM each over all S steps
 (`mac_linear_fwd`), the recurrence is one launch per step for both directions with the gate math, the length masking and
 the backward direction's per-row time reversal fused behind the `[B,h] x [h,4h]` product; BPTT mirrors it and turns the
-weight / input gradients of all steps into GEMMs over the `[B*S, 4h]` gate-gradient matrix.  Variable names follow the
+weight / input gradients of all steps into GEMMs over the `[B*S, 4h]` gate-gradient matrix.  `prec="bf16"` runs every
+LSTM product on wgmma tensor cores (csrc/encoder_tc.cuh: bf16 operands, fp32 accumulation, state and element-wise math),
+the recurrence and BPTT as one persistent cluster launch each (h = 256 only).  Variable names follow the
 reference's scopes (`qEmbeddings/emb`, `encoder/birnnLayer/bidirectional_rnn/{fw,bw}/basic_lstm_cell/{kernel,bias}`)."""
 import collections
 import ctypes
@@ -27,6 +29,7 @@ SITE_ENC_INPUT = 48       # Philox sites of the encoder's two dropouts
 SITE_ENC_QUESTION = 49
 ENC = "encoder/birnnLayer/bidirectional_rnn/"
 ENC_UNI = "encoder/rnnLayer/rnn/"          # ops.fwRNNLayer (encBi off): scope "rnnLayer", dynamic_rnn's default "rnn"
+TC_H = 256                # the hidden size the tensor-core encoder supports
 
 
 def encoder_specs(vocab, wrd_emb_dim, enc_dim, ctrl_dim=None, bi=True, proj=False):
@@ -67,7 +70,14 @@ class QuestionEncoder(object):
     """Forward / backward of the question input unit on device tensors.  `params` (and `grads` for backward): dict
     TF-name -> CUDA fp32 tensor (e.g. views into the trainer's flat buckets)."""
 
-    def __init__(self, params, keep_input=1.0, keep_question=1.0, seed=0, forget_bias=1.0):
+    def __init__(self, params, keep_input=1.0, keep_question=1.0, seed=0, forget_bias=1.0, prec="fp32", version=None):
+        """`prec="bf16"`: the LSTM's products on tensor cores (DESIGN.md section 9 item 3); needs h = encDim / 2 = 256 (or
+        encDim = 256 without encBi).  `version`: optional callable returning a counter that changes whenever the parameter
+        values do (`MACParams.version`): the bf16 packs of kernel[0:E] are rebuilt when it moves, as in `Stem`.  The
+        `encProj` linears stay fp32."""
+        if prec not in ("fp32", "bf16"):
+            raise ValueError("QuestionEncoder prec must be 'fp32' or 'bf16', got %r" % (prec,))
+        self.prec = prec
         self.lib = _lib.load()
         self.p = params
         self.keep_input, self.keep_question, self.seed = float(keep_input), float(keep_question), int(seed)
@@ -83,6 +93,12 @@ class QuestionEncoder(object):
             raise ValueError("LSTM kernel rows do not match the embedding width")
         self.proj = "encoder/linearLayerprojCW/weights/weight" in params
         self.device = k0.device
+        if prec == "bf16" and self.h != TC_H:
+            raise NotImplementedError("the bf16 encoder needs h = %d hidden units per direction (encDim %d with encBi), got "
+                                      "h = %d; use prec='fp32'" % (TC_H, 2 * TC_H, self.h))
+        self.Ep = (self.E + 127) // 128 * 128          # E padded to whole 128-column tiles in the bf16 operands
+        self._packed = {}
+        self._version_fn, self._packed_version = version, None
         self._lws_bytes = 4096 + 32 * 64 * 4096 * 4
         self._lws = torch.zeros(self._lws_bytes, dtype=torch.uint8, device=self.device)
         self._saved = None
@@ -113,6 +129,45 @@ class QuestionEncoder(object):
                                       ptr(dW), ptr(db), xs[0].shape[0], dy.shape[1], ptr(self._lws), self._lws_bytes,
                                       stream_ptr()), "mac_linear_bwd")
 
+    def _wx_pack(self, i):
+        """bf16 [4h, Ep] pack of kernel[0:E] of direction i (zero columns E..Ep-1), cached per parameter version."""
+        v = self._version_fn() if self._version_fn is not None else None
+        if v != self._packed_version:
+            self._packed.clear()
+            self._packed_version = v
+        if i not in self._packed:
+            K = self.p[self.scopes[i] + "basic_lstm_cell/kernel"]
+            Wt = torch.empty((4 * self.h, self.Ep), dtype=torch.bfloat16, device=self.device)
+            check(self.lib.mac_pack_weight_bf16_kpad(ptr(K), ptr(Wt), self.E, self.Ep, 4 * self.h, stream_ptr()),
+                  "mac_pack_weight_bf16_kpad")
+            self._packed[i] = Wt
+        return self._packed[i]
+
+    def _lstm_bf16(self, qIndices, lengths, step, save_for_backward):
+        """Embedding + both LSTM directions on tensor cores: (words, x16, cntx, vecq, sg, sc, shp)."""
+        B, S = qIndices.shape
+        E, h, nd, M = self.E, self.h, self.ndir, qIndices.numel()
+        words = self._new(B, S, E)
+        x16 = torch.empty((M, self.Ep), dtype=torch.bfloat16, device=self.device)
+        check(self.lib.mac_embed_fwd_tc(ptr(self.p["qEmbeddings/emb"]), ptr(qIndices), self.keep_input, self.seed,
+                                        SITE_ENC_INPUT, step, ptr(words), ptr(x16), B, S, self.V, E, stream_ptr()),
+              "mac_embed_fwd_tc")
+        gx = []
+        for i, sc in enumerate(self.scopes):
+            g = self._new(M, 4 * h)
+            check(self.lib.mac_linear_tc_fwd(ptr(x16), ptr(self._wx_pack(i)), ptr(self.p[sc + "basic_lstm_cell/bias"]),
+                                             0, ptr(g), 0, M, self.Ep, 4 * h, stream_ptr()), "mac_linear_tc_fwd")
+            gx.append(g)
+        Wh = [self.p[sc + "basic_lstm_cell/kernel"][E:] for sc in self.scopes]
+        cntx, vecq = self._new(B, S, nd * h), self._new(B, nd * h)
+        sg = sc_ = shp = None
+        if save_for_backward:
+            sg, sc_, shp = self._new(nd, M, 4 * h), self._new(nd, M, h), self._new(nd, M, h)
+        check(self.lib.mac_lstm_fwd_tc(ptr(gx[0]), ptr(gx[1]) if nd == 2 else None, ptr(Wh[0]), ptr(Wh[1]) if nd == 2 else None,
+                                       ptr(lengths), self.forget_bias, ptr(cntx), ptr(vecq), ptr(sg), ptr(sc_), ptr(shp),
+                                       B, S, h, nd, stream_ptr()), "mac_lstm_fwd_tc")
+        return words, x16, cntx, vecq, sg, sc_, shp
+
     # ------------------------------------------------------------------ forward
     def forward(self, qIndices, questionLengths, step=0, save_for_backward=False):
         """qIndices int32 [B,S] (0 = padding), questionLengths int32 [B] (1 <= len <= S).
@@ -120,6 +175,14 @@ class QuestionEncoder(object):
         if not (qIndices.is_cuda and qIndices.dtype == torch.int32 and qIndices.is_contiguous()):
             raise ValueError("qIndices must be a contiguous CUDA int32 tensor")
         lengths = questionLengths.to(torch.int32).contiguous()
+        ws = wsb = None
+        if self.prec == "bf16":
+            words, x2, cntx, vecq, sg, sc_, shp = self._lstm_bf16(qIndices, lengths, step, save_for_backward)
+        else:
+            words, x2, cntx, vecq, sg, sc_, shp, ws, wsb = self._lstm_fp32(qIndices, lengths, step, save_for_backward)
+        return self._finish(words, x2, cntx, vecq, sg, sc_, shp, ws, wsb, qIndices, lengths, step, save_for_backward)
+
+    def _lstm_fp32(self, qIndices, lengths, step, save_for_backward):
         B, S = qIndices.shape
         E, h, nd = self.E, self.h, self.ndir
         words = self._new(B, S, E)
@@ -143,6 +206,11 @@ class QuestionEncoder(object):
         check(self.lib.mac_lstm_fwd(ptr(gx[0]), ptr(gx[1]) if nd == 2 else None, ptr(Wh[0]), ptr(Wh[1]) if nd == 2 else None,
                                     ptr(lengths), self.forget_bias, ptr(cntx), ptr(vecq), ptr(sg), ptr(sc_), ptr(shp),
                                     ptr(ws), wsb, B, S, h, nd, stream_ptr()), "mac_lstm_fwd")
+        return words, x2, cntx, vecq, sg, sc_, shp, ws, wsb
+
+    def _finish(self, words, x2, cntx, vecq, sg, sc_, shp, ws, wsb, qIndices, lengths, step, save_for_backward):
+        B, S = qIndices.shape
+        nd, h = self.ndir, self.h
         if self.keep_question < 1.0:                                                       # model.py:297
             check(self.lib.mac_dropout_fwd(ptr(vecq), self.keep_question, self.seed, SITE_ENC_QUESTION, step, ptr(vecq),
                                            vecq.numel(), stream_ptr()), "mac_dropout_fwd")
@@ -181,6 +249,22 @@ class QuestionEncoder(object):
                                            ptr(dq), dq.numel(), stream_ptr()), "mac_dropout_fwd")
             d_vecq = dq
         Ks = [self.p[sc + "basic_lstm_cell/kernel"] for sc in self.scopes]
+        if self.prec == "bf16":
+            M = B * S
+            dx = self._new(M, E)
+            gk = [grads[sc + "basic_lstm_cell/kernel"] for sc in self.scopes]
+            gb = [grads[sc + "basic_lstm_cell/bias"] for sc in self.scopes]
+            two = nd == 2
+            wsb = int(self.lib.mac_lstm_bwd_tc_workspace_bytes(B, S, E, h, nd))
+            ws = torch.empty(wsb, dtype=torch.uint8, device=self.device)
+            check(self.lib.mac_lstm_bwd_tc(ptr(sv["x2"]), ptr(Ks[0]), ptr(Ks[1]) if two else None, ptr(sv["lengths"]),
+                                           ptr(sv["sg"]), ptr(sv["sc"]), ptr(sv["shp"]), ptr(d_cntx), ptr(d_vecq),
+                                           ptr(gk[0]), ptr(gk[1]) if two else None, ptr(gb[0]), ptr(gb[1]) if two else None,
+                                           ptr(dx), ptr(ws), wsb, B, S, E, h, nd, stream_ptr()), "mac_lstm_bwd_tc")
+            check(self.lib.mac_embed_bwd(ptr(dx), ptr(sv["qIndices"]), self.keep_input, self.seed, SITE_ENC_INPUT,
+                                         sv["step"], ptr(grads["qEmbeddings/emb"]), B, S, self.V, E, stream_ptr()),
+                  "mac_embed_bwd")
+            return
         dG = [self._new(B * S, 4 * h) for _ in range(nd)]
         check(self.lib.mac_lstm_bwd(ptr(Ks[0][E:]), ptr(Ks[1][E:]) if nd == 2 else None, ptr(sv["lengths"]), ptr(sv["sg"]),
                                     ptr(sv["sc"]), ptr(d_cntx), ptr(d_vecq), ptr(dG[0]), ptr(dG[1]) if nd == 2 else None,

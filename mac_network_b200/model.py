@@ -34,13 +34,17 @@ from .stem import Stem
 class MACnet(object):
     def __init__(self, cfg, netLength, vocab, n_answers, wrd_emb_dim=300, image_in_dim=1024, classifier_dims=(512,),
                  stem_layers=2, seed=0, rank=0, world=1, lr=1e-4, prec="bf16", use_ema=False, answer_decoder=None,
-                 device="cuda", eval_stem_prec=None, **trainer_kw):
+                 device="cuda", eval_stem_prec=None, eval_enc_prec=None, **trainer_kw):
         """`vocab`: rows of the question-embedding variable (ids 1..vocab; 0 is padding); `answer_decoder`: optional
         id -> answer string (`answerDict.decodeId`, model.py:699).  `prec`: arithmetic of the evaluation forward; with
         "fp8" the cell's read step runs on e4m3 and the image stem in bf16.  `eval_stem_prec="fp8"` runs the evaluation
-        stem in e4m3 (`Stem(prec="fp8")`) whatever `prec` is; None keeps the stem `prec` implies.  Training is unaffected."""
+        stem in e4m3 (`Stem(prec="fp8")`) whatever `prec` is; None keeps the stem `prec` implies.  `eval_enc_prec="bf16"` runs
+        the evaluation question encoder on tensor cores (`QuestionEncoder(prec="bf16")`); None keeps it fp32.  Training is
+        unaffected (see `DPTrainer(enc_prec=)`)."""
         if eval_stem_prec not in (None, "fp8"):
             raise ValueError("eval_stem_prec must be None or 'fp8', got %r" % (eval_stem_prec,))
+        if eval_enc_prec not in (None, "bf16"):
+            raise ValueError("eval_enc_prec must be None or 'bf16', got %r" % (eval_enc_prec,))
         self.cfg, self.L, self.prec, self.use_ema = cfg, netLength, prec, bool(use_ema)
         self.decode = answer_decoder
         self.trainer = DPTrainer(cfg, netLength, seed=seed, rank=rank, world=world, lr=lr, device=device,
@@ -49,7 +53,8 @@ class MACnet(object):
         p = self.trainer.params
         t = self.trainer
         # evaluation-mode views of the same variables: every dropout at 1.0 (model.py:118-125)
-        self._enc = QuestionEncoder({k: p.t[k] for k in t._enc_specs}, keep_input=1.0, keep_question=1.0)
+        self._enc = QuestionEncoder({k: p.t[k] for k in t._enc_specs}, keep_input=1.0, keep_question=1.0,
+                                    prec=eval_enc_prec or "fp32", version=lambda: p.version)
         stem_prec = eval_stem_prec or ("bf16" if prec == "fp8" else prec)
         self._stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=stem_prec, version=lambda: p.version)
         self._out = OutputUnit({k: p.t[k] for k in p.specs if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu,
@@ -100,6 +105,7 @@ class MACnet(object):
         t.params.touch()
         self._out.invalidate()
         self._stem._packed.clear()
+        self._enc._packed.clear()
 
     # ------------------------------------------------------------------ model.py:732-760
     def runBatch(self, sess, data, images, train, getAtt=False):
@@ -116,6 +122,7 @@ class MACnet(object):
             gradNorm = float(t.norm[0].item())
             self._out.invalidate()
             self._stem._packed.clear()
+            self._enc._packed.clear()
         else:
             if self.use_ema:
                 self._swap_ema()
