@@ -317,6 +317,25 @@ int mac_read_bwd_tc(const float* kb, const float* memory_in, const float* contro
                     float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2, float* dbm2_part, float* dwr_part,
                     float* dbr_part, void* workspace, size_t workspace_bytes, int B, int N, int d, mac_stream_t stream);
 size_t mac_read_bwd_tc_workspace_bytes(int B, int N, int d);
+/* ops.linear on tensor cores for the [B*N, .] products of the composed read unit (csrc/linear_tc.cuh; MACCell(prec="bf16")
+ * with read-unit flags outside mac_read_fwd): bf16 operands (round to nearest even), fp32 accumulation, fp32 in / fp32 out.
+ * mac_linear_tc_seg_fwd: mac_linear_fwd's y[M, n_out] = act(concat(x_0 .. x_{nseg-1}) @ W + b + bias_const) with W given as
+ *   the packed bf16 Wt [n_out, K] (mac_pack_weight_bf16); b may be NULL; act any MAC_ACT_*.  The segments are cast into one
+ *   bf16 [M, K] operand in the workspace (mac_linear_tc_seg_workspace_bytes(M, K), K = sum k_segs).
+ * mac_linear_bwd_tc: mac_linear_bwd's arguments and accumulation conventions, except that W is the fp32 weight [K, n_out] in
+ *   its own layout (not its transpose): dx_s (+)= bf16(dy) @ bf16(W_s)^T (dx_accum[s]); dW [K, n_out] += bf16(x)^T @ bf16(dy)
+ *   (split-K over M rounded up to 64); db [n_out] += colsum(dy) in a fixed order (needs ldy == n_out).  Reruns are
+ *   bit-identical.  Workspace: mac_linear_bwd_tc_workspace_bytes(M, k_segs, nseg, n_out), need not be zeroed.
+ * Both need every k_segs[i] and n_out to be multiples of 128 (any M >= 1), else MAC_ERR_UNSUPPORTED; all checks precede any
+ * launch. */
+int mac_linear_tc_seg_fwd(const float* const* x_segs, const int* k_segs, const int* ldx, int nseg, const void* wt_bf16,
+                          const float* b, float bias_const, int act, float* y, int ldy, int M, int n_out,
+                          void* workspace, size_t workspace_bytes, mac_stream_t stream);
+size_t mac_linear_tc_seg_workspace_bytes(int M, int K);
+int mac_linear_bwd_tc(const float* const* x_segs, const int* k_segs, const int* ldx, int nseg, const float* W,
+                      const float* dy, int ldy, float* const* dx_segs, const int* ld_dx, const int* dx_accum,
+                      float* dW, float* db, int M, int n_out, void* workspace, size_t workspace_bytes, mac_stream_t stream);
+size_t mac_linear_bwd_tc_workspace_bytes(int M, const int* k_segs, int nseg, int n_out);
 /* write gate (mac_cell.py:358-367): dmnew = g*z; dmprev += g*(1-z); dpre = g*(mnew-mprev)*z*(1-z) */
 int mac_gate_bwd(const float* g, const float* z, const float* mnew, const float* mprev, float* dmnew, float* dmprev,
                  float* dpre, long long n, mac_stream_t stream);

@@ -126,6 +126,13 @@ PROTOTYPES = {
     "mac_linear_tc_small_fwd": (c_int, [ctypes.POINTER(c_fp), ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_fp, c_fp,
                                         c_fp, c_f, c_int, c_fp, c_int, c_fp, c_int, c_fp, c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_linear_tc_fwd": (c_int, [c_fp, c_fp, c_fp, c_int, c_fp, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_linear_tc_seg_fwd": (c_int, [ctypes.POINTER(c_fp), ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_fp, c_fp,
+                                      c_f, c_int, c_fp, c_int, c_int, c_int, c_fp, c_sz, c_fp]),
+    "mac_linear_tc_seg_workspace_bytes": (c_sz, [c_int, c_int]),
+    "mac_linear_bwd_tc": (c_int, [ctypes.POINTER(c_fp), ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_int, c_fp, c_fp, c_int,
+                                  ctypes.POINTER(c_fp), ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_fp, c_fp, c_int, c_int,
+                                  c_fp, c_sz, c_fp]),
+    "mac_linear_bwd_tc_workspace_bytes": (c_sz, [c_int, ctypes.POINTER(c_int), c_int, c_int]),
 }
 
 _lib = None

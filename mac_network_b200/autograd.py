@@ -305,6 +305,11 @@ def mac_backward(cell, d_control, d_memory, bucket=None, zero_bucket=True, d_vec
         raise RuntimeError("construct the MACCell with save_for_backward=True and run the forward first")
     if getattr(cell, "_tape", None) is not None:       # flags outside the hand-scheduled sweep: node-by-node (tape.py)
         if tc:
-            raise NotImplementedError("the tape backward runs the fp32 kernels")
-        return cell._tape.run(d_control, d_memory, bucket, zero_bucket, d_vecq)
+            # tensor cores on the tape: the composed read unit's [B*N, .] linears (mac_linear_bwd_tc, any B*N) and the fused
+            # read unit (mac_read_bwd_tc); everything else on the tape stays on its fp32 kernels
+            if cell.prec != _lib.PREC["bf16"]:
+                raise NotImplementedError("the tape backward runs the fp32 kernels")
+            if cell._fused_read and (cell.d % 128 or (cell.B * cell.N) % 64):
+                raise NotImplementedError("tensor-core backward needs d % 128 == 0 and (B*N) % 64 == 0")
+        return cell._tape.run(d_control, d_memory, bucket, zero_bucket, d_vecq, tc=tc)
     return _Bwd(cell, bucket, zero_bucket, tc=tc).run(d_control, d_memory, d_vecq)

@@ -16,7 +16,7 @@
 //   TC_EPI_ACT     act(acc + b)            -> bf16                               (mac_cell.py:236-238)
 //   TC_EPI_LOGITS  I1 = acc + bm2; t = ELU(I1 * control[b]); (dropout); parts[m, ntile] = sum_n t * wr[n]
 //                                                                                (ops.py:325-328, mac_cell.py:248-266)
-//   TC_EPI_F32     act(acc + b)            -> fp32                               (generic ops.linear)
+//   TC_EPI_F32     act(acc + b + bias_const) -> fp32, stored or added (accum)   (generic ops.linear; act in every MAC_ACT_*)
 //   TC_EPI_ADDACT  act(acc + b + add[m,n]) -> bf16, add = bf16 [M, N]           (eval-mode read: step-invariant half of
 //                                                                                 the memKbProj concat, mac_cell.py:236-238)
 //   TC_EPI_ACT_SPLIT  x = act(acc + b + addf[m,n]) (addf fp32, optional) -> bf16 hi at out0[m, n] and bf16 lo = x - hi at
@@ -53,6 +53,8 @@ struct TcGemmParams {
   int e_site, step;
   int ksplit;              // split-K (TC_EPI_F32 only): the K range is cut into `ksplit` equal slices (grid z), each writing
   long long split_stride;  //   its fp32 partial to outf + slice * split_stride; 0 / 1 = off
+  float bias_const;        // TC_EPI_F32: added to every pre-activation (ops.linear's bias_const, mac_linear_fwd)
+  int accum;               // TC_EPI_F32: outf (+)= act(...) -- the data gradients of mac_linear_bwd_tc with dx_accum
 };
 
 // ------------------------------------------------------------------ wgmma PTX wrappers
@@ -280,7 +282,19 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
               pack_bf16(x0 - __uint_as_float(hw << 16), x1 - __uint_as_float(hw & 0xffff0000u));
         }
       } else if constexpr (EPI == TC_EPI_F32) {
-        if (row_ok) *reinterpret_cast<float2*>(outf_t + o) = make_float2(act_ct<ACT>(x0), act_ct<ACT>(x1));
+        if (row_ok) {
+          if (p.bias_const != 0.f) {
+            x0 += p.bias_const;
+            x1 += p.bias_const;
+          }
+          float2 v = make_float2(act_ct<ACT>(x0), act_ct<ACT>(x1));
+          if (p.accum) {
+            const float2 prev = *reinterpret_cast<const float2*>(outf_t + o);
+            v.x += prev.x;
+            v.y += prev.y;
+          }
+          *reinterpret_cast<float2*>(outf_t + o) = v;
+        }
       } else {  // TC_EPI_LOGITS
         const float2 cc = __ldg(reinterpret_cast<const float2*>(p.ctrl + (size_t)bidx * p.N + n));
         const float2 ww = make_float2(__ldg(p.wr + n), __ldg(p.wr + n + 1));
@@ -397,11 +411,13 @@ __global__ void pack_weight_bf16_kernel(const float* __restrict__ W, __nv_bfloat
 // data gradient) from the same read.  64x64 tiles: 256-byte row reads, 128-byte row writes.
 //   MODE 0 plain; 1 x * rowvec[row / rows_per_batch, col] (P * y, ops.py:694-703); 2 dropout(x) with the forward's Philox stream
 //   (one draw per aligned column quad, element index row*N + col: mac_dropout_fwd's numbering).      N % 4 == 0, K % 2 == 0.
+// ldx is the row pitch of X (elements); Xt rows have pitch ldt >= K, and columns K..ldt-1 of Xt are written as zeros (a
+// contraction length padded to the 64-wide k-block).
 template <int MODE>
 __global__ void __launch_bounds__(256) pack_t_bf16_kernel(const float* __restrict__ X, __nv_bfloat16* __restrict__ Xt,
                                                          __nv_bfloat16* __restrict__ Xrm, int K, int N,
                                                          const float* __restrict__ rowvec, int rows_per_batch, uint32_t thresh,
-                                                         float scale, uint64_t seed, int site, int step) {
+                                                         float scale, uint64_t seed, int site, int step, int ldx, int ldt) {
   __shared__ float tile[64][65];                              // [col][row]
   const int k0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
   const int tq = threadIdx.x & 15, tr = threadIdx.x >> 4;     // 16 column quads x 16 rows per pass
@@ -411,7 +427,7 @@ __global__ void __launch_bounds__(256) pack_t_bf16_kernel(const float* __restric
     const int k = k0 + kk, n = n0 + tq * 4;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (k < K && n < N) {
-      v = *reinterpret_cast<const float4*>(X + (size_t)k * N + n);
+      v = *reinterpret_cast<const float4*>(X + (size_t)k * ldx + n);
       if (MODE == 1) {
         const float4 y = *reinterpret_cast<const float4*>(rowvec + (size_t)(k / rows_per_batch) * N + n);
         v.x *= y.x; v.y *= y.y; v.z *= y.z; v.w *= y.w;
@@ -435,8 +451,8 @@ __global__ void __launch_bounds__(256) pack_t_bf16_kernel(const float* __restric
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int r = warp; r < 64; r += 8) {
     const int n = n0 + r, k = k0 + 2 * lane;
-    if (n < N && k + 1 < K)
-      *reinterpret_cast<uint32_t*>(Xt + (size_t)n * K + k) = pack_bf16(tile[r][2 * lane], tile[r][2 * lane + 1]);
+    if (n < N && k + 1 < ldt)
+      *reinterpret_cast<uint32_t*>(Xt + (size_t)n * ldt + k) = pack_bf16(tile[r][2 * lane], tile[r][2 * lane + 1]);
   }
 }
 
@@ -449,18 +465,22 @@ struct PackTArgs {
   int site = 0, step = 0;
 };
 
+// ldx: row pitch of X (0: N); ldt: row pitch of Xt (0: K), >= K and even -- columns K..ldt-1 are written as zeros
 inline int pack_t_bf16_launch(int mode, const float* X, void* Xt, void* Xrm, int K, int N, const PackTArgs& a,
-                              cudaStream_t stream) {
-  if (!X || !Xt || K <= 0 || N <= 0 || (N & 3) || (K & 1)) return MAC_ERR_INVALID;
-  dim3 grid((N + 63) / 64, (K + 63) / 64);
+                              cudaStream_t stream, int ldx = 0, int ldt = 0) {
+  if (ldx == 0) ldx = N;
+  if (ldt == 0) ldt = K;
+  if (!X || !Xt || K <= 0 || N <= 0 || (N & 3) || (ldx & 3) || ldx < N || (ldt & 1) || ldt < K) return MAC_ERR_INVALID;
+  dim3 grid((N + 63) / 64, (ldt + 63) / 64);
   __nv_bfloat16* t = reinterpret_cast<__nv_bfloat16*>(Xt);
   __nv_bfloat16* r = reinterpret_cast<__nv_bfloat16*>(Xrm);
   if (mode == 0)
-    pack_t_bf16_kernel<0><<<grid, 256, 0, stream>>>(X, t, r, K, N, nullptr, 1, 0u, 1.f, 0, 0, 0);
+    pack_t_bf16_kernel<0><<<grid, 256, 0, stream>>>(X, t, r, K, N, nullptr, 1, 0u, 1.f, 0, 0, 0, ldx, ldt);
   else if (mode == 1)
-    pack_t_bf16_kernel<1><<<grid, 256, 0, stream>>>(X, t, r, K, N, a.rowvec, a.rows_per_batch, 0u, 1.f, 0, 0, 0);
+    pack_t_bf16_kernel<1><<<grid, 256, 0, stream>>>(X, t, r, K, N, a.rowvec, a.rows_per_batch, 0u, 1.f, 0, 0, 0, ldx, ldt);
   else
-    pack_t_bf16_kernel<2><<<grid, 256, 0, stream>>>(X, t, r, K, N, nullptr, 1, a.thresh, a.scale, a.seed, a.site, a.step);
+    pack_t_bf16_kernel<2><<<grid, 256, 0, stream>>>(X, t, r, K, N, nullptr, 1, a.thresh, a.scale, a.seed, a.site, a.step, ldx,
+                                                    ldt);
   MAC_LAUNCH_CHECK();
   return MAC_OK;
 }

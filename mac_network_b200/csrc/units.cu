@@ -8,6 +8,7 @@
 #include "tc_gemm_fp8.cuh"
 #include "skinny_tc.cuh"
 #include "encoder_tc.cuh"
+#include "linear_tc.cuh"
 
 using namespace mac;
 

@@ -44,6 +44,10 @@ class DPTrainer(object):
         all-reduce and the one fused optimizer pass cover the whole model (`train_step_full`).
         `prec="bf16"` runs the read unit's forward projections on tensor cores in training too (activations saved in bf16,
         widened for the backward); `bwd_tc=True` runs its six backward products on tensor cores (`mac_read_bwd_tc`).
+        Both hold for every working flag combination, not only the shipped flag files: with read-unit flags outside the
+        fused kernel the composed read unit's [B*N, .] products run on `mac_linear_tc_seg_fwd` / `mac_linear_bwd_tc`
+        (memDim and attDim multiples of 128), and a cell differentiated on the tape (`tape.py`) runs its fused read unit
+        backward on `mac_read_bwd_tc` (B*N a multiple of 64); the batch-sized products stay fp32 (DESIGN.md section 9).
         `stem_prec="bf16"` trains the image stem on tensor cores too (forward `mac_linear_tc_fwd`, backward
         `mac_conv3x3_bwd_tc`; every stem channel count must be a multiple of 128).  `enc_prec="bf16"` trains the question
         encoder's LSTM on tensor cores (`QuestionEncoder(prec="bf16")`; needs ctrlDim = 512, i.e. h = 256 per direction).

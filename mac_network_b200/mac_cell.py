@@ -218,13 +218,20 @@ class MACCell(object):
         self._use_tape = self.save_for_backward and (not scheduled_bwd_ok or tape_bwd)
         self._tape = None
         if self._use_tape:
-            if self.prec != PREC["fp32"]:
+            if self.prec not in (PREC["fp32"], PREC["bf16"]):
                 raise NotImplementedError("the tape backward (flags outside the shipped files) runs the fp32 kernels")
             self._hoist = False              # per-step control(): every launch is a tape node
         if self.save_for_backward and self.prec != PREC["fp32"] and (d % 128 or self._kb_given_bf16):
             raise NotImplementedError("training forward on tensor cores needs d % 128 == 0 and an fp32 knowledge base")
-        if self.prec != PREC["fp32"] and not self._fused_read:
+        if self.prec not in (PREC["fp32"], PREC["bf16"]) and not self._fused_read:
             raise NotImplementedError("the tensor-core projections cover the fused read unit only")
+        # bf16 with the composed read unit (read flags outside the fused kernel): its [B*N, .] products run on tensor cores
+        # (mac_linear_tc_seg_fwd), whose widths (memDim, attDim) must fill whole 128-wide wgmma tiles
+        self._tc_general = self.prec == PREC["bf16"] and not self._fused_read
+        if self._tc_general and (d % 128 or c.attDim % 128):
+            raise NotImplementedError('prec="bf16" with the composed read unit needs d %% 128 == 0 and attDim %% 128 == 0 '
+                                      "(got d = %d, attDim = %d)" % (d, c.attDim))
+        self._lin_tc_ws = None
         if self.prec == PREC["tc32"] and (save_for_backward or not self._read_hoist or float(readDropout) < 1.0 or d % 128):
             raise NotImplementedError('prec="tc32" (split-bf16 tensor-core projections inside the 1e-4 bar) is the inference '
                                       "form of the fused read unit: shared cells, readDropout = 1, d % 128 == 0")
@@ -246,20 +253,39 @@ class MACCell(object):
         return 1                                                     # mac_cell.py:91-93
 
     # ------------------------------------------------------------------ thin wrappers over the C ABI
-    def _linear(self, xs, W, b, out, act="NON", bias_const=0.0):
-        """ops.linear (ops.py:298-333) on [M, sum k] segments; `xs` is a list of 2-D row-major views."""
+    def _linear(self, xs, W, b, out, act="NON", bias_const=0.0, bn_rows=False):
+        """ops.linear (ops.py:298-333) on [M, sum k] segments; `xs` is a list of 2-D row-major views.  `bn_rows`: a product
+        of the composed read unit over the B*N knowledge-base rows -- on tensor cores with prec="bf16"."""
         n = len(xs)
         M = xs[0].shape[0]
         arr_p = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
         arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
         arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
         code = ACT["ELU"] if (act == "RELU" and self.cfg.relu == "ELU") else ACT["RELU_STD"] if act == "RELU" else ACT[act]
-        check(self.lib.mac_linear_fwd(arr_p, arr_k, arr_ld, n, ptr(W), ptr(b), float(bias_const), code, ptr(out),
-                                      out.stride(0), M, W.shape[1], ptr(self.ws.lin), self.ws.lin_bytes, stream_ptr()),
-              "mac_linear_fwd")
+        if bn_rows and self._tc_general:
+            K = sum(x.shape[1] for x in xs)
+            need = int(self.lib.mac_linear_tc_seg_workspace_bytes(M, K))
+            if self._lin_tc_ws is None or self._lin_tc_ws.numel() < need:
+                self._lin_tc_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            check(self.lib.mac_linear_tc_seg_fwd(arr_p, arr_k, arr_ld, n, ptr(self._bf16_weight(W)), ptr(b),
+                                                 float(bias_const), code, ptr(out), out.stride(0), M, W.shape[1],
+                                                 ptr(self._lin_tc_ws), self._lin_tc_ws.numel(), stream_ptr()),
+                  "mac_linear_tc_seg_fwd")
+        else:
+            check(self.lib.mac_linear_fwd(arr_p, arr_k, arr_ld, n, ptr(W), ptr(b), float(bias_const), code, ptr(out),
+                                          out.stride(0), M, W.shape[1], ptr(self.ws.lin), self.ws.lin_bytes, stream_ptr()),
+                  "mac_linear_fwd")
         if self._tape is not None:
-            self._tape.linear(xs, W, b, out, code)
+            self._tape.linear(xs, W, b, out, code, bn_rows=bn_rows)
         return out
+
+    def _bf16_weight(self, W):
+        """bf16 [out, in] pack of an fp32 [in, out] weight (mac_pack_weight_bf16), cached per parameter version."""
+        def pack():
+            o = torch.empty((W.shape[1], W.shape[0]), dtype=torch.bfloat16, device=W.device)
+            check(self.lib.mac_pack_weight_bf16(ptr(W), ptr(o), W.shape[0], W.shape[1], stream_ptr()), "pack")
+            return o
+        return self.params.derived(("bf16lin", W.data_ptr()), pack)
 
     def _split_weight(self, key, W):
         """bf16 hi / lo halves [out, in] of an fp32 [in, out] weight (mac_pack_weight_bf16_split), cached per parameter version."""
@@ -343,7 +369,7 @@ class MACCell(object):
         self._gate = self._new(L, B, d) if c.writeGate else None
         if self._kb_given_bf16:
             self.kb_bf16 = self.knowledgeBase
-        elif self.prec in (PREC["bf16"], PREC["fp8"]):
+        elif self.prec in (PREC["bf16"], PREC["fp8"]) and self._fused_read:
             self.kb_bf16 = torch.empty(self.knowledgeBase.shape, dtype=torch.bfloat16, device=self.device)
             check(self.lib.mac_cast_bf16(ptr(self.knowledgeBase), ptr(self.kb_bf16), self.knowledgeBase.numel(),
                                          stream_ptr()), "mac_cast_bf16")
@@ -663,13 +689,13 @@ class MACCell(object):
     def _act_code(self, act):
         return ACT["ELU"] if (act == "RELU" and self.cfg.relu == "ELU") else ACT["RELU_STD"] if act == "RELU" else ACT[act]
 
-    def _ops_linear(self, xs, scope, name, act="NON", bias_const=0.0):
+    def _ops_linear(self, xs, scope, name, act="NON", bias_const=0.0, bn_rows=False):
         """ops.linear incl. the nested "<name>_2" layer when act != NON (ops.py:298-333); xs: list of 2-D segments."""
         W, b = self.params.lin(scope, name)
-        y = self._linear(xs, W, b, self._new(xs[0].shape[0], W.shape[1]), act=act, bias_const=bias_const)
+        y = self._linear(xs, W, b, self._new(xs[0].shape[0], W.shape[1]), act=act, bias_const=bias_const, bn_rows=bn_rows)
         if act != "NON":
             W2, b2 = self.params.lin(scope + "linearLayer" + name + "/", name + "_2")
-            y = self._linear([y], W2, b2, self._new(y.shape[0], W2.shape[1]))
+            y = self._linear([y], W2, b2, self._new(y.shape[0], W2.shape[1]), bn_rows=bn_rows)
         return y
 
     def _rowdot(self, xs, lscope):
@@ -722,14 +748,14 @@ class MACCell(object):
                 x2d = self._dropout(x2d, proj["dropout"], _lib.SITE_READ_KB, i, self._new(*x2d.shape))
                 y = self._dropout(y, proj["dropout"], _lib.SITE_READ_MEM, i, self._new(*y.shape))
             xn, yn = ("proj", "proj") if proj["shared"] else ("projX", "projY")
-            x2d = self._ops_linear([x2d], sc, xn)
+            x2d = self._ops_linear([x2d], sc, xn, bn_rows=True)
             y = self._ops_linear([y], sc, yn)
             proj_x = x2d
         if inter_mod == "MUL":
             inter = self._bcast(x2d, y, 0, N)
         elif inter_mod == "BL":
             W, b = self.params[sc + "weights/weight"], self.params[sc + "biases/bias"]
-            xw = self._linear([x2d], W, None, self._new(x2d.shape[0], W.shape[1]))
+            xw = self._linear([x2d], W, None, self._new(x2d.shape[0], W.shape[1]), bn_rows=True)
             inter = self._bcast(xw, y, 1, N, bias=b)
         else:  # ADD
             inter = self._bcast(x2d, y, 2, N)
@@ -748,7 +774,7 @@ class MACCell(object):
         segs, projectedKB = self._mul_general(kb2, memory, c.memDim, N, sc, "memInter", proj, c.readMemAttType,
                                               c.readMemConcatKB, c.readMemConcatProj)
         if c.readMemProj:
-            segs = [self._ops_linear(segs, sc, "memKbProj", act=c.readMemAct)]
+            segs = [self._ops_linear(segs, sc, "memKbProj", act=c.readMemAct, bn_rows=True)]
         if c.readCtrl:
             segs, _ = self._mul_general(segs[0], control, 0, N, sc, "ctrlInter", None, c.readCtrlAttType, False, False)
             if c.readCtrlConcatKB:

@@ -33,6 +33,8 @@ class Tape(object):
         self.g = None
         self.lws_bytes = 4096 + 32 * 4 * max(int(t.numel()) for t in self.p.t.values())
         self.lws = None
+        self.tc = False              # run(tc=True): the [B*N, .] products of the backward on tensor cores
+        self._tcws = None
 
     # ------------------------------------------------------------------ buffers
     def z(self, *shape):
@@ -89,9 +91,26 @@ class Tape(object):
                                       ptr(self.G(wname)), ptr(self.G(bname)) if bname else None, M, n_out,
                                       ptr(self.lws), self.lws_bytes, stream_ptr()), "mac_linear_bwd")
 
+    def linear_bwd_tc(self, xs, W, wname, bname, dy, dxs):
+        """linear_bwd with bf16 operands on tensor cores (mac_linear_bwd_tc): the composed read unit's [B*N, .] products."""
+        n = len(xs)
+        M, n_out = dy.shape
+        arr_x = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
+        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
+        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
+        arr_dx = (ctypes.c_void_p * n)(*[d.data_ptr() for d in dxs])
+        arr_ldd = (ctypes.c_int * n)(*[d.stride(0) for d in dxs])
+        arr_acc = (ctypes.c_int * n)(*[1] * n)
+        need = int(self.lib.mac_linear_bwd_tc_workspace_bytes(M, arr_k, n, n_out))
+        if self._tcws is None or self._tcws.numel() < need:
+            self._tcws = torch.empty(need, dtype=torch.uint8, device=self.dev)
+        check(self.lib.mac_linear_bwd_tc(arr_x, arr_k, arr_ld, n, ptr(W), ptr(dy), dy.stride(0), arr_dx, arr_ldd, arr_acc,
+                                         ptr(self.G(wname)), ptr(self.G(bname)) if bname else None, M, n_out,
+                                         ptr(self._tcws), self._tcws.numel(), stream_ptr()), "mac_linear_bwd_tc")
+
     # ------------------------------------------------------------------ recorders (called from the forward)
-    def linear(self, xs, W, b, out, code):
-        """y = act(concat(xs) @ W + b)   (ops.py:298-333)"""
+    def linear(self, xs, W, b, out, code, bn_rows=False):
+        """y = act(concat(xs) @ W + b)   (ops.py:298-333); bn_rows: a [B*N, .] product of the composed read unit"""
         xs = list(xs)
         wname = self.name_of(W)
         bname = self.name_of(b) if b is not None else None
@@ -102,7 +121,10 @@ class Tape(object):
             if code != ACT["NON"]:
                 dpre = self.e(*out.shape)
                 check(self.lib.mac_activation_bwd(ptr(out), ptr(g), code, ptr(dpre), out.numel(), stream_ptr()), "act bwd")
-            self.linear_bwd(xs, W, wname, bname, dpre, [self.grad(x) for x in xs])
+            if bn_rows and self.tc:
+                self.linear_bwd_tc(xs, W, wname, bname, dpre, [self.grad(x) for x in xs])
+            else:
+                self.linear_bwd(xs, W, wname, bname, dpre, [self.grad(x) for x in xs])
         self.add(bwd)
 
     def act(self, x, out, code):
@@ -255,7 +277,8 @@ class Tape(object):
         self.finalizers.append(fin)
 
     def fused_read(self, i, name, knowledgeBase, memory_in, control, info):
-        """mac_read_fwd with the activations saved in cell._save[i] -> mac_read_bwd (csrc/backward.cu)."""
+        """mac_read_fwd with the activations saved in cell._save[i] -> mac_read_bwd (csrc/backward.cu), or mac_read_bwd_tc
+        (its six [B*N, .] products on tensor cores) when the sweep runs with tc=True."""
         cell = self.cell
         B, N, d = cell.B, cell.N, cell.d
         rsc = "MACCell/read" + name + "/"
@@ -275,17 +298,27 @@ class Tape(object):
             part = {k: self.z(B, d) for k in ("wr", "bx", "bm", "bm2")}
             dbr = self.z(B)
             dmem_in = self.e(B, d)
-            ws_bytes = int(self.lib.mac_read_bwd_workspace_bytes(B, N, d))
+            ws_bytes = int((self.lib.mac_read_bwd_tc_workspace_bytes if self.tc else self.lib.mac_read_bwd_workspace_bytes)(
+                B, N, d))
             if getattr(self, "_rws", None) is None or self._rws.numel() < ws_bytes:
                 self._rws = torch.zeros(ws_bytes, dtype=torch.uint8, device=self.dev)
-            check(self.lib.mac_read_bwd(ptr(knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
-                                        ptr(T(nWx)), ptr(T(nWy)), ptr(T(nWm)), ptr(T(nWm2)), ptr(cell._att_kb[i]),
-                                        ptr(cell._save[i]), ptr(self.grad(info)), float(cell.dropouts["read"]), cell.seed, i,
-                                        ptr(self.grad(knowledgeBase)), ptr(dmem_in), ptr(self.grad(control)),
-                                        ptr(self.G(nWx)), ptr(part["bx"]), ptr(self.G(nWy)), ptr(self.G(nby)),
-                                        ptr(self.G(nWm)), ptr(part["bm"]), ptr(self.G(nWm2)), ptr(part["bm2"]),
-                                        ptr(part["wr"]), ptr(dbr), ptr(self._rws), ws_bytes, B, N, d, stream_ptr()),
-                  "mac_read_bwd")
+            if self.tc:
+                check(self.lib.mac_read_bwd_tc(ptr(knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
+                                               ptr(T(nWy)), ptr(cell._att_kb[i]), ptr(cell._save[i]), ptr(self.grad(info)),
+                                               float(cell.dropouts["read"]), cell.seed, i, ptr(self.grad(knowledgeBase)),
+                                               ptr(dmem_in), ptr(self.grad(control)), ptr(self.G(nWx)), ptr(part["bx"]),
+                                               ptr(self.G(nWy)), ptr(self.G(nby)), ptr(self.G(nWm)), ptr(part["bm"]),
+                                               ptr(self.G(nWm2)), ptr(part["bm2"]), ptr(part["wr"]), ptr(dbr), ptr(self._rws),
+                                               ws_bytes, B, N, d, stream_ptr()), "mac_read_bwd_tc")
+            else:
+                check(self.lib.mac_read_bwd(ptr(knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
+                                            ptr(T(nWx)), ptr(T(nWy)), ptr(T(nWm)), ptr(T(nWm2)), ptr(cell._att_kb[i]),
+                                            ptr(cell._save[i]), ptr(self.grad(info)), float(cell.dropouts["read"]), cell.seed,
+                                            i, ptr(self.grad(knowledgeBase)), ptr(dmem_in), ptr(self.grad(control)),
+                                            ptr(self.G(nWx)), ptr(part["bx"]), ptr(self.G(nWy)), ptr(self.G(nby)),
+                                            ptr(self.G(nWm)), ptr(part["bm"]), ptr(self.G(nWm2)), ptr(part["bm2"]),
+                                            ptr(part["wr"]), ptr(dbr), ptr(self._rws), ws_bytes, B, N, d, stream_ptr()),
+                      "mac_read_bwd")
             self.axpy(self.grad(memory_in), dmem_in)
             self.colsum_B(part["wr"], self.G(PREFIX + lsc + "weights/weight"))
             self.colsum_B(part["bx"], self.G(nbx))
@@ -316,9 +349,10 @@ class Tape(object):
         self.add(bwd)
 
     # ------------------------------------------------------------------ the sweep
-    def run(self, d_control, d_memory, bucket=None, zero_bucket=True, d_vecq=None):
+    def run(self, d_control, d_memory, bucket=None, zero_bucket=True, d_vecq=None, tc=False):
         from .mac_cell import views_of
         cell, c = self.cell, self.cell.cfg
+        self.tc = bool(tc)
         self.bucket = bucket if bucket is not None else torch.zeros_like(self.p.flat)
         if bucket is not None and zero_bucket:
             self.bucket.zero_()
