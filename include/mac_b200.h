@@ -113,6 +113,8 @@ int mac_control_attend_fwd(const float* cc, long long cc_tstride, long long cc_b
  *   att = softmax_n(kl);  info = sum_n att * KB             (ops.py:143, 149-150; original KB, mac_cell.py:271-275)
  * Training: keep_read < 1 draws Philox4x32-10 masks from (seed, step) (see mac_dropout_uniform);
  * `save` (may be NULL) receives P, H, I1 ([B*N,d] each, in that order) and y ([B,d]) for backward.
+ * MAC_PREC_FP32 takes every d % 4 == 0 up to d <= 2048 when B*N < 512 and d <= 4096 otherwise (at most 32 partial logits
+ * per row, one per 64- or 128-column tile); a wider d returns MAC_ERR_UNSUPPORTED before any launch.
  * --------------------------------------------------------------------------------------------- */
 typedef struct mac_read_weights {
   const float* Wx;  const float* bx;   /* read/mulmemInter/linearLayerprojX            [d,d],[d]  */
@@ -172,7 +174,7 @@ int mac_read_step_fused_supported(int B, int N, int d);
 
 /* The HBM-bound tail of the read unit on its own (ops.py:143, 149-150):
  *   att[b,:] = softmax_n( sum_p logit_parts[(b*N+n)*nparts + p] + br );  info[b,:] = sum_n att[b,n] * KB[b,n,:]
- * kb_is_bf16 != 0: `kb` points at bf16 data. */
+ * kb_is_bf16 != 0: `kb` points at bf16 data.  Needs d % 4 == 0 for an fp32 and d % 64 == 0 for a bf16 knowledge base. */
 int mac_kb_attend_fwd(const float* logit_parts, int nparts, float br, const void* kb, int kb_is_bf16,
                       float* att, float* info, int B, int N, int d, mac_stream_t stream);
 

@@ -317,5 +317,8 @@ extern "C" int mac_kb_attend_fwd(const float* logit_parts, int nparts, float br,
   if (d % 64 == 0) return launch_kb_attend<float, 64>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
   if (d % 32 == 0) return launch_kb_attend<float, 32>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
   if (d % 16 == 0) return launch_kb_attend<float, 16>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
+  // narrow slices for the widths the fp32 read unit accepts (d % 4 == 0): a 4-column box is 16 bytes, the TMA minimum
+  if (d % 8 == 0) return launch_kb_attend<float, 8>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
+  if (d % 4 == 0) return launch_kb_attend<float, 4>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
   return MAC_ERR_UNSUPPORTED;
 }

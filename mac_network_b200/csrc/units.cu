@@ -228,11 +228,15 @@ static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, 
   if ((kb && !mac_aligned16(kb)) || !mac_aligned16(memory_in) || !mac_aligned16(control) || !mac_aligned16(workspace))
     return MAC_ERR_ALIGN;
   if (workspace_bytes < mac_read_workspace_bytes(B, N, d, prec)) return MAC_ERR_WORKSPACE;
+  const int M = B * N;
+  // the fp32 logits GEMM leaves one partial logit per column tile of I1 in a [B*N, 32] region: refuse wider d here,
+  // before anything is launched or written
+  const bool fp32_chain = prec != MAC_PREC_BF16 && prec != MAC_PREC_TC32 && prec != MAC_PREC_FP8;
+  if (fp32_chain && (d + sgemm_tile_n(M, d, d) - 1) / sgemm_tile_n(M, d, d) > 32) return MAC_ERR_UNSUPPORTED;
   size_t o_md, o_y, o_P, o_H, o_parts, o_sk;
   const size_t fp32_total = read_ws_layout(B, N, d, &o_md, &o_y, &o_P, &o_H, &o_parts, &o_sk);
   char* ws = reinterpret_cast<char*>(workspace);
   float* md = reinterpret_cast<float*>(ws + o_md);
-  const int M = B * N;
   // saved activations for backward live in the caller's `save` when given: [P | H | I1 | y]
   float* P = save ? save : reinterpret_cast<float*>(ws + o_P);
   float* H = save ? save + (size_t)M * d : reinterpret_cast<float*>(ws + o_H);

@@ -1,4 +1,5 @@
-"""Kernel-level GPU tests through the C ABI: K1 (control attention), K3 (KB attention), linear, dropout RNG."""
+"""Kernel-level GPU tests through the C ABI: K1 (control attention), K3 (KB attention), dropout RNG, the tensor-core
+linear.  mac_linear_fwd is checked in tests/test_gpu_forward_kernels.py."""
 import ctypes
 
 import numpy as np
@@ -16,37 +17,65 @@ def _lib():
     return L, L.load()
 
 
-@pytest.mark.parametrize("B,N,d,nparts", [(64, 196, 512, 4), (3, 49, 512, 1), (2, 1, 64, 2), (5, 700, 128, 3),
-                                          (2, 1500, 512, 1), (7, 33, 16, 1)])
+# (B, N, d, nparts): N = 1 and N < 64 load one box; N >= 64 four resident boxes; N = 1500 and 5000 a ring of recycled boxes
+# whose stage count is not a multiple of the buffer count and whose last box is partial.  B = 3 with N = 257: the last
+# batch row's last box runs past B*N (zero fill).  fp32 d covers every slice width (128 .. 4 columns); bf16 runs where
+# d % 64 == 0.
+KB_CASES_MAXNORM = [(64, 196, 512, 4), (3, 49, 512, 1), (2, 1, 64, 2), (5, 700, 128, 3), (2, 1500, 512, 1),
+                    (7, 33, 16, 1)]
+KB_CASES = (KB_CASES_MAXNORM
+            + [(3, N, d, (1, 8, 32)[(i + j) % 3]) for i, d in enumerate((4, 8, 16, 32, 64, 128, 512))
+               for j, N in enumerate((1, 63, 64, 257, 1500, 5000))])
+
+
+@pytest.mark.parametrize("B,N,d,nparts", KB_CASES)
 def test_kb_attend(B, N, d, nparts):
+    """mac_kb_attend_fwd against fp64, element-wise (tests/test_gpu_forward_kernels.py, softmax_bound), with the logits
+    at their drawn values and offset by +80 and -80 (only the max subtraction keeps expf finite there)"""
+    from tests.test_gpu_forward_kernels import TOL_ATT, kb_attend_reference
+    from tests.test_gpu_backward_kernels import Report, run_twice
     L, lib = _lib()
-    rng = np.random.RandomState(0)
-    parts = rng.standard_normal((B, N, nparts)).astype(np.float32)
+    rng = np.random.RandomState(B * 10000 + N * 10 + d)
     kb = rng.standard_normal((B, N, d)).astype(np.float32)
     br = 0.3
-    tp, tk = torch.from_numpy(parts).cuda(), torch.from_numpy(kb).cuda()
-    att = torch.empty(B, N, device="cuda")
-    info = torch.empty(B, d, device="cuda")
-    L.check(lib.mac_kb_attend_fwd(L.ptr(tp), nparts, br, L.ptr(tk), 0, L.ptr(att), L.ptr(info), B, N, d,
-                                  L.stream_ptr()))
-    torch.cuda.synchronize()
-    logits = parts.astype(np.float64).sum(-1) + br
-    a = O.softmax(logits)
-    r = O.att2smry(a, kb.astype(np.float64))
-    assert np.max(np.abs(att.cpu().numpy() - a)) < 1e-6
-    assert max_rel(info.cpu().numpy(), r) < 1e-5
-    # bf16 knowledge base (headline configuration): same attention, summary within bf16 rounding of KB
-    if d % 64 == 0:
-        tkb = tk.to(torch.bfloat16)
-        L.check(lib.mac_kb_attend_fwd(L.ptr(tp), nparts, br, L.ptr(tkb), 1, L.ptr(att), L.ptr(info), B, N, d,
-                                      L.stream_ptr()))
-        torch.cuda.synchronize()
-        r16 = O.att2smry(a, tkb.float().cpu().numpy().astype(np.float64))
-        assert max_rel(info.cpu().numpy(), r16) < 1e-5
+    tk = torch.from_numpy(kb).cuda()
+    kbs = [(0, tk)] + ([(1, tk.to(torch.bfloat16))] if d % 64 == 0 else [])
+    for off in (0.0, 80.0, -80.0):
+        parts = (rng.standard_normal((B, N, nparts)) + off / nparts).astype(np.float32)
+        tp = torch.from_numpy(parts).cuda()
+        for is16, kbt in kbs:
+            att = torch.full((B, N), float("nan"), device="cuda")
+            info = torch.full((B, d), float("nan"), device="cuda")
+            got, same = run_twice(lambda: L.check(lib.mac_kb_attend_fwd(L.ptr(tp), nparts, br, L.ptr(kbt), is16, L.ptr(att),
+                                                                        L.ptr(info), B, N, d, L.stream_ptr())),
+                                  {"att": att, "info": info})
+            a, aa, r, ar = kb_attend_reference(tp, br, kbt.float())
+            rep = Report("mac_kb_attend_fwd B=%d N=%d d=%d nparts=%d offset %g%s" % (B, N, d, nparts, off,
+                                                                                     " bf16" if is16 else ""))
+            rep.add("att", got["att"], a, aa, TOL_ATT)
+            rep.add("info", got["info"], r, ar, TOL_ATT)
+            rep.check(same, "bit-identical rerun")
+            rep.done()
+            if off == 0.0 and (B, N, d, nparts) in KB_CASES_MAXNORM:    # the max-norm bars of these cases
+                a_np, r_np = a.cpu().numpy(), r.cpu().numpy()
+                assert np.max(np.abs(got["att"].cpu().numpy() - a_np)) < 1e-6
+                assert max_rel(got["info"].cpu().numpy(), r_np) < 1e-5
 
 
-@pytest.mark.parametrize("T,B,S,d", [(12, 64, 40, 512), (1, 3, 1, 64), (4, 5, 45, 512), (3, 2, 7, 16)])
+# (T, B, S, d): nsteps 1, 12, 13 at B = 3 (steps split over gridDim.y) and B = 300 (one step group: B > 2 x SMs); S*d at
+# the shared-memory limit with separate words (S = 54, d = 512: 221 KB); d = 20
+CTRL_FWD_CASES = [(12, 64, 40, 512), (1, 3, 1, 64), (4, 5, 45, 512), (3, 2, 7, 16),
+                  (1, 3, 40, 512), (12, 3, 40, 64), (13, 3, 40, 64), (1, 300, 30, 128), (12, 300, 30, 128),
+                  (13, 300, 30, 128), (3, 3, 54, 512), (13, 5, 7, 20)]
+
+
+@pytest.mark.parametrize("T,B,S,d", CTRL_FWD_CASES)
 def test_control_attend(T, B, S, d):
+    """mac_control_attend_fwd against fp64, element-wise: shared and separate words, batch-major words (one bulk copy per
+    batch row) and the step-major history layout (rstride = B*d, bstride = d: one bulk copy per word row), lengths of 0
+    (uniform attention), > S and negative (clamped)"""
+    from tests.test_gpu_forward_kernels import TOL_ATT, softmax_bound
+    from tests.test_gpu_backward_kernels import Report, run_twice
     L, lib = _lib()
     rng = np.random.RandomState(1)
     cc = rng.standard_normal((T, B, d)).astype(np.float32)
@@ -57,55 +86,53 @@ def test_control_attend(T, B, S, d):
     lengths[0] = S
     if B > 1:
         lengths[1] = 1
+    for i, n in zip(range(2, B), (0, S + 5, -3)):
+        lengths[i] = n
+    lens = np.clip(lengths, 0, S)
     b = -0.2
-    for separate in (False, True):
-        ov = outw if separate else words
-        t = {k: torch.from_numpy(v).cuda() for k, v in dict(cc=cc, words=words, ov=ov, w=w, lengths=lengths).items()}
-        att = torch.empty(T, B, S, device="cuda")
-        out = torch.empty(T, B, d, device="cuda")
-        L.check(lib.mac_control_attend_fwd(L.ptr(t["cc"]), B * d, d, L.ptr(t["words"]), S * d, d,
-                                           L.ptr(t["ov"] if separate else t["words"]), S * d, d, L.ptr(t["lengths"]),
-                                           L.ptr(t["w"]), b, L.ptr(att), L.ptr(out), T, B, S, d, L.stream_ptr()))
-        torch.cuda.synchronize()
-        c64 = cc.astype(np.float64)
-        logits = np.einsum("tbk,bsk,k->tbs", c64, words.astype(np.float64), w.astype(np.float64)) + b
-        a = O.softmax(np.stack([O.exp_mask(l, lengths) for l in logits]))
-        r = np.einsum("tbs,bsk->tbk", a, ov.astype(np.float64))
-        got = att.cpu().numpy()
-        assert np.max(np.abs(got - a)) < 2e-6
-        for bi, n in enumerate(lengths):
-            assert np.all(got[:, bi, n:] == 0.0)
-        assert max_rel(out.cpu().numpy(), r) < 1e-5
+    for layout in ("batch", "history"):
+        for separate in (False, True):
+            ov = outw if separate else words
+            if layout == "batch":
+                wbuf, obuf, bstride, rstride = words, ov, S * d, d
+            else:
+                wbuf, obuf = (np.ascontiguousarray(x.transpose(1, 0, 2)) for x in (words, ov))
+                bstride, rstride = d, B * d
+            t = {k: torch.from_numpy(v).cuda() for k, v in dict(cc=cc, words=wbuf, ov=obuf, w=w, lengths=lengths).items()}
+            att = torch.full((T, B, S), float("nan"), device="cuda")
+            out = torch.full((T, B, d), float("nan"), device="cuda")
 
+            def call():
+                L.check(lib.mac_control_attend_fwd(L.ptr(t["cc"]), B * d, d, L.ptr(t["words"]), bstride, rstride,
+                                                   L.ptr(t["ov"] if separate else t["words"]), bstride, rstride,
+                                                   L.ptr(t["lengths"]), L.ptr(t["w"]), b, L.ptr(att), L.ptr(out), T, B, S, d,
+                                                   L.stream_ptr()))
 
-@pytest.mark.parametrize("M,ks,n_out,act", [(64, [512], 512, "TANH"), (64, [512, 512], 512, "NON"),
-                                            (64, [512, 512, 512], 512, "ELU"), (12544, [512], 512, "NON"),
-                                            (37, [64, 16], 20, "SIGMOID"), (64, [512], 6144, "NON"),
-                                            (700, [128], 128, "RELU_STD")])
-def test_linear(M, ks, n_out, act):
-    L, lib = _lib()
-    rng = np.random.RandomState(2)
-    xs = [rng.standard_normal((M, k)).astype(np.float32) for k in ks]
-    K = sum(ks)
-    W = (rng.standard_normal((K, n_out)) / np.sqrt(K)).astype(np.float32)
-    b = rng.standard_normal((n_out,)).astype(np.float32)
-    txs = [torch.from_numpy(x).cuda() for x in xs]
-    tW, tb = torch.from_numpy(W).cuda(), torch.from_numpy(b).cuda()
-    y = torch.empty(M, n_out, device="cuda")
-    wsb = int(lib.mac_linear_workspace_bytes(M, K, n_out))
-    ws = torch.zeros(wsb, dtype=torch.uint8, device="cuda")
-    n = len(xs)
-    for rep in range(2):      # twice: the split-K counters must be left at zero
-        arr_p = (ctypes.c_void_p * n)(*[t.data_ptr() for t in txs])
-        arr_k = (ctypes.c_int * n)(*ks)
-        L.check(lib.mac_linear_fwd(arr_p, arr_k, arr_k, n, L.ptr(tW), L.ptr(tb), 0.25, L.ACT[act], L.ptr(y), n_out,
-                                   M, n_out, L.ptr(ws), wsb, L.stream_ptr()))
-        torch.cuda.synchronize()
-        z = np.concatenate(xs, -1).astype(np.float64) @ W.astype(np.float64) + b + 0.25
-        ref = {"NON": z, "TANH": np.tanh(z), "ELU": O.elu(z), "SIGMOID": 1 / (1 + np.exp(-z)),
-               "RELU_STD": np.maximum(z, 0)}[act]
-        assert max_rel(y.cpu().numpy(), ref) < 2e-5
-    assert int(ws[:4096].to(torch.int32).abs().sum().item()) == 0
+            got, same = run_twice(call, {"att": att, "out": out})
+            c64 = cc.astype(np.float64)
+            logits = np.einsum("tbk,bsk,k->tbs", c64, words.astype(np.float64), w.astype(np.float64)) + b
+            alog = np.einsum("tbk,bsk,k->tbs", np.abs(c64), np.abs(words.astype(np.float64)), np.abs(w.astype(np.float64))) + abs(b)
+            valid = np.arange(S)[None, :] < lens[:, None]
+            valid |= (lens == 0)[:, None]           # length 0: every logit is -1e30 in both, the softmax is uniform
+            tl = torch.from_numpy(np.where((lens == 0)[None, :, None], 0.0, logits))
+            ta = torch.from_numpy(np.where((lens == 0)[None, :, None], 0.0, alog))
+            a, aa = softmax_bound(tl, ta, torch.from_numpy(np.broadcast_to(valid, logits.shape).copy()))
+            ovd = torch.from_numpy(ov.astype(np.float64))
+            rep = Report("mac_control_attend_fwd T=%d B=%d S=%d d=%d %s%s" % (T, B, S, d, layout,
+                                                                               " separate" if separate else ""))
+            rep.add("att", got["att"].cpu(), a, aa, TOL_ATT)
+            rep.add("out", got["out"].cpu(), torch.einsum("tbs,bsk->tbk", a, ovd), torch.einsum("tbs,bsk->tbk", aa, ovd.abs()),
+                    TOL_ATT)
+            rep.check(same, "bit-identical rerun")
+            rep.done()
+            # the bars this test has always had
+            a_np = a.numpy()
+            g_att = got["att"].cpu().numpy()
+            assert np.max(np.abs(g_att - a_np)) < 2e-6
+            for bi, n in enumerate(lens):
+                if n > 0:
+                    assert np.all(g_att[:, bi, n:] == 0.0)
+            assert max_rel(got["out"].cpu().numpy(), torch.einsum("tbs,bsk->tbk", a, ovd).numpy()) < 1e-5
 
 
 def test_dropout_rng_matches_independent_philox():
