@@ -52,8 +52,11 @@ enum {
   MAC_PREC_FP32 = 0, /* fp32 FMA pipe, fp32 accumulate: the <=1e-4 parity configuration */
   MAC_PREC_BF16 = 1, /* bf16 operands on wgmma tensor cores, fp32 accumulate: the headline configuration */
   MAC_PREC_TC32 = 2, /* split-bf16 on wgmma (x = hi + lo, three of the four partial products, fp32 accumulate): a tensor-core
-                        path inside the 1e-4 parity bar.  Inference form only (mac_read_invariant / mac_read_fwd_inv); fp32
-                        knowledge base; everything outside the three [B*N, .] projections as in MAC_PREC_FP32 */
+                        path inside the 1e-4 parity bar.  Inference form: mac_read_invariant / mac_read_fwd_inv.  Training
+                        form: mac_read_fwd without `inv` (any keep_read, `save` = [P | H | I1 | y] in fp32 as MAC_PREC_FP32
+                        writes it; needs the Wx_s3, Wm_s3 and Wm2_s3 packs) and its backward mac_read_bwd_tc32.  fp32
+                        knowledge base; d % 128 == 0 (else MAC_ERR_UNSUPPORTED before any launch); everything outside the
+                        three [B*N, .] projections as in MAC_PREC_FP32 */
   MAC_PREC_FP8 = 3   /* e4m3 operands on wgmma for the two per-step products of the read step, fp32 accumulate, per-row /
                         per-column fp32 scales (csrc/read_step_fp8.cuh).  Inference form only (mac_read_invariant /
                         mac_read_fwd_inv), the shapes of mac_read_step_fused_supported, bf16 knowledge base; P and Q as in
@@ -129,6 +132,9 @@ typedef struct mac_read_weights {
   /* MAC_PREC_FP8 only (read under no other precision): e4m3 [out, in] copies of Wm[0:d] and Wm2 with their per-output-column
    * fp32 scales [d] (mac_pack_weight_fp8) */
   const void* Wm_fp8; const float* Wm_fp8_scale; const void* Wm2_fp8; const float* Wm2_fp8_scale;
+  /* MAC_PREC_TC32 training form only (mac_read_fwd without `inv`): split-bf16 copy [d, 6d] of the whole Wm [2d, d]
+   * (mac_pack_weight_split3 with K = 2d), the B operand of H = ELU([P*y | P] @ Wm + bm) as one product over K = 2d */
+  const void* Wm_s3;
 } mac_read_weights;
 
 int mac_read_fwd(const float* kb, const void* kb_bf16, const float* memory_in, const float* control,
@@ -157,6 +163,11 @@ int mac_read_fwd_inv(const float* kb, const void* kb_bf16, const void* inv, cons
                      float* info, float* att, void* workspace, size_t workspace_bytes, int B, int N, int d,
                      mac_stream_t stream);
 /* y_pre (may be NULL): y = memory_in @ Wy + by [B, d] when the caller already has it, see mac_write_fwd_next_y. */
+/* mac_read_fwd with MAC_PREC_TC32 (the training form): dropout(KB) is split into [hi | lo] with the fp32 path's Philox
+ * numbering; P = KBd @ Wx + bx (Wx_s3), H = ELU([P*y | P] @ Wm + bm) as ONE product over K = 2d (Wm_s3, the split3 pack of
+ * the whole [2d, d] Wm) and I1 = H @ Wm2 + bm2 (Wm2_s3, the read-inter dropout in the logits epilogue) are split-bf16 products;
+ * P, H and I1 are stored in fp32 as their epilogues computed them, then kb_attend on the fp32 knowledge base.  Any B*N.  The
+ * workspace query is unchanged: the split operands reuse the fp32 layout's P and H regions and the tc32 slabs behind it. */
 
 /* One inference read step (csrc/read_step.cuh): given inv = [P | Q] from mac_read_invariant (bf16), the bf16 knowledge base,
  * y = memory @ Wy + by [B, d] (ops.py:689) and the control state [B, d], computes
@@ -319,6 +330,18 @@ int mac_read_bwd_tc(const float* kb, const float* memory_in, const float* contro
                     float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2, float* dbm2_part, float* dwr_part,
                     float* dbr_part, void* workspace, size_t workspace_bytes, int B, int N, int d, mac_stream_t stream);
 size_t mac_read_bwd_tc_workspace_bytes(int B, int N, int d);
+/* Backward of the MAC_PREC_TC32 training forward: mac_read_bwd_tc's arguments and accumulation conventions, with its six
+ * [B*N, .] products as split-bf16 products (x = hi + lo, three of the four partial products, fp32 accumulation), so the
+ * gradients keep the forward's fp32-class accuracy.  Data gradients: [G_hi | G_lo] against [W_hi | W_hi | W_lo] per row of W
+ * in its own [in, out] layout, packed into the workspace on every call.  Weight gradients: ONE split-K launch over the
+ * contraction B*N rounded up to 64 (zero columns written on every call), slices summed in a fixed order: reruns are
+ * bit-identical.  Any B*N; needs d % 128 == 0, else MAC_ERR_UNSUPPORTED before any launch. */
+int mac_read_bwd_tc32(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
+                      const float* Wy_t, const float* att, const float* save, const float* dinfo, float keep_read,
+                      uint64_t seed, int step, float* dkb, float* dmem_in, float* dcontrol, float* dWx, float* dbx_part,
+                      float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2, float* dbm2_part, float* dwr_part,
+                      float* dbr_part, void* workspace, size_t workspace_bytes, int B, int N, int d, mac_stream_t stream);
+size_t mac_read_bwd_tc32_workspace_bytes(int B, int N, int d);
 /* ops.linear on tensor cores for the [B*N, .] products of the composed read unit (csrc/linear_tc.cuh; MACCell(prec="bf16")
  * with read-unit flags outside mac_read_fwd): bf16 operands (round to nearest even), fp32 accumulation, fp32 in / fp32 out.
  * mac_linear_tc_seg_fwd: mac_linear_fwd's y[M, n_out] = act(concat(x_0 .. x_{nseg-1}) @ W + b + bias_const) with W given as

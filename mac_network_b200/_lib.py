@@ -28,7 +28,8 @@ class ReadWeights(ctypes.Structure):
                 ("Wm2", c_fp), ("bm2", c_fp), ("wr", c_fp), ("br", c_f),
                 ("Wx_bf16", c_fp), ("Wm_bf16", c_fp), ("Wm2_bf16", c_fp),
                 ("Wx_s3", c_fp), ("Wma_s3", c_fp), ("Wmb_s3", c_fp), ("Wm2_s3", c_fp),
-                ("Wm_fp8", c_fp), ("Wm_fp8_scale", c_fp), ("Wm2_fp8", c_fp), ("Wm2_fp8_scale", c_fp)]
+                ("Wm_fp8", c_fp), ("Wm_fp8_scale", c_fp), ("Wm2_fp8", c_fp), ("Wm2_fp8_scale", c_fp),
+                ("Wm_s3", c_fp)]
 
 
 # name -> (restype, argtypes); every symbol include/mac_b200.h declares
@@ -79,6 +80,9 @@ PROTOTYPES = {
     "mac_read_bwd_tc": (c_int, [c_fp, c_fp, c_fp, ctypes.POINTER(ReadWeights), c_fp, c_fp, c_fp, c_fp, c_f, c_u64, c_int]
                         + [c_fp] * 13 + [c_fp, c_sz, c_int, c_int, c_int, c_fp]),
     "mac_read_bwd_tc_workspace_bytes": (c_sz, [c_int, c_int, c_int]),
+    "mac_read_bwd_tc32": (c_int, [c_fp, c_fp, c_fp, ctypes.POINTER(ReadWeights), c_fp, c_fp, c_fp, c_fp, c_f, c_u64, c_int]
+                          + [c_fp] * 13 + [c_fp, c_sz, c_int, c_int, c_int, c_fp]),
+    "mac_read_bwd_tc32_workspace_bytes": (c_sz, [c_int, c_int, c_int]),
     "mac_gate_bwd": (c_int, [c_fp] * 7 + [c_ll, c_fp]),
     "mac_activation_bwd": (c_int, [c_fp, c_fp, c_int, c_fp, c_ll, c_fp]),
     "mac_widen_bf16": (c_int, [ctypes.POINTER(c_fp), ctypes.POINTER(c_fp), c_int, c_ll, c_fp]),

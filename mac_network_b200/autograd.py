@@ -31,8 +31,13 @@ class _Bwd(object):
         self.cell, self.lib = cell, cell.lib
         # tc: the read unit's six big products on wgmma tensor cores (mac_read_bwd_tc) instead of the fp32 FMA GEMMs
         self.tc = bool(tc)
-        if self.tc and (cell.d % 128 or (cell.B * cell.N) % 64):
+        # a tc32 cell keeps its forward's accuracy class in backward: split-bf16 products (mac_read_bwd_tc32, any B*N)
+        self.tc32 = self.tc and cell.prec == _lib.PREC["tc32"]
+        if self.tc32 and cell.d % 128:
+            raise NotImplementedError("split-bf16 tensor-core backward needs d % 128 == 0")
+        if self.tc and not self.tc32 and (cell.d % 128 or (cell.B * cell.N) % 64):
             raise NotImplementedError("tensor-core backward needs d % 128 == 0 and (B*N) % 64 == 0")
+        mode = "tc32" if self.tc32 else self.tc
         self.p = cell.params
         c = cell.cfg
         if c.controlWholeQ or c.controlContinuous:
@@ -51,14 +56,15 @@ class _Bwd(object):
             self.bucket.zero_()
         self.g = views_of(self.bucket, self.p.specs, self.p.offsets)
         cache = getattr(cell, "_bwd_ws", None)            # scratch is allocated once per cell and reused every step
-        if cache is not None and cache[4] != self.tc:
+        if cache is not None and cache[4] != mode:
             cache = None
         if cache is None:
-            ws_bytes = int((self.lib.mac_read_bwd_tc_workspace_bytes if self.tc else self.lib.mac_read_bwd_workspace_bytes)(
-                self.B, self.N, self.d))
+            query = (self.lib.mac_read_bwd_tc32_workspace_bytes if self.tc32 else
+                     self.lib.mac_read_bwd_tc_workspace_bytes if self.tc else self.lib.mac_read_bwd_workspace_bytes)
+            ws_bytes = int(query(self.B, self.N, self.d))
             lws_bytes = 4096 + 32 * 1536 * 512 * 4
             cache = (ws_bytes, torch.zeros(ws_bytes, dtype=torch.uint8, device=dev), lws_bytes,
-                     torch.zeros(lws_bytes, dtype=torch.uint8, device=dev), self.tc)
+                     torch.zeros(lws_bytes, dtype=torch.uint8, device=dev), mode)
             cell._bwd_ws = cache
         self.ws_bytes, self.ws, self.lws_bytes, self.lws = cache[:4]
 
@@ -164,13 +170,14 @@ class _Bwd(object):
                                           stream_ptr()), "dropout bwd")
             # ---------------- read unit backward (mac_cell.py:209-277)
             if self.tc:
-                check(lib.mac_read_bwd_tc(ptr(cell.knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
-                                          ptr(_t(self.p, Wy, nWy)), ptr(cell._att_kb[i]), ptr(cell._save[i]), ptr(dinfo),
-                                          keep_r, cell.seed, i, ptr(dkb), ptr(dmem_in), ptr(gC[i + 1]), ptr(self.G(nWx)),
-                                          ptr(part["bx"]), ptr(self.G(nWy)), ptr(self.G(nby)), ptr(self.G(nWm)),
-                                          ptr(part["bm"]), ptr(self.G(nWm2)), ptr(part["bm2"]), ptr(part["wr"]),
-                                          ptr(spart["br"]), ptr(self.ws), self.ws_bytes, B, N, d, stream_ptr()),
-                      "mac_read_bwd_tc")
+                # bf16 cell: mac_read_bwd_tc; tc32 cell: the split-bf16 form with the same arguments
+                name = "mac_read_bwd_tc32" if self.tc32 else "mac_read_bwd_tc"
+                check(getattr(lib, name)(ptr(cell.knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
+                                         ptr(_t(self.p, Wy, nWy)), ptr(cell._att_kb[i]), ptr(cell._save[i]), ptr(dinfo),
+                                         keep_r, cell.seed, i, ptr(dkb), ptr(dmem_in), ptr(gC[i + 1]), ptr(self.G(nWx)),
+                                         ptr(part["bx"]), ptr(self.G(nWy)), ptr(self.G(nby)), ptr(self.G(nWm)),
+                                         ptr(part["bm"]), ptr(self.G(nWm2)), ptr(part["bm2"]), ptr(part["wr"]),
+                                         ptr(spart["br"]), ptr(self.ws), self.ws_bytes, B, N, d, stream_ptr()), name)
             else:
                 check(lib.mac_read_bwd(ptr(cell.knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
                                      ptr(_t(self.p, Wx, nWx)), ptr(_t(self.p, Wy, nWy)), ptr(_t(self.p, Wm, nWm)),

@@ -923,26 +923,24 @@ extern "C" int mac_pack_t_bf16_(int mode, const float* X, void* Xt, void* Xrm, i
                                 mac_stream_t stream_);
 static size_t rbt_align(size_t x) { return (x + 1023) & ~(size_t)1023; }
 
-extern "C" size_t mac_read_bwd_tc_workspace_bytes(int B, int N, int d) {
-  const size_t M = (size_t)B * N;
-  return mac_read_bwd_workspace_bytes(B, N, d) + 1024 + rbt_align(M * 2 * d * 2) /*g16*/ + rbt_align(2 * d * M * 2) /*xT16*/ +
-         rbt_align(d * M * 2) /*gT16*/ + rbt_align((size_t)2 * d * d * 2) /*w16*/ + rbt_align(M * 2 * d * 4) /*tmp32*/ +
-         rbt_align(mac_tc_wgrad_partial_bytes_(2 * d, d)) /*dWtmp: split-K partials of the largest weight gradient*/;
-}
-
-extern "C" int mac_read_bwd_tc(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
-                               const float* Wy_t, const float* att, const float* save, const float* dinfo, float keep_read,
-                               uint64_t seed, int step, float* dkb, float* dmem_in, float* dcontrol, float* dWx,
-                               float* dbx_part, float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2,
-                               float* dbm2_part, float* dwr_part, float* dbr_part, void* workspace, size_t workspace_bytes,
-                               int B, int N, int d, mac_stream_t stream_) {
+namespace mac {
+// The schedule both tensor-core read backwards share (mac_read_bwd_tc, mac_read_bwd_tc32): mac_read_bwd's seven steps with
+// its six [B*N, .] products delegated to the caller's operations on its own scratch (behind the fp32 layout of mac_read_bwd,
+// whose bufA / bufB / bufC / dka / dkl / dy / md / dmd this function carves):
+//   packX(mode, X, half, rowvec)  activations [M, d] -> the transposed operand of the next wgrad, rows d*half .. (mode 0
+//                                 plain, 1 P*y, 2 the forward's KB dropout)
+//   wgrad(in, G, dW)              dW[in, d] += X^T G with X from the packX calls; leaves G's operand for the next dgrad
+//   dgrad(W, in, out)             out[M, in] = G W^T with W fp32 in its own [in, d] layout and G from the preceding wgrad
+// tmp32 is fp32 scratch [M, d].
+template <class PackX, class WGrad, class DGrad>
+static int read_bwd_tc_schedule(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
+                                const float* Wy_t, const float* att, const float* save, const float* dinfo, float keep_read,
+                                uint64_t seed, int step, float* dkb, float* dmem_in, float* dcontrol, float* dWx,
+                                float* dbx_part, float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2,
+                                float* dbm2_part, float* dwr_part, float* dbr_part, void* workspace, float* tmp32, int B,
+                                int N, int d, mac_stream_t stream_, PackX packX, WGrad wgrad, DGrad dgrad) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!kb || !memory_in || !control || !w || !att || !save || !dinfo || !dmem_in || !dcontrol || !workspace || !dWx ||
-      !dWm || !dWm2)
-    return MAC_ERR_INVALID;
   const int M = B * N;
-  if ((d % 128) || (M % 64)) return MAC_ERR_UNSUPPORTED;
-  if (workspace_bytes < mac_read_bwd_tc_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
   const size_t Md = (size_t)M * d;
   char* ws = reinterpret_cast<char*>(workspace);
   float* f = reinterpret_cast<float*>(ws + BW_HEADER);
@@ -955,15 +953,6 @@ extern "C" int mac_read_bwd_tc(const float* kb, const float* memory_in, const fl
   float* dy = dkl + BNp;           // [B,d]
   float* md = dy + (size_t)B * d;  // [B,d]
   float* dmd = md + (size_t)B * d; // [B,d]
-  // tensor-core operands behind the fp32 layout of mac_read_bwd
-  char* x = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(ws + mac_read_bwd_workspace_bytes(B, N, d)) + 1023) &
-                                    ~(uintptr_t)1023);
-  void* g16 = x;   x += rbt_align((size_t)M * 2 * d * 2);        // bf16 [M, <=2d]   gradient as the A operand of a dgrad
-  void* xT16 = x;  x += rbt_align((size_t)2 * d * M * 2);        // bf16 [<=2d, M]   activations, transposed
-  void* gT16 = x;  x += rbt_align((size_t)d * M * 2);            // bf16 [d, M]      gradient, transposed
-  void* w16 = x;   x += rbt_align((size_t)2 * d * d * 2);        // bf16 weight in its own [in, out] layout
-  float* tmp32 = reinterpret_cast<float*>(x); x += rbt_align((size_t)M * 2 * d * 4);
-  float* dWtmp = reinterpret_cast<float*>(x);
   const float* P = save;
   const float* H = save + Md;
   const float* I1 = save + 2 * Md;
@@ -977,23 +966,6 @@ extern "C" int mac_read_bwd_tc(const float* kb, const float* memory_in, const fl
     st = (call);                  \
     if (st != MAC_OK) return st;  \
   } while (0)
-  // activations / gradients for the tensor-core operands: fp32 [M, d] -> bf16 transposed [d, M] (+ optionally the row-major
-  // bf16 copy), with the forward's P*y scaling or KB dropout applied on the way (pack_t_bf16_kernel, csrc/tc_gemm.cuh)
-  auto packT = [&](int mode, const float* X, void* Xt, void* Xrm, const float* rowvec) -> int {
-    return mac_pack_t_bf16_(mode, X, Xt, Xrm, M, d, rowvec, N, thr, scale, seed, MAC_SITE_READ_KB, step, stream_);
-  };
-  // wgrad: dW[in, out] += X^T @ G with X^T already packed as xT [in, M]; leaves bf16(G) row-major in g16 for the dgrad below
-  auto wgrad = [&](const void* xT, int in, const float* G, float* dW) -> int {
-    int s = packT(0, G, gT16, g16, nullptr);                                                 // G [M, d] -> G^T [d, M], bf16(G)
-    if (s != MAC_OK) return s;
-    return mac_tc_wgrad_splitk_(xT, gT16, dW, dWtmp, in, d, M, stream_);                          // dW[in, d] += xT @ (G^T)^T, split-K
-  };
-  // dgrad: out[M, in] = G[M, d] @ W[in, d]^T   (W fp32 in its own [in, out = d] layout; G = the g16 of the preceding wgrad)
-  auto dgrad = [&](const float* W, int in, float* out) -> int {
-    int s = mac_cast_bf16(W, w16, (long long)in * d, stream_);
-    if (s != MAC_OK) return s;
-    return mac_linear_tc_fwd(g16, w16, nullptr, MAC_ACT_NON, out, 0, M, d, in, stream_);
-  };
   // (1) info = sum_n att*KB ; att = softmax(kl):  dkl, dKB += att (x) dinfo
   RBT(mac_kb_attend_bwd(kb, att, dinfo, dka, dkl, dkb, dbr_part, B, N, d, stream_));
   // (2) logits epilogue backward -> dI1 (bufA), dcontrol, dwr, dbm2
@@ -1001,22 +973,22 @@ extern "C" int mac_read_bwd_tc(const float* kb, const float* memory_in, const fl
                                                                       bufA, dcontrol, dwr_part, dbm2_part, N, d);
   MAC_LAUNCH_CHECK();
   // (3) I1 = H @ Wm2 + bm2:  dWm2 += H^T dI1 ;  dZ = (dI1 @ Wm2^T) * ELU'(H) ; dbm += colsum(dZ)
-  RBT(packT(0, H, xT16, nullptr, nullptr));
-  RBT(wgrad(xT16, d, bufA, dWm2));
+  RBT(packX(0, H, 0, nullptr));
+  RBT(wgrad(d, bufA, dWm2));
   RBT(dgrad(w->Wm2, d, tmp32));
   elu_bwd_colsum_kernel<<<dim3((d + 127) / 128, B), 256, 0, stream>>>(H, tmp32, bufB, dbm_part, N, d);
   MAC_LAUNCH_CHECK();
   // (4) Z = [P*y, P] @ Wm + bm:  dWm += [P*y, P]^T dZ ;  dI0 = dZ @ Wm^T
-  RBT(packT(1, P, xT16, nullptr, y));                                                            // rows 0..d-1   of [2d, M]: (P*y)^T
-  RBT(packT(0, P, reinterpret_cast<__nv_bfloat16*>(xT16) + (size_t)d * M, nullptr, nullptr));    // rows d..2d-1: P^T
-  RBT(wgrad(xT16, 2 * d, bufB, dWm));
+  RBT(packX(1, P, 0, y));                                                                     // rows 0..d-1:   (P*y)^T
+  RBT(packX(0, P, 1, nullptr));                                                               // rows d..2d-1: P^T
+  RBT(wgrad(2 * d, bufB, dWm));
   RBT(dgrad(w->Wm, 2 * d, bufC));
   // (5) I0 = [P*y, P]:  dP (bufA), dy, dbx
   read_bwd_p_kernel<<<dim3((d + 127) / 128, B), 256, 0, stream>>>(bufC, P, y, bufA, dy, dbx_part, N, d);
   MAC_LAUNCH_CHECK();
   // (6) P = dropout(KB) @ Wx + bx:  dWx += Kd^T dP ;  dKB += (dP @ Wx^T) * mask/keep
-  RBT(packT(drop ? 2 : 0, kb, xT16, nullptr, nullptr));                                          // dropout(KB)^T: the forward's mask
-  RBT(wgrad(xT16, d, bufA, dWx));
+  RBT(packX(drop ? 2 : 0, kb, 0, nullptr));                                                   // dropout(KB)^T: the forward's mask
+  RBT(wgrad(d, bufA, dWx));
   if (dkb) {
     RBT(dgrad(w->Wx, d, tmp32));
     if (drop) {
@@ -1044,4 +1016,140 @@ extern "C" int mac_read_bwd_tc(const float* kb, const float* memory_in, const fl
   }
 #undef RBT
   return MAC_OK;
+}
+}  // namespace mac
+
+extern "C" size_t mac_read_bwd_tc_workspace_bytes(int B, int N, int d) {
+  const size_t M = (size_t)B * N;
+  return mac_read_bwd_workspace_bytes(B, N, d) + 1024 + rbt_align(M * 2 * d * 2) /*g16*/ + rbt_align(2 * d * M * 2) /*xT16*/ +
+         rbt_align(d * M * 2) /*gT16*/ + rbt_align((size_t)2 * d * d * 2) /*w16*/ + rbt_align(M * 2 * d * 4) /*tmp32*/ +
+         rbt_align(mac_tc_wgrad_partial_bytes_(2 * d, d)) /*dWtmp: split-K partials of the largest weight gradient*/;
+}
+
+extern "C" int mac_read_bwd_tc(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
+                               const float* Wy_t, const float* att, const float* save, const float* dinfo, float keep_read,
+                               uint64_t seed, int step, float* dkb, float* dmem_in, float* dcontrol, float* dWx,
+                               float* dbx_part, float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2,
+                               float* dbm2_part, float* dwr_part, float* dbr_part, void* workspace, size_t workspace_bytes,
+                               int B, int N, int d, mac_stream_t stream_) {
+  if (!kb || !memory_in || !control || !w || !att || !save || !dinfo || !dmem_in || !dcontrol || !workspace || !dWx ||
+      !dWm || !dWm2)
+    return MAC_ERR_INVALID;
+  const int M = B * N;
+  if ((d % 128) || (M % 64)) return MAC_ERR_UNSUPPORTED;
+  if (workspace_bytes < mac_read_bwd_tc_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
+  // tensor-core operands behind the fp32 layout of mac_read_bwd
+  char* x = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(reinterpret_cast<char*>(workspace) +
+                                                                 mac_read_bwd_workspace_bytes(B, N, d)) + 1023) &
+                                    ~(uintptr_t)1023);
+  void* g16 = x;   x += rbt_align((size_t)M * 2 * d * 2);        // bf16 [M, <=2d]   gradient as the A operand of a dgrad
+  void* xT16 = x;  x += rbt_align((size_t)2 * d * M * 2);        // bf16 [<=2d, M]   activations, transposed
+  void* gT16 = x;  x += rbt_align((size_t)d * M * 2);            // bf16 [d, M]      gradient, transposed
+  void* w16 = x;   x += rbt_align((size_t)2 * d * d * 2);        // bf16 weight in its own [in, out] layout
+  float* tmp32 = reinterpret_cast<float*>(x); x += rbt_align((size_t)M * 2 * d * 4);
+  float* dWtmp = reinterpret_cast<float*>(x);
+  const bool drop = keep_read < 1.f;
+  const uint32_t thr = drop ? keep_threshold(keep_read) : 0u;
+  const float scale = drop ? 1.f / keep_read : 1.f;
+  // activations / gradients for the tensor-core operands: fp32 [M, d] -> bf16 transposed [d, M] (+ optionally the row-major
+  // bf16 copy), with the forward's P*y scaling or KB dropout applied on the way (pack_t_bf16_kernel, csrc/tc_gemm.cuh)
+  auto packT = [&](int mode, const float* X, void* Xt, void* Xrm, const float* rowvec) -> int {
+    return mac_pack_t_bf16_(mode, X, Xt, Xrm, M, d, rowvec, N, thr, scale, seed, MAC_SITE_READ_KB, step, stream_);
+  };
+  auto packX = [&](int mode, const float* X, int half, const float* rowvec) -> int {
+    return packT(mode, X, reinterpret_cast<__nv_bfloat16*>(xT16) + (size_t)half * d * M, nullptr, rowvec);
+  };
+  // wgrad: dW[in, out] += X^T @ G with X^T already packed as xT [in, M]; leaves bf16(G) row-major in g16 for the dgrad below
+  auto wgrad = [&](int in, const float* G, float* dW) -> int {
+    int s = packT(0, G, gT16, g16, nullptr);                                                 // G [M, d] -> G^T [d, M], bf16(G)
+    if (s != MAC_OK) return s;
+    return mac_tc_wgrad_splitk_(xT16, gT16, dW, dWtmp, in, d, M, stream_);                        // dW[in, d] += xT @ (G^T)^T, split-K
+  };
+  // dgrad: out[M, in] = G[M, d] @ W[in, d]^T   (W fp32 in its own [in, out = d] layout; G = the g16 of the preceding wgrad)
+  auto dgrad = [&](const float* W, int in, float* out) -> int {
+    int s = mac_cast_bf16(W, w16, (long long)in * d, stream_);
+    if (s != MAC_OK) return s;
+    return mac_linear_tc_fwd(g16, w16, nullptr, MAC_ACT_NON, out, 0, M, d, in, stream_);
+  };
+  return read_bwd_tc_schedule(kb, memory_in, control, w, Wy_t, att, save, dinfo, keep_read, seed, step, dkb, dmem_in, dcontrol,
+                              dWx, dbx_part, dWy, dby, dWm, dbm_part, dWm2, dbm2_part, dwr_part, dbr_part, workspace, tmp32, B,
+                              N, d, stream_, packX, wgrad, dgrad);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Backward of the split-bf16 ("tc32") training read: the schedule of mac_read_bwd_tc with its six [B*N, .] products as
+// split-bf16 products (x = hi + lo, three of the four partial products, one fp32 accumulator), so the backward keeps the
+// forward's fp32-class accuracy:
+//   dgrad  dX[M, in] = G @ W^T:  A' = [G_hi | G_lo] [M, 2 out] (written by the transposing pack from the same read of G),
+//          W' = [W_hi | W_hi | W_lo] [in, 3 out] per row of W in its own [in, out] layout; one tc3_gemm, fp32 out
+//   wgrad  dW += X^T G over Mp = B*N rounded up to 64:  [X_hi^T | X_lo^T] [in, 2Mp] against [G_hi^T | G_hi^T | G_lo^T]
+//          [out, 3Mp], ONE split-K launch (tc3_wgrad_splitk; faster on the H100 than three accumulating tc_wgrad_splitk
+//          calls, DESIGN.md section 9 item 5); the zero columns M..Mp-1 are written on every call
+// The transposing pack applies P*y (mode 1) and the forward's KB dropout mask (mode 2) as in mac_read_bwd_tc; the element-wise
+// kernels are mac_read_bwd's.  Any B*N; d % 128 == 0, else MAC_ERR_UNSUPPORTED before any launch.
+// ------------------------------------------------------------------------------------------------------------------
+extern "C" int mac_pack_t_split_(int mode, const float* X, void* Xt, void* Xrm, int K, int N, int segs, const float* rowvec,
+                                 int rows_per_batch, uint32_t thresh, float scale, uint64_t seed, int site, int step,
+                                 mac_stream_t stream_);
+extern "C" int mac_tc3_wgrad_splitk_(const void* xT2, const void* gT3, float* dW, float* partial, int in_dim, int out_dim,
+                                     int kp, mac_stream_t stream_);
+extern "C" int mac_split3_rows_(const float* W, void* W3, int R, int C, mac_stream_t stream_);
+extern "C" int mac_tc3_linear_(const void* a_split, const void* wt3, float* y, int M, int K, int n_out, mac_stream_t stream_);
+
+extern "C" size_t mac_read_bwd_tc32_workspace_bytes(int B, int N, int d) {
+  const size_t M = (size_t)B * N, Mp = (M + 63) & ~(size_t)63;
+  return mac_read_bwd_workspace_bytes(B, N, d) + 1024 + rbt_align(M * 2 * d * 2) /*g2: [G_hi | G_lo]*/ +
+         rbt_align((size_t)2 * d * 2 * Mp * 2) /*xT2*/ + rbt_align((size_t)d * 3 * Mp * 2) /*gT3*/ +
+         rbt_align((size_t)2 * d * 3 * d * 2) /*w3*/ + rbt_align(M * d * 4) /*tmp32*/ +
+         rbt_align(mac_tc_wgrad_partial_bytes_(2 * d, d)) /*split-K partials of the largest weight gradient*/;
+}
+
+extern "C" int mac_read_bwd_tc32(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
+                                 const float* Wy_t, const float* att, const float* save, const float* dinfo, float keep_read,
+                                 uint64_t seed, int step, float* dkb, float* dmem_in, float* dcontrol, float* dWx,
+                                 float* dbx_part, float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2,
+                                 float* dbm2_part, float* dwr_part, float* dbr_part, void* workspace, size_t workspace_bytes,
+                                 int B, int N, int d, mac_stream_t stream_) {
+  if (!kb || !memory_in || !control || !w || !att || !save || !dinfo || !dmem_in || !dcontrol || !workspace || !dWx ||
+      !dWm || !dWm2)
+    return MAC_ERR_INVALID;
+  if (B <= 0 || N <= 0 || d <= 0) return MAC_ERR_INVALID;
+  if (d % 128) return MAC_ERR_UNSUPPORTED;
+  if (!(keep_read > 0.f && keep_read <= 1.f)) return MAC_ERR_INVALID;
+  if (workspace_bytes < mac_read_bwd_tc32_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
+  const int M = B * N;
+  const size_t Mp = ((size_t)M + 63) & ~(size_t)63;
+  // split operands behind the fp32 layout of mac_read_bwd
+  char* x = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(reinterpret_cast<char*>(workspace) +
+                                                                 mac_read_bwd_workspace_bytes(B, N, d)) + 1023) &
+                                    ~(uintptr_t)1023);
+  void* g2 = x;    x += rbt_align((size_t)M * 2 * d * 2);          // bf16 [M, 2d]        [G_hi | G_lo], A' of a dgrad
+  void* xT2 = x;   x += rbt_align((size_t)2 * d * 2 * Mp * 2);     // bf16 [<=2d, 2Mp]    [X_hi^T | X_lo^T]
+  void* gT3 = x;   x += rbt_align((size_t)d * 3 * Mp * 2);         // bf16 [d, 3Mp]       [G_hi^T | G_hi^T | G_lo^T]
+  void* w3 = x;    x += rbt_align((size_t)2 * d * 3 * d * 2);      // bf16 [<=2d, 3d]     [W_hi | W_hi | W_lo] per row of W
+  float* tmp32 = reinterpret_cast<float*>(x); x += rbt_align((size_t)M * d * 4);
+  float* dWtmp = reinterpret_cast<float*>(x);
+  const bool drop = keep_read < 1.f;
+  const uint32_t thr = drop ? keep_threshold(keep_read) : 0u;
+  const float scale = drop ? 1.f / keep_read : 1.f;
+  // activations [M, d] -> [X_hi^T | X_lo^T] rows of xT2 (row pitch 2Mp), with P*y or the KB dropout applied on the way
+  auto packX = [&](int mode, const float* X, int half, const float* rowvec) -> int {
+    return mac_pack_t_split_(mode, X, reinterpret_cast<__nv_bfloat16*>(xT2) + (size_t)half * d * 2 * Mp, nullptr, M, d, 2,
+                             rowvec, N, thr, scale, seed, MAC_SITE_READ_KB, step, stream_);
+  };
+  // wgrad: dW[in, d] += X^T G with X already in xT2; leaves [G_hi | G_lo] row-major in g2 for the dgrad below
+  auto wgrad = [&](int in, const float* G, float* dW) -> int {
+    int s = mac_pack_t_split_(0, G, gT3, g2, M, d, 3, nullptr, 1, 0u, 1.f, 0, 0, 0, stream_);
+    if (s != MAC_OK) return s;
+    return mac_tc3_wgrad_splitk_(xT2, gT3, dW, dWtmp, in, d, (int)Mp, stream_);
+  };
+  // dgrad: out[M, in] = G[M, d] @ W[in, d]^T   (W fp32 in its own [in, out = d] layout; G = the g2 of the preceding wgrad)
+  auto dgrad = [&](const float* W, int in, float* out) -> int {
+    int s = mac_split3_rows_(W, w3, in, d, stream_);
+    if (s != MAC_OK) return s;
+    return mac_tc3_linear_(g2, w3, out, M, d, in, stream_);
+  };
+  return read_bwd_tc_schedule(kb, memory_in, control, w, Wy_t, att, save, dinfo, keep_read, seed, step, dkb, dmem_in, dcontrol,
+                              dWx, dbx_part, dWy, dby, dWm, dbm_part, dWm2, dbm2_part, dwr_part, dbr_part, workspace, tmp32, B,
+                              N, d, stream_, packX, wgrad, dgrad);
 }

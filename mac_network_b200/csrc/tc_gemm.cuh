@@ -16,11 +16,13 @@
 //   TC_EPI_ACT     act(acc + b)            -> bf16                               (mac_cell.py:236-238)
 //   TC_EPI_LOGITS  I1 = acc + bm2; t = ELU(I1 * control[b]); (dropout); parts[m, ntile] = sum_n t * wr[n]
 //                                                                                (ops.py:325-328, mac_cell.py:248-266)
+//                  outf != NULL also stores I1 in fp32 at outf[m * N + n] (the tc32 training forward's saved I1)
 //   TC_EPI_F32     act(acc + b + bias_const) -> fp32, stored or added (accum)   (generic ops.linear; act in every MAC_ACT_*)
 //   TC_EPI_ADDACT  act(acc + b + add[m,n]) -> bf16, add = bf16 [M, N]           (eval-mode read: step-invariant half of
 //                                                                                 the memKbProj concat, mac_cell.py:236-238)
 //   TC_EPI_ACT_SPLIT  x = act(acc + b + addf[m,n]) (addf fp32, optional) -> bf16 hi at out0[m, n] and bf16 lo = x - hi at
-//                     out0[m, N + n] (ldo = 2N): the A operand of the next split-bf16 ("tc32") product
+//                     out0[m, N + n] (ldo = 2N): the A operand of the next split-bf16 ("tc32") product; outf != NULL also
+//                     stores x in fp32 at outf[m * N + n] (the tc32 training forward's saved H, exactly as computed here)
 #pragma once
 #include "common.cuh"
 #include "tmap.cuh"
@@ -157,7 +159,9 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
-template <int EPI, int ACT>
+// SAVE (TC_EPI_ACT_SPLIT / TC_EPI_LOGITS with outf != NULL): a separate instantiation, so the inference form's kernels
+// (outf == NULL) are compiled exactly as without the fp32 store
+template <int EPI, int ACT, bool SAVE = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
                const __grid_constant__ CUtensorMap map_b, const TcGemmParams p) {
@@ -276,6 +280,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
           }
           x0 = act_ct<ACT>(x0);
           x1 = act_ct<ACT>(x1);
+          if constexpr (SAVE) *reinterpret_cast<float2*>(p.outf + (size_t)row * p.N + n) = make_float2(x0, x1);
           const uint32_t hw = pack_bf16(x0, x1);
           *reinterpret_cast<uint32_t*>(p.out0 + o) = hw;
           *reinterpret_cast<uint32_t*>(p.out0 + o + p.N) =
@@ -299,6 +304,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         const float2 cc = __ldg(reinterpret_cast<const float2*>(p.ctrl + (size_t)bidx * p.N + n));
         const float2 ww = make_float2(__ldg(p.wr + n), __ldg(p.wr + n + 1));
         if (p.out0 && row_ok) *reinterpret_cast<uint32_t*>(p.out0 + o) = pack_bf16(x0, x1);   // I1 kept for backward
+        if constexpr (SAVE)
+          if (row_ok) *reinterpret_cast<float2*>(p.outf + (size_t)row * p.N + n) = make_float2(x0, x1);
         float t0 = elu_fast(x0 * cc.x), t1 = elu_fast(x1 * cc.y);
         if (p.e_thresh) {
           // one Philox draw per aligned column quad of element index row * N + n (the fp32 path's numbering)
@@ -324,10 +331,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
 // ------------------------------------------------------------------ host side
 inline int tc_num_sms() { return mac_num_sms(); }
 
-template <int EPI, int ACT>
+template <int EPI, int ACT, bool SAVE = false>
 inline int tc_gemm_launch_t(const CUtensorMap& ma0, const CUtensorMap& ma1, const CUtensorMap& mb,
                             const TcGemmParams& p, cudaStream_t stream) {
-  auto kern = tc_gemm_kernel<EPI, ACT>;
+  auto kern = tc_gemm_kernel<EPI, ACT, SAVE>;
   // the shared-memory opt-in belongs to the current device's context: set it on every launch
   MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
   const dim3 grid(p.N / TC_BN, (p.M + TC_BM - 1) / TC_BM, p.ksplit > 1 ? p.ksplit : 1);
@@ -343,8 +350,14 @@ inline int tc_gemm_dispatch(const CUtensorMap& ma0, const CUtensorMap& ma1, cons
     case TC_EPI_ADDACT:
       if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<TC_EPI_ADDACT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
       return MAC_ERR_UNSUPPORTED;
-    case TC_EPI_LOGITS: return tc_gemm_launch_t<TC_EPI_LOGITS, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
+    case TC_EPI_LOGITS:
+      if (p.outf) return tc_gemm_launch_t<TC_EPI_LOGITS, MAC_ACT_NON, true>(ma0, ma1, mb, p, stream);
+      return tc_gemm_launch_t<TC_EPI_LOGITS, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
     case TC_EPI_ACT_SPLIT:
+      if (p.outf) {
+        if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<TC_EPI_ACT_SPLIT, MAC_ACT_ELU, true>(ma0, ma1, mb, p, stream);
+        return MAC_ERR_UNSUPPORTED;
+      }
       if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<TC_EPI_ACT_SPLIT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
       if (p.act == MAC_ACT_NON) return tc_gemm_launch_t<TC_EPI_ACT_SPLIT, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
       return MAC_ERR_UNSUPPORTED;
@@ -413,11 +426,15 @@ __global__ void pack_weight_bf16_kernel(const float* __restrict__ W, __nv_bfloat
 //   (one draw per aligned column quad, element index row*N + col: mac_dropout_fwd's numbering).      N % 4 == 0, K % 2 == 0.
 // ldx is the row pitch of X (elements); Xt rows have pitch ldt >= K, and columns K..ldt-1 of Xt are written as zeros (a
 // contraction length padded to the 64-wide k-block).
-template <int MODE>
+// Split mode (SEGS = 2 or 3, the operands of the split-bf16 "tc32" weight gradients): every value v is written as hi = bf16(v)
+// and lo = bf16(v - hi) into segments of kp columns of an Xt row (pitch ldt = SEGS * kp): [hi | lo] (SEGS 2) or [hi | hi | lo]
+// (SEGS 3), each with zero columns K..kp-1; Xrm (if given) receives the row-major [hi | lo] copy [K, 2N].
+template <int MODE, int SEGS = 0>
 __global__ void __launch_bounds__(256) pack_t_bf16_kernel(const float* __restrict__ X, __nv_bfloat16* __restrict__ Xt,
                                                          __nv_bfloat16* __restrict__ Xrm, int K, int N,
                                                          const float* __restrict__ rowvec, int rows_per_batch, uint32_t thresh,
-                                                         float scale, uint64_t seed, int site, int step, int ldx, int ldt) {
+                                                         float scale, uint64_t seed, int site, int step, int ldx, int ldt,
+                                                         int kp = 0) {
   __shared__ float tile[64][65];                              // [col][row]
   const int k0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
   const int tq = threadIdx.x & 15, tr = threadIdx.x >> 4;     // 16 column quads x 16 rows per pass
@@ -440,7 +457,15 @@ __global__ void __launch_bounds__(256) pack_t_bf16_kernel(const float* __restric
         v.z = ((r.z >> 8) >= thresh) ? v.z * scale : 0.f;
         v.w = ((r.w >> 8) >= thresh) ? v.w * scale : 0.f;
       }
-      if (Xrm) *reinterpret_cast<uint2*>(Xrm + (size_t)k * N + n) = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+      if (Xrm && SEGS == 0) {
+        *reinterpret_cast<uint2*>(Xrm + (size_t)k * N + n) = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+      } else if (Xrm) {
+        const uint32_t h01 = pack_bf16(v.x, v.y), h23 = pack_bf16(v.z, v.w);
+        const uint32_t l01 = pack_bf16(v.x - __uint_as_float(h01 << 16), v.y - __uint_as_float(h01 & 0xffff0000u));
+        const uint32_t l23 = pack_bf16(v.z - __uint_as_float(h23 << 16), v.w - __uint_as_float(h23 & 0xffff0000u));
+        *reinterpret_cast<uint2*>(Xrm + (size_t)k * 2 * N + n) = make_uint2(h01, h23);
+        *reinterpret_cast<uint2*>(Xrm + (size_t)k * 2 * N + N + n) = make_uint2(l01, l23);
+      }
     }
     tile[tq * 4 + 0][kk] = v.x;
     tile[tq * 4 + 1][kk] = v.y;
@@ -449,10 +474,25 @@ __global__ void __launch_bounds__(256) pack_t_bf16_kernel(const float* __restric
   }
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if constexpr (SEGS == 0) {
+    for (int r = warp; r < 64; r += 8) {
+      const int n = n0 + r, k = k0 + 2 * lane;
+      if (n < N && k + 1 < ldt)
+        *reinterpret_cast<uint32_t*>(Xt + (size_t)n * ldt + k) = pack_bf16(tile[r][2 * lane], tile[r][2 * lane + 1]);
+    }
+  } else {
   for (int r = warp; r < 64; r += 8) {
     const int n = n0 + r, k = k0 + 2 * lane;
-    if (n < N && k + 1 < ldt)
-      *reinterpret_cast<uint32_t*>(Xt + (size_t)n * ldt + k) = pack_bf16(tile[r][2 * lane], tile[r][2 * lane + 1]);
+    if (n < N && k + 1 < kp) {
+      const float a = tile[r][2 * lane], b = tile[r][2 * lane + 1];
+      const uint32_t hw = pack_bf16(a, b);
+      const uint32_t lw = pack_bf16(a - __uint_as_float(hw << 16), b - __uint_as_float(hw & 0xffff0000u));
+      __nv_bfloat16* row = Xt + (size_t)n * ldt + k;
+      *reinterpret_cast<uint32_t*>(row) = hw;
+      *reinterpret_cast<uint32_t*>(row + kp) = SEGS == 3 ? hw : lw;
+      if (SEGS == 3) *reinterpret_cast<uint32_t*>(row + 2 * kp) = lw;
+    }
+  }
   }
 }
 
@@ -481,6 +521,32 @@ inline int pack_t_bf16_launch(int mode, const float* X, void* Xt, void* Xrm, int
   else
     pack_t_bf16_kernel<2><<<grid, 256, 0, stream>>>(X, t, r, K, N, nullptr, 1, a.thresh, a.scale, a.seed, a.site, a.step, ldx,
                                                     ldt);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+// split mode of pack_t_bf16 (see the kernel): X [K, N] (pitch N) -> Xt [N, segs * kp] with kp = K rounded up to 64, segs 2
+// ([hi | lo], modes 0, 1, 2: the activations) or 3 ([hi | hi | lo], mode 0: the gradients), row pitch segs * kp; Xrm (may
+// be NULL): [K, 2N] [hi | lo]
+inline int pack_t_split_launch(int mode, const float* X, void* Xt, void* Xrm, int K, int N, int segs, const PackTArgs& a,
+                               cudaStream_t stream) {
+  if (!X || !Xt || K <= 0 || N <= 0 || (N & 3) || (segs != 2 && segs != 3) || mode < 0 || mode > 2 || (segs == 3 && mode))
+    return MAC_ERR_INVALID;
+  const int kp = (K + 63) & ~63;
+  const int ldt = segs * kp;
+  dim3 grid((N + 63) / 64, kp / 64);
+  __nv_bfloat16* t = reinterpret_cast<__nv_bfloat16*>(Xt);
+  __nv_bfloat16* r = reinterpret_cast<__nv_bfloat16*>(Xrm);
+  if (segs == 3)
+    pack_t_bf16_kernel<0, 3><<<grid, 256, 0, stream>>>(X, t, r, K, N, nullptr, 1, 0u, 1.f, 0, 0, 0, N, ldt, kp);
+  else if (mode == 0)
+    pack_t_bf16_kernel<0, 2><<<grid, 256, 0, stream>>>(X, t, r, K, N, nullptr, 1, 0u, 1.f, 0, 0, 0, N, ldt, kp);
+  else if (mode == 1)
+    pack_t_bf16_kernel<1, 2><<<grid, 256, 0, stream>>>(X, t, r, K, N, a.rowvec, a.rows_per_batch, 0u, 1.f, 0, 0, 0, N, ldt,
+                                                       kp);
+  else
+    pack_t_bf16_kernel<2, 2><<<grid, 256, 0, stream>>>(X, t, r, K, N, nullptr, 1, a.thresh, a.scale, a.seed, a.site, a.step,
+                                                       N, ldt, kp);
   MAC_LAUNCH_CHECK();
   return MAC_OK;
 }
@@ -711,7 +777,9 @@ inline int tc_wgrad_splitk(const void* xT, const void* gT, float* dW, float* par
 // With A' = [A_hi | A_lo] ([M, 2K]) and W' = [W_hi | W_hi | W_lo] ([N, 3K], K-major) this is the existing two-segment GEMM:
 // segment 0 = A'[:, 0:2K] against W'[:, 0:2K], segment 1 = A'[:, 0:K] against W'[:, 2K:3K] -- K triples, nothing else
 // changes.  Producers write their outputs directly as hi | lo pairs (TC_EPI_ACT_SPLIT) or as fp32 (TC_EPI_F32).
-// Inference form only (P, Q hoisted, mac_read_invariant): inv = [P fp32 | Q fp32 | scratch [M, 2d] bf16].
+// Inference form (P, Q hoisted, mac_read_invariant): inv = [P fp32 | Q fp32 | scratch [M, 2d] bf16].
+// Training form (tc3_read_chain_train): P = dropout(KB) @ Wx + bx, H = ELU([P*y | P] @ Wm + bm) as ONE split product over
+// K = 2d (A' = [(P*y)_hi | P_hi | (P*y)_lo | P_lo], W' = split3 of the whole Wm), I1 = H @ Wm2 + bm2, all saved in fp32.
 // ---------------------------------------------------------------------------------------------------------------
 // out[m, c] = hi(x[m, c] * y[m / rows_per_batch, c]), out[m, d + c] = lo(...)     (y == NULL: plain split); 4 columns / thread
 __global__ void split_rows_kernel(const float4* __restrict__ x, const float* __restrict__ y, uint2* __restrict__ out,
@@ -740,6 +808,76 @@ inline int split_rows_launch(const float* x, const float* y, void* out, int rows
                                                                       reinterpret_cast<uint2*>(out), rows_per_batch, d, n4);
   MAC_LAUNCH_CHECK();
   return MAC_OK;
+}
+
+// The training form's splits (tc3_read_chain_train):
+struct SplitRowsArgs {
+  const float* y = nullptr;    // row scale y[m / rows_per_batch, c] (NULL: none)
+  int rows_per_batch = 1;
+  int both = 0;                // also write the unscaled x at columns d .. 2d of each half ([x*y | x] per half)
+  uint32_t thresh = 0;         // dropout(x) with the forward's Philox stream (0: none): one draw per aligned column quad of
+  float scale = 1.f;           //   element index m*d + c (mac_dropout_fwd's, dropout_cast_bf16_kernel's numbering)
+  uint64_t seed = 0;
+  int site = 0, step = 0;
+};
+// out[m, c] = hi(v), out[m, H + c] = lo(v) with v = dropout(x)[m, c] (* y[m / rows_per_batch, c]) and H = d (both: H = 2d,
+// and the unscaled x goes to columns d + c and H + d + c); 4 columns / thread
+__global__ void split_rows_train_kernel(const float4* __restrict__ x, uint2* __restrict__ out, int d, long long n4,
+                                        const SplitRowsArgs a) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n4) return;
+  const int d4 = d / 4;
+  const long long m = i / d4;
+  const int c4 = (int)(i - m * d4);
+  float4 v = x[i];
+  if (a.thresh) {
+    const Philox4 r = philox4x32_10(a.seed, (uint64_t)i, (uint32_t)a.site, (uint32_t)a.step);
+    v.x = ((r.x >> 8) >= a.thresh) ? v.x * a.scale : 0.f;
+    v.y = ((r.y >> 8) >= a.thresh) ? v.y * a.scale : 0.f;
+    v.z = ((r.z >> 8) >= a.thresh) ? v.z * a.scale : 0.f;
+    v.w = ((r.w >> 8) >= a.thresh) ? v.w * a.scale : 0.f;
+  }
+  const int half4 = a.both ? 2 * d4 : d4;
+  uint2* row = out + m * (2 * half4);
+  auto put = [&](float4 u, int col4) {
+    const uint32_t h01 = pack_bf16(u.x, u.y), h23 = pack_bf16(u.z, u.w);
+    const uint32_t l01 = pack_bf16(u.x - __uint_as_float(h01 << 16), u.y - __uint_as_float(h01 & 0xffff0000u));
+    const uint32_t l23 = pack_bf16(u.z - __uint_as_float(h23 << 16), u.w - __uint_as_float(h23 & 0xffff0000u));
+    row[col4] = make_uint2(h01, h23);
+    row[half4 + col4] = make_uint2(l01, l23);
+  };
+  if (a.both) put(v, d4 + c4);
+  if (a.y) {
+    const float4 s = __ldg(reinterpret_cast<const float4*>(a.y + (m / a.rows_per_batch) * d) + c4);
+    v.x *= s.x; v.y *= s.y; v.z *= s.z; v.w *= s.w;
+  }
+  put(v, c4);
+}
+inline int split_rows_train_launch(const float* x, void* out, int d, long long M, const SplitRowsArgs& a,
+                                   cudaStream_t stream) {
+  const long long n4 = M * d / 4;
+  split_rows_train_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(x),
+                                                                            reinterpret_cast<uint2*>(out), d, n4, a);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+// fp32 W[R, C] row-major -> bf16 W3[R, 3C] = [hi | hi | lo] per row, no transpose: the B operand of a split data gradient
+// dX = G @ W^T with W in its own [in, out] layout (rows = in = the output columns of dX, K = out).  C % 4 == 0.
+__global__ void split3_rows_kernel(const float4* __restrict__ W, uint2* __restrict__ W3, int C, long long n4) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n4) return;
+  const int c4n = C / 4;
+  const long long r = i / c4n;
+  const int c4 = (int)(i - r * c4n);
+  const float4 u = W[i];
+  const uint32_t h01 = pack_bf16(u.x, u.y), h23 = pack_bf16(u.z, u.w);
+  const uint32_t l01 = pack_bf16(u.x - __uint_as_float(h01 << 16), u.y - __uint_as_float(h01 & 0xffff0000u));
+  const uint32_t l23 = pack_bf16(u.z - __uint_as_float(h23 << 16), u.w - __uint_as_float(h23 & 0xffff0000u));
+  uint2* row = W3 + r * (3 * c4n);
+  row[c4] = make_uint2(h01, h23);
+  row[c4n + c4] = make_uint2(h01, h23);
+  row[2 * c4n + c4] = make_uint2(l01, l23);
 }
 
 // fp32 W[K, N] (rows k0 .. k0+K of a wider [*, N] weight are passed as W + k0*N) -> bf16 Wt3[N, 3K] = [hi | hi | lo]
@@ -818,6 +956,62 @@ inline int tc3_read_chain_inv(const void* inv, const float* y, const float* cont
   p.epi = TC_EPI_LOGITS; p.act = MAC_ACT_NON; p.bias = w->bm2; p.addf = nullptr; p.out0 = nullptr; p.ldo = d;
   p.ctrl = control; p.wr = w->wr; p.parts = parts;
   return tc3_gemm(Hs, d, w->Wm2_s3, p, stream, nparts);                  // logits partial sums         (mac_cell.py:248-266)
+}
+
+// Training form (mac_read_fwd with MAC_PREC_TC32 and no `inv`): P, H, I1 in fp32 into P_f32 / H_f32 / I1_f32 (the caller's
+// `save`, or P into scratch and H, I1 not stored when there is none).  Scratch:
+//   s2   [M, 4d] bf16 (= M*d*8 bytes, 16-byte aligned): dropout(KB) as [hi | lo] in its first half, then A' of the H product
+//   ws   tc3_extra_workspace_bytes: H as [hi | lo] [M, 2d] in slab 1; slab 0 holds P when P_f32 is NULL
+// The caller has checked d % 128 == 0 and the packs (Wx_s3, Wm_s3, Wm2_s3) before any launch.
+inline int tc3_read_chain_train(const float* kb, const float* y, const float* control, const mac_read_weights* w, uint32_t thr,
+                                float scale, uint64_t seed, int step, float* P_f32, float* H_f32, float* I1_f32, float* parts,
+                                int* nparts, void* s2, void* ws, int B, int N, int d, cudaStream_t stream) {
+  const int M = B * N;
+  char* base = tc_align1k(ws);
+  float* P = P_f32 ? P_f32 : reinterpret_cast<float*>(base);
+  void* Hs = base + tc3_slab(B, N, d);
+  SplitRowsArgs sa;
+  sa.thresh = thr; sa.scale = scale; sa.seed = seed; sa.site = MAC_SITE_READ_KB; sa.step = step;
+  int st = split_rows_train_launch(kb, s2, d, M, sa, stream);                  // dropout(KB) as hi | lo   (ops.py:678)
+  if (st != MAC_OK) return st;
+  TcGemmParams p{};
+  p.M = M; p.N = d; p.rows_per_batch = N; p.ldo = d; p.seed = seed; p.step = step;
+  p.epi = TC_EPI_F32; p.act = MAC_ACT_NON; p.bias = w->bx; p.outf = P;
+  st = tc3_gemm(s2, d, w->Wx_s3, p, stream);                             // P = dropout(KB) @ Wx + bx  (ops.py:688)
+  if (st != MAC_OK) return st;
+  SplitRowsArgs sb;
+  sb.y = y; sb.rows_per_batch = N; sb.both = 1;
+  st = split_rows_train_launch(P, s2, d, M, sb, stream);                       // [(P*y)_hi | P_hi | (P*y)_lo | P_lo]
+  if (st != MAC_OK) return st;
+  p.epi = TC_EPI_ACT_SPLIT; p.act = MAC_ACT_ELU; p.bias = w->bm; p.outf = H_f32; p.out0 = reinterpret_cast<__nv_bfloat16*>(Hs);
+  p.ldo = 2 * d;
+  st = tc3_gemm(s2, 2 * d, w->Wm_s3, p, stream);                         // H = ELU([P*y | P] @ Wm + bm)  (mac_cell.py:236-238)
+  if (st != MAC_OK) return st;
+  p.epi = TC_EPI_LOGITS; p.act = MAC_ACT_NON; p.bias = w->bm2; p.outf = I1_f32; p.out0 = nullptr; p.ldo = d;
+  p.ctrl = control; p.wr = w->wr; p.parts = parts;
+  p.e_thresh = thr; p.e_scale = scale; p.e_site = MAC_SITE_READ_INTER;
+  return tc3_gemm(Hs, d, w->Wm2_s3, p, stream, nparts);                  // I1, logits partial sums  (mac_cell.py:248-266)
+}
+
+// Split-bf16 weight gradient dW[in, out] += X^T G over a contraction of kp (= M rounded up to 64) rows:
+//   xT2 = [X_hi^T | X_lo^T] [in, 2kp], gT3 = [G_hi^T | G_hi^T | G_lo^T] [out, 3kp] (pack_t_split_launch, zero columns M..kp-1)
+// is tc3_gemm's two-segment product (X_hi G_hi + X_lo G_hi + X_hi G_lo) as ONE split-K launch over K = 3kp, whose slices are
+// summed in slice order (deterministic).  `partial` holds tc_wgrad_partial_bytes(in, out).
+inline int tc3_wgrad_splitk(const void* xT2, const void* gT3, float* dW, float* partial, int in_dim, int out_dim, int kp,
+                            cudaStream_t stream) {
+  if ((in_dim % 128) || (out_dim % 128) || (kp % TC_BK)) return MAC_ERR_UNSUPPORTED;
+  TcGemmParams p{};
+  p.M = in_dim; p.N = out_dim; p.act = MAC_ACT_NON; p.bias = nullptr; p.ldo = out_dim; p.rows_per_batch = 1;
+  p.epi = TC_EPI_F32; p.outf = partial;
+  const int S = tc_pick_ksplit(3 * kp, (in_dim / TC_BM) * (out_dim / TC_BN));
+  p.ksplit = S; p.split_stride = (long long)in_dim * out_dim;
+  int st = tc3_gemm(xT2, kp, gT3, p, stream);
+  if (st != MAC_OK) return st;
+  const long long n4 = (long long)in_dim * out_dim / 4;
+  splitk_accum_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(partial),
+                                                                       reinterpret_cast<float4*>(dW), n4, S, n4, 1);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
 }
 
 }  // namespace mac

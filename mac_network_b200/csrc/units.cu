@@ -220,6 +220,10 @@ static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, 
   // e4m3: the inference read step only, checked before anything is launched
   if (prec == MAC_PREC_FP8 && (!inv || !kb_bf16 || keep_read < 1.f || save || !read_step_supported(B, N, d)))
     return MAC_ERR_UNSUPPORTED;
+  // split-bf16 training form: whole 128-wide wgmma tiles and its three packs, checked before anything is launched
+  const bool tc3_train = prec == MAC_PREC_TC32 && !inv;
+  if (tc3_train && (d <= 0 || d % 128)) return MAC_ERR_UNSUPPORTED;
+  if (tc3_train && (!w || !w->Wx_s3 || !w->Wm_s3 || !w->Wm2_s3)) return MAC_ERR_INVALID;
   // eval bf16 / fp8 path: only the bf16 copy is read
   const bool kb_opt = inv && (prec == MAC_PREC_BF16 || prec == MAC_PREC_FP8) && kb_bf16;
   if ((!kb && !kb_opt) || !memory_in || !control || !w || !info || !att || !workspace) return MAC_ERR_INVALID;
@@ -274,8 +278,12 @@ static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, 
     // the whole step (P*y, both projections, logits, softmax, weighted sum) as ONE kernel: read_step.cuh
     return read_step_launch(inv, kb_bf16, y, control, w, att, info, B, N, d, stream);
   }
-  if (prec == MAC_PREC_TC32) {
-    if (!inv) return MAC_ERR_UNSUPPORTED;          // split-bf16 products: inference form only
+  if (tc3_train) {
+    // the fp32 layout's P and H regions (contiguous, [M, 4d] bf16 together) hold the split operands; P, H, I1 go to `save`
+    int st = tc3_read_chain_train(kb, y, control, w, thr, scale, seed, step, save ? P : nullptr, save ? H : nullptr, I1,
+                                  parts, &nparts, ws + o_P, ws + fp32_total, B, N, d, stream);
+    if (st != MAC_OK) return st;
+  } else if (prec == MAC_PREC_TC32) {
     int st = tc3_read_chain_inv(inv, y, control, w, parts, &nparts, ws + fp32_total, workspace_bytes - fp32_total, B, N, d,
                                 stream);
     if (st != MAC_OK) return st;
@@ -499,6 +507,36 @@ extern "C" int mac_pack_t_bf16_(int mode, const float* X, void* Xt, void* Xrm, i
   a.rowvec = rowvec; a.rows_per_batch = rows_per_batch; a.thresh = thresh; a.scale = scale; a.seed = seed; a.site = site;
   a.step = step;
   return pack_t_bf16_launch(mode, X, Xt, Xrm, K, N, a, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+// internal: the split-bf16 ("tc32") pieces of mac_read_bwd_tc32 (backward.cu)
+extern "C" int mac_pack_t_split_(int mode, const float* X, void* Xt, void* Xrm, int K, int N, int segs, const float* rowvec,
+                                 int rows_per_batch, uint32_t thresh, float scale, uint64_t seed, int site, int step,
+                                 mac_stream_t stream_) {
+  PackTArgs a;
+  a.rowvec = rowvec; a.rows_per_batch = rows_per_batch; a.thresh = thresh; a.scale = scale; a.seed = seed; a.site = site;
+  a.step = step;
+  return pack_t_split_launch(mode, X, Xt, Xrm, K, N, segs, a, reinterpret_cast<cudaStream_t>(stream_));
+}
+extern "C" int mac_tc3_wgrad_splitk_(const void* xT2, const void* gT3, float* dW, float* partial, int in_dim, int out_dim,
+                                     int kp, mac_stream_t stream_) {
+  return tc3_wgrad_splitk(xT2, gT3, dW, partial, in_dim, out_dim, kp, reinterpret_cast<cudaStream_t>(stream_));
+}
+// W [R, C] fp32 -> [R, 3C] = [hi | hi | lo] per row (split3_rows_kernel)
+extern "C" int mac_split3_rows_(const float* W, void* W3, int R, int C, mac_stream_t stream_) {
+  if (!W || !W3 || R <= 0 || C <= 0 || (C & 3)) return MAC_ERR_INVALID;
+  const long long n4 = (long long)R * C / 4;
+  split3_rows_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      reinterpret_cast<const float4*>(W), reinterpret_cast<uint2*>(W3), C, n4);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+// y[M, n_out] = A @ W with A' = [A_hi | A_lo] [M, 2K] and W' [n_out, 3K] (tc3_gemm, fp32 out, stored)
+extern "C" int mac_tc3_linear_(const void* a_split, const void* wt3, float* y, int M, int K, int n_out, mac_stream_t stream_) {
+  TcGemmParams p{};
+  p.M = M; p.N = n_out; p.act = MAC_ACT_NON; p.bias = nullptr; p.ldo = n_out; p.rows_per_batch = 1;
+  p.epi = TC_EPI_F32; p.outf = y;
+  return tc3_gemm(a_split, K, wt3, p, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int mac_widen_bf16(const void* const* src_bf16, float* const* dst, int nslab, long long n, mac_stream_t stream_) {

@@ -48,6 +48,9 @@ class DPTrainer(object):
         fused kernel the composed read unit's [B*N, .] products run on `mac_linear_tc_seg_fwd` / `mac_linear_bwd_tc`
         (memDim and attDim multiples of 128), and a cell differentiated on the tape (`tape.py`) runs its fused read unit
         backward on `mac_read_bwd_tc` (B*N a multiple of 64); the batch-sized products stay fp32 (DESIGN.md section 9).
+        `prec="tc32"` trains the fused read unit's [B*N, .] products as split-bf16 tensor-core products inside the fp32
+        parity bar (shipped flag files, memDim a multiple of 128, any B*N); with `bwd_tc=True` its backward products are
+        split-bf16 too (`mac_read_bwd_tc32`), with `bwd_tc=False` they run on the fp32 `mac_read_bwd`.
         `stem_prec="bf16"` trains the image stem on tensor cores too (forward `mac_linear_tc_fwd`, backward
         `mac_conv3x3_bwd_tc`; every stem channel count must be a multiple of 128).  `enc_prec="bf16"` trains the question
         encoder's LSTM on tensor cores (`QuestionEncoder(prec="bf16")`; needs ctrlDim = 512, i.e. h = 256 per direction).

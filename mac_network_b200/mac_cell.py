@@ -232,9 +232,12 @@ class MACCell(object):
             raise NotImplementedError('prec="bf16" with the composed read unit needs d %% 128 == 0 and attDim %% 128 == 0 '
                                       "(got d = %d, attDim = %d)" % (d, c.attDim))
         self._lin_tc_ws = None
-        if self.prec == PREC["tc32"] and (save_for_backward or not self._read_hoist or float(readDropout) < 1.0 or d % 128):
-            raise NotImplementedError('prec="tc32" (split-bf16 tensor-core projections inside the 1e-4 bar) is the inference '
-                                      "form of the fused read unit: shared cells, readDropout = 1, d % 128 == 0")
+        # tc32 training (save_for_backward) runs mac_read_fwd's split-bf16 training form and mac_read_bwd_tc32 under the
+        # scheduled backward: the fused read unit, d % 128 == 0 and an fp32 knowledge base (checked above; the tape rejects it)
+        if self.prec == PREC["tc32"] and not save_for_backward and (not self._read_hoist or float(readDropout) < 1.0
+                                                                    or d % 128):
+            raise NotImplementedError('prec="tc32" (split-bf16 tensor-core projections inside the 1e-4 bar) in inference is '
+                                      "the hoisted form of the fused read unit: shared cells, readDropout = 1, d % 128 == 0")
         if self.prec == PREC["fp8"] and (save_for_backward or not self._read_hoist or float(readDropout) < 1.0
                                          or not (d == 512 and 1 <= N <= 256 and B < 2 ** 22)):
             raise NotImplementedError('prec="fp8" (e4m3 read step, csrc/read_step_fp8.cuh) is the inference form of the fused '
@@ -497,6 +500,8 @@ class MACCell(object):
             d_ = self.d
             keep3 = p.derived(("split3", sc), lambda: (pack3(Wx), pack3(Wm[:d_]), pack3(Wm[d_:]), pack3(Wm2)))
             rw.Wx_s3, rw.Wma_s3, rw.Wmb_s3, rw.Wm2_s3 = (t.data_ptr() for t in keep3)
+            if self.save_for_backward:   # training form: H = ELU([P*y | P] @ Wm + bm) as one product over K = 2d
+                rw.Wm_s3 = p.derived(("split3_wm", sc), lambda: pack3(Wm)).data_ptr()
         if self.prec == PREC["fp8"]:
             def pack8(t):      # fp32 [in, out] -> e4m3 [out, in] and the fp32 scale of each output column
                 o = torch.empty((t.shape[1], t.shape[0]), dtype=torch.uint8, device=t.device)
