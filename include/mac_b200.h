@@ -115,9 +115,13 @@ int mac_control_attend_fwd(const float* cc, long long cc_tstride, long long cc_b
  *   kl = dropout(I2, keep_read) . wr + br                   (mac_cell.py:266, ops.py:312-317)
  *   att = softmax_n(kl);  info = sum_n att * KB             (ops.py:143, 149-150; original KB, mac_cell.py:271-275)
  * Training: keep_read < 1 draws Philox4x32-10 masks from (seed, step) (see mac_dropout_uniform);
- * `save` (may be NULL) receives P, H, I1 ([B*N,d] each, in that order) and y ([B,d]) for backward.
+ * `save` (may be NULL, 16-byte aligned) receives P, H, I1 ([B*N,d] each, in that order) and y ([B,d]) for backward, in
+ * fp32 for every precision: MAC_PREC_BF16 computes P, H and I1 in bf16 and widens them into `save` (one more launch).
  * MAC_PREC_FP32 takes every d % 4 == 0 up to d <= 2048 when B*N < 512 and d <= 4096 otherwise (at most 32 partial logits
- * per row, one per 64- or 128-column tile); a wider d returns MAC_ERR_UNSUPPORTED before any launch.
+ * per row, one per 64- or 128-column tile).  MAC_PREC_BF16 and MAC_PREC_TC32 take d % 128 == 0 up to d <= 4096 and need
+ * the packs they read (see mac_read_weights; MAC_PREC_BF16 also kb_bf16).
+ * mac_read_fwd, mac_read_fwd_inv and mac_read_invariant return every MAC_ERR_* before any launch and before any write:
+ * a refused call leaves info, att, save, inv and the workspace as they were.
  * --------------------------------------------------------------------------------------------- */
 typedef struct mac_read_weights {
   const float* Wx;  const float* bx;   /* read/mulmemInter/linearLayerprojX            [d,d],[d]  */

@@ -345,29 +345,28 @@ read_step_kernel(const __grid_constant__ CUtensorMap map_p, const __grid_constan
   }
 }
 
-// inv = [P | Q] (tc_read_invariant); y, control [B, d] fp32; att [B, N], info [B, d]
-inline int read_step_launch(const void* inv, const void* kb_bf16, const float* y, const float* control,
-                            const mac_read_weights* w, float* att, float* info, int B, int N, int d, cudaStream_t stream) {
-  if (!read_step_supported(B, N, d)) return MAC_ERR_UNSUPPORTED;
-  if (!inv || !kb_bf16 || !y || !control || !w->Wm_bf16 || !w->Wm2_bf16 || !att || !info) return MAC_ERR_INVALID;
+// P, Q bf16 [B*N, d] and the logits [B*N] from mac_read_invariant's `inv` (read_inv_layout); y, control [B, d] fp32; att [B, N],
+// info [B, d].  The caller has checked read_step_supported and every pointer (Wm_bf16, Wm2_bf16 included).
+inline int read_step_launch(const void* P, const void* Q, float* logits, const void* kb_bf16, const float* y,
+                            const float* control, const mac_read_weights* w, float* att, float* info, int B, int N, int d,
+                            cudaStream_t stream) {
   const int M = B * N;
-  const TcReadScratch s = tc_read_scratch(const_cast<void*>(inv), B, N, d);
   CUtensorMap mp, mq, mw1, mw2;
-  int st = make_tmap_2d(&mp, s.P, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS128_BM, TC_BK, 1);
+  int st = make_tmap_2d(&mp, P, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS128_BM, TC_BK, 1);
   if (st != MAC_OK) return st;
-  st = make_tmap_2d(&mq, s.Q, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS128_BM, TC_BK, 1);
+  st = make_tmap_2d(&mq, Q, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS128_BM, TC_BK, 1);
   if (st != MAC_OK) return st;
   st = make_tmap_2d(&mw1, w->Wm_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)2 * d * 2, 256, TC_BK, 1);   // Wm[0:d] of [d, 2d]
   if (st != MAC_OK) return st;
   st = make_tmap_2d(&mw2, w->Wm2_bf16, 1, (uint64_t)d, (uint64_t)d, (uint64_t)d * 2, 256, TC_BK, 1);
   if (st != MAC_OK) return st;
   ReadStepParams p{};
-  p.M = M; p.N = N; p.y = y; p.ctrl = control; p.bm2 = w->bm2; p.wr = w->wr; p.logits = s.parts;
+  p.M = M; p.N = N; p.y = y; p.ctrl = control; p.bm2 = w->bm2; p.wr = w->wr; p.logits = logits;
   // the opt-in is per device context: set it on every launch
   MAC_CUDA_TRY(cudaFuncSetAttribute(read_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RS128_SMEM_BYTES));
   read_step_kernel<<<(M + RS128_BM - 1) / RS128_BM, RS128_THREADS, RS128_SMEM_BYTES, stream>>>(mp, mq, mw1, mw2, p);
   MAC_LAUNCH_CHECK();
-  return mac_kb_attend_fwd(s.parts, 1, w->br, kb_bf16, 1, att, info, B, N, d, stream);
+  return mac_kb_attend_fwd(logits, 1, w->br, kb_bf16, 1, att, info, B, N, d, stream);
 }
 
 }  // namespace mac

@@ -387,69 +387,17 @@ __global__ void __launch_bounds__(256) quant_rows_e4m3_kernel(const __nv_bfloat1
   if (lane == 0) sP[m] = s;
 }
 
-// inv = [P8 | sP | Q | logit scratch | P]: P8 [M, d] e4m3, sP [M] fp32, Q [M, d] bf16 (the bf16 path's Q), one logit per row,
-// and the bf16 P that P8 and Q are made from; each slab 1 KB aligned
-struct Fp8ReadScratch {
-  uint8_t* P8;
-  float* sP;
-  __nv_bfloat16* Q;
-  float* parts;
-  __nv_bfloat16* P;
-};
-inline size_t fp8_align1k(size_t b) { return (b + 1023) & ~(size_t)1023; }
-inline size_t fp8_read_invariant_bytes(int B, int N, int d) {
-  const size_t M = (size_t)B * N;
-  return fp8_align1k(M * d) + fp8_align1k(M * 4) + 2 * fp8_align1k(M * d * 2) + fp8_align1k(M * 4) + 1024;
-}
-inline Fp8ReadScratch fp8_read_scratch(void* inv, int B, int N, int d) {
-  const size_t M = (size_t)B * N;
-  char* o = tc_align1k(inv);
-  Fp8ReadScratch s;
-  s.P8 = reinterpret_cast<uint8_t*>(o);
-  o += fp8_align1k(M * d);
-  s.sP = reinterpret_cast<float*>(o);
-  o += fp8_align1k(M * 4);
-  s.Q = reinterpret_cast<__nv_bfloat16*>(o);
-  o += fp8_align1k(M * d * 2);
-  s.parts = reinterpret_cast<float*>(o);
-  o += fp8_align1k(M * 4);
-  s.P = reinterpret_cast<__nv_bfloat16*>(o);
-  return s;
-}
-
-// P = KB @ Wx + bx and Q = P @ Wm[d:2d] + bm exactly as tc_read_invariant computes them (bf16), then P8 and sP from P
-inline int fp8_read_invariant(const void* kb_bf16, const mac_read_weights* w, void* inv, size_t inv_bytes, int B, int N, int d,
-                              cudaStream_t stream) {
-  if (!read_step_supported(B, N, d)) return MAC_ERR_UNSUPPORTED;
-  if (!kb_bf16 || !w->Wx_bf16 || !w->Wm_bf16) return MAC_ERR_INVALID;
-  if (inv_bytes < fp8_read_invariant_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
+// one e4m3 read step: P8, sP, Q and the logits from mac_read_invariant's `inv` (read_inv_layout); y, control [B, d] fp32;
+// att [B, N], info [B, d].  The caller has checked read_step_supported, every pointer (the e4m3 packs and their scales
+// included) and the packs' alignment.
+inline int read_step_fp8_launch(const uint8_t* P8, const float* sP, const void* Q, float* logits, const void* kb_bf16,
+                                const float* y, const float* control, const mac_read_weights* w, float* att, float* info,
+                                int B, int N, int d, cudaStream_t stream) {
   const int M = B * N;
-  const Fp8ReadScratch s = fp8_read_scratch(inv, B, N, d);
-  TcGemmParams p{};
-  p.M = M; p.N = d; p.rows_per_batch = N; p.ldo = d;
-  p.epi = TC_EPI_ACT; p.act = MAC_ACT_NON; p.bias = w->bx; p.out0 = s.P;
-  int st = tc_gemm_launch(kb_bf16, d, nullptr, 0, w->Wx_bf16, p, stream);
-  if (st != MAC_OK) return st;
-  p.bias = w->bm; p.out0 = s.Q;
-  st = tc_gemm_launch(s.P, d, nullptr, 0, reinterpret_cast<const __nv_bfloat16*>(w->Wm_bf16) + d, p, stream, nullptr, 2 * d);
-  if (st != MAC_OK) return st;
-  quant_rows_e4m3_kernel<<<(M + 7) / 8, 256, 0, stream>>>(s.P, s.P8, s.sP, M);
-  MAC_LAUNCH_CHECK();
-  return MAC_OK;
-}
-
-// one e4m3 read step: inv from fp8_read_invariant; y, control [B, d] fp32; att [B, N], info [B, d]
-inline int read_step_fp8_launch(const void* inv, const void* kb_bf16, const float* y, const float* control,
-                                const mac_read_weights* w, float* att, float* info, int B, int N, int d, cudaStream_t stream) {
-  if (!read_step_supported(B, N, d)) return MAC_ERR_UNSUPPORTED;
-  if (!inv || !kb_bf16 || !y || !control || !w->Wm_fp8 || !w->Wm_fp8_scale || !w->Wm2_fp8 || !w->Wm2_fp8_scale || !att || !info)
-    return MAC_ERR_INVALID;
-  const int M = B * N;
-  const Fp8ReadScratch s = fp8_read_scratch(const_cast<void*>(inv), B, N, d);
   CUtensorMap mp, mq, mw1, mw2;
-  int st = make_tmap_2d(&mp, s.P8, 2, (uint64_t)M, (uint64_t)d, (uint64_t)d, RS_BM, R8_BK, 1);
+  int st = make_tmap_2d(&mp, P8, 2, (uint64_t)M, (uint64_t)d, (uint64_t)d, RS_BM, R8_BK, 1);
   if (st != MAC_OK) return st;
-  st = make_tmap_2d(&mq, s.Q, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS_BM, TC_BK, 1);
+  st = make_tmap_2d(&mq, Q, 1, (uint64_t)M, (uint64_t)d, (uint64_t)d * 2, RS_BM, TC_BK, 1);
   if (st != MAC_OK) return st;
   st = make_tmap_2d(&mw1, w->Wm_fp8, 2, (uint64_t)d, (uint64_t)d, (uint64_t)d, 256, R8_BK, 1);
   if (st != MAC_OK) return st;
@@ -457,12 +405,12 @@ inline int read_step_fp8_launch(const void* inv, const void* kb_bf16, const floa
   if (st != MAC_OK) return st;
   ReadStepFp8Params p{};
   p.M = M; p.N = N; p.y = y; p.ctrl = control; p.bm2 = w->bm2; p.wr = w->wr;
-  p.sP = s.sP; p.sw1 = w->Wm_fp8_scale; p.sw2 = w->Wm2_fp8_scale; p.logits = s.parts;
+  p.sP = sP; p.sw1 = w->Wm_fp8_scale; p.sw2 = w->Wm2_fp8_scale; p.logits = logits;
   // the opt-in is per device context: set it on every launch
   MAC_CUDA_TRY(cudaFuncSetAttribute(read_step_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, R8_SMEM_BYTES));
   read_step_fp8_kernel<<<(M + RS_BM - 1) / RS_BM, RS_THREADS, R8_SMEM_BYTES, stream>>>(mp, mq, mw1, mw2, p);
   MAC_LAUNCH_CHECK();
-  return mac_kb_attend_fwd(s.parts, 1, w->br, kb_bf16, 1, att, info, B, N, d, stream);
+  return mac_kb_attend_fwd(logits, 1, w->br, kb_bf16, 1, att, info, B, N, d, stream);
 }
 
 }  // namespace mac

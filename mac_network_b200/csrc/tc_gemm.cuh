@@ -380,14 +380,13 @@ inline int tc_gemm_dispatch(const CUtensorMap& ma0, const CUtensorMap& ma1, cons
 
 // A = [a0 (K0 cols) | a1 (K1 cols)] bf16 row-major (ld = own K), Wt bf16 [N, K0+K1]
 inline int tc_gemm_launch(const void* a0, int K0, const void* a1, int K1, const void* wt, TcGemmParams p,
-                          cudaStream_t stream, int* nparts_per_row = nullptr, int ldw = 0, int lda0 = 0, int lda1 = 0) {
+                          cudaStream_t stream, int ldw = 0, int lda0 = 0, int lda1 = 0) {
   if (ldw == 0) ldw = K0 + K1;                  // row pitch of Wt in elements (> K: a column block of a wider weight)
   if (lda0 == 0) lda0 = K0;                     // row pitch of the A segments (> K: a column block of a wider matrix)
   if (lda1 == 0) lda1 = K1;
   if (p.M <= 0 || p.N <= 0 || (p.N % TC_BN) || (K0 % TC_BK) || (K1 % TC_BK) || K0 <= 0) return MAC_ERR_UNSUPPORTED;
   if (!mac_aligned16(a0) || !mac_aligned16(wt)) return MAC_ERR_ALIGN;
   if (p.ksplit > 1 && ((K0 + K1) / TC_BK) % p.ksplit) return MAC_ERR_UNSUPPORTED;
-  if (nparts_per_row) *nparts_per_row = p.N / TC_BN;
   p.K = K0 + K1;
   p.kblocks0 = K0 / TC_BK;
   CUtensorMap ma0, ma1, mb;
@@ -566,162 +565,24 @@ __global__ void __launch_bounds__(256) widen3_bf16_kernel(const uint4* __restric
                                __uint_as_float(v.w & 0xffff0000u));
   }
 }
-
-// training mode: bf16 copy of dropout(KB) for this step (ops.py:678), same Philox stream as the fp32 path
-__global__ void dropout_cast_bf16_kernel(const float4* __restrict__ x, uint2* __restrict__ out, uint32_t thresh,
-                                         float scale, uint64_t seed, int site, int step, long long n4) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n4) return;
-  const float4 v = x[i];
-  const Philox4 r = philox4x32_10(seed, (uint64_t)i, (uint32_t)site, (uint32_t)step);
-  const float a = ((r.x >> 8) >= thresh) ? v.x * scale : 0.f, b = ((r.y >> 8) >= thresh) ? v.y * scale : 0.f;
-  const float c = ((r.z >> 8) >= thresh) ? v.z * scale : 0.f, d = ((r.w >> 8) >= thresh) ? v.w * scale : 0.f;
-  out[i] = make_uint2(pack_bf16(a, b), pack_bf16(c, d));
-}
-
-// extra workspace of the bf16 read chain: P, P*y, H (+ I1 when saving for backward), each [B*N, d] bf16
-inline size_t tc_read_extra_workspace_bytes(int B, int N, int d) {
-  return (size_t)5 * (((size_t)B * N * d * 2 + 1023) & ~(size_t)1023) + 1024;     // P, P*y, H, I1, dropout(KB)
-}
-
-// The read unit's three projections on tensor cores (see mac_read_fwd in mac_b200.h).
-inline int tc_read_chain(const float* kb_f32, const void* kb_bf16, const float* y, const float* control, const mac_read_weights* w,
-                         uint32_t thr, float scale, uint64_t seed, int step, float* /*P_f32*/, float* /*H_f32*/,
-                         float* /*I1_f32*/, float* parts, int* nparts, void* ws, size_t ws_bytes, int B, int N, int d,
-                         bool save, cudaStream_t stream) {
-  if (!kb_bf16 || !w->Wx_bf16 || !w->Wm_bf16 || !w->Wm2_bf16) return MAC_ERR_INVALID;
-  if (d % 128) return MAC_ERR_UNSUPPORTED;
-  if (ws_bytes < tc_read_extra_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
-  const int M = B * N;
-  const size_t slab = (((size_t)M * d * 2 + 1023) & ~(size_t)1023);
-  char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(ws) + 1023) & ~(uintptr_t)1023);
-  __nv_bfloat16* P = reinterpret_cast<__nv_bfloat16*>(base);
-  __nv_bfloat16* PY = reinterpret_cast<__nv_bfloat16*>(base + slab);
-  __nv_bfloat16* H = reinterpret_cast<__nv_bfloat16*>(base + 2 * slab);
-  __nv_bfloat16* I1 = save ? reinterpret_cast<__nv_bfloat16*>(base + 3 * slab) : nullptr;
-  if (thr != 0) {
-    // A operand of the first projection = dropout(KB) (ops.py:678): TMA cannot mask in flight, so make this step's copy
-    __nv_bfloat16* kbd = reinterpret_cast<__nv_bfloat16*>(base + 4 * slab);
-    const long long n4 = (long long)M * d / 4;
-    dropout_cast_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(
-        reinterpret_cast<const float4*>(kb_f32), reinterpret_cast<uint2*>(kbd), thr, scale, seed, MAC_SITE_READ_KB, step, n4);
-    MAC_LAUNCH_CHECK();
-    kb_bf16 = kbd;
+// dst[i][0, n) = fp32(src[i][0, n)) for nslab <= 3 slabs: n % 8 == 0, every pointer 16-byte aligned
+inline int widen3_bf16_launch(const void* const* src, float* const* dst, int nslab, long long n, cudaStream_t stream) {
+  const uint4* s[3] = {nullptr, nullptr, nullptr};
+  float4* d[3] = {nullptr, nullptr, nullptr};
+  for (int i = 0; i < nslab; ++i) {
+    s[i] = reinterpret_cast<const uint4*>(src[i]);
+    d[i] = reinterpret_cast<float4*>(dst[i]);
   }
-  TcGemmParams p{};
-  p.M = M; p.N = d; p.rows_per_batch = N; p.ldo = d; p.seed = seed; p.step = step;
-  // P = KB @ Wx + bx ; also P*y
-  p.epi = TC_EPI_P; p.bias = w->bx; p.out0 = P; p.out1 = PY; p.y = y;
-  int st = tc_gemm_launch(kb_bf16, d, nullptr, 0, w->Wx_bf16, p, stream);
-  if (st != MAC_OK) return st;
-  // H = ELU([P*y, P] @ Wm + bm)
-  p.epi = TC_EPI_ACT; p.act = MAC_ACT_ELU; p.bias = w->bm; p.out0 = H; p.out1 = nullptr;
-  st = tc_gemm_launch(PY, d, P, d, w->Wm_bf16, p, stream);
-  if (st != MAC_OK) return st;
-  // logits parts = sum_n ELU((H @ Wm2 + bm2) * control) * wr
-  p.epi = TC_EPI_LOGITS; p.bias = w->bm2; p.out0 = I1; p.ctrl = control; p.wr = w->wr; p.parts = parts;
-  p.e_thresh = thr; p.e_scale = scale; p.e_site = MAC_SITE_READ_INTER;
-  st = tc_gemm_launch(H, d, nullptr, 0, w->Wm2_bf16, p, stream, nparts);
-  if (st != MAC_OK) return st;
+  const long long n8 = n / 8;
+  const unsigned gx = (unsigned)std::min<long long>((n8 + 255) / 256, (long long)mac_num_sms() * 16);
+  widen3_bf16_kernel<<<dim3(gx, nslab), 256, 0, stream>>>(s[0], s[1], s[2], d[0], d[1], d[2], n8);
+  MAC_LAUNCH_CHECK();
   return MAC_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Eval-mode read (readDropout == 1): dropout(KB) == KB at every step and the read weights are shared over the steps
-// (mac_cell.py:209-277 is called with the same variables for each of the netLength cells), so
-//   P = KB @ Wx + bx                (ops.py:688)                       and
-//   Q = P @ Wm[d:2d, :] + bm        (the projected-KB half of the [P*y, P] concat, mac_cell.py:236-238)
-// do not depend on the step.  They are computed once per forward into `inv` = [P | Q] (bf16), and each step runs
-//   PY = P * y_b ;  H = ELU(PY @ Wm[0:d, :] + Q) ;  logits = ... (unchanged)
-// i.e. 2 x d instead of 4 x d MACs per knowledge-base element and step.
-// [P | Q] bf16 slabs, then the fused read step's (read_step.cuh) logits, one per knowledge-base row [B*N]
-inline size_t tc_read_invariant_bytes(int B, int N, int d) {
-  const size_t slab = (((size_t)B * N * d * 2 + 1023) & ~(size_t)1023);
-  return 2 * slab + (size_t)B * N * 4 + 1024;
-}
-
-// PY[m, :] = P[m, :] * y[m / rows_per_batch, :]   (8 bf16 per thread)
-__global__ void scale_rows_bf16_kernel(const uint4* __restrict__ P, const float* __restrict__ y, uint4* __restrict__ out,
-                                       int rows_per_batch, int d, long long n8) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n8) return;
-  const long long e = i * 8;
-  const int c = (int)(e % d);
-  const long long b = (e / d) / rows_per_batch;
-  const uint4 v = P[i];
-  const float4 y0 = __ldg(reinterpret_cast<const float4*>(y + b * d + c));
-  const float4 y1 = __ldg(reinterpret_cast<const float4*>(y + b * d + c + 4));
-  auto lo = [](uint32_t w) { return __uint_as_float(w << 16); };
-  auto hi = [](uint32_t w) { return __uint_as_float(w & 0xffff0000u); };
-  out[i] = make_uint4(pack_bf16(lo(v.x) * y0.x, hi(v.x) * y0.y), pack_bf16(lo(v.y) * y0.z, hi(v.y) * y0.w),
-                      pack_bf16(lo(v.z) * y1.x, hi(v.z) * y1.y), pack_bf16(lo(v.w) * y1.z, hi(v.w) * y1.w));
 }
 
 inline char* tc_align1k(void* p) {
   return reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~(uintptr_t)1023);
 }
-
-struct TcReadScratch {
-  __nv_bfloat16 *P, *Q;
-  float* parts;
-};
-inline TcReadScratch tc_read_scratch(void* inv, int B, int N, int d) {
-  const size_t slab = (((size_t)B * N * d * 2 + 1023) & ~(size_t)1023);
-  char* base = tc_align1k(inv);
-  TcReadScratch s;
-  s.P = reinterpret_cast<__nv_bfloat16*>(base);
-  s.Q = reinterpret_cast<__nv_bfloat16*>(base + slab);
-  s.parts = reinterpret_cast<float*>(base + 2 * slab);
-  return s;
-}
-
-inline int tc_read_invariant(const void* kb_bf16, const mac_read_weights* w, void* inv, size_t inv_bytes, int B, int N,
-                             int d, cudaStream_t stream) {
-  if (!kb_bf16 || !w->Wx_bf16 || !w->Wm_bf16 || !inv) return MAC_ERR_INVALID;
-  if (d % 128) return MAC_ERR_UNSUPPORTED;
-  if (inv_bytes < tc_read_invariant_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
-  const int M = B * N;
-  const size_t slab = (((size_t)M * d * 2 + 1023) & ~(size_t)1023);
-  char* base = tc_align1k(inv);
-  __nv_bfloat16* P = reinterpret_cast<__nv_bfloat16*>(base);
-  __nv_bfloat16* Q = reinterpret_cast<__nv_bfloat16*>(base + slab);
-  TcGemmParams p{};
-  p.M = M; p.N = d; p.rows_per_batch = N; p.ldo = d;
-  p.epi = TC_EPI_ACT; p.act = MAC_ACT_NON; p.bias = w->bx; p.out0 = P;
-  int st = tc_gemm_launch(kb_bf16, d, nullptr, 0, w->Wx_bf16, p, stream);
-  if (st != MAC_OK) return st;
-  p.bias = w->bm; p.out0 = Q;
-  return tc_gemm_launch(P, d, nullptr, 0, reinterpret_cast<const __nv_bfloat16*>(w->Wm_bf16) + d, p, stream, nullptr, 2 * d);
-}
-
-inline int tc_read_chain_inv(const void* inv, const float* y, const float* control, const mac_read_weights* w, float* parts,
-                             int* nparts, void* ws, size_t ws_bytes, int B, int N, int d, cudaStream_t stream) {
-  if (!inv || !w->Wm_bf16 || !w->Wm2_bf16) return MAC_ERR_INVALID;
-  if (d % 128) return MAC_ERR_UNSUPPORTED;
-  if (ws_bytes < tc_read_extra_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
-  const int M = B * N;
-  const size_t slab = (((size_t)M * d * 2 + 1023) & ~(size_t)1023);
-  const char* ibase = tc_align1k(const_cast<void*>(inv));
-  const __nv_bfloat16* P = reinterpret_cast<const __nv_bfloat16*>(ibase);
-  const __nv_bfloat16* Q = reinterpret_cast<const __nv_bfloat16*>(ibase + slab);
-  char* base = tc_align1k(ws);
-  __nv_bfloat16* PY = reinterpret_cast<__nv_bfloat16*>(base + slab);
-  __nv_bfloat16* H = reinterpret_cast<__nv_bfloat16*>(base + 2 * slab);
-  const long long n8 = (long long)M * d / 8;
-  scale_rows_bf16_kernel<<<(unsigned)((n8 + 255) / 256), 256, 0, stream>>>(
-      reinterpret_cast<const uint4*>(P), y, reinterpret_cast<uint4*>(PY), N, d, n8);
-  MAC_LAUNCH_CHECK();
-  TcGemmParams p{};
-  p.M = M; p.N = d; p.rows_per_batch = N; p.ldo = d;
-  // H = ELU(PY @ Wm[0:d] + Q)      (bm is inside Q)
-  p.epi = TC_EPI_ADDACT; p.act = MAC_ACT_ELU; p.bias = nullptr; p.out0 = H; p.add = Q;
-  int st = tc_gemm_launch(PY, d, nullptr, 0, w->Wm_bf16, p, stream, nullptr, 2 * d);
-  if (st != MAC_OK) return st;
-  p.epi = TC_EPI_LOGITS; p.act = MAC_ACT_NON; p.bias = w->bm2; p.out0 = nullptr; p.add = nullptr;
-  p.ctrl = control; p.wr = w->wr; p.parts = parts;
-  return tc_gemm_launch(H, d, nullptr, 0, w->Wm2_bf16, p, stream, nparts);
-}
-
 
 // ---------------------------------------------------------------------------------------------------------------
 // Weight gradients on tensor cores: dW[in, out] (+)= X^T[in, M] @ G^T[out, M]^T with K = M = B*N (12 544 at the headline shape)
@@ -770,98 +631,14 @@ inline int tc_wgrad_splitk(const void* xT, const void* gT, float* dW, float* par
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// "tc32": the read unit's three [B*N, .] projections as SPLIT-bf16 products on the tensor cores, for the <= 1e-4 parity bar
-// of BASELINE.json (the plain bf16 path is at ~1e-3).  Every fp32 operand x is carried as two bf16 values x_hi = bf16(x),
+// "tc32": [B*N, .] products as SPLIT-bf16 products on the tensor cores (the read unit's, read_fwd.cuh, and their gradients),
+// for the <= 1e-4 parity bar of BASELINE.json (the plain bf16 path is at ~1e-3).  Every fp32 operand x is carried as two bf16 values x_hi = bf16(x),
 // x_lo = bf16(x - x_hi) and the product uses three of the four partial products, accumulated in ONE fp32 accumulator:
 //     A W  ~=  A_hi W_hi + A_lo W_hi + A_hi W_lo                      (A_lo W_lo ~ 2^-16 relative is dropped)
 // With A' = [A_hi | A_lo] ([M, 2K]) and W' = [W_hi | W_hi | W_lo] ([N, 3K], K-major) this is the existing two-segment GEMM:
 // segment 0 = A'[:, 0:2K] against W'[:, 0:2K], segment 1 = A'[:, 0:K] against W'[:, 2K:3K] -- K triples, nothing else
 // changes.  Producers write their outputs directly as hi | lo pairs (TC_EPI_ACT_SPLIT) or as fp32 (TC_EPI_F32).
-// Inference form (P, Q hoisted, mac_read_invariant): inv = [P fp32 | Q fp32 | scratch [M, 2d] bf16].
-// Training form (tc3_read_chain_train): P = dropout(KB) @ Wx + bx, H = ELU([P*y | P] @ Wm + bm) as ONE split product over
-// K = 2d (A' = [(P*y)_hi | P_hi | (P*y)_lo | P_lo], W' = split3 of the whole Wm), I1 = H @ Wm2 + bm2, all saved in fp32.
 // ---------------------------------------------------------------------------------------------------------------
-// out[m, c] = hi(x[m, c] * y[m / rows_per_batch, c]), out[m, d + c] = lo(...)     (y == NULL: plain split); 4 columns / thread
-__global__ void split_rows_kernel(const float4* __restrict__ x, const float* __restrict__ y, uint2* __restrict__ out,
-                                  int rows_per_batch, int d, long long n4) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n4) return;
-  const int d4 = d / 4;
-  const long long m = i / d4;
-  const int c4 = (int)(i - m * d4);
-  float4 v = x[i];
-  if (y) {
-    const float4 s = __ldg(reinterpret_cast<const float4*>(y + (m / rows_per_batch) * d) + c4);
-    v.x *= s.x; v.y *= s.y; v.z *= s.z; v.w *= s.w;
-  }
-  const uint32_t h01 = pack_bf16(v.x, v.y), h23 = pack_bf16(v.z, v.w);
-  const uint32_t l01 = pack_bf16(v.x - __uint_as_float(h01 << 16), v.y - __uint_as_float(h01 & 0xffff0000u));
-  const uint32_t l23 = pack_bf16(v.z - __uint_as_float(h23 << 16), v.w - __uint_as_float(h23 & 0xffff0000u));
-  uint2* row = out + m * (2 * d4);
-  row[c4] = make_uint2(h01, h23);
-  row[d4 + c4] = make_uint2(l01, l23);
-}
-inline int split_rows_launch(const float* x, const float* y, void* out, int rows_per_batch, int d, long long M,
-                             cudaStream_t stream) {
-  const long long n4 = M * d / 4;
-  split_rows_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(x), y,
-                                                                      reinterpret_cast<uint2*>(out), rows_per_batch, d, n4);
-  MAC_LAUNCH_CHECK();
-  return MAC_OK;
-}
-
-// The training form's splits (tc3_read_chain_train):
-struct SplitRowsArgs {
-  const float* y = nullptr;    // row scale y[m / rows_per_batch, c] (NULL: none)
-  int rows_per_batch = 1;
-  int both = 0;                // also write the unscaled x at columns d .. 2d of each half ([x*y | x] per half)
-  uint32_t thresh = 0;         // dropout(x) with the forward's Philox stream (0: none): one draw per aligned column quad of
-  float scale = 1.f;           //   element index m*d + c (mac_dropout_fwd's, dropout_cast_bf16_kernel's numbering)
-  uint64_t seed = 0;
-  int site = 0, step = 0;
-};
-// out[m, c] = hi(v), out[m, H + c] = lo(v) with v = dropout(x)[m, c] (* y[m / rows_per_batch, c]) and H = d (both: H = 2d,
-// and the unscaled x goes to columns d + c and H + d + c); 4 columns / thread
-__global__ void split_rows_train_kernel(const float4* __restrict__ x, uint2* __restrict__ out, int d, long long n4,
-                                        const SplitRowsArgs a) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n4) return;
-  const int d4 = d / 4;
-  const long long m = i / d4;
-  const int c4 = (int)(i - m * d4);
-  float4 v = x[i];
-  if (a.thresh) {
-    const Philox4 r = philox4x32_10(a.seed, (uint64_t)i, (uint32_t)a.site, (uint32_t)a.step);
-    v.x = ((r.x >> 8) >= a.thresh) ? v.x * a.scale : 0.f;
-    v.y = ((r.y >> 8) >= a.thresh) ? v.y * a.scale : 0.f;
-    v.z = ((r.z >> 8) >= a.thresh) ? v.z * a.scale : 0.f;
-    v.w = ((r.w >> 8) >= a.thresh) ? v.w * a.scale : 0.f;
-  }
-  const int half4 = a.both ? 2 * d4 : d4;
-  uint2* row = out + m * (2 * half4);
-  auto put = [&](float4 u, int col4) {
-    const uint32_t h01 = pack_bf16(u.x, u.y), h23 = pack_bf16(u.z, u.w);
-    const uint32_t l01 = pack_bf16(u.x - __uint_as_float(h01 << 16), u.y - __uint_as_float(h01 & 0xffff0000u));
-    const uint32_t l23 = pack_bf16(u.z - __uint_as_float(h23 << 16), u.w - __uint_as_float(h23 & 0xffff0000u));
-    row[col4] = make_uint2(h01, h23);
-    row[half4 + col4] = make_uint2(l01, l23);
-  };
-  if (a.both) put(v, d4 + c4);
-  if (a.y) {
-    const float4 s = __ldg(reinterpret_cast<const float4*>(a.y + (m / a.rows_per_batch) * d) + c4);
-    v.x *= s.x; v.y *= s.y; v.z *= s.z; v.w *= s.w;
-  }
-  put(v, c4);
-}
-inline int split_rows_train_launch(const float* x, void* out, int d, long long M, const SplitRowsArgs& a,
-                                   cudaStream_t stream) {
-  const long long n4 = M * d / 4;
-  split_rows_train_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(x),
-                                                                            reinterpret_cast<uint2*>(out), d, n4, a);
-  MAC_LAUNCH_CHECK();
-  return MAC_OK;
-}
-
 // fp32 W[R, C] row-major -> bf16 W3[R, 3C] = [hi | hi | lo] per row, no transpose: the B operand of a split data gradient
 // dX = G @ W^T with W in its own [in, out] layout (rows = in = the output columns of dX, K = out).  C % 4 == 0.
 __global__ void split3_rows_kernel(const float4* __restrict__ W, uint2* __restrict__ W3, int C, long long n4) {
@@ -902,95 +679,9 @@ __global__ void pack_weight_split3_kernel(const float* __restrict__ W, __nv_bflo
   }
 }
 
-inline size_t tc3_slab(int B, int N, int d) { return (((size_t)B * N * 2 * d * 2 + 1023) & ~(size_t)1023); }   // [M, 2d] bf16
-inline size_t tc3_invariant_bytes(int B, int N, int d) {
-  return (size_t)2 * B * N * d * 4 + tc3_slab(B, N, d) + 2048;
-}
-inline size_t tc3_extra_workspace_bytes(int B, int N, int d) { return 2 * tc3_slab(B, N, d) + 1024; }
-
 // C = epilogue(A W) with A' = [A_hi | A_lo] ([M, 2K] bf16) and W' = [W_hi | W_hi | W_lo] ([N, 3K] bf16)
-inline int tc3_gemm(const void* a_split, int K, const void* wt3, TcGemmParams p, cudaStream_t stream, int* nparts = nullptr) {
-  return tc_gemm_launch(a_split, 2 * K, a_split, K, wt3, p, stream, nparts, 3 * K, 2 * K, 2 * K);
-}
-
-inline int tc3_read_invariant(const float* kb, const mac_read_weights* w, void* inv, size_t inv_bytes, int B, int N, int d,
-                              cudaStream_t stream) {
-  if (!kb || !w->Wx_s3 || !w->Wmb_s3 || !inv) return MAC_ERR_INVALID;
-  if (d % 128) return MAC_ERR_UNSUPPORTED;
-  if (inv_bytes < tc3_invariant_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
-  const int M = B * N;
-  float* P = reinterpret_cast<float*>(inv);
-  float* Q = P + (size_t)M * d;
-  void* scratch = tc_align1k(Q + (size_t)M * d);
-  TcGemmParams p{};
-  p.M = M; p.N = d; p.rows_per_batch = N; p.ldo = d; p.epi = TC_EPI_F32; p.act = MAC_ACT_NON;
-  int st = split_rows_launch(kb, nullptr, scratch, N, d, M, stream);
-  if (st != MAC_OK) return st;
-  p.bias = w->bx; p.outf = P;
-  st = tc3_gemm(scratch, d, w->Wx_s3, p, stream);                       // P = KB @ Wx + bx            (ops.py:688)
-  if (st != MAC_OK) return st;
-  st = split_rows_launch(P, nullptr, scratch, N, d, M, stream);
-  if (st != MAC_OK) return st;
-  p.bias = w->bm; p.outf = Q;
-  return tc3_gemm(scratch, d, w->Wmb_s3, p, stream);                    // Q = P @ Wm[d:2d] + bm       (mac_cell.py:236-238)
-}
-
-inline int tc3_read_chain_inv(const void* inv, const float* y, const float* control, const mac_read_weights* w, float* parts,
-                              int* nparts, void* ws, size_t ws_bytes, int B, int N, int d, cudaStream_t stream) {
-  if (!inv || !w->Wma_s3 || !w->Wm2_s3) return MAC_ERR_INVALID;
-  if (d % 128) return MAC_ERR_UNSUPPORTED;
-  if (ws_bytes < tc3_extra_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
-  const int M = B * N;
-  const float* P = reinterpret_cast<const float*>(inv);
-  const float* Q = P + (size_t)M * d;
-  char* base = tc_align1k(ws);
-  void* PYs = base;
-  __nv_bfloat16* Hs = reinterpret_cast<__nv_bfloat16*>(base + tc3_slab(B, N, d));
-  int st = split_rows_launch(P, y, PYs, N, d, M, stream);                // (P * y_b) as hi | lo       (ops.py:694-703)
-  if (st != MAC_OK) return st;
-  TcGemmParams p{};
-  p.M = M; p.N = d; p.rows_per_batch = N;
-  p.epi = TC_EPI_ACT_SPLIT; p.act = MAC_ACT_ELU; p.bias = nullptr; p.addf = Q; p.ldaf = d; p.out0 = Hs; p.ldo = 2 * d;
-  st = tc3_gemm(PYs, d, w->Wma_s3, p, stream);                           // H = ELU((P*y) @ Wm[0:d] + Q) as hi | lo
-  if (st != MAC_OK) return st;
-  p.epi = TC_EPI_LOGITS; p.act = MAC_ACT_NON; p.bias = w->bm2; p.addf = nullptr; p.out0 = nullptr; p.ldo = d;
-  p.ctrl = control; p.wr = w->wr; p.parts = parts;
-  return tc3_gemm(Hs, d, w->Wm2_s3, p, stream, nparts);                  // logits partial sums         (mac_cell.py:248-266)
-}
-
-// Training form (mac_read_fwd with MAC_PREC_TC32 and no `inv`): P, H, I1 in fp32 into P_f32 / H_f32 / I1_f32 (the caller's
-// `save`, or P into scratch and H, I1 not stored when there is none).  Scratch:
-//   s2   [M, 4d] bf16 (= M*d*8 bytes, 16-byte aligned): dropout(KB) as [hi | lo] in its first half, then A' of the H product
-//   ws   tc3_extra_workspace_bytes: H as [hi | lo] [M, 2d] in slab 1; slab 0 holds P when P_f32 is NULL
-// The caller has checked d % 128 == 0 and the packs (Wx_s3, Wm_s3, Wm2_s3) before any launch.
-inline int tc3_read_chain_train(const float* kb, const float* y, const float* control, const mac_read_weights* w, uint32_t thr,
-                                float scale, uint64_t seed, int step, float* P_f32, float* H_f32, float* I1_f32, float* parts,
-                                int* nparts, void* s2, void* ws, int B, int N, int d, cudaStream_t stream) {
-  const int M = B * N;
-  char* base = tc_align1k(ws);
-  float* P = P_f32 ? P_f32 : reinterpret_cast<float*>(base);
-  void* Hs = base + tc3_slab(B, N, d);
-  SplitRowsArgs sa;
-  sa.thresh = thr; sa.scale = scale; sa.seed = seed; sa.site = MAC_SITE_READ_KB; sa.step = step;
-  int st = split_rows_train_launch(kb, s2, d, M, sa, stream);                  // dropout(KB) as hi | lo   (ops.py:678)
-  if (st != MAC_OK) return st;
-  TcGemmParams p{};
-  p.M = M; p.N = d; p.rows_per_batch = N; p.ldo = d; p.seed = seed; p.step = step;
-  p.epi = TC_EPI_F32; p.act = MAC_ACT_NON; p.bias = w->bx; p.outf = P;
-  st = tc3_gemm(s2, d, w->Wx_s3, p, stream);                             // P = dropout(KB) @ Wx + bx  (ops.py:688)
-  if (st != MAC_OK) return st;
-  SplitRowsArgs sb;
-  sb.y = y; sb.rows_per_batch = N; sb.both = 1;
-  st = split_rows_train_launch(P, s2, d, M, sb, stream);                       // [(P*y)_hi | P_hi | (P*y)_lo | P_lo]
-  if (st != MAC_OK) return st;
-  p.epi = TC_EPI_ACT_SPLIT; p.act = MAC_ACT_ELU; p.bias = w->bm; p.outf = H_f32; p.out0 = reinterpret_cast<__nv_bfloat16*>(Hs);
-  p.ldo = 2 * d;
-  st = tc3_gemm(s2, 2 * d, w->Wm_s3, p, stream);                         // H = ELU([P*y | P] @ Wm + bm)  (mac_cell.py:236-238)
-  if (st != MAC_OK) return st;
-  p.epi = TC_EPI_LOGITS; p.act = MAC_ACT_NON; p.bias = w->bm2; p.outf = I1_f32; p.out0 = nullptr; p.ldo = d;
-  p.ctrl = control; p.wr = w->wr; p.parts = parts;
-  p.e_thresh = thr; p.e_scale = scale; p.e_site = MAC_SITE_READ_INTER;
-  return tc3_gemm(Hs, d, w->Wm2_s3, p, stream, nparts);                  // I1, logits partial sums  (mac_cell.py:248-266)
+inline int tc3_gemm(const void* a_split, int K, const void* wt3, TcGemmParams p, cudaStream_t stream) {
+  return tc_gemm_launch(a_split, 2 * K, a_split, K, wt3, p, stream, 3 * K, 2 * K, 2 * K);
 }
 
 // Split-bf16 weight gradient dW[in, out] += X^T G over a contraction of kp (= M rounded up to 64) rows:

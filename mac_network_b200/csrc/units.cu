@@ -120,242 +120,7 @@ extern "C" int mac_linear_fwd(const float* const* x_segs, const int* k_segs, con
 }
 
 // ------------------------------------------------------------------------------------------------ read unit
-// workspace layout: [header 4 KB | md [B,d] | y [B,d] | P [BN,d] | H [BN,d] | logit parts [BN, <=32] | split-K]
-static size_t read_ws_layout(int B, int N, int d, size_t* off_md, size_t* off_y, size_t* off_P, size_t* off_H,
-                             size_t* off_parts, size_t* off_splitk) {
-  size_t o = WS_HEADER;
-  auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
-  *off_md = take((size_t)B * d * 4);
-  *off_y = take((size_t)B * d * 4);
-  *off_P = take((size_t)B * N * d * 4);
-  *off_H = take((size_t)B * N * d * 4);
-  *off_parts = take((size_t)B * N * 32 * 4);
-  *off_splitk = o;
-  o += sgemm_workspace_bytes(B, d, d);
-  return o;
-}
-
-extern "C" size_t mac_read_workspace_bytes(int B, int N, int d, int prec) {
-  size_t a, b, c, e, f, g;
-  size_t fp32 = read_ws_layout(B, N, d, &a, &b, &c, &e, &f, &g);
-  if (prec == MAC_PREC_BF16) return fp32 + tc_read_extra_workspace_bytes(B, N, d);
-  if (prec == MAC_PREC_TC32) return fp32 + tc3_extra_workspace_bytes(B, N, d);
-  return fp32;
-}
-
-// ---- step-invariant part of the eval-mode read unit (see tc_read_invariant in tc_gemm.cuh): inv = [P | Q]
-static size_t read_inv_fp32_bytes(int B, int N, int d) { return (size_t)2 * B * N * d * 4 + 256; }
-
-extern "C" size_t mac_read_invariant_bytes(int B, int N, int d, int prec) {
-  if (prec == MAC_PREC_TC32) return tc3_invariant_bytes(B, N, d);
-  if (prec == MAC_PREC_FP8) return fp8_read_invariant_bytes(B, N, d);
-  return prec == MAC_PREC_BF16 ? tc_read_invariant_bytes(B, N, d) : read_inv_fp32_bytes(B, N, d);
-}
-
-extern "C" int mac_read_invariant(const float* kb, const void* kb_bf16, const mac_read_weights* w, int prec, void* inv,
-                                  size_t inv_bytes, int B, int N, int d, mac_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (prec == MAC_PREC_FP8 && (!kb_bf16 || !read_step_supported(B, N, d))) return MAC_ERR_UNSUPPORTED;
-  // the bf16 and fp8 paths read only kb_bf16: the fp32 knowledge base may be absent (host-cast front end)
-  const bool kb_opt = (prec == MAC_PREC_BF16 || prec == MAC_PREC_FP8) && kb_bf16;
-  if ((!kb && !kb_opt) || !w || !inv || B <= 0 || N <= 0 || d <= 0 || (d & 3)) return MAC_ERR_INVALID;
-  if ((kb && !mac_aligned16(kb)) || !mac_aligned16(inv)) return MAC_ERR_ALIGN;
-  if (inv_bytes < mac_read_invariant_bytes(B, N, d, prec)) return MAC_ERR_WORKSPACE;
-  if (prec == MAC_PREC_BF16) return tc_read_invariant(kb_bf16, w, inv, inv_bytes, B, N, d, stream);
-  if (prec == MAC_PREC_TC32) return tc3_read_invariant(kb, w, inv, inv_bytes, B, N, d, stream);
-  if (prec == MAC_PREC_FP8) return fp8_read_invariant(kb_bf16, w, inv, inv_bytes, B, N, d, stream);
-  const int M = B * N;
-  float* P = reinterpret_cast<float*>(inv);
-  float* Q = P + (size_t)M * d;
-  SgemmParams p{};
-  // P = KB @ Wx + bx   (ops.py:688)
-  p.a_mode = A_SEGS; p.nseg = 1; p.a[0] = kb; p.ak[0] = d; p.lda[0] = d;
-  p.W = w->Wx; p.ldw = d; p.M = M; p.N = d; p.K = d;
-  p.epi = EPI_BIAS_ACT; p.bias = w->bx; p.act = MAC_ACT_NON; p.Y = P; p.ldy = d;
-  int st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-  if (st != MAC_OK) return st;
-  // Q = P @ Wm[d:2d, :] + bm   (the un-scaled half of the concat, mac_cell.py:236-238)
-  p.a[0] = P; p.W = w->Wm + (size_t)d * d; p.bias = w->bm; p.Y = Q;
-  return sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-}
-
-static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, const float* y_pre,
-                         const float* memory_in, const float* control, const mac_read_weights* w, float keep_read,
-                         uint64_t seed, int step, int prec, float* info, float* att, float* save, void* workspace,
-                         size_t workspace_bytes, int B, int N, int d, mac_stream_t stream_);
-
-extern "C" int mac_read_step_fused(const void* inv, const void* kb_bf16, const float* y, const float* control,
-                                   const mac_read_weights* w, float* info, float* att, int B, int N, int d,
-                                   mac_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!inv || !kb_bf16 || !y || !control || !w || !info || !att || B <= 0 || N <= 0 || d <= 0) return MAC_ERR_INVALID;
-  if (!mac_aligned16(inv) || !mac_aligned16(kb_bf16) || !mac_aligned16(y) || !mac_aligned16(control)) return MAC_ERR_ALIGN;
-  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
-  return read_step_launch(inv, kb_bf16, y, control, w, att, info, B, N, d, stream);
-}
-extern "C" int mac_read_step_fused_supported(int B, int N, int d) { return read_step_supported(B, N, d) ? 1 : 0; }
-
-extern "C" int mac_read_fwd(const float* kb, const void* kb_bf16, const float* memory_in, const float* control,
-                            const mac_read_weights* w, float keep_read, uint64_t seed, int step, int prec, float* info,
-                            float* att, float* save, void* workspace, size_t workspace_bytes, int B, int N, int d,
-                            mac_stream_t stream_) {
-  return read_fwd_impl(kb, kb_bf16, nullptr, nullptr, memory_in, control, w, keep_read, seed, step, prec, info, att,
-                       save, workspace, workspace_bytes, B, N, d, stream_);
-}
-
-extern "C" int mac_read_fwd_inv(const float* kb, const void* kb_bf16, const void* inv, const float* y_pre,
-                                const float* memory_in, const float* control, const mac_read_weights* w, int prec,
-                                float* info, float* att, void* workspace, size_t workspace_bytes, int B, int N, int d,
-                                mac_stream_t stream_) {
-  if (!inv || !mac_aligned16(inv) || (y_pre && !mac_aligned16(y_pre))) return MAC_ERR_INVALID;
-  return read_fwd_impl(kb, kb_bf16, inv, y_pre, memory_in, control, w, 1.f, 0, 0, prec, info, att, nullptr, workspace,
-                       workspace_bytes, B, N, d, stream_);
-}
-
-static int read_fwd_impl(const float* kb, const void* kb_bf16, const void* inv, const float* y_pre,
-                         const float* memory_in, const float* control, const mac_read_weights* w, float keep_read,
-                         uint64_t seed, int step, int prec, float* info, float* att, float* save, void* workspace,
-                         size_t workspace_bytes, int B, int N, int d, mac_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  // e4m3: the inference read step only, checked before anything is launched
-  if (prec == MAC_PREC_FP8 && (!inv || !kb_bf16 || keep_read < 1.f || save || !read_step_supported(B, N, d)))
-    return MAC_ERR_UNSUPPORTED;
-  // split-bf16 training form: whole 128-wide wgmma tiles and its three packs, checked before anything is launched
-  const bool tc3_train = prec == MAC_PREC_TC32 && !inv;
-  if (tc3_train && (d <= 0 || d % 128)) return MAC_ERR_UNSUPPORTED;
-  if (tc3_train && (!w || !w->Wx_s3 || !w->Wm_s3 || !w->Wm2_s3)) return MAC_ERR_INVALID;
-  // eval bf16 / fp8 path: only the bf16 copy is read
-  const bool kb_opt = inv && (prec == MAC_PREC_BF16 || prec == MAC_PREC_FP8) && kb_bf16;
-  if ((!kb && !kb_opt) || !memory_in || !control || !w || !info || !att || !workspace) return MAC_ERR_INVALID;
-  if (B <= 0 || N <= 0 || d <= 0 || (d & 3)) return MAC_ERR_INVALID;
-  if (!(keep_read > 0.f && keep_read <= 1.f)) return MAC_ERR_INVALID;
-  if ((kb && !mac_aligned16(kb)) || !mac_aligned16(memory_in) || !mac_aligned16(control) || !mac_aligned16(workspace))
-    return MAC_ERR_ALIGN;
-  if (workspace_bytes < mac_read_workspace_bytes(B, N, d, prec)) return MAC_ERR_WORKSPACE;
-  const int M = B * N;
-  // the fp32 logits GEMM leaves one partial logit per column tile of I1 in a [B*N, 32] region: refuse wider d here,
-  // before anything is launched or written
-  const bool fp32_chain = prec != MAC_PREC_BF16 && prec != MAC_PREC_TC32 && prec != MAC_PREC_FP8;
-  if (fp32_chain && (d + sgemm_tile_n(M, d, d) - 1) / sgemm_tile_n(M, d, d) > 32) return MAC_ERR_UNSUPPORTED;
-  size_t o_md, o_y, o_P, o_H, o_parts, o_sk;
-  const size_t fp32_total = read_ws_layout(B, N, d, &o_md, &o_y, &o_P, &o_H, &o_parts, &o_sk);
-  char* ws = reinterpret_cast<char*>(workspace);
-  float* md = reinterpret_cast<float*>(ws + o_md);
-  // saved activations for backward live in the caller's `save` when given: [P | H | I1 | y]
-  float* P = save ? save : reinterpret_cast<float*>(ws + o_P);
-  float* H = save ? save + (size_t)M * d : reinterpret_cast<float*>(ws + o_H);
-  float* I1 = save ? save + (size_t)2 * M * d : nullptr;
-  float* y = save ? save + (size_t)3 * M * d : reinterpret_cast<float*>(ws + o_y);
-  float* parts = reinterpret_cast<float*>(ws + o_parts);
-  const bool drop = keep_read < 1.f;
-  const uint32_t thr = drop ? keep_threshold(keep_read) : 0u;
-  const float scale = drop ? 1.f / keep_read : 1.f;
-
-  // md = dropout(memory_in, keep_read)   (ops.py:679)
-  const float* mem = memory_in;
-  if (drop) {
-    const long long n = (long long)B * d;
-    dropout_kernel<<<(unsigned)(((n + 3) / 4 + 255) / 256), 256, 0, stream>>>(memory_in, thr, scale, seed,
-                                                                            MAC_SITE_READ_MEM, step, md, nullptr, n);
-    MAC_LAUNCH_CHECK();
-    mem = md;
-  }
-  // y = md @ Wy + by   (ops.py:689) -- unless the caller already has it (mac_write_fwd_next_y of the previous step)
-  if (y_pre) {
-    y = const_cast<float*>(y_pre);
-  } else {
-    SgemmParams p{};
-    p.a_mode = A_SEGS; p.nseg = 1; p.a[0] = mem; p.ak[0] = d; p.lda[0] = d;
-    p.W = w->Wy; p.ldw = d; p.M = B; p.N = d; p.K = d;
-    p.epi = EPI_BIAS_ACT; p.bias = w->by; p.act = MAC_ACT_NON; p.Y = y; p.ldy = d;
-    int st = sgemm_launch(p, reinterpret_cast<unsigned int*>(ws), reinterpret_cast<float*>(ws + o_sk),
-                          fp32_total - o_sk, stream);
-    if (st != MAC_OK) return st;
-  }
-  int nparts = 0;
-  if (prec == MAC_PREC_FP8) return read_step_fp8_launch(inv, kb_bf16, y, control, w, att, info, B, N, d, stream);
-  if (inv && prec == MAC_PREC_BF16 && kb_bf16 && read_step_supported(B, N, d)) {
-    // the whole step (P*y, both projections, logits, softmax, weighted sum) as ONE kernel: read_step.cuh
-    return read_step_launch(inv, kb_bf16, y, control, w, att, info, B, N, d, stream);
-  }
-  if (tc3_train) {
-    // the fp32 layout's P and H regions (contiguous, [M, 4d] bf16 together) hold the split operands; P, H, I1 go to `save`
-    int st = tc3_read_chain_train(kb, y, control, w, thr, scale, seed, step, save ? P : nullptr, save ? H : nullptr, I1,
-                                  parts, &nparts, ws + o_P, ws + fp32_total, B, N, d, stream);
-    if (st != MAC_OK) return st;
-  } else if (prec == MAC_PREC_TC32) {
-    int st = tc3_read_chain_inv(inv, y, control, w, parts, &nparts, ws + fp32_total, workspace_bytes - fp32_total, B, N, d,
-                                stream);
-    if (st != MAC_OK) return st;
-  } else if (inv && prec == MAC_PREC_BF16) {
-    int st = tc_read_chain_inv(inv, y, control, w, parts, &nparts, ws + fp32_total, workspace_bytes - fp32_total, B, N,
-                               d, stream);
-    if (st != MAC_OK) return st;
-  } else if (inv) {
-    const float* Pi = reinterpret_cast<const float*>(inv);
-    const float* Qi = Pi + (size_t)M * d;
-    // H = ELU((P*y) @ Wm[0:d, :] + Q)   (bm is inside Q)
-    {
-      SgemmParams p{};
-      p.a_mode = A_ROWSCALE_CONCAT; p.rs_half = d; p.nseg = 1; p.a[0] = Pi; p.lda[0] = d; p.rowvec = y; p.rows_per_batch = N;
-      p.W = w->Wm; p.ldw = d; p.M = M; p.N = d; p.K = d;
-      p.epi = EPI_BIAS_ACT; p.bias = nullptr; p.aux = Qi; p.ldaux = d; p.act = MAC_ACT_ELU; p.Y = H; p.ldy = d;
-      int st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-      if (st != MAC_OK) return st;
-    }
-    {
-      SgemmParams p{};
-      p.a_mode = A_SEGS; p.nseg = 1; p.a[0] = H; p.ak[0] = d; p.lda[0] = d;
-      p.W = w->Wm2; p.ldw = d; p.M = M; p.N = d; p.K = d; p.rows_per_batch = N;
-      p.epi = EPI_READ_LOGITS; p.bias = w->bm2; p.Y = nullptr; p.ldy = d;
-      p.ctrl = control; p.wr = w->wr; p.logit_parts = parts; p.e_thresh = 0u; p.e_scale = 1.f;
-      int st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-      if (st != MAC_OK) return st;
-      nparts = (d + sgemm_tile_n(M, d, d) - 1) / sgemm_tile_n(M, d, d);
-    }
-  } else if (prec == MAC_PREC_BF16) {
-    int st = tc_read_chain(kb, kb_bf16, y, control, w, thr, scale, seed, step, P, H, I1, parts, &nparts,
-                           ws + fp32_total, workspace_bytes - fp32_total, B, N, d, save != nullptr, stream);
-    if (st != MAC_OK) return st;
-  } else {
-    // P = dropout(KB) @ Wx + bx   (ops.py:678, 688)
-    {
-      SgemmParams p{};
-      p.a_mode = drop ? A_DROPOUT : A_SEGS; p.nseg = 1; p.a[0] = kb; p.ak[0] = d; p.lda[0] = d;
-      p.a_thresh = thr; p.a_scale = scale; p.seed = seed; p.a_site = MAC_SITE_READ_KB; p.step = step;
-      p.W = w->Wx; p.ldw = d; p.M = M; p.N = d; p.K = d;
-      p.epi = EPI_BIAS_ACT; p.bias = w->bx; p.act = MAC_ACT_NON; p.Y = P; p.ldy = d;
-      int st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-      if (st != MAC_OK) return st;
-    }
-    // H = ELU([P*y, P] @ Wm + bm)   (ops.py:694-719, mac_cell.py:236-238)
-    {
-      SgemmParams p{};
-      p.a_mode = A_ROWSCALE_CONCAT; p.nseg = 1; p.a[0] = P; p.lda[0] = d; p.rowvec = y; p.rows_per_batch = N;
-      p.W = w->Wm; p.ldw = d; p.M = M; p.N = d; p.K = 2 * d;
-      p.epi = EPI_BIAS_ACT; p.bias = w->bm; p.act = MAC_ACT_ELU; p.Y = H; p.ldy = d;
-      int st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-      if (st != MAC_OK) return st;
-    }
-    // I1 = H @ Wm2 + bm2 ; I2 = ELU(I1 * control) ; logits = dropout(I2) . wr   (ops.py:325-328, mac_cell.py:248-266)
-    {
-      SgemmParams p{};
-      p.a_mode = A_SEGS; p.nseg = 1; p.a[0] = H; p.ak[0] = d; p.lda[0] = d;
-      p.W = w->Wm2; p.ldw = d; p.M = M; p.N = d; p.K = d; p.rows_per_batch = N;
-      p.epi = EPI_READ_LOGITS; p.bias = w->bm2; p.Y = I1; p.ldy = d;
-      p.ctrl = control; p.wr = w->wr; p.logit_parts = parts;
-      p.e_thresh = thr; p.e_scale = scale; p.e_site = MAC_SITE_READ_INTER; p.seed = seed; p.step = step;
-      int st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-      if (st != MAC_OK) return st;
-      nparts = (d + sgemm_tile_n(M, d, d) - 1) / sgemm_tile_n(M, d, d);
-    }
-  }
-  if (nparts > 32) return MAC_ERR_UNSUPPORTED;
-  // att = softmax(logits); info = sum_n att * KB   (original, un-dropped KB: mac_cell.py:271-275)
-  if (prec == MAC_PREC_BF16 && kb_bf16 != nullptr)
-    return mac_kb_attend_fwd(parts, nparts, w->br, kb_bf16, 1, att, info, B, N, d, stream_);
-  return mac_kb_attend_fwd(parts, nparts, w->br, kb, 0, att, info, B, N, d, stream_);
-}
+#include "read_fwd.cuh"
 
 // ------------------------------------------------------------------------------------------------ write unit
 extern "C" size_t mac_write_workspace_bytes(int B, int d) {
@@ -542,19 +307,11 @@ extern "C" int mac_tc3_linear_(const void* a_split, const void* wt3, float* y, i
 extern "C" int mac_widen_bf16(const void* const* src_bf16, float* const* dst, int nslab, long long n, mac_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!src_bf16 || !dst || nslab < 1 || nslab > 3 || n <= 0 || (n & 7)) return MAC_ERR_INVALID;
-  const uint4* s[3] = {nullptr, nullptr, nullptr};
-  float4* d[3] = {nullptr, nullptr, nullptr};
   for (int i = 0; i < nslab; ++i) {
     if (!src_bf16[i] || !dst[i]) return MAC_ERR_INVALID;
     if ((reinterpret_cast<uintptr_t>(src_bf16[i]) | reinterpret_cast<uintptr_t>(dst[i])) & 15) return MAC_ERR_ALIGN;
-    s[i] = reinterpret_cast<const uint4*>(src_bf16[i]);
-    d[i] = reinterpret_cast<float4*>(dst[i]);
   }
-  const long long n8 = n / 8;
-  const unsigned gx = (unsigned)std::min<long long>((n8 + 255) / 256, (long long)mac_num_sms() * 16);
-  widen3_bf16_kernel<<<dim3(gx, nslab), 256, 0, stream>>>(s[0], s[1], s[2], d[0], d[1], d[2], n8);
-  MAC_LAUNCH_CHECK();
-  return MAC_OK;
+  return widen3_bf16_launch(src_bf16, dst, nslab, n, stream);
 }
 
 extern "C" int mac_pack_weight_split3(const float* W, void* Wt3_bf16, int K, int N, mac_stream_t stream_) {

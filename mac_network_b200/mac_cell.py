@@ -556,32 +556,10 @@ class MACCell(object):
                                     ctypes.byref(rw), float(self.dropouts["read"]), self.seed, i, self.prec,
                                     ptr(info), ptr(att), ptr(_save), ptr(self.ws.read), self.ws.read_bytes, B, N, d,
                                     stream_ptr()), "mac_read_fwd")
-        if _save is not None and self.prec == PREC["bf16"]:
-            self._upcast_saved(_save)
         if self._tape is not None:
             self._tape.fused_read(i, name, knowledgeBase, memory, control, info)
         self.attentions["kb"].append(att)
         return info
-
-    def _upcast_saved(self, save):
-        """Training forward on tensor cores: the chain leaves P, P*y, H, I1 as bf16 slabs in the read workspace (behind its
-        fp32 part, 1 KB aligned: tc_read_chain in csrc/tc_gemm.cuh); the backward kernels read `save` = [P | H | I1 | y] in
-        fp32, so widen the three it needs (a dtype-converting copy: memory plumbing; y is already there in fp32)."""
-        B, N, d = self.B, self.N, self.d
-        M = B * N
-        fp32_total = int(self.lib.mac_read_workspace_bytes(B, N, d, PREC["fp32"]))
-        base = self.ws.read.data_ptr()
-        off = ((base + fp32_total + 1023) & ~1023) - base
-        slab = (M * d * 2 + 1023) & ~1023
-        n = M * d
-        if n % 8 == 0:                                                 # one launch for the three slabs (mac_widen_bf16)
-            srcs = (ctypes.c_void_p * 3)(*[base + off + s_ * slab for s_ in (0, 2, 3)])       # P, H, I1  (slab 1 is P*y)
-            dsts = (ctypes.c_void_p * 3)(*[save.data_ptr() + 4 * k * n for k in range(3)])
-            check(self.lib.mac_widen_bf16(srcs, dsts, 3, n, stream_ptr()), "mac_widen_bf16")
-            return
-        for k, src_slab in enumerate((0, 2, 3)):
-            src = self.ws.read[off + src_slab * slab: off + src_slab * slab + M * d * 2].view(torch.bfloat16)
-            save[k * M * d:(k + 1) * M * d].copy_(src)
 
     # ------------------------------------------------------------------ write unit
     def _folded_write_weights(self, name):

@@ -459,6 +459,9 @@ def test_bf16_training_read_chain_matches_fp64(B, N, d):
     off = align1k(ws, lb.mac_read_workspace_bytes(B, N, d, 0))
     slab = (M * d * 2 + 1023) & ~1023
     P16, PY16, H16, I116 = (bf16_slab(ws, off + i * slab, M, d).double() for i in range(4))
+    # `save` = [P | H | I1 | y] in fp32: the library widens its bf16 slabs, bit for bit
+    for k, s16 in enumerate((P16, H16, I116)):
+        assert torch.equal(save[k * M * d:(k + 1) * M * d].view(M, d), s16.float()), "save slab %d" % k
     y = save[3 * M * d:].view(B, d)
     scale = np.float32(1.0) / np.float32(keep)
     # y = dropout(memory) @ Wy + by (fp32 path)

@@ -164,9 +164,6 @@ def test_cell_tensor_core_training_host_calls(monkeypatch, prec, tc):
     cfg = MACConfig.args("args", netLength=L, memDim=d, ctrlDim=d, attDim=d)
     params = MACParams(cfg, L, seed=1, device="cpu")
     x = {k: torch.from_numpy(v) for k, v in make_inputs(B, S, N, d, seed=2).items()}
-    # the mock's size queries return 64 KB; give the read workspace its real extent so the bf16 slab views exist
-    monkeypatch.setattr(mock, "mac_read_workspace_bytes",
-                        lambda b, n, dd, pr: 4096 + (2 + pr * 3) * b * n * dd * 4 + 8192, raising=False)
     cell = MACCell(x["vecQuestions"], x["questionWords"], x["questionCntxWords"], x["questionLengths"], x["knowledgeBase"],
                    0.85, 0.85, 1.0, B, True, config=cfg, params=params, prec=prec, save_for_backward=True)
     mac_network(cell, L)

@@ -45,9 +45,6 @@ def rec(monkeypatch):
     r = _Recorder(mock)
     monkeypatch.setattr(L_, "load", lambda: r)
     monkeypatch.setattr(torch.Tensor, "is_cuda", property(lambda self: True), raising=False)
-    # the mock's size queries return 64 KB; give the read workspace its real extent so the bf16 slab views exist
-    monkeypatch.setattr(mock, "mac_read_workspace_bytes",
-                        lambda b, n, dd, pr: 4096 + (2 + pr * 3) * b * n * dd * 4 + 8192, raising=False)
     return r
 
 
