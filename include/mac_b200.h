@@ -315,7 +315,21 @@ int mac_control_attend_bwd(const float* cc, long long cc_tstride, long long cc_b
 /* backward of mac_kb_attend_fwd: dkl [B,N] = softmax-backward of the logits; dkb [B,N,d] += att (x) dinfo (dkb may be NULL) */
 int mac_kb_attend_bwd(const float* kb, const float* att, const float* dinfo, float* dka_scratch, float* dkl,
                       float* dkb, float* dbr_part, int B, int N, int d, mac_stream_t stream);
-/* backward of mac_read_fwd (MAC_PREC_FP32); `save` is what the forward wrote; W*_t are the transposed weights */
+/* Backward of mac_read_fwd's training forms; `save` is what the forward wrote.  Three forms with the same outputs and
+ * accumulation conventions: dkb (may be NULL: not computed) +=, dmem_in =, dcontrol +=, dWx, dWy, dWm, dWm2 += [in, out],
+ * dby += [d], the bias and wr gradients as per-sample partials dbx_part, dbm_part, dbm2_part, dwr_part [B, d] +=,
+ * dbr_part [B] += (may be NULL); dWy and dby may be NULL (not computed).  Every one returns all its MAC_ERR_* before any
+ * launch and any write, so a refused call leaves the outputs and the workspace as they were:
+ *   MAC_ERR_INVALID      a required pointer NULL (kb, memory_in, control, w, w->wr, att, save, dinfo, dmem_in, dcontrol,
+ *                        Wy_t, dbx_part, dbm_part, dbm2_part, dwr_part, workspace, the form's weights below); B, N or d <= 0;
+ *                        d % 4 != 0; keep_read outside (0, 1]
+ *   MAC_ERR_UNSUPPORTED  the form's shape limits below
+ *   MAC_ERR_ALIGN        kb, memory_in, control, w->wr, save, dinfo, dmem_in, Wy_t, workspace, the form's weights, or a
+ *                        given dkb, dWx, dWy, dWm, dWm2 not 16-byte aligned
+ *   MAC_ERR_WORKSPACE    workspace_bytes below the form's *_workspace_bytes
+ *   MAC_ERR_ARCH         (tensor-core forms) not an sm_90 device
+ * mac_read_bwd (MAC_PREC_FP32): the FMA pipe.  Weights: the transposed Wm_t, Wm2_t, and Wx_t when dkb is given; dWx, dWm
+ * and dWm2 may be NULL (not computed). */
 int mac_read_bwd(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
                  const float* Wx_t, const float* Wy_t, const float* Wm_t, const float* Wm2_t,
                  const float* att, const float* save, const float* dinfo, float keep_read, uint64_t seed, int step,
@@ -326,8 +340,8 @@ size_t mac_read_bwd_workspace_bytes(int B, int N, int d);
 /* mac_read_bwd with its six [B*N, .] products on wgmma tensor cores (bf16 operands, fp32 accumulation; all element-wise
  * work in fp32): dgrad = mac_linear_tc_fwd(bf16(dY), bf16(W) in its own [in,out] layout), wgrad = mac_linear_tc_fwd(bf16(X)^T,
  * bf16(dY)^T) with K = B*N, fed by mac_cast_bf16 / mac_pack_weight_bf16.  Same arguments and accumulation conventions as
- * mac_read_bwd (the transposed fp32 weights are not needed except Wy_t); dWx, dWm, dWm2 are required.
- * Needs d % 128 == 0 and (B*N) % 64 == 0, else MAC_ERR_UNSUPPORTED. */
+ * mac_read_bwd (the transposed fp32 weights are not needed except Wy_t).  Weights: w->Wm, w->Wm2, and w->Wx when dkb is
+ * given; dWx, dWm, dWm2 are required.  Needs d % 128 == 0 and (B*N) % 64 == 0, else MAC_ERR_UNSUPPORTED. */
 int mac_read_bwd_tc(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
                     const float* Wy_t, const float* att, const float* save, const float* dinfo, float keep_read,
                     uint64_t seed, int step, float* dkb, float* dmem_in, float* dcontrol, float* dWx, float* dbx_part,
@@ -339,7 +353,8 @@ size_t mac_read_bwd_tc_workspace_bytes(int B, int N, int d);
  * gradients keep the forward's fp32-class accuracy.  Data gradients: [G_hi | G_lo] against [W_hi | W_hi | W_lo] per row of W
  * in its own [in, out] layout, packed into the workspace on every call.  Weight gradients: ONE split-K launch over the
  * contraction B*N rounded up to 64 (zero columns written on every call), slices summed in a fixed order: reruns are
- * bit-identical.  Any B*N; needs d % 128 == 0, else MAC_ERR_UNSUPPORTED before any launch. */
+ * bit-identical.  Weights and required gradients as mac_read_bwd_tc.  Any B*N; needs d % 128 == 0, else
+ * MAC_ERR_UNSUPPORTED. */
 int mac_read_bwd_tc32(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
                       const float* Wy_t, const float* att, const float* save, const float* dinfo, float keep_read,
                       uint64_t seed, int step, float* dkb, float* dmem_in, float* dcontrol, float* dWx, float* dbx_part,

@@ -26,6 +26,24 @@ def _t(params, W, key):
     return params.derived(("T", key), lambda: W.t().contiguous())
 
 
+# the forms of the read unit's backward (csrc/backward.cu): fp32 FMA pipe, bf16 tensor cores, split-bf16 tensor cores
+READ_BWD = {"fp32": "mac_read_bwd", "tc": "mac_read_bwd_tc", "tc32": "mac_read_bwd_tc32"}
+
+
+def read_bwd_workspace_bytes(lib, form, B, N, d):
+    return int(getattr(lib, READ_BWD[form] + "_workspace_bytes")(B, N, d))
+
+
+def read_bwd(lib, form, cell, i, kb, control, rw, Wt, dinfo, grads, ws, ws_bytes):
+    """The read unit's backward of step i in `form`.  Wt(name) gives the transposed fp32 weight "Wx", "Wy", "Wm" or "Wm2" (the
+    tensor-core forms read only Wy's); grads are the 13 gradient outputs dkb .. dbr_part in the order of the C ABI."""
+    wt = ("Wx", "Wy", "Wm", "Wm2") if form == "fp32" else ("Wy",)
+    check(getattr(lib, READ_BWD[form])(ptr(kb), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
+                                       *[ptr(Wt(k)) for k in wt], ptr(cell._att_kb[i]), ptr(cell._save[i]), ptr(dinfo),
+                                       float(cell.dropouts["read"]), cell.seed, i, *[ptr(g) for g in grads], ptr(ws), ws_bytes,
+                                       cell.B, cell.N, cell.d, stream_ptr()), READ_BWD[form])
+
+
 class _Bwd(object):
     def __init__(self, cell, bucket=None, zero_bucket=True, tc=False):
         self.cell, self.lib = cell, cell.lib
@@ -37,7 +55,7 @@ class _Bwd(object):
             raise NotImplementedError("split-bf16 tensor-core backward needs d % 128 == 0")
         if self.tc and not self.tc32 and (cell.d % 128 or (cell.B * cell.N) % 64):
             raise NotImplementedError("tensor-core backward needs d % 128 == 0 and (B*N) % 64 == 0")
-        mode = "tc32" if self.tc32 else self.tc
+        self.form = "tc32" if self.tc32 else "tc" if self.tc else "fp32"
         self.p = cell.params
         c = cell.cfg
         if c.controlWholeQ or c.controlContinuous:
@@ -56,15 +74,13 @@ class _Bwd(object):
             self.bucket.zero_()
         self.g = views_of(self.bucket, self.p.specs, self.p.offsets)
         cache = getattr(cell, "_bwd_ws", None)            # scratch is allocated once per cell and reused every step
-        if cache is not None and cache[4] != mode:
+        if cache is not None and cache[4] != self.form:
             cache = None
         if cache is None:
-            query = (self.lib.mac_read_bwd_tc32_workspace_bytes if self.tc32 else
-                     self.lib.mac_read_bwd_tc_workspace_bytes if self.tc else self.lib.mac_read_bwd_workspace_bytes)
-            ws_bytes = int(query(self.B, self.N, self.d))
+            ws_bytes = read_bwd_workspace_bytes(self.lib, self.form, self.B, self.N, self.d)
             lws_bytes = 4096 + 32 * 1536 * 512 * 4
             cache = (ws_bytes, torch.zeros(ws_bytes, dtype=torch.uint8, device=dev), lws_bytes,
-                     torch.zeros(lws_bytes, dtype=torch.uint8, device=dev), mode)
+                     torch.zeros(lws_bytes, dtype=torch.uint8, device=dev), self.form)
             cell._bwd_ws = cache
         self.ws_bytes, self.ws, self.lws_bytes, self.lws = cache[:4]
 
@@ -124,13 +140,13 @@ class _Bwd(object):
         wsc = "MACCell/write/"
         rsc = "MACCell/read/"
         rw = cell._read_weights("")
-        Wx, Wy = self.p.lin(rsc + "mulmemInter/", "projX")[0], self.p.lin(rsc + "mulmemInter/", "projY")[0]
-        Wm, Wm2 = self.p.lin(rsc, "memKbProj")[0], self.p.lin(rsc + "linearLayermemKbProj/", "memKbProj_2")[0]
         nWx, nbx = self.lin_names(rsc + "mulmemInter/", "projX")
         nWy, nby = self.lin_names(rsc + "mulmemInter/", "projY")
         nWm, nbm = self.lin_names(rsc, "memKbProj")
         nWm2, nbm2 = self.lin_names(rsc + "linearLayermemKbProj/", "memKbProj_2")
-        keep_m, keep_r, keep_w = cell.dropouts["memory"], cell.dropouts["read"], cell.dropouts["write"]
+        wnames = {"Wx": nWx, "Wy": nWy, "Wm": nWm, "Wm2": nWm2}
+        Wt = lambda k: _t(self.p, self.p[wnames[k]], wnames[k])
+        keep_m, keep_w = cell.dropouts["memory"], cell.dropouts["write"]
         hc, hm, hi = cell._hc, cell._hm, cell._hi
 
         for i in reversed(range(L)):
@@ -169,23 +185,9 @@ class _Bwd(object):
                 check(lib.mac_dropout_fwd(ptr(dinfo), keep_w, cell.seed, _lib.SITE_WRITE_INFO, i, ptr(dinfo), B * d,
                                           stream_ptr()), "dropout bwd")
             # ---------------- read unit backward (mac_cell.py:209-277)
-            if self.tc:
-                # bf16 cell: mac_read_bwd_tc; tc32 cell: the split-bf16 form with the same arguments
-                name = "mac_read_bwd_tc32" if self.tc32 else "mac_read_bwd_tc"
-                check(getattr(lib, name)(ptr(cell.knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
-                                         ptr(_t(self.p, Wy, nWy)), ptr(cell._att_kb[i]), ptr(cell._save[i]), ptr(dinfo),
-                                         keep_r, cell.seed, i, ptr(dkb), ptr(dmem_in), ptr(gC[i + 1]), ptr(self.G(nWx)),
-                                         ptr(part["bx"]), ptr(self.G(nWy)), ptr(self.G(nby)), ptr(self.G(nWm)),
-                                         ptr(part["bm"]), ptr(self.G(nWm2)), ptr(part["bm2"]), ptr(part["wr"]),
-                                         ptr(spart["br"]), ptr(self.ws), self.ws_bytes, B, N, d, stream_ptr()), name)
-            else:
-                check(lib.mac_read_bwd(ptr(cell.knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
-                                     ptr(_t(self.p, Wx, nWx)), ptr(_t(self.p, Wy, nWy)), ptr(_t(self.p, Wm, nWm)),
-                                     ptr(_t(self.p, Wm2, nWm2)), ptr(cell._att_kb[i]), ptr(cell._save[i]), ptr(dinfo),
-                                     keep_r, cell.seed, i, ptr(dkb), ptr(dmem_in), ptr(gC[i + 1]), ptr(self.G(nWx)),
-                                     ptr(part["bx"]), ptr(self.G(nWy)), ptr(self.G(nby)), ptr(self.G(nWm)), ptr(part["bm"]),
-                                     ptr(self.G(nWm2)), ptr(part["bm2"]), ptr(part["wr"]), ptr(spart["br"]), ptr(self.ws),
-                                     self.ws_bytes, B, N, d, stream_ptr()), "mac_read_bwd")
+            read_bwd(lib, self.form, cell, i, cell.knowledgeBase, control, rw, Wt, dinfo,
+                     [dkb, dmem_in, gC[i + 1], self.G(nWx), part["bx"], self.G(nWy), self.G(nby), self.G(nWm), part["bm"],
+                      self.G(nWm2), part["bm2"], part["wr"], spart["br"]], self.ws, self.ws_bytes)
             # memory_in = (variational) dropout of m_{i-1}  (mac_cell.py:214-217)
             if keep_m < 1.0:
                 site, st = (_lib.SITE_MEM_VAR, 0) if c.memoryVariationalDropout else (_lib.SITE_MEM_PLAIN, i)

@@ -766,15 +766,287 @@ extern "C" int mac_kb_attend_bwd(const float* kb, const float* att, const float*
   return MAC_OK;
 }
 
-// Backward of mac_read_fwd (fp32 path).  `save` = [P | H | I1 | y] from the forward.  Gradients in:
-//   dinfo [B,d].  Gradients out / accumulated:
-//   dkb [B,N,d] += (may be NULL), dmem_in [B,d] = gradient w.r.t. memory_in (the tensor handed to mac_read_fwd),
-//   dcontrol [B,d] +=, parameter gradients += (dWx..dWm2 full; bias / wr gradients as per-sample partials [B,d] that
-//   the caller reduces over B once per backward pass; dbr_part [B]).
-extern "C" size_t mac_read_bwd_workspace_bytes(int B, int N, int d) {
-  const size_t Md = (size_t)B * N * d * 4;
-  return BW_HEADER + 4 * Md /*dI1|dZ, dI0 (2x), dP*/ + ((size_t)B * N + 4) * 8 + (size_t)4 * B * d * 4 + 4096 +
-         (size_t)32 * 2 * d * d * 4 /*split-K partials of the largest wgrad*/;
+
+// ================================================================================================ read unit backward
+// Backward of mac_read_fwd's training forms (mac_cell.py:209-277; see mac_read_bwd* in mac_b200.h) in three forms that run
+// one seven-step schedule (read_bwd_run) and differ only in how they form its six [B*N, .] products:
+//   RB_FP32  mac_read_bwd       on the FMA pipe (sgemm), data gradients from the transposed fp32 weights, with the fused
+//                               prologues / epilogues of sgemm.cuh (P*y concat, KB dropout, * ELU'(H), dropout on dKB)
+//   RB_TC    mac_read_bwd_tc    bf16 operands on wgmma tensor cores (fp32 accumulation)
+//   RB_TC32  mac_read_bwd_tc32  split-bf16 operands on wgmma tensor cores (x = hi + lo, three of the four partial products)
+// The tensor-core forms build their operands with the transposing pack of tc_gemm.cuh, which applies P*y and the forward's KB
+// dropout mask on the way, and reach the tensor-core templates through the internal exports of units.cu below:
+//   wgrad  dW[in, d] += X^T G  (K = B*N)   X^T and G^T packed into the workspace, one split-K launch; the pack of G also
+//                                          leaves its row-major copy for the dgrad that follows
+//   dgrad  dX[M, in] = G W^T               W fp32 in its own [in, d] layout, cast (tc) or split (tc32) on every call
+// Every call is checked against everything its form reads and every limit of the kernels it launches (read_bwd_check), and
+// only then run: a refusal never follows a launch or a write, and nothing behind the check checks anything.
+extern "C" int mac_tc_wgrad_splitk_(const void* xT, const void* gT, float* dW, float* partial, int in_dim, int out_dim, int K,
+                                    mac_stream_t stream_);
+extern "C" size_t mac_tc_wgrad_partial_bytes_(int in_dim, int out_dim);
+extern "C" int mac_pack_t_bf16_(int mode, const float* X, void* Xt, void* Xrm, int K, int N, const float* rowvec,
+                                int rows_per_batch, uint32_t thresh, float scale, uint64_t seed, int site, int step,
+                                mac_stream_t stream_);
+extern "C" int mac_pack_t_split_(int mode, const float* X, void* Xt, void* Xrm, int K, int N, int segs, const float* rowvec,
+                                 int rows_per_batch, uint32_t thresh, float scale, uint64_t seed, int site, int step,
+                                 mac_stream_t stream_);
+extern "C" int mac_tc3_wgrad_splitk_(const void* xT2, const void* gT3, float* dW, float* partial, int in_dim, int out_dim,
+                                     int kp, mac_stream_t stream_);
+extern "C" int mac_split3_rows_(const float* W, void* W3, int R, int C, mac_stream_t stream_);
+extern "C" int mac_tc3_linear_(const void* a_split, const void* wt3, float* y, int M, int K, int n_out, mac_stream_t stream_);
+
+namespace mac {
+enum ReadBwdForm { RB_FP32, RB_TC, RB_TC32 };
+
+// The workspace of every form, first the fp32 part (M = B*N; dka and dkl padded to a multiple of 4 floats):
+//   [header 4 KB: split-K counters | bufA [M,d]: dI1, later dP | bufB [M,d]: dZ | bufC [M,2d]: dI0 | dka [M] | dkl [M] |
+//    dy [B,d] | md [B,d]: dropout(memory_in) | dmd [B,d] | unused [B,d] and 4 KB | split-K partials of the fp32 form's
+//    largest weight gradient, 32 x [2d, d]]
+// (the unused slab and gap have always been part of mac_read_bwd_workspace_bytes, which must not change), then for the
+// tensor-core forms, 1 KB aligned and each slab 1 KB aligned, with the contraction Mp = M (tc) or M rounded up to 64 (tc32):
+//   g [M, 2d] bf16      G of the last wgrad, row-major: bf16(G) (tc) or [G_hi | G_lo] (tc32), the dgrad's A operand
+//   xT [2d, Mp] bf16    the wgrad's activations transposed: X^T (tc) or [X_hi^T | X_lo^T] ([2d, 2Mp], tc32)
+//   gT [d, Mp] bf16     G transposed: G^T (tc) or [G_hi^T | G_hi^T | G_lo^T] ([d, 3Mp], tc32)
+//   w [2d, d] bf16      the dgrad's weight in its own layout: bf16(W) (tc) or [W_hi | W_hi | W_lo] per row ([2d, 3d], tc32)
+//   tmp32 fp32          a dgrad's output before its element-wise pass: [M, 2d] (tc) or [M, d] (tc32)
+//   dWtmp               split-K partials of the largest weight gradient
+// ws may be NULL when only `bytes` is wanted.
+struct ReadBwdWs {
+  unsigned int* counters;
+  float *bufA, *bufB, *bufC, *dka, *dkl, *dy, *md, *dmd, *partial;
+  size_t partial_bytes;
+  int Mp;
+  __nv_bfloat16 *g, *xT, *gT, *w;
+  float *tmp32, *dWtmp;
+  size_t bytes;          // mac_read_bwd*_workspace_bytes
+};
+static ReadBwdWs read_bwd_layout(ReadBwdForm f, void* ws, int B, int N, int d) {
+  const size_t M = (size_t)B * N, Md = M * d, Bd = (size_t)B * d, Mp4 = (M + 3) & ~(size_t)3;
+  const uintptr_t base = reinterpret_cast<uintptr_t>(ws);
+  auto fp = [&](size_t o) { return reinterpret_cast<float*>(base + o); };
+  ReadBwdWs L{};
+  L.counters = reinterpret_cast<unsigned int*>(base);
+  L.bufA = fp(BW_HEADER);
+  L.bufB = L.bufA + Md;
+  L.bufC = L.bufB + Md;
+  L.dka = L.bufC + 2 * Md;
+  L.dkl = L.dka + Mp4;
+  L.dy = L.dkl + Mp4;
+  L.md = L.dy + Bd;
+  L.dmd = L.md + Bd;
+  L.partial = L.dmd + 2 * Bd + 1024;
+  L.partial_bytes = (size_t)32 * 2 * d * d * 4;            // sgemm_launch cuts a product into at most 32 slices
+  // (M + 4) * 8 bytes cover dka and dkl with their padding
+  const size_t fp32 = BW_HEADER + 4 * Md * 4 + (M + 4) * 8 + 4 * Bd * 4 + 4096 + L.partial_bytes;
+  const bool split = f == RB_TC32;
+  L.Mp = split ? (int)((M + 63) & ~(size_t)63) : (int)M;
+  L.bytes = fp32;
+  if (f == RB_FP32) return L;
+  const uintptr_t tc = (base + fp32 + 1023) & ~(uintptr_t)1023;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { const size_t r = o; o += (bytes + 1023) & ~(size_t)1023; return tc + r; };
+  L.g = reinterpret_cast<__nv_bfloat16*>(take(M * 2 * d * 2));
+  L.xT = reinterpret_cast<__nv_bfloat16*>(take((size_t)2 * d * (split ? 2 : 1) * L.Mp * 2));
+  L.gT = reinterpret_cast<__nv_bfloat16*>(take((size_t)d * (split ? 3 : 1) * L.Mp * 2));
+  L.w = reinterpret_cast<__nv_bfloat16*>(take((size_t)2 * d * (split ? 3 : 1) * d * 2));
+  L.tmp32 = reinterpret_cast<float*>(take(M * (split ? 1 : 2) * d * 4));
+  L.dWtmp = reinterpret_cast<float*>(take(mac_tc_wgrad_partial_bytes_(2 * d, d)));
+  L.bytes = fp32 + 1024 + o;
+  return L;
+}
+
+// What one mac_read_bwd* call was given, with the layout, the dropout threshold and scale and the parts of `save` filled in
+// by read_bwd_run.  Wx_t, Wm_t, Wm2_t: the fp32 form's dgrad weights (the tensor-core forms read w->Wx, w->Wm, w->Wm2).
+struct ReadBwdCall {
+  ReadBwdForm f;
+  const float *kb, *memory_in, *control; const mac_read_weights* w;
+  const float *Wx_t, *Wy_t, *Wm_t, *Wm2_t;
+  const float *att, *save, *dinfo; float keep; uint64_t seed; int step;
+  float *dkb, *dmem_in, *dcontrol, *dWx, *dbx_part, *dWy, *dby, *dWm, *dbm_part, *dWm2, *dbm2_part, *dwr_part, *dbr_part;
+  void* ws; size_t ws_bytes; int B, N, d;
+  cudaStream_t s;
+  ReadBwdWs L; uint32_t thr; float scale;      // thr != 0 exactly when keep < 1
+  const float *P, *H, *I1, *y;
+};
+
+// Everything a form can refuse, before any CUDA call.  Pointers:
+//   required   kb, memory_in, control, w, w->wr, att, save, dinfo, dmem_in, dcontrol, Wy_t, dbx_part, dbm_part, dbm2_part,
+//              dwr_part, workspace, the dgrad weights of dI1 and dZ (Wm2_t, Wm_t or w->Wm2, w->Wm), and with dkb that of
+//              dP (Wx_t or w->Wx); dWx, dWm and dWm2 for the tensor-core forms
+//   optional   dkb, dWy, dby, dbr_part; dWx, dWm, dWm2 for RB_FP32 (their products are skipped)
+//   16-byte    kb, memory_in, control, w->wr, save, dinfo, dmem_in, Wy_t, workspace, the dgrad weights, and dkb, dWx, dWy,
+//   aligned    dWm, dWm2 when given: the float4 / cp.async accesses of kb_dot, kb_attend_bwd, read_bwd_logits, read_bwd_p,
+//              the sgemm and skinny products, elu_bwd_colsum, axpy_dropout, mac_cast_bf16, split3_rows and splitk_accum
+// Shapes: B, N, d > 0 (INVALID); d % 128 == 0 for the tensor-core forms and (B*N) % 64 == 0 for RB_TC, whose weight
+// gradients contract over B*N in 64-row k-blocks (UNSUPPORTED); d % 4 == 0 (INVALID).  keep_read in (0, 1] (INVALID).
+// MAC_ERR_ARCH last.
+static int read_bwd_check(const ReadBwdCall& c) {
+  if (!c.kb || !c.memory_in || !c.control || !c.w || !c.w->wr || !c.att || !c.save || !c.dinfo || !c.dmem_in ||
+      !c.dcontrol || !c.Wy_t || !c.dbx_part || !c.dbm_part || !c.dbm2_part || !c.dwr_part || !c.ws)
+    return MAC_ERR_INVALID;
+  const bool tc = c.f != RB_FP32;
+  const float* Wx = c.dkb ? (tc ? c.w->Wx : c.Wx_t) : nullptr;
+  const float *Wm = tc ? c.w->Wm : c.Wm_t, *Wm2 = tc ? c.w->Wm2 : c.Wm2_t;
+  if (!Wm || !Wm2 || (c.dkb && !Wx) || (tc && (!c.dWx || !c.dWm || !c.dWm2))) return MAC_ERR_INVALID;
+  if (c.B <= 0 || c.N <= 0 || c.d <= 0) return MAC_ERR_INVALID;
+  if (tc && ((c.d % 128) || (c.f == RB_TC && (c.B * c.N) % 64))) return MAC_ERR_UNSUPPORTED;
+  if ((c.d & 3) || !(c.keep > 0.f && c.keep <= 1.f)) return MAC_ERR_INVALID;
+  const void* vec[] = {c.kb, c.memory_in, c.control, c.w->wr, c.save, c.dinfo, c.dmem_in, c.Wy_t, c.ws, Wx, Wm, Wm2,
+                       c.dkb, c.dWx, c.dWy, c.dWm, c.dWm2};
+  for (const void* p : vec)
+    if (p && !mac_aligned16(p)) return MAC_ERR_ALIGN;
+  if (c.ws_bytes < read_bwd_layout(c.f, nullptr, c.B, c.N, c.d).bytes) return MAC_ERR_WORKSPACE;
+  return tc && !mac_b200_device_ok() ? MAC_ERR_ARCH : MAC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ the four form-specific steps
+// The activation X of a weight gradient dW += X^T G: H, [P*y | P] (K = 2d) or dropout(KB) with the forward's mask
+enum ReadBwdAct { RB_H, RB_PY_P, RB_KB };
+
+// tensor-core forms: X [M, d] -> Xt (tc: bf16 X^T; tc32: `segs` split segments of Mp columns per row, see the layout) with
+// x*y (mode 1) or the forward's KB dropout (mode 2) applied; Xrm (may be NULL) receives the row-major copy
+static int rb_pack(const ReadBwdCall& c, int mode, const float* X, void* Xt, void* Xrm, int segs) {
+  if (c.f == RB_TC)
+    return mac_pack_t_bf16_(mode, X, Xt, Xrm, c.B * c.N, c.d, c.y, c.N, c.thr, c.scale, c.seed, MAC_SITE_READ_KB, c.step, c.s);
+  return mac_pack_t_split_(mode, X, Xt, Xrm, c.B * c.N, c.d, segs, c.y, c.N, c.thr, c.scale, c.seed, MAC_SITE_READ_KB, c.step,
+                           c.s);
+}
+
+// dW[in, d] += X^T G, skipped by RB_FP32 when dW is NULL
+static int rb_wgrad(const ReadBwdCall& c, ReadBwdAct a, const float* G, float* dW) {
+  const ReadBwdWs& L = c.L;
+  const int M = c.B * c.N, d = c.d, in = a == RB_PY_P ? 2 * d : d;
+  const float* X = a == RB_H ? c.H : a == RB_PY_P ? c.P : c.kb;
+  const bool drop = a == RB_KB && c.thr;
+  if (c.f == RB_FP32) {
+    if (!dW) return MAC_OK;
+    SgemmParams p{};
+    p.a_mode = a == RB_PY_P ? A_TRANS_ROWSCALE_CONCAT : drop ? A_TRANS_DROPOUT : A_TRANS;
+    p.nseg = 1; p.a[0] = X; p.lda[0] = d; p.rowvec = c.y; p.rows_per_batch = c.N;
+    p.a_thresh = c.thr; p.a_scale = c.scale; p.seed = c.seed; p.a_site = MAC_SITE_READ_KB; p.step = c.step;
+    p.W = G; p.ldw = d; p.M = in; p.N = d; p.K = M;
+    p.epi = EPI_BIAS_ACT; p.Y = dW; p.ldy = d; p.accumulate = 1;
+    return sgemm_launch(p, L.counters, L.partial, L.partial_bytes, c.s);
+  }
+  int st = rb_pack(c, a == RB_PY_P ? 1 : drop ? 2 : 0, X, L.xT, nullptr, 2);                   // rows 0..d-1: X or P*y
+  if (st == MAC_OK && a == RB_PY_P)                                                            // rows d..2d-1: P
+    st = rb_pack(c, 0, X, L.xT + (size_t)d * (c.f == RB_TC32 ? 2 : 1) * L.Mp, nullptr, 2);
+  if (st == MAC_OK) st = rb_pack(c, 0, G, L.gT, L.g, 3);
+  if (st != MAC_OK) return st;
+  return c.f == RB_TC ? mac_tc_wgrad_splitk_(L.xT, L.gT, dW, L.dWtmp, in, d, M, c.s)
+                      : mac_tc3_wgrad_splitk_(L.xT, L.gT, dW, L.dWtmp, in, d, L.Mp, c.s);
+}
+
+// out[M, in] = G W^T: RB_FP32 from G and the transposed weight Wt [d, in] with the sgemm epilogue `epi`; the tensor-core
+// forms from the weight W [in, d] in its own layout and the copy of G the preceding rb_wgrad left in L.g, stored in fp32
+static int rb_dgrad(const ReadBwdCall& c, const float* G, const float* Wt, const float* W, int in, int epi, float* out) {
+  const int M = c.B * c.N, d = c.d;
+  int st;
+  switch (c.f) {
+    case RB_FP32: {
+      SgemmParams p{};
+      p.a_mode = A_SEGS; p.nseg = 1; p.a[0] = G; p.ak[0] = d; p.lda[0] = d;
+      p.W = Wt; p.ldw = in; p.M = M; p.N = in; p.K = d;
+      p.epi = epi; p.act = MAC_ACT_NON; p.Y = out; p.ldy = in;
+      if (epi == EPI_MUL_ELUGRAD) { p.aux = c.H; p.ldaux = d; }
+      p.e_thresh = c.thr; p.e_scale = c.scale; p.e_site = MAC_SITE_READ_KB; p.seed = c.seed; p.step = c.step;
+      return sgemm_launch(p, nullptr, nullptr, 0, c.s, false);
+    }
+    case RB_TC:
+      st = mac_cast_bf16(W, c.L.w, (long long)in * d, c.s);
+      return st != MAC_OK ? st : mac_linear_tc_fwd(c.L.g, c.L.w, nullptr, MAC_ACT_NON, out, 0, M, d, in, c.s);
+    default:
+      st = mac_split3_rows_(W, c.L.w, in, d, c.s);
+      return st != MAC_OK ? st : mac_tc3_linear_(c.L.g, c.L.w, out, M, d, in, c.s);
+  }
+}
+
+// dZ = (dI1 @ Wm2^T) * ELU'(H) into bufB, dbm_part += its column sums
+static int rb_dz(const ReadBwdCall& c) {
+  const ReadBwdWs& L = c.L;
+  if (c.f == RB_FP32) {
+    const int st = rb_dgrad(c, L.bufA, c.Wm2_t, nullptr, c.d, EPI_MUL_ELUGRAD, L.bufB);
+    return st != MAC_OK ? st : launch_colsum(L.bufB, c.dbm_part, c.B, c.N, c.d, 1, c.s);
+  }
+  const int st = rb_dgrad(c, nullptr, nullptr, c.w->Wm2, c.d, 0, L.tmp32);
+  if (st != MAC_OK) return st;
+  elu_bwd_colsum_kernel<<<dim3((c.d + 127) / 128, c.B), 256, 0, c.s>>>(c.H, L.tmp32, L.bufB, c.dbm_part, c.N, c.d);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+// dKB += (dP @ Wx^T) * mask/keep
+static int rb_dkb(const ReadBwdCall& c) {
+  const ReadBwdWs& L = c.L;
+  if (c.f == RB_FP32) return rb_dgrad(c, L.bufA, c.Wx_t, nullptr, c.d, EPI_ACCUM_DROPOUT, c.dkb);
+  const int st = rb_dgrad(c, nullptr, nullptr, c.w->Wx, c.d, 0, L.tmp32);
+  if (st != MAC_OK) return st;
+  const long long n4 = (long long)c.B * c.N * c.d / 4;
+  if (!c.thr) return mac_axpy(c.dkb, L.tmp32, 1.f, 4 * n4, c.s);
+  axpy_dropout_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, c.s>>>(reinterpret_cast<float4*>(c.dkb),
+                                                                     reinterpret_cast<const float4*>(L.tmp32), c.thr, c.scale,
+                                                                     c.seed, MAC_SITE_READ_KB, c.step, n4);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ the schedule
+static int read_bwd_run(ReadBwdCall c) {
+  const int B = c.B, N = c.N, d = c.d;
+  const size_t Md = (size_t)B * N * d;
+  c.L = read_bwd_layout(c.f, c.ws, B, N, d);
+  c.thr = c.keep < 1.f ? keep_threshold(c.keep) : 0u;
+  c.scale = c.keep < 1.f ? 1.f / c.keep : 1.f;
+  c.P = c.save; c.H = c.save + Md; c.I1 = c.save + 2 * Md; c.y = c.save + 3 * Md;     // `save` = [P | H | I1 | y]
+  const ReadBwdWs& L = c.L;
+  // (1) info = sum_n att*KB ; att = softmax(kl):  dkl, dKB += att (x) dinfo
+  int st = mac_kb_attend_bwd(c.kb, c.att, c.dinfo, L.dka, L.dkl, c.dkb, c.dbr_part, B, N, d, c.s);
+  if (st != MAC_OK) return st;
+  // (2) logits epilogue backward -> dI1 (bufA), dcontrol, dwr, dbm2
+  read_bwd_logits_kernel<<<dim3((d + 127) / 128, B), 256, 0, c.s>>>(c.I1, c.control, c.w->wr, L.dkl, c.thr, c.scale, c.seed,
+                                                                    c.step, L.bufA, c.dcontrol, c.dwr_part, c.dbm2_part, N, d);
+  MAC_LAUNCH_CHECK();
+  // (3) I1 = H @ Wm2 + bm2:  dWm2 += H^T dI1 ;  dZ = (dI1 @ Wm2^T) * ELU'(H) ; dbm += colsum(dZ)
+  st = rb_wgrad(c, RB_H, L.bufA, c.dWm2);
+  if (st == MAC_OK) st = rb_dz(c);
+  // (4) H = ELU([P*y, P] @ Wm + bm):  dWm += [P*y, P]^T dZ ;  dI0 = dZ @ Wm^T
+  if (st == MAC_OK) st = rb_wgrad(c, RB_PY_P, L.bufB, c.dWm);
+  if (st == MAC_OK) st = rb_dgrad(c, L.bufB, c.Wm_t, c.w->Wm, 2 * d, EPI_BIAS_ACT, L.bufC);
+  if (st != MAC_OK) return st;
+  // (5) I0 = [P*y, P]:  dP (bufA), dy, dbx
+  read_bwd_p_kernel<<<dim3((d + 127) / 128, B), 256, 0, c.s>>>(L.bufC, c.P, c.y, L.bufA, L.dy, c.dbx_part, N, d);
+  MAC_LAUNCH_CHECK();
+  // (6) P = dropout(KB) @ Wx + bx:  dWx += Kd^T dP ;  dKB += (dP @ Wx^T) * mask/keep
+  st = rb_wgrad(c, RB_KB, L.bufA, c.dWx);
+  if (st == MAC_OK && c.dkb) st = rb_dkb(c);
+  if (st != MAC_OK) return st;
+  // (7) y = md @ Wy + by with md = dropout(memory_in):  dWy += md^T dy ; dby += colsum(dy) ; dmem_in = (dy @ Wy^T)*mask/keep
+  // An M = B product in fp32 for every form.  mac_linear_bwd gets no workspace, so it runs without split-K: its partials
+  // would start at bufA, and at small N (B*N*4 < splitk*d) they would overwrite its own inputs dy, md and dmd behind it.
+  const bool drop = c.thr != 0;
+  if (drop) {
+    st = mac_dropout_fwd(c.memory_in, c.keep, c.seed, MAC_SITE_READ_MEM, c.step, L.md, (long long)B * d, c.s);
+    if (st != MAC_OK) return st;
+  }
+  const float* xs[1] = {drop ? L.md : c.memory_in};
+  const int ks[1] = {d}, acc0[1] = {0};
+  float* dxs[1] = {drop ? L.dmd : c.dmem_in};
+  st = mac_linear_bwd(xs, ks, ks, 1, c.Wy_t, L.dy, d, dxs, ks, acc0, c.dWy, c.dby, B, d, nullptr, 0, c.s);
+  if (st != MAC_OK || !drop) return st;
+  return mac_dropout_fwd(L.dmd, c.keep, c.seed, MAC_SITE_READ_MEM, c.step, c.dmem_in, (long long)B * d, c.s);
+}
+
+static int read_bwd(ReadBwdCall c) {
+  const int st = read_bwd_check(c);
+  return st != MAC_OK ? st : read_bwd_run(c);
+}
+}  // namespace mac
+
+// ------------------------------------------------------------------------------------------------ entry points
+extern "C" size_t mac_read_bwd_workspace_bytes(int B, int N, int d) { return read_bwd_layout(RB_FP32, nullptr, B, N, d).bytes; }
+extern "C" size_t mac_read_bwd_tc_workspace_bytes(int B, int N, int d) { return read_bwd_layout(RB_TC, nullptr, B, N, d).bytes; }
+extern "C" size_t mac_read_bwd_tc32_workspace_bytes(int B, int N, int d) {
+  return read_bwd_layout(RB_TC32, nullptr, B, N, d).bytes;
 }
 
 extern "C" int mac_read_bwd(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
@@ -784,246 +1056,9 @@ extern "C" int mac_read_bwd(const float* kb, const float* memory_in, const float
                             float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2, float* dbm2_part,
                             float* dwr_part, float* dbr_part, void* workspace, size_t workspace_bytes, int B, int N,
                             int d, mac_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!kb || !memory_in || !control || !w || !att || !save || !dinfo || !dmem_in || !dcontrol || !workspace)
-    return MAC_ERR_INVALID;
-  if (workspace_bytes < mac_read_bwd_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
-  const int M = B * N;
-  const size_t Md = (size_t)M * d;
-  char* ws = reinterpret_cast<char*>(workspace);
-  unsigned int* counters = reinterpret_cast<unsigned int*>(ws);
-  float* f = reinterpret_cast<float*>(ws + BW_HEADER);
-  float* bufA = f;                 // dI1, then dZ (in place is not possible: separate GEMM output) -> dI1 here
-  float* bufB = f + Md;            // dZ
-  float* bufC = f + 2 * Md;        // dI0 [M, 2d]
-  float* dka = f + 4 * Md;         // [B,N]
-  const size_t BNp = ((size_t)B * N + 3) & ~(size_t)3;   // keep the [B,d] buffers behind it 16-byte aligned
-  float* dkl = dka + BNp;
-  float* dy = dkl + BNp;           // [B,d]
-  float* md = dy + (size_t)B * d;  // [B,d] recomputed dropped memory
-  float* dmd = md + (size_t)B * d; // [B,d]
-  float* partial = dmd + (size_t)2 * B * d + 1024;
-  const size_t pbytes = workspace_bytes - (reinterpret_cast<char*>(partial) - ws);
-  const float* P = save;
-  const float* H = save + Md;
-  const float* I1 = save + 2 * Md;
-  const float* y = save + 3 * Md;
-  const bool drop = keep_read < 1.f;
-  const uint32_t thr = drop ? keep_threshold(keep_read) : 0u;
-  const float scale = drop ? 1.f / keep_read : 1.f;
-  int st;
-  // (1) info = sum_n att*KB ; att = softmax(kl):  dkl, dKB += att (x) dinfo
-  st = mac_kb_attend_bwd(kb, att, dinfo, dka, dkl, dkb, dbr_part, B, N, d, stream_);
-  if (st != MAC_OK) return st;
-  // (2) logits epilogue backward -> dI1, dcontrol, dwr, dbm2
-  read_bwd_logits_kernel<<<dim3((d + 127) / 128, B), 256, 0, stream>>>(I1, control, w->wr, dkl, thr, scale, seed, step,
-                                                                      bufA, dcontrol, dwr_part, dbm2_part, N, d);
-  MAC_LAUNCH_CHECK();
-  // (3) I1 = H @ Wm2 + bm2:  dWm2 += H^T dI1 ;  dZ = (dI1 @ Wm2^T) * ELU'(Z)
-  if (dWm2) {
-    SgemmParams p{};
-    p.a_mode = A_TRANS; p.nseg = 1; p.a[0] = H; p.lda[0] = d;
-    p.W = bufA; p.ldw = d; p.M = d; p.N = d; p.K = M;
-    p.epi = EPI_BIAS_ACT; p.Y = dWm2; p.ldy = d; p.accumulate = 1;
-    st = sgemm_launch(p, counters, partial, pbytes, stream);
-    if (st != MAC_OK) return st;
-  }
-  {
-    SgemmParams p{};
-    p.a_mode = A_SEGS; p.nseg = 1; p.a[0] = bufA; p.ak[0] = d; p.lda[0] = d;
-    p.W = Wm2_t; p.ldw = d; p.M = M; p.N = d; p.K = d;
-    p.epi = EPI_MUL_ELUGRAD; p.aux = H; p.ldaux = d; p.Y = bufB; p.ldy = d;
-    st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-    if (st != MAC_OK) return st;
-  }
-  st = launch_colsum(bufB, dbm_part, B, N, d, 1, stream);
-  if (st != MAC_OK) return st;
-  // (4) Z = [P*y, P] @ Wm + bm:  dWm += I0^T dZ ;  dI0 = dZ @ Wm^T
-  if (dWm) {
-    SgemmParams p{};
-    p.a_mode = A_TRANS_ROWSCALE_CONCAT; p.nseg = 1; p.a[0] = P; p.lda[0] = d; p.rowvec = y; p.rows_per_batch = N;
-    p.W = bufB; p.ldw = d; p.M = 2 * d; p.N = d; p.K = M;
-    p.epi = EPI_BIAS_ACT; p.Y = dWm; p.ldy = d; p.accumulate = 1;
-    st = sgemm_launch(p, counters, partial, pbytes, stream);
-    if (st != MAC_OK) return st;
-  }
-  {
-    SgemmParams p{};
-    p.a_mode = A_SEGS; p.nseg = 1; p.a[0] = bufB; p.ak[0] = d; p.lda[0] = d;
-    p.W = Wm_t; p.ldw = 2 * d; p.M = M; p.N = 2 * d; p.K = d;
-    p.epi = EPI_BIAS_ACT; p.act = MAC_ACT_NON; p.Y = bufC; p.ldy = 2 * d;
-    st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-    if (st != MAC_OK) return st;
-  }
-  // (5) I0 = [P*y, P]:  dP, dy, dbx   (dP overwrites bufA)
-  read_bwd_p_kernel<<<dim3((d + 127) / 128, B), 256, 0, stream>>>(bufC, P, y, bufA, dy, dbx_part, N, d);
-  MAC_LAUNCH_CHECK();
-  // (6) P = dropout(KB) @ Wx + bx:  dWx += Kd^T dP ;  dKB += (dP @ Wx^T) * mask/keep
-  if (dWx) {
-    SgemmParams p{};
-    p.a_mode = drop ? A_TRANS_DROPOUT : A_TRANS; p.nseg = 1; p.a[0] = kb; p.lda[0] = d;
-    p.a_thresh = thr; p.a_scale = scale; p.seed = seed; p.a_site = MAC_SITE_READ_KB; p.step = step;
-    p.W = bufA; p.ldw = d; p.M = d; p.N = d; p.K = M;
-    p.epi = EPI_BIAS_ACT; p.Y = dWx; p.ldy = d; p.accumulate = 1;
-    st = sgemm_launch(p, counters, partial, pbytes, stream);
-    if (st != MAC_OK) return st;
-  }
-  if (dkb) {
-    SgemmParams p{};
-    p.a_mode = A_SEGS; p.nseg = 1; p.a[0] = bufA; p.ak[0] = d; p.lda[0] = d;
-    p.W = Wx_t; p.ldw = d; p.M = M; p.N = d; p.K = d;
-    p.epi = EPI_ACCUM_DROPOUT; p.Y = dkb; p.ldy = d;
-    p.e_thresh = thr; p.e_scale = scale; p.e_site = MAC_SITE_READ_KB; p.seed = seed; p.step = step;
-    st = sgemm_launch(p, nullptr, nullptr, 0, stream, false);
-    if (st != MAC_OK) return st;
-  }
-  // (7) y = md @ Wy + by with md = dropout(memory_in):  dWy += md^T dy ; dby += colsum(dy) ; dmem_in = (dy @ Wy^T)*mask/keep
-  // mac_linear_bwd gets no workspace, so these K = B products run without split-K.  Its split-K partials would start at
-  // ws + BW_HEADER = f, and at small N (B*N*4 < splitk*d) they would overwrite its own inputs dy, md and dmd, which live
-  // in f behind the [B*N] buffers.
-  const float* mdp = memory_in;
-  if (drop) {
-    st = mac_dropout_fwd(memory_in, keep_read, seed, MAC_SITE_READ_MEM, step, md, (long long)B * d, stream_);
-    if (st != MAC_OK) return st;
-    mdp = md;
-  }
-  {
-    const float* xs[1] = {mdp};
-    const int ks[1] = {d};
-    float* dxs[1] = {drop ? dmd : dmem_in};
-    const int acc0[1] = {0};
-    st = mac_linear_bwd(xs, ks, ks, 1, Wy_t, dy, d, dxs, ks, acc0, dWy, dby, B, d, nullptr, 0, stream_);
-    if (st != MAC_OK) return st;
-    if (drop) {
-      st = mac_dropout_fwd(dmd, keep_read, seed, MAC_SITE_READ_MEM, step, dmem_in, (long long)B * d, stream_);
-      if (st != MAC_OK) return st;
-    }
-  }
-  return MAC_OK;
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Backward of the read unit with the six [B*N, .] x [., .] products on wgmma tensor cores (bf16 operands, fp32
-// accumulation; everything element-wise stays fp32).  Same inputs, outputs and accumulation conventions as
-// mac_read_bwd; the GEMMs go through the entry points the forward uses (mac_linear_tc_fwd), fed by the cast / transposing
-// cast kernels (mac_cast_bf16, mac_pack_weight_bf16):
-//   dgrad  dX[M, in]   = dY[M, out] @ W^T        x = bf16(dY) [M, out],  Wt operand = bf16(W) in its own [in, out] layout
-//   wgrad  dW[in, out] = X^T[in, M] @ dY[M, out]  x = bf16(X)^T [in, M],  Wt operand = bf16(dY)^T [out, M]   (K = M = B*N)
-// The prologue fusions of the fp32 kernels live in the transposing cast here (pack_t_bf16_kernel applies P*y / the KB dropout
-// mask while it builds the bf16 operand, and writes the row-major bf16 copy of a gradient from the same read); * ELU'(H) with
-// its column sums and the dropout mask on dKB are one fp32 pass each.  The arithmetic of every pass is the forward's, so the
-// masks and saved tensors are shared.
-// Requires d % 128 == 0 and (B*N) % 64 == 0 (the wgmma k-block of the weight-gradient products, K = B*N); otherwise MAC_ERR_UNSUPPORTED (use mac_read_bwd).
-// ------------------------------------------------------------------------------------------------------------------
-extern "C" int mac_tc_wgrad_splitk_(const void* xT, const void* gT, float* dW, float* partial, int in_dim, int out_dim, int K,
-                                    mac_stream_t stream_);
-extern "C" size_t mac_tc_wgrad_partial_bytes_(int in_dim, int out_dim);
-extern "C" int mac_pack_t_bf16_(int mode, const float* X, void* Xt, void* Xrm, int K, int N, const float* rowvec,
-                                int rows_per_batch, uint32_t thresh, float scale, uint64_t seed, int site, int step,
-                                mac_stream_t stream_);
-static size_t rbt_align(size_t x) { return (x + 1023) & ~(size_t)1023; }
-
-namespace mac {
-// The schedule both tensor-core read backwards share (mac_read_bwd_tc, mac_read_bwd_tc32): mac_read_bwd's seven steps with
-// its six [B*N, .] products delegated to the caller's operations on its own scratch (behind the fp32 layout of mac_read_bwd,
-// whose bufA / bufB / bufC / dka / dkl / dy / md / dmd this function carves):
-//   packX(mode, X, half, rowvec)  activations [M, d] -> the transposed operand of the next wgrad, rows d*half .. (mode 0
-//                                 plain, 1 P*y, 2 the forward's KB dropout)
-//   wgrad(in, G, dW)              dW[in, d] += X^T G with X from the packX calls; leaves G's operand for the next dgrad
-//   dgrad(W, in, out)             out[M, in] = G W^T with W fp32 in its own [in, d] layout and G from the preceding wgrad
-// tmp32 is fp32 scratch [M, d].
-template <class PackX, class WGrad, class DGrad>
-static int read_bwd_tc_schedule(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
-                                const float* Wy_t, const float* att, const float* save, const float* dinfo, float keep_read,
-                                uint64_t seed, int step, float* dkb, float* dmem_in, float* dcontrol, float* dWx,
-                                float* dbx_part, float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2,
-                                float* dbm2_part, float* dwr_part, float* dbr_part, void* workspace, float* tmp32, int B,
-                                int N, int d, mac_stream_t stream_, PackX packX, WGrad wgrad, DGrad dgrad) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const int M = B * N;
-  const size_t Md = (size_t)M * d;
-  char* ws = reinterpret_cast<char*>(workspace);
-  float* f = reinterpret_cast<float*>(ws + BW_HEADER);
-  float* bufA = f;                 // dI1, later dP
-  float* bufB = f + Md;            // dZ
-  float* bufC = f + 2 * Md;        // dI0 [M, 2d]
-  float* dka = f + 4 * Md;         // [B,N]
-  const size_t BNp = ((size_t)B * N + 3) & ~(size_t)3;
-  float* dkl = dka + BNp;
-  float* dy = dkl + BNp;           // [B,d]
-  float* md = dy + (size_t)B * d;  // [B,d]
-  float* dmd = md + (size_t)B * d; // [B,d]
-  const float* P = save;
-  const float* H = save + Md;
-  const float* I1 = save + 2 * Md;
-  const float* y = save + 3 * Md;
-  const bool drop = keep_read < 1.f;
-  const uint32_t thr = drop ? keep_threshold(keep_read) : 0u;
-  const float scale = drop ? 1.f / keep_read : 1.f;
-  int st;
-#define RBT(call)                 \
-  do {                            \
-    st = (call);                  \
-    if (st != MAC_OK) return st;  \
-  } while (0)
-  // (1) info = sum_n att*KB ; att = softmax(kl):  dkl, dKB += att (x) dinfo
-  RBT(mac_kb_attend_bwd(kb, att, dinfo, dka, dkl, dkb, dbr_part, B, N, d, stream_));
-  // (2) logits epilogue backward -> dI1 (bufA), dcontrol, dwr, dbm2
-  read_bwd_logits_kernel<<<dim3((d + 127) / 128, B), 256, 0, stream>>>(I1, control, w->wr, dkl, thr, scale, seed, step,
-                                                                      bufA, dcontrol, dwr_part, dbm2_part, N, d);
-  MAC_LAUNCH_CHECK();
-  // (3) I1 = H @ Wm2 + bm2:  dWm2 += H^T dI1 ;  dZ = (dI1 @ Wm2^T) * ELU'(H) ; dbm += colsum(dZ)
-  RBT(packX(0, H, 0, nullptr));
-  RBT(wgrad(d, bufA, dWm2));
-  RBT(dgrad(w->Wm2, d, tmp32));
-  elu_bwd_colsum_kernel<<<dim3((d + 127) / 128, B), 256, 0, stream>>>(H, tmp32, bufB, dbm_part, N, d);
-  MAC_LAUNCH_CHECK();
-  // (4) Z = [P*y, P] @ Wm + bm:  dWm += [P*y, P]^T dZ ;  dI0 = dZ @ Wm^T
-  RBT(packX(1, P, 0, y));                                                                     // rows 0..d-1:   (P*y)^T
-  RBT(packX(0, P, 1, nullptr));                                                               // rows d..2d-1: P^T
-  RBT(wgrad(2 * d, bufB, dWm));
-  RBT(dgrad(w->Wm, 2 * d, bufC));
-  // (5) I0 = [P*y, P]:  dP (bufA), dy, dbx
-  read_bwd_p_kernel<<<dim3((d + 127) / 128, B), 256, 0, stream>>>(bufC, P, y, bufA, dy, dbx_part, N, d);
-  MAC_LAUNCH_CHECK();
-  // (6) P = dropout(KB) @ Wx + bx:  dWx += Kd^T dP ;  dKB += (dP @ Wx^T) * mask/keep
-  RBT(packX(drop ? 2 : 0, kb, 0, nullptr));                                                   // dropout(KB)^T: the forward's mask
-  RBT(wgrad(d, bufA, dWx));
-  if (dkb) {
-    RBT(dgrad(w->Wx, d, tmp32));
-    if (drop) {
-      axpy_dropout_kernel<<<(unsigned)((Md / 4 + 255) / 256), 256, 0, stream>>>(
-          reinterpret_cast<float4*>(dkb), reinterpret_cast<const float4*>(tmp32), thr, scale, seed, MAC_SITE_READ_KB, step,
-          (long long)(Md / 4));
-      MAC_LAUNCH_CHECK();
-    } else {
-      RBT(mac_axpy(dkb, tmp32, 1.f, (long long)Md, stream_));
-    }
-  }
-  // (7) y = md @ Wy + by with md = dropout(memory_in): an M = B product, fp32 (mac_linear_bwd)
-  const float* mdp = memory_in;
-  if (drop) {
-    RBT(mac_dropout_fwd(memory_in, keep_read, seed, MAC_SITE_READ_MEM, step, md, (long long)B * d, stream_));
-    mdp = md;
-  }
-  {
-    const float* xs[1] = {mdp};
-    const int ks[1] = {d};
-    float* dxs[1] = {drop ? dmd : dmem_in};
-    const int acc0[1] = {0};
-    RBT(mac_linear_bwd(xs, ks, ks, 1, Wy_t, dy, d, dxs, ks, acc0, dWy, dby, B, d, nullptr, 0, stream_));
-    if (drop) RBT(mac_dropout_fwd(dmd, keep_read, seed, MAC_SITE_READ_MEM, step, dmem_in, (long long)B * d, stream_));
-  }
-#undef RBT
-  return MAC_OK;
-}
-}  // namespace mac
-
-extern "C" size_t mac_read_bwd_tc_workspace_bytes(int B, int N, int d) {
-  const size_t M = (size_t)B * N;
-  return mac_read_bwd_workspace_bytes(B, N, d) + 1024 + rbt_align(M * 2 * d * 2) /*g16*/ + rbt_align(2 * d * M * 2) /*xT16*/ +
-         rbt_align(d * M * 2) /*gT16*/ + rbt_align((size_t)2 * d * d * 2) /*w16*/ + rbt_align(M * 2 * d * 4) /*tmp32*/ +
-         rbt_align(mac_tc_wgrad_partial_bytes_(2 * d, d)) /*dWtmp: split-K partials of the largest weight gradient*/;
+  return read_bwd({RB_FP32, kb, memory_in, control, w, Wx_t, Wy_t, Wm_t, Wm2_t, att, save, dinfo, keep_read, seed, step, dkb,
+                   dmem_in, dcontrol, dWx, dbx_part, dWy, dby, dWm, dbm_part, dWm2, dbm2_part, dwr_part, dbr_part, workspace,
+                   workspace_bytes, B, N, d, reinterpret_cast<cudaStream_t>(stream_)});
 }
 
 extern "C" int mac_read_bwd_tc(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
@@ -1032,76 +1067,9 @@ extern "C" int mac_read_bwd_tc(const float* kb, const float* memory_in, const fl
                                float* dbx_part, float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2,
                                float* dbm2_part, float* dwr_part, float* dbr_part, void* workspace, size_t workspace_bytes,
                                int B, int N, int d, mac_stream_t stream_) {
-  if (!kb || !memory_in || !control || !w || !att || !save || !dinfo || !dmem_in || !dcontrol || !workspace || !dWx ||
-      !dWm || !dWm2)
-    return MAC_ERR_INVALID;
-  const int M = B * N;
-  if ((d % 128) || (M % 64)) return MAC_ERR_UNSUPPORTED;
-  if (workspace_bytes < mac_read_bwd_tc_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
-  // tensor-core operands behind the fp32 layout of mac_read_bwd
-  char* x = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(reinterpret_cast<char*>(workspace) +
-                                                                 mac_read_bwd_workspace_bytes(B, N, d)) + 1023) &
-                                    ~(uintptr_t)1023);
-  void* g16 = x;   x += rbt_align((size_t)M * 2 * d * 2);        // bf16 [M, <=2d]   gradient as the A operand of a dgrad
-  void* xT16 = x;  x += rbt_align((size_t)2 * d * M * 2);        // bf16 [<=2d, M]   activations, transposed
-  void* gT16 = x;  x += rbt_align((size_t)d * M * 2);            // bf16 [d, M]      gradient, transposed
-  void* w16 = x;   x += rbt_align((size_t)2 * d * d * 2);        // bf16 weight in its own [in, out] layout
-  float* tmp32 = reinterpret_cast<float*>(x); x += rbt_align((size_t)M * 2 * d * 4);
-  float* dWtmp = reinterpret_cast<float*>(x);
-  const bool drop = keep_read < 1.f;
-  const uint32_t thr = drop ? keep_threshold(keep_read) : 0u;
-  const float scale = drop ? 1.f / keep_read : 1.f;
-  // activations / gradients for the tensor-core operands: fp32 [M, d] -> bf16 transposed [d, M] (+ optionally the row-major
-  // bf16 copy), with the forward's P*y scaling or KB dropout applied on the way (pack_t_bf16_kernel, csrc/tc_gemm.cuh)
-  auto packT = [&](int mode, const float* X, void* Xt, void* Xrm, const float* rowvec) -> int {
-    return mac_pack_t_bf16_(mode, X, Xt, Xrm, M, d, rowvec, N, thr, scale, seed, MAC_SITE_READ_KB, step, stream_);
-  };
-  auto packX = [&](int mode, const float* X, int half, const float* rowvec) -> int {
-    return packT(mode, X, reinterpret_cast<__nv_bfloat16*>(xT16) + (size_t)half * d * M, nullptr, rowvec);
-  };
-  // wgrad: dW[in, out] += X^T @ G with X^T already packed as xT [in, M]; leaves bf16(G) row-major in g16 for the dgrad below
-  auto wgrad = [&](int in, const float* G, float* dW) -> int {
-    int s = packT(0, G, gT16, g16, nullptr);                                                 // G [M, d] -> G^T [d, M], bf16(G)
-    if (s != MAC_OK) return s;
-    return mac_tc_wgrad_splitk_(xT16, gT16, dW, dWtmp, in, d, M, stream_);                        // dW[in, d] += xT @ (G^T)^T, split-K
-  };
-  // dgrad: out[M, in] = G[M, d] @ W[in, d]^T   (W fp32 in its own [in, out = d] layout; G = the g16 of the preceding wgrad)
-  auto dgrad = [&](const float* W, int in, float* out) -> int {
-    int s = mac_cast_bf16(W, w16, (long long)in * d, stream_);
-    if (s != MAC_OK) return s;
-    return mac_linear_tc_fwd(g16, w16, nullptr, MAC_ACT_NON, out, 0, M, d, in, stream_);
-  };
-  return read_bwd_tc_schedule(kb, memory_in, control, w, Wy_t, att, save, dinfo, keep_read, seed, step, dkb, dmem_in, dcontrol,
-                              dWx, dbx_part, dWy, dby, dWm, dbm_part, dWm2, dbm2_part, dwr_part, dbr_part, workspace, tmp32, B,
-                              N, d, stream_, packX, wgrad, dgrad);
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Backward of the split-bf16 ("tc32") training read: the schedule of mac_read_bwd_tc with its six [B*N, .] products as
-// split-bf16 products (x = hi + lo, three of the four partial products, one fp32 accumulator), so the backward keeps the
-// forward's fp32-class accuracy:
-//   dgrad  dX[M, in] = G @ W^T:  A' = [G_hi | G_lo] [M, 2 out] (written by the transposing pack from the same read of G),
-//          W' = [W_hi | W_hi | W_lo] [in, 3 out] per row of W in its own [in, out] layout; one tc3_gemm, fp32 out
-//   wgrad  dW += X^T G over Mp = B*N rounded up to 64:  [X_hi^T | X_lo^T] [in, 2Mp] against [G_hi^T | G_hi^T | G_lo^T]
-//          [out, 3Mp], ONE split-K launch (tc3_wgrad_splitk; faster on the H100 than three accumulating tc_wgrad_splitk
-//          calls, DESIGN.md section 9 item 5); the zero columns M..Mp-1 are written on every call
-// The transposing pack applies P*y (mode 1) and the forward's KB dropout mask (mode 2) as in mac_read_bwd_tc; the element-wise
-// kernels are mac_read_bwd's.  Any B*N; d % 128 == 0, else MAC_ERR_UNSUPPORTED before any launch.
-// ------------------------------------------------------------------------------------------------------------------
-extern "C" int mac_pack_t_split_(int mode, const float* X, void* Xt, void* Xrm, int K, int N, int segs, const float* rowvec,
-                                 int rows_per_batch, uint32_t thresh, float scale, uint64_t seed, int site, int step,
-                                 mac_stream_t stream_);
-extern "C" int mac_tc3_wgrad_splitk_(const void* xT2, const void* gT3, float* dW, float* partial, int in_dim, int out_dim,
-                                     int kp, mac_stream_t stream_);
-extern "C" int mac_split3_rows_(const float* W, void* W3, int R, int C, mac_stream_t stream_);
-extern "C" int mac_tc3_linear_(const void* a_split, const void* wt3, float* y, int M, int K, int n_out, mac_stream_t stream_);
-
-extern "C" size_t mac_read_bwd_tc32_workspace_bytes(int B, int N, int d) {
-  const size_t M = (size_t)B * N, Mp = (M + 63) & ~(size_t)63;
-  return mac_read_bwd_workspace_bytes(B, N, d) + 1024 + rbt_align(M * 2 * d * 2) /*g2: [G_hi | G_lo]*/ +
-         rbt_align((size_t)2 * d * 2 * Mp * 2) /*xT2*/ + rbt_align((size_t)d * 3 * Mp * 2) /*gT3*/ +
-         rbt_align((size_t)2 * d * 3 * d * 2) /*w3*/ + rbt_align(M * d * 4) /*tmp32*/ +
-         rbt_align(mac_tc_wgrad_partial_bytes_(2 * d, d)) /*split-K partials of the largest weight gradient*/;
+  return read_bwd({RB_TC, kb, memory_in, control, w, nullptr, Wy_t, nullptr, nullptr, att, save, dinfo, keep_read, seed, step,
+                   dkb, dmem_in, dcontrol, dWx, dbx_part, dWy, dby, dWm, dbm_part, dWm2, dbm2_part, dwr_part, dbr_part,
+                   workspace, workspace_bytes, B, N, d, reinterpret_cast<cudaStream_t>(stream_)});
 }
 
 extern "C" int mac_read_bwd_tc32(const float* kb, const float* memory_in, const float* control, const mac_read_weights* w,
@@ -1110,46 +1078,7 @@ extern "C" int mac_read_bwd_tc32(const float* kb, const float* memory_in, const 
                                  float* dbx_part, float* dWy, float* dby, float* dWm, float* dbm_part, float* dWm2,
                                  float* dbm2_part, float* dwr_part, float* dbr_part, void* workspace, size_t workspace_bytes,
                                  int B, int N, int d, mac_stream_t stream_) {
-  if (!kb || !memory_in || !control || !w || !att || !save || !dinfo || !dmem_in || !dcontrol || !workspace || !dWx ||
-      !dWm || !dWm2)
-    return MAC_ERR_INVALID;
-  if (B <= 0 || N <= 0 || d <= 0) return MAC_ERR_INVALID;
-  if (d % 128) return MAC_ERR_UNSUPPORTED;
-  if (!(keep_read > 0.f && keep_read <= 1.f)) return MAC_ERR_INVALID;
-  if (workspace_bytes < mac_read_bwd_tc32_workspace_bytes(B, N, d)) return MAC_ERR_WORKSPACE;
-  const int M = B * N;
-  const size_t Mp = ((size_t)M + 63) & ~(size_t)63;
-  // split operands behind the fp32 layout of mac_read_bwd
-  char* x = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(reinterpret_cast<char*>(workspace) +
-                                                                 mac_read_bwd_workspace_bytes(B, N, d)) + 1023) &
-                                    ~(uintptr_t)1023);
-  void* g2 = x;    x += rbt_align((size_t)M * 2 * d * 2);          // bf16 [M, 2d]        [G_hi | G_lo], A' of a dgrad
-  void* xT2 = x;   x += rbt_align((size_t)2 * d * 2 * Mp * 2);     // bf16 [<=2d, 2Mp]    [X_hi^T | X_lo^T]
-  void* gT3 = x;   x += rbt_align((size_t)d * 3 * Mp * 2);         // bf16 [d, 3Mp]       [G_hi^T | G_hi^T | G_lo^T]
-  void* w3 = x;    x += rbt_align((size_t)2 * d * 3 * d * 2);      // bf16 [<=2d, 3d]     [W_hi | W_hi | W_lo] per row of W
-  float* tmp32 = reinterpret_cast<float*>(x); x += rbt_align((size_t)M * d * 4);
-  float* dWtmp = reinterpret_cast<float*>(x);
-  const bool drop = keep_read < 1.f;
-  const uint32_t thr = drop ? keep_threshold(keep_read) : 0u;
-  const float scale = drop ? 1.f / keep_read : 1.f;
-  // activations [M, d] -> [X_hi^T | X_lo^T] rows of xT2 (row pitch 2Mp), with P*y or the KB dropout applied on the way
-  auto packX = [&](int mode, const float* X, int half, const float* rowvec) -> int {
-    return mac_pack_t_split_(mode, X, reinterpret_cast<__nv_bfloat16*>(xT2) + (size_t)half * d * 2 * Mp, nullptr, M, d, 2,
-                             rowvec, N, thr, scale, seed, MAC_SITE_READ_KB, step, stream_);
-  };
-  // wgrad: dW[in, d] += X^T G with X already in xT2; leaves [G_hi | G_lo] row-major in g2 for the dgrad below
-  auto wgrad = [&](int in, const float* G, float* dW) -> int {
-    int s = mac_pack_t_split_(0, G, gT3, g2, M, d, 3, nullptr, 1, 0u, 1.f, 0, 0, 0, stream_);
-    if (s != MAC_OK) return s;
-    return mac_tc3_wgrad_splitk_(xT2, gT3, dW, dWtmp, in, d, (int)Mp, stream_);
-  };
-  // dgrad: out[M, in] = G[M, d] @ W[in, d]^T   (W fp32 in its own [in, out = d] layout; G = the g2 of the preceding wgrad)
-  auto dgrad = [&](const float* W, int in, float* out) -> int {
-    int s = mac_split3_rows_(W, w3, in, d, stream_);
-    if (s != MAC_OK) return s;
-    return mac_tc3_linear_(g2, w3, out, M, d, in, stream_);
-  };
-  return read_bwd_tc_schedule(kb, memory_in, control, w, Wy_t, att, save, dinfo, keep_read, seed, step, dkb, dmem_in, dcontrol,
-                              dWx, dbx_part, dWy, dby, dWm, dbm_part, dWm2, dbm2_part, dwr_part, dbr_part, workspace, tmp32, B,
-                              N, d, stream_, packX, wgrad, dgrad);
+  return read_bwd({RB_TC32, kb, memory_in, control, w, nullptr, Wy_t, nullptr, nullptr, att, save, dinfo, keep_read, seed,
+                   step, dkb, dmem_in, dcontrol, dWx, dbx_part, dWy, dby, dWm, dbm_part, dWm2, dbm2_part, dwr_part, dbr_part,
+                   workspace, workspace_bytes, B, N, d, reinterpret_cast<cudaStream_t>(stream_)});
 }

@@ -18,6 +18,7 @@ import ctypes
 import torch
 
 from ._lib import ACT, check, ptr, stream_ptr
+from .autograd import read_bwd, read_bwd_workspace_bytes
 from .params import PREFIX
 
 
@@ -294,31 +295,18 @@ class Tape(object):
             nWy, nby = lin_names(rsc + "mulmemInter/", "projY")
             nWm, nbm = lin_names(rsc, "memKbProj")
             nWm2, nbm2 = lin_names(rsc + "linearLayermemKbProj/", "memKbProj_2")
-            T = lambda nm: self.p.derived(("T", nm), lambda: self.p.t[nm].t().contiguous())
+            wnames = {"Wx": nWx, "Wy": nWy, "Wm": nWm, "Wm2": nWm2}
+            Wt = lambda k: self.p.derived(("T", wnames[k]), lambda: self.p.t[wnames[k]].t().contiguous())
             part = {k: self.z(B, d) for k in ("wr", "bx", "bm", "bm2")}
             dbr = self.z(B)
             dmem_in = self.e(B, d)
-            ws_bytes = int((self.lib.mac_read_bwd_tc_workspace_bytes if self.tc else self.lib.mac_read_bwd_workspace_bytes)(
-                B, N, d))
+            form = "tc" if self.tc else "fp32"
+            ws_bytes = read_bwd_workspace_bytes(self.lib, form, B, N, d)
             if getattr(self, "_rws", None) is None or self._rws.numel() < ws_bytes:
                 self._rws = torch.zeros(ws_bytes, dtype=torch.uint8, device=self.dev)
-            if self.tc:
-                check(self.lib.mac_read_bwd_tc(ptr(knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
-                                               ptr(T(nWy)), ptr(cell._att_kb[i]), ptr(cell._save[i]), ptr(self.grad(info)),
-                                               float(cell.dropouts["read"]), cell.seed, i, ptr(self.grad(knowledgeBase)),
-                                               ptr(dmem_in), ptr(self.grad(control)), ptr(self.G(nWx)), ptr(part["bx"]),
-                                               ptr(self.G(nWy)), ptr(self.G(nby)), ptr(self.G(nWm)), ptr(part["bm"]),
-                                               ptr(self.G(nWm2)), ptr(part["bm2"]), ptr(part["wr"]), ptr(dbr), ptr(self._rws),
-                                               ws_bytes, B, N, d, stream_ptr()), "mac_read_bwd_tc")
-            else:
-                check(self.lib.mac_read_bwd(ptr(knowledgeBase), ptr(cell._mem_in_hist[i]), ptr(control), ctypes.byref(rw),
-                                            ptr(T(nWx)), ptr(T(nWy)), ptr(T(nWm)), ptr(T(nWm2)), ptr(cell._att_kb[i]),
-                                            ptr(cell._save[i]), ptr(self.grad(info)), float(cell.dropouts["read"]), cell.seed,
-                                            i, ptr(self.grad(knowledgeBase)), ptr(dmem_in), ptr(self.grad(control)),
-                                            ptr(self.G(nWx)), ptr(part["bx"]), ptr(self.G(nWy)), ptr(self.G(nby)),
-                                            ptr(self.G(nWm)), ptr(part["bm"]), ptr(self.G(nWm2)), ptr(part["bm2"]),
-                                            ptr(part["wr"]), ptr(dbr), ptr(self._rws), ws_bytes, B, N, d, stream_ptr()),
-                      "mac_read_bwd")
+            read_bwd(self.lib, form, cell, i, knowledgeBase, control, rw, Wt, self.grad(info),
+                     [self.grad(knowledgeBase), dmem_in, self.grad(control), self.G(nWx), part["bx"], self.G(nWy),
+                      self.G(nby), self.G(nWm), part["bm"], self.G(nWm2), part["bm2"], part["wr"], dbr], self._rws, ws_bytes)
             self.axpy(self.grad(memory_in), dmem_in)
             self.colsum_B(part["wr"], self.G(PREFIX + lsc + "weights/weight"))
             self.colsum_B(part["bx"], self.G(nbx))
