@@ -469,6 +469,25 @@ int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* dy, const fl
                        int site, int step, float* dkernel, float* dbias, float* dx, void* workspace, size_t workspace_bytes,
                        int B, int H, int W, int C, int Cout, mac_stream_t stream);
 size_t mac_conv3x3_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx);
+/* The stem layer as split-bf16 ("tc32") tensor-core products inside the fp32 parity bar (Stem(prec="bf16x3"); tc3_gemm in
+ * csrc/tc_gemm.cuh: x = hi + lo with hi = bf16(x), lo = bf16(x - hi); A W ~ A_hi W_hi + A_lo W_hi + A_hi W_lo in one fp32
+ * accumulator).
+ * mac_im2col3x3_split: the patch matrix of mac_im2col3x3 as cols2 [M, 2*9C] bf16, row m = [hi(patch_m) | lo(patch_m)] of the
+ *   fp32 value mac_im2col3x3 writes (same column order, same keep-mask bit for bit).  C % 64 == 0, else MAC_ERR_UNSUPPORTED.
+ * mac_linear_tc32_fwd: y[M, n_out] = act(A W + b) in fp32 from a_split [M, 2K] = [A_hi | A_lo] and wt3 [n_out, 3K]
+ *   (mac_pack_weight_split3).  b may be NULL; act any MAC_ACT_*.  K % 64 == 0 and n_out % 128 == 0, else
+ *   MAC_ERR_UNSUPPORTED; any M >= 1.
+ * mac_conv3x3_bwd_tc32: mac_conv3x3_bwd_tc's signature and contract with split-bf16 operands for both GEMMs (the weight
+ *   gradient is one split-K launch over 3 * Mp, Mp = B*H*W rounded up to 64); its own workspace query.
+ * All checks precede any launch. */
+int mac_im2col3x3_split(const float* x, void* cols2_bf16, float keep, uint64_t seed, int site, int step, int B, int H, int W,
+                        int C, mac_stream_t stream);
+int mac_linear_tc32_fwd(const void* a_split, const void* wt3, const float* b, int act, float* y, int M, int K, int n_out,
+                        mac_stream_t stream);
+int mac_conv3x3_bwd_tc32(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep, uint64_t seed,
+                         int site, int step, float* dkernel, float* dbias, float* dx, void* workspace, size_t workspace_bytes,
+                         int B, int H, int W, int C, int Cout, mac_stream_t stream);
+size_t mac_conv3x3_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx);
 
 /* ------------------------------------------------------------------------------------------------
  * Question input unit ("next" row, model.py:208-220, 279-307; ops.py:859-905): embedding lookup + bi-LSTM encoder.

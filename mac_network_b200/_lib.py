@@ -123,6 +123,11 @@ PROTOTYPES = {
     "mac_conv3x3_bwd_tc": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_fp, c_fp, c_sz,
                                    c_int, c_int, c_int, c_int, c_int, c_fp]),
     "mac_conv3x3_bwd_tc_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "mac_im2col3x3_split": (c_int, [c_fp, c_fp, c_f, c_u64, c_int, c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_linear_tc32_fwd": (c_int, [c_fp, c_fp, c_fp, c_int, c_fp, c_int, c_int, c_int, c_fp]),
+    "mac_conv3x3_bwd_tc32": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_fp, c_fp, c_sz,
+                                     c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_conv3x3_bwd_tc32_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "mac_pack_weight_bf16": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_split3": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_fp8": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_fp]),

@@ -296,10 +296,20 @@ extern "C" int mac_split3_rows_(const float* W, void* W3, int R, int C, mac_stre
   MAC_LAUNCH_CHECK();
   return MAC_OK;
 }
-// y[M, n_out] = A @ W with A' = [A_hi | A_lo] [M, 2K] and W' [n_out, 3K] (tc3_gemm, fp32 out, stored)
+// y[M, n_out] = A @ W with A' = [A_hi | A_lo] [M, 2K] and W' [n_out, 3K]: mac_linear_tc32_fwd without bias or activation
 extern "C" int mac_tc3_linear_(const void* a_split, const void* wt3, float* y, int M, int K, int n_out, mac_stream_t stream_) {
+  return mac_linear_tc32_fwd(a_split, wt3, nullptr, MAC_ACT_NON, y, M, K, n_out, stream_);
+}
+
+extern "C" int mac_linear_tc32_fwd(const void* a_split, const void* wt3, const float* b, int act, float* y, int M, int K,
+                                   int n_out, mac_stream_t stream_) {
+  if (!a_split || !wt3 || !y || M <= 0 || K <= 0 || n_out <= 0) return MAC_ERR_INVALID;
+  if ((K % TC_BK) || (n_out % TC_BN) || act < MAC_ACT_NON || act > MAC_ACT_RELU) return MAC_ERR_UNSUPPORTED;
+  if ((M + TC_BM - 1) / TC_BM > 65535) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(a_split) || !mac_aligned16(wt3) || (reinterpret_cast<uintptr_t>(y) & 7)) return MAC_ERR_ALIGN;
+  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
   TcGemmParams p{};
-  p.M = M; p.N = n_out; p.act = MAC_ACT_NON; p.bias = nullptr; p.ldo = n_out; p.rows_per_batch = 1;
+  p.M = M; p.N = n_out; p.act = act; p.bias = b; p.ldo = n_out; p.rows_per_batch = 1;
   p.epi = TC_EPI_F32; p.outf = y;
   return tc3_gemm(a_split, K, wt3, p, reinterpret_cast<cudaStream_t>(stream_));
 }
@@ -580,6 +590,72 @@ extern "C" int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float ke
   return MAC_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ stem: split-bf16 patches
+// The patch matrix of mac_im2col3x3 as the A operand of tc3_gemm: cols2[m, k] = bf16(v), cols2[m, 9C + k] = bf16(v - hi) with
+// v the fp32 value mac_im2col3x3 writes at cols[m, k] (same Philox draw: the quad index of the SOURCE element).  Eight
+// channels per thread: two 16-byte loads, one 16-byte store per half.
+namespace mac {
+__device__ __forceinline__ uint32_t pack_bf16_lo(float a, float b, uint32_t hw) {      // lo of the pair whose hi is `hw`
+  return pack_bf16(a - __uint_as_float(hw << 16), b - __uint_as_float(hw & 0xffff0000u));
+}
+
+__global__ void __launch_bounds__(256) im2col3x3_split_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ cols2,
+                                                             uint32_t thresh, float scale, uint64_t seed, int site, int step,
+                                                             int B, int H, int W, int C) {
+  const int c8n = C / 8;
+  const long long total = (long long)B * H * W * 9 * c8n;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int c8 = (int)(i % c8n);
+  long long r = i / c8n;
+  const int tap = (int)(r % 9);
+  const long long m = r / 9;
+  const int w = (int)(m % W);
+  r = m / W;
+  const int h = (int)(r % H), b = (int)(r / H);
+  const int hs = h + tap / 3 - 1, wsrc = w + tap % 3 - 1;
+  float4 v[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+  if (hs >= 0 && hs < H && wsrc >= 0 && wsrc < W) {
+    const long long e = (((long long)b * H + hs) * W + wsrc) * C + c8 * 8;
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      v[q] = __ldg(reinterpret_cast<const float4*>(x + e) + q);
+      if (thresh) {
+        const Philox4 p = philox4x32_10(seed, ((uint64_t)e >> 2) + q, (uint32_t)site, (uint32_t)step);
+        v[q].x = ((p.x >> 8) >= thresh) ? v[q].x * scale : 0.f;
+        v[q].y = ((p.y >> 8) >= thresh) ? v[q].y * scale : 0.f;
+        v[q].z = ((p.z >> 8) >= thresh) ? v[q].z * scale : 0.f;
+        v[q].w = ((p.w >> 8) >= thresh) ? v[q].w * scale : 0.f;
+      }
+    }
+  }
+  uint4 hi, lo;
+  hi.x = pack_bf16(v[0].x, v[0].y); hi.y = pack_bf16(v[0].z, v[0].w);
+  hi.z = pack_bf16(v[1].x, v[1].y); hi.w = pack_bf16(v[1].z, v[1].w);
+  lo.x = pack_bf16_lo(v[0].x, v[0].y, hi.x); lo.y = pack_bf16_lo(v[0].z, v[0].w, hi.y);
+  lo.z = pack_bf16_lo(v[1].x, v[1].y, hi.z); lo.w = pack_bf16_lo(v[1].z, v[1].w, hi.w);
+  __nv_bfloat16* row = cols2 + (m * 18 + tap) * C + c8 * 8;
+  *reinterpret_cast<uint4*>(row) = hi;
+  *reinterpret_cast<uint4*>(row + 9 * C) = lo;
+}
+}  // namespace mac
+
+extern "C" int mac_im2col3x3_split(const float* x, void* cols2, float keep, uint64_t seed, int site, int step, int B, int H,
+                                   int W, int C, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x || !cols2 || B <= 0 || H <= 0 || W <= 0 || C <= 0 || !(keep > 0.f && keep <= 1.f)) return MAC_ERR_INVALID;
+  if ((long long)B * H * W > (1LL << 30)) return MAC_ERR_INVALID;
+  if (C % TC_BK) return MAC_ERR_UNSUPPORTED;                 // 9C = whole k-blocks of mac_linear_tc32_fwd
+  if (!mac_aligned16(x) || !mac_aligned16(cols2)) return MAC_ERR_ALIGN;
+  const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
+  const float scale = keep < 1.f ? 1.f / keep : 1.f;
+  const long long total = (long long)B * H * W * 9 * (C / 8);
+  im2col3x3_split_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(x, reinterpret_cast<__nv_bfloat16*>(cols2), thr,
+                                                                             scale, seed, site, step, B, H, W, C);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ stem: e4m3 inference
 // (tc_gemm_fp8.cuh)
 extern "C" size_t mac_im2col3x3_fp8_workspace_bytes(int B, int H, int W, int C) {
@@ -661,16 +737,21 @@ extern "C" int mac_col2im3x3(const float* dcols, float* dx, float keep, uint64_t
 }
 
 // ------------------------------------------------------------------------------------------------ stem: backward on wgmma
-// One 3x3 convolution layer's backward with its two GEMMs on tensor cores (bf16 operands, fp32 accumulation, fp32
-// element-wise work), M = B*H*W rows, Mp = M rounded up to the 64-row k-block of the weight gradient:
+// One 3x3 convolution layer's backward with its two GEMMs on tensor cores (fp32 accumulation, fp32 element-wise work),
+// M = B*H*W rows, Mp = M rounded up to the 64-row k-block of the weight gradient.  mac_conv3x3_bwd_tc (bf16 operands):
 //   dZ = dy * act'(y)                      -> bf16 dZ [M, Cout] (dgrad A operand), bf16 dZ^T [Cout, Mp], fp32 column partials
 //   colsT = bf16(dropout(x)) patches^T     -> [9C, Mp], the forward's keep-mask (mac_im2col3x3's Philox numbering)
 //   dKernel [9C, Cout] += colsT @ dZ       (tc_wgrad_splitk, K = Mp; the HWIO kernel viewed as [9C, Cout] is its output)
 //   dBias += column sums of dZ             (fixed order: per-64-row-tile partials, then mac_colsum)
 //   dcols [M, 9C] = dZ @ Kernel^T          (mac_linear_tc_fwd with bf16(Kernel) in its own [9C, Cout] layout as the
 //                                           K-major B operand);  dx = col2im(dcols) * mask / keep   (mac_col2im3x3)
-// Columns M..Mp-1 of both transposed operands are written as zeros on every call: the workspace is not assumed zero.
+// mac_conv3x3_bwd_tc32 (SPLIT: split-bf16 operands, see tc3_gemm) is the same schedule on hi | lo operands:
+//   dZ -> [dZ_hi | dZ_lo] [M, 2 Cout] (only when dx is wanted) and [dZ_hi^T | dZ_hi^T | dZ_lo^T] [Cout, 3 Mp];
+//   colsT -> [cols_hi^T | cols_lo^T] [9C, 2 Mp];  dKernel by tc3_wgrad_splitk (one split-K launch over K = 3 Mp);
+//   dcols = mac_linear_tc32_fwd([dZ_hi | dZ_lo], split3_rows(Kernel) [9C, 3 Cout]).
+// Columns M..Mp-1 of every transposed segment are written as zeros on every call: the workspace is not assumed zero.
 namespace mac {
+template <bool SPLIT>
 __global__ void __launch_bounds__(256) conv_dz_pack_kernel(const float* __restrict__ y, const float* __restrict__ dy, int act,
                                                           __nv_bfloat16* __restrict__ dz, __nv_bfloat16* __restrict__ dzT,
                                                           float* __restrict__ bpart, int M, int Mp, int N) {
@@ -689,7 +770,14 @@ __global__ void __launch_bounds__(256) conv_dz_pack_kernel(const float* __restri
       g.y = d.y * act_grad_from_output(act, v.y);
       g.z = d.z * act_grad_from_output(act, v.z);
       g.w = d.w * act_grad_from_output(act, v.w);
-      *reinterpret_cast<uint2*>(dz + o) = make_uint2(pack_bf16(g.x, g.y), pack_bf16(g.z, g.w));
+      if constexpr (!SPLIT) {
+        *reinterpret_cast<uint2*>(dz + o) = make_uint2(pack_bf16(g.x, g.y), pack_bf16(g.z, g.w));
+      } else if (dz) {                                        // [hi | lo] rows: the data gradient's A operand
+        const uint32_t h01 = pack_bf16(g.x, g.y), h23 = pack_bf16(g.z, g.w);
+        __nv_bfloat16* row = dz + (size_t)m * 2 * N + n;
+        *reinterpret_cast<uint2*>(row) = make_uint2(h01, h23);
+        *reinterpret_cast<uint2*>(row + N) = make_uint2(pack_bf16_lo(g.x, g.y, h01), pack_bf16_lo(g.z, g.w, h23));
+      }
     }
     tile[tq * 4 + 0][mm] = g.x;
     tile[tq * 4 + 1][mm] = g.y;
@@ -700,14 +788,24 @@ __global__ void __launch_bounds__(256) conv_dz_pack_kernel(const float* __restri
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int r = warp; r < 64; r += 8) {
     const float a = tile[r][2 * lane], b = tile[r][2 * lane + 1];
-    *reinterpret_cast<uint32_t*>(dzT + (size_t)(n0 + r) * Mp + m0 + 2 * lane) = pack_bf16(a, b);
+    if constexpr (!SPLIT) {
+      *reinterpret_cast<uint32_t*>(dzT + (size_t)(n0 + r) * Mp + m0 + 2 * lane) = pack_bf16(a, b);
+    } else {                                                  // [hi | hi | lo], each Mp wide
+      const uint32_t hw = pack_bf16(a, b);
+      __nv_bfloat16* row = dzT + (size_t)(n0 + r) * 3 * Mp + m0 + 2 * lane;
+      *reinterpret_cast<uint32_t*>(row) = hw;
+      *reinterpret_cast<uint32_t*>(row + Mp) = hw;
+      *reinterpret_cast<uint32_t*>(row + 2 * Mp) = pack_bf16_lo(a, b, hw);
+    }
     const float s = warp_sum(a + b);
     if (lane == 0) bpart[(size_t)blockIdx.y * N + n0 + r] = s;
   }
 }
 
-// colsT[tap*C + c, m] = bf16(dropout(x))[pixel m shifted by tap, c], zero outside the image and for m >= M.  One 64 (k) x
-// 64 (pixel) tile per block; C % 64 == 0, so a tile lies within one tap.  256-byte channel reads, 128-byte row writes.
+// colsT[tap*C + c, m] = bf16(dropout(x))[pixel m shifted by tap, c], zero outside the image and for m >= M; with SPLIT the
+// row is [hi | lo], each Mp wide.  One 64 (k) x 64 (pixel) tile per block; C % 64 == 0, so a tile lies within one tap.
+// 256-byte channel reads, 128-byte row writes.
+template <bool SPLIT>
 __global__ void __launch_bounds__(256) im2col3x3_t_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ colsT,
                                                          uint32_t thresh, float scale, uint64_t seed, int site, int step,
                                                          int B, int H, int W, int C, int Mp) {
@@ -744,45 +842,50 @@ __global__ void __launch_bounds__(256) im2col3x3_t_kernel(const float* __restric
   }
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int r = warp; r < 64; r += 8)
-    *reinterpret_cast<uint32_t*>(colsT + (size_t)(k0 + r) * Mp + m0 + 2 * lane) =
-        pack_bf16(tile[r][2 * lane], tile[r][2 * lane + 1]);
+  for (int r = warp; r < 64; r += 8) {
+    if constexpr (!SPLIT) {
+      *reinterpret_cast<uint32_t*>(colsT + (size_t)(k0 + r) * Mp + m0 + 2 * lane) =
+          pack_bf16(tile[r][2 * lane], tile[r][2 * lane + 1]);
+    } else {
+      const float a = tile[r][2 * lane], b = tile[r][2 * lane + 1];
+      const uint32_t hw = pack_bf16(a, b);
+      __nv_bfloat16* row = colsT + (size_t)(k0 + r) * 2 * Mp + m0 + 2 * lane;
+      *reinterpret_cast<uint32_t*>(row) = hw;
+      *reinterpret_cast<uint32_t*>(row + Mp) = pack_bf16_lo(a, b, hw);
+    }
+  }
 }
 
-// workspace of mac_conv3x3_bwd_tc: 1 KB-aligned slabs behind a 1 KB alignment slack
+// workspace of mac_conv3x3_bwd_tc / _tc32: 1 KB-aligned slabs behind a 1 KB alignment slack.  `split`: the bf16 operands
+// carry 2 (dz rows, colsT) or 3 (dzT, kernel) segments, and the weight gradient contracts over 3 Mp.
 struct ConvBwdLayout {
   size_t dz, dzT, colsT, bpart, wpart, k16, dcols, total;
 };
-inline ConvBwdLayout conv_bwd_layout(int B, int H, int W, int C, int Cout, bool with_dx) {
+inline ConvBwdLayout conv_bwd_layout(int B, int H, int W, int C, int Cout, bool with_dx, bool split) {
   auto al = [](size_t v) { return (v + 1023) & ~(size_t)1023; };
   const size_t M = (size_t)B * H * W, Mp = (M + 63) & ~(size_t)63, K = (size_t)9 * C;
-  // the split-K partials for the slice count the weight gradient will use on this device (tc_wgrad_splitk)
-  const int S = tc_pick_ksplit((int)Mp, (int)(K / TC_BM) * (Cout / TC_BN));
+  const size_t s2 = split ? 2 : 1, s3 = split ? 3 : 1;
+  // the split-K partials for the slice count the weight gradient will use on this device (tc_wgrad_splitk / tc3_wgrad_splitk)
+  const int S = tc_pick_ksplit((int)(s3 * Mp), (int)(K / TC_BM) * (Cout / TC_BN));
   ConvBwdLayout l;
   size_t o = 0;
-  l.dz = o;    o += al(M * Cout * 2);
-  l.dzT = o;   o += al((size_t)Cout * Mp * 2);
-  l.colsT = o; o += al(K * Mp * 2);
+  l.dz = o;    o += (split && !with_dx) ? 0 : al(M * Cout * 2 * s2);
+  l.dzT = o;   o += al((size_t)Cout * Mp * 2 * s3);
+  l.colsT = o; o += al(K * Mp * 2 * s2);
   l.bpart = o; o += al(Mp / 64 * Cout * 4);
   l.wpart = o; o += al((size_t)S * K * Cout * 4);
   l.k16 = l.dcols = o;
   if (with_dx) {
-    o += al(K * Cout * 2);
+    o += al(K * Cout * 2 * s3);
     l.dcols = o; o += al(M * K * 4);
   }
   l.total = o + 1024;
   return l;
 }
-}  // namespace mac
 
-extern "C" size_t mac_conv3x3_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx) {
-  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return 0;
-  return conv_bwd_layout(B, H, W, C, Cout, with_dx != 0).total;
-}
-
-extern "C" int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
-                                  uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
-                                  size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
+static int conv3x3_bwd_wgmma(bool split, const float* x, const float* y, const float* dy, const float* kernel, int act,
+                             float keep, uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
+                      size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x || !y || !dy || !kernel || !dkernel || !dbias || !workspace) return MAC_ERR_INVALID;
   if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0 || !(keep > 0.f && keep <= 1.f)) return MAC_ERR_INVALID;
@@ -791,7 +894,7 @@ extern "C" int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* d
   if (!mac_aligned16(x) || !mac_aligned16(y) || !mac_aligned16(dy) || !mac_aligned16(kernel) || !mac_aligned16(dkernel) ||
       (dx && !mac_aligned16(dx)))
     return MAC_ERR_ALIGN;
-  const ConvBwdLayout l = conv_bwd_layout(B, H, W, C, Cout, dx != nullptr);
+  const ConvBwdLayout l = conv_bwd_layout(B, H, W, C, Cout, dx != nullptr, split);
   if (workspace_bytes < l.total) return MAC_ERR_WORKSPACE;
   if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
   const int M = B * H * W, Mp = (M + 63) & ~63, K = 9 * C;
@@ -801,21 +904,60 @@ extern "C" int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* d
   __nv_bfloat16* colsT = reinterpret_cast<__nv_bfloat16*>(base + l.colsT);
   float* bpart = reinterpret_cast<float*>(base + l.bpart);
   float* wpart = reinterpret_cast<float*>(base + l.wpart);
-  conv_dz_pack_kernel<<<dim3(Cout / 64, Mp / 64), 256, 0, stream>>>(y, dy, act, dz, dzT, bpart, M, Mp, Cout);
-  MAC_LAUNCH_CHECK();
+  const dim3 gz(Cout / 64, Mp / 64), gc(Mp / 64, K / 64);
   const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
   const float scale = keep < 1.f ? 1.f / keep : 1.f;
-  im2col3x3_t_kernel<<<dim3(Mp / 64, K / 64), 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, B, H, W, C, Mp);
+  if (split) {
+    conv_dz_pack_kernel<true><<<gz, 256, 0, stream>>>(y, dy, act, dx ? dz : nullptr, dzT, bpart, M, Mp, Cout);
+    MAC_LAUNCH_CHECK();
+    im2col3x3_t_kernel<true><<<gc, 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, B, H, W, C, Mp);
+  } else {
+    conv_dz_pack_kernel<false><<<gz, 256, 0, stream>>>(y, dy, act, dz, dzT, bpart, M, Mp, Cout);
+    MAC_LAUNCH_CHECK();
+    im2col3x3_t_kernel<false><<<gc, 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, B, H, W, C, Mp);
+  }
   MAC_LAUNCH_CHECK();
   int st = mac_colsum(bpart, dbias, 1, Mp / 64, Cout, 1, stream_);
   if (st != MAC_OK) return st;
-  st = tc_wgrad_splitk(colsT, dzT, dkernel, wpart, K, Cout, Mp, stream);
+  st = split ? tc3_wgrad_splitk(colsT, dzT, dkernel, wpart, K, Cout, Mp, stream)
+             : tc_wgrad_splitk(colsT, dzT, dkernel, wpart, K, Cout, Mp, stream);
   if (st != MAC_OK || !dx) return st;
-  void* k16 = base + l.k16;
+  void* k16 = base + l.k16;                                     // the kernel in its own [9C, Cout] layout: K-major B operand
   float* dcols = reinterpret_cast<float*>(base + l.dcols);
-  st = mac_cast_bf16(kernel, k16, (long long)K * Cout, stream_);
-  if (st != MAC_OK) return st;
-  st = mac_linear_tc_fwd(dz, k16, nullptr, MAC_ACT_NON, dcols, 0, M, Cout, K, stream_);
+  if (split) {
+    st = mac_split3_rows_(kernel, k16, K, Cout, stream_);
+    if (st != MAC_OK) return st;
+    st = mac_linear_tc32_fwd(dz, k16, nullptr, MAC_ACT_NON, dcols, M, Cout, K, stream_);
+  } else {
+    st = mac_cast_bf16(kernel, k16, (long long)K * Cout, stream_);
+    if (st != MAC_OK) return st;
+    st = mac_linear_tc_fwd(dz, k16, nullptr, MAC_ACT_NON, dcols, 0, M, Cout, K, stream_);
+  }
   if (st != MAC_OK) return st;
   return mac_col2im3x3(dcols, dx, keep, seed, site, step, B, H, W, C, stream_);
+}
+}  // namespace mac
+
+extern "C" size_t mac_conv3x3_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx) {
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return 0;
+  return conv_bwd_layout(B, H, W, C, Cout, with_dx != 0, false).total;
+}
+
+extern "C" int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                                  uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
+                                  size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
+  return conv3x3_bwd_wgmma(false, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
+                           B, H, W, C, Cout, stream_);
+}
+
+extern "C" size_t mac_conv3x3_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx) {
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return 0;
+  return conv_bwd_layout(B, H, W, C, Cout, with_dx != 0, true).total;
+}
+
+extern "C" int mac_conv3x3_bwd_tc32(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                                    uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
+                                    size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
+  return conv3x3_bwd_wgmma(true, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
+                           B, H, W, C, Cout, stream_);
 }

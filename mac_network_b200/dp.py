@@ -54,18 +54,20 @@ class DPTrainer(object):
         `stem_prec="bf16"` trains the image stem on tensor cores too (forward `mac_linear_tc_fwd`, backward
         `mac_conv3x3_bwd_tc`; every stem channel count must be a multiple of 128).  `enc_prec="bf16"` trains the question
         encoder's LSTM on tensor cores (`QuestionEncoder(prec="bf16")`; needs ctrlDim = 512, i.e. h = 256 per direction).
-        All are mixed precision: bf16 operands, fp32 accumulation, fp32 master weights / gradients / optimizer state
-        (DESIGN.md section 9)."""
+        `stem_prec="bf16x3"` trains the stem as split-bf16 tensor-core products inside the fp32 parity bar (the stem's
+        counterpart of `prec="tc32"`: `mac_linear_tc32_fwd`, `mac_conv3x3_bwd_tc32`; same channel rule, independent of `prec`
+        and `bwd_tc`).  The others are mixed precision: bf16 operands, fp32 accumulation, fp32 master weights / gradients /
+        optimizer state (DESIGN.md section 9)."""
         from .mac_cell import MACParams, views_of
         from .params import init_params
-        if stem_prec not in ("fp32", "bf16"):
-            raise ValueError("stem_prec must be 'fp32' or 'bf16', got %r" % (stem_prec,))
+        if stem_prec not in ("fp32", "bf16", "bf16x3"):
+            raise ValueError("stem_prec must be 'fp32', 'bf16' or 'bf16x3', got %r" % (stem_prec,))
         if stem_prec != "fp32":
             if stem is None:
                 raise ValueError("stem_prec=%r needs stem=" % (stem_prec,))
             if stem[0] % 128 or cfg.memDim % 128:
-                raise NotImplementedError("stem_prec='bf16' needs the image channels (%d) and memDim (%d) to be multiples of "
-                                          "128 (the wgmma tiles of mac_conv3x3_bwd_tc)" % (stem[0], cfg.memDim))
+                raise NotImplementedError("stem_prec=%r needs the image channels (%d) and memDim (%d) to be multiples of "
+                                          "128 (the wgmma tiles of mac_conv3x3_bwd_tc)" % (stem_prec, stem[0], cfg.memDim))
         if enc_prec not in ("fp32", "bf16"):
             raise ValueError("enc_prec must be 'fp32' or 'bf16', got %r" % (enc_prec,))
         if enc_prec != "fp32":

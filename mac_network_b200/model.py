@@ -38,11 +38,12 @@ class MACnet(object):
         """`vocab`: rows of the question-embedding variable (ids 1..vocab; 0 is padding); `answer_decoder`: optional
         id -> answer string (`answerDict.decodeId`, model.py:699).  `prec`: arithmetic of the evaluation forward; with
         "fp8" the cell's read step runs on e4m3 and the image stem in bf16.  `eval_stem_prec="fp8"` runs the evaluation
-        stem in e4m3 (`Stem(prec="fp8")`) whatever `prec` is; None keeps the stem `prec` implies.  `eval_enc_prec="bf16"` runs
+        stem in e4m3 (`Stem(prec="fp8")`) and `eval_stem_prec="bf16x3"` in split bf16 inside the fp32 parity bar
+        (`Stem(prec="bf16x3")`), whatever `prec` is; None keeps the stem `prec` implies.  `eval_enc_prec="bf16"` runs
         the evaluation question encoder on tensor cores (`QuestionEncoder(prec="bf16")`); None keeps it fp32.  Training is
         unaffected (see `DPTrainer(enc_prec=)`)."""
-        if eval_stem_prec not in (None, "fp8"):
-            raise ValueError("eval_stem_prec must be None or 'fp8', got %r" % (eval_stem_prec,))
+        if eval_stem_prec not in (None, "fp8", "bf16x3"):
+            raise ValueError("eval_stem_prec must be None, 'fp8' or 'bf16x3', got %r" % (eval_stem_prec,))
         if eval_enc_prec not in (None, "bf16"):
             raise ValueError("eval_enc_prec must be None or 'bf16', got %r" % (eval_enc_prec,))
         self.cfg, self.L, self.prec, self.use_ema = cfg, netLength, prec, bool(use_ema)

@@ -7,7 +7,10 @@ GPU formulation: convolution as GEMM.  `mac_im2col3x3` builds the `[B*H*W, 9*C]`
 -- exactly the row-major reshape of the HWIO kernel to `[9*C, Cout]`) with the input dropout fused (the Philox mask is
 indexed by the SOURCE element, so all nine copies of a pixel share its mask), in bf16 for the wgmma GEMM
 (`mac_linear_tc_fwd`, ELU epilogue) or fp32 for the parity GEMM (`mac_linear_fwd`).  `prec="fp8"` is an inference-only
-forward in e4m3: `mac_im2col3x3_fp8` (per-row scales, no dropout) and `mac_linear_fp8_fwd` (csrc/tc_gemm_fp8.cuh)."""
+forward in e4m3: `mac_im2col3x3_fp8` (per-row scales, no dropout) and `mac_linear_fp8_fwd` (csrc/tc_gemm_fp8.cuh).
+`prec="bf16x3"` is the parity arithmetic on tensor cores, for inference and training: every fp32 operand as hi + lo bf16
+halves and three bf16 products per fp32 product (`mac_im2col3x3_split`, `mac_linear_tc32_fwd`, `mac_conv3x3_bwd_tc32`;
+the split-bf16 scheme the cell calls "tc32", DESIGN.md section 9 item 6)."""
 import collections
 import ctypes
 
@@ -59,11 +62,11 @@ class Stem(object):
         self.device = dev
 
     def _weights(self, i):
-        """(W, packed): the fp32 [9*Cin, Cout] view and, for bf16, the bf16 [Cout, 9*Cin] pack; for fp8, the e4m3
-        [Cout, 9*Cin] pack and its per-column scales as a pair."""
+        """(W, packed): the fp32 [9*Cin, Cout] view and, for bf16, the bf16 [Cout, 9*Cin] pack; for bf16x3, the split pack
+        [Cout, 3*9*Cin] = [hi | hi | lo]; for fp8, the e4m3 [Cout, 9*Cin] pack and its per-column scales as a pair."""
         K = self.p["stem/cnnLayercnn_%d/kernels/kernel" % i]
         W = K.reshape(-1, K.shape[3])                       # [9*Cin, Cout], row-major view of the HWIO kernel
-        if self.prec in ("bf16", "fp8"):
+        if self.prec in ("bf16", "bf16x3", "fp8"):
             v = self._version_fn() if self._version_fn is not None else None
             if v != self._packed_version:
                 self._packed.clear()
@@ -72,6 +75,11 @@ class Stem(object):
                 if self.prec == "bf16":
                     Wt = torch.empty((W.shape[1], W.shape[0]), dtype=torch.bfloat16, device=W.device)
                     check(self.lib.mac_pack_weight_bf16(ptr(W), ptr(Wt), W.shape[0], W.shape[1], stream_ptr()), "pack")
+                    self._packed[i] = Wt
+                elif self.prec == "bf16x3":
+                    Wt = torch.empty((W.shape[1], 3 * W.shape[0]), dtype=torch.bfloat16, device=W.device)
+                    check(self.lib.mac_pack_weight_split3(ptr(W), ptr(Wt), W.shape[0], W.shape[1], stream_ptr()),
+                          "mac_pack_weight_split3")
                     self._packed[i] = Wt
                 else:
                     Wt = torch.empty((W.shape[1], W.shape[0]), dtype=torch.uint8, device=W.device)
@@ -110,18 +118,21 @@ class Stem(object):
             x = y.view(B, H, Wd, Nout)
         return x.view(B, H * Wd, x.shape[3])
 
-    def _check_trainable(self, in_dim):
-        """Training (forward with save_for_backward + backward) runs in fp32, or in bf16 on tensor cores
-        (`mac_conv3x3_bwd_tc`, DESIGN.md section 9 item 2), whose GEMM tiles need every layer's input and output channel
-        counts to be multiples of 128.  Raises before any launch."""
-        if self.prec == "fp32":
-            return
-        if self.prec != "bf16":
-            raise NotImplementedError("stem training runs in fp32 or bf16, not %r (DESIGN.md section 9)" % self.prec)
+    def _check_tiles(self, in_dim, what):
         dims = [in_dim] + [int(self.p["stem/cnnLayercnn_%d/kernels/kernel" % i].shape[3]) for i in range(self.nlayers)]
         if any(c % 128 for c in dims):
-            raise NotImplementedError("bf16 stem training needs channel counts that are multiples of 128 (the wgmma tiles of "
-                                      "mac_conv3x3_bwd_tc), got %s; use prec='fp32' (DESIGN.md section 9)" % dims)
+            raise NotImplementedError("%s needs channel counts that are multiples of 128 (the wgmma tiles of "
+                                      "mac_conv3x3_bwd_tc), got %s; use prec='fp32' (DESIGN.md section 9)" % (what, dims))
+
+    def _check_trainable(self, in_dim):
+        """Training (forward with save_for_backward + backward) runs in fp32, or on tensor cores in bf16
+        (`mac_conv3x3_bwd_tc`, DESIGN.md section 9 item 2) or split bf16 ("bf16x3", `mac_conv3x3_bwd_tc32`, item 6), whose
+        GEMM tiles need every layer's input and output channel counts to be multiples of 128.  Raises before any launch."""
+        if self.prec == "fp32":
+            return
+        if self.prec not in ("bf16", "bf16x3"):
+            raise NotImplementedError("stem training runs in fp32, bf16 or bf16x3, not %r (DESIGN.md section 9)" % self.prec)
+        self._check_tiles(in_dim, "%s stem training" % self.prec)
 
     def forward(self, images, keep=1.0, step=0, save_for_backward=False):
         """images: [B,H,W,C] fp32 NHWC (the reference transposes the NCHW h5 features first, model.py:~770).
@@ -135,6 +146,8 @@ class Stem(object):
         if self.prec == "fp8":
             self._check_fp8(C, keep)
             return self._forward_fp8(x, act)
+        if self.prec == "bf16x3":
+            self._check_tiles(C, "the bf16x3 stem")
         for i in range(self.nlayers):
             if save_for_backward:
                 self._saved["xs"].append(x)
@@ -143,10 +156,20 @@ class Stem(object):
             C = x.shape[3]
             M, K, Nout = B * H * Wd, 9 * C, W.shape[1]
             bf16 = self.prec == "bf16"
+            y = torch.empty((M, Nout), dtype=torch.float32, device=self.device)
+            if self.prec == "bf16x3":
+                cols = torch.empty((M, 2 * K), dtype=torch.bfloat16, device=self.device)          # [hi | lo]
+                check(self.lib.mac_im2col3x3_split(ptr(x), ptr(cols), float(keep), self.seed, SITE_STEM + i, step, B, H, Wd,
+                                                   C, stream_ptr()), "mac_im2col3x3_split")
+                check(self.lib.mac_linear_tc32_fwd(ptr(cols), ptr(Wt), ptr(b), act, ptr(y), M, K, Nout, stream_ptr()),
+                      "mac_linear_tc32_fwd")
+                if save_for_backward:
+                    self._saved["ys"].append(y)
+                x = y.view(B, H, Wd, Nout)
+                continue
             cols = torch.empty((M, K), dtype=torch.bfloat16 if bf16 else torch.float32, device=self.device)
             check(self.lib.mac_im2col3x3(ptr(x), ptr(cols), 1 if bf16 else 0, float(keep), self.seed, SITE_STEM + i, step,
                                          B, H, Wd, C, stream_ptr()), "mac_im2col3x3")
-            y = torch.empty((M, Nout), dtype=torch.float32, device=self.device)
             if bf16:
                 check(self.lib.mac_linear_tc_fwd(ptr(cols), ptr(Wt), ptr(b), act, ptr(y), 0, M, K, Nout, stream_ptr()),
                       "mac_linear_tc_fwd")
@@ -166,7 +189,8 @@ class Stem(object):
         parameter).  Per layer, last to first:  dZ = dY * act'(Y);  dKernel += cols^T @ dZ, dBias += colsum(dZ)
         (`mac_linear_bwd` on the re-generated patch matrix);  dcols = dZ @ Kernel^T;  dX = col2im(dcols) * dropout mask.
         The gradient w.r.t. the images (and with it layer 0's largest GEMM) is skipped unless asked for.
-        With prec="bf16" each layer is one `mac_conv3x3_bwd_tc` call: the same steps with both GEMMs on tensor cores."""
+        With prec="bf16" each layer is one `mac_conv3x3_bwd_tc` call: the same steps with both GEMMs on tensor cores; with
+        prec="bf16x3" one `mac_conv3x3_bwd_tc32` call: the same again on split-bf16 operands."""
         sv = getattr(self, "_saved", None)
         if sv is None:
             raise RuntimeError("forward(save_for_backward=True) must run first")
@@ -179,14 +203,15 @@ class Stem(object):
             C, Nout = x.shape[3], y.shape[1]
             K = 9 * C
             W, _ = self._weights(i)
-            if self.prec == "bf16":
+            if self.prec in ("bf16", "bf16x3"):
+                name = "mac_conv3x3_bwd_tc" if self.prec == "bf16" else "mac_conv3x3_bwd_tc32"
                 dx = torch.empty_like(x) if (need_d_images or i > 0) else None
-                nbytes = int(self.lib.mac_conv3x3_bwd_tc_workspace_bytes(B, H, Wd, C, Nout, int(dx is not None)))
+                nbytes = int(getattr(self.lib, name + "_workspace_bytes")(B, H, Wd, C, Nout, int(dx is not None)))
                 ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-                check(self.lib.mac_conv3x3_bwd_tc(ptr(x), ptr(y), ptr(dy), ptr(W), sv["act"], sv["keep"], self.seed,
-                                                  SITE_STEM + i, sv["step"], ptr(grads["stem/cnnLayercnn_%d/kernels/kernel" % i]),
-                                                  ptr(grads["stem/cnnLayercnn_%d/biases/bias" % i]), ptr(dx), ptr(ws), nbytes,
-                                                  B, H, Wd, C, Nout, stream_ptr()), "mac_conv3x3_bwd_tc")
+                check(getattr(self.lib, name)(ptr(x), ptr(y), ptr(dy), ptr(W), sv["act"], sv["keep"], self.seed,
+                                              SITE_STEM + i, sv["step"], ptr(grads["stem/cnnLayercnn_%d/kernels/kernel" % i]),
+                                              ptr(grads["stem/cnnLayercnn_%d/biases/bias" % i]), ptr(dx), ptr(ws), nbytes,
+                                              B, H, Wd, C, Nout, stream_ptr()), name)
                 if dx is not None:
                     dy = dx.view(M, C)
                 continue
