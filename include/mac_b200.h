@@ -496,13 +496,14 @@ size_t mac_conv3x3_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout
  *   receives the undropped words (`questionWords`).  E % 4 == 0.
  * mac_embed_bwd: d_emb[v,:] += sum_{(b,s): idx == v+1} d_out[b,s,:] * keep-mask / keep, positions in a fixed order.
  * mac_lstm_fwd: tf.nn.(bidirectional_)dynamic_rnn over BasicLSTMCell (gate order i,j,f,o; TF kernel [E+h, 4h]) with
- *   sequence_length = lengths.  The caller supplies the hoisted input projection gx_dir [B*S, 4h] = X @ kernel[0:E] + bias
+ *   sequence_length = lengths, each clamped to [0, S] (a length > S acts as S, one < 0 as 0: the kernels never address
+ *   a row outside [b*S, b*S + S)).  The caller supplies the hoisted input projection gx_dir [B*S, 4h] = X @ kernel[0:E] + bias
  *   (mac_linear_fwd) and Wh_dir = kernel + E*4h (the recurrent rows).  Direction 1 walks t = len-1 .. 0 (reverse_sequence).
  *   out_seq [B,S,ndir*h] = [fw | bw] outputs, zero for t >= len; vecq [B,ndir*h] (may be NULL) = the final h of each
  *   direction (ops.py:893-898).  save_gates [ndir,B*S,4h], save_c / save_hprev [ndir,B*S,h] (all or none NULL) keep what
  *   the backward needs, indexed by time; save_hprev is zero for t >= len.  Issues S launches (one per step, both directions)
  *   on `stream`.
- * mac_lstm_bwd: BPTT.  dG_dir [B*S, 4h] receives the gradient w.r.t. the pre-activation gates; parameter and input
+ * mac_lstm_bwd: BPTT, with mac_lstm_fwd's clamped lengths.  dG_dir [B*S, 4h] receives the gradient w.r.t. the pre-activation gates; parameter and input
  *   gradients are then GEMMs over all steps: mac_linear_bwd(x_segs = [dropout(X), save_hprev_dir], dy = dG_dir).
  * --------------------------------------------------------------------------------------------- */
 int mac_embed_fwd(const float* emb, const int32_t* idx, float keep, uint64_t seed, int site, int step, float* out_raw,
@@ -519,7 +520,7 @@ int mac_lstm_bwd(const float* Wh_fw, const float* Wh_bw, const int32_t* lengths,
 /* The question encoder on wgmma tensor cores (csrc/encoder_tc.cuh; QuestionEncoder(prec="bf16")): bf16 matrix-product
  * operands, fp32 accumulation; the cell state, gate non-linearities, outputs, saved tensors and element-wise backward steps
  * are fp32.  Ep = E rounded up to a multiple of 128; the bf16 operands carry zero columns E..Ep-1.  h must be 256
- * (MAC_ERR_UNSUPPORTED otherwise).  All checks precede any launch.
+ * (MAC_ERR_UNSUPPORTED otherwise).  Lengths are clamped to [0, S] as in mac_lstm_fwd.  All checks precede any launch.
  * mac_embed_fwd_tc: mac_embed_fwd's out_raw (required) and x_bf16 [B*S, Ep] = bf16(dropout(words)) with the same keep-mask.
  * mac_pack_weight_bf16_kpad: fp32 W[K, n_out] -> bf16 Wt[n_out, Kp] with zero columns K..Kp-1 (Kp >= K); with W = kernel[0:E]
  *   and Kp = Ep it is the B operand of gx_dir = mac_linear_tc_fwd(x_bf16, Wt, bias_dir, NON, gx_dir, 0, B*S, Ep, 4h).

@@ -33,6 +33,11 @@ static inline int mac_num_sms() {
 
 namespace mac {
 
+// the question length of batch row b as the LSTM kernels use it: clamped to [0, S], as mac_control_attend_fwd clamps it.  A
+// length outside that range is a data bug; unclamped, the backward direction's time index len-1-s would address rows of the
+// next sample (past the buffer's end for the last one).
+__device__ __forceinline__ int seq_len(const int32_t* lengths, int b, int S) { return min(max(lengths[b], 0), S); }
+
 // ------------------------------------------------------------------ activations (ops.py:161-187)
 __device__ __forceinline__ float elu_f(float x) { return x > 0.f ? x : expm1f(x); }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }

@@ -142,7 +142,7 @@ __global__ void __launch_bounds__(LS_THREADS) lstm_step_kernel(const LstmFwdPara
   for (int r = 0; r < 2; ++r) {
     const int lr = bg + 32 * r, b = b_base + lr;
     if (b >= p.B) continue;
-    const int len = p.lengths[b];
+    const int len = seq_len(p.lengths, b, p.S);
     const bool live = p.s < len;
     const float hold = hs[lr * hp + col];
     const size_t sidx = ((size_t)dir * p.B + b) * h + col;
@@ -205,7 +205,7 @@ static __global__ void __launch_bounds__(LP_THREADS) lstm_seq_kernel(const LstmF
   for (int e = tid; e < 2 * LP_RB * hp; e += LP_THREADS) hbuf[e] = 0.f;     // cell.zero_state
   cluster.sync();                                // every CTA's buffers are zeroed before any remote store can land
   const bool valid = b < p.B;
-  const int len = valid ? p.lengths[b] : 0;
+  const int len = valid ? seq_len(p.lengths, b, p.S) : 0;
   const int W2 = p.ndir * h;
   const float* __restrict__ gxd = dir ? p.gx[1] : p.gx[0];
   const size_t dbase = (size_t)dir * p.B * p.S;
@@ -304,7 +304,7 @@ __global__ void __launch_bounds__(LS_THREADS) lstm_step_bwd_kernel(const LstmBwd
         const int b = b_base + r;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (b < p.B && kc + k4 * 4 < G) {
-          const int len = p.lengths[b];
+          const int len = seq_len(p.lengths, b, p.S);
           if (p.s + 1 < len) {         // the row was live at step s+1: its gate gradients sit at that step's time index
             const int t1 = dir ? (len - 2 - p.s) : (p.s + 1);
             v = *(reinterpret_cast<const float4*>(dGd + ((size_t)b * p.S + t1) * G + kc) + k4);
@@ -335,7 +335,7 @@ __global__ void __launch_bounds__(LS_THREADS) lstm_step_bwd_kernel(const LstmBwd
   for (int r = 0; r < 2; ++r) {
     const int b = b_base + bg + 32 * r;
     if (b >= p.B) continue;
-    const int len = p.lengths[b];
+    const int len = seq_len(p.lengths, b, p.S);
     if (p.s >= len) continue;          // past the end: state was carried through, nothing to differentiate
     const int t = dir ? (len - 1 - p.s) : p.s;
     const size_t row = (size_t)b * p.S + t;

@@ -130,7 +130,7 @@ __global__ void __launch_bounds__(ET_THREADS, 1) lstm_fwd_tc_kernel(const LstmTc
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     brow[hh] = b_base + 16 * warp + (lane >> 2) + 8 * hh;
-    len[hh] = brow[hh] < p.B ? p.lengths[brow[hh]] : 0;
+    len[hh] = brow[hh] < p.B ? seq_len(p.lengths, brow[hh], p.S) : 0;
   }
   const float* __restrict__ gxd = (dir ? p.gx[1] : p.gx[0]);
   const size_t dbase = (size_t)dir * p.B * p.S;
@@ -289,7 +289,7 @@ __global__ void __launch_bounds__(ET_THREADS, 1) lstm_bwd_tc_kernel(const LstmTc
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     brow[hh] = b_base + 16 * warp + (lane >> 2) + 8 * hh;
-    len[hh] = brow[hh] < p.B ? p.lengths[brow[hh]] : 0;
+    len[hh] = brow[hh] < p.B ? seq_len(p.lengths, brow[hh], p.S) : 0;
   }
   float dcc[2][4][2];
 #pragma unroll

@@ -170,7 +170,8 @@ class QuestionEncoder(object):
 
     # ------------------------------------------------------------------ forward
     def forward(self, qIndices, questionLengths, step=0, save_for_backward=False):
-        """qIndices int32 [B,S] (0 = padding), questionLengths int32 [B] (1 <= len <= S).
+        """qIndices int32 [B,S] (0 = padding), questionLengths int32 [B] (1 <= len <= S; the kernels clamp a length to
+        [0, S], so one > S acts as S and one < 0 as 0, and neither indexes outside the [B, S] buffers).
         Returns (questionWords [B,S,E], questionCntxWords [B,S,D], vecQuestions [B,D])."""
         if not (qIndices.is_cuda and qIndices.dtype == torch.int32 and qIndices.is_contiguous()):
             raise ValueError("qIndices must be a contiguous CUDA int32 tensor")
