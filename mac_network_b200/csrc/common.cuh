@@ -74,7 +74,8 @@ __device__ __forceinline__ float warp_max(float v) {
 // ------------------------------------------------------------------ Philox4x32-10 (counter-based dropout RNG)
 // counter = (elem/4 lo, elem/4 hi, site, step), key = seed.  u = (x >> 8) * 2^-24 in [0,1).
 // keep-mask = [u >= 1 - keep]  (== floor(keep + u), ops.py:1054-1059 / tf.nn.dropout), evaluated on the 24-bit
-// integer so that fp32 and the fp64 oracle agree bit-for-bit.
+// integer so that fp32 and the fp64 oracle agree bit-for-bit -- given the same keep: the kernels take keep as a float, so
+// the oracle's keep is float32(keep) (with the fp64 keep 0.85 the element with u = 1 - float32(0.85) differs).
 struct Philox4 { uint32_t x, y, z, w; };
 __host__ __device__ __forceinline__ uint32_t mulhi32(uint32_t a, uint32_t b) {
 #ifdef __CUDA_ARCH__
