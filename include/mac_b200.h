@@ -430,6 +430,11 @@ size_t mac_optimizer_workspace_bytes(void);
  * --------------------------------------------------------------------------------------------- */
 int mac_softmax_xent(const float* logits, const int32_t* labels, float* losses, float* dlogits, float scale,
                      int B, int A, mac_stream_t stream);
+/* Answers without labels (addPredOp, model.py:603-612): per row of logits [B, A], the k largest logits' answer ids [B, k]
+ * (descending; equal logits in ascending id order, so ids[:, 0] is the argmax prediction) and their softmax probabilities
+ * probs [B, k] (max-subtracted, fp32).  One warp per row.  1 <= k <= min(8, A), else MAC_ERR_INVALID before any launch.  A
+ * row that holds NaN gives id -1 and probability NaN where no comparable element is left. */
+int mac_answer_topk(const float* logits, int B, int A, int k, int32_t* ids, float* probs, mac_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Image stem ("next" row, model.py:165-204, ops.py:380-438): convolution as GEMM.
@@ -438,6 +443,16 @@ int mac_softmax_xent(const float* logits, const int32_t* labels, float* losses, 
  * --------------------------------------------------------------------------------------------- */
 int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float keep, uint64_t seed, int site, int step,
                   int B, int H, int W, int C, mac_stream_t stream);
+/* Layer-0 ingest from channel-major features (csrc/ingest.cuh; Stem.forward_nchw): x_nchw [B, C, H, W] as the feature
+ * extractor wrote it, fp32 or (x_bf16 != 0) bf16, read once.
+ *   MAC_INGEST_NHWC_F32:   out = fp32 [B, H, W, C], the permuted tensor (bf16 input is widened).
+ *   MAC_INGEST_PATCH_BF16: out = bf16 [B*H*W, 9*C], bit for bit the patch matrix mac_im2col3x3(cols_bf16 = 1, keep = 1)
+ *                          makes of the permuted tensor (fp32 input rounds to nearest even; bf16 input is moved).
+ * One CTA per (sample, 64-channel slab): C % 64 == 0, and the slab with its transposed tile must fit one SM's shared memory
+ * (227 KB less the kernel's 128 static bytes: H*W <= 440 for fp32 -> NHWC, 580 for fp32 -> patches and bf16 -> NHWC, 854 for
+ * bf16 -> patches), else MAC_ERR_UNSUPPORTED; B <= 65535.  All checks precede any launch. */
+enum { MAC_INGEST_NHWC_F32 = 0, MAC_INGEST_PATCH_BF16 = 1 };
+int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mode, int B, int C, int H, int W, mac_stream_t stream);
 /* Inference stem layer in e4m3 (csrc/tc_gemm_fp8.cuh; Stem(prec="fp8")), no dropout.  All scales fp32; e4m3 rounds to nearest
  * even and saturates at +-448.
  * mac_im2col3x3_fp8: the patch matrix of mac_im2col3x3 (same tap-major, channel-fastest layout) as e4m3 cols_e4m3 [M, 9C],

@@ -1,0 +1,123 @@
+// Layer-0 ingest of the image stem from channel-major features: [B, C, H, W] (fp32 or bf16, as the feature extractor wrote
+// them) -> either the fp32 NHWC tensor Stem.forward takes, or directly the bf16 patch matrix of mac_im2col3x3
+// ([B*H*W, 9*C], tap-major, channel fastest, zero rows outside the image, no dropout), so that the bf16 stem never makes the
+// NHWC copy.  The input is read from HBM once and the output written once.
+//
+// One CTA owns (sample, 64-channel slab).  The slab is one contiguous run of 64*H*W elements in NCHW, brought into shared
+// memory by ONE 1-D bulk copy (cp.async.bulk + mbarrier; 16-byte aligned for any H*W because 64 elements are >= 128 bytes).
+// A bulk copy cannot pad the rows it lands, and a channel-major slab read across channels at a fixed pixel strides by H*W
+// words -- 196 at 14x14, four banks apart, an 8-way conflict for the 16-byte vectors the output wants.  So the slab is
+// transposed inside shared memory first: lanes run along the pixels (conflict-free reads of the landed slab), each thread
+// packs one 16-byte vector of consecutive channels and stores it to a pixel-major tile whose row stride is 64 channels + 16
+// bytes (a quarter warp's eight 16-byte stores then cover all 32 banks).  The write-out reads that tile as 16-byte vectors
+// (eight or sixteen consecutive lanes = one pixel's 128 or 256 contiguous bytes) and stores 128 contiguous bytes per pixel and
+// tap (patch mode) or 256 per pixel (NHWC mode).
+#pragma once
+#include "common.cuh"
+
+namespace mac {
+
+constexpr int ING_CS = 64;          // channels per CTA
+constexpr int ING_THREADS = 256;
+constexpr size_t ING_STATIC_SMEM = 128;   // the mbarrier, padded to the dynamic tile's alignment (-Xptxas -v)
+
+template <typename IT, bool PATCH>
+struct IngestShape {
+  static constexpr int OSZ = PATCH ? 2 : 4;                  // bytes per output element (bf16 patches / fp32 NHWC)
+  static constexpr int V = 16 / OSZ;                         // channels per 16-byte vector
+  static constexpr int G = ING_CS / V;                       // vectors per pixel
+  static constexpr int TROW = ING_CS * OSZ + 16;             // padded row of the pixel-major tile, bytes
+  __host__ __device__ static size_t in_bytes(int HW) { return (size_t)ING_CS * HW * sizeof(IT); }
+  __host__ __device__ static size_t smem_bytes(int HW) { return in_bytes(HW) + (size_t)HW * TROW; }
+};
+
+__device__ __forceinline__ uint32_t ingest_pair(float a, float b) {          // the rounding of mac_im2col3x3(cols_bf16 = 1)
+  __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&p);
+}
+__device__ __forceinline__ uint32_t ingest_pair(__nv_bfloat16 a, __nv_bfloat16 b) {  // bf16 in, bf16 out: a move
+  return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
+}
+__device__ __forceinline__ float ingest_f32(float a) { return a; }
+__device__ __forceinline__ float ingest_f32(__nv_bfloat16 a) { return __bfloat162float(a); }
+
+template <typename IT, bool PATCH>
+__global__ void __launch_bounds__(ING_THREADS) ingest_nchw_kernel(const IT* __restrict__ x, void* __restrict__ out, int C,
+                                                                  int H, int W) {
+  using SH = IngestShape<IT, PATCH>;
+  extern __shared__ __align__(128) unsigned char ing_smem[];
+  __shared__ uint64_t bar;
+  const int HW = H * W, tid = threadIdx.x, b = blockIdx.y, c0 = blockIdx.x * ING_CS;
+  const IT* s_in = reinterpret_cast<const IT*>(ing_smem);                    // [64][HW] as it lies in NCHW
+  unsigned char* s_t = ing_smem + SH::in_bytes(HW);                          // [HW][TROW bytes], pixel-major
+  if (tid == 0) {
+    mbar_init(&bar, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const uint32_t bytes = (uint32_t)SH::in_bytes(HW);
+    mbar_expect_tx(&bar, bytes);
+    bulk_g2s(ing_smem, x + ((size_t)b * C + c0) * HW, bytes, &bar);
+  }
+  mbar_wait(&bar, 0);
+  // transpose: one 16-byte vector of V consecutive channels per (vector g, pixel p); lanes along p
+  for (int i = tid; i < SH::G * HW; i += ING_THREADS) {
+    const int g = i / HW, p = i - g * HW;
+    const IT* src = s_in + (size_t)(g * SH::V) * HW + p;
+    uint4 q;
+    if constexpr (PATCH) {
+      q.x = ingest_pair(src[0], src[HW]);
+      q.y = ingest_pair(src[2 * HW], src[3 * HW]);
+      q.z = ingest_pair(src[4 * HW], src[5 * HW]);
+      q.w = ingest_pair(src[6 * HW], src[7 * HW]);
+    } else {
+      q.x = __float_as_uint(ingest_f32(src[0]));
+      q.y = __float_as_uint(ingest_f32(src[HW]));
+      q.z = __float_as_uint(ingest_f32(src[2 * HW]));
+      q.w = __float_as_uint(ingest_f32(src[3 * HW]));
+    }
+    *reinterpret_cast<uint4*>(s_t + (size_t)p * SH::TROW + g * 16) = q;
+  }
+  __syncthreads();
+  if constexpr (PATCH) {
+    // cols[(b,h,w), tap*C + c] = x[b, c, h + tap/3 - 1, w + tap%3 - 1], zero outside the image
+    __nv_bfloat16* cols = reinterpret_cast<__nv_bfloat16*>(out);
+    for (int i = tid; i < HW * 9 * SH::G; i += ING_THREADS) {
+      const int g = i % SH::G, r = i / SH::G;
+      const int tap = r % 9, pix = r / 9;
+      const int h = pix / W, w = pix - h * W;
+      const int hs = h + tap / 3 - 1, wsrc = w + tap % 3 - 1;
+      uint4 v = make_uint4(0u, 0u, 0u, 0u);
+      if (hs >= 0 && hs < H && wsrc >= 0 && wsrc < W)
+        v = *reinterpret_cast<const uint4*>(s_t + (size_t)(hs * W + wsrc) * SH::TROW + g * 16);
+      *reinterpret_cast<uint4*>(cols + (((size_t)b * HW + pix) * 9 + tap) * C + c0 + g * SH::V) = v;
+    }
+  } else {
+    float* y = reinterpret_cast<float*>(out);
+    for (int i = tid; i < HW * SH::G; i += ING_THREADS) {
+      const int g = i % SH::G, pix = i / SH::G;
+      const uint4 v = *reinterpret_cast<const uint4*>(s_t + (size_t)pix * SH::TROW + g * 16);
+      *reinterpret_cast<uint4*>(y + ((size_t)b * HW + pix) * C + c0 + g * SH::V) = v;
+    }
+  }
+}
+
+template <typename IT, bool PATCH>
+static int ingest_nchw_launch(const void* x, void* out, int B, int C, int H, int W, cudaStream_t stream) {
+  using SH = IngestShape<IT, PATCH>;
+  const size_t smem = SH::smem_bytes(H * W);
+  auto kern = ingest_nchw_kernel<IT, PATCH>;
+  MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kern<<<dim3(C / ING_CS, B), ING_THREADS, smem, stream>>>(reinterpret_cast<const IT*>(x), out, C, H, W);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+// shared memory one CTA needs; the entry point refuses shapes beyond one SM's 227 KB or the mbarrier's tx-count range
+static inline size_t ingest_smem_bytes(int x_bf16, int mode, int HW) {
+  if (x_bf16) return mode ? IngestShape<__nv_bfloat16, true>::smem_bytes(HW) : IngestShape<__nv_bfloat16, false>::smem_bytes(HW);
+  return mode ? IngestShape<float, true>::smem_bytes(HW) : IngestShape<float, false>::smem_bytes(HW);
+}
+
+}  // namespace mac

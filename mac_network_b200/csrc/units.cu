@@ -9,6 +9,7 @@
 #include "skinny_tc.cuh"
 #include "encoder_tc.cuh"
 #include "linear_tc.cuh"
+#include "ingest.cuh"
 
 using namespace mac;
 
@@ -527,6 +528,58 @@ extern "C" int mac_softmax_xent(const float* logits, const int32_t* labels, floa
   return MAC_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ answers without labels
+// Per row: softmax probabilities (max-subtracted, fp32) and the k largest logits with their answer ids, ties to the lower id
+// (torch.argmax / tf.argmax order, model.py:603-612).  One warp per row; round r picks the largest element that sorts after
+// round r-1's pick in (logit descending, id ascending) order, so nothing is marked and the row is only read.
+namespace mac {
+__global__ void __launch_bounds__(256) answer_topk_kernel(const float* __restrict__ logits, int B, int A, int k,
+                                                         int32_t* __restrict__ ids, float* __restrict__ probs) {
+  const int b = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (b >= B) return;
+  const float* row = logits + (size_t)b * A;
+  float mx = -INFINITY;
+  for (int a = lane; a < A; a += 32) mx = fmaxf(mx, row[a]);
+  mx = warp_max(mx);
+  float sum = 0.f;
+  for (int a = lane; a < A; a += 32) sum += expf(row[a] - mx);
+  sum = warp_sum(sum);
+  const float inv = 1.f / sum;
+  float pv = INFINITY;
+  int pi = -1;
+  for (int r = 0; r < k; ++r) {
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;                                     // no candidate yet (a row of NaNs never finds one: id -1)
+    for (int a = lane; a < A; a += 32) {
+      const float v = row[a];
+      const bool after_prev = v < pv || (v == pv && a > pi);
+      if (after_prev && (bi == 0x7fffffff || v > bv)) { bv = v; bi = a; }      // ascending a: the first of equals stays
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (oi != 0x7fffffff && (bi == 0x7fffffff || ov > bv || (ov == bv && oi < bi))) { bv = ov; bi = oi; }
+    }
+    if (lane == 0) {
+      ids[(size_t)b * k + r] = bi == 0x7fffffff ? -1 : bi;
+      probs[(size_t)b * k + r] = bi == 0x7fffffff ? __int_as_float(0x7fc00000) : expf(bv - mx) * inv;
+    }
+    pv = bv;
+    pi = bi;
+  }
+}
+}  // namespace mac
+
+extern "C" int mac_answer_topk(const float* logits, int B, int A, int k, int32_t* ids, float* probs, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!logits || !ids || !probs || B <= 0 || A <= 0) return MAC_ERR_INVALID;
+  if (k < 1 || k > 8 || k > A) return MAC_ERR_INVALID;
+  answer_topk_kernel<<<(B + 7) / 8, 256, 0, stream>>>(logits, B, A, k, ids, probs);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ stem: im2col
 // cols[(b,h,w), (kh*3+kw)*C + c] = dropout(x)[b, h+kh-1, w+kw-1, c]  (zero outside the image: SAME padding, ops.py:395)
 // The keep-mask is a function of the SOURCE element's flat index, so every copy of a pixel carries the same mask
@@ -588,6 +641,24 @@ extern "C" int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float ke
                                                      W, C);
   MAC_LAUNCH_CHECK();
   return MAC_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ stem: ingest from NCHW
+extern "C" int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mode, int B, int C, int H, int W,
+                               mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x_nchw || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0) return MAC_ERR_INVALID;
+  if (!mac_aligned16(x_nchw) || !mac_aligned16(out)) return MAC_ERR_ALIGN;
+  if ((C % ING_CS) || (mode != MAC_INGEST_NHWC_F32 && mode != MAC_INGEST_PATCH_BF16)) return MAC_ERR_UNSUPPORTED;
+  // one slab, its transposed tile and the kernel's static shared memory in one SM's 227 KB, the slab inside the mbarrier's
+  // tx-count range; gridDim.y
+  if ((long long)H * W > 4096 || ingest_smem_bytes(x_bf16, mode, H * W) + ING_STATIC_SMEM > 227 * 1024 || B > 65535)
+    return MAC_ERR_UNSUPPORTED;
+  if (x_bf16)
+    return mode == MAC_INGEST_PATCH_BF16 ? ingest_nchw_launch<__nv_bfloat16, true>(x_nchw, out, B, C, H, W, stream)
+                                         : ingest_nchw_launch<__nv_bfloat16, false>(x_nchw, out, B, C, H, W, stream);
+  return mode == MAC_INGEST_PATCH_BF16 ? ingest_nchw_launch<float, true>(x_nchw, out, B, C, H, W, stream)
+                                       : ingest_nchw_launch<float, false>(x_nchw, out, B, C, H, W, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ stem: split-bf16 patches

@@ -246,6 +246,18 @@ class MACCell(object):
                                         and float(readDropout) >= 1.0):
             raise NotImplementedError("a bf16 knowledge base is accepted by the bf16 and fp8 inference paths only")
 
+    def rebind(self, vecQuestions, questionWords, questionCntxWords, knowledgeBase):
+        """Point the cell at another batch's input tensors of the same shapes and types (the next `mac_network` reads
+        them): what a caller whose encoder and stem produce fresh tensors on every pass needs to keep one cell -- its scratch
+        workspaces and cached weight structures; `zero_state` still allocates the histories and attention buffers of each
+        pass -- across passes (serving.ModelPipeline)."""
+        for new, old in ((vecQuestions, self.vecQuestions), (questionWords, self.questionWords),
+                         (questionCntxWords, self.questionCntxWords), (knowledgeBase, self.knowledgeBase)):
+            if not (new.shape == old.shape and new.dtype == old.dtype and new.device == old.device and new.is_contiguous()):
+                raise ValueError("rebind needs contiguous tensors of the shapes and types the cell was built over")
+        self.vecQuestions, self.questionWords = vecQuestions, questionWords
+        self.questionCntxWords, self.knowledgeBase = questionCntxWords, knowledgeBase
+
     # ------------------------------------------------------------------ reference properties
     @property
     def state_size(self):

@@ -45,6 +45,19 @@ def init_output_params(specs, seed=0, dtype=np.float32, bias_scale=0.1):
     return out
 
 
+def answer_topk(logits, k=1, ids=None, probs=None):
+    """(ids int32 [B, k], probs fp32 [B, k]): the k most probable answers of each row of `logits` [B, A] and their softmax
+    probabilities, equal logits in ascending id order (`mac_answer_topk`); ids[:, 0] is the prediction of `addPredOp`
+    (`model.py:603-612`).  1 <= k <= min(8, A).  `ids` / `probs`: optional output tensors to write into."""
+    B, A = logits.shape
+    if not 1 <= int(k) <= min(8, A):
+        raise ValueError("k must be in 1..min(8, A = %d), got %r" % (A, k))
+    ids = torch.empty((B, k), dtype=torch.int32, device=logits.device) if ids is None else ids
+    probs = torch.empty((B, k), dtype=torch.float32, device=logits.device) if probs is None else probs
+    check(_lib.load().mac_answer_topk(ptr(logits), B, A, int(k), ptr(ids), ptr(probs), stream_ptr()), "mac_answer_topk")
+    return ids, probs
+
+
 class OutputUnit(object):
     """Forward / loss / backward of the output unit on device tensors.  `params` / `grads`: dict name -> tensor
     (e.g. views into the trainer's flat buckets)."""
@@ -88,7 +101,8 @@ class OutputUnit(object):
         return out
 
     def forward(self, memory, vecQuestions, answers, step=0, loss_scale=None):
-        """Returns (logits, losses [B], dlogits [B, A]) -- dlogits = (softmax - onehot) * loss_scale (default 1/B)."""
+        """Returns (logits, losses [B], dlogits [B, A]) -- dlogits = (softmax - onehot) * loss_scale (default 1/B).  The three
+        stay reachable as `last_logits`, `losses` and `dlogits` (`logits` is the label-free method)."""
         B = memory.shape[0]
         act = ACT["ELU"] if self.relu == "ELU" else ACT["RELU_STD"]
         self.eq = self._linear([vecQuestions], self.p["outputUnit/linearLayeroutQuestion/weights/weight"],
@@ -111,14 +125,26 @@ class OutputUnit(object):
             x = self._linear(xs, W, b, act if i < self.nfc - 1 else 0)
             if i < self.nfc - 1:
                 setattr(self, "_h%d" % i, x)
-        self.logits = x
+        self.last_logits = x
         A = x.shape[1]
         self.losses = self._new(B)
         self.dlogits = self._new(B, A)
         scale = (1.0 / B) if loss_scale is None else float(loss_scale)
-        check(self.lib.mac_softmax_xent(ptr(self.logits), ptr(answers), ptr(self.losses), ptr(self.dlogits), scale, B, A,
+        check(self.lib.mac_softmax_xent(ptr(self.last_logits), ptr(answers), ptr(self.losses), ptr(self.dlogits), scale, B, A,
                                         stream_ptr()), "mac_softmax_xent")
-        return self.logits, self.losses, self.dlogits
+        return self.last_logits, self.losses, self.dlogits
+
+    def logits(self, memory, vecQuestions):
+        """The answer logits [B, A] without labels: the linears of `forward` with every dropout at 1, no loss, no `dlogits`,
+        nothing kept for a backward.  Bit for bit `forward(...)[0]` of a unit with keep = 1."""
+        act = ACT["ELU"] if self.relu == "ELU" else ACT["RELU_STD"]
+        eq = self._linear([vecQuestions], self.p["outputUnit/linearLayeroutQuestion/weights/weight"],
+                          self.p["outputUnit/linearLayeroutQuestion/biases/bias"])
+        xs = [memory, eq]
+        for i in range(self.nfc):
+            xs = [self._linear(xs, self.p["classifier/linearLayerfc_%d/weights/weight" % i],
+                               self.p["classifier/linearLayerfc_%d/biases/bias" % i], act if i < self.nfc - 1 else 0)]
+        return xs[0]
 
     def invalidate(self):
         """Call after the parameters were updated in place (optimizer step): drops the cached transposes."""

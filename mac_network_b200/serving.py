@@ -7,6 +7,9 @@ stream -> the captured netLength unroll -> D2H of the final state and the attent
 of the others.  The knowledge base is 83 % of a batch's bytes; the bf16 read unit only ever reads its bf16 copy
 (mac_cast_bf16 would make it on the device), so casting on the host (mac_host_cast_bf16, a thread pool inside the
 C library; same bits) halves the H2D traffic -- PCIe, not the GPU, bounds this path.
+
+`HostPipeline` is that path for the cell alone (its inputs are the encoder's and the stem's outputs); `ModelPipeline` is the
+same scheme for the whole model: question ids and channel-major image features in, answers and attention maps out.
 """
 import ctypes
 import os
@@ -116,6 +119,81 @@ def bind_to_gpu_numa(device_index):
     return info
 
 
+def _pinned(numel, dtype):
+    return torch.empty(numel, dtype=dtype).pin_memory()
+
+
+def _time_cast(lib, n, threads):
+    """Best of four host casts of n fp32 elements to bf16 on the library's pool, in ms."""
+    import time
+    src = _pinned(n, torch.float32).zero_()
+    dst = _pinned(n, torch.bfloat16)
+    best = float("inf")
+    for _ in range(4):
+        t0 = time.perf_counter()
+        lib.mac_host_cast_bf16(ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(dst.data_ptr()), n, threads)
+        best = min(best, time.perf_counter() - t0)
+    return best * 1e3
+
+
+def _cast_pays(cast_ms, numel):
+    """The host cast pays off only if it is faster than the PCIe time of the bytes it saves (2 B per element at a
+    conservative 25 GB/s); with few host threads per rank (torchrun on a small CPU quota) it is not."""
+    return cast_ms <= 0.8 * (numel * 2 / 25e9 * 1e3)
+
+
+class _CastRing(object):
+    """Host cast of one fp32 tensor per batch to bf16 on the library's thread pool (mac_host_cast_bf16_begin returns at once;
+    no Python threads, so no GIL hand-offs in the submit loop), one batch ahead of the copies, through a SMALL ring of
+    pinned staging buffers (not one buffer per device slot), so that what the cast writes and the H2D engine reads stays in
+    the socket's last-level cache -- the cast then costs DRAM only its fp32 read."""
+
+    def __init__(self, lib, numel, ring, threads):
+        self.lib, self.threads = lib, threads
+        self.stages = [_pinned(numel, torch.bfloat16) for _ in range(ring)]
+        self.busy = [None] * ring           # event after the copy that last read each buffer
+        self.casts = 0                      # casts started so far: the next one's place in the ring
+        self.pending = None                 # (ticket, source tensor, ring index) of the cast in flight
+
+    def begin(self, src):
+        """Start the cast of `src` into the next staging buffer; returns that buffer's ring index."""
+        si = self.casts % len(self.stages)
+        self.casts += 1
+        if self.busy[si] is not None:
+            self.busy[si].synchronize()              # the previous copy out of this staging buffer has finished
+            self.busy[si] = None
+        st = self.lib.mac_host_cast_bf16_begin(ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(self.stages[si].data_ptr()),
+                                               self.stages[si].numel(), self.threads)
+        if st != 0:
+            raise _lib.MacB200Error("mac_host_cast_bf16_begin failed: %d" % st)
+        return si
+
+    def prefetch(self, ticket, src):
+        """Start the cast of `src` for the submit that will carry `ticket`, unless it is the one already in flight."""
+        if self.pending is not None:
+            if self.pending[0] == ticket and self.pending[1] is src:
+                return
+            self.lib.mac_host_cast_bf16_end()
+            self.casts -= 1                          # that cast is discarded: its staging buffer is taken again
+        self.pending = (ticket, src, self.begin(src))
+
+    def take(self, ticket, src):
+        """Ring index of the staging buffer that holds (or is receiving) bf16(src); `end()` before copying out of it."""
+        self.prefetch(ticket, src)                   # no-op when the caller (or the previous submit) already started it
+        si = self.pending[2]
+        self.pending = None
+        return si
+
+    def end(self):
+        self.lib.mac_host_cast_bf16_end()
+
+    def copied(self, si, stream):
+        """Call after enqueueing the copy out of staging buffer `si` on `stream`."""
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        self.busy[si] = ev
+
+
 class _Slot(object):
     def __init__(self, cfg, params, shape, prec, host_kb_bf16, use_graph, fold_y=None, small_tc=None):
         B, S, N, d, L = shape
@@ -170,99 +248,51 @@ class HostPipeline(object):
         self.cast_threads = int(cast_threads) if cast_threads else max(1, min(12, usable_cpus() - 2))
         self.cast_ms = None
         if self.host_kb_bf16 and host_cast is None:
-            # the cast pays off only if it is faster than the PCIe time of the bytes it saves (2 B per KB element at a
-            # conservative 25 GB/s); with few host threads per rank (torchrun on a small CPU quota) it is not
-            self.cast_ms = self._time_cast(shape)
-            saved_ms = shape[0] * shape[2] * shape[3] * 2 / 25e9 * 1e3
-            if self.cast_ms > 0.8 * saved_ms:
-                self.host_kb_bf16 = False
+            self.cast_ms = _time_cast(self.lib, shape[0] * shape[2] * shape[3], self.cast_threads)
+            self.host_kb_bf16 = _cast_pays(self.cast_ms, shape[0] * shape[2] * shape[3])
         if fold_y is None:
             fold_y = slots < 4          # several batches in flight: the unfolded write + projY GEMMs pack better (mac_cell.py)
         # several batches in flight: the tensor-core form of the batch-sized projections (see MACCell.__init__)
         self.slots = [_Slot(cfg, params, shape, prec, self.host_kb_bf16, use_graph, fold_y, small_tc=(slots >= 2))
                       for _ in range(max(1, slots))]
-        self._cast_for = None
         self._next = 0
         B, S, N, d, L = shape
-        # bf16 staging of the knowledge base through a SMALL ring of pinned buffers (not one buffer per device slot), so that
-        # what the cast writes and the H2D engine reads stays in the socket's last-level cache -- the cast then costs DRAM only
-        # its fp32 read.  Measured with two ranks on one socket (reasoning-steps/s, both ranks): 30.3k with 12 full-size buffers
-        # per rank, 36.9k with 3, 43.4k with 2; no cast: 40.0k.  One rank: 28.4k / 28.9k / 25.2k with 2 / 3 / 12.
+        # bf16 staging of the knowledge base through _CastRing's small ring of pinned buffers.  Measured with two ranks on one
+        # socket (reasoning-steps/s, both ranks): 30.3k with 12 full-size buffers per rank, 36.9k with 3, 43.4k with 2; no
+        # cast: 40.0k.  One rank: 28.4k / 28.9k / 25.2k with 2 / 3 / 12.
         # Each buffer takes a whole knowledge base: casting it in several pieces, the cast of piece c+1 under the copy of
         # piece c, measured WORSE (4 pieces: 18.6k with one rank, 18.8-24.3k with two) -- every piece is one more wake-up of
         # the cast pool and one more blocking wait in the submit loop.
         # `stage_ring`: 3 full-size buffers when this rank has its socket to itself (one more pass of slack between a buffer's
         # copy and its next cast), 2 when the socket's cache is shared with another rank's ring (callers pass it; default 3)
         ring = max(2, int(stage_ring) if stage_ring else 3)
-        self._stages = ([torch.empty(B * N * d, dtype=torch.bfloat16).pin_memory() for _ in range(ring)]
-                        if self.host_kb_bf16 else [])
-        self._stage_busy = [None] * len(self._stages)      # event after the copy that last read each buffer
-        self._casts = 0                                     # casts started so far: the next one's place in the ring
+        self._ring = _CastRing(self.lib, B * N * d, ring, self.cast_threads) if self.host_kb_bf16 else None
+        self._stages = self._ring.stages if self._ring else []
         kb_bytes = B * N * d * (2 if self.host_kb_bf16 else 4)
         self.h2d_bytes = kb_bytes + B * S * d * 4 + B * d * 4 + B * 4
         self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.slots[0].outs_host.values())
 
-    def _time_cast(self, shape):
-        import time
-        n = shape[0] * shape[2] * shape[3]
-        src = torch.zeros(n, dtype=torch.float32).pin_memory()
-        dst = torch.empty(n, dtype=torch.bfloat16).pin_memory()
-        best = float("inf")
-        for _ in range(4):
-            t0 = time.perf_counter()
-            self.lib.mac_host_cast_bf16(ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(dst.data_ptr()), n, self.cast_threads)
-            best = min(best, time.perf_counter() - t0)
-        return best * 1e3
-
-    # -- host cast of the knowledge base on the library's thread pool, one batch ahead of the copies
-    #    (mac_host_cast_bf16_begin returns at once; no Python threads, so no GIL hand-offs in the submit loop)
-    def _cast_begin(self, kb):
-        """Start the cast of `kb` into the next staging buffer; returns that buffer's ring index."""
-        si = self._casts % len(self._stages)
-        self._casts += 1
-        if self._stage_busy[si] is not None:
-            self._stage_busy[si].synchronize()         # the previous copy out of this staging buffer has finished
-            self._stage_busy[si] = None
-        st = self.lib.mac_host_cast_bf16_begin(ctypes.c_void_p(kb.data_ptr()), ctypes.c_void_p(self._stages[si].data_ptr()),
-                                               self._stages[si].numel(), self.cast_threads)
-        if st != 0:
-            raise _lib.MacB200Error("mac_host_cast_bf16_begin failed: %d" % st)
-        return si
-
     def prefetch(self, batch):
         """Optional: start the host cast for the batch that the NEXT submit() will take."""
-        if not self.host_kb_bf16:
-            return
-        kb = batch["knowledgeBase"]
-        if self._cast_for is not None:
-            if self._cast_for[0] == self._next and self._cast_for[1] is kb:
-                return
-            self.lib.mac_host_cast_bf16_end()
-            self._casts -= 1                           # that cast is discarded: its staging buffer is taken again
-        si = self._cast_begin(kb)
-        self._cast_for = (self._next, kb, si)
+        if self.host_kb_bf16:
+            self._ring.prefetch(self._next, batch["knowledgeBase"])
 
     def submit(self, batch, next_batch=None):
         t = self._next
         slot = self.slots[t % len(self.slots)]
         if self.host_kb_bf16:
-            self.prefetch(batch)                       # no-op when the caller (or the previous submit) already started it
-            si = self._cast_for[2]
-            self._cast_for = None
+            si = self._ring.take(t, batch["knowledgeBase"])
         self._next = t + 1
         with torch.cuda.stream(slot.stream):
             slot.x["vecQuestions"].copy_(batch["vecQuestions"], non_blocking=True)
             slot.x["questionCntxWords"].copy_(batch["questionCntxWords"], non_blocking=True)
             slot.x["questionLengths"].copy_(batch["questionLengths"], non_blocking=True)
             if self.host_kb_bf16:
-                self.lib.mac_host_cast_bf16_end()                      # the knowledge base is in its staging buffer
+                self._ring.end()                                       # the knowledge base is in its staging buffer
                 if next_batch is not None:                             # the next batch's cast runs under this copy
-                    nsi = self._cast_begin(next_batch["knowledgeBase"])
-                    self._cast_for = (self._next, next_batch["knowledgeBase"], nsi)
+                    self._ring.prefetch(self._next, next_batch["knowledgeBase"])
                 slot.x["knowledgeBase"].view(-1).copy_(self._stages[si], non_blocking=True)
-                ev = torch.cuda.Event()
-                ev.record(slot.stream)
-                self._stage_busy[si] = ev
+                self._ring.copied(si, slot.stream)
             else:
                 slot.x["knowledgeBase"].copy_(batch["knowledgeBase"], non_blocking=True)
                 if next_batch is not None:
@@ -299,3 +329,227 @@ class HostPipeline(object):
         for s in self.slots:
             if s.busy:
                 stream.wait_event(s.done)
+
+
+class _ModelSlot(object):
+    """One batch in flight through the whole model: its own stream, persistent device inputs, its own evaluation-mode
+    encoder / stem / cell / output unit over the model's parameter tensors, the forward captured as one CUDA graph, pinned
+    host outputs."""
+
+    def __init__(self, model, shape, images_bf16, use_graph, topk):
+        B, S, H, W = shape
+        t, cfg = model.trainer, model.cfg
+        p = t.params
+        self.model, self.B, self.topk, self.use_graph = model, B, topk, use_graph
+        C = p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2]
+        self.stream = torch.cuda.Stream()
+        self.x = {"questions": torch.zeros(B, S, dtype=torch.int32, device=p.device),
+                  "questionLengths": torch.full((B,), S, dtype=torch.int32, device=p.device),
+                  "images": torch.zeros(B, C, H, W, device=p.device,
+                                        dtype=torch.bfloat16 if images_bf16 else torch.float32)}
+        from .encoder import QuestionEncoder
+        from .output_unit import OutputUnit
+        from .stem import Stem
+        version = lambda: p.version
+        self.enc = QuestionEncoder({k: p.t[k] for k in t._enc_specs}, keep_input=1.0, keep_question=1.0,
+                                   prec=model._enc.prec, version=version)
+        self.stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=model._stem.prec, version=version)
+        self.out = OutputUnit({k: p.t[k] for k in p.specs if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu,
+                              keep=1.0, version=version)
+        self.cell = None
+        self.graph = None
+        self.outs_host = None
+        self.done = torch.cuda.Event()
+        self.busy = False
+        self.capture()
+
+    def _forward(self):
+        from .output_unit import answer_topk
+        m, x = self.model, self.x
+        words, cntx, vecq = self.enc.forward(x["questions"], x["questionLengths"])
+        kb = self.stem.forward_nchw(x["images"])
+        if self.cell is None:       # MACCell's own errors (flag set / precision outside its inference forms) pass through
+            self.cell = MACCell(vecq, words, cntx, x["questionLengths"], kb, 1.0, 1.0, 1.0, self.B, False, config=m.cfg,
+                                params=m.trainer.params, prec=m.prec)
+        else:
+            self.cell.rebind(vecq, words, cntx, kb)
+        c = self.cell
+        _, memory = mac_network(c, m.L)
+        logits = self.out.logits(memory, vecq)
+        ids, probs = answer_topk(logits, self.topk)
+        outs = {"answers": ids, "probs": probs, "logits": logits, "memory": memory, "att_kb": c._att_kb,
+                "att_question": c._att_q}
+        if c.attentions["gate"]:
+            outs["gate"] = torch.stack(c.attentions["gate"])
+        if c.attentions["self"]:            # step i attends over its i + 1 history rows: zero-padded to [L, B, L]
+            outs["self"] = torch.zeros(m.L, self.B, m.L, device=memory.device)
+            for i, a in enumerate(c.attentions["self"]):
+                outs["self"][i, :, :i + 1].copy_(a)
+        return outs
+
+    def capture(self):
+        """One eager pass (weight packs and folded weights of the current parameter version are built outside the graph),
+        then the capture.  The outputs of the pass that was captured are the graph's static output tensors.  The slot's
+        stream first waits for the caller's current stream: whatever wrote the parameters there (an optimizer step, a
+        checkpoint restore) or built packs from them (`runBatch`) is enqueued, not necessarily done."""
+        self.graph = None                   # a previous capture's memory goes back before the new one takes its own
+        self.cell = None                    # a cell holds pointers into its parameter version's packed weights
+        self.stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(self.stream):
+            self.outs_dev = self._forward()
+            self.stream.synchronize()
+            if self.use_graph:
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g, stream=self.stream):
+                    self.outs_dev = self._forward()
+                self.graph = g
+        if self.outs_host is None:
+            self.outs_host = {k: _pinned(v.numel(), v.dtype).view(v.shape) for k, v in self.outs_dev.items()}
+
+    def enqueue(self, questions, lengths, images, copied=None):
+        """H2D copies -> forward -> D2H copies on this slot's stream; returns after enqueueing.  `images` is host memory of
+        the slot's image type (the caller's fp32 tensor or a bf16 staging buffer), any shape with the right element count,
+        or a callable that returns it, called once the small copies are enqueued (the host cast is waited for there);
+        `copied(stream)` is called once the image copy is enqueued."""
+        with torch.cuda.stream(self.stream):
+            self.x["questions"].copy_(questions, non_blocking=True)
+            self.x["questionLengths"].copy_(lengths, non_blocking=True)
+            if callable(images):
+                images = images()
+            self.x["images"].view(-1).copy_(images.view(-1), non_blocking=True)
+            if copied is not None:
+                copied(self.stream)
+            if self.graph is not None:
+                self.graph.replay()
+            else:
+                self.outs_dev = self._forward()
+            for k, src in self.outs_dev.items():
+                self.outs_host[k].copy_(src, non_blocking=True)
+            self.done.record(self.stream)
+        self.busy = True
+
+
+class ModelPipeline(object):
+    """The whole model from host buffers: what a caller who has questions and image features -- not the encoder's and the
+    stem's outputs `HostPipeline` takes -- uses to ask the model for answers, with no labels.
+
+        pipe = ModelPipeline(model, shape=(B, S, H, W), slots=4)
+        t = pipe.submit({"questions": int32 [B, S] (0-padded), "questionLengths": int32 [B], "images": fp32 [B, C, H, W]})
+        out = pipe.result(t)          # pinned host tensors, valid until the slot is reused `slots` submits later
+
+    `model` is a `MACnet`: the pipeline serves the weights in `model.trainer.params` with the model's `prec` and evaluation
+    stem / encoder precisions (to serve EMA shadows, load them first: `load_checkpoint(use_ema=True)`; `runBatch`'s per-batch
+    EMA swap has no counterpart here).  Each of the `slots` batches in flight has its own stream and runs
+    `mac_ingest_nchw` -> stem -> encoder -> `mac_network` -> `OutputUnit.logits` -> `mac_answer_topk` as ONE captured CUDA
+    graph, so one batch's PCIe copies overlap another's kernels.  Images are 96 % of a batch's bytes; the bf16 stem reads
+    only bf16(x), so with it `host_cast` (None: decide by timing, as `HostPipeline` does; True / False: forced) casts them
+    on the host and halves the H2D traffic.  With any other stem the features stay fp32.  Measured on an H100 (DESIGN.md
+    section 8) the fp32 copies ran at 27-36 GB/s with four slots and the cast, bound by the host's cores, was the slower
+    path; callers who see the copies keep up should pass `host_cast=False`.
+
+    `out`: `answers` int32 [B, topk] (column 0 is the prediction), `probs` [B, topk], `logits` [B, A], `memory` [B, d],
+    `att_kb` [L, B, H*W], `att_question` [L, B, S], and `gate` [L, B, d] / `self` [L, B, L] (step i's i + 1 weights, zero
+    beyond) when the flag set has them.
+
+    Questions are padded with 0 to the pipeline's fixed S (a captured graph cannot trim a batch to its longest question as
+    `runBatch` does); the kernels mask by length, so attention at positions >= length is exactly 0.
+
+    When the parameter values move (`params.version`: optimizer step, checkpoint restore), the packed weights are rebuilt as
+    new tensors a captured graph would not see: the next `submit` drains the pipeline and captures every slot again before
+    it takes the batch.  Each slot's stream waits there for the caller's current stream, so an update enqueued on that
+    stream (`DPTrainer`'s optimizer step does not synchronise) is complete before the packs are rebuilt from it.  The
+    other direction is the caller's: batches in flight read the parameters, so `drain()` before writing them.
+
+    Memory: every slot has its own encoder and stem and with them its own weight packs (about 14 MB per slot at 1024 -> 512
+    -> 512), and its graph's private pool holds its own patch matrices (231 MB for layer 0 at 64x1024x14x14)."""
+
+    def __init__(self, model, shape, slots=4, use_graph=True, topk=1, host_cast=None, cast_threads=None, stage_ring=None):
+        B, S, H, W = [int(v) for v in shape]
+        p = model.trainer.params
+        C = int(p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2])
+        nfc = len([k for k in p.t if k.startswith("classifier/linearLayerfc_") and k.endswith("weights/weight")])
+        A = int(p.t["classifier/linearLayerfc_%d/weights/weight" % (nfc - 1)].shape[1])
+        if min(B, S, H, W) <= 0 or slots < 1:
+            raise ValueError("shape (B, S, H, W) and slots must be positive, got %r, slots = %r" % (shape, slots))
+        if C % 64:
+            raise ValueError("the image features have %d channels: mac_ingest_nchw needs a multiple of 64" % C)
+        if not 1 <= int(topk) <= min(8, A):
+            raise ValueError("topk must be in 1..min(8, %d answers), got %r" % (A, topk))
+        self.lib = _lib.load()
+        self.model, self.params, self.shape, self.C, self.topk = model, p, (B, S, H, W), C, int(topk)
+        self.use_graph = bool(use_graph)
+        self.cast_threads = int(cast_threads) if cast_threads else max(1, min(12, usable_cpus() - 2))
+        numel = B * C * H * W
+        self.host_cast = model._stem.prec == "bf16" and host_cast is not False
+        self.cast_ms = None
+        if self.host_cast and host_cast is None:
+            self.cast_ms = _time_cast(self.lib, numel, self.cast_threads)
+            self.host_cast = _cast_pays(self.cast_ms, numel)
+        self._version = p.version
+        self.slots = [_ModelSlot(model, self.shape, self.host_cast, self.use_graph, self.topk) for _ in range(int(slots))]
+        self._ring = (_CastRing(self.lib, numel, max(2, int(stage_ring) if stage_ring else 3), self.cast_threads)
+                      if self.host_cast else None)
+        self._next = 0
+        self._ahead = None                  # (next_batch["images"] as given, its host tensor) of the cast in flight
+        self.h2d_bytes = numel * (2 if self.host_cast else 4) + B * S * 4 + B * 4
+        self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.slots[0].outs_host.values())
+
+    def _host(self, batch):
+        """The batch's three host tensors, checked against the pipeline's shape; ValueError before anything is enqueued."""
+        B, S, H, W = self.shape
+        want = (("questions", (B, S), torch.int32), ("questionLengths", (B,), torch.int32),
+                ("images", (B, self.C, H, W), torch.float32))
+        out = []
+        for key, shp, dtype in want:
+            v = torch.as_tensor(batch[key])
+            if v.device.type != "cpu" or tuple(v.shape) != shp:
+                raise ValueError("%s must be a host tensor of shape %s, got %s on %s" % (key, shp, tuple(v.shape), v.device))
+            out.append(v.to(dtype).contiguous())
+        return out
+
+    def submit(self, batch, next_batch=None):
+        """Enqueue one batch (numpy arrays or host tensors; pinned memory makes the copies asynchronous) and return its
+        ticket.  `next_batch`: the batch the next submit will take, whose host cast then runs under this batch's copies."""
+        q, ql, img = self._host(batch)
+        if self._ahead is not None and self._ahead[0] is batch["images"]:
+            img = self._ahead[1]                           # the tensor whose cast the previous submit started
+        nxt = self._host(next_batch)[2] if (next_batch is not None and self.host_cast) else None
+        self._ahead = None if nxt is None else (next_batch["images"], nxt)
+        if self.params.version != self._version:
+            self.drain()
+            for s in self.slots:
+                s.capture()
+            self._version = self.params.version
+        t = self._next
+        slot = self.slots[t % len(self.slots)]
+        self._next = t + 1
+        if not self.host_cast:
+            slot.enqueue(q, ql, img)
+            return t
+        si = self._ring.take(t, img)
+
+        def staged():                                      # after the small copies are enqueued, as in HostPipeline.submit
+            self._ring.end()                               # the images are in their staging buffer
+            if nxt is not None:                            # the next batch's cast runs under this batch's copies
+                self._ring.prefetch(self._next, nxt)
+            return self._ring.stages[si]
+        slot.enqueue(q, ql, staged, copied=lambda stream: self._ring.copied(si, stream))
+        return t
+
+    def result(self, ticket):
+        """Block until the batch of `ticket` is done; its outputs stay valid until `slots` further submits."""
+        if not self._next - len(self.slots) <= ticket < self._next:
+            raise ValueError("ticket %r is not one of the last %d submits" % (ticket, len(self.slots)))
+        slot = self.slots[ticket % len(self.slots)]
+        slot.done.synchronize()
+        return slot.outs_host
+
+    def predictions(self, out):
+        """The answers of a `result` as the model's `answer_decoder` spells them (ids without one)."""
+        dec = self.model.decode
+        return [dec(int(i)) if dec else int(i) for i in out["answers"][:, 0]]
+
+    def drain(self):
+        for s in self.slots:
+            if s.busy:
+                s.done.synchronize()

@@ -21,6 +21,7 @@ from . import _lib
 from ._lib import ACT, check, ptr, stream_ptr
 
 SITE_STEM = 32            # Philox site base for the stem's input dropouts (site + layer index)
+INGEST_NHWC_F32, INGEST_PATCH_BF16 = 0, 1       # enum MAC_INGEST_* (include/mac_b200.h)
 
 
 def stem_specs(in_dim, out_dim, num_layers=2, ksize=3, stem_dim=None):
@@ -134,9 +135,10 @@ class Stem(object):
             raise NotImplementedError("stem training runs in fp32, bf16 or bf16x3, not %r (DESIGN.md section 9)" % self.prec)
         self._check_tiles(in_dim, "%s stem training" % self.prec)
 
-    def forward(self, images, keep=1.0, step=0, save_for_backward=False):
+    def forward(self, images, keep=1.0, step=0, save_for_backward=False, _cols0=None):
         """images: [B,H,W,C] fp32 NHWC (the reference transposes the NCHW h5 features first, model.py:~770).
-        Returns the knowledge base [B, H*W, outDim] fp32."""
+        Returns the knowledge base [B, H*W, outDim] fp32.  `_cols0` (`forward_nchw`, bf16 inference): layer 0's bf16 patch
+        matrix, already built; `images` then only gives the shape."""
         x = images
         B, H, Wd, C = x.shape
         act = ACT["ELU"] if self.relu == "ELU" else ACT["RELU_STD"]
@@ -167,9 +169,12 @@ class Stem(object):
                     self._saved["ys"].append(y)
                 x = y.view(B, H, Wd, Nout)
                 continue
-            cols = torch.empty((M, K), dtype=torch.bfloat16 if bf16 else torch.float32, device=self.device)
-            check(self.lib.mac_im2col3x3(ptr(x), ptr(cols), 1 if bf16 else 0, float(keep), self.seed, SITE_STEM + i, step,
-                                         B, H, Wd, C, stream_ptr()), "mac_im2col3x3")
+            if i == 0 and _cols0 is not None:
+                cols = _cols0
+            else:
+                cols = torch.empty((M, K), dtype=torch.bfloat16 if bf16 else torch.float32, device=self.device)
+                check(self.lib.mac_im2col3x3(ptr(x), ptr(cols), 1 if bf16 else 0, float(keep), self.seed, SITE_STEM + i, step,
+                                             B, H, Wd, C, stream_ptr()), "mac_im2col3x3")
             if bf16:
                 check(self.lib.mac_linear_tc_fwd(ptr(cols), ptr(Wt), ptr(b), act, ptr(y), 0, M, K, Nout, stream_ptr()),
                       "mac_linear_tc_fwd")
@@ -182,6 +187,34 @@ class Stem(object):
                 self._saved["ys"].append(y)
             x = y.view(B, H, Wd, Nout)
         return x.view(B, H * Wd, x.shape[3])
+
+    def forward_nchw(self, images):
+        """Inference forward (keep = 1) from the features in the layout they are stored in: images [B,C,H,W], contiguous,
+        fp32 or -- `prec="bf16"` only, whose layer 0 reads nothing but bf16(x) -- bf16.  `mac_ingest_nchw` (csrc/ingest.cuh)
+        replaces the NHWC permute: for the bf16 stem it writes layer 0's bf16 patch matrix directly, for the other
+        precisions the fp32 NHWC tensor their own patch passes read.  Returns what `forward(images.permute(0, 2, 3, 1))`
+        returns, bit for bit.  C must be a multiple of 64.  Raises before any launch."""
+        if images.dim() != 4 or not images.is_contiguous():
+            raise ValueError("images must be a contiguous [B, C, H, W] tensor")
+        if images.dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError("images must be float32 or bfloat16, got %s" % images.dtype)
+        x_bf16 = int(images.dtype == torch.bfloat16)
+        if x_bf16 and self.prec != "bf16":
+            raise ValueError("bf16 images are for the bf16 stem only: prec=%r reads the fp32 features" % self.prec)
+        B, C, H, Wd = images.shape
+        if C % 64:
+            raise NotImplementedError("forward_nchw needs a channel count that is a multiple of 64, got %d" % C)
+        if self.prec != "bf16":
+            if self.prec == "fp8":
+                self._check_fp8(C, 1.0)
+            x = torch.empty((B, H, Wd, C), dtype=torch.float32, device=self.device)
+            check(self.lib.mac_ingest_nchw(ptr(images), x_bf16, ptr(x), INGEST_NHWC_F32, B, C, H, Wd, stream_ptr()),
+                  "mac_ingest_nchw")
+            return self.forward(x)
+        cols = torch.empty((B * H * Wd, 9 * C), dtype=torch.bfloat16, device=self.device)
+        check(self.lib.mac_ingest_nchw(ptr(images), x_bf16, ptr(cols), INGEST_PATCH_BF16, B, C, H, Wd, stream_ptr()),
+              "mac_ingest_nchw")
+        return self.forward(images.permute(0, 2, 3, 1), _cols0=cols)     # a view: layer 0 reads `cols`, not the image
 
     def backward(self, d_kb, grads, need_d_images=False):
         """Backward of `forward(save_for_backward=True)` (the reference differentiates the graph with TF autodiff,
