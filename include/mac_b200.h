@@ -120,6 +120,11 @@ int mac_control_attend_fwd(const float* cc, long long cc_tstride, long long cc_b
  * MAC_PREC_FP32 takes every d % 4 == 0 up to d <= 2048 when B*N < 512 and d <= 4096 otherwise (at most 32 partial logits
  * per row, one per 64- or 128-column tile).  MAC_PREC_BF16 and MAC_PREC_TC32 take d % 128 == 0 up to d <= 4096 and need
  * the packs they read (see mac_read_weights; MAC_PREC_BF16 also kb_bf16).
+ * Row limits (a launch grid's y extent is at most 65535 tiles), each MAC_ERR_UNSUPPORTED: the tensor-core forms and the
+ * tensor-core parts of mac_read_invariant (MAC_PREC_BF16, TC32, FP8) need ceil(B*N / 128) <= 65535; MAC_PREC_FP32 needs
+ * ceil(B*N / 128) <= 65535 (B*N >= 512 and d >= 256, or enough 128-row tiles to fill the device's SMs), else
+ * ceil(B*N / 64) <= 65535.  The fused read steps (mac_read_step_fused_supported) take every B < 2^22.  kb_attend, the tail of
+ * every form, needs B * d / s <= 2^31 - 1 with s its column slice (128 when d % 128 == 0, so 4 CTAs per sample at d = 512).
  * mac_read_fwd, mac_read_fwd_inv and mac_read_invariant return every MAC_ERR_* before any launch and before any write:
  * a refused call leaves info, att, save, inv and the workspace as they were.
  * --------------------------------------------------------------------------------------------- */

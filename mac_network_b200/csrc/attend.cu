@@ -125,7 +125,8 @@ __global__ void __launch_bounds__(K1_THREADS) control_attend_kernel(
 }
 
 // =====================================================================================
-// K3: grid = (d / DS column slices, B).  Each CTA pulls its [N x DS] slab of the knowledge
+// K3: one CTA per (batch row b, column slice), blockIdx.x = b * (d / DS) + slice (slices of a row adjacent; a 1-D grid so
+// that B is not held to gridDim.y's 65535).  Each CTA pulls its [N x DS] slab of the knowledge
 // base into shared memory with bulk copies issued up-front (all bytes in flight at once),
 // computes the softmax of the row's N logits while they fly, then accumulates the weighted sum.
 // KB bytes are read exactly once; logits are re-read per slice (N*4 B, L2 hits).
@@ -144,7 +145,8 @@ __global__ void __launch_bounds__(K3_THREADS) kb_attend_kernel(
   __shared__ __align__(8) uint64_t bar[MAXBUF];
   __shared__ float s_red[K3_THREADS / 32];
 
-  const int slice = blockIdx.x, b = blockIdx.y;
+  const int nslices = d / DS;
+  const int b = blockIdx.x / nslices, slice = blockIdx.x - b * nslices;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int NW = K3_THREADS / 32;
   constexpr int GROUPS = K3_THREADS / DS;       // row groups working on the same columns
@@ -236,6 +238,7 @@ __global__ void __launch_bounds__(K3_THREADS) kb_attend_kernel(
 template <typename KT, int DS>
 static int launch_kb_attend(const float* logit_parts, int nparts, float br, const KT* kb, float* att, float* info,
                             int B, int N, int d, cudaStream_t stream) {
+  if (!kb_attend_grid_ok(B, d, sizeof(KT) == 2)) return MAC_ERR_UNSUPPORTED;   // before any CUDA call
   // stage sizing: the [N x DS] slab is cut into <= 8 boxes that are all requested up-front and consumed as they
   // land (the weighted sum of box i overlaps the flight of boxes i+1..); when the slab exceeds ~100 KB (two CTAs
   // per SM) the boxes are recycled as a ring
@@ -260,9 +263,8 @@ static int launch_kb_attend(const float* logit_parts, int nparts, float br, cons
                       (size_t)K3_THREADS * sizeof(float) + 16;
   auto kern = kb_attend_kernel<KT, DS>;
   MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  dim3 grid(d / DS, B);
-  kern<<<grid, K3_THREADS, smem, stream>>>(logit_parts, nparts, br, map, att, info, B, N, d, rows_per_stage, nstages, nbuf,
-                                           (int)(buf_bytes / sizeof(KT)));
+  kern<<<(unsigned)(B * (d / DS)), K3_THREADS, smem, stream>>>(logit_parts, nparts, br, map, att, info, B, N, d,
+                                                                rows_per_stage, nstages, nbuf, (int)(buf_bytes / sizeof(KT)));
   MAC_LAUNCH_CHECK();
   return MAC_OK;
 }
@@ -308,17 +310,17 @@ extern "C" int mac_kb_attend_fwd(const float* logit_parts, int nparts, float br,
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!logit_parts || !kb || !att || !info || nparts <= 0 || B <= 0 || N <= 0 || d <= 0) return MAC_ERR_INVALID;
   if (!mac_aligned16(kb)) return MAC_ERR_ALIGN;
+  const int ds = kb_attend_slice(d, kb_is_bf16 != 0);
   if (kb_is_bf16) {
-    if (d % 128 == 0) return launch_kb_attend<__nv_bfloat16, 128>(logit_parts, nparts, br, (const __nv_bfloat16*)kb, att, info, B, N, d, stream);
-    if (d % 64 == 0) return launch_kb_attend<__nv_bfloat16, 64>(logit_parts, nparts, br, (const __nv_bfloat16*)kb, att, info, B, N, d, stream);
+    if (ds == 128) return launch_kb_attend<__nv_bfloat16, 128>(logit_parts, nparts, br, (const __nv_bfloat16*)kb, att, info, B, N, d, stream);
+    if (ds == 64) return launch_kb_attend<__nv_bfloat16, 64>(logit_parts, nparts, br, (const __nv_bfloat16*)kb, att, info, B, N, d, stream);
     return MAC_ERR_UNSUPPORTED;
   }
-  if (d % 128 == 0) return launch_kb_attend<float, 128>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
-  if (d % 64 == 0) return launch_kb_attend<float, 64>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
-  if (d % 32 == 0) return launch_kb_attend<float, 32>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
-  if (d % 16 == 0) return launch_kb_attend<float, 16>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
-  // narrow slices for the widths the fp32 read unit accepts (d % 4 == 0): a 4-column box is 16 bytes, the TMA minimum
-  if (d % 8 == 0) return launch_kb_attend<float, 8>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
-  if (d % 4 == 0) return launch_kb_attend<float, 4>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
+  if (ds == 128) return launch_kb_attend<float, 128>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
+  if (ds == 64) return launch_kb_attend<float, 64>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
+  if (ds == 32) return launch_kb_attend<float, 32>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
+  if (ds == 16) return launch_kb_attend<float, 16>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
+  if (ds == 8) return launch_kb_attend<float, 8>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
+  if (ds == 4) return launch_kb_attend<float, 4>(logit_parts, nparts, br, (const float*)kb, att, info, B, N, d, stream);
   return MAC_ERR_UNSUPPORTED;
 }

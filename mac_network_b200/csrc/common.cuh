@@ -38,6 +38,19 @@ namespace mac {
 // next sample (past the buffer's end for the last one).
 __device__ __forceinline__ int seq_len(const int32_t* lengths, int b, int S) { return min(max(lengths[b], 0), S); }
 
+// kb_attend's column slice (attend.cu): the widest of 128, 64 (bf16) or down to 4 (fp32) dividing d; 0 when none does.  The
+// narrow fp32 slices serve the widths the fp32 read unit accepts (d % 4 == 0): a 4-column box is 16 bytes, the TMA minimum.
+inline int kb_attend_slice(int d, bool kb_bf16) {
+  for (int ds = 128; ds >= (kb_bf16 ? 64 : 4); ds /= 2)
+    if (d % ds == 0) return ds;
+  return 0;
+}
+// kb_attend runs B * d / slice CTAs on a 1-D grid (gridDim.x <= 2^31 - 1)
+inline bool kb_attend_grid_ok(long long B, int d, bool kb_bf16) {
+  const int ds = kb_attend_slice(d, kb_bf16);
+  return ds > 0 && B * (d / ds) <= 0x7fffffffLL;
+}
+
 // ------------------------------------------------------------------ activations (ops.py:161-187)
 __device__ __forceinline__ float elu_f(float x) { return x > 0.f ? x : expm1f(x); }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }

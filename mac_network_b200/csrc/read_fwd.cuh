@@ -474,6 +474,20 @@ static int read_check_form(ReadForm f, bool inv, const float* kb, const void* kb
   return bf16_kb && kb_bf16 && !mac_aligned16(kb_bf16) ? MAC_ERR_ALIGN : MAC_OK;
 }
 
+// gridDim.y <= 65535 caps the row tiles of every [B*N, d] product a form launches: tc_gemm and tc3_gemm cut the rows into
+// tiles of TC_BM = 128, sgemm into the 128 or 64 rows sgemm_big_tiles picks (the fp32 forms' products all have N = d and
+// K >= d; 64 when any of them takes it).  The y projection's B rows are no more than B*N and take 128-row tiles from 512
+// rows on at these widths.  Step forms (`inv` false): read_step_supported bounds their rows, and their kernels put the
+// tiles on gridDim.x.  M = B * N in 64 bits: the forms compute it as an int only once this holds.
+inline bool read_rows_ok(ReadForm f, bool inv, long long M, int d) {
+  if (f == RF_FP32_TRAIN || f == RF_FP32_INV) {
+    const int bm = M <= 0x7fffffffLL && sgemm_big_tiles((int)M, d, d) ? 128 : 64;
+    return (M + bm - 1) / bm <= 65535;
+  }
+  if (!inv && (f == RF_BF16_STEP || f == RF_FP8_STEP)) return true;
+  return (M + TC_BM - 1) / TC_BM <= 65535;
+}
+
 static int read_fwd_check(ReadForm f, const ReadCall& c) {
   const int st = read_check_form(f, false, c.kb, c.kb_bf16, c.w, c.d);
   if (st != MAC_OK) return st;
@@ -486,6 +500,9 @@ static int read_fwd_check(ReadForm f, const ReadCall& c) {
     return MAC_ERR_ALIGN;
   if (f == RF_BF16_TRAIN && c.save && !mac_aligned16(c.save)) return MAC_ERR_ALIGN;    // widened into with 16-byte stores
   if (c.ws_bytes < read_ws_layout(c.prec, nullptr, c.B, c.N, c.d).bytes) return MAC_ERR_WORKSPACE;
+  // the launches' grids: the form's [B*N, d] products and kb_attend's B * d / slice CTAs
+  const bool kb16 = f == RF_BF16_STEP || f == RF_FP8_STEP || (c.prec == MAC_PREC_BF16 && c.kb_bf16);
+  if (!read_rows_ok(f, false, (long long)c.B * c.N, c.d) || !kb_attend_grid_ok(c.B, c.d, kb16)) return MAC_ERR_UNSUPPORTED;
   // the logits GEMM leaves one partial logit per column tile in a [B*N, 32] region
   return read_nparts(f, c.B * c.N, c.d) > 32 ? MAC_ERR_UNSUPPORTED : MAC_OK;
 }
@@ -497,7 +514,8 @@ static int read_inv_check(ReadForm f, const float* kb, const void* kb_bf16, cons
   const bool kb_opt = (prec == MAC_PREC_BF16 || prec == MAC_PREC_FP8) && kb_bf16;
   if ((!kb && !kb_opt) || !inv || B <= 0 || N <= 0 || d <= 0 || (d & 3)) return MAC_ERR_INVALID;
   if ((kb && !mac_aligned16(kb)) || !mac_aligned16(inv)) return MAC_ERR_ALIGN;
-  return inv_bytes < read_inv_layout(prec, nullptr, B, N, d).bytes ? MAC_ERR_WORKSPACE : MAC_OK;
+  if (inv_bytes < read_inv_layout(prec, nullptr, B, N, d).bytes) return MAC_ERR_WORKSPACE;
+  return read_rows_ok(f, true, (long long)B * N, d) ? MAC_OK : MAC_ERR_UNSUPPORTED;
 }
 
 // ------------------------------------------------------------------------------------------------ dispatch

@@ -89,14 +89,20 @@ def keep_mask(seed, site, step, shape, keep, device="cuda"):
 
 def attention_bound_check(att, info, I1_ref, absI1, c, wr, br, kbv, B, N, tol, ms=None):
     """att = softmax_n(sum_k ELU(I1 * c_b) * ms * wr + br), info = sum_n att * kb, with I1 known to tol * absI1 (the
-    accumulation bound of its product): the logit error is bounded through |d ELU(I1 c)/d I1| <= |c|, the softmax moves by
-    at most att * expm1(2 max|dlogit|), and fp32 evaluation adds a few 1e-6 relative.  Returns the worst fraction of the
-    bound used by att and by info."""
+    accumulation bound of its product): the logit error is bounded through |d ELU(I1 c)/d I1| <= |c|, and fp32 evaluation
+    adds a few 1e-6 relative.  Returns the worst fraction of the bound used by att and by info (softmax_bound_check)."""
     cb = c.double().repeat_interleave(N, 0)
     t = elu(I1_ref * cb)
     f = wr.double()[None, :] * (1.0 if ms is None else ms)
     logits = (t * f).sum(1) + br
     dL = (f.abs() * cb.abs() * tol * absI1).sum(1) + (f.abs() * (1e-7 + 1e-6 * t.abs())).sum(1) + 1e-6 * (logits.abs() + 1)
+    return softmax_bound_check(att, info, logits, dL, kbv, B, N)
+
+
+def softmax_bound_check(att, info, logits, dL, kbv, B, N):
+    """att = softmax_n(logits), info = sum_n att * kb, with each of the B*N logits known to dL: the softmax moves by at most
+    att * expm1(2 max|dlogit| of the sample), and its fp32 evaluation adds a few 1e-6 relative.  Returns the worst fraction
+    of the bound used by att and by info."""
     dL = dL.view(B, N).amax(1, keepdim=True)
     att_ref = torch.softmax(logits.view(B, N), 1)
     att_bnd = att_ref * (torch.expm1(2 * dL) + 4e-6) + 1e-12

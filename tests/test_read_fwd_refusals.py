@@ -95,10 +95,8 @@ def call(lib, c, ops, info, att, save, ws, inv):
                             None)
 
 
-@pytest.mark.parametrize("c,expect", CASES)
-def test_read_fwd_refuses_before_any_cuda_call(c, expect):
-    if torch.cuda.is_available():
-        pytest.skip("host pointers stand in for device buffers: the GPU twin below covers this device")
+def check_host_refusal(c, expect):
+    """the call with aligned host buffers the library never dereferences: the refusal, and no launch counted"""
     lib = L_.load()
     buf = (ctypes.c_char * 4096)()
     p = (ctypes.addressof(buf) + 15) & ~15              # 16-byte aligned, never dereferenced
@@ -108,9 +106,9 @@ def test_read_fwd_refuses_before_any_cuda_call(c, expect):
     assert lib.mac_b200_launch_count() == before
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("c,expect", CASES)
-def test_read_fwd_refuses_before_any_launch_or_write(c, expect):
+def check_device_refusal(c, expect):
+    """the call with device buffers as large as the form reads: the refusal, no launch, info / att / save still NaN, the
+    workspace, inv and every operand still zero"""
     lib = L_.load()
     prec, B, N, d = c["prec"], c["B"], c["N"], c["d"]
     M = B * N
@@ -128,3 +126,16 @@ def test_read_fwd_refuses_before_any_launch_or_write(c, expect):
     assert lib.mac_b200_launch_count() == before
     assert bool(info.isnan().all()) and bool(att.isnan().all()) and bool(save.isnan().all())
     assert not bool(ws.any()) and not bool(inv.any()) and not bool(ops.any())
+
+
+@pytest.mark.parametrize("c,expect", CASES)
+def test_read_fwd_refuses_before_any_cuda_call(c, expect):
+    if torch.cuda.is_available():
+        pytest.skip("host pointers stand in for device buffers: the GPU twin below covers this device")
+    check_host_refusal(c, expect)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("c,expect", CASES)
+def test_read_fwd_refuses_before_any_launch_or_write(c, expect):
+    check_device_refusal(c, expect)
