@@ -185,3 +185,31 @@ def ptr(t):
 def stream_ptr():
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def segments(ts):
+    """(pointers, widths, leading dimensions): the arrays a segmented entry point takes for a list of 2-D row-major tensors.
+    A None entry (an output segment nobody asked for) gives a null pointer, width 0 and leading dimension 0."""
+    n = len(ts)
+    return ((c_fp * n)(*[None if t is None else t.data_ptr() for t in ts]),
+            (c_int * n)(*[0 if t is None else t.shape[1] for t in ts]),
+            (c_int * n)(*[0 if t is None else t.stride(0) for t in ts]))
+
+
+def act_code(act, relu):
+    """ACT code of an activation name; "RELU" is the configured `relu`: ELU when relu == "ELU", else max(x, 0)."""
+    if act == "RELU":
+        return ACT["ELU"] if relu == "ELU" else ACT["RELU_STD"]
+    return ACT[act]
+
+
+def linear_bwd(xs, Wt, dy, dxs, accum, dW, db, ws, ws_bytes, stream):
+    """Backward of y = concat(xs) @ W + b (mac_linear_bwd): dxs[i] = (or += where accum[i]) dy @ Wt's rows of segment i
+    (a None dxs[i] is skipped; Wt = W^T, needed only when some dxs[i] is given), dW += concat(xs)^T @ dy, db += colsum(dy)
+    (each skipped when None).  `ws`: the caller's split-K workspace; its size chooses the summation order."""
+    n = len(xs)
+    x_p, x_k, x_ld = segments(xs)
+    dx_p, _, dx_ld = segments(dxs)
+    check(load().mac_linear_bwd(x_p, x_k, x_ld, n, ptr(Wt), ptr(dy), dy.stride(0), dx_p, dx_ld,
+                                (c_int * n)(*[int(a) for a in accum]), ptr(dW), ptr(db), dy.shape[0], dy.shape[1], ptr(ws),
+                                ws_bytes, stream), "mac_linear_bwd")

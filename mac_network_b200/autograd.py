@@ -16,14 +16,9 @@ import ctypes
 
 import torch
 
-from . import _lib
-from ._lib import ACT, check, ptr, stream_ptr
+from . import _lib, packs
+from ._lib import act_code, check, ptr, stream_ptr
 from .params import PREFIX
-
-
-def _t(params, W, key):
-    """Transposed fp32 copy of a weight (memory plumbing, cached until params.touch())."""
-    return params.derived(("T", key), lambda: W.t().contiguous())
 
 
 # the forms of the read unit's backward (csrc/backward.cu): fp32 FMA pipe, bf16 tensor cores, split-bf16 tensor cores
@@ -94,19 +89,9 @@ class _Bwd(object):
     def linear_bwd(self, xs, wname, bname, dy, dxs, accum, wgrad=True):
         """ops.linear backward: xs/dxs lists of 2-D views (dxs entries may be None).  wgrad=False: data gradients only (the
         weight / bias gradients of this call are formed later, batched over the steps)."""
-        n = len(xs)
-        W = self.p[wname]
-        Wt = _t(self.p, W, wname) if any(d is not None for d in dxs) else None
-        M, n_out = dy.shape
-        arr_x = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
-        arr_dx = (ctypes.c_void_p * n)(*[(d.data_ptr() if d is not None else None) for d in dxs])
-        arr_ldd = (ctypes.c_int * n)(*[(d.stride(0) if d is not None else 0) for d in dxs])
-        arr_acc = (ctypes.c_int * n)(*[int(a) for a in accum])
-        check(self.lib.mac_linear_bwd(arr_x, arr_k, arr_ld, n, ptr(Wt), ptr(dy), dy.stride(0), arr_dx, arr_ldd, arr_acc,
-                                      ptr(self.G(wname)) if wgrad else None, ptr(self.G(bname)) if (bname and wgrad) else None,
-                                      M, n_out, ptr(self.lws), self.lws_bytes, stream_ptr()), "mac_linear_bwd")
+        Wt = self.p.cache.pack(packs.transposed, self.p[wname]) if any(d is not None for d in dxs) else None
+        _lib.linear_bwd(xs, Wt, dy, dxs, accum, self.G(wname) if wgrad else None,
+                        self.G(bname) if (bname and wgrad) else None, self.lws, self.lws_bytes, stream_ptr())
 
     def axpy(self, dst, src, alpha=1.0):
         check(self.lib.mac_axpy(ptr(dst), ptr(src), float(alpha), src.numel(), stream_ptr()), "mac_axpy")
@@ -145,7 +130,7 @@ class _Bwd(object):
         nWm, nbm = self.lin_names(rsc, "memKbProj")
         nWm2, nbm2 = self.lin_names(rsc + "linearLayermemKbProj/", "memKbProj_2")
         wnames = {"Wx": nWx, "Wy": nWy, "Wm": nWm, "Wm2": nWm2}
-        Wt = lambda k: _t(self.p, self.p[wnames[k]], wnames[k])
+        Wt = lambda k: self.p.cache.pack(packs.transposed, self.p[wnames[k]])
         keep_m, keep_w = cell.dropouts["memory"], cell.dropouts["write"]
         hc, hm, hi = cell._hc, cell._hm, cell._hi
 
@@ -218,14 +203,10 @@ class _Bwd(object):
         du = z(B, d)
         if unshared:
             # one backward against the packed [d, L*d] weight; gradients scattered back to the per-step variables
-            Wc, bc = self.p.derived("qInputCat", lambda: None)
+            Wc, bc = self.p.q_input_cat()
             gW, gb = torch.zeros_like(Wc), torch.zeros_like(bc)
-            Wct = self.p.derived(("T", "qInputCat"), lambda: Wc.t().contiguous())
-            arr = lambda T, v: (T * 1)(v)
-            check(lib.mac_linear_bwd(arr(ctypes.c_void_p, u.data_ptr()), arr(ctypes.c_int, d), arr(ctypes.c_int, d), 1,
-                                     ptr(Wct), ptr(dci), L * d, arr(ctypes.c_void_p, du.data_ptr()), arr(ctypes.c_int, d),
-                                     arr(ctypes.c_int, 0), ptr(gW), ptr(gb), B, L * d, ptr(self.lws), self.lws_bytes,
-                                     stream_ptr()), "qInputCat bwd")
+            _lib.linear_bwd([u], self.p.cache.pack(packs.transposed, Wc), dci, [du], [0], gW, gb, self.lws, self.lws_bytes,
+                            stream_ptr())
             for i in range(L):
                 nW, nb = self.lin_names("MACCell/", "qInput%d" % i)
                 self.G(nW).copy_(gW[:, i * d:(i + 1) * d])
@@ -254,9 +235,8 @@ class _Bwd(object):
             dh = self.e(B, d)
             self.linear_bwd([hidden], nW2, nb2, dcc, [dh], [0])
             dpre = self.e(B, d)
-            act = c.controlContAct
-            code = ACT["ELU"] if (act == "RELU" and c.relu == "ELU") else ACT["RELU_STD"] if act == "RELU" else ACT[act]
-            check(lib.mac_activation_bwd(ptr(hidden), ptr(dh), code, ptr(dpre), B * d, stream_ptr()), "act bwd")
+            check(lib.mac_activation_bwd(ptr(hidden), ptr(dh), act_code(c.controlContAct, c.relu), ptr(dpre), B * d,
+                                         stream_ptr()), "act bwd")
             dy = dpre
         nW, nb = self.lin_names(sc, "contControl")
         dci = self.e(B, d)
@@ -277,9 +257,8 @@ class _Bwd(object):
         B, d = self.B, self.d
         u = cell._u_saved
         dpre = self.e(B, d)
-        act = c.controlInputAct
-        code = ACT["ELU"] if (act == "RELU" and c.relu == "ELU") else ACT["RELU_STD"] if act == "RELU" else ACT[act]
-        check(lib.mac_activation_bwd(ptr(u), ptr(du), code, ptr(dpre), B * d, stream_ptr()), "act bwd")
+        check(lib.mac_activation_bwd(ptr(u), ptr(du), act_code(c.controlInputAct, c.relu), ptr(dpre), B * d, stream_ptr()),
+              "act bwd")
         nW, nb = self.lin_names("MACCell/", "qInput")
         self.linear_bwd([cell.vecQuestions], nW, nb, dpre, [dq], [1])
         # ---------------- initial state (mac_cell.py:496-505)

@@ -117,8 +117,6 @@ def load_training_state(path, trainer):
         dst.copy_(torch.from_numpy(host))
     trainer.step_id = int(z["mac_b200/step"])
     p.touch()                      # packed / transposed / bf16 copies of the old weights are stale
-    if getattr(trainer, "out", None) is not None:
-        trainer.out.invalidate()
     return trainer.step_id
 
 

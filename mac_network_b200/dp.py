@@ -179,7 +179,6 @@ class DPTrainer(object):
         from .autograd import mac_backward
         from .mac_cell import mac_network
         cell = self.cell_for(key, batch)
-        cell._rw.clear()
         # per-(step, rank) dropout stream: masks differ across ranks and steps, reproducibly
         cell.seed = (self.base_seed * 1000003 + self.step_id * 7919 + self.rank * 104729 + 1) & 0x7FFFFFFFFFFFFFFF
         control, memory = mac_network(cell, self.L)
@@ -205,7 +204,6 @@ class DPTrainer(object):
         from .autograd import mac_backward
         from .mac_cell import mac_network
         cell = self.cell_for(key, batch)
-        cell._rw.clear()
         cell.seed = (self.base_seed * 1000003 + self.step_id * 7919 + self.rank * 104729 + 1) & 0x7FFFFFFFFFFFFFFF
         self.out.seed = cell.seed
         control, memory = mac_network(cell, self.L)
@@ -217,7 +215,6 @@ class DPTrainer(object):
         self.out.backward(gviews, d_mem, d_q)
         mac_backward(cell, None, d_mem, bucket=self.bucket, zero_bucket=False, d_vecq=d_q, tc=self.bwd_tc)
         self.apply()
-        self.out.invalidate()
         return logits, losses
 
     def full_forward_backward(self, key, data, global_batch):
@@ -240,7 +237,6 @@ class DPTrainer(object):
         bufs = {"vecQuestions": vecq, "questionWords": words, "questionCntxWords": cntx, "knowledgeBase": kb,
                 "questionLengths": data["questionLengths"]}
         cell = self.cell_for(key, bufs)
-        cell._rw.clear()
         cell.seed = seed
         control, memory = mac_network(cell, self.L)
         self.bucket.zero_()
@@ -260,9 +256,6 @@ class DPTrainer(object):
         """One data-parallel step of the whole model: `full_forward_backward` -> all-reduce -> clip / Adam / EMA."""
         logits, losses = self.full_forward_backward(key, data, global_batch)
         self.apply()
-        self.out.invalidate()
-        self.stem._packed.clear()
-        self.enc._packed.clear()
         return logits, losses
 
     def train_step(self, key, batch, t_control, t_memory, global_batch):

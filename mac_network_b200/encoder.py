@@ -17,13 +17,12 @@ LSTM product on wgmma tensor cores (csrc/encoder_tc.cuh: bf16 operands, fp32 acc
 the recurrence and BPTT as one persistent cluster launch each (h = 256 only).  Variable names follow the
 reference's scopes (`qEmbeddings/emb`, `encoder/birnnLayer/bidirectional_rnn/{fw,bw}/basic_lstm_cell/{kernel,bias}`)."""
 import collections
-import ctypes
 
 import numpy as np
 import torch
 
-from . import _lib
-from ._lib import check, ptr, stream_ptr
+from . import _lib, packs
+from ._lib import check, ptr, segments, stream_ptr
 
 SITE_ENC_INPUT = 48       # Philox sites of the encoder's two dropouts
 SITE_ENC_QUESTION = 49
@@ -97,8 +96,7 @@ class QuestionEncoder(object):
             raise NotImplementedError("the bf16 encoder needs h = %d hidden units per direction (encDim %d with encBi), got "
                                       "h = %d; use prec='fp32'" % (TC_H, 2 * TC_H, self.h))
         self.Ep = (self.E + 127) // 128 * 128          # E padded to whole 128-column tiles in the bf16 operands
-        self._packed = {}
-        self._version_fn, self._packed_version = version, None
+        self._cache = packs.Cache(version)
         self._lws_bytes = 4096 + 32 * 64 * 4096 * 4
         self._lws = torch.zeros(self._lws_bytes, dtype=torch.uint8, device=self.device)
         self._saved = None
@@ -109,39 +107,16 @@ class QuestionEncoder(object):
 
     def _linear(self, xs, W, b, out, n_out=None):
         n = len(xs)
-        arr_p = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
+        arr_p, arr_k, arr_ld = segments(xs)
         n_out = W.shape[1] if n_out is None else n_out
         check(self.lib.mac_linear_fwd(arr_p, arr_k, arr_ld, n, ptr(W), ptr(b), 0.0, 0, ptr(out), out.stride(0),
                                       xs[0].shape[0], n_out, ptr(self._lws), self._lws_bytes, stream_ptr()), "mac_linear_fwd")
         return out
 
-    def _linear_bwd(self, xs, Wt, dy, dxs, dx_accum, dW, db):
-        n = len(xs)
-        arr_p = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
-        arr_dx = (ctypes.c_void_p * n)(*[None if t is None else t.data_ptr() for t in dxs])
-        arr_lddx = (ctypes.c_int * n)(*[0 if t is None else t.stride(0) for t in dxs])
-        arr_acc = (ctypes.c_int * n)(*[int(a) for a in dx_accum])
-        check(self.lib.mac_linear_bwd(arr_p, arr_k, arr_ld, n, ptr(Wt), ptr(dy), dy.stride(0), arr_dx, arr_lddx, arr_acc,
-                                      ptr(dW), ptr(db), xs[0].shape[0], dy.shape[1], ptr(self._lws), self._lws_bytes,
-                                      stream_ptr()), "mac_linear_bwd")
-
     def _wx_pack(self, i):
         """bf16 [4h, Ep] pack of kernel[0:E] of direction i (zero columns E..Ep-1), cached per parameter version."""
-        v = self._version_fn() if self._version_fn is not None else None
-        if v != self._packed_version:
-            self._packed.clear()
-            self._packed_version = v
-        if i not in self._packed:
-            K = self.p[self.scopes[i] + "basic_lstm_cell/kernel"]
-            Wt = torch.empty((4 * self.h, self.Ep), dtype=torch.bfloat16, device=self.device)
-            check(self.lib.mac_pack_weight_bf16_kpad(ptr(K), ptr(Wt), self.E, self.Ep, 4 * self.h, stream_ptr()),
-                  "mac_pack_weight_bf16_kpad")
-            self._packed[i] = Wt
-        return self._packed[i]
+        return self._cache.pack(packs.bf16_kpad, self.p[self.scopes[i] + "basic_lstm_cell/kernel"][:self.E], self.Ep,
+                                stream=stream_ptr())
 
     def _lstm_bf16(self, qIndices, lengths, step, save_for_backward):
         """Embedding + both LSTM directions on tensor cores: (words, x16, cntx, vecq, sg, sc, shp)."""
@@ -239,10 +214,12 @@ class QuestionEncoder(object):
         if self.proj:
             Wc, Wq = self.p["encoder/linearLayerprojCW/weights/weight"], self.p["encoder/linearLayerprojQ/weights/weight"]
             dc, dq = self._new(B * S, nd * h), self._new(B, nd * h)
-            self._linear_bwd([sv["cntx"].view(B * S, nd * h)], Wc.t().contiguous(), d_cntx.view(B * S, -1), [dc], [0],
-                             grads["encoder/linearLayerprojCW/weights/weight"], grads["encoder/linearLayerprojCW/biases/bias"])
-            self._linear_bwd([sv["vecq"]], Wq.t().contiguous(), d_vecq, [dq], [0],
-                             grads["encoder/linearLayerprojQ/weights/weight"], grads["encoder/linearLayerprojQ/biases/bias"])
+            _lib.linear_bwd([sv["cntx"].view(B * S, nd * h)], Wc.t().contiguous(), d_cntx.view(B * S, -1), [dc], [0],
+                            grads["encoder/linearLayerprojCW/weights/weight"], grads["encoder/linearLayerprojCW/biases/bias"],
+                            self._lws, self._lws_bytes, stream_ptr())
+            _lib.linear_bwd([sv["vecq"]], Wq.t().contiguous(), d_vecq, [dq], [0],
+                            grads["encoder/linearLayerprojQ/weights/weight"], grads["encoder/linearLayerprojQ/biases/bias"],
+                            self._lws, self._lws_bytes, stream_ptr())
             d_cntx, d_vecq = dc.view(B, S, nd * h), dq
         if self.keep_question < 1.0:                 # gradient through tf.nn.dropout: the same mask and 1/keep
             dq = self._new(B, nd * h)
@@ -273,8 +250,9 @@ class QuestionEncoder(object):
         dx = self._new(B * S, E)
         for i, sc in enumerate(self.scopes):
             # dKernel += [dropout(X), h_prev]^T @ dG;  dBias += colsum(dG);  dX (+)= dG @ kernel[0:E]^T
-            self._linear_bwd([sv["x2"], sv["shp"][i]], Ks[i].t().contiguous(), dG[i], [dx, None], [1 if i else 0, 0],
-                             grads[sc + "basic_lstm_cell/kernel"], grads[sc + "basic_lstm_cell/bias"])
+            _lib.linear_bwd([sv["x2"], sv["shp"][i]], Ks[i].t().contiguous(), dG[i], [dx, None], [1 if i else 0, 0],
+                            grads[sc + "basic_lstm_cell/kernel"], grads[sc + "basic_lstm_cell/bias"], self._lws,
+                            self._lws_bytes, stream_ptr())
         check(self.lib.mac_embed_bwd(ptr(dx), ptr(sv["qIndices"]), self.keep_input, self.seed, SITE_ENC_INPUT, sv["step"],
                                      ptr(grads["qEmbeddings/emb"]), B, S, self.V, E, stream_ptr()), "mac_embed_bwd")
 

@@ -24,8 +24,8 @@ import ctypes
 import numpy as np
 import torch
 
-from . import _lib
-from ._lib import ACT, PREC, ReadWeights, check, ptr, stream_ptr
+from . import _lib, packs
+from ._lib import PREC, ReadWeights, act_code, check, ptr, segments, stream_ptr
 from .config import MACConfig
 from .params import PREFIX, init_params, param_specs
 
@@ -92,7 +92,7 @@ class MACParams(object):
             view.copy_(torch.from_numpy(np.ascontiguousarray(v).reshape(view.shape)))
             self.t[name] = view
         self.version = 0
-        self._derived = {}
+        self.cache = packs.Cache()          # weight-derived tensors of this version: packs, transposes, folded weights
 
     def __getitem__(self, name):
         return self.t[PREFIX + name]
@@ -108,18 +108,22 @@ class MACParams(object):
         return collections.OrderedDict((k, v.detach().cpu().numpy()) for k, v in self.t.items())
 
     def touch(self):
-        """Call after updating parameter values in place (optimizer step): drops packed/bf16 copies."""
+        """Call after updating parameter values in place (optimizer step, checkpoint restore): moves `version` and drops
+        every weight-derived tensor."""
         self.version += 1
-        self._derived.clear()
-
-    def derived(self, key, fn):
-        if key not in self._derived:
-            self._derived[key] = fn()
-        return self._derived[key]
+        self.cache.clear()
 
     def scalar(self, name):
         """0-d bias of an outDim == 1 linear (ops.py:304-305) as a python float (read once, cached)."""
-        return self.derived(("scalar", name), lambda: float(self[name].item()))
+        return self.cache.get(("scalar", name), lambda: float(self[name].item()))
+
+    def q_input_cat(self):
+        """([d, L*d], [L*d]): the per-step qInput{i} weights and biases side by side (controlInputUnshared), so that the
+        control inputs of all steps are one product."""
+        def build():
+            Ws = [self.lin("MACCell/", "qInput%d" % i) for i in range(self.L)]
+            return torch.cat([w for w, _ in Ws], dim=1).contiguous(), torch.cat([b for _, b in Ws]).contiguous()
+        return self.cache.get("qInputCat", build)
 
 
 class _Workspaces(object):
@@ -183,7 +187,6 @@ class MACCell(object):
         self.ws = _Workspaces(self.lib, B, N, d, self.prec, self.device)
         self._hoist = (not (c.controlFeedPrev or c.controlWholeQ or c.controlContinuous or c.unsharedCells)
                        and self._fused_control)
-        self._rw = {}
         self._read_inv = {}
         # eval-mode hoist of the step-invariant read projections (shared cells only)
         self._read_hoist = self._fused_read and not c.unsharedCells and not save_for_backward
@@ -273,18 +276,18 @@ class MACCell(object):
         of the composed read unit over the B*N knowledge-base rows -- on tensor cores with prec="bf16"."""
         n = len(xs)
         M = xs[0].shape[0]
-        arr_p = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
-        code = ACT["ELU"] if (act == "RELU" and self.cfg.relu == "ELU") else ACT["RELU_STD"] if act == "RELU" else ACT[act]
+        arr_p, arr_k, arr_ld = segments(xs)
+        code = act_code(act, self.cfg.relu)
         if bn_rows and self._tc_general:
             K = sum(x.shape[1] for x in xs)
             need = int(self.lib.mac_linear_tc_seg_workspace_bytes(M, K))
             if self._lin_tc_ws is None or self._lin_tc_ws.numel() < need:
                 self._lin_tc_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-            check(self.lib.mac_linear_tc_seg_fwd(arr_p, arr_k, arr_ld, n, ptr(self._bf16_weight(W)), ptr(b),
-                                                 float(bias_const), code, ptr(out), out.stride(0), M, W.shape[1],
-                                                 ptr(self._lin_tc_ws), self._lin_tc_ws.numel(), stream_ptr()),
+            s = stream_ptr()
+            W16 = self.params.cache.pack(packs.bf16, W, stream=s)
+            check(self.lib.mac_linear_tc_seg_fwd(arr_p, arr_k, arr_ld, n, ptr(W16), ptr(b), float(bias_const), code,
+                                                 ptr(out), out.stride(0), M, W.shape[1], ptr(self._lin_tc_ws),
+                                                 self._lin_tc_ws.numel(), s),
                   "mac_linear_tc_seg_fwd")
         else:
             check(self.lib.mac_linear_fwd(arr_p, arr_k, arr_ld, n, ptr(W), ptr(b), float(bias_const), code, ptr(out),
@@ -294,35 +297,17 @@ class MACCell(object):
             self._tape.linear(xs, W, b, out, code, bn_rows=bn_rows)
         return out
 
-    def _bf16_weight(self, W):
-        """bf16 [out, in] pack of an fp32 [in, out] weight (mac_pack_weight_bf16), cached per parameter version."""
-        def pack():
-            o = torch.empty((W.shape[1], W.shape[0]), dtype=torch.bfloat16, device=W.device)
-            check(self.lib.mac_pack_weight_bf16(ptr(W), ptr(o), W.shape[0], W.shape[1], stream_ptr()), "pack")
-            return o
-        return self.params.derived(("bf16lin", W.data_ptr()), pack)
-
-    def _split_weight(self, key, W):
-        """bf16 hi / lo halves [out, in] of an fp32 [in, out] weight (mac_pack_weight_bf16_split), cached per parameter version."""
-        def build():
-            hi = torch.empty((W.shape[1], W.shape[0]), dtype=torch.bfloat16, device=W.device)
-            lo = torch.empty_like(hi)
-            check(self.lib.mac_pack_weight_bf16_split(ptr(W), ptr(hi), ptr(lo), W.shape[0], W.shape[1], stream_ptr()), "pack_split")
-            return hi, lo
-        return self.params.derived(("split16", key), build)
-
-    def _linear_tc(self, xs, key, W, b, out, act="NON", bias_const=0.0, y2=None, n_split=0, gate=None):
+    def _linear_tc(self, xs, W, b, out, act="NON", bias_const=0.0, y2=None, n_split=0, gate=None):
         """ops.linear on [M <= 128, sum k] segments as a three-pass split-bf16 wgmma product (mac_linear_tc_small_fwd).
         `gate` = (new, old, z_out): the write gate epilogue (mac_cell.py:358-367)."""
         n = len(xs)
-        hi, lo = self._split_weight(key, W)
-        arr_p = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
+        s = stream_ptr()
+        hi, lo = self.params.cache.pack(packs.bf16_split, W, stream=s)
+        arr_p, arr_k, arr_ld = segments(xs)
         gn, go, gz = gate if gate is not None else (None, None, None)
         check(self.lib.mac_linear_tc_small_fwd(arr_p, arr_k, arr_ld, n, ptr(hi), ptr(lo), ptr(b), float(bias_const),
-                                               self._act_code(act), ptr(out), out.stride(0), ptr(y2), int(n_split), ptr(gn),
-                                               ptr(go), ptr(gz), xs[0].shape[0], W.shape[1], stream_ptr()),
+                                               act_code(act, self.cfg.relu), ptr(out), out.stride(0), ptr(y2), int(n_split),
+                                               ptr(gn), ptr(go), ptr(gz), xs[0].shape[0], W.shape[1], s),
               "mac_linear_tc_small_fwd")
         return out
 
@@ -423,10 +408,7 @@ class MACCell(object):
         c, B, d, L = self.cfg, self.B, self.d, self.L
         u = self._question_input()
         if c.controlInputUnshared:
-            def pack():
-                Ws = [self.params.lin("MACCell/", "qInput%d" % i) for i in range(L)]
-                return (torch.cat([w for w, _ in Ws], dim=1).contiguous(), torch.cat([b for _, b in Ws]).contiguous())
-            Wc, bc = self.params.derived("qInputCat", pack)
+            Wc, bc = self.params.q_input_cat()
             self._ci = self._linear([u], Wc, bc, self._new(B, L * d))              # [B, L*d]: ci_i = [:, i*d:(i+1)*d]
             cc_t, cc_b = d, L * d
         else:
@@ -486,9 +468,14 @@ class MACCell(object):
 
     # ------------------------------------------------------------------ read unit
     def _read_weights(self, name):
-        if name in self._rw:
-            return self._rw[name]
-        p, sc = self.params, "MACCell/read" + name + "/"
+        """The read unit's weights as the library reads them, with the packs of this cell's precision.  An entry of the
+        parameters' cache, so it is rebuilt together with the packs it points into whenever the values move."""
+        return self.params.cache.get(("ReadWeights", name, self.prec, self.save_for_backward),
+                                     lambda: self._build_read_weights(name))
+
+    def _build_read_weights(self, name):
+        p, sc, d, s = self.params, "MACCell/read" + name + "/", self.d, stream_ptr()
+        pack = lambda builder, W: p.cache.pack(builder, W, stream=s)
         Wx, bx = p.lin(sc + "mulmemInter/", "projX")
         Wy, by = p.lin(sc + "mulmemInter/", "projY")
         Wm, bm = p.lin(sc, "memKbProj")
@@ -498,32 +485,15 @@ class MACCell(object):
                          Wm2.data_ptr(), bm2.data_ptr(), p[lsc + "weights/weight"].data_ptr(),
                          p.scalar(lsc + "biases/bias"), None, None, None)
         if self.prec in (PREC["bf16"], PREC["fp8"]):     # fp8: P and Q are the bf16 path's (mac_read_invariant)
-            def pack(t):       # fp32 [in, out] -> bf16 [out, in] (K-major B operand of wgmma)
-                o = torch.empty((t.shape[1], t.shape[0]), dtype=torch.bfloat16, device=t.device)
-                check(self.lib.mac_pack_weight_bf16(ptr(t), ptr(o), t.shape[0], t.shape[1], stream_ptr()), "pack")
-                return o
-            keep = p.derived(("bf16", sc), lambda: (pack(Wx), pack(Wm), pack(Wm2)))
-            rw.Wx_bf16, rw.Wm_bf16, rw.Wm2_bf16 = (t.data_ptr() for t in keep)
+            rw.Wx_bf16, rw.Wm_bf16, rw.Wm2_bf16 = (pack(packs.bf16, t).data_ptr() for t in (Wx, Wm, Wm2))
         if self.prec == PREC["tc32"]:
-            def pack3(t):      # fp32 [in, out] -> bf16 [out, 3*in] = [hi | hi | lo]
-                o = torch.empty((t.shape[1], 3 * t.shape[0]), dtype=torch.bfloat16, device=t.device)
-                check(self.lib.mac_pack_weight_split3(ptr(t), ptr(o), t.shape[0], t.shape[1], stream_ptr()), "pack3")
-                return o
-            d_ = self.d
-            keep3 = p.derived(("split3", sc), lambda: (pack3(Wx), pack3(Wm[:d_]), pack3(Wm[d_:]), pack3(Wm2)))
-            rw.Wx_s3, rw.Wma_s3, rw.Wmb_s3, rw.Wm2_s3 = (t.data_ptr() for t in keep3)
+            rw.Wx_s3, rw.Wma_s3, rw.Wmb_s3, rw.Wm2_s3 = (pack(packs.split3, t).data_ptr()
+                                                         for t in (Wx, Wm[:d], Wm[d:], Wm2))
             if self.save_for_backward:   # training form: H = ELU([P*y | P] @ Wm + bm) as one product over K = 2d
-                rw.Wm_s3 = p.derived(("split3_wm", sc), lambda: pack3(Wm)).data_ptr()
+                rw.Wm_s3 = pack(packs.split3, Wm).data_ptr()
         if self.prec == PREC["fp8"]:
-            def pack8(t):      # fp32 [in, out] -> e4m3 [out, in] and the fp32 scale of each output column
-                o = torch.empty((t.shape[1], t.shape[0]), dtype=torch.uint8, device=t.device)
-                s_ = torch.empty(t.shape[1], dtype=torch.float32, device=t.device)
-                check(self.lib.mac_pack_weight_fp8(ptr(t), ptr(o), ptr(s_), t.shape[0], t.shape[1], stream_ptr()), "pack8")
-                return o, s_
-            d_ = self.d
-            keep8 = p.derived(("fp8", sc), lambda: pack8(Wm[:d_]) + pack8(Wm2))
-            rw.Wm_fp8, rw.Wm_fp8_scale, rw.Wm2_fp8, rw.Wm2_fp8_scale = (t.data_ptr() for t in keep8)
-        self._rw[name] = rw
+            (w8, s8), (w8_2, s8_2) = pack(packs.fp8, Wm[:d]), pack(packs.fp8, Wm2)
+            rw.Wm_fp8, rw.Wm_fp8_scale, rw.Wm2_fp8, rw.Wm2_fp8_scale = (t.data_ptr() for t in (w8, s8, w8_2, s8_2))
         return rw
 
     def read(self, knowledgeBase, memory, control, name="", reuse=None, _att_out=None, _out=None, _save=None,
@@ -557,7 +527,7 @@ class MACCell(object):
                 self._read_inv[name] = inv
             if _y_pre is None and self._small_tc:
                 Wy, by = self.params.lin("MACCell/read" + name + "/mulmemInter/", "projY")
-                _y_pre = self._linear_tc([memory], ("projY", name), Wy, by, self._y_next)
+                _y_pre = self._linear_tc([memory], Wy, by, self._y_next)
             check(self.lib.mac_read_fwd_inv(kb32, ptr(self.kb_bf16), ptr(self._read_inv[name]), ptr(_y_pre),
                                             ptr(memory), ptr(control), ctypes.byref(rw), self.prec, ptr(info), ptr(att),
                                             ptr(self.ws.read), self.ws.read_bytes, B, N, d, stream_ptr()),
@@ -588,7 +558,7 @@ class MACCell(object):
             self._linear([Ww], Wy, None, Wf[:, d:])                       # Ww @ Wy        (ldy = 2d)
             self._linear([bw.view(1, d)], Wy, by, bf[d:].view(1, d))      # bw @ Wy + by
             return Wf, bf
-        return self.params.derived(("foldY", name), build)
+        return self.params.cache.get(("foldY", name), build)
 
     def write(self, memory, info, control, contControl=None, name="", reuse=None, _out=None, _gate_out=None,
               _y_next=None):
@@ -624,7 +594,7 @@ class MACCell(object):
         if _y_next is not None and self._small_tc:
             Wf, bf = self._folded_write_weights(name)
             out = _out if _out is not None else self._new(B, d)
-            return self._linear_tc([memory, info], ("foldY", name), Wf, bf, out, y2=_y_next, n_split=d)
+            return self._linear_tc([memory, info], Wf, bf, out, y2=_y_next, n_split=d)
         if _y_next is not None:
             Wf, bf = self._folded_write_weights(name)
             out = _out if _out is not None else self._new(B, d)
@@ -638,7 +608,7 @@ class MACCell(object):
             W, b = self.params.lin(sc, "ctrlProj")
             keep = self.save_for_backward
             if self._small_tc:
-                selfControl = self._linear_tc([selfControl], ("ctrlProj", name), W, b, self._new(B, d))
+                selfControl = self._linear_tc([selfControl], W, b, self._new(B, d))
             else:
                 selfControl = self._linear([selfControl], W, b, self._sc[i] if keep else self._new(B, d))
             lsc = sc + "inter2attselfAttention/inter2logits/linearLayerlogits/"
@@ -661,12 +631,12 @@ class MACCell(object):
         if self._small_tc:
             segs = [memory, info] + ([selfSmry] if selfSmry is not None else [])
             if c.writeGate:
-                mnew = self._linear_tc(segs, ("newMemory", name), Ww, bw, self._new(B, d))
-                self._linear_tc([control], ("gate", name), Wg, bg, out, bias_const=float(c.writeGateBias),
+                mnew = self._linear_tc(segs, Ww, bw, self._new(B, d))
+                self._linear_tc([control], Wg, bg, out, bias_const=float(c.writeGateBias),
                                 gate=(mnew, memory, gate))
                 self.attentions["gate"].append(gate)
             else:
-                self._linear_tc(segs, ("newMemory", name), Ww, bw, out)
+                self._linear_tc(segs, Ww, bw, out)
             return out
         check(self.lib.mac_write_fwd(ptr(memory), ptr(info), ptr(selfSmry), ptr(control), ptr(Ww), ptr(bw), ptr(Wg),
                                      ptr(bg), float(c.writeGateBias), ptr(out), ptr(gate), ptr(self.ws.write),
@@ -681,9 +651,6 @@ class MACCell(object):
         return out
 
     # ------------------------------------------------------------------ general (composed) path
-    def _act_code(self, act):
-        return ACT["ELU"] if (act == "RELU" and self.cfg.relu == "ELU") else ACT["RELU_STD"] if act == "RELU" else ACT[act]
-
     def _ops_linear(self, xs, scope, name, act="NON", bias_const=0.0, bn_rows=False):
         """ops.linear incl. the nested "<name>_2" layer when act != NON (ops.py:298-333); xs: list of 2-D segments."""
         W, b = self.params.lin(scope, name)
@@ -697,9 +664,7 @@ class MACCell(object):
         """outDim == 1 linear (vector weight, scalar bias) over concatenated segments -> [R]."""
         n, R = len(xs), xs[0].shape[0]
         out = self._new(R)
-        arr_p = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
+        arr_p, arr_k, arr_ld = segments(xs)
         check(self.lib.mac_rowdot_fwd(arr_p, arr_k, arr_ld, n, ptr(self.params[lscope + "weights/weight"]),
                                       self.params.scalar(lscope + "biases/bias"), ptr(out), R, stream_ptr()), "mac_rowdot_fwd")
         if self._tape is not None:
@@ -728,9 +693,10 @@ class MACCell(object):
         if act == "NON":
             return x
         out = self._new(*x.shape)
-        check(self.lib.mac_activation(ptr(x), self._act_code(act), ptr(out), x.numel(), stream_ptr()), "mac_activation")
+        code = act_code(act, self.cfg.relu)
+        check(self.lib.mac_activation(ptr(x), code, ptr(out), x.numel(), stream_ptr()), "mac_activation")
         if self._tape is not None:
-            self._tape.act(x, out, self._act_code(act))
+            self._tape.act(x, out, code)
         return out
 
     def _mul_general(self, x2d, y, dim, N, scope, name, proj, inter_mod, concat_x, concat_proj):

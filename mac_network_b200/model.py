@@ -104,9 +104,6 @@ class MACnet(object):
         t.params.flat.copy_(t.ema)
         t.ema.copy_(tmp)
         t.params.touch()
-        self._out.invalidate()
-        self._stem._packed.clear()
-        self._enc._packed.clear()
 
     # ------------------------------------------------------------------ model.py:732-760
     def runBatch(self, sess, data, images, train, getAtt=False):
@@ -121,9 +118,6 @@ class MACnet(object):
             logits, losses = t.train_step_full((B, S), dev, global_batch=B * t.world)
             self.macCell = t._cells[(B, S)][0]
             gradNorm = float(t.norm[0].item())
-            self._out.invalidate()
-            self._stem._packed.clear()
-            self._enc._packed.clear()
         else:
             if self.use_ema:
                 self._swap_ema()

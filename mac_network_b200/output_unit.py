@@ -10,13 +10,12 @@
 It supplies dL/dmemory and dL/dvecQuestions to the cell's backward, so data-parallel training runs on the reference's
 real loss.  Variable names follow the reference's scopes (siblings of "MACnetwork/" under "macModel/")."""
 import collections
-import ctypes
 
 import numpy as np
 import torch
 
-from . import _lib
-from ._lib import ACT, check, ptr, stream_ptr
+from . import _lib, packs
+from ._lib import act_code, check, ptr, segments, stream_ptr
 
 SITE_OUTPUT = 16          # Philox site base for the output unit's dropouts (site + layer index)
 
@@ -67,7 +66,7 @@ class OutputUnit(object):
         (`MACParams.version`): the transposed weight copies of the backward are rebuilt when it moves."""
         self.lib = _lib.load()
         self.p = params
-        self._version_fn, self._wt_version = version, None
+        self._cache = packs.Cache(version)
         self.relu, self.keep, self.seed = relu, float(keep), int(seed)
         self.nfc = len([k for k in params if k.startswith("classifier/linearLayerfc_") and k.endswith("weights/weight")])
         for k, v in params.items():
@@ -77,7 +76,6 @@ class OutputUnit(object):
         dev = next(iter(params.values())).device
         self.lws_bytes = 4096 + 32 * 64 * 2048 * 4
         self.lws = torch.zeros(self.lws_bytes, dtype=torch.uint8, device=dev)
-        self._wt = {}
 
     def _new(self, *shape):
         return torch.empty(shape, dtype=torch.float32, device=self.lws.device)
@@ -85,9 +83,7 @@ class OutputUnit(object):
     def _linear(self, xs, W, b, act=0):
         n, M = len(xs), xs[0].shape[0]
         y = self._new(M, W.shape[1])
-        arr_p = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
+        arr_p, arr_k, arr_ld = segments(xs)
         check(self.lib.mac_linear_fwd(arr_p, arr_k, arr_ld, n, ptr(W), ptr(b), 0.0, act, ptr(y), y.stride(0), M, W.shape[1],
                                       ptr(self.lws), self.lws_bytes, stream_ptr()), "mac_linear_fwd")
         return y
@@ -104,7 +100,7 @@ class OutputUnit(object):
         """Returns (logits, losses [B], dlogits [B, A]) -- dlogits = (softmax - onehot) * loss_scale (default 1/B).  The three
         stay reachable as `last_logits`, `losses` and `dlogits` (`logits` is the label-free method)."""
         B = memory.shape[0]
-        act = ACT["ELU"] if self.relu == "ELU" else ACT["RELU_STD"]
+        act = act_code("RELU", self.relu)
         self.eq = self._linear([vecQuestions], self.p["outputUnit/linearLayeroutQuestion/weights/weight"],
                                self.p["outputUnit/linearLayeroutQuestion/biases/bias"])
         self.memory, self.vecq, self.step = memory, vecQuestions, step
@@ -137,7 +133,7 @@ class OutputUnit(object):
     def logits(self, memory, vecQuestions):
         """The answer logits [B, A] without labels: the linears of `forward` with every dropout at 1, no loss, no `dlogits`,
         nothing kept for a backward.  Bit for bit `forward(...)[0]` of a unit with keep = 1."""
-        act = ACT["ELU"] if self.relu == "ELU" else ACT["RELU_STD"]
+        act = act_code("RELU", self.relu)
         eq = self._linear([vecQuestions], self.p["outputUnit/linearLayeroutQuestion/weights/weight"],
                           self.p["outputUnit/linearLayeroutQuestion/biases/bias"])
         xs = [memory, eq]
@@ -146,36 +142,15 @@ class OutputUnit(object):
                                self.p["classifier/linearLayerfc_%d/biases/bias" % i], act if i < self.nfc - 1 else 0)]
         return xs[0]
 
-    def invalidate(self):
-        """Call after the parameters were updated in place (optimizer step): drops the cached transposes."""
-        self._wt.clear()
-
-    def _wt_of(self, name):
-        v = self._version_fn() if self._version_fn is not None else None
-        if v != self._wt_version:
-            self._wt.clear()
-            self._wt_version = v
-        if name not in self._wt:
-            self._wt[name] = self.p[name].t().contiguous()
-        return self._wt[name]
-
     def backward(self, grads, d_memory, d_vecq):
         """Accumulates parameter gradients into `grads` (dict name -> tensor) and ADDS dL/dmemory, dL/dvecQuestions."""
         B = self.memory.shape[0]
         dy = self.dlogits
-        act = ACT["ELU"] if self.relu == "ELU" else ACT["RELU_STD"]
+        act = act_code("RELU", self.relu)
 
         def lin_bwd(xs, wname, bname, dy, dxs, accum):
-            n = len(xs)
-            arr_x = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-            arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-            arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
-            arr_dx = (ctypes.c_void_p * n)(*[d.data_ptr() for d in dxs])
-            arr_ldd = (ctypes.c_int * n)(*[d.stride(0) for d in dxs])
-            arr_acc = (ctypes.c_int * n)(*accum)
-            check(self.lib.mac_linear_bwd(arr_x, arr_k, arr_ld, n, ptr(self._wt_of(wname)), ptr(dy), dy.stride(0), arr_dx,
-                                          arr_ldd, arr_acc, ptr(grads[wname]), ptr(grads[bname]), dy.shape[0], dy.shape[1],
-                                          ptr(self.lws), self.lws_bytes, stream_ptr()), "mac_linear_bwd")
+            _lib.linear_bwd(xs, self._cache.pack(packs.transposed, self.p[wname]), dy, dxs, accum, grads[wname],
+                            grads[bname], self.lws, self.lws_bytes, stream_ptr())
         for i in reversed(range(self.nfc)):
             xs = self.inputs[i]
             wn, bn = "classifier/linearLayerfc_%d/weights/weight" % i, "classifier/linearLayerfc_%d/biases/bias" % i

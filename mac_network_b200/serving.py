@@ -393,7 +393,7 @@ class _ModelSlot(object):
         stream first waits for the caller's current stream: whatever wrote the parameters there (an optimizer step, a
         checkpoint restore) or built packs from them (`runBatch`) is enqueued, not necessarily done."""
         self.graph = None                   # a previous capture's memory goes back before the new one takes its own
-        self.cell = None                    # a cell holds pointers into its parameter version's packed weights
+        self.cell = None                    # built again by the eager pass below
         self.stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(self.stream):
             self.outs_dev = self._forward()

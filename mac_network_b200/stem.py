@@ -12,13 +12,12 @@ forward in e4m3: `mac_im2col3x3_fp8` (per-row scales, no dropout) and `mac_linea
 halves and three bf16 products per fp32 product (`mac_im2col3x3_split`, `mac_linear_tc32_fwd`, `mac_conv3x3_bwd_tc32`;
 the split-bf16 scheme the cell calls "tc32", DESIGN.md section 9 item 6)."""
 import collections
-import ctypes
 
 import numpy as np
 import torch
 
-from . import _lib
-from ._lib import ACT, check, ptr, stream_ptr
+from . import _lib, packs
+from ._lib import act_code, check, ptr, segments, stream_ptr
 
 SITE_STEM = 32            # Philox site base for the stem's input dropouts (site + layer index)
 INGEST_NHWC_F32, INGEST_PATCH_BF16 = 0, 1       # enum MAC_INGEST_* (include/mac_b200.h)
@@ -57,8 +56,7 @@ class Stem(object):
         self.p = params
         self.relu, self.prec, self.seed = relu, prec, int(seed)
         self.nlayers = len([k for k in params if k.endswith("kernels/kernel")])
-        self._packed = {}
-        self._version_fn, self._packed_version = version, None
+        self._cache = packs.Cache(version)
         dev = next(iter(params.values())).device
         self.device = dev
 
@@ -67,29 +65,8 @@ class Stem(object):
         [Cout, 3*9*Cin] = [hi | hi | lo]; for fp8, the e4m3 [Cout, 9*Cin] pack and its per-column scales as a pair."""
         K = self.p["stem/cnnLayercnn_%d/kernels/kernel" % i]
         W = K.reshape(-1, K.shape[3])                       # [9*Cin, Cout], row-major view of the HWIO kernel
-        if self.prec in ("bf16", "bf16x3", "fp8"):
-            v = self._version_fn() if self._version_fn is not None else None
-            if v != self._packed_version:
-                self._packed.clear()
-                self._packed_version = v
-            if i not in self._packed:
-                if self.prec == "bf16":
-                    Wt = torch.empty((W.shape[1], W.shape[0]), dtype=torch.bfloat16, device=W.device)
-                    check(self.lib.mac_pack_weight_bf16(ptr(W), ptr(Wt), W.shape[0], W.shape[1], stream_ptr()), "pack")
-                    self._packed[i] = Wt
-                elif self.prec == "bf16x3":
-                    Wt = torch.empty((W.shape[1], 3 * W.shape[0]), dtype=torch.bfloat16, device=W.device)
-                    check(self.lib.mac_pack_weight_split3(ptr(W), ptr(Wt), W.shape[0], W.shape[1], stream_ptr()),
-                          "mac_pack_weight_split3")
-                    self._packed[i] = Wt
-                else:
-                    Wt = torch.empty((W.shape[1], W.shape[0]), dtype=torch.uint8, device=W.device)
-                    sw = torch.empty(W.shape[1], dtype=torch.float32, device=W.device)
-                    check(self.lib.mac_pack_weight_fp8(ptr(W), ptr(Wt), ptr(sw), W.shape[0], W.shape[1], stream_ptr()),
-                          "mac_pack_weight_fp8")
-                    self._packed[i] = (Wt, sw)
-            return W, self._packed[i]
-        return W, None
+        build = {"bf16": packs.bf16, "bf16x3": packs.split3, "fp8": packs.fp8}.get(self.prec)
+        return W, None if build is None else self._cache.pack(build, W, stream=stream_ptr())
 
     def _check_fp8(self, in_dim, keep):
         """The e4m3 stem is the inference forward only (no dropout) with every channel count a multiple of 128 (whole
@@ -141,7 +118,7 @@ class Stem(object):
         matrix, already built; `images` then only gives the shape."""
         x = images
         B, H, Wd, C = x.shape
-        act = ACT["ELU"] if self.relu == "ELU" else ACT["RELU_STD"]
+        act = act_code("RELU", self.relu)
         if save_for_backward:
             self._check_trainable(C)
             self._saved = {"xs": [], "ys": [], "keep": float(keep), "step": int(step), "act": act}
@@ -179,9 +156,8 @@ class Stem(object):
                 check(self.lib.mac_linear_tc_fwd(ptr(cols), ptr(Wt), ptr(b), act, ptr(y), 0, M, K, Nout, stream_ptr()),
                       "mac_linear_tc_fwd")
             else:
-                arr_p = (ctypes.c_void_p * 1)(cols.data_ptr())
-                arr_k = (ctypes.c_int * 1)(K)
-                check(self.lib.mac_linear_fwd(arr_p, arr_k, arr_k, 1, ptr(W), ptr(b), 0.0, act, ptr(y), Nout, M, Nout, None,
+                arr_p, arr_k, arr_ld = segments([cols])
+                check(self.lib.mac_linear_fwd(arr_p, arr_k, arr_ld, 1, ptr(W), ptr(b), 0.0, act, ptr(y), Nout, M, Nout, None,
                                               0, stream_ptr()), "mac_linear_fwd")
             if save_for_backward:
                 self._saved["ys"].append(y)
@@ -256,12 +232,8 @@ class Stem(object):
             need_dx = need_d_images or i > 0
             dcols = torch.empty((M, K), dtype=torch.float32, device=self.device) if need_dx else None
             Wt = W.t().contiguous() if need_dx else None
-            one = lambda v, t=ctypes.c_int: (t * 1)(v)
-            check(self.lib.mac_linear_bwd(one(cols.data_ptr(), ctypes.c_void_p), one(K), one(K), 1, ptr(Wt), ptr(dz), Nout,
-                                          one(None if dcols is None else dcols.data_ptr(), ctypes.c_void_p), one(K), one(0),
-                                          ptr(grads["stem/cnnLayercnn_%d/kernels/kernel" % i]),
-                                          ptr(grads["stem/cnnLayercnn_%d/biases/bias" % i]), M, Nout, None, 0, stream_ptr()),
-                  "mac_linear_bwd")
+            _lib.linear_bwd([cols], Wt, dz, [dcols], [0], grads["stem/cnnLayercnn_%d/kernels/kernel" % i],
+                            grads["stem/cnnLayercnn_%d/biases/bias" % i], None, 0, stream_ptr())
             if need_dx:
                 dx = torch.empty_like(x)
                 check(self.lib.mac_col2im3x3(ptr(dcols), ptr(dx), sv["keep"], self.seed, SITE_STEM + i, sv["step"], B, H, Wd,

@@ -17,7 +17,8 @@ import ctypes
 
 import torch
 
-from ._lib import ACT, check, ptr, stream_ptr
+from . import _lib, packs
+from ._lib import ACT, check, ptr, segments, stream_ptr
 from .autograd import read_bwd, read_bwd_workspace_bytes
 from .params import PREFIX
 
@@ -79,28 +80,16 @@ class Tape(object):
         check(self.lib.mac_colsum(ptr(part), ptr(out_flat), 1, Bp, d, 1, stream_ptr()), "mac_colsum")
 
     def linear_bwd(self, xs, W, wname, bname, dy, dxs):
-        n = len(xs)
-        Wt = self.p.derived(("T", wname), lambda: W.t().contiguous()) if any(d is not None for d in dxs) else None
-        M, n_out = dy.shape
-        arr_x = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
-        arr_dx = (ctypes.c_void_p * n)(*[(d.data_ptr() if d is not None else None) for d in dxs])
-        arr_ldd = (ctypes.c_int * n)(*[(d.stride(0) if d is not None else 0) for d in dxs])
-        arr_acc = (ctypes.c_int * n)(*[1] * n)
-        check(self.lib.mac_linear_bwd(arr_x, arr_k, arr_ld, n, ptr(Wt), ptr(dy), dy.stride(0), arr_dx, arr_ldd, arr_acc,
-                                      ptr(self.G(wname)), ptr(self.G(bname)) if bname else None, M, n_out,
-                                      ptr(self.lws), self.lws_bytes, stream_ptr()), "mac_linear_bwd")
+        Wt = self.p.cache.pack(packs.transposed, W) if any(d is not None for d in dxs) else None
+        _lib.linear_bwd(xs, Wt, dy, dxs, [1] * len(xs), self.G(wname), self.G(bname) if bname else None, self.lws,
+                        self.lws_bytes, stream_ptr())
 
     def linear_bwd_tc(self, xs, W, wname, bname, dy, dxs):
         """linear_bwd with bf16 operands on tensor cores (mac_linear_bwd_tc): the composed read unit's [B*N, .] products."""
         n = len(xs)
         M, n_out = dy.shape
-        arr_x = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-        arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-        arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
-        arr_dx = (ctypes.c_void_p * n)(*[d.data_ptr() for d in dxs])
-        arr_ldd = (ctypes.c_int * n)(*[d.stride(0) for d in dxs])
+        arr_x, arr_k, arr_ld = segments(xs)
+        arr_dx, _, arr_ldd = segments(dxs)
         arr_acc = (ctypes.c_int * n)(*[1] * n)
         need = int(self.lib.mac_linear_bwd_tc_workspace_bytes(M, arr_k, n, n_out))
         if self._tcws is None or self._tcws.numel() < need:
@@ -161,12 +150,8 @@ class Tape(object):
             ktot = sum(x.shape[1] for x in xs)
             nbytes = int(self.lib.mac_rowdot_bwd_workspace_bytes(R, ktot))
             ws = torch.empty(nbytes, dtype=torch.uint8, device=self.dev)
-            dxs = [self.grad(x) for x in xs]
-            arr_x = (ctypes.c_void_p * n)(*[x.data_ptr() for x in xs])
-            arr_k = (ctypes.c_int * n)(*[x.shape[1] for x in xs])
-            arr_ld = (ctypes.c_int * n)(*[x.stride(0) for x in xs])
-            arr_dx = (ctypes.c_void_p * n)(*[d.data_ptr() for d in dxs])
-            arr_ldd = (ctypes.c_int * n)(*[d.stride(0) for d in dxs])
+            arr_x, arr_k, arr_ld = segments(xs)
+            arr_dx, _, arr_ldd = segments([self.grad(x) for x in xs])
             check(self.lib.mac_rowdot_bwd(arr_x, arr_k, arr_ld, n, ptr(w), ptr(self.grad(out)), arr_dx, arr_ldd,
                                           ptr(self.G(wname)), ptr(self.G(bname)), ptr(ws), nbytes, R, stream_ptr()),
                   "mac_rowdot_bwd")
@@ -296,7 +281,7 @@ class Tape(object):
             nWm, nbm = lin_names(rsc, "memKbProj")
             nWm2, nbm2 = lin_names(rsc + "linearLayermemKbProj/", "memKbProj_2")
             wnames = {"Wx": nWx, "Wy": nWy, "Wm": nWm, "Wm2": nWm2}
-            Wt = lambda k: self.p.derived(("T", wnames[k]), lambda: self.p.t[wnames[k]].t().contiguous())
+            Wt = lambda k: self.p.cache.pack(packs.transposed, self.p.t[wnames[k]])
             part = {k: self.z(B, d) for k in ("wr", "bx", "bm", "bm2")}
             dbr = self.z(B)
             dmem_in = self.e(B, d)

@@ -201,9 +201,6 @@ def test_full_model_p2_bf16_matches_its_fp32_twin():
         torch.cuda.synchronize()
         bucket = tr.bucket.double().cpu()
         tr.apply()
-        tr.out.invalidate()
-        tr.stem._packed.clear()
-        tr.enc._packed.clear()
         _, losses2 = tr.train_step_full("t", dev, global_batch=B)
         torch.cuda.synchronize()
         res[prec] = (float(losses.double().mean()), bucket, float(losses2.double().mean()))

@@ -34,7 +34,8 @@ def test_stem_bf16x3_forward_calls_and_pack_cache(monkeypatch):
     assert kb.shape == (2, 35, 256)
     assert [n for n, _ in rec.log] == ["mac_pack_weight_split3", "mac_im2col3x3_split", "mac_linear_tc32_fwd"] * 2
     assert [a[2:4] for a in rec.args_of("mac_pack_weight_split3")] == [(9 * 128, 256), (9 * 256, 256)]
-    assert st._packed[0].shape == (256, 3 * 9 * 128) and st._packed[0].dtype == torch.bfloat16
+    _, W3 = st._weights(0)
+    assert W3.shape == (256, 3 * 9 * 128) and W3.dtype == torch.bfloat16
     im = rec.args_of("mac_im2col3x3_split")
     assert [a[-5:-1] for a in im] == [(2, 5, 7, 128), (2, 5, 7, 256)]
     assert [a[4] for a in im] == [SITE_STEM, SITE_STEM + 1] and all(a[2] == pytest.approx(0.82) and a[5] == 3 for a in im)

@@ -89,7 +89,7 @@ def test_stem_fp8_host_calls(monkeypatch):
     version[0] += 1
     st.forward(torch.zeros(2, 5, 7, 128))
     assert mock.calls.count("mac_pack_weight_fp8") == 4                  # a parameter update repacks both layers
-    st._packed.clear()                                                   # what MACnet._swap_ema does
+    version[0] += 1                                                      # as MACnet._swap_ema's touch() does
     st.forward(torch.zeros(2, 5, 7, 128))
     assert mock.calls.count("mac_pack_weight_fp8") == 6
 

@@ -65,11 +65,9 @@ def test_wm_s3_is_cached_and_repacked_after_touch(rec):
     mac_network(cell, L)
     assert len(whole()) == 1
     rec.log.clear()
-    cell._rw.clear()
     mac_network(cell, L)
     assert whole() == []
     cell.params.touch()
-    cell._rw.clear()
     rec.log.clear()
     mac_network(cell, L)
     assert len(whole()) == 1
