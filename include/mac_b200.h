@@ -458,6 +458,16 @@ int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float keep, uint64_
  * bf16 -> patches), else MAC_ERR_UNSUPPORTED; B <= 65535.  All checks precede any launch. */
 enum { MAC_INGEST_NHWC_F32 = 0, MAC_INGEST_PATCH_BF16 = 1 };
 int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mode, int B, int C, int H, int W, mac_stream_t stream);
+/* Knowledge bases of B questions about U distinct images (csrc/ingest.cuh; MACCell(kbIndex=), serving.ModelPipeline(images=)):
+ *   out[b, n, :] = kb_u[index[b], n, :]   for b < B
+ * kb_u: the stem's fp32 output for the U images, [U, N, d]; index: int32 [B] in device memory; out: fp32 [B, N, d], or with
+ * out_bf16 = 1 bf16 rounded to nearest even, bit for bit what mac_cast_bf16 makes of the fp32 rows.  A row whose index lies
+ * outside [0, U) is written as NaN and nothing is read for it.  Reads each used kb_u row once per question that uses it
+ * (repeats come from L2) and writes every out row once, 16-byte accesses.  Before any launch: a null pointer or B, U, N,
+ * d <= 0 -> MAC_ERR_INVALID; out_bf16 not 0 or 1, d % 8 != 0 or N*d/8 > 2^31 - 1 -> MAC_ERR_UNSUPPORTED; kb_u, index or
+ * out not 16-byte aligned -> MAC_ERR_ALIGN. */
+int mac_kb_gather(const float* kb_u, const int32_t* index, void* out, int out_bf16, int B, int U, int N, int d,
+                  mac_stream_t stream);
 /* Inference stem layer in e4m3 (csrc/tc_gemm_fp8.cuh; Stem(prec="fp8")), no dropout.  All scales fp32; e4m3 rounds to nearest
  * even and saturates at +-448.
  * mac_im2col3x3_fp8: the patch matrix of mac_im2col3x3 (same tap-major, channel-fastest layout) as e4m3 cols_e4m3 [M, 9C],

@@ -120,4 +120,60 @@ static inline size_t ingest_smem_bytes(int x_bf16, int mode, int HW) {
   return mode ? IngestShape<float, true>::smem_bytes(HW) : IngestShape<float, false>::smem_bytes(HW);
 }
 
+// ------------------------------------------------------------------------------------------------ knowledge-base gather
+// Several questions about one image: the stem runs once per distinct image, kb_u [U, N*d] fp32, and each question's knowledge
+// base is gathered from it, out[b] = kb_u[index[b]] (fp32, or bf16 rounded to nearest even as cast_bf16_kernel rounds).  A
+// sample's N*d elements are contiguous in both, so the gather is a copy of B runs of N*d elements: blockIdx.x cuts a run
+// into GATHER_V-element vectors (two 16-byte loads each), blockIdx.y (striding by gridDim.y past 65535) picks the sample.
+// An index outside [0, U) writes a NaN row and reads nothing.
+constexpr int GATHER_THREADS = 256;
+constexpr int GATHER_V = 8;                 // elements per thread: 32 bytes read, 16 (bf16) or 32 (fp32) written
+
+template <bool BF16>
+__global__ void __launch_bounds__(GATHER_THREADS) kb_gather_kernel(const float4* __restrict__ kb_u,
+                                                                   const int* __restrict__ index, void* __restrict__ out,
+                                                                   int B, int U, int nvec) {
+  const int j = blockIdx.x * GATHER_THREADS + threadIdx.x;          // vector within the sample's run
+  if (j >= nvec) return;
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const int u = __ldg(index + b);
+    const size_t o = (size_t)b * nvec + j;
+    float4 lo, hi;
+    if (u >= 0 && u < U) {
+      const float4* src = kb_u + ((size_t)u * nvec + j) * 2;
+      lo = __ldg(src);
+      hi = __ldg(src + 1);
+    } else {
+      lo = hi = make_float4(__int_as_float(0x7fc00000), __int_as_float(0x7fc00000), __int_as_float(0x7fc00000),
+                            __int_as_float(0x7fc00000));
+    }
+    if constexpr (BF16) {
+      __nv_bfloat162 p0 = __floats2bfloat162_rn(lo.x, lo.y), p1 = __floats2bfloat162_rn(lo.z, lo.w);
+      __nv_bfloat162 p2 = __floats2bfloat162_rn(hi.x, hi.y), p3 = __floats2bfloat162_rn(hi.z, hi.w);
+      uint4 v;
+      v.x = *reinterpret_cast<uint32_t*>(&p0);
+      v.y = *reinterpret_cast<uint32_t*>(&p1);
+      v.z = *reinterpret_cast<uint32_t*>(&p2);
+      v.w = *reinterpret_cast<uint32_t*>(&p3);
+      reinterpret_cast<uint4*>(out)[o] = v;
+    } else {
+      float4* dst = reinterpret_cast<float4*>(out) + o * 2;
+      dst[0] = lo;
+      dst[1] = hi;
+    }
+  }
+}
+
+static int kb_gather_launch(const float* kb_u, const int* index, void* out, int out_bf16, int B, int U, int nvec,
+                            cudaStream_t stream) {
+  const dim3 grid((unsigned)((nvec + GATHER_THREADS - 1) / GATHER_THREADS), (unsigned)(B < 65535 ? B : 65535));
+  const float4* src = reinterpret_cast<const float4*>(kb_u);
+  if (out_bf16)
+    kb_gather_kernel<true><<<grid, GATHER_THREADS, 0, stream>>>(src, index, out, B, U, nvec);
+  else
+    kb_gather_kernel<false><<<grid, GATHER_THREADS, 0, stream>>>(src, index, out, B, U, nvec);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
 }  // namespace mac

@@ -661,6 +661,18 @@ extern "C" int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mo
                                        : ingest_nchw_launch<float, false>(x_nchw, out, B, C, H, W, stream);
 }
 
+// ------------------------------------------------------------------------------------------------ knowledge-base gather
+extern "C" int mac_kb_gather(const float* kb_u, const int* index, void* out, int out_bf16, int B, int U, int N, int d,
+                             mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!kb_u || !index || !out || B <= 0 || U <= 0 || N <= 0 || d <= 0) return MAC_ERR_INVALID;
+  // one sample's run of N*d elements in GATHER_V-element vectors, counted in an int
+  if ((out_bf16 != 0 && out_bf16 != 1) || (d % GATHER_V) || (long long)N * d / GATHER_V > 0x7fffffffLL)
+    return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(kb_u) || !mac_aligned16(index) || !mac_aligned16(out)) return MAC_ERR_ALIGN;
+  return kb_gather_launch(kb_u, index, out, out_bf16, B, U, (int)((long long)N * d / GATHER_V), stream);
+}
+
 // ------------------------------------------------------------------------------------------------ stem: split-bf16 patches
 // The patch matrix of mac_im2col3x3 as the A operand of tc3_gemm: cols2[m, k] = bf16(v), cols2[m, 9C + k] = bf16(v - hi) with
 // v the fp32 value mac_im2col3x3 writes at cols[m, k] (same Philox draw: the quad index of the SOURCE element).  Eight

@@ -144,7 +144,11 @@ class MACCell(object):
     def __init__(self, vecQuestions, questionWords, questionCntxWords, questionLengths, knowledgeBase,
                  memoryDropout, readDropout, writeDropout, batchSize, train, reuse=None, *,
                  config=None, params=None, prec="fp32", seed=0, save_for_backward=False, fold_y=None, small_tc=None,
-                 tape_bwd=False):
+                 tape_bwd=False, kbIndex=None):
+        """`kbIndex` (inference only): CUDA int32 [batchSize], contiguous.  `knowledgeBase` is then the fp32 [U, N, d] of U
+        distinct images and question b reads image kbIndex[b]; `zero_state` gathers each question's rows (mac_kb_gather)
+        into the operand its read unit reads -- directly into the bf16 copy for the bf16 and fp8 inference forms, which
+        read nothing else, into an fp32 [batchSize, N, d] buffer of the cell for every other form."""
         self.lib = _lib.load()
         self.cfg = config if config is not None else _defaults["config"]
         self.params = params if params is not None else _defaults["params"]
@@ -166,6 +170,16 @@ class MACCell(object):
                 raise ValueError("inputs must be contiguous CUDA float32 tensors")
         if self._kb_given_bf16 and not (knowledgeBase.is_cuda and knowledgeBase.is_contiguous()):
             raise ValueError("a bf16 knowledge base must be a contiguous CUDA tensor")
+        self.kbIndex = kbIndex
+        if kbIndex is not None:
+            # training draws the read dropout (and the stem's) per question, and dKB would be a segmented sum over the
+            # questions of each image: shared knowledge bases are an inference form
+            if save_for_backward or min(float(memoryDropout), float(readDropout), float(writeDropout)) < 1.0:
+                raise NotImplementedError("kbIndex (knowledge bases shared between questions) is inference only: "
+                                          "save_for_backward=False and every dropout 1.0")
+            if self._kb_given_bf16:
+                raise NotImplementedError("kbIndex gathers from the stem's fp32 output: a bf16 knowledge base is not accepted")
+            self._check_kb_index(kbIndex, int(batchSize), knowledgeBase.device)
         self.vecQuestions = vecQuestions
         self.questionWords = questionWords
         self.questionCntxWords = questionCntxWords
@@ -179,6 +193,10 @@ class MACCell(object):
         self.seed = int(seed)
         self.device = knowledgeBase.device
         B, N, d = knowledgeBase.shape
+        if kbIndex is not None:
+            self.U, B = B, self.batchSize
+            if d % 8:
+                raise NotImplementedError("kbIndex needs memDim %% 8 == 0 (mac_kb_gather's 16-byte vectors), got %d" % d)
         self.B, self.N, self.d = B, N, d
         assert B == self.batchSize and d == c.memDim == c.ctrlDim
         self.none = torch.zeros((B, 1), dtype=torch.float32, device=self.device)     # mac_cell.py:75
@@ -248,16 +266,33 @@ class MACCell(object):
         if self._kb_given_bf16 and not (self.prec in (PREC["bf16"], PREC["fp8"]) and self._read_hoist
                                         and float(readDropout) >= 1.0):
             raise NotImplementedError("a bf16 knowledge base is accepted by the bf16 and fp8 inference paths only")
+        # kbIndex: the bf16 and fp8 hoisted inference forms (fused step or unfused chain) read only kb_bf16, which the gather
+        # writes directly; every other form reads an fp32 per-question knowledge base, gathered into this cell's buffer
+        self._kb_gather_bf16 = kbIndex is not None and self.prec in (PREC["bf16"], PREC["fp8"]) and self._read_hoist
+        self._kb_rows = (torch.empty((B, N, d), dtype=torch.float32, device=self.device)
+                         if kbIndex is not None and not self._kb_gather_bf16 else None)
 
-    def rebind(self, vecQuestions, questionWords, questionCntxWords, knowledgeBase):
+    def _check_kb_index(self, kbIndex, B, device):
+        if not (torch.is_tensor(kbIndex) and kbIndex.dtype == torch.int32 and kbIndex.is_cuda and kbIndex.device == device
+                and kbIndex.dim() == 1 and kbIndex.is_contiguous() and kbIndex.shape[0] == B):
+            raise ValueError("kbIndex must be a contiguous CUDA int32 tensor of shape [batchSize = %d] on the knowledge "
+                             "base's device" % B)
+
+    def rebind(self, vecQuestions, questionWords, questionCntxWords, knowledgeBase, kbIndex=None):
         """Point the cell at another batch's input tensors of the same shapes and types (the next `mac_network` reads
         them): what a caller whose encoder and stem produce fresh tensors on every pass needs to keep one cell -- its scratch
         workspaces and cached weight structures; `zero_state` still allocates the histories and attention buffers of each
-        pass -- across passes (serving.ModelPipeline)."""
+        pass -- across passes (serving.ModelPipeline).  A cell built with `kbIndex` takes the new index here, one without
+        takes none."""
         for new, old in ((vecQuestions, self.vecQuestions), (questionWords, self.questionWords),
                          (questionCntxWords, self.questionCntxWords), (knowledgeBase, self.knowledgeBase)):
             if not (new.shape == old.shape and new.dtype == old.dtype and new.device == old.device and new.is_contiguous()):
                 raise ValueError("rebind needs contiguous tensors of the shapes and types the cell was built over")
+        if (kbIndex is None) != (self.kbIndex is None):
+            raise ValueError("rebind takes a kbIndex exactly when the cell was built with one")
+        if kbIndex is not None:
+            self._check_kb_index(kbIndex, self.B, self.device)
+            self.kbIndex = kbIndex
         self.vecQuestions, self.questionWords = vecQuestions, questionWords
         self.questionCntxWords, self.knowledgeBase = questionCntxWords, knowledgeBase
 
@@ -367,12 +402,19 @@ class MACCell(object):
         self._att_q = self._new(L, B, words.shape[1])
         self._att_kb = self._new(L, B, self.N)
         self._gate = self._new(L, B, d) if c.writeGate else None
+        # the per-question knowledge base the read unit takes (`_kb_q`): the caller's, or gathered from the U images
+        self._kb_q = self.knowledgeBase
+        if self._kb_gather_bf16:
+            self.kb_bf16 = self._kb_q = torch.empty((B, self.N, d), dtype=torch.bfloat16, device=self.device)
+            self._kb_gather(self.kb_bf16, 1)
+        elif self.kbIndex is not None:
+            self._kb_q = self._kb_gather(self._kb_rows, 0)
         if self._kb_given_bf16:
             self.kb_bf16 = self.knowledgeBase
-        elif self.prec in (PREC["bf16"], PREC["fp8"]) and self._fused_read:
-            self.kb_bf16 = torch.empty(self.knowledgeBase.shape, dtype=torch.bfloat16, device=self.device)
-            check(self.lib.mac_cast_bf16(ptr(self.knowledgeBase), ptr(self.kb_bf16), self.knowledgeBase.numel(),
-                                         stream_ptr()), "mac_cast_bf16")
+        elif self.prec in (PREC["bf16"], PREC["fp8"]) and self._fused_read and not self._kb_gather_bf16:
+            self.kb_bf16 = torch.empty(self._kb_q.shape, dtype=torch.bfloat16, device=self.device)
+            check(self.lib.mac_cast_bf16(ptr(self._kb_q), ptr(self.kb_bf16), self._kb_q.numel(), stream_ptr()),
+                  "mac_cast_bf16")
         self._mem_in = self._new(B, d)
         self._y_next = self._new(B, d)
         self._y_for = -1
@@ -387,6 +429,12 @@ class MACCell(object):
         if self._hoist:
             self._control_all_steps()
         return MACCellTuple(c0, m0)
+
+    def _kb_gather(self, out, bf16):
+        """out[b] = knowledgeBase[kbIndex[b]] (mac_kb_gather), fp32 or bf16."""
+        check(self.lib.mac_kb_gather(ptr(self.knowledgeBase), ptr(self.kbIndex), ptr(out), int(bf16), self.B, self.U, self.N,
+                                     self.d, stream_ptr()), "mac_kb_gather")
+        return out
 
     def _set_histories(self, i):
         self.controls = self._hc[:i + 1].permute(1, 0, 2)      # [B, i+1, d] like mac_cell.py:549, 472
@@ -847,7 +895,7 @@ class MACCell(object):
             if self._tape is not None:
                 self._tape.copy(self._hc[i + 1], self.vecQuestions)
             newControl = self._hc[i + 1]
-        info = self.read(self.knowledgeBase, memory, newControl, name=cellName, _att_out=self._att_kb[i],
+        info = self.read(self._kb_q, memory, newControl, name=cellName, _att_out=self._att_kb[i],
                          _out=self._hi[i + 1], _y_pre=self._y_next if self._y_for == i else None)
         if c.writeDropout < 1.0 and self.dropouts["write"] < 1.0:                      # mac_cell.py:461-463
             info = self._dropout(info, self.dropouts["write"], _lib.SITE_WRITE_INFO, i, self._hi[i + 1])

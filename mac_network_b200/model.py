@@ -86,12 +86,29 @@ class MACnet(object):
         return predsList
 
     # ------------------------------------------------------------------ feed (model.py:101-128, 68)
-    def _to_device(self, data, images):
+    @staticmethod
+    def shared_images(images):
+        """(rows, inverse) when `images["imageIds"]` (the reference's key, main.py:325-334) repeats an id, else None:
+        `rows` are the batch rows that hold the first occurrence of each distinct id (in ascending id order), `inverse[b]`
+        the position in `rows` of question b's image."""
+        ids = images.get("imageIds") if isinstance(images, dict) else None
+        if ids is None:
+            return None
+        ids = np.asarray(ids)
+        _, rows, inverse = np.unique(ids, return_index=True, return_inverse=True)
+        if len(rows) == len(ids):
+            return None
+        return rows, inverse.reshape(-1).astype(np.int32)
+
+    def _to_device(self, data, images, rows=None):
+        """`rows`: copy only these rows of the images (the first occurrence of each distinct image)."""
         q = np.ascontiguousarray(data["questions"], dtype=np.int32)
         dev = {"questions": torch.from_numpy(q).to(self.device),
                "questionLengths": torch.from_numpy(np.ascontiguousarray(data["questionLengths"], dtype=np.int32)).to(self.device),
                "answers": torch.from_numpy(np.ascontiguousarray(data["answers"], dtype=np.int32)).to(self.device)}
         img = images["images"]
+        if rows is not None:
+            img = img[torch.from_numpy(rows)] if torch.is_tensor(img) else np.asarray(img)[rows]
         img = img if torch.is_tensor(img) else torch.from_numpy(np.ascontiguousarray(img, dtype=np.float32))
         # the reference feeds [B, C, H, W] and transposes to channels-last first (model.py:68)
         dev["images"] = img.to(self.device).permute(0, 2, 3, 1).contiguous()
@@ -109,7 +126,10 @@ class MACnet(object):
     def runBatch(self, sess, data, images, train, getAtt=False):
         data = self.trimData(dict(data))
         time0 = time.time()
-        dev = self._to_device(data, images)
+        # evaluation with repeated imageIds: the stem runs once per distinct image and the cell gathers each question's
+        # knowledge base (MACCell(kbIndex=)); training draws its dropouts per question, so it keeps one image per question
+        shared = None if train else self.shared_images(images)
+        dev = self._to_device(data, images, rows=None if shared is None else shared[0])
         B, S = dev["questions"].shape
         time1 = time.time()
         t = self.trainer
@@ -124,8 +144,9 @@ class MACnet(object):
             try:
                 words, cntx, vecq = self._enc.forward(dev["questions"], dev["questionLengths"])
                 kb = self._stem.forward(dev["images"])
+                kbIndex = None if shared is None else torch.from_numpy(shared[1]).to(self.device)
                 cell = MACCell(vecq, words, cntx, dev["questionLengths"], kb, 1.0, 1.0, 1.0, B, False, config=self.cfg,
-                               params=t.params, prec=self.prec)
+                               params=t.params, prec=self.prec, kbIndex=kbIndex)
                 _, memory = mac_network(cell, self.L)
                 logits, losses, _ = self._out.forward(memory, vecq, dev["answers"])
                 self.macCell = cell

@@ -156,14 +156,15 @@ class _CastRing(object):
         self.pending = None                 # (ticket, source tensor, ring index) of the cast in flight
 
     def begin(self, src):
-        """Start the cast of `src` into the next staging buffer; returns that buffer's ring index."""
+        """Start the cast of `src` (at most a staging buffer's elements) into the front of the next staging buffer; returns
+        that buffer's ring index."""
         si = self.casts % len(self.stages)
         self.casts += 1
         if self.busy[si] is not None:
             self.busy[si].synchronize()              # the previous copy out of this staging buffer has finished
             self.busy[si] = None
         st = self.lib.mac_host_cast_bf16_begin(ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(self.stages[si].data_ptr()),
-                                               self.stages[si].numel(), self.threads)
+                                               min(src.numel(), self.stages[si].numel()), self.threads)
         if st != 0:
             raise _lib.MacB200Error("mac_host_cast_bf16_begin failed: %d" % st)
         return si
@@ -336,7 +337,7 @@ class _ModelSlot(object):
     encoder / stem / cell / output unit over the model's parameter tensors, the forward captured as one CUDA graph, pinned
     host outputs."""
 
-    def __init__(self, model, shape, images_bf16, use_graph, topk):
+    def __init__(self, model, shape, images_bf16, use_graph, topk, images=None):
         B, S, H, W = shape
         t, cfg = model.trainer, model.cfg
         p = t.params
@@ -345,8 +346,10 @@ class _ModelSlot(object):
         self.stream = torch.cuda.Stream()
         self.x = {"questions": torch.zeros(B, S, dtype=torch.int32, device=p.device),
                   "questionLengths": torch.full((B,), S, dtype=torch.int32, device=p.device),
-                  "images": torch.zeros(B, C, H, W, device=p.device,
+                  "images": torch.zeros(B if images is None else images, C, H, W, device=p.device,
                                         dtype=torch.bfloat16 if images_bf16 else torch.float32)}
+        if images is not None:      # question b reads image imageIndex[b] of the U the stem runs over
+            self.x["imageIndex"] = torch.zeros(B, dtype=torch.int32, device=p.device)
         from .encoder import QuestionEncoder
         from .output_unit import OutputUnit
         from .stem import Stem
@@ -368,11 +371,12 @@ class _ModelSlot(object):
         m, x = self.model, self.x
         words, cntx, vecq = self.enc.forward(x["questions"], x["questionLengths"])
         kb = self.stem.forward_nchw(x["images"])
+        idx = x.get("imageIndex")
         if self.cell is None:       # MACCell's own errors (flag set / precision outside its inference forms) pass through
             self.cell = MACCell(vecq, words, cntx, x["questionLengths"], kb, 1.0, 1.0, 1.0, self.B, False, config=m.cfg,
-                                params=m.trainer.params, prec=m.prec)
+                                params=m.trainer.params, prec=m.prec, kbIndex=idx)
         else:
-            self.cell.rebind(vecq, words, cntx, kb)
+            self.cell.rebind(vecq, words, cntx, kb, kbIndex=idx)
         c = self.cell
         _, memory = mac_network(c, m.L)
         logits = self.out.logits(memory, vecq)
@@ -406,17 +410,20 @@ class _ModelSlot(object):
         if self.outs_host is None:
             self.outs_host = {k: _pinned(v.numel(), v.dtype).view(v.shape) for k, v in self.outs_dev.items()}
 
-    def enqueue(self, questions, lengths, images, copied=None):
+    def enqueue(self, questions, lengths, images, copied=None, index=None):
         """H2D copies -> forward -> D2H copies on this slot's stream; returns after enqueueing.  `images` is host memory of
-        the slot's image type (the caller's fp32 tensor or a bf16 staging buffer), any shape with the right element count,
-        or a callable that returns it, called once the small copies are enqueued (the host cast is waited for there);
-        `copied(stream)` is called once the image copy is enqueued."""
+        the slot's image type (the caller's fp32 tensor or a bf16 staging buffer), any shape with the element count of the
+        slot's images or, with `index` (the slot's imageIndex), of their first k, or a callable that returns it, called once
+        the small copies are enqueued (the host cast is waited for there); `copied(stream)` is called once the image copy is
+        enqueued."""
         with torch.cuda.stream(self.stream):
             self.x["questions"].copy_(questions, non_blocking=True)
             self.x["questionLengths"].copy_(lengths, non_blocking=True)
+            if index is not None:
+                self.x["imageIndex"].copy_(index, non_blocking=True)
             if callable(images):
                 images = images()
-            self.x["images"].view(-1).copy_(images.view(-1), non_blocking=True)
+            self.x["images"].view(-1)[:images.numel()].copy_(images.view(-1), non_blocking=True)
             if copied is not None:
                 copied(self.stream)
             if self.graph is not None:
@@ -451,6 +458,17 @@ class ModelPipeline(object):
     `att_kb` [L, B, H*W], `att_question` [L, B, S], and `gate` [L, B, d] / `self` [L, B, L] (step i's i + 1 weights, zero
     beyond) when the flag set has them.
 
+    Several questions per image: with `images=U` (1 <= U <= B) a batch carries k <= U distinct images and each question's
+    image number,
+
+        pipe = ModelPipeline(model, shape=(B, S, H, W), slots=4, images=8)
+        t = pipe.submit({"questions": ..., "questionLengths": ..., "images": fp32 [k, C, H, W], "imageIndex": int32 [B]})
+
+    with 1 <= k <= U and every imageIndex[b] in [0, k).  Only the k images cross PCIe; the captured graph runs the ingest and
+    the stem over the slot's U image rows (rows k..U-1 hold a previous batch's data that no question reads) and the cell
+    gathers each question's knowledge base from them (`MACCell(kbIndex=)`, `mac_kb_gather`).  The index is a device input
+    of the graph like the questions: a new index pattern or a new k needs no new capture.
+
     Questions are padded with 0 to the pipeline's fixed S (a captured graph cannot trim a batch to its longest question as
     `runBatch` does); the kernels mask by length, so attention at positions >= length is exactly 0.
 
@@ -463,7 +481,8 @@ class ModelPipeline(object):
     Memory: every slot has its own encoder and stem and with them its own weight packs (about 14 MB per slot at 1024 -> 512
     -> 512), and its graph's private pool holds its own patch matrices (231 MB for layer 0 at 64x1024x14x14)."""
 
-    def __init__(self, model, shape, slots=4, use_graph=True, topk=1, host_cast=None, cast_threads=None, stage_ring=None):
+    def __init__(self, model, shape, slots=4, use_graph=True, topk=1, host_cast=None, cast_threads=None, stage_ring=None,
+                 images=None):
         B, S, H, W = [int(v) for v in shape]
         p = model.trainer.params
         C = int(p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2])
@@ -475,42 +494,65 @@ class ModelPipeline(object):
             raise ValueError("the image features have %d channels: mac_ingest_nchw needs a multiple of 64" % C)
         if not 1 <= int(topk) <= min(8, A):
             raise ValueError("topk must be in 1..min(8, %d answers), got %r" % (A, topk))
+        if images is not None and not (isinstance(images, int) and 1 <= images <= B):
+            raise ValueError("images must be None or an int in 1..B = %d, got %r" % (B, images))
+        self.images = images
         self.lib = _lib.load()
         self.model, self.params, self.shape, self.C, self.topk = model, p, (B, S, H, W), C, int(topk)
         self.use_graph = bool(use_graph)
         self.cast_threads = int(cast_threads) if cast_threads else max(1, min(12, usable_cpus() - 2))
-        numel = B * C * H * W
+        numel = (B if images is None else images) * C * H * W
         self.host_cast = model._stem.prec == "bf16" and host_cast is not False
         self.cast_ms = None
         if self.host_cast and host_cast is None:
             self.cast_ms = _time_cast(self.lib, numel, self.cast_threads)
             self.host_cast = _cast_pays(self.cast_ms, numel)
         self._version = p.version
-        self.slots = [_ModelSlot(model, self.shape, self.host_cast, self.use_graph, self.topk) for _ in range(int(slots))]
+        self.slots = [_ModelSlot(model, self.shape, self.host_cast, self.use_graph, self.topk, images)
+                      for _ in range(int(slots))]
         self._ring = (_CastRing(self.lib, numel, max(2, int(stage_ring) if stage_ring else 3), self.cast_threads)
                       if self.host_cast else None)
         self._next = 0
         self._ahead = None                  # (next_batch["images"] as given, its host tensor) of the cast in flight
-        self.h2d_bytes = numel * (2 if self.host_cast else 4) + B * S * 4 + B * 4
+        # with images=U: a batch of k images copies k of the U counted here
+        self.h2d_bytes = numel * (2 if self.host_cast else 4) + B * S * 4 + B * 4 + (0 if images is None else B * 4)
         self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.slots[0].outs_host.values())
 
     def _host(self, batch):
-        """The batch's three host tensors, checked against the pipeline's shape; ValueError before anything is enqueued."""
+        """The batch's host tensors (questions, lengths, images, and with images=U the image index, else None), checked
+        against the pipeline's shape; ValueError before anything is enqueued."""
         B, S, H, W = self.shape
+        k = B
+        if self.images is None:
+            if "imageIndex" in batch:
+                raise ValueError("imageIndex is for a pipeline built with images=U")
+        else:
+            if "imageIndex" not in batch:
+                raise ValueError("a pipeline built with images=%d needs the batch's imageIndex" % self.images)
+            k = torch.as_tensor(batch["images"]).shape[0]
+            if not 1 <= k <= self.images:
+                raise ValueError("a batch carries 1..%d images, got %d" % (self.images, k))
         want = (("questions", (B, S), torch.int32), ("questionLengths", (B,), torch.int32),
-                ("images", (B, self.C, H, W), torch.float32))
+                ("images", (k, self.C, H, W), torch.float32))
+        if self.images is not None:
+            want += (("imageIndex", (B,), torch.int32),)
         out = []
         for key, shp, dtype in want:
             v = torch.as_tensor(batch[key])
             if v.device.type != "cpu" or tuple(v.shape) != shp:
                 raise ValueError("%s must be a host tensor of shape %s, got %s on %s" % (key, shp, tuple(v.shape), v.device))
             out.append(v.to(dtype).contiguous())
+        if self.images is None:
+            return out + [None]
+        idx = torch.as_tensor(batch["imageIndex"])
+        if idx.dtype.is_floating_point or idx.dtype == torch.bool or not bool(((idx >= 0) & (idx < k)).all()):
+            raise ValueError("imageIndex must hold integers in [0, %d) (the batch's images)" % k)
         return out
 
     def submit(self, batch, next_batch=None):
         """Enqueue one batch (numpy arrays or host tensors; pinned memory makes the copies asynchronous) and return its
         ticket.  `next_batch`: the batch the next submit will take, whose host cast then runs under this batch's copies."""
-        q, ql, img = self._host(batch)
+        q, ql, img, idx = self._host(batch)
         if self._ahead is not None and self._ahead[0] is batch["images"]:
             img = self._ahead[1]                           # the tensor whose cast the previous submit started
         nxt = self._host(next_batch)[2] if (next_batch is not None and self.host_cast) else None
@@ -524,7 +566,7 @@ class ModelPipeline(object):
         slot = self.slots[t % len(self.slots)]
         self._next = t + 1
         if not self.host_cast:
-            slot.enqueue(q, ql, img)
+            slot.enqueue(q, ql, img, index=idx)
             return t
         si = self._ring.take(t, img)
 
@@ -532,8 +574,8 @@ class ModelPipeline(object):
             self._ring.end()                               # the images are in their staging buffer
             if nxt is not None:                            # the next batch's cast runs under this batch's copies
                 self._ring.prefetch(self._next, nxt)
-            return self._ring.stages[si]
-        slot.enqueue(q, ql, staged, copied=lambda stream: self._ring.copied(si, stream))
+            return self._ring.stages[si][:img.numel()]
+        slot.enqueue(q, ql, staged, copied=lambda stream: self._ring.copied(si, stream), index=idx)
         return t
 
     def result(self, ticket):
