@@ -196,9 +196,12 @@ class _CastRing(object):
 
 
 class _Slot(object):
+    """One batch in flight through the cell: its own stream, persistent device inputs, a cell over them, the netLength
+    unroll captured as one CUDA graph, pinned host outputs."""
+
     def __init__(self, cfg, params, shape, prec, host_kb_bf16, use_graph, fold_y=None, small_tc=None):
         B, S, N, d, L = shape
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = params.device
         self.stream = torch.cuda.Stream()
         self.x = {
             "vecQuestions": torch.zeros(B, d, device=dev),
@@ -206,35 +209,51 @@ class _Slot(object):
             "questionLengths": torch.full((B,), S, dtype=torch.int32, device=dev),
             "knowledgeBase": torch.zeros(B, N, d, device=dev, dtype=torch.bfloat16 if host_kb_bf16 else torch.float32),
         }
-        x = self.x
-        # questionWords is unused with controlContextual (mac_cell.py:570); the cell takes the contextual words for both
-        self.cell = MACCell(x["vecQuestions"], x["questionCntxWords"], x["questionCntxWords"], x["questionLengths"],
-                            x["knowledgeBase"], 1.0, 1.0, 1.0, B, False, config=cfg, params=params, prec=prec, fold_y=fold_y,
-                            small_tc=small_tc)
-        self.L = L
+        self.B, self.L, self.use_graph = B, L, use_graph
+        self._cell_kw = dict(config=cfg, params=params, prec=prec, fold_y=fold_y, small_tc=small_tc)
+        self.cell = None
         self.graph = None
-        with torch.cuda.stream(self.stream):
-            mac_network(self.cell, L)                      # warm-up: packed weights, folded weights, attributes
-            self.stream.synchronize()
-            if use_graph:
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, stream=self.stream):
-                    mac_network(self.cell, L)
-                self.graph = g
-        c = self.cell
-        self.outs_dev = {"control": c._hc[L], "memory": c._hm[L], "att_kb": c._att_kb, "att_question": c._att_q}
-        self.outs_host = {k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in self.outs_dev.items()}
+        self.outs_host = None
         self.kb_stage = None        # assigned per submit from HostPipeline's small staging ring
         self.h2d_done = torch.cuda.Event()
         self.done = torch.cuda.Event()
         self.busy = False
+        self.capture()
+
+    def capture(self):
+        """A new cell over the slot's inputs, one eager pass (weight packs, folded weights and the scalar biases the kernels
+        take as arguments, all of the current parameter version, are built outside the graph), then the capture.  The
+        slot's stream first waits for the caller's current stream: whatever wrote the parameters there (an optimizer step, a
+        checkpoint restore) is enqueued, not necessarily done, and so are the zeroed workspaces of the new cell."""
+        self.graph = None                   # a previous capture's memory goes back before the new one takes its own
+        x = self.x
+        # questionWords is unused with controlContextual (mac_cell.py:570); the cell takes the contextual words for both
+        self.cell = MACCell(x["vecQuestions"], x["questionCntxWords"], x["questionCntxWords"], x["questionLengths"],
+                            x["knowledgeBase"], 1.0, 1.0, 1.0, self.B, False, **self._cell_kw)
+        self.stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(self.stream):
+            mac_network(self.cell, self.L)                 # warm-up: packed weights, folded weights, attributes
+            self.stream.synchronize()
+            if self.use_graph:
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g, stream=self.stream):
+                    mac_network(self.cell, self.L)
+                self.graph = g
+        c, L = self.cell, self.L
+        self.outs_dev = {"control": c._hc[L], "memory": c._hm[L], "att_kb": c._att_kb, "att_question": c._att_q}
+        if self.outs_host is None:          # the shapes do not change with the weights
+            self.outs_host = {k: _pinned(v.numel(), v.dtype).view(v.shape) for k, v in self.outs_dev.items()}
 
 
 class HostPipeline(object):
     """`submit(batch)` takes one batch of HOST tensors (fp32; pinned for asynchronous copies) with the keys
     vecQuestions [B,d], questionCntxWords [B,S,d], questionLengths [B] (int32) and knowledgeBase [B,N,d]; it returns a
     ticket.  `result(ticket)` blocks until that batch is done and returns pinned host tensors (final control / memory
-    state, per-step KB and question attention maps) that stay valid until the slot is reused `slots` submits later."""
+    state, per-step KB and question attention maps) that stay valid until the slot is reused `slots` submits later.
+
+    When the parameter values move (`params.version`: optimizer step, checkpoint restore), the packed weights and the scalar
+    biases a captured graph holds by value are stale: the next `submit` drains the pipeline and gives every slot a new cell,
+    eager pass and capture before it takes the batch, as `ModelPipeline` does.  `drain()` before writing the parameters."""
 
     def __init__(self, cfg, params, shape, prec="bf16", slots=4, use_graph=True, cast_threads=None, fold_y=None,
                  host_cast=None, stage_ring=None):
@@ -253,6 +272,8 @@ class HostPipeline(object):
             self.host_kb_bf16 = _cast_pays(self.cast_ms, shape[0] * shape[2] * shape[3])
         if fold_y is None:
             fold_y = slots < 4          # several batches in flight: the unfolded write + projY GEMMs pack better (mac_cell.py)
+        self.params = params
+        self._version = params.version
         # several batches in flight: the tensor-core form of the batch-sized projections (see MACCell.__init__)
         self.slots = [_Slot(cfg, params, shape, prec, self.host_kb_bf16, use_graph, fold_y, small_tc=(slots >= 2))
                       for _ in range(max(1, slots))]
@@ -279,6 +300,11 @@ class HostPipeline(object):
             self._ring.prefetch(self._next, batch["knowledgeBase"])
 
     def submit(self, batch, next_batch=None):
+        if self.params.version != self._version:
+            self.drain()
+            for s in self.slots:
+                s.capture()
+            self._version = self.params.version
         t = self._next
         slot = self.slots[t % len(self.slots)]
         if self.host_kb_bf16:

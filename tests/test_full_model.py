@@ -64,6 +64,12 @@ def test_full_model_forward_and_gradient(flags):
     ref = _oracle_loss(cfg, L, values, data)
     assert max_rel(logits.cpu().numpy(), ref["logits"]) < 1e-4
     assert max_rel(losses.cpu().numpy(), ref["losses"]) < 1e-4
+    check_directional_derivatives(cfg, L, values, data, tr, flags)
+
+
+def check_directional_derivatives(cfg, L, values, data, tr, tag):
+    """The trainer's gradient bucket (of the loss at `values` on `data`) along one random direction per sub-model's
+    variables against central differences of the fp64 oracle chain."""
     bucket = tr.bucket.cpu().numpy().astype(np.float64)
     offs, specs = tr.params.offsets, tr.params.specs
     groups = {"encoder": ("encoder/", "qEmbeddings/"), "stem": ("stem/",), "cell": ("MACnetwork/",),
@@ -84,7 +90,7 @@ def test_full_model_forward_and_gradient(flags):
             hi[n] = values[n].astype(np.float64) + eps * direction[n]
             lo[n] = values[n].astype(np.float64) - eps * direction[n]
         numeric = (_oracle_loss(cfg, L, hi, data)["loss"] - _oracle_loss(cfg, L, lo, data)["loss"]) / (2 * eps)
-        print("%s %-8s directional derivative: analytic %.6e numeric %.6e" % (flags, gname, analytic, numeric))
+        print("%s %-8s directional derivative: analytic %.6e numeric %.6e" % (tag, gname, analytic, numeric))
         assert abs(analytic - numeric) <= 2e-3 * max(abs(numeric), 1e-3), (gname, analytic, numeric)
 
 
