@@ -458,6 +458,18 @@ int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float keep, uint64_
  * bf16 -> patches), else MAC_ERR_UNSUPPORTED; B <= 65535.  All checks precede any launch. */
 enum { MAC_INGEST_NHWC_F32 = 0, MAC_INGEST_PATCH_BF16 = 1 };
 int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mode, int B, int C, int H, int W, mac_stream_t stream);
+/* Training form of the layer-0 ingest (csrc/ingest.cuh; Stem.forward_nchw with a dropout or save_for_backward): x_nchw fp32
+ * [B, C, H, W], read once, and two outputs:
+ *   x_nhwc: fp32 [B, H, W, C], the permuted tensor, undropped (the stem saves it as layer 0's input);
+ *   cols:   layer 0's dropped-out patch matrix of x_nhwc, bit for bit what mac_im2col3x3(cols_bf16 = 1, keep, seed, site, step)
+ *           writes (MAC_INGEST_COLS_BF16: bf16 [B*H*W, 9*C]) or mac_im2col3x3_split(keep, seed, site, step) writes
+ *           (MAC_INGEST_COLS_SPLIT: bf16 [B*H*W, 2*9*C] = [hi | lo]).
+ * The keep-mask is mac_im2col3x3's: one philox4x32_10(seed, e >> 2, site, step) per channel quad of the NHWC flat index e,
+ * keep in (0, 1] (1: no mask).  C % 64 == 0, H*W <= 345 (MAC_INGEST_COLS_BF16) or 284 (MAC_INGEST_COLS_SPLIT), B <= 65535,
+ * else MAC_ERR_UNSUPPORTED; 16-byte aligned pointers.  All checks precede any launch. */
+enum { MAC_INGEST_COLS_BF16 = 0, MAC_INGEST_COLS_SPLIT = 1 };
+int mac_ingest_nchw_train(const float* x_nchw, float* x_nhwc, void* cols, int cols_form, float keep, uint64_t seed, int site,
+                          int step, int B, int C, int H, int W, mac_stream_t stream);
 /* Knowledge bases of B questions about U distinct images (csrc/ingest.cuh; MACCell(kbIndex=), serving.ModelPipeline(images=)):
  *   out[b, n, :] = kb_u[index[b], n, :]   for b < B
  * kb_u: the stem's fp32 output for the U images, [U, N, d]; index: int32 [B] in device memory; out: fp32 [B, N, d], or with

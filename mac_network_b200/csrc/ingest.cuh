@@ -14,6 +14,7 @@
 // tap (patch mode) or 256 per pixel (NHWC mode).
 #pragma once
 #include "common.cuh"
+#include "tc_gemm.cuh"      // pack_bf16, pack_bf16_lo: the split-bf16 rounding of mac_im2col3x3_split
 
 namespace mac {
 
@@ -118,6 +119,120 @@ static int ingest_nchw_launch(const void* x, void* out, int B, int C, int H, int
 static inline size_t ingest_smem_bytes(int x_bf16, int mode, int HW) {
   if (x_bf16) return mode ? IngestShape<__nv_bfloat16, true>::smem_bytes(HW) : IngestShape<__nv_bfloat16, false>::smem_bytes(HW);
   return mode ? IngestShape<float, true>::smem_bytes(HW) : IngestShape<float, false>::smem_bytes(HW);
+}
+
+// ------------------------------------------------------------------------------------------------ training ingest
+// The training form of ingest_nchw_kernel: the same CTA (sample, 64-channel slab), the same one bulk copy, and two outputs
+// from the one read -- the UNDROPPED fp32 NHWC tensor (the stem saves it as layer 0's input; the backward regenerates the
+// mask from it) and layer 0's DROPPED-OUT patch matrix, bit for bit what mac_im2col3x3(cols_bf16 = 1) or
+// mac_im2col3x3_split writes.  The mask is drawn once per source element while transposing, not once per tap: one
+// philox4x32_10(seed, e >> 2, site, step) per (pixel, channel quad), e the NHWC flat index -- mac_im2col3x3's counter.
+// Shared memory, per pixel: the slab (256 B), the fp32 pixel-major tile (64 * 4 + 16 B) and the bf16 tile (64 * 2 + 16 B),
+// and for the split form a second bf16 tile for the lo halves: 672 / 816 B, 131.7 / 159.9 KB at 14x14, one CTA per SM, so
+// 512 threads keep more loads and stores in flight than ING_THREADS would.
+constexpr int INGT_THREADS = 512;
+constexpr int INGT_FROW = ING_CS * 4 + 16;     // fp32 tile row, bytes
+constexpr int INGT_HROW = ING_CS * 2 + 16;     // bf16 tile row, bytes
+
+template <bool SPLIT>
+struct IngestTrainShape {
+  static constexpr int PIX = ING_CS * 4 + INGT_FROW + INGT_HROW * (SPLIT ? 2 : 1);     // shared bytes per pixel
+  __host__ __device__ static size_t smem_bytes(int HW) { return (size_t)HW * PIX; }
+};
+
+template <bool SPLIT>
+__global__ void __launch_bounds__(INGT_THREADS, 1) ingest_nchw_train_kernel(const float* __restrict__ x,
+                                                                            float* __restrict__ x_nhwc,
+                                                                            __nv_bfloat16* __restrict__ cols, uint32_t thresh,
+                                                                            float scale, uint64_t seed, int site, int step,
+                                                                            int C, int H, int W) {
+  extern __shared__ __align__(128) unsigned char ing_smem[];
+  __shared__ uint64_t bar;
+  const int HW = H * W, tid = threadIdx.x, b = blockIdx.y, c0 = blockIdx.x * ING_CS;
+  const float* s_in = reinterpret_cast<const float*>(ing_smem);              // [64][HW] as it lies in NCHW
+  unsigned char* s_f = ing_smem + (size_t)HW * ING_CS * 4;                   // [HW][FROW], undropped fp32
+  unsigned char* s_h = s_f + (size_t)HW * INGT_FROW;                         // [HW][HROW], bf16(dropped) or its hi half
+  unsigned char* s_l = s_h + (size_t)HW * INGT_HROW;                         // [HW][HROW], the lo half (SPLIT)
+  if (tid == 0) {
+    mbar_init(&bar, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const uint32_t bytes = (uint32_t)((size_t)HW * ING_CS * 4);
+    mbar_expect_tx(&bar, bytes);
+    bulk_g2s(ing_smem, x + ((size_t)b * C + c0) * HW, bytes, &bar);
+  }
+  mbar_wait(&bar, 0);
+  // transpose + mask: eight consecutive channels (two Philox quads) of one pixel per item; lanes along the pixels
+  for (int i = tid; i < 8 * HW; i += INGT_THREADS) {
+    const int g = i / HW, p = i - g * HW;
+    const float* src = s_in + (size_t)(g * 8) * HW + p;
+    float v[8], d[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = d[j] = src[j * HW];
+    if (thresh) {
+      const uint64_t q = (((uint64_t)b * HW + p) * C + c0 + g * 8) >> 2;
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const Philox4 r = philox4x32_10(seed, q + k, (uint32_t)site, (uint32_t)step);
+        // __fmul_rn: the product is rounded on its own, never contracted into the split form's lo subtraction
+        d[4 * k + 0] = ((r.x >> 8) >= thresh) ? __fmul_rn(v[4 * k + 0], scale) : 0.f;
+        d[4 * k + 1] = ((r.y >> 8) >= thresh) ? __fmul_rn(v[4 * k + 1], scale) : 0.f;
+        d[4 * k + 2] = ((r.z >> 8) >= thresh) ? __fmul_rn(v[4 * k + 2], scale) : 0.f;
+        d[4 * k + 3] = ((r.w >> 8) >= thresh) ? __fmul_rn(v[4 * k + 3], scale) : 0.f;
+      }
+    }
+    float4* f = reinterpret_cast<float4*>(s_f + (size_t)p * INGT_FROW + g * 32);
+    f[0] = make_float4(v[0], v[1], v[2], v[3]);
+    f[1] = make_float4(v[4], v[5], v[6], v[7]);
+    uint4 hi;
+    hi.x = pack_bf16(d[0], d[1]); hi.y = pack_bf16(d[2], d[3]);
+    hi.z = pack_bf16(d[4], d[5]); hi.w = pack_bf16(d[6], d[7]);
+    *reinterpret_cast<uint4*>(s_h + (size_t)p * INGT_HROW + g * 16) = hi;
+    if constexpr (SPLIT) {
+      uint4 lo;
+      lo.x = pack_bf16_lo(d[0], d[1], hi.x); lo.y = pack_bf16_lo(d[2], d[3], hi.y);
+      lo.z = pack_bf16_lo(d[4], d[5], hi.z); lo.w = pack_bf16_lo(d[6], d[7], hi.w);
+      *reinterpret_cast<uint4*>(s_l + (size_t)p * INGT_HROW + g * 16) = lo;
+    }
+  }
+  __syncthreads();
+  // NHWC: 256 contiguous bytes per pixel
+  for (int i = tid; i < HW * 16; i += INGT_THREADS) {
+    const int g = i & 15, pix = i >> 4;
+    const uint4 v = *reinterpret_cast<const uint4*>(s_f + (size_t)pix * INGT_FROW + g * 16);
+    *reinterpret_cast<uint4*>(x_nhwc + ((size_t)b * HW + pix) * C + c0 + g * 4) = v;
+  }
+  // patches: cols[(b,h,w), tap*C + c] (and, split, cols[(b,h,w), 9C + tap*C + c]); 128 contiguous bytes per pixel and tap
+  constexpr int ROW = SPLIT ? 18 : 9;          // row length in units of C
+  for (int i = tid; i < HW * 9 * 8; i += INGT_THREADS) {
+    const int g = i & 7, r = i >> 3;
+    const int tap = r % 9, pix = r / 9;
+    const int h = pix / W, w = pix - h * W;
+    const int hs = h + tap / 3 - 1, wsrc = w + tap % 3 - 1;
+    uint4 hv = make_uint4(0u, 0u, 0u, 0u), lv = hv;
+    if (hs >= 0 && hs < H && wsrc >= 0 && wsrc < W) {
+      const size_t o = (size_t)(hs * W + wsrc) * INGT_HROW + g * 16;
+      hv = *reinterpret_cast<const uint4*>(s_h + o);
+      if constexpr (SPLIT) lv = *reinterpret_cast<const uint4*>(s_l + o);
+    }
+    __nv_bfloat16* row = cols + (((size_t)b * HW + pix) * ROW + tap) * C + c0 + g * 8;
+    *reinterpret_cast<uint4*>(row) = hv;
+    if constexpr (SPLIT) *reinterpret_cast<uint4*>(row + 9 * (size_t)C) = lv;
+  }
+}
+
+template <bool SPLIT>
+static int ingest_nchw_train_launch(const float* x, float* x_nhwc, void* cols, uint32_t thresh, float scale, uint64_t seed,
+                                    int site, int step, int B, int C, int H, int W, cudaStream_t stream) {
+  const size_t smem = IngestTrainShape<SPLIT>::smem_bytes(H * W);
+  auto kern = ingest_nchw_train_kernel<SPLIT>;
+  MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kern<<<dim3(C / ING_CS, B), INGT_THREADS, smem, stream>>>(x, x_nhwc, reinterpret_cast<__nv_bfloat16*>(cols), thresh, scale,
+                                                            seed, site, step, C, H, W);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ knowledge-base gather

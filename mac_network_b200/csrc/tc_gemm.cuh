@@ -158,6 +158,9 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&t);
 }
+__device__ __forceinline__ uint32_t pack_bf16_lo(float a, float b, uint32_t hw) {      // lo of the pair whose hi is `hw`
+  return pack_bf16(a - __uint_as_float(hw << 16), b - __uint_as_float(hw & 0xffff0000u));
+}
 
 // SAVE (TC_EPI_ACT_SPLIT / TC_EPI_LOGITS with outf != NULL): a separate instantiation, so the inference form's kernels
 // (outf == NULL) are compiled exactly as without the fp32 store

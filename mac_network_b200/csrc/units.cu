@@ -661,6 +661,26 @@ extern "C" int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mo
                                        : ingest_nchw_launch<float, false>(x_nchw, out, B, C, H, W, stream);
 }
 
+extern "C" int mac_ingest_nchw_train(const float* x_nchw, float* x_nhwc, void* cols, int cols_form, float keep, uint64_t seed,
+                                     int site, int step, int B, int C, int H, int W, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x_nchw || !x_nhwc || !cols || B <= 0 || C <= 0 || H <= 0 || W <= 0 || !(keep > 0.f && keep <= 1.f))
+    return MAC_ERR_INVALID;
+  if (!mac_aligned16(x_nchw) || !mac_aligned16(x_nhwc) || !mac_aligned16(cols)) return MAC_ERR_ALIGN;
+  if ((C % ING_CS) || (cols_form != MAC_INGEST_COLS_BF16 && cols_form != MAC_INGEST_COLS_SPLIT) || B > 65535)
+    return MAC_ERR_UNSUPPORTED;
+  // the slab and its tiles with the kernel's static shared memory in one SM's 227 KB (H*W <= 345 / 284)
+  const bool split = cols_form == MAC_INGEST_COLS_SPLIT;
+  if ((long long)H * W > 4096 ||
+      (split ? IngestTrainShape<true>::smem_bytes(H * W) : IngestTrainShape<false>::smem_bytes(H * W)) + ING_STATIC_SMEM >
+          227 * 1024)
+    return MAC_ERR_UNSUPPORTED;
+  const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
+  const float scale = keep < 1.f ? 1.f / keep : 1.f;
+  return split ? ingest_nchw_train_launch<true>(x_nchw, x_nhwc, cols, thr, scale, seed, site, step, B, C, H, W, stream)
+               : ingest_nchw_train_launch<false>(x_nchw, x_nhwc, cols, thr, scale, seed, site, step, B, C, H, W, stream);
+}
+
 // ------------------------------------------------------------------------------------------------ knowledge-base gather
 extern "C" int mac_kb_gather(const float* kb_u, const int* index, void* out, int out_bf16, int B, int U, int N, int d,
                              mac_stream_t stream_) {
@@ -678,10 +698,6 @@ extern "C" int mac_kb_gather(const float* kb_u, const int* index, void* out, int
 // v the fp32 value mac_im2col3x3 writes at cols[m, k] (same Philox draw: the quad index of the SOURCE element).  Eight
 // channels per thread: two 16-byte loads, one 16-byte store per half.
 namespace mac {
-__device__ __forceinline__ uint32_t pack_bf16_lo(float a, float b, uint32_t hw) {      // lo of the pair whose hi is `hw`
-  return pack_bf16(a - __uint_as_float(hw << 16), b - __uint_as_float(hw & 0xffff0000u));
-}
-
 __global__ void __launch_bounds__(256) im2col3x3_split_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ cols2,
                                                              uint32_t thresh, float scale, uint64_t seed, int site, int step,
                                                              int B, int H, int W, int C) {

@@ -221,17 +221,30 @@ class DPTrainer(object):
         """The reference's whole training graph (`MACnet.build`, model.py:774-821) on the local shard, gradients into the
         flat bucket (not yet reduced):  embeddings + bi-LSTM encoder -> stem -> netLength MAC steps -> output unit ->
         classifier -> mean softmax-CE over the GLOBAL batch, then the hand-written backward of each in reverse order.
-        `data`: questions int32 [B,S] (0 = padding), questionLengths int32 [B], images fp32 [B,H,W,C] (NHWC: the
-        reference transposes its NCHW feed first, model.py:68), answers int32 [B].  Returns (logits, per-sample losses)."""
+        `data`: questions int32 [B,S] (0 = padding), questionLengths int32 [B], answers int32 [B], and the images as exactly
+        one of `images` fp32 [B,H,W,C] (NHWC: the reference transposes its NCHW feed first, model.py:68) or `images_nchw`
+        fp32 [B,C,H,W], contiguous, as the features are stored (`Stem.forward_nchw`: the ingest kernel replaces the permute
+        and, for the bf16 and bf16x3 stems, layer 0's patch pass; the same results bit for bit).  Returns (logits,
+        per-sample losses)."""
         from .autograd import mac_backward
         from .mac_cell import mac_network
         if self.enc is None:
             raise RuntimeError("construct the trainer with classifier=, encoder= and stem=")
+        if ("images" in data) == ("images_nchw" in data):
+            raise ValueError("data needs exactly one of images (NHWC) and images_nchw, got %s"
+                             % sorted(k for k in data if k.startswith("images")))
+        nchw = data.get("images_nchw")
+        if nchw is not None and (nchw.device != self.params.flat.device or nchw.dtype != torch.float32 or nchw.dim() != 4
+                                 or not nchw.is_contiguous()):
+            raise ValueError("images_nchw must be a contiguous fp32 [B, C, H, W] tensor on %s" % self.params.flat.device)
         seed = (self.base_seed * 1000003 + self.step_id * 7919 + self.rank * 104729 + 1) & 0x7FFFFFFFFFFFFFFF
         self.enc.seed = self.stem.seed = self.out.seed = seed
         words, cntx, vecq = self.enc.forward(data["questions"], data["questionLengths"], step=self.step_id,
                                              save_for_backward=True)
-        kb = self.stem.forward(data["images"], keep=self.stem_dropout, step=self.step_id, save_for_backward=True)
+        if nchw is not None:
+            kb = self.stem.forward_nchw(nchw, keep=self.stem_dropout, step=self.step_id, save_for_backward=True)
+        else:
+            kb = self.stem.forward(data["images"], keep=self.stem_dropout, step=self.step_id, save_for_backward=True)
         # the cell captures its inputs at construction (mac_cell.py:59-79): cell_for owns persistent buffers per key and
         # copies this step's encoder / stem outputs into them
         bufs = {"vecQuestions": vecq, "questionWords": words, "questionCntxWords": cntx, "knowledgeBase": kb,

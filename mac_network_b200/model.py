@@ -34,14 +34,16 @@ from .stem import Stem
 class MACnet(object):
     def __init__(self, cfg, netLength, vocab, n_answers, wrd_emb_dim=300, image_in_dim=1024, classifier_dims=(512,),
                  stem_layers=2, seed=0, rank=0, world=1, lr=1e-4, prec="bf16", use_ema=False, answer_decoder=None,
-                 device="cuda", eval_stem_prec=None, eval_enc_prec=None, **trainer_kw):
+                 device="cuda", eval_stem_prec=None, eval_enc_prec=None, train_prec="fp32", **trainer_kw):
         """`vocab`: rows of the question-embedding variable (ids 1..vocab; 0 is padding); `answer_decoder`: optional
         id -> answer string (`answerDict.decodeId`, model.py:699).  `prec`: arithmetic of the evaluation forward; with
         "fp8" the cell's read step runs on e4m3 and the image stem in bf16.  `eval_stem_prec="fp8"` runs the evaluation
         stem in e4m3 (`Stem(prec="fp8")`) and `eval_stem_prec="bf16x3"` in split bf16 inside the fp32 parity bar
         (`Stem(prec="bf16x3")`), whatever `prec` is; None keeps the stem `prec` implies.  `eval_enc_prec="bf16"` runs
         the evaluation question encoder on tensor cores (`QuestionEncoder(prec="bf16")`); None keeps it fp32.  Training is
-        unaffected (see `DPTrainer(enc_prec=)`)."""
+        unaffected (see `DPTrainer(enc_prec=)`).  `train_prec` is the training cell's arithmetic (`DPTrainer(prec=)`: "fp32",
+        "bf16" or "tc32"); the other training precisions pass through as `DPTrainer` keywords (`bwd_tc`, `stem_prec`,
+        `enc_prec`)."""
         if eval_stem_prec not in (None, "fp8", "bf16x3"):
             raise ValueError("eval_stem_prec must be None, 'fp8' or 'bf16x3', got %r" % (eval_stem_prec,))
         if eval_enc_prec not in (None, "bf16"):
@@ -50,7 +52,7 @@ class MACnet(object):
         self.decode = answer_decoder
         self.trainer = DPTrainer(cfg, netLength, seed=seed, rank=rank, world=world, lr=lr, device=device,
                                  classifier=(n_answers, list(classifier_dims)), encoder=(vocab, wrd_emb_dim),
-                                 stem=(image_in_dim, stem_layers), **trainer_kw)
+                                 stem=(image_in_dim, stem_layers), prec=train_prec, **trainer_kw)
         p = self.trainer.params
         t = self.trainer
         # evaluation-mode views of the same variables: every dropout at 1.0 (model.py:118-125)

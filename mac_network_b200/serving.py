@@ -10,9 +10,12 @@ C library; same bits) halves the H2D traffic -- PCIe, not the GPU, bounds this p
 
 `HostPipeline` is that path for the cell alone (its inputs are the encoder's and the stem's outputs); `ModelPipeline` is the
 same scheme for the whole model: question ids and channel-major image features in, answers and attention maps out.
+`TrainPipeline` trains the whole model from host batches: the next batch is staged and copied under the current step.
 """
 import ctypes
 import os
+
+import numpy as np
 import torch
 
 from . import _lib
@@ -618,6 +621,177 @@ class ModelPipeline(object):
         return [dec(int(i)) if dec else int(i) for i in out["answers"][:, 0]]
 
     def drain(self):
+        for s in self.slots:
+            if s.busy:
+                s.done.synchronize()
+
+
+class _TrainSlot(object):
+    """One training batch in flight: pinned host staging and device inputs, the step's pinned results, and the event of the
+    step that reads them."""
+
+    def __init__(self, B, S, C, H, W, device):
+        self.host = {"questions": _pinned(B * S, torch.int32), "questionLengths": _pinned(B, torch.int32),
+                     "answers": _pinned(B, torch.int32), "images": _pinned(B * C * H * W, torch.float32)}
+        self.dev = {k: torch.empty(v.numel(), dtype=v.dtype, device=device) for k, v in self.host.items()}
+        self.out = {"loss": _pinned(1, torch.float32), "gradNorm": _pinned(1, torch.float32),
+                    "correctNum": _pinned(1, torch.int64), "predictions": _pinned(B, torch.int32)}
+        self.copied = torch.cuda.Event()        # the H2D copies, on the copy stream
+        self.done = torch.cuda.Event()          # the step and its D2H copies, on the step's stream
+        self.busy = False
+
+
+class TrainPipeline(object):
+    """Training of the whole model from host buffers: what a caller with numpy or pinned-host batches uses in place of
+    `MACnet.runBatch(train=True)`, with the same steps and the same results.
+
+        pipe = TrainPipeline(model, shape=(B, S_max, H, W), depth=2)
+        t = pipe.submit({"questions": int32 [B, S <= S_max] (0-padded), "questionLengths": int32 [B],
+                         "answers": int32 [B], "images": fp32 [B, C, H, W]})
+        res = pipe.result(t)      # {"loss", "correctNum", "acc", "gradNorm", "predictions" (pinned int32 [B])}
+
+    Per batch, `submit` trims the questions to the longest one (as `runBatch` does, so the trainer's cells are keyed alike),
+    stages the batch into the next of `depth` pinned buffers on `stage_threads` host threads (a pinned `images` tensor is
+    copied from where it lies), copies it to the slot's device buffers on a copy stream, and enqueues
+    `DPTrainer.train_step_full` on the caller's current stream behind that copy's event, with the NCHW features going
+    straight into `Stem.forward_nchw`: the training ingest writes the fp32 NHWC tensor and layer 0's dropped-out patch
+    matrix in one pass (`mac_ingest_nchw_train`).  The loss (mean over the batch), correct count, gradient norm and int32
+    predictions go to pinned memory asynchronously; `result(ticket)` waits for that ticket's step only, and its values stay
+    readable until `depth` further submits.  A slot's pinned and device buffers are written again only after the event of
+    the step that read them.
+
+    `submit` adds no synchronise of its own.  One remains inside the step: the cell reads the scalar logit biases with
+    `.item()` (`MACParams.scalar`) after each optimizer step, so enqueueing step t waits for step t-1 to finish.  The
+    staging and the copy of batch t run before that point, under step t-1's kernels.
+
+    Batches in flight read and write the parameters: call `drain()` before evaluating (`runBatch(train=False)`,
+    `ModelPipeline`, an EMA swap) or saving a checkpoint; training then continues with the next `submit` exactly as if it
+    had not stopped.  With data-parallel training every rank runs its own pipeline over its shard (`global_batch = B * world`).
+    A pinned `images` tensor must not be written until its ticket's result is read."""
+
+    def __init__(self, model, shape, depth=2, stage_threads=None):
+        B, S, H, W = [int(v) for v in shape]
+        t = model.trainer
+        if t.stem is None:
+            raise ValueError("the model's trainer has no stem: TrainPipeline trains the whole model")
+        p = t.params
+        C = int(p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2])
+        nfc = len([k for k in p.t if k.startswith("classifier/linearLayerfc_") and k.endswith("weights/weight")])
+        self.A = int(p.t["classifier/linearLayerfc_%d/weights/weight" % (nfc - 1)].shape[1])
+        if min(B, S, H, W) <= 0 or int(depth) < 1:
+            raise ValueError("shape (B, S_max, H, W) and depth must be positive, got %r, depth = %r" % (shape, depth))
+        if C % 64:
+            raise ValueError("the image features have %d channels: mac_ingest_nchw_train needs a multiple of 64" % C)
+        self.model, self.trainer, self.shape, self.C = model, t, (B, S, H, W), C
+        self.stage_threads = int(stage_threads) if stage_threads else max(1, min(8, usable_cpus() // 2))
+        self._pool = None
+        if self.stage_threads > 1:
+            from concurrent.futures import ThreadPoolExecutor
+            self._pool = ThreadPoolExecutor(self.stage_threads)
+        self.copy_stream = torch.cuda.Stream()
+        self.slots = [_TrainSlot(B, S, C, H, W, p.flat.device) for _ in range(int(depth))]
+        self._next = 0
+
+    def _host(self, batch):
+        """The batch's host tensors and its longest question, checked against the pipeline's shape; ValueError before
+        anything is enqueued."""
+        B, S, H, W = self.shape
+        out = {}
+        for key, dtype in (("questions", torch.int32), ("questionLengths", torch.int32), ("answers", torch.int32),
+                           ("images", torch.float32)):
+            if key not in batch:
+                raise ValueError("the batch has no %s" % key)
+            v = torch.as_tensor(batch[key])
+            if v.device.type != "cpu":
+                raise ValueError("%s must be host memory, got a tensor on %s" % (key, v.device))
+            if key != "images" and (v.dtype.is_floating_point or v.dtype == torch.bool):
+                raise ValueError("%s must hold integers, got %s" % (key, v.dtype))
+            out[key] = v if v.dtype == dtype and v.is_contiguous() else v.to(dtype).contiguous()
+        q, ql, a, img = out["questions"], out["questionLengths"], out["answers"], out["images"]
+        if q.dim() != 2 or q.shape[0] != B or not 1 <= q.shape[1] <= S:
+            raise ValueError("questions must be [%d, S <= %d], got %s" % (B, S, tuple(q.shape)))
+        for key, v in (("questionLengths", ql), ("answers", a)):
+            if tuple(v.shape) != (B,):
+                raise ValueError("%s must be [%d], got %s" % (key, B, tuple(v.shape)))
+        if tuple(img.shape) != (B, self.C, H, W):
+            raise ValueError("images must be [%d, %d, %d, %d] (NCHW), got %s" % (B, self.C, H, W, tuple(img.shape)))
+        longest = int(ql.max())
+        if int(ql.min()) < 0 or not 1 <= longest <= q.shape[1]:
+            raise ValueError("questionLengths must lie in [0, %d] with at least one question, got %d..%d"
+                             % (q.shape[1], int(ql.min()), longest))
+        if int(a.min()) < 0 or int(a.max()) >= self.A:
+            raise ValueError("answers must lie in [0, %d), got %d..%d" % (self.A, int(a.min()), int(a.max())))
+        return q, ql, a, img, longest
+
+    def _stage_images(self, dst, src):
+        """Copy the flat fp32 `src` into the pinned `dst` on the staging threads (numpy copies release the GIL)."""
+        d, s = dst.numpy(), src.reshape(-1).numpy()
+        if self._pool is None:
+            np.copyto(d, s)
+            return
+        n, k = s.size, self.stage_threads
+        cuts = [n * i // k for i in range(k + 1)]
+        list(self._pool.map(lambda i: np.copyto(d[cuts[i]:cuts[i + 1]], s[cuts[i]:cuts[i + 1]]), range(k)))
+
+    def submit(self, batch):
+        """Stage, copy and enqueue one training step; returns its ticket."""
+        q, ql, a, img, S = self._host(batch)
+        B = self.shape[0]
+        tk = self._next
+        slot = self.slots[tk % len(self.slots)]
+        if slot.busy:
+            slot.done.synchronize()             # the step that read this slot's buffers (depth submits back) has finished
+        self._next = tk + 1
+        h, dv = slot.host, slot.dev
+        h["questions"][:B * S].view(B, S).copy_(q[:, :S])
+        h["questionLengths"].copy_(ql)
+        h["answers"].copy_(a)
+        src = img.reshape(-1)
+        if not img.is_pinned():
+            self._stage_images(h["images"], img)
+            src = h["images"]
+        with torch.cuda.stream(self.copy_stream):
+            dv["questions"][:B * S].copy_(h["questions"][:B * S], non_blocking=True)
+            for k in ("questionLengths", "answers"):
+                dv[k].copy_(h[k], non_blocking=True)
+            dv["images"].copy_(src, non_blocking=True)
+            slot.copied.record(self.copy_stream)
+        stream = torch.cuda.current_stream()
+        stream.wait_event(slot.copied)
+        t = self.trainer
+        data = {"questions": dv["questions"][:B * S].view(B, S), "questionLengths": dv["questionLengths"],
+                "answers": dv["answers"], "images_nchw": dv["images"].view(B, self.C, *self.shape[2:])}
+        logits, losses = t.train_step_full((B, S), data, global_batch=B * t.world)
+        self.model.macCell = t._cells[(B, S)][0]
+        preds = torch.argmax(logits, dim=-1).to(torch.int32)                    # as runBatch computes them
+        o = slot.out
+        o["predictions"].copy_(preds, non_blocking=True)
+        o["correctNum"].copy_((preds == data["answers"]).sum().view(1), non_blocking=True)
+        o["loss"].copy_(losses.mean().view(1), non_blocking=True)
+        o["gradNorm"].copy_(t.norm[:1], non_blocking=True)
+        slot.done.record(stream)
+        slot.busy = True
+        return tk
+
+    def result(self, ticket):
+        """Block until the step of `ticket` is done: {"loss", "correctNum", "acc", "gradNorm"} as runBatch(train=True)
+        reports them and "predictions", the pinned int32 [B] answer ids, valid until `depth` further submits."""
+        if not self._next - len(self.slots) <= ticket < self._next:
+            raise ValueError("ticket %r is not one of the last %d submits" % (ticket, len(self.slots)))
+        slot = self.slots[ticket % len(self.slots)]
+        slot.done.synchronize()
+        o = slot.out
+        n = int(o["correctNum"][0])
+        return {"loss": float(o["loss"][0]), "correctNum": n, "acc": n / float(self.shape[0]),
+                "gradNorm": float(o["gradNorm"][0]), "predictions": o["predictions"]}
+
+    def predictions(self, out):
+        """The predictions of a `result` as the model's `answer_decoder` spells them (ids without one)."""
+        dec = self.model.decode
+        return [dec(int(i)) if dec else int(i) for i in out["predictions"]]
+
+    def drain(self):
+        """Wait for every step in flight: afterwards the parameters, optimizer state and EMA are the last step's."""
         for s in self.slots:
             if s.busy:
                 s.done.synchronize()

@@ -21,6 +21,7 @@ from ._lib import act_code, check, ptr, segments, stream_ptr
 
 SITE_STEM = 32            # Philox site base for the stem's input dropouts (site + layer index)
 INGEST_NHWC_F32, INGEST_PATCH_BF16 = 0, 1       # enum MAC_INGEST_* (include/mac_b200.h)
+INGEST_COLS_BF16, INGEST_COLS_SPLIT = 0, 1      # enum MAC_INGEST_COLS_*
 
 
 def stem_specs(in_dim, out_dim, num_layers=2, ksize=3, stem_dim=None):
@@ -114,8 +115,8 @@ class Stem(object):
 
     def forward(self, images, keep=1.0, step=0, save_for_backward=False, _cols0=None):
         """images: [B,H,W,C] fp32 NHWC (the reference transposes the NCHW h5 features first, model.py:~770).
-        Returns the knowledge base [B, H*W, outDim] fp32.  `_cols0` (`forward_nchw`, bf16 inference): layer 0's bf16 patch
-        matrix, already built; `images` then only gives the shape."""
+        Returns the knowledge base [B, H*W, outDim] fp32.  `_cols0` (`forward_nchw`, bf16 and bf16x3 stems): layer 0's patch
+        matrix, already built with this call's keep and step; `images` is then read only by the backward, if at all."""
         x = images
         B, H, Wd, C = x.shape
         act = act_code("RELU", self.relu)
@@ -137,9 +138,12 @@ class Stem(object):
             bf16 = self.prec == "bf16"
             y = torch.empty((M, Nout), dtype=torch.float32, device=self.device)
             if self.prec == "bf16x3":
-                cols = torch.empty((M, 2 * K), dtype=torch.bfloat16, device=self.device)          # [hi | lo]
-                check(self.lib.mac_im2col3x3_split(ptr(x), ptr(cols), float(keep), self.seed, SITE_STEM + i, step, B, H, Wd,
-                                                   C, stream_ptr()), "mac_im2col3x3_split")
+                if i == 0 and _cols0 is not None:
+                    cols = _cols0
+                else:
+                    cols = torch.empty((M, 2 * K), dtype=torch.bfloat16, device=self.device)          # [hi | lo]
+                    check(self.lib.mac_im2col3x3_split(ptr(x), ptr(cols), float(keep), self.seed, SITE_STEM + i, step, B, H,
+                                                       Wd, C, stream_ptr()), "mac_im2col3x3_split")
                 check(self.lib.mac_linear_tc32_fwd(ptr(cols), ptr(Wt), ptr(b), act, ptr(y), M, K, Nout, stream_ptr()),
                       "mac_linear_tc32_fwd")
                 if save_for_backward:
@@ -164,29 +168,49 @@ class Stem(object):
             x = y.view(B, H, Wd, Nout)
         return x.view(B, H * Wd, x.shape[3])
 
-    def forward_nchw(self, images):
-        """Inference forward (keep = 1) from the features in the layout they are stored in: images [B,C,H,W], contiguous,
-        fp32 or -- `prec="bf16"` only, whose layer 0 reads nothing but bf16(x) -- bf16.  `mac_ingest_nchw` (csrc/ingest.cuh)
-        replaces the NHWC permute: for the bf16 stem it writes layer 0's bf16 patch matrix directly, for the other
-        precisions the fp32 NHWC tensor their own patch passes read.  Returns what `forward(images.permute(0, 2, 3, 1))`
-        returns, bit for bit.  C must be a multiple of 64.  Raises before any launch."""
+    def forward_nchw(self, images, keep=1.0, step=0, save_for_backward=False):
+        """`forward` from the features in the layout they are stored in: images [B,C,H,W], contiguous, fp32 or -- `prec="bf16"`
+        inference only, whose layer 0 then reads nothing but bf16(x) -- bf16.  The ingest kernels (csrc/ingest.cuh) replace
+        the NHWC permute.  Inference (keep = 1, no save_for_backward): `mac_ingest_nchw` writes the bf16 stem's layer-0 patch
+        matrix directly, for the other precisions the fp32 NHWC tensor their own patch passes read.  Training (a dropout or
+        save_for_backward): the bf16 and bf16x3 stems run `mac_ingest_nchw_train`, which writes the undropped fp32 NHWC tensor
+        (saved as layer 0's input) and layer 0's dropped-out bf16 or split patch matrix from one read; the fp32 stem runs the
+        NHWC ingest and its usual pass.  Returns -- and saves, and differentiates -- what
+        `forward(images.permute(0, 2, 3, 1).contiguous(), keep, step, save_for_backward)` does, bit for bit.  C must be a
+        multiple of 64.  Raises before any launch."""
         if images.dim() != 4 or not images.is_contiguous():
             raise ValueError("images must be a contiguous [B, C, H, W] tensor")
         if images.dtype not in (torch.float32, torch.bfloat16):
             raise ValueError("images must be float32 or bfloat16, got %s" % images.dtype)
         x_bf16 = int(images.dtype == torch.bfloat16)
-        if x_bf16 and self.prec != "bf16":
-            raise ValueError("bf16 images are for the bf16 stem only: prec=%r reads the fp32 features" % self.prec)
+        train = save_for_backward or float(keep) != 1.0
+        if x_bf16 and (self.prec != "bf16" or train):
+            raise ValueError("bf16 images are for the bf16 stem's inference only: prec=%r%s reads the fp32 features"
+                             % (self.prec, " in training" if train else ""))
         B, C, H, Wd = images.shape
         if C % 64:
             raise NotImplementedError("forward_nchw needs a channel count that is a multiple of 64, got %d" % C)
+        if save_for_backward:
+            self._check_trainable(C)
+        if self.prec == "fp8":
+            self._check_fp8(C, keep)
+        if self.prec == "bf16x3":
+            self._check_tiles(C, "the bf16x3 stem")
+        if train and self.prec in ("bf16", "bf16x3"):
+            split = self.prec == "bf16x3"
+            x = torch.empty((B, H, Wd, C), dtype=torch.float32, device=self.device)
+            cols = torch.empty((B * H * Wd, 9 * C * (2 if split else 1)), dtype=torch.bfloat16, device=self.device)
+            check(self.lib.mac_ingest_nchw_train(ptr(images), ptr(x), ptr(cols), INGEST_COLS_SPLIT if split else INGEST_COLS_BF16,
+                                                 float(keep), self.seed, SITE_STEM, int(step), B, C, H, Wd, stream_ptr()),
+                  "mac_ingest_nchw_train")
+            return self.forward(x, keep, step, save_for_backward, _cols0=cols)
         if self.prec != "bf16":
             if self.prec == "fp8":
                 self._check_fp8(C, 1.0)
             x = torch.empty((B, H, Wd, C), dtype=torch.float32, device=self.device)
             check(self.lib.mac_ingest_nchw(ptr(images), x_bf16, ptr(x), INGEST_NHWC_F32, B, C, H, Wd, stream_ptr()),
                   "mac_ingest_nchw")
-            return self.forward(x)
+            return self.forward(x, keep, step, save_for_backward)
         cols = torch.empty((B * H * Wd, 9 * C), dtype=torch.bfloat16, device=self.device)
         check(self.lib.mac_ingest_nchw(ptr(images), x_bf16, ptr(cols), INGEST_PATCH_BF16, B, C, H, Wd, stream_ptr()),
               "mac_ingest_nchw")
