@@ -480,6 +480,17 @@ int mac_ingest_nchw_train(const float* x_nchw, float* x_nhwc, void* cols, int co
  * out not 16-byte aligned -> MAC_ERR_ALIGN. */
 int mac_kb_gather(const float* kb_u, const int32_t* index, void* out, int out_bf16, int B, int U, int N, int d,
                   mac_stream_t stream);
+/* Backward of mac_kb_gather (csrc/ingest.cuh; DPTrainer with data["imageIndex"], serving.TrainPipeline(images=)):
+ *   d_kb_u[u, n, :] = sum over b ascending with index[b] == u of d_out[b, n, :]   for u < U
+ * d_out: fp32 [B, N, d], the gradient of the gathered knowledge bases; index: int32 [B] in device memory; d_kb_u: fp32
+ * [U, N, d].  The sum is fp32 and starts from the first matching row itself (a lone term is copied exactly, -0.0 included);
+ * each later term is added in ascending b, so the result is that sequential float32 sum bit for bit, and reruns are
+ * identical (no atomics).  Every d_kb_u row is written, never read: an image no question uses gets zeros.  An index outside
+ * [0, U) contributes nothing.  Reads each d_out row once and writes each d_kb_u row once, 16-byte accesses.  Before any
+ * launch: a null pointer or B, U, N, d <= 0 -> MAC_ERR_INVALID; d % 8 != 0 or N*d/8 > 2^31 - 1 -> MAC_ERR_UNSUPPORTED;
+ * d_out, index or d_kb_u not 16-byte aligned -> MAC_ERR_ALIGN. */
+int mac_kb_gather_bwd(const float* d_out, const int32_t* index, float* d_kb_u, int B, int U, int N, int d,
+                      mac_stream_t stream);
 /* Inference stem layer in e4m3 (csrc/tc_gemm_fp8.cuh; Stem(prec="fp8")), no dropout.  All scales fp32; e4m3 rounds to nearest
  * even and saturates at +-448.
  * mac_im2col3x3_fp8: the patch matrix of mac_im2col3x3 (same tap-major, channel-fastest layout) as e4m3 cols_e4m3 [M, 9C],

@@ -291,4 +291,60 @@ static int kb_gather_launch(const float* kb_u, const int* index, void* out, int 
   return MAC_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ knowledge-base gather: backward
+// The gradient of the gather: d_kb_u[u] = sum over b ascending with index[b] == u of d_out[b], in fp32, starting from the first
+// matching row itself (a lone term is copied, -0.0 included) and adding the later ones in ascending b; an image no question
+// uses gets zeros, an index outside [0, U) contributes nothing.  The order is fixed, so the result is that sequential float32
+// sum bit for bit, with no atomics.  Same vectors as the gather: blockIdx.x cuts a sample's run of N*d elements into GATHER_V
+// -element vectors, blockIdx.y (striding by gridDim.y past 65535) picks the image.  Every thread of a block scans the same
+// index entries, staged through shared memory GATHER_BWD_CHUNK at a time (any B), so the branch on a match is uniform.  Each
+// question row is read by the one block column of its image: B*N*d*4 bytes read, U*N*d*4 written.
+constexpr int GATHER_BWD_CHUNK = 1024;
+
+__global__ void __launch_bounds__(GATHER_THREADS) kb_gather_bwd_kernel(const float4* __restrict__ d_out,
+                                                                       const int* __restrict__ index,
+                                                                       float4* __restrict__ d_kb_u, int B, int U, int nvec) {
+  __shared__ int s_idx[GATHER_BWD_CHUNK];
+  const int j = blockIdx.x * GATHER_THREADS + threadIdx.x;          // vector within the sample's run
+  const bool live = j < nvec;                                        // the others still stage the index
+  for (int u = blockIdx.y; u < U; u += gridDim.y) {
+    float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
+    bool first = true;
+    for (int b0 = 0; b0 < B; b0 += GATHER_BWD_CHUNK) {
+      const int n = min(GATHER_BWD_CHUNK, B - b0);
+      __syncthreads();                                               // the previous chunk has been scanned
+      for (int i = threadIdx.x; i < n; i += GATHER_THREADS) s_idx[i] = __ldg(index + b0 + i);
+      __syncthreads();
+      if (!live) continue;
+      for (int i = 0; i < n; ++i) {
+        if (s_idx[i] != u) continue;
+        const float4* src = d_out + ((size_t)(b0 + i) * nvec + j) * 2;
+        const float4 a = __ldg(src), c = __ldg(src + 1);
+        if (first) {
+          lo = a;
+          hi = c;
+          first = false;
+        } else {
+          lo.x += a.x; lo.y += a.y; lo.z += a.z; lo.w += a.w;
+          hi.x += c.x; hi.y += c.y; hi.z += c.z; hi.w += c.w;
+        }
+      }
+    }
+    if (live) {
+      float4* dst = d_kb_u + ((size_t)u * nvec + j) * 2;
+      dst[0] = lo;
+      dst[1] = hi;
+    }
+  }
+}
+
+static int kb_gather_bwd_launch(const float* d_out, const int* index, float* d_kb_u, int B, int U, int nvec,
+                                cudaStream_t stream) {
+  const dim3 grid((unsigned)((nvec + GATHER_THREADS - 1) / GATHER_THREADS), (unsigned)(U < 65535 ? U : 65535));
+  kb_gather_bwd_kernel<<<grid, GATHER_THREADS, 0, stream>>>(reinterpret_cast<const float4*>(d_out), index,
+                                                            reinterpret_cast<float4*>(d_kb_u), B, U, nvec);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
 }  // namespace mac

@@ -693,6 +693,15 @@ extern "C" int mac_kb_gather(const float* kb_u, const int* index, void* out, int
   return kb_gather_launch(kb_u, index, out, out_bf16, B, U, (int)((long long)N * d / GATHER_V), stream);
 }
 
+extern "C" int mac_kb_gather_bwd(const float* d_out, const int* index, float* d_kb_u, int B, int U, int N, int d,
+                                 mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!d_out || !index || !d_kb_u || B <= 0 || U <= 0 || N <= 0 || d <= 0) return MAC_ERR_INVALID;
+  if ((d % GATHER_V) || (long long)N * d / GATHER_V > 0x7fffffffLL) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(d_out) || !mac_aligned16(index) || !mac_aligned16(d_kb_u)) return MAC_ERR_ALIGN;
+  return kb_gather_bwd_launch(d_out, index, d_kb_u, B, U, (int)((long long)N * d / GATHER_V), stream);
+}
+
 // ------------------------------------------------------------------------------------------------ stem: split-bf16 patches
 // The patch matrix of mac_im2col3x3 as the A operand of tc3_gemm: cols2[m, k] = bf16(v), cols2[m, 9C + k] = bf16(v - hi) with
 // v the fp32 value mac_im2col3x3 writes at cols[m, k] (same Philox draw: the quad index of the SOURCE element).  Eight

@@ -225,7 +225,17 @@ class DPTrainer(object):
         one of `images` fp32 [B,H,W,C] (NHWC: the reference transposes its NCHW feed first, model.py:68) or `images_nchw`
         fp32 [B,C,H,W], contiguous, as the features are stored (`Stem.forward_nchw`: the ingest kernel replaces the permute
         and, for the bf16 and bf16x3 stems, layer 0's patch pass; the same results bit for bit).  Returns (logits,
-        per-sample losses)."""
+        per-sample losses).
+
+        Several questions per image: with `imageIndex`, a contiguous int32 [B] tensor on the trainer's device, the images
+        carry k <= B distinct rows and question b asks about image imageIndex[b], which must lie in [0, k) (the caller's
+        contract; `serving.TrainPipeline(images=U)` checks it on the host).  The stem runs over the k images, so its
+        dropout is drawn once per image -- image u gets the mask that batch row u gets without an index -- where the
+        per-question step draws one per question.  `mac_kb_gather` writes each question's knowledge base into the cell's
+        fp32 input, and after the cell's backward `mac_kb_gather_bwd` sums each image's knowledge-base gradient over its
+        questions (fp32, ascending question order) for the stem's backward: the exact gradient of that objective.
+        Everything after the stem -- the cell and its per-question read dropout, the encoder, the output unit, the loss --
+        is the step without an index.  With imageIndex = arange(B) and all B images the step is that step bit for bit."""
         from .autograd import mac_backward
         from .mac_cell import mac_network
         if self.enc is None:
@@ -237,6 +247,9 @@ class DPTrainer(object):
         if nchw is not None and (nchw.device != self.params.flat.device or nchw.dtype != torch.float32 or nchw.dim() != 4
                                  or not nchw.is_contiguous()):
             raise ValueError("images_nchw must be a contiguous fp32 [B, C, H, W] tensor on %s" % self.params.flat.device)
+        idx = data.get("imageIndex")
+        if idx is not None:
+            self._check_image_index(idx, data["questions"].shape[0], (data["images"] if nchw is None else nchw).shape[0])
         seed = (self.base_seed * 1000003 + self.step_id * 7919 + self.rank * 104729 + 1) & 0x7FFFFFFFFFFFFFFF
         self.enc.seed = self.stem.seed = self.out.seed = seed
         words, cntx, vecq = self.enc.forward(data["questions"], data["questionLengths"], step=self.step_id,
@@ -245,6 +258,8 @@ class DPTrainer(object):
             kb = self.stem.forward_nchw(nchw, keep=self.stem_dropout, step=self.step_id, save_for_backward=True)
         else:
             kb = self.stem.forward(data["images"], keep=self.stem_dropout, step=self.step_id, save_for_backward=True)
+        if idx is not None:
+            kb_u, kb = kb, self._gather_kb(key, kb, idx)
         # the cell captures its inputs at construction (mac_cell.py:59-79): cell_for owns persistent buffers per key and
         # copies this step's encoder / stem outputs into them
         bufs = {"vecQuestions": vecq, "questionWords": words, "questionCntxWords": cntx, "knowledgeBase": kb,
@@ -259,11 +274,45 @@ class DPTrainer(object):
         d_mem, d_q = torch.zeros_like(memory), torch.zeros_like(memory)
         self.out.backward(gviews, d_mem, d_q)
         g = mac_backward(cell, None, d_mem, bucket=self.bucket, zero_bucket=False, d_vecq=d_q, tc=self.bwd_tc)
-        self.stem.backward(g["knowledgeBase"], gviews)
+        d_kb = g["knowledgeBase"]
+        if idx is not None:
+            d_kb = self._sum_kb_grad(d_kb.contiguous(), idx, kb_u.shape[0])
+        self.stem.backward(d_kb, gviews)
         if not self.cfg.controlContextual:
             raise NotImplementedError("the raw-word control inputs (controlContextual off) need wrdEmbDim == ctrlDim")
         self.enc.backward(g["questionCntxWords"], g["vecQuestions"], gviews)
         return logits, losses
+
+    def _check_image_index(self, idx, B, k):
+        """Refuse a malformed `imageIndex` or image count before any launch (no synchronise: the values are not read)."""
+        dev = self.params.flat.device
+        if not (torch.is_tensor(idx) and idx.dtype == torch.int32 and idx.is_cuda and idx.device == dev and idx.dim() == 1
+                and idx.is_contiguous() and idx.shape[0] == B and idx.data_ptr() % 16 == 0):
+            raise ValueError("imageIndex must be a contiguous, 16-byte aligned int32 tensor of shape [%d] on %s" % (B, dev))
+        if not 1 <= k <= B:
+            raise ValueError("with imageIndex the images carry 1..%d distinct rows (one per image), got %d" % (B, k))
+        if self.cfg.memDim % 8:
+            raise NotImplementedError("imageIndex needs memDim %% 8 == 0 (mac_kb_gather's 16-byte vectors), got %d"
+                                      % self.cfg.memDim)
+
+    def _gather_kb(self, key, kb_u, idx):
+        """Each question's knowledge base from the k images' [k, N, d]: straight into the persistent buffer of `key`'s cell
+        when it exists (so `cell_for` copies nothing), else into a new tensor that the new cell's buffer is made from."""
+        B, (_, N, d) = idx.shape[0], kb_u.shape
+        ent = self._cells.get(key)
+        out = ent[1]["knowledgeBase"] if ent is not None else None
+        if out is None or tuple(out.shape) != (B, N, d) or out.dtype != torch.float32:
+            out = torch.empty((B, N, d), dtype=torch.float32, device=kb_u.device)
+        check(self.lib.mac_kb_gather(ptr(kb_u), ptr(idx), ptr(out), 0, B, kb_u.shape[0], N, d, stream_ptr()),
+              "mac_kb_gather")
+        return out
+
+    def _sum_kb_grad(self, d_kb, idx, k):
+        """The k images' knowledge-base gradient [k, N, d]: each question's [B, N, d] row summed over its image's questions."""
+        B, N, d = d_kb.shape
+        out = torch.empty((k, N, d), dtype=torch.float32, device=d_kb.device)
+        check(self.lib.mac_kb_gather_bwd(ptr(d_kb), ptr(idx), ptr(out), B, k, N, d, stream_ptr()), "mac_kb_gather_bwd")
+        return out
 
     def train_step_full(self, key, data, global_batch):
         """One data-parallel step of the whole model: `full_forward_backward` -> all-reduce -> clip / Adam / EMA."""

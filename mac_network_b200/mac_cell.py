@@ -172,8 +172,9 @@ class MACCell(object):
             raise ValueError("a bf16 knowledge base must be a contiguous CUDA tensor")
         self.kbIndex = kbIndex
         if kbIndex is not None:
-            # training draws the read dropout (and the stem's) per question, and dKB would be a segmented sum over the
-            # questions of each image: shared knowledge bases are an inference form
+            # training draws the read dropout per question and needs dKB per image, a sum over each image's questions: the
+            # trainer gathers outside the cell instead (DPTrainer.full_forward_backward with data["imageIndex"],
+            # mac_kb_gather_bwd), so the cell's shared knowledge bases are an inference form
             if save_for_backward or min(float(memoryDropout), float(readDropout), float(writeDropout)) < 1.0:
                 raise NotImplementedError("kbIndex (knowledge bases shared between questions) is inference only: "
                                           "save_for_backward=False and every dropout 1.0")

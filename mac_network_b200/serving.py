@@ -630,9 +630,12 @@ class _TrainSlot(object):
     """One training batch in flight: pinned host staging and device inputs, the step's pinned results, and the event of the
     step that reads them."""
 
-    def __init__(self, B, S, C, H, W, device):
+    def __init__(self, B, S, C, H, W, device, images=None):
         self.host = {"questions": _pinned(B * S, torch.int32), "questionLengths": _pinned(B, torch.int32),
-                     "answers": _pinned(B, torch.int32), "images": _pinned(B * C * H * W, torch.float32)}
+                     "answers": _pinned(B, torch.int32),
+                     "images": _pinned((B if images is None else images) * C * H * W, torch.float32)}
+        if images is not None:      # question b asks about image imageIndex[b] of the batch's k <= U
+            self.host["imageIndex"] = _pinned(B, torch.int32)
         self.dev = {k: torch.empty(v.numel(), dtype=v.dtype, device=device) for k, v in self.host.items()}
         self.out = {"loss": _pinned(1, torch.float32), "gradNorm": _pinned(1, torch.float32),
                     "correctNum": _pinned(1, torch.int64), "predictions": _pinned(B, torch.int32)}
@@ -667,9 +670,22 @@ class TrainPipeline(object):
     Batches in flight read and write the parameters: call `drain()` before evaluating (`runBatch(train=False)`,
     `ModelPipeline`, an EMA swap) or saving a checkpoint; training then continues with the next `submit` exactly as if it
     had not stopped.  With data-parallel training every rank runs its own pipeline over its shard (`global_batch = B * world`).
-    A pinned `images` tensor must not be written until its ticket's result is read."""
+    A pinned `images` tensor must not be written until its ticket's result is read.
 
-    def __init__(self, model, shape, depth=2, stage_threads=None):
+    Several questions per image: with `images=U` (1 <= U <= B) a batch carries k <= U distinct images and each question's
+    image number, as `ModelPipeline(images=U)` takes them,
+
+        pipe = TrainPipeline(model, shape=(B, S_max, H, W), depth=2, images=16)
+        t = pipe.submit({"questions": ..., "questionLengths": ..., "answers": ..., "images": fp32 [k, C, H, W],
+                         "imageIndex": int32 [B]})
+
+    with 1 <= k <= U and every imageIndex[b] in [0, k).  The slots' pinned and device image buffers hold U images; only the k
+    images are staged and copied, and the stem runs forward and backward over those k
+    (`DPTrainer.full_forward_backward` with `imageIndex`: `mac_kb_gather`, `mac_kb_gather_bwd`).  The stem's input dropout is
+    then drawn once per image, not once per question; everything after the stem is the step without an index.  With each
+    rank's shard, each rank passes its own images and index.  Bad batches raise `ValueError` before anything is staged."""
+
+    def __init__(self, model, shape, depth=2, stage_threads=None, images=None):
         B, S, H, W = [int(v) for v in shape]
         t = model.trainer
         if t.stem is None:
@@ -682,6 +698,9 @@ class TrainPipeline(object):
             raise ValueError("shape (B, S_max, H, W) and depth must be positive, got %r, depth = %r" % (shape, depth))
         if C % 64:
             raise ValueError("the image features have %d channels: mac_ingest_nchw_train needs a multiple of 64" % C)
+        if images is not None and not (isinstance(images, int) and not isinstance(images, bool) and 1 <= images <= B):
+            raise ValueError("images must be None or an int in 1..B = %d, got %r" % (B, images))
+        self.images = images
         self.model, self.trainer, self.shape, self.C = model, t, (B, S, H, W), C
         self.stage_threads = int(stage_threads) if stage_threads else max(1, min(8, usable_cpus() // 2))
         self._pool = None
@@ -689,16 +708,21 @@ class TrainPipeline(object):
             from concurrent.futures import ThreadPoolExecutor
             self._pool = ThreadPoolExecutor(self.stage_threads)
         self.copy_stream = torch.cuda.Stream()
-        self.slots = [_TrainSlot(B, S, C, H, W, p.flat.device) for _ in range(int(depth))]
+        self.slots = [_TrainSlot(B, S, C, H, W, p.flat.device, images) for _ in range(int(depth))]
         self._next = 0
 
     def _host(self, batch):
-        """The batch's host tensors and its longest question, checked against the pipeline's shape; ValueError before
-        anything is enqueued."""
+        """The batch's host tensors (with images=U also its image index, else None) and its longest question, checked against
+        the pipeline's shape; ValueError before anything is enqueued."""
         B, S, H, W = self.shape
+        if self.images is None and "imageIndex" in batch:
+            raise ValueError("imageIndex is for a pipeline built with images=U")
         out = {}
-        for key, dtype in (("questions", torch.int32), ("questionLengths", torch.int32), ("answers", torch.int32),
-                           ("images", torch.float32)):
+        keys = (("questions", torch.int32), ("questionLengths", torch.int32), ("answers", torch.int32),
+                ("images", torch.float32))
+        if self.images is not None:
+            keys += (("imageIndex", torch.int32),)
+        for key, dtype in keys:
             if key not in batch:
                 raise ValueError("the batch has no %s" % key)
             v = torch.as_tensor(batch[key])
@@ -713,15 +737,27 @@ class TrainPipeline(object):
         for key, v in (("questionLengths", ql), ("answers", a)):
             if tuple(v.shape) != (B,):
                 raise ValueError("%s must be [%d], got %s" % (key, B, tuple(v.shape)))
-        if tuple(img.shape) != (B, self.C, H, W):
-            raise ValueError("images must be [%d, %d, %d, %d] (NCHW), got %s" % (B, self.C, H, W, tuple(img.shape)))
+        idx = None
+        if self.images is None:
+            if tuple(img.shape) != (B, self.C, H, W):
+                raise ValueError("images must be [%d, %d, %d, %d] (NCHW), got %s" % (B, self.C, H, W, tuple(img.shape)))
+        else:
+            if img.dim() != 4 or tuple(img.shape[1:]) != (self.C, H, W) or not 1 <= img.shape[0] <= self.images:
+                raise ValueError("images must be [k, %d, %d, %d] (NCHW) with 1 <= k <= %d, got %s"
+                                 % (self.C, H, W, self.images, tuple(img.shape)))
+            idx = out["imageIndex"]
+            if tuple(idx.shape) != (B,):
+                raise ValueError("imageIndex must be [%d], got %s" % (B, tuple(idx.shape)))
+            if int(idx.min()) < 0 or int(idx.max()) >= img.shape[0]:
+                raise ValueError("imageIndex must lie in [0, %d) (the batch's images), got %d..%d"
+                                 % (img.shape[0], int(idx.min()), int(idx.max())))
         longest = int(ql.max())
         if int(ql.min()) < 0 or not 1 <= longest <= q.shape[1]:
             raise ValueError("questionLengths must lie in [0, %d] with at least one question, got %d..%d"
                              % (q.shape[1], int(ql.min()), longest))
         if int(a.min()) < 0 or int(a.max()) >= self.A:
             raise ValueError("answers must lie in [0, %d), got %d..%d" % (self.A, int(a.min()), int(a.max())))
-        return q, ql, a, img, longest
+        return q, ql, a, img, idx, longest
 
     def _stage_images(self, dst, src):
         """Copy the flat fp32 `src` into the pinned `dst` on the staging threads (numpy copies release the GIL)."""
@@ -735,8 +771,9 @@ class TrainPipeline(object):
 
     def submit(self, batch):
         """Stage, copy and enqueue one training step; returns its ticket."""
-        q, ql, a, img, S = self._host(batch)
+        q, ql, a, img, idx, S = self._host(batch)
         B = self.shape[0]
+        n = img.numel()                         # B images, or the batch's k <= U with images=U
         tk = self._next
         slot = self.slots[tk % len(self.slots)]
         if slot.busy:
@@ -746,21 +783,27 @@ class TrainPipeline(object):
         h["questions"][:B * S].view(B, S).copy_(q[:, :S])
         h["questionLengths"].copy_(ql)
         h["answers"].copy_(a)
+        small = ("questionLengths", "answers")
+        if idx is not None:
+            h["imageIndex"].copy_(idx)
+            small += ("imageIndex",)
         src = img.reshape(-1)
         if not img.is_pinned():
-            self._stage_images(h["images"], img)
-            src = h["images"]
+            self._stage_images(h["images"][:n], img)
+            src = h["images"][:n]
         with torch.cuda.stream(self.copy_stream):
             dv["questions"][:B * S].copy_(h["questions"][:B * S], non_blocking=True)
-            for k in ("questionLengths", "answers"):
+            for k in small:
                 dv[k].copy_(h[k], non_blocking=True)
-            dv["images"].copy_(src, non_blocking=True)
+            dv["images"][:n].copy_(src, non_blocking=True)
             slot.copied.record(self.copy_stream)
         stream = torch.cuda.current_stream()
         stream.wait_event(slot.copied)
         t = self.trainer
         data = {"questions": dv["questions"][:B * S].view(B, S), "questionLengths": dv["questionLengths"],
-                "answers": dv["answers"], "images_nchw": dv["images"].view(B, self.C, *self.shape[2:])}
+                "answers": dv["answers"], "images_nchw": dv["images"][:n].view(img.shape[0], self.C, *self.shape[2:])}
+        if idx is not None:
+            data["imageIndex"] = dv["imageIndex"]
         logits, losses = t.train_step_full((B, S), data, global_batch=B * t.world)
         self.model.macCell = t._cells[(B, S)][0]
         preds = torch.argmax(logits, dim=-1).to(torch.int32)                    # as runBatch computes them
