@@ -480,6 +480,21 @@ int mac_ingest_nchw_train(const float* x_nchw, float* x_nhwc, void* cols, int co
  * out not 16-byte aligned -> MAC_ERR_ALIGN. */
 int mac_kb_gather(const float* kb_u, const int32_t* index, void* out, int out_bf16, int B, int U, int N, int d,
                   mac_stream_t stream);
+/* A device-resident cache of knowledge bases (csrc/ingest.cuh; serving.ModelPipeline(cache=C)): a pool of `capacity` rows
+ * [capacity, N, d], fp32 (pool_bf16 = 0) or bf16 (pool_bf16 = 1).
+ *   pool[slot[u], n, :] = kb_u[u, n, :]   for every u < U with 0 <= slot[u] < capacity
+ * kb_u: the stem's fp32 output [U, N, d]; slot: int32 [U] in device memory (a captured graph replays with a new one).  A
+ * bf16 row is rounded to nearest even, bit for bit what mac_cast_bf16 makes of the fp32 row.  Any other slot value (-1 for
+ * the stem's padding rows) writes nothing and reads nothing.  Two u with the same slot in one call: the row written is then
+ * unspecified.  16-byte accesses.  Before any launch: a null pointer or U, capacity, N, d <= 0 -> MAC_ERR_INVALID; pool_bf16
+ * not 0 or 1, d % 8 != 0 or N*d/8 > 2^31 - 1 -> MAC_ERR_UNSUPPORTED; kb_u, slot or pool not 16-byte aligned -> MAC_ERR_ALIGN. */
+int mac_kb_pool_insert(const float* kb_u, const int32_t* slot, void* pool, int pool_bf16, int U, int capacity, int N, int d,
+                       mac_stream_t stream);
+/* mac_kb_gather from a bf16 source: out[b, n, :] = kb_u[index[b], n, :] for b < B, kb_u bf16 [U, N, d] (the bf16 pool of
+ * mac_kb_pool_insert), out bf16 [B, N, d]: a copy.  A row whose index lies outside [0, U) is written as bf16 NaN (0x7fc0)
+ * and nothing is read for it.  16-byte accesses.  Before any launch: a null pointer or B, U, N, d <= 0 -> MAC_ERR_INVALID;
+ * d % 8 != 0 or N*d/8 > 2^31 - 1 -> MAC_ERR_UNSUPPORTED; kb_u, index or out not 16-byte aligned -> MAC_ERR_ALIGN. */
+int mac_kb_gather_bf16(const void* kb_u, const int32_t* index, void* out, int B, int U, int N, int d, mac_stream_t stream);
 /* Backward of mac_kb_gather (csrc/ingest.cuh; DPTrainer with data["imageIndex"], serving.TrainPipeline(images=)):
  *   d_kb_u[u, n, :] = sum over b ascending with index[b] == u of d_out[b, n, :]   for u < U
  * d_out: fp32 [B, N, d], the gradient of the gathered knowledge bases; index: int32 [B] in device memory; d_kb_u: fp32

@@ -107,6 +107,8 @@ PROTOTYPES = {
     "mac_ingest_nchw_train": (c_int, [c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_int, c_int, c_int, c_int, c_fp]),
     "mac_kb_gather": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_int, c_int, c_int, c_fp]),
     "mac_kb_gather_bwd": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_kb_pool_insert": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_kb_gather_bf16": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_int, c_int, c_fp]),
     "mac_im2col3x3": (c_int, [c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_int, c_int, c_int, c_int, c_fp]),
     "mac_im2col3x3_fp8": (c_int, [c_fp, c_fp, c_fp, c_fp, c_sz, c_int, c_int, c_int, c_int, c_fp]),
     "mac_im2col3x3_fp8_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int]),

@@ -291,6 +291,75 @@ static int kb_gather_launch(const float* kb_u, const int* index, void* out, int 
   return MAC_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ knowledge-base pool
+// The device-resident cache of knowledge bases (serving.ModelPipeline(cache=C)): a pool of `capacity` rows of N*d elements,
+// fp32 or bf16.  The insert writes the stem's output rows into it, pool[slot[u]] = kb_u[u] (bf16 rounded to nearest even as
+// cast_bf16_kernel rounds); a slot outside [0, capacity) -- the stem's padding rows carry -1 -- writes nothing.  Same vectors
+// and grid as the gather, with blockIdx.y picking the stem row u.  Two rows u with the same slot race: the caller's error.
+template <bool BF16>
+__global__ void __launch_bounds__(GATHER_THREADS) kb_pool_insert_kernel(const float4* __restrict__ kb_u,
+                                                                        const int* __restrict__ slot, void* __restrict__ pool,
+                                                                        int U, int capacity, int nvec) {
+  const int j = blockIdx.x * GATHER_THREADS + threadIdx.x;          // vector within the sample's run
+  if (j >= nvec) return;
+  for (int u = blockIdx.y; u < U; u += gridDim.y) {
+    const int r = __ldg(slot + u);
+    if (r < 0 || r >= capacity) continue;
+    const float4* src = kb_u + ((size_t)u * nvec + j) * 2;
+    const float4 lo = __ldg(src), hi = __ldg(src + 1);
+    const size_t o = (size_t)r * nvec + j;
+    if constexpr (BF16) {
+      __nv_bfloat162 p0 = __floats2bfloat162_rn(lo.x, lo.y), p1 = __floats2bfloat162_rn(lo.z, lo.w);
+      __nv_bfloat162 p2 = __floats2bfloat162_rn(hi.x, hi.y), p3 = __floats2bfloat162_rn(hi.z, hi.w);
+      uint4 v;
+      v.x = *reinterpret_cast<uint32_t*>(&p0);
+      v.y = *reinterpret_cast<uint32_t*>(&p1);
+      v.z = *reinterpret_cast<uint32_t*>(&p2);
+      v.w = *reinterpret_cast<uint32_t*>(&p3);
+      reinterpret_cast<uint4*>(pool)[o] = v;
+    } else {
+      float4* dst = reinterpret_cast<float4*>(pool) + o * 2;
+      dst[0] = lo;
+      dst[1] = hi;
+    }
+  }
+}
+
+static int kb_pool_insert_launch(const float* kb_u, const int* slot, void* pool, int pool_bf16, int U, int capacity, int nvec,
+                                 cudaStream_t stream) {
+  const dim3 grid((unsigned)((nvec + GATHER_THREADS - 1) / GATHER_THREADS), (unsigned)(U < 65535 ? U : 65535));
+  const float4* src = reinterpret_cast<const float4*>(kb_u);
+  if (pool_bf16)
+    kb_pool_insert_kernel<true><<<grid, GATHER_THREADS, 0, stream>>>(src, slot, pool, U, capacity, nvec);
+  else
+    kb_pool_insert_kernel<false><<<grid, GATHER_THREADS, 0, stream>>>(src, slot, pool, U, capacity, nvec);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+// The gather from the bf16 pool: out[b] = kb_u[index[b]], bf16 to bf16, a copy.  One 16-byte vector (eight elements) per
+// thread and question; an index outside [0, U) writes a row of bf16 quiet NaNs (0x7fc0) and reads nothing.
+__global__ void __launch_bounds__(GATHER_THREADS) kb_gather_bf16_kernel(const uint4* __restrict__ kb_u,
+                                                                        const int* __restrict__ index,
+                                                                        uint4* __restrict__ out, int B, int U, int nvec) {
+  const int j = blockIdx.x * GATHER_THREADS + threadIdx.x;          // vector within the sample's run
+  if (j >= nvec) return;
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const int u = __ldg(index + b);
+    const uint4 v = (u >= 0 && u < U) ? __ldg(kb_u + (size_t)u * nvec + j)
+                                      : make_uint4(0x7fc07fc0u, 0x7fc07fc0u, 0x7fc07fc0u, 0x7fc07fc0u);
+    out[(size_t)b * nvec + j] = v;
+  }
+}
+
+static int kb_gather_bf16_launch(const void* kb_u, const int* index, void* out, int B, int U, int nvec, cudaStream_t stream) {
+  const dim3 grid((unsigned)((nvec + GATHER_THREADS - 1) / GATHER_THREADS), (unsigned)(B < 65535 ? B : 65535));
+  kb_gather_bf16_kernel<<<grid, GATHER_THREADS, 0, stream>>>(reinterpret_cast<const uint4*>(kb_u), index,
+                                                             reinterpret_cast<uint4*>(out), B, U, nvec);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ knowledge-base gather: backward
 // The gradient of the gather: d_kb_u[u] = sum over b ascending with index[b] == u of d_out[b], in fp32, starting from the first
 // matching row itself (a lone term is copied, -0.0 included) and adding the later ones in ascending b; an image no question

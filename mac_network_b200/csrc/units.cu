@@ -693,6 +693,25 @@ extern "C" int mac_kb_gather(const float* kb_u, const int* index, void* out, int
   return kb_gather_launch(kb_u, index, out, out_bf16, B, U, (int)((long long)N * d / GATHER_V), stream);
 }
 
+extern "C" int mac_kb_pool_insert(const float* kb_u, const int* slot, void* pool, int pool_bf16, int U, int capacity, int N,
+                                  int d, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!kb_u || !slot || !pool || U <= 0 || capacity <= 0 || N <= 0 || d <= 0) return MAC_ERR_INVALID;
+  if ((pool_bf16 != 0 && pool_bf16 != 1) || (d % GATHER_V) || (long long)N * d / GATHER_V > 0x7fffffffLL)
+    return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(kb_u) || !mac_aligned16(slot) || !mac_aligned16(pool)) return MAC_ERR_ALIGN;
+  return kb_pool_insert_launch(kb_u, slot, pool, pool_bf16, U, capacity, (int)((long long)N * d / GATHER_V), stream);
+}
+
+extern "C" int mac_kb_gather_bf16(const void* kb_u, const int* index, void* out, int B, int U, int N, int d,
+                                  mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!kb_u || !index || !out || B <= 0 || U <= 0 || N <= 0 || d <= 0) return MAC_ERR_INVALID;
+  if ((d % GATHER_V) || (long long)N * d / GATHER_V > 0x7fffffffLL) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(kb_u) || !mac_aligned16(index) || !mac_aligned16(out)) return MAC_ERR_ALIGN;
+  return kb_gather_bf16_launch(kb_u, index, out, B, U, (int)((long long)N * d / GATHER_V), stream);
+}
+
 extern "C" int mac_kb_gather_bwd(const float* d_out, const int* index, float* d_kb_u, int B, int U, int N, int d,
                                  mac_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);

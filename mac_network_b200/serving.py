@@ -12,6 +12,7 @@ C library; same bits) halves the H2D traffic -- PCIe, not the GPU, bounds this p
 same scheme for the whole model: question ids and channel-major image features in, answers and attention maps out.
 `TrainPipeline` trains the whole model from host batches: the next batch is staged and copied under the current step.
 """
+import collections
 import ctypes
 import os
 
@@ -19,6 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import check, ptr, stream_ptr
 from .mac_cell import MACCell, mac_network
 
 
@@ -377,8 +379,7 @@ class _ModelSlot(object):
                   "questionLengths": torch.full((B,), S, dtype=torch.int32, device=p.device),
                   "images": torch.zeros(B if images is None else images, C, H, W, device=p.device,
                                         dtype=torch.bfloat16 if images_bf16 else torch.float32)}
-        if images is not None:      # question b reads image imageIndex[b] of the U the stem runs over
-            self.x["imageIndex"] = torch.zeros(B, dtype=torch.int32, device=p.device)
+        self.x.update(self._index_inputs(B, images, p.device))
         from .encoder import QuestionEncoder
         from .output_unit import OutputUnit
         from .stem import Stem
@@ -395,14 +396,23 @@ class _ModelSlot(object):
         self.busy = False
         self.capture()
 
+    def _index_inputs(self, B, images, device):
+        """The graph's device index inputs: with images=U, question b reads image imageIndex[b] of the U the stem runs over."""
+        return {} if images is None else {"imageIndex": torch.zeros(B, dtype=torch.int32, device=device)}
+
     def _forward(self):
-        from .output_unit import answer_topk
-        m, x = self.model, self.x
+        x = self.x
         words, cntx, vecq = self.enc.forward(x["questions"], x["questionLengths"])
         kb = self.stem.forward_nchw(x["images"])
-        idx = x.get("imageIndex")
+        return self._answer(vecq, words, cntx, kb, x.get("imageIndex"))
+
+    def _answer(self, vecq, words, cntx, kb, idx):
+        """The cell over the knowledge base `kb` (gathered by `idx` when given), the output unit and the top-k: the outputs
+        of one pass."""
+        from .output_unit import answer_topk
+        m = self.model
         if self.cell is None:       # MACCell's own errors (flag set / precision outside its inference forms) pass through
-            self.cell = MACCell(vecq, words, cntx, x["questionLengths"], kb, 1.0, 1.0, 1.0, self.B, False, config=m.cfg,
+            self.cell = MACCell(vecq, words, cntx, self.x["questionLengths"], kb, 1.0, 1.0, 1.0, self.B, False, config=m.cfg,
                                 params=m.trainer.params, prec=m.prec, kbIndex=idx)
         else:
             self.cell.rebind(vecq, words, cntx, kb, kbIndex=idx)
@@ -420,6 +430,10 @@ class _ModelSlot(object):
                 outs["self"][i, :, :i + 1].copy_(a)
         return outs
 
+    def _host_outputs(self):
+        if self.outs_host is None:          # the shapes do not change with the weights
+            self.outs_host = {k: _pinned(v.numel(), v.dtype).view(v.shape) for k, v in self.outs_dev.items()}
+
     def capture(self):
         """One eager pass (weight packs and folded weights of the current parameter version are built outside the graph),
         then the capture.  The outputs of the pass that was captured are the graph's static output tensors.  The slot's
@@ -436,8 +450,7 @@ class _ModelSlot(object):
                 with torch.cuda.graph(g, stream=self.stream):
                     self.outs_dev = self._forward()
                 self.graph = g
-        if self.outs_host is None:
-            self.outs_host = {k: _pinned(v.numel(), v.dtype).view(v.shape) for k, v in self.outs_dev.items()}
+        self._host_outputs()
 
     def enqueue(self, questions, lengths, images, copied=None, index=None):
         """H2D copies -> forward -> D2H copies on this slot's stream; returns after enqueueing.  `images` is host memory of
@@ -463,6 +476,167 @@ class _ModelSlot(object):
                 self.outs_host[k].copy_(src, non_blocking=True)
             self.done.record(self.stream)
         self.busy = True
+
+
+class _CachedSlot(_ModelSlot):
+    """A `_ModelSlot` that reads its knowledge bases from the pipeline's device pool (`ModelPipeline(cache=C)`), with two
+    captured graphs: the stem graph (ingest and stem over the slot's U image rows, then `mac_kb_pool_insert` into the pool
+    rows `insertSlot` names) and the cell graph (encoder, then for a bf16 pool `mac_kb_gather_bf16` of the rows `kbSlot`
+    names, then the cell -- over the fp32 pool itself with kbIndex = kbSlot otherwise --, the output unit and the top-k)."""
+
+    def __init__(self, model, shape, use_graph, topk, images, pool):
+        B = int(shape[0])
+        self.pool = pool
+        self.lib = _lib.load()
+        self.kb16 = (torch.empty((B,) + tuple(pool.shape[1:]), dtype=torch.bfloat16, device=pool.device)
+                     if pool.dtype == torch.bfloat16 else None)
+        self.stem_graph = None
+        self.chunks = -(-B // images)       # stem passes of a batch with B misses
+        # insert slots of each stem pass, then the batch's kbSlot: written on the host before any copy out of it is enqueued
+        self.index_host = _pinned(self.chunks * images + B, torch.int32)
+        self.index_copied = torch.cuda.Event()      # after the last copy out of index_host
+        self.index_busy = False
+        self.covered = {}       # other slot -> (ticket, stem pass) of its latest work this slot's stream has waited for
+        super(_CachedSlot, self).__init__(model, shape, False, use_graph, topk, images)
+
+    def _index_inputs(self, B, images, device):
+        return {"insertSlot": torch.full((images,), -1, dtype=torch.int32, device=device),
+                "kbSlot": torch.zeros(B, dtype=torch.int32, device=device)}
+
+    def _stem_pass(self):
+        kb = self.stem.forward_nchw(self.x["images"])
+        U, N, d = kb.shape
+        check(self.lib.mac_kb_pool_insert(ptr(kb), ptr(self.x["insertSlot"]), ptr(self.pool), int(self.kb16 is not None), U,
+                                          self.pool.shape[0], N, d, stream_ptr()), "mac_kb_pool_insert")
+
+    def _forward(self):
+        x = self.x
+        words, cntx, vecq = self.enc.forward(x["questions"], x["questionLengths"])
+        if self.kb16 is None:
+            return self._answer(vecq, words, cntx, self.pool, x["kbSlot"])
+        C, N, d = self.pool.shape
+        check(self.lib.mac_kb_gather_bf16(ptr(self.pool), ptr(x["kbSlot"]), ptr(self.kb16), self.B, C, N, d, stream_ptr()),
+              "mac_kb_gather_bf16")
+        return self._answer(vecq, words, cntx, self.kb16, None)
+
+    def capture(self):
+        """As `_ModelSlot.capture`, for both graphs.  The insert slots are set to -1 first, so neither the eager nor the
+        captured stem pass writes a pool row."""
+        self.graph = self.stem_graph = None
+        self.cell = None
+        self.stream.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(self.stream):
+            self.x["insertSlot"].fill_(-1)
+            self._stem_pass()
+            self.outs_dev = self._forward()
+            self.stream.synchronize()
+            if self.use_graph:
+                gs, g = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+                with torch.cuda.graph(gs, stream=self.stream):
+                    self._stem_pass()
+                with torch.cuda.graph(g, stream=self.stream):
+                    self.outs_dev = self._forward()
+                self.stem_graph, self.graph = gs, g
+        self._host_outputs()
+
+    def enqueue_cached(self, questions, lengths, waits, passes, kb_slots, done):
+        """Wait for `waits` (events of other slots) -> H2D of the questions -> per stem pass (images [n <= U, C, H, W] host,
+        insert slots [U]): its slots and images, the stem graph, an event -> kbSlot -> the cell graph -> D2H -> `done`, a
+        fresh event of this batch that becomes the slot's `done`, on this slot's stream.  Returns the events recorded after
+        each stem pass."""
+        U = self.x["insertSlot"].shape[0]
+        h = self.index_host
+        if self.index_busy:
+            self.index_copied.synchronize()         # the copies out of index_host of this slot's previous batch are done
+        for j, (_, slots) in enumerate(passes):
+            h[j * U:(j + 1) * U].copy_(torch.from_numpy(slots))
+        h[self.chunks * U:].copy_(torch.from_numpy(kb_slots))
+        events = []
+        with torch.cuda.stream(self.stream):
+            for ev in waits:
+                self.stream.wait_event(ev)
+            self.x["questions"].copy_(questions, non_blocking=True)
+            self.x["questionLengths"].copy_(lengths, non_blocking=True)
+            for j, (images, _) in enumerate(passes):
+                self.x["insertSlot"].copy_(h[j * U:(j + 1) * U], non_blocking=True)
+                self.x["images"][:images.shape[0]].copy_(images, non_blocking=True)
+                if self.stem_graph is not None:
+                    self.stem_graph.replay()
+                else:
+                    self._stem_pass()
+                ev = torch.cuda.Event()
+                ev.record(self.stream)
+                events.append(ev)
+            self.x["kbSlot"].copy_(h[self.chunks * U:], non_blocking=True)
+            self.index_copied.record(self.stream)
+            self.index_busy = True
+            if self.graph is not None:
+                self.graph.replay()
+            else:
+                self.outs_dev = self._forward()
+            for k, src in self.outs_dev.items():
+                self.outs_host[k].copy_(src, non_blocking=True)
+            self.done = done
+            self.done.record(self.stream)
+        self.busy = True
+        return events
+
+
+_Plan = collections.namedtuple("_Plan", "hits miss rows victims")
+
+
+class _KBCache(object):
+    """Host bookkeeping of `ModelPipeline(cache=C)`'s device pool: which image key each of the C rows holds (`key`, and
+    `rows`: key -> row in least-recently-used order), per row the (ticket, stem pass, event) of the stem pass that wrote it
+    and, on each of the `slots` streams, the last batch that read it as (ticket, that batch's own done event) -- reads on
+    different streams are not ordered, so the last reader alone does not cover the others.  `plan` changes nothing;
+    `commit` applies a plan once the batch has been checked."""
+
+    def __init__(self, capacity, slots):
+        self.capacity, self.slots = int(capacity), int(slots)
+        self.stats = {"hits": 0, "misses": 0, "evictions": 0, "image_bytes": 0}
+        self.clear()
+
+    def clear(self):
+        self.rows = collections.OrderedDict()       # key -> row, least recently used first
+        self.key = [None] * self.capacity
+        self.written = [None] * self.capacity       # (ticket, stem pass, event) of the pass that wrote the row
+        self.reader = [[None] * self.slots for _ in range(self.capacity)]   # per row and slot: (ticket, done) of a reader
+        self.free = list(range(self.capacity))      # rows that hold no key, taken from the front
+
+    def plan(self, keys):
+        """`keys`: a batch's distinct image keys in first-occurrence order.  Their rows where held (hits), the missing keys
+        in that order, the row each will be written to -- free rows first, then the least recently used rows the batch does
+        not read -- and which of those are evictions."""
+        hits = [self.rows[k] for k in keys if k in self.rows]
+        miss = [k for k in keys if k not in self.rows]
+        rows = self.free[:len(miss)]
+        victims = []
+        if len(rows) < len(miss):
+            used = set(hits)
+            for r in self.rows.values():
+                if r not in used:
+                    victims.append(r)
+                    if len(rows) + len(victims) == len(miss):
+                        break
+        return _Plan(hits, miss, rows + victims, victims)
+
+    def commit(self, plan, ticket, done=None):
+        """Apply `plan` for the batch `ticket`, whose done event (recorded after its cell pass) is `done`."""
+        for r in plan.hits:
+            self.rows.move_to_end(self.key[r])
+            self.reader[r][ticket % self.slots] = (ticket, done)
+        for r in plan.victims:
+            del self.rows[self.key[r]]
+        del self.free[:len(plan.rows) - len(plan.victims)]
+        for k, r in zip(plan.miss, plan.rows):
+            self.key[r], self.written[r] = k, None
+            self.reader[r] = [None] * self.slots
+            self.reader[r][ticket % self.slots] = (ticket, done)
+            self.rows[k] = r
+        self.stats["hits"] += len(plan.hits)
+        self.stats["misses"] += len(plan.miss)
+        self.stats["evictions"] += len(plan.victims)
 
 
 class ModelPipeline(object):
@@ -498,6 +672,28 @@ class ModelPipeline(object):
     gathers each question's knowledge base from them (`MACCell(kbIndex=)`, `mac_kb_gather`).  The index is a device input
     of the graph like the questions: a new index pattern or a new k needs no new capture.
 
+    Knowledge bases kept on the device across batches: with `cache=C` (C >= B, and `images=U` the number of images one stem
+    pass takes) the pipeline keeps the knowledge bases of the last C distinct images it has seen in one device pool
+    [C, H*W, d], shared by all slots, keyed by the caller's integer image ids,
+
+        pipe = ModelPipeline(model, shape=(B, S, H, W), slots=4, images=16, cache=15000)
+        t = pipe.submit({"questions": ..., "questionLengths": ..., "imageIds": int [B], "images": load})
+
+    where `load(ids)` is given the batch's ids that are not in the cache (int64 numpy [m], first-occurrence order; called
+    only when m > 0) and returns their fp32 features [m, C, H, W], numpy or a host tensor (pinned makes the copy
+    asynchronous; a pinned result must not be written until its ticket's result is read).  Per slot there are two captured
+    graphs: the stem graph, replayed once per U missing images, runs the ingest and the stem over the slot's U image rows
+    and writes them into the pool rows its device input `insertSlot` names (`mac_kb_pool_insert`); the cell graph runs the
+    encoder and the cell over the pool rows of `kbSlot` [B].  A batch whose images are all cached copies no image byte and
+    launches no ingest or stem kernel.  The pool is bf16 where the cell's read unit reads only bf16 (the bf16 and e4m3
+    hoisted forms: the cell graph gathers it with `mac_kb_gather_bf16`) and fp32 otherwise (the cell gathers it itself,
+    `MACCell(kbIndex=)`); either way the outputs are bit for bit those of `images=U` without a cache.  When a pool row is
+    evicted (least recently used first, never a row the batch reads) the slot's stream first waits for the batches of
+    other slots that read it, and a batch that reads a row written by a batch still in flight on another slot waits for that
+    write; neither waits on the host.  A key must name one feature map for the cache's lifetime (CLEVR's image_index
+    repeats across its splits: one pipeline per image file, or `clear_cache()` between them); a weight update empties the
+    cache.  `host_cast` is off with a cache.  `cache_stats()` counts hits, misses, evictions and image bytes copied.
+
     Questions are padded with 0 to the pipeline's fixed S (a captured graph cannot trim a batch to its longest question as
     `runBatch` does); the kernels mask by length, so attention at positions >= length is exactly 0.
 
@@ -511,7 +707,7 @@ class ModelPipeline(object):
     -> 512), and its graph's private pool holds its own patch matrices (231 MB for layer 0 at 64x1024x14x14)."""
 
     def __init__(self, model, shape, slots=4, use_graph=True, topk=1, host_cast=None, cast_threads=None, stage_ring=None,
-                 images=None):
+                 images=None, cache=None):
         B, S, H, W = [int(v) for v in shape]
         p = model.trainer.params
         C = int(p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2])
@@ -525,26 +721,48 @@ class ModelPipeline(object):
             raise ValueError("topk must be in 1..min(8, %d answers), got %r" % (A, topk))
         if images is not None and not (isinstance(images, int) and 1 <= images <= B):
             raise ValueError("images must be None or an int in 1..B = %d, got %r" % (B, images))
+        if cache is not None:
+            if images is None:
+                raise ValueError("cache=C needs images=U: the number of images one stem pass takes")
+            if isinstance(cache, bool) or not isinstance(cache, int) or cache < B:
+                raise ValueError("cache must be None or an int >= B = %d (every batch's images must fit), got %r" % (B, cache))
+            if model.cfg.memDim % 8:
+                raise ValueError("cache=C needs memDim %% 8 == 0 (the pool kernels' 16-byte vectors), got %d" % model.cfg.memDim)
         self.images = images
         self.lib = _lib.load()
         self.model, self.params, self.shape, self.C, self.topk = model, p, (B, S, H, W), C, int(topk)
         self.use_graph = bool(use_graph)
         self.cast_threads = int(cast_threads) if cast_threads else max(1, min(12, usable_cpus() - 2))
         numel = (B if images is None else images) * C * H * W
-        self.host_cast = model._stem.prec == "bf16" and host_cast is not False
+        self.host_cast = model._stem.prec == "bf16" and host_cast is not False and cache is None
         self.cast_ms = None
         if self.host_cast and host_cast is None:
             self.cast_ms = _time_cast(self.lib, numel, self.cast_threads)
             self.host_cast = _cast_pays(self.cast_ms, numel)
         self._version = p.version
-        self.slots = [_ModelSlot(model, self.shape, self.host_cast, self.use_graph, self.topk, images)
-                      for _ in range(int(slots))]
+        self._cache = self.pool = None
+        if cache is None:
+            self.slots = [_ModelSlot(model, self.shape, self.host_cast, self.use_graph, self.topk, images)
+                          for _ in range(int(slots))]
+        else:
+            # the pool holds what the cell's read unit reads: bf16 for the bf16 and e4m3 hoisted forms (MACCell's
+            # _kb_gather_bf16 condition), the stem's fp32 rows for every other form
+            cfg = model.cfg
+            pool_bf16 = model.prec in ("bf16", "fp8") and cfg.is_fast_path and not cfg.unsharedCells
+            self.pool = torch.zeros(cache, H * W, cfg.memDim, dtype=torch.bfloat16 if pool_bf16 else torch.float32,
+                                    device=p.device)
+            self._cache = _KBCache(cache, slots)
+            self.slots = [_CachedSlot(model, self.shape, self.use_graph, self.topk, images, self.pool)
+                          for _ in range(int(slots))]
         self._ring = (_CastRing(self.lib, numel, max(2, int(stage_ring) if stage_ring else 3), self.cast_threads)
                       if self.host_cast else None)
         self._next = 0
         self._ahead = None                  # (next_batch["images"] as given, its host tensor) of the cast in flight
-        # with images=U: a batch of k images copies k of the U counted here
+        # with images=U: a batch of k images copies k of the U counted here; with cache=C only the questions, their lengths
+        # and kbSlot are counted (cache_stats() counts the image bytes, and each stem pass adds U * 4 bytes of insert slots)
         self.h2d_bytes = numel * (2 if self.host_cast else 4) + B * S * 4 + B * 4 + (0 if images is None else B * 4)
+        if cache is not None:
+            self.h2d_bytes = B * S * 4 + B * 4 + B * 4
         self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.slots[0].outs_host.values())
 
     def _host(self, batch):
@@ -581,6 +799,8 @@ class ModelPipeline(object):
     def submit(self, batch, next_batch=None):
         """Enqueue one batch (numpy arrays or host tensors; pinned memory makes the copies asynchronous) and return its
         ticket.  `next_batch`: the batch the next submit will take, whose host cast then runs under this batch's copies."""
+        if self._cache is not None:
+            return self._submit_cached(batch)
         q, ql, img, idx = self._host(batch)
         if self._ahead is not None and self._ahead[0] is batch["images"]:
             img = self._ahead[1]                           # the tensor whose cast the previous submit started
@@ -606,6 +826,105 @@ class ModelPipeline(object):
             return self._ring.stages[si][:img.numel()]
         slot.enqueue(q, ql, staged, copied=lambda stream: self._ring.copied(si, stream), index=idx)
         return t
+
+    def _checked_ids(self, batch):
+        """With cache=C: the batch's questions and lengths as host tensors, its image keys as Python ints and its loader,
+        checked against the pipeline's shape; ValueError before anything is enqueued."""
+        B, S = self.shape[:2]
+        if "imageIndex" in batch:
+            raise ValueError("a pipeline built with cache=C takes imageIds and a loader, not imageIndex")
+        for key in ("questions", "questionLengths", "imageIds", "images"):
+            if key not in batch:
+                raise ValueError("the batch has no %s" % key)
+        out = []
+        for key, shp in (("questions", (B, S)), ("questionLengths", (B,))):
+            v = torch.as_tensor(batch[key])
+            if v.device.type != "cpu" or tuple(v.shape) != shp:
+                raise ValueError("%s must be a host tensor of shape %s, got %s on %s" % (key, shp, tuple(v.shape), v.device))
+            out.append(v.to(torch.int32).contiguous())
+        ids = torch.as_tensor(batch["imageIds"])
+        if (ids.device.type != "cpu" or tuple(ids.shape) != (B,) or ids.dtype.is_floating_point or ids.dtype.is_complex
+                or ids.dtype == torch.bool):
+            raise ValueError("imageIds must be a host array of %d integers, got %s %s" % (B, ids.dtype, tuple(ids.shape)))
+        if not callable(batch["images"]):
+            raise ValueError("with cache=C the batch's images are a loader: a callable that takes the missing ids")
+        return out + [ids.tolist(), batch["images"]]
+
+    def _loaded(self, load, miss):
+        """The loader's features of the missing keys, checked: a host fp32 tensor [m, C, H, W]."""
+        H, W = self.shape[2:]
+        res = load(np.asarray(miss, dtype=np.int64))
+        try:
+            v = torch.as_tensor(res)
+        except (TypeError, RuntimeError) as exc:
+            raise ValueError("the images loader must return an array of fp32 features: %s" % exc)
+        want = (len(miss), self.C, H, W)
+        if v.device.type != "cpu" or v.dtype != torch.float32 or tuple(v.shape) != want:
+            raise ValueError("the images loader must return host fp32 features of shape %s (NCHW), got %s %s on %s"
+                             % (want, v.dtype, tuple(v.shape), v.device))
+        return v.contiguous()
+
+    def _submit_cached(self, batch):
+        q, ql, ids, load = self._checked_ids(batch)
+        if self.params.version != self._version:
+            self.drain()
+            self._cache.clear()
+            for s in self.slots:
+                s.capture()
+            self._version = self.params.version
+        cache, U, n = self._cache, self.images, len(self.slots)
+        keys = list(dict.fromkeys(ids))                     # distinct keys, first-occurrence order
+        plan = cache.plan(keys)
+        imgs = self._loaded(load, plan.miss) if plan.miss else None
+        # nothing has changed so far; from here on the batch is enqueued
+        t = self._next
+        si = t % n
+        slot = self.slots[si]
+        self._next = t + 1
+        waits = []
+        done = torch.cuda.Event()             # this batch's: recorded after its cell pass, the last read of the pool
+
+        def wait_for(sj, upto, ev):           # make slot si's stream wait for slot sj's work up to (ticket, pass)
+            if sj != si and slot.covered.get(sj, (-1, -1)) < upto:
+                slot.covered[sj] = upto
+                waits.append(ev)
+        for r in plan.victims:                # write after read: the row's last reader on every slot has finished
+            for sj, reader in enumerate(cache.reader[r]):
+                if reader is not None:        # that reader's own done event, not the slot's latest batch
+                    wait_for(sj, (reader[0], float("inf")), reader[1])
+        for r in plan.hits:                   # read after write: the stem pass that wrote the row has finished
+            if cache.written[r] is not None:
+                wt, wp, ev = cache.written[r]
+                wait_for(wt % n, (wt, wp), ev)
+        cache.commit(plan, t, done)
+        passes = []
+        for j in range(0, len(plan.miss), U):
+            slots_j = np.full(U, -1, dtype=np.int32)
+            rows_j = plan.rows[j:j + U]
+            slots_j[:len(rows_j)] = rows_j
+            passes.append((imgs[j:j + U], slots_j))
+        kb_slots = np.asarray([cache.rows[k] for k in ids], dtype=np.int32)
+        events = slot.enqueue_cached(q, ql, waits, passes, kb_slots, done)
+        for j, ev in enumerate(events):
+            for r in plan.rows[j * U:(j + 1) * U]:
+                cache.written[r] = (t, j, ev)
+        cache.stats["image_bytes"] += 0 if imgs is None else imgs.numel() * 4
+        return t
+
+    def cache_stats(self):
+        """With cache=C: {"hits", "misses"} (distinct images of each batch found in the cache / run through the stem),
+        "evictions", "image_bytes" (features copied to the device) since construction, and "resident" (images held now)."""
+        if self._cache is None:
+            raise ValueError("cache_stats() is for a pipeline built with cache=C")
+        return dict(self._cache.stats, resident=len(self._cache.rows))
+
+    def clear_cache(self):
+        """With cache=C: wait for the batches in flight, then forget every cached image (the statistics keep counting).
+        Use it between image files whose keys overlap."""
+        if self._cache is None:
+            raise ValueError("clear_cache() is for a pipeline built with cache=C")
+        self.drain()
+        self._cache.clear()
 
     def result(self, ticket):
         """Block until the batch of `ticket` is done; its outputs stay valid until `slots` further submits."""
