@@ -1,0 +1,1 @@
+from .modules import ImageStem, MACModel, MACNetwork, OutputUnit, QuestionEncoder, answer_loss  # noqa: F401

@@ -46,10 +46,7 @@ class _Bwd(object):
         self.tc = bool(tc)
         # a tc32 cell keeps its forward's accuracy class in backward: split-bf16 products (mac_read_bwd_tc32, any B*N)
         self.tc32 = self.tc and cell.prec == _lib.PREC["tc32"]
-        if self.tc32 and cell.d % 128:
-            raise NotImplementedError("split-bf16 tensor-core backward needs d % 128 == 0")
-        if self.tc and not self.tc32 and (cell.d % 128 or (cell.B * cell.N) % 64):
-            raise NotImplementedError("tensor-core backward needs d % 128 == 0 and (B*N) % 64 == 0")
+        check_backward(cell, tc)
         self.form = "tc32" if self.tc32 else "tc" if self.tc else "fp32"
         self.p = cell.params
         c = cell.cfg
@@ -286,12 +283,10 @@ class _Bwd(object):
         return out
 
 
-def mac_backward(cell, d_control, d_memory, bucket=None, zero_bucket=True, d_vecq=None, tc=False):
-    """Gradients of sum(d_control * control_L) + sum(d_memory * memory_L) w.r.t. every cell parameter and input.
-    `tc=True`: the read unit's projections on tensor cores in backward too (bf16 operands, fp32 accumulation)."""
-    if not getattr(cell, "save_for_backward", False):
-        raise RuntimeError("construct the MACCell with save_for_backward=True and run the forward first")
-    if getattr(cell, "_tape", None) is not None:       # flags outside the hand-scheduled sweep: node-by-node (tape.py)
+def check_backward(cell, tc):
+    """Refuses, before any launch, a backward `mac_backward(cell, ..., tc=tc)` cannot run: the shape rules of the tensor-core
+    forms.  Needs only the constructed cell, so a caller can check before its forward."""
+    if getattr(cell, "_use_tape", False):
         if tc:
             # tensor cores on the tape: the composed read unit's [B*N, .] linears (mac_linear_bwd_tc, any B*N) and the fused
             # read unit (mac_read_bwd_tc); everything else on the tape stays on its fp32 kernels
@@ -299,5 +294,20 @@ def mac_backward(cell, d_control, d_memory, bucket=None, zero_bucket=True, d_vec
                 raise NotImplementedError("the tape backward runs the fp32 kernels")
             if cell._fused_read and (cell.d % 128 or (cell.B * cell.N) % 64):
                 raise NotImplementedError("tensor-core backward needs d % 128 == 0 and (B*N) % 64 == 0")
+        return
+    tc32 = tc and cell.prec == _lib.PREC["tc32"]
+    if tc32 and cell.d % 128:
+        raise NotImplementedError("split-bf16 tensor-core backward needs d % 128 == 0")
+    if tc and not tc32 and (cell.d % 128 or (cell.B * cell.N) % 64):
+        raise NotImplementedError("tensor-core backward needs d % 128 == 0 and (B*N) % 64 == 0")
+
+
+def mac_backward(cell, d_control, d_memory, bucket=None, zero_bucket=True, d_vecq=None, tc=False):
+    """Gradients of sum(d_control * control_L) + sum(d_memory * memory_L) w.r.t. every cell parameter and input.
+    `tc=True`: the read unit's projections on tensor cores in backward too (bf16 operands, fp32 accumulation)."""
+    if not getattr(cell, "save_for_backward", False):
+        raise RuntimeError("construct the MACCell with save_for_backward=True and run the forward first")
+    if getattr(cell, "_tape", None) is not None:       # flags outside the hand-scheduled sweep: node-by-node (tape.py)
+        check_backward(cell, tc)
         return cell._tape.run(d_control, d_memory, bucket, zero_bucket, d_vecq, tc=tc)
     return _Bwd(cell, bucket, zero_bucket, tc=tc).run(d_control, d_memory, d_vecq)

@@ -32,6 +32,56 @@ def allreduce_sum_(bucket, group=None):
     return bucket
 
 
+def check_model_precisions(cfg, encoder, stem, stem_prec, enc_prec):
+    """The stem's and the encoder's training precisions against the model's shapes (DPTrainer, modules.MACModel): raises
+    before anything is allocated or launched."""
+    if stem_prec not in ("fp32", "bf16", "bf16x3"):
+        raise ValueError("stem_prec must be 'fp32', 'bf16' or 'bf16x3', got %r" % (stem_prec,))
+    if stem_prec != "fp32":
+        if stem is None:
+            raise ValueError("stem_prec=%r needs stem=" % (stem_prec,))
+        if stem[0] % 128 or cfg.memDim % 128:
+            raise NotImplementedError("stem_prec=%r needs the image channels (%d) and memDim (%d) to be multiples of "
+                                      "128 (the wgmma tiles of mac_conv3x3_bwd_tc)" % (stem_prec, stem[0], cfg.memDim))
+    if enc_prec not in ("fp32", "bf16"):
+        raise ValueError("enc_prec must be 'fp32' or 'bf16', got %r" % (enc_prec,))
+    if enc_prec != "fp32":
+        if encoder is None:
+            raise ValueError("enc_prec=%r needs encoder=" % (enc_prec,))
+        if cfg.ctrlDim != 512:
+            raise NotImplementedError("enc_prec='bf16' needs ctrlDim = 512 (h = 256 per LSTM direction), got %d"
+                                      % cfg.ctrlDim)
+
+
+def model_parameters(cfg, netLength, seed, classifier=None, encoder=None, stem=None, param_values=None):
+    """The variables of the model DPTrainer trains, initialised as the reference does from `seed`: (cell values -- the
+    caller's `param_values` when given --, output / encoder / stem specs and values in one OrderedDict each, encoder specs,
+    stem specs).  The last four are None where the model has no such part."""
+    from .params import init_params
+    extra_specs = extra_values = None
+    if classifier is not None:
+        from .output_unit import output_specs, init_output_params
+        extra_specs = output_specs(cfg.ctrlDim, cfg.memDim, list(classifier[1]), classifier[0])
+        extra_values = init_output_params(extra_specs, seed=seed + 17, bias_scale=0.0)
+    enc_specs = stem_specs_ = None
+    if encoder is not None or stem is not None:
+        import collections
+        if classifier is None or encoder is None or stem is None:
+            raise ValueError("the full model needs classifier=, encoder= and stem= together")
+        from .encoder import encoder_specs, init_encoder_params
+        from .stem import stem_specs, init_stem_params
+        enc_specs = encoder_specs(encoder[0], encoder[1], cfg.ctrlDim, ctrl_dim=cfg.ctrlDim, bi=True)
+        stem_specs_ = stem_specs(stem[0], cfg.memDim, num_layers=stem[1])
+        extra_specs = collections.OrderedDict(list(extra_specs.items()) + list(enc_specs.items())
+                                              + list(stem_specs_.items()))
+        extra_values = dict(extra_values)
+        extra_values.update(init_encoder_params(enc_specs, seed=seed + 19, bias_scale=0.0))   # TF: zero biases
+        extra_values.update(init_stem_params(stem_specs_, seed=seed + 23, bias_scale=0.0))
+    if extra_specs is not None and param_values is None:
+        param_values = init_params(cfg, netLength, seed=seed)
+    return param_values, extra_specs, extra_values, enc_specs, stem_specs_
+
+
 class DPTrainer(object):
     def __init__(self, cfg, netLength, param_values=None, seed=0, rank=0, world=1, lr=1e-4, clip=8.0, ema_decay=0.999,
                  beta1=0.9, beta2=0.999, eps=1e-8, dropouts=None, device="cuda", classifier=None, output_dropout=0.85,
@@ -59,47 +109,12 @@ class DPTrainer(object):
         and `bwd_tc`).  The others are mixed precision: bf16 operands, fp32 accumulation, fp32 master weights / gradients /
         optimizer state (DESIGN.md section 9)."""
         from .mac_cell import MACParams, views_of
-        from .params import init_params
-        if stem_prec not in ("fp32", "bf16", "bf16x3"):
-            raise ValueError("stem_prec must be 'fp32', 'bf16' or 'bf16x3', got %r" % (stem_prec,))
-        if stem_prec != "fp32":
-            if stem is None:
-                raise ValueError("stem_prec=%r needs stem=" % (stem_prec,))
-            if stem[0] % 128 or cfg.memDim % 128:
-                raise NotImplementedError("stem_prec=%r needs the image channels (%d) and memDim (%d) to be multiples of "
-                                          "128 (the wgmma tiles of mac_conv3x3_bwd_tc)" % (stem_prec, stem[0], cfg.memDim))
-        if enc_prec not in ("fp32", "bf16"):
-            raise ValueError("enc_prec must be 'fp32' or 'bf16', got %r" % (enc_prec,))
-        if enc_prec != "fp32":
-            if encoder is None:
-                raise ValueError("enc_prec=%r needs encoder=" % (enc_prec,))
-            if cfg.ctrlDim != 512:
-                raise NotImplementedError("enc_prec='bf16' needs ctrlDim = 512 (h = 256 per LSTM direction), got %d"
-                                          % cfg.ctrlDim)
+        check_model_precisions(cfg, encoder, stem, stem_prec, enc_prec)
         self.cfg, self.L, self.rank, self.world = cfg, netLength, rank, world
         self.prec, self.bwd_tc, self.stem_prec, self.enc_prec = prec, bool(bwd_tc), stem_prec, enc_prec
         self.lib = _lib.load()
-        extra_specs = extra_values = None
-        if classifier is not None:
-            from .output_unit import output_specs, init_output_params
-            extra_specs = output_specs(cfg.ctrlDim, cfg.memDim, list(classifier[1]), classifier[0])
-            extra_values = init_output_params(extra_specs, seed=seed + 17, bias_scale=0.0)
-        self._enc_specs = self._stem_specs = None
-        if encoder is not None or stem is not None:
-            import collections
-            if classifier is None or encoder is None or stem is None:
-                raise ValueError("the full model needs classifier=, encoder= and stem= together")
-            from .encoder import encoder_specs, init_encoder_params
-            from .stem import stem_specs, init_stem_params
-            self._enc_specs = encoder_specs(encoder[0], encoder[1], cfg.ctrlDim, ctrl_dim=cfg.ctrlDim, bi=True)
-            self._stem_specs = stem_specs(stem[0], cfg.memDim, num_layers=stem[1])
-            extra_specs = collections.OrderedDict(list(extra_specs.items()) + list(self._enc_specs.items())
-                                                  + list(self._stem_specs.items()))
-            extra_values = dict(extra_values)
-            extra_values.update(init_encoder_params(self._enc_specs, seed=seed + 19, bias_scale=0.0))   # TF: zero biases
-            extra_values.update(init_stem_params(self._stem_specs, seed=seed + 23, bias_scale=0.0))
-        if extra_specs is not None and param_values is None:
-            param_values = init_params(cfg, netLength, seed=seed)
+        param_values, extra_specs, extra_values, self._enc_specs, self._stem_specs = model_parameters(
+            cfg, netLength, seed, classifier, encoder, stem, param_values)
         self.params = MACParams(cfg, netLength, values=param_values, seed=seed, device=device, extra_specs=extra_specs,
                                 extra_values=extra_values)   # replicated
         self.out = None

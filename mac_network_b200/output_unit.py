@@ -100,6 +100,18 @@ class OutputUnit(object):
         """Returns (logits, losses [B], dlogits [B, A]) -- dlogits = (softmax - onehot) * loss_scale (default 1/B).  The three
         stay reachable as `last_logits`, `losses` and `dlogits` (`logits` is the label-free method)."""
         B = memory.shape[0]
+        self.forward_logits(memory, vecQuestions, step)
+        A = self.last_logits.shape[1]
+        self.losses = self._new(B)
+        self.dlogits = self._new(B, A)
+        scale = (1.0 / B) if loss_scale is None else float(loss_scale)
+        check(self.lib.mac_softmax_xent(ptr(self.last_logits), ptr(answers), ptr(self.losses), ptr(self.dlogits), scale, B, A,
+                                        stream_ptr()), "mac_softmax_xent")
+        return self.last_logits, self.losses, self.dlogits
+
+    def forward_logits(self, memory, vecQuestions, step=0):
+        """The training forward up to the logits (this unit's dropouts, its inputs kept for `backward`), without the loss:
+        `backward(dlogits=)` then takes the gradient of the logits from the caller.  Returns the logits [B, A]."""
         act = act_code("RELU", self.relu)
         self.eq = self._linear([vecQuestions], self.p["outputUnit/linearLayeroutQuestion/weights/weight"],
                                self.p["outputUnit/linearLayeroutQuestion/biases/bias"])
@@ -122,13 +134,7 @@ class OutputUnit(object):
             if i < self.nfc - 1:
                 setattr(self, "_h%d" % i, x)
         self.last_logits = x
-        A = x.shape[1]
-        self.losses = self._new(B)
-        self.dlogits = self._new(B, A)
-        scale = (1.0 / B) if loss_scale is None else float(loss_scale)
-        check(self.lib.mac_softmax_xent(ptr(self.last_logits), ptr(answers), ptr(self.losses), ptr(self.dlogits), scale, B, A,
-                                        stream_ptr()), "mac_softmax_xent")
-        return self.last_logits, self.losses, self.dlogits
+        return x
 
     def logits(self, memory, vecQuestions):
         """The answer logits [B, A] without labels: the linears of `forward` with every dropout at 1, no loss, no `dlogits`,
@@ -142,10 +148,11 @@ class OutputUnit(object):
                                self.p["classifier/linearLayerfc_%d/biases/bias" % i], act if i < self.nfc - 1 else 0)]
         return xs[0]
 
-    def backward(self, grads, d_memory, d_vecq):
-        """Accumulates parameter gradients into `grads` (dict name -> tensor) and ADDS dL/dmemory, dL/dvecQuestions."""
+    def backward(self, grads, d_memory, d_vecq, dlogits=None):
+        """Accumulates parameter gradients into `grads` (dict name -> tensor) and ADDS dL/dmemory, dL/dvecQuestions.
+        `dlogits`: the gradient of the logits [B, A]; by default the loss's, `self.dlogits`, from `forward`."""
         B = self.memory.shape[0]
-        dy = self.dlogits
+        dy = self.dlogits if dlogits is None else dlogits
         act = act_code("RELU", self.relu)
 
         def lin_bwd(xs, wname, bname, dy, dxs, accum):
