@@ -470,6 +470,16 @@ int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mode, int B, 
 enum { MAC_INGEST_COLS_BF16 = 0, MAC_INGEST_COLS_SPLIT = 1 };
 int mac_ingest_nchw_train(const float* x_nchw, float* x_nhwc, void* cols, int cols_form, float keep, uint64_t seed, int site,
                           int step, int B, int C, int H, int W, mac_stream_t stream);
+/* The two ingests from fp16 features (csrc/ingest.cuh; Stem.forward_nchw with torch.float16 images, the pipelines'
+ * image_dtype=torch.float16): x_f16 [B, C, H, W] fp16, read once and widened to fp32 exactly, then the outputs of the fp32
+ * entry point fed those fp32 values, bit for bit -- the widened NHWC tensor (MAC_INGEST_NHWC_F32), the patch matrix rounded
+ * to nearest even from the fp32 value (MAC_INGEST_PATCH_BF16), and the training form's two outputs with the same Philox
+ * mask; zero padding, infinities and NaNs included.  The same refusals and status codes as the fp32 entry points, all
+ * before any launch; the fp16 slab is half the fp32 one, so the shared-memory limits are H*W <= 580 (-> NHWC), 854
+ * (-> patches), 427 (MAC_INGEST_COLS_BF16) and 337 (MAC_INGEST_COLS_SPLIT). */
+int mac_ingest_nchw_f16(const void* x_f16, void* out, int mode, int B, int C, int H, int W, mac_stream_t stream);
+int mac_ingest_nchw_train_f16(const void* x_f16, float* x_nhwc, void* cols, int cols_form, float keep, uint64_t seed, int site,
+                              int step, int B, int C, int H, int W, mac_stream_t stream);
 /* Knowledge bases of B questions about U distinct images (csrc/ingest.cuh; MACCell(kbIndex=), serving.ModelPipeline(images=)):
  *   out[b, n, :] = kb_u[index[b], n, :]   for b < B
  * kb_u: the stem's fp32 output for the U images, [U, N, d]; index: int32 [B] in device memory; out: fp32 [B, N, d], or with

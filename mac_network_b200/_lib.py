@@ -105,6 +105,9 @@ PROTOTYPES = {
     "mac_answer_topk": (c_int, [c_fp, c_int, c_int, c_int, c_fp, c_fp, c_fp]),
     "mac_ingest_nchw": (c_int, [c_fp, c_int, c_fp, c_int, c_int, c_int, c_int, c_int, c_fp]),
     "mac_ingest_nchw_train": (c_int, [c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_ingest_nchw_f16": (c_int, [c_fp, c_fp, c_int, c_int, c_int, c_int, c_int, c_fp]),
+    "mac_ingest_nchw_train_f16": (c_int, [c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_int, c_int, c_int, c_int,
+                                          c_fp]),
     "mac_kb_gather": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_int, c_int, c_int, c_fp]),
     "mac_kb_gather_bwd": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_int, c_int, c_fp]),
     "mac_kb_pool_insert": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_int, c_int, c_int, c_fp]),

@@ -1,7 +1,9 @@
-// Layer-0 ingest of the image stem from channel-major features: [B, C, H, W] (fp32 or bf16, as the feature extractor wrote
-// them) -> either the fp32 NHWC tensor Stem.forward takes, or directly the bf16 patch matrix of mac_im2col3x3
-// ([B*H*W, 9*C], tap-major, channel fastest, zero rows outside the image, no dropout), so that the bf16 stem never makes the
-// NHWC copy.  The input is read from HBM once and the output written once.
+// Layer-0 ingest of the image stem from channel-major features: [B, C, H, W] (fp32, bf16 or fp16, as the feature extractor or
+// the feature file stored them) -> either the fp32 NHWC tensor Stem.forward takes, or directly the bf16 patch matrix of
+// mac_im2col3x3 ([B*H*W, 9*C], tap-major, channel fastest, zero rows outside the image, no dropout), so that the bf16 stem never
+// makes the NHWC copy.  The input is read from HBM once and the output written once.  The kernels are templates on the input
+// element type IT; its one widening function ingest_f32 (exact for all three types) is the only place the type matters, so
+// every input shares the slab copy, the transpose, the patch writes and the training mask.
 //
 // One CTA owns (sample, 64-channel slab).  The slab is one contiguous run of 64*H*W elements in NCHW, brought into shared
 // memory by ONE 1-D bulk copy (cp.async.bulk + mbarrier; 16-byte aligned for any H*W because 64 elements are >= 128 bytes).
@@ -13,6 +15,7 @@
 // (eight or sixteen consecutive lanes = one pixel's 128 or 256 contiguous bytes) and stores 128 contiguous bytes per pixel and
 // tap (patch mode) or 256 per pixel (NHWC mode).
 #pragma once
+#include <cuda_fp16.h>
 #include "common.cuh"
 #include "tc_gemm.cuh"      // pack_bf16, pack_bf16_lo: the split-bf16 rounding of mac_im2col3x3_split
 
@@ -32,15 +35,21 @@ struct IngestShape {
   __host__ __device__ static size_t smem_bytes(int HW) { return in_bytes(HW) + (size_t)HW * TROW; }
 };
 
-__device__ __forceinline__ uint32_t ingest_pair(float a, float b) {          // the rounding of mac_im2col3x3(cols_bf16 = 1)
-  __nv_bfloat162 p = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&p);
-}
-__device__ __forceinline__ uint32_t ingest_pair(__nv_bfloat16 a, __nv_bfloat16 b) {  // bf16 in, bf16 out: a move
-  return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
-}
+// the widening of each input type to fp32: exact; for fp16 the conversion torch's Tensor.float() makes on the device, so a
+// NaN keeps the payload it gets there
 __device__ __forceinline__ float ingest_f32(float a) { return a; }
 __device__ __forceinline__ float ingest_f32(__nv_bfloat16 a) { return __bfloat162float(a); }
+__device__ __forceinline__ float ingest_f32(__half a) { return __half2float(a); }
+// two channels of the bf16 patch matrix: the rounding of mac_im2col3x3(cols_bf16 = 1) of the widened values; bf16 in is a move
+template <typename IT>
+__device__ __forceinline__ uint32_t ingest_pair(IT a, IT b) {
+  __nv_bfloat162 p = __floats2bfloat162_rn(ingest_f32(a), ingest_f32(b));
+  return *reinterpret_cast<uint32_t*>(&p);
+}
+template <>
+__device__ __forceinline__ uint32_t ingest_pair<__nv_bfloat16>(__nv_bfloat16 a, __nv_bfloat16 b) {
+  return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
+}
 
 template <typename IT, bool PATCH>
 __global__ void __launch_bounds__(ING_THREADS) ingest_nchw_kernel(const IT* __restrict__ x, void* __restrict__ out, int C,
@@ -116,9 +125,9 @@ static int ingest_nchw_launch(const void* x, void* out, int B, int C, int H, int
 }
 
 // shared memory one CTA needs; the entry point refuses shapes beyond one SM's 227 KB or the mbarrier's tx-count range
-static inline size_t ingest_smem_bytes(int x_bf16, int mode, int HW) {
-  if (x_bf16) return mode ? IngestShape<__nv_bfloat16, true>::smem_bytes(HW) : IngestShape<__nv_bfloat16, false>::smem_bytes(HW);
-  return mode ? IngestShape<float, true>::smem_bytes(HW) : IngestShape<float, false>::smem_bytes(HW);
+template <typename IT>
+static inline size_t ingest_smem_bytes(int mode, int HW) {
+  return mode ? IngestShape<IT, true>::smem_bytes(HW) : IngestShape<IT, false>::smem_bytes(HW);
 }
 
 // ------------------------------------------------------------------------------------------------ training ingest
@@ -127,21 +136,23 @@ static inline size_t ingest_smem_bytes(int x_bf16, int mode, int HW) {
 // mask from it) and layer 0's DROPPED-OUT patch matrix, bit for bit what mac_im2col3x3(cols_bf16 = 1) or
 // mac_im2col3x3_split writes.  The mask is drawn once per source element while transposing, not once per tap: one
 // philox4x32_10(seed, e >> 2, site, step) per (pixel, channel quad), e the NHWC flat index -- mac_im2col3x3's counter.
-// Shared memory, per pixel: the slab (256 B), the fp32 pixel-major tile (64 * 4 + 16 B) and the bf16 tile (64 * 2 + 16 B),
-// and for the split form a second bf16 tile for the lo halves: 672 / 816 B, 131.7 / 159.9 KB at 14x14, one CTA per SM, so
-// 512 threads keep more loads and stores in flight than ING_THREADS would.
+// Shared memory, per pixel: the slab (256 B fp32, 128 B fp16), the fp32 pixel-major tile (64 * 4 + 16 B) and the bf16 tile
+// (64 * 2 + 16 B), and for the split form a second bf16 tile for the lo halves: 672 / 816 B for fp32 input (131.7 / 159.9 KB
+// at 14x14), 544 / 688 B for fp16 (104.1 / 131.7 KB), one CTA per SM, so 512 threads keep more loads and stores in flight
+// than ING_THREADS would.
 constexpr int INGT_THREADS = 512;
 constexpr int INGT_FROW = ING_CS * 4 + 16;     // fp32 tile row, bytes
 constexpr int INGT_HROW = ING_CS * 2 + 16;     // bf16 tile row, bytes
 
-template <bool SPLIT>
+template <typename IT, bool SPLIT>
 struct IngestTrainShape {
-  static constexpr int PIX = ING_CS * 4 + INGT_FROW + INGT_HROW * (SPLIT ? 2 : 1);     // shared bytes per pixel
+  static constexpr int PIX = ING_CS * (int)sizeof(IT) + INGT_FROW + INGT_HROW * (SPLIT ? 2 : 1);     // shared bytes per pixel
+  __host__ __device__ static size_t in_bytes(int HW) { return (size_t)ING_CS * HW * sizeof(IT); }
   __host__ __device__ static size_t smem_bytes(int HW) { return (size_t)HW * PIX; }
 };
 
-template <bool SPLIT>
-__global__ void __launch_bounds__(INGT_THREADS, 1) ingest_nchw_train_kernel(const float* __restrict__ x,
+template <typename IT, bool SPLIT>
+__global__ void __launch_bounds__(INGT_THREADS, 1) ingest_nchw_train_kernel(const IT* __restrict__ x,
                                                                             float* __restrict__ x_nhwc,
                                                                             __nv_bfloat16* __restrict__ cols, uint32_t thresh,
                                                                             float scale, uint64_t seed, int site, int step,
@@ -149,8 +160,9 @@ __global__ void __launch_bounds__(INGT_THREADS, 1) ingest_nchw_train_kernel(cons
   extern __shared__ __align__(128) unsigned char ing_smem[];
   __shared__ uint64_t bar;
   const int HW = H * W, tid = threadIdx.x, b = blockIdx.y, c0 = blockIdx.x * ING_CS;
-  const float* s_in = reinterpret_cast<const float*>(ing_smem);              // [64][HW] as it lies in NCHW
-  unsigned char* s_f = ing_smem + (size_t)HW * ING_CS * 4;                   // [HW][FROW], undropped fp32
+  using SH = IngestTrainShape<IT, SPLIT>;
+  const IT* s_in = reinterpret_cast<const IT*>(ing_smem);                    // [64][HW] as it lies in NCHW
+  unsigned char* s_f = ing_smem + SH::in_bytes(HW);                          // [HW][FROW], undropped fp32
   unsigned char* s_h = s_f + (size_t)HW * INGT_FROW;                         // [HW][HROW], bf16(dropped) or its hi half
   unsigned char* s_l = s_h + (size_t)HW * INGT_HROW;                         // [HW][HROW], the lo half (SPLIT)
   if (tid == 0) {
@@ -159,7 +171,7 @@ __global__ void __launch_bounds__(INGT_THREADS, 1) ingest_nchw_train_kernel(cons
   }
   __syncthreads();
   if (tid == 0) {
-    const uint32_t bytes = (uint32_t)((size_t)HW * ING_CS * 4);
+    const uint32_t bytes = (uint32_t)SH::in_bytes(HW);
     mbar_expect_tx(&bar, bytes);
     bulk_g2s(ing_smem, x + ((size_t)b * C + c0) * HW, bytes, &bar);
   }
@@ -167,10 +179,10 @@ __global__ void __launch_bounds__(INGT_THREADS, 1) ingest_nchw_train_kernel(cons
   // transpose + mask: eight consecutive channels (two Philox quads) of one pixel per item; lanes along the pixels
   for (int i = tid; i < 8 * HW; i += INGT_THREADS) {
     const int g = i / HW, p = i - g * HW;
-    const float* src = s_in + (size_t)(g * 8) * HW + p;
+    const IT* src = s_in + (size_t)(g * 8) * HW + p;
     float v[8], d[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = d[j] = src[j * HW];
+    for (int j = 0; j < 8; ++j) v[j] = d[j] = ingest_f32(src[j * HW]);
     if (thresh) {
       const uint64_t q = (((uint64_t)b * HW + p) * C + c0 + g * 8) >> 2;
 #pragma unroll
@@ -223,13 +235,13 @@ __global__ void __launch_bounds__(INGT_THREADS, 1) ingest_nchw_train_kernel(cons
   }
 }
 
-template <bool SPLIT>
-static int ingest_nchw_train_launch(const float* x, float* x_nhwc, void* cols, uint32_t thresh, float scale, uint64_t seed,
+template <typename IT, bool SPLIT>
+static int ingest_nchw_train_launch(const void* x, float* x_nhwc, void* cols, uint32_t thresh, float scale, uint64_t seed,
                                     int site, int step, int B, int C, int H, int W, cudaStream_t stream) {
-  const size_t smem = IngestTrainShape<SPLIT>::smem_bytes(H * W);
-  auto kern = ingest_nchw_train_kernel<SPLIT>;
+  const size_t smem = IngestTrainShape<IT, SPLIT>::smem_bytes(H * W);
+  auto kern = ingest_nchw_train_kernel<IT, SPLIT>;
   MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<dim3(C / ING_CS, B), INGT_THREADS, smem, stream>>>(x, x_nhwc, reinterpret_cast<__nv_bfloat16*>(cols), thresh, scale,
+  kern<<<dim3(C / ING_CS, B), INGT_THREADS, smem, stream>>>(reinterpret_cast<const IT*>(x), x_nhwc, reinterpret_cast<__nv_bfloat16*>(cols), thresh, scale,
                                                             seed, site, step, C, H, W);
   MAC_LAUNCH_CHECK();
   return MAC_OK;

@@ -644,41 +644,62 @@ extern "C" int mac_im2col3x3(const float* x, void* cols, int cols_bf16, float ke
 }
 
 // ------------------------------------------------------------------------------------------------ stem: ingest from NCHW
-extern "C" int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mode, int B, int C, int H, int W,
-                               mac_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// The checks and the launch of one input type: every refusal precedes any CUDA call.
+template <typename IT>
+static int ingest_nchw_checked(const void* x_nchw, void* out, int mode, int B, int C, int H, int W, cudaStream_t stream) {
   if (!x_nchw || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0) return MAC_ERR_INVALID;
   if (!mac_aligned16(x_nchw) || !mac_aligned16(out)) return MAC_ERR_ALIGN;
   if ((C % ING_CS) || (mode != MAC_INGEST_NHWC_F32 && mode != MAC_INGEST_PATCH_BF16)) return MAC_ERR_UNSUPPORTED;
   // one slab, its transposed tile and the kernel's static shared memory in one SM's 227 KB, the slab inside the mbarrier's
   // tx-count range; gridDim.y
-  if ((long long)H * W > 4096 || ingest_smem_bytes(x_bf16, mode, H * W) + ING_STATIC_SMEM > 227 * 1024 || B > 65535)
+  if ((long long)H * W > 4096 || ingest_smem_bytes<IT>(mode, H * W) + ING_STATIC_SMEM > 227 * 1024 || B > 65535)
     return MAC_ERR_UNSUPPORTED;
-  if (x_bf16)
-    return mode == MAC_INGEST_PATCH_BF16 ? ingest_nchw_launch<__nv_bfloat16, true>(x_nchw, out, B, C, H, W, stream)
-                                         : ingest_nchw_launch<__nv_bfloat16, false>(x_nchw, out, B, C, H, W, stream);
-  return mode == MAC_INGEST_PATCH_BF16 ? ingest_nchw_launch<float, true>(x_nchw, out, B, C, H, W, stream)
-                                       : ingest_nchw_launch<float, false>(x_nchw, out, B, C, H, W, stream);
+  return mode == MAC_INGEST_PATCH_BF16 ? ingest_nchw_launch<IT, true>(x_nchw, out, B, C, H, W, stream)
+                                       : ingest_nchw_launch<IT, false>(x_nchw, out, B, C, H, W, stream);
 }
 
-extern "C" int mac_ingest_nchw_train(const float* x_nchw, float* x_nhwc, void* cols, int cols_form, float keep, uint64_t seed,
-                                     int site, int step, int B, int C, int H, int W, mac_stream_t stream_) {
+extern "C" int mac_ingest_nchw(const void* x_nchw, int x_bf16, void* out, int mode, int B, int C, int H, int W,
+                               mac_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  return x_bf16 ? ingest_nchw_checked<__nv_bfloat16>(x_nchw, out, mode, B, C, H, W, stream)
+                : ingest_nchw_checked<float>(x_nchw, out, mode, B, C, H, W, stream);
+}
+
+extern "C" int mac_ingest_nchw_f16(const void* x_f16, void* out, int mode, int B, int C, int H, int W, mac_stream_t stream_) {
+  return ingest_nchw_checked<__half>(x_f16, out, mode, B, C, H, W, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+template <typename IT>
+static int ingest_nchw_train_checked(const void* x_nchw, float* x_nhwc, void* cols, int cols_form, float keep, uint64_t seed,
+                                     int site, int step, int B, int C, int H, int W, cudaStream_t stream) {
   if (!x_nchw || !x_nhwc || !cols || B <= 0 || C <= 0 || H <= 0 || W <= 0 || !(keep > 0.f && keep <= 1.f))
     return MAC_ERR_INVALID;
   if (!mac_aligned16(x_nchw) || !mac_aligned16(x_nhwc) || !mac_aligned16(cols)) return MAC_ERR_ALIGN;
   if ((C % ING_CS) || (cols_form != MAC_INGEST_COLS_BF16 && cols_form != MAC_INGEST_COLS_SPLIT) || B > 65535)
     return MAC_ERR_UNSUPPORTED;
-  // the slab and its tiles with the kernel's static shared memory in one SM's 227 KB (H*W <= 345 / 284)
+  // the slab and its tiles with the kernel's static shared memory in one SM's 227 KB (H*W <= 345 / 284 for fp32 input,
+  // 427 / 337 for fp16)
   const bool split = cols_form == MAC_INGEST_COLS_SPLIT;
   if ((long long)H * W > 4096 ||
-      (split ? IngestTrainShape<true>::smem_bytes(H * W) : IngestTrainShape<false>::smem_bytes(H * W)) + ING_STATIC_SMEM >
-          227 * 1024)
+      (split ? IngestTrainShape<IT, true>::smem_bytes(H * W) : IngestTrainShape<IT, false>::smem_bytes(H * W)) +
+              ING_STATIC_SMEM > 227 * 1024)
     return MAC_ERR_UNSUPPORTED;
   const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
   const float scale = keep < 1.f ? 1.f / keep : 1.f;
-  return split ? ingest_nchw_train_launch<true>(x_nchw, x_nhwc, cols, thr, scale, seed, site, step, B, C, H, W, stream)
-               : ingest_nchw_train_launch<false>(x_nchw, x_nhwc, cols, thr, scale, seed, site, step, B, C, H, W, stream);
+  return split ? ingest_nchw_train_launch<IT, true>(x_nchw, x_nhwc, cols, thr, scale, seed, site, step, B, C, H, W, stream)
+               : ingest_nchw_train_launch<IT, false>(x_nchw, x_nhwc, cols, thr, scale, seed, site, step, B, C, H, W, stream);
+}
+
+extern "C" int mac_ingest_nchw_train(const float* x_nchw, float* x_nhwc, void* cols, int cols_form, float keep, uint64_t seed,
+                                     int site, int step, int B, int C, int H, int W, mac_stream_t stream_) {
+  return ingest_nchw_train_checked<float>(x_nchw, x_nhwc, cols, cols_form, keep, seed, site, step, B, C, H, W,
+                                          reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int mac_ingest_nchw_train_f16(const void* x_f16, float* x_nhwc, void* cols, int cols_form, float keep,
+                                         uint64_t seed, int site, int step, int B, int C, int H, int W, mac_stream_t stream_) {
+  return ingest_nchw_train_checked<__half>(x_f16, x_nhwc, cols, cols_form, keep, seed, site, step, B, C, H, W,
+                                           reinterpret_cast<cudaStream_t>(stream_));
 }
 
 // ------------------------------------------------------------------------------------------------ knowledge-base gather

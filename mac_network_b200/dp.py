@@ -238,9 +238,9 @@ class DPTrainer(object):
         classifier -> mean softmax-CE over the GLOBAL batch, then the hand-written backward of each in reverse order.
         `data`: questions int32 [B,S] (0 = padding), questionLengths int32 [B], answers int32 [B], and the images as exactly
         one of `images` fp32 [B,H,W,C] (NHWC: the reference transposes its NCHW feed first, model.py:68) or `images_nchw`
-        fp32 [B,C,H,W], contiguous, as the features are stored (`Stem.forward_nchw`: the ingest kernel replaces the permute
-        and, for the bf16 and bf16x3 stems, layer 0's patch pass; the same results bit for bit).  Returns (logits,
-        per-sample losses).
+        fp32 or fp16 [B,C,H,W], contiguous, as the features are stored (`Stem.forward_nchw`: the ingest kernel replaces the
+        permute and, for the bf16 and bf16x3 stems, layer 0's patch pass; the same results bit for bit; fp16 features are
+        widened on the device and give the step of `images_nchw.float()` bit for bit).  Returns (logits, per-sample losses).
 
         Several questions per image: with `imageIndex`, a contiguous int32 [B] tensor on the trainer's device, the images
         carry k <= B distinct rows and question b asks about image imageIndex[b], which must lie in [0, k) (the caller's
@@ -259,9 +259,9 @@ class DPTrainer(object):
             raise ValueError("data needs exactly one of images (NHWC) and images_nchw, got %s"
                              % sorted(k for k in data if k.startswith("images")))
         nchw = data.get("images_nchw")
-        if nchw is not None and (nchw.device != self.params.flat.device or nchw.dtype != torch.float32 or nchw.dim() != 4
-                                 or not nchw.is_contiguous()):
-            raise ValueError("images_nchw must be a contiguous fp32 [B, C, H, W] tensor on %s" % self.params.flat.device)
+        if nchw is not None and (nchw.device != self.params.flat.device or nchw.dtype not in (torch.float32, torch.float16)
+                                 or nchw.dim() != 4 or not nchw.is_contiguous()):
+            raise ValueError("images_nchw must be a contiguous fp32 or fp16 [B, C, H, W] tensor on %s" % self.params.flat.device)
         idx = data.get("imageIndex")
         if idx is not None:
             self._check_image_index(idx, data["questions"].shape[0], (data["images"] if nchw is None else nchw).shape[0])

@@ -428,9 +428,9 @@ def _encoder_fn(mod, grads, seed_step, questions, lengths):
 
 
 class ImageStem(_KernelModule):
-    """The image stem (model.py:165-204): `forward(images=NHWC fp32)` or `forward(images_nchw=NCHW fp32)` -> the knowledge
-    base [B, H*W, out_dim].  The gradient w.r.t. the images is computed exactly when they require grad.  `prec`: "fp32",
-    "bf16" or "bf16x3" (training and inference) or "fp8" (inference)."""
+    """The image stem (model.py:165-204): `forward(images=NHWC fp32)` or `forward(images_nchw=NCHW fp32 or fp16)` -> the
+    knowledge base [B, H*W, out_dim].  The gradient w.r.t. the images is computed exactly when they require grad, and
+    comes back in their dtype.  `prec`: "fp32", "bf16" or "bf16x3" (training and inference) or "fp8" (inference)."""
 
     def __init__(self, in_dim, out_dim, num_layers=2, relu="ELU", prec="fp32", values=None, seed=0, device="cuda"):
         super(ImageStem, self).__init__()
@@ -556,8 +556,11 @@ class MACModel(_KernelModule):
 
     def forward(self, questions, questionLengths, images=None, images_nchw=None, imageIndex=None):
         """questions int32 [B, S] (0 = padding), questionLengths [B], and the images as exactly one of `images` fp32 NHWC
-        [k, H, W, C] or `images_nchw` fp32 NCHW [k, C, H, W]; k = B, or with `imageIndex` (int32 [B]) k distinct images of
-        which question b asks about imageIndex[b] (the stem runs once per image).  Returns (logits [B, A], memory [B, d])."""
+        [k, H, W, C] or `images_nchw` fp32 or fp16 NCHW [k, C, H, W]; k = B, or with `imageIndex` (int32 [B]) k distinct
+        images of which question b asks about imageIndex[b] (the stem runs once per image).  fp16 features are widened on the
+        device (`Stem.forward_nchw`): everything equals the forward and backward of `images_nchw.float()` bit for bit, except
+        that when the images require grad their gradient comes back in their dtype, fp16, as autograd returns the gradient of
+        any input.  Returns (logits [B, A], memory [B, d])."""
         self._refresh()
         x, nchw = _pick_images(images, images_nchw)
         lengths = _int32(questionLengths)

@@ -363,12 +363,24 @@ class HostPipeline(object):
                 stream.wait_event(s.done)
 
 
+def _check_image_dtype(image_dtype):
+    """The pipelines' `image_dtype`: the stored format of the features, fp32 (the default) or fp16."""
+    if image_dtype not in (torch.float32, torch.float16):
+        raise ValueError("image_dtype must be torch.float32 or torch.float16, got %r" % (image_dtype,))
+
+
+def _check_f16(v, what):
+    """An fp16 pipeline takes fp16 features only: rounding fp32 ones here would change the model's input silently."""
+    if v.dtype != torch.float16:
+        raise ValueError("%s must be fp16 with image_dtype=torch.float16, got %s" % (what, v.dtype))
+
+
 class _ModelSlot(object):
     """One batch in flight through the whole model: its own stream, persistent device inputs, its own evaluation-mode
     encoder / stem / cell / output unit over the model's parameter tensors, the forward captured as one CUDA graph, pinned
     host outputs."""
 
-    def __init__(self, model, shape, images_bf16, use_graph, topk, images=None):
+    def __init__(self, model, shape, image_dtype, use_graph, topk, images=None):
         B, S, H, W = shape
         t, cfg = model.trainer, model.cfg
         p = t.params
@@ -377,8 +389,7 @@ class _ModelSlot(object):
         self.stream = torch.cuda.Stream()
         self.x = {"questions": torch.zeros(B, S, dtype=torch.int32, device=p.device),
                   "questionLengths": torch.full((B,), S, dtype=torch.int32, device=p.device),
-                  "images": torch.zeros(B if images is None else images, C, H, W, device=p.device,
-                                        dtype=torch.bfloat16 if images_bf16 else torch.float32)}
+                  "images": torch.zeros(B if images is None else images, C, H, W, device=p.device, dtype=image_dtype)}
         self.x.update(self._index_inputs(B, images, p.device))
         from .encoder import QuestionEncoder
         from .output_unit import OutputUnit
@@ -484,7 +495,7 @@ class _CachedSlot(_ModelSlot):
     rows `insertSlot` names) and the cell graph (encoder, then for a bf16 pool `mac_kb_gather_bf16` of the rows `kbSlot`
     names, then the cell -- over the fp32 pool itself with kbIndex = kbSlot otherwise --, the output unit and the top-k)."""
 
-    def __init__(self, model, shape, use_graph, topk, images, pool):
+    def __init__(self, model, shape, use_graph, topk, images, pool, image_dtype=torch.float32):
         B = int(shape[0])
         self.pool = pool
         self.lib = _lib.load()
@@ -497,7 +508,7 @@ class _CachedSlot(_ModelSlot):
         self.index_copied = torch.cuda.Event()      # after the last copy out of index_host
         self.index_busy = False
         self.covered = {}       # other slot -> (ticket, stem pass) of its latest work this slot's stream has waited for
-        super(_CachedSlot, self).__init__(model, shape, False, use_graph, topk, images)
+        super(_CachedSlot, self).__init__(model, shape, image_dtype, use_graph, topk, images)
 
     def _index_inputs(self, B, images, device):
         return {"insertSlot": torch.full((images,), -1, dtype=torch.int32, device=device),
@@ -694,6 +705,13 @@ class ModelPipeline(object):
     repeats across its splits: one pipeline per image file, or `clear_cache()` between them); a weight update empties the
     cache.  `host_cast` is off with a cache.  `cache_stats()` counts hits, misses, evictions and image bytes copied.
 
+    Features stored in fp16: with `image_dtype=torch.float16` the batch's images (and a cache's loader results) must be
+    fp16 host arrays -- anything else raises `ValueError` before anything is staged, so fp32 features are never rounded
+    silently.  The slots' pinned staging and the graphs' device image inputs are fp16, half the bytes cross PCIe (counted by
+    `h2d_bytes` and `cache_stats()`), and the captured ingest is `mac_ingest_nchw_f16`, which widens on the device: every
+    output is bit for bit what the default pipeline computes from the fp32 widening of the same features.  `host_cast=True`
+    is refused with it (there is nothing left to cast).  The default, `torch.float32`, widens an fp16 batch on the host.
+
     Questions are padded with 0 to the pipeline's fixed S (a captured graph cannot trim a batch to its longest question as
     `runBatch` does); the kernels mask by length, so attention at positions >= length is exactly 0.
 
@@ -707,8 +725,12 @@ class ModelPipeline(object):
     -> 512), and its graph's private pool holds its own patch matrices (231 MB for layer 0 at 64x1024x14x14)."""
 
     def __init__(self, model, shape, slots=4, use_graph=True, topk=1, host_cast=None, cast_threads=None, stage_ring=None,
-                 images=None, cache=None):
+                 images=None, cache=None, image_dtype=torch.float32):
         B, S, H, W = [int(v) for v in shape]
+        _check_image_dtype(image_dtype)
+        if image_dtype == torch.float16 and host_cast:
+            raise ValueError("host_cast=True casts fp32 features to bf16 on the host: with image_dtype=torch.float16 the "
+                             "features cross PCIe as stored and are widened on the device")
         p = model.trainer.params
         C = int(p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2])
         nfc = len([k for k in p.t if k.startswith("classifier/linearLayerfc_") and k.endswith("weights/weight")])
@@ -728,13 +750,14 @@ class ModelPipeline(object):
                 raise ValueError("cache must be None or an int >= B = %d (every batch's images must fit), got %r" % (B, cache))
             if model.cfg.memDim % 8:
                 raise ValueError("cache=C needs memDim %% 8 == 0 (the pool kernels' 16-byte vectors), got %d" % model.cfg.memDim)
-        self.images = images
+        self.images, self.image_dtype = images, image_dtype
         self.lib = _lib.load()
         self.model, self.params, self.shape, self.C, self.topk = model, p, (B, S, H, W), C, int(topk)
         self.use_graph = bool(use_graph)
         self.cast_threads = int(cast_threads) if cast_threads else max(1, min(12, usable_cpus() - 2))
         numel = (B if images is None else images) * C * H * W
-        self.host_cast = model._stem.prec == "bf16" and host_cast is not False and cache is None
+        self.host_cast = (model._stem.prec == "bf16" and host_cast is not False and cache is None
+                          and image_dtype == torch.float32)
         self.cast_ms = None
         if self.host_cast and host_cast is None:
             self.cast_ms = _time_cast(self.lib, numel, self.cast_threads)
@@ -742,7 +765,8 @@ class ModelPipeline(object):
         self._version = p.version
         self._cache = self.pool = None
         if cache is None:
-            self.slots = [_ModelSlot(model, self.shape, self.host_cast, self.use_graph, self.topk, images)
+            slot_dtype = torch.bfloat16 if self.host_cast else image_dtype
+            self.slots = [_ModelSlot(model, self.shape, slot_dtype, self.use_graph, self.topk, images)
                           for _ in range(int(slots))]
         else:
             # the pool holds what the cell's read unit reads: bf16 for the bf16 and e4m3 hoisted forms (MACCell's
@@ -752,7 +776,7 @@ class ModelPipeline(object):
             self.pool = torch.zeros(cache, H * W, cfg.memDim, dtype=torch.bfloat16 if pool_bf16 else torch.float32,
                                     device=p.device)
             self._cache = _KBCache(cache, slots)
-            self.slots = [_CachedSlot(model, self.shape, self.use_graph, self.topk, images, self.pool)
+            self.slots = [_CachedSlot(model, self.shape, self.use_graph, self.topk, images, self.pool, image_dtype)
                           for _ in range(int(slots))]
         self._ring = (_CastRing(self.lib, numel, max(2, int(stage_ring) if stage_ring else 3), self.cast_threads)
                       if self.host_cast else None)
@@ -760,7 +784,8 @@ class ModelPipeline(object):
         self._ahead = None                  # (next_batch["images"] as given, its host tensor) of the cast in flight
         # with images=U: a batch of k images copies k of the U counted here; with cache=C only the questions, their lengths
         # and kbSlot are counted (cache_stats() counts the image bytes, and each stem pass adds U * 4 bytes of insert slots)
-        self.h2d_bytes = numel * (2 if self.host_cast else 4) + B * S * 4 + B * 4 + (0 if images is None else B * 4)
+        self.h2d_bytes = (numel * (2 if self.host_cast or image_dtype == torch.float16 else 4) + B * S * 4 + B * 4
+                          + (0 if images is None else B * 4))
         if cache is not None:
             self.h2d_bytes = B * S * 4 + B * 4 + B * 4
         self.d2h_bytes = sum(v.numel() * v.element_size() for v in self.slots[0].outs_host.values())
@@ -788,6 +813,9 @@ class ModelPipeline(object):
             v = torch.as_tensor(batch[key])
             if v.device.type != "cpu" or tuple(v.shape) != shp:
                 raise ValueError("%s must be a host tensor of shape %s, got %s on %s" % (key, shp, tuple(v.shape), v.device))
+            if key == "images" and self.image_dtype == torch.float16:
+                _check_f16(v, "the batch's images")
+                dtype = torch.float16
             out.append(v.to(dtype).contiguous())
         if self.images is None:
             return out + [None]
@@ -851,17 +879,18 @@ class ModelPipeline(object):
         return out + [ids.tolist(), batch["images"]]
 
     def _loaded(self, load, miss):
-        """The loader's features of the missing keys, checked: a host fp32 tensor [m, C, H, W]."""
+        """The loader's features of the missing keys, checked: a host tensor [m, C, H, W] of the pipeline's image dtype."""
         H, W = self.shape[2:]
         res = load(np.asarray(miss, dtype=np.int64))
+        name = "fp16" if self.image_dtype == torch.float16 else "fp32"
         try:
             v = torch.as_tensor(res)
         except (TypeError, RuntimeError) as exc:
-            raise ValueError("the images loader must return an array of fp32 features: %s" % exc)
+            raise ValueError("the images loader must return an array of %s features: %s" % (name, exc))
         want = (len(miss), self.C, H, W)
-        if v.device.type != "cpu" or v.dtype != torch.float32 or tuple(v.shape) != want:
-            raise ValueError("the images loader must return host fp32 features of shape %s (NCHW), got %s %s on %s"
-                             % (want, v.dtype, tuple(v.shape), v.device))
+        if v.device.type != "cpu" or v.dtype != self.image_dtype or tuple(v.shape) != want:
+            raise ValueError("the images loader must return host %s features of shape %s (NCHW), got %s %s on %s"
+                             % (name, want, v.dtype, tuple(v.shape), v.device))
         return v.contiguous()
 
     def _submit_cached(self, batch):
@@ -908,7 +937,7 @@ class ModelPipeline(object):
         for j, ev in enumerate(events):
             for r in plan.rows[j * U:(j + 1) * U]:
                 cache.written[r] = (t, j, ev)
-        cache.stats["image_bytes"] += 0 if imgs is None else imgs.numel() * 4
+        cache.stats["image_bytes"] += 0 if imgs is None else imgs.numel() * imgs.element_size()
         return t
 
     def cache_stats(self):
@@ -949,10 +978,10 @@ class _TrainSlot(object):
     """One training batch in flight: pinned host staging and device inputs, the step's pinned results, and the event of the
     step that reads them."""
 
-    def __init__(self, B, S, C, H, W, device, images=None):
+    def __init__(self, B, S, C, H, W, device, images=None, image_dtype=torch.float32):
         self.host = {"questions": _pinned(B * S, torch.int32), "questionLengths": _pinned(B, torch.int32),
                      "answers": _pinned(B, torch.int32),
-                     "images": _pinned((B if images is None else images) * C * H * W, torch.float32)}
+                     "images": _pinned((B if images is None else images) * C * H * W, image_dtype)}
         if images is not None:      # question b asks about image imageIndex[b] of the batch's k <= U
             self.host["imageIndex"] = _pinned(B, torch.int32)
         self.dev = {k: torch.empty(v.numel(), dtype=v.dtype, device=device) for k, v in self.host.items()}
@@ -1002,10 +1031,17 @@ class TrainPipeline(object):
     images are staged and copied, and the stem runs forward and backward over those k
     (`DPTrainer.full_forward_backward` with `imageIndex`: `mac_kb_gather`, `mac_kb_gather_bwd`).  The stem's input dropout is
     then drawn once per image, not once per question; everything after the stem is the step without an index.  With each
-    rank's shard, each rank passes its own images and index.  Bad batches raise `ValueError` before anything is staged."""
+    rank's shard, each rank passes its own images and index.  Bad batches raise `ValueError` before anything is staged.
 
-    def __init__(self, model, shape, depth=2, stage_threads=None, images=None):
+    Features stored in fp16: with `image_dtype=torch.float16` the batch's images must be fp16 host arrays (anything else
+    raises `ValueError` before anything is staged); the pinned staging and device image buffers are fp16, half the bytes are
+    staged and copied, and the step's ingest is `mac_ingest_nchw_train_f16`, which widens on the device: the step is bit for
+    bit the default pipeline's step on the fp32 widening of the same features.  The default, `torch.float32`, widens an fp16
+    batch on the host."""
+
+    def __init__(self, model, shape, depth=2, stage_threads=None, images=None, image_dtype=torch.float32):
         B, S, H, W = [int(v) for v in shape]
+        _check_image_dtype(image_dtype)
         t = model.trainer
         if t.stem is None:
             raise ValueError("the model's trainer has no stem: TrainPipeline trains the whole model")
@@ -1019,7 +1055,7 @@ class TrainPipeline(object):
             raise ValueError("the image features have %d channels: mac_ingest_nchw_train needs a multiple of 64" % C)
         if images is not None and not (isinstance(images, int) and not isinstance(images, bool) and 1 <= images <= B):
             raise ValueError("images must be None or an int in 1..B = %d, got %r" % (B, images))
-        self.images = images
+        self.images, self.image_dtype = images, image_dtype
         self.model, self.trainer, self.shape, self.C = model, t, (B, S, H, W), C
         self.stage_threads = int(stage_threads) if stage_threads else max(1, min(8, usable_cpus() // 2))
         self._pool = None
@@ -1027,7 +1063,7 @@ class TrainPipeline(object):
             from concurrent.futures import ThreadPoolExecutor
             self._pool = ThreadPoolExecutor(self.stage_threads)
         self.copy_stream = torch.cuda.Stream()
-        self.slots = [_TrainSlot(B, S, C, H, W, p.flat.device, images) for _ in range(int(depth))]
+        self.slots = [_TrainSlot(B, S, C, H, W, p.flat.device, images, image_dtype) for _ in range(int(depth))]
         self._next = 0
 
     def _host(self, batch):
@@ -1049,6 +1085,9 @@ class TrainPipeline(object):
                 raise ValueError("%s must be host memory, got a tensor on %s" % (key, v.device))
             if key != "images" and (v.dtype.is_floating_point or v.dtype == torch.bool):
                 raise ValueError("%s must hold integers, got %s" % (key, v.dtype))
+            if key == "images" and self.image_dtype == torch.float16:
+                _check_f16(v, "the batch's images")
+                dtype = torch.float16
             out[key] = v if v.dtype == dtype and v.is_contiguous() else v.to(dtype).contiguous()
         q, ql, a, img = out["questions"], out["questionLengths"], out["answers"], out["images"]
         if q.dim() != 2 or q.shape[0] != B or not 1 <= q.shape[1] <= S:
@@ -1079,7 +1118,7 @@ class TrainPipeline(object):
         return q, ql, a, img, idx, longest
 
     def _stage_images(self, dst, src):
-        """Copy the flat fp32 `src` into the pinned `dst` on the staging threads (numpy copies release the GIL)."""
+        """Copy the flat `src` into the pinned `dst` of its dtype on the staging threads (numpy copies release the GIL)."""
         d, s = dst.numpy(), src.reshape(-1).numpy()
         if self._pool is None:
             np.copyto(d, s)

@@ -169,20 +169,23 @@ class Stem(object):
         return x.view(B, H * Wd, x.shape[3])
 
     def forward_nchw(self, images, keep=1.0, step=0, save_for_backward=False):
-        """`forward` from the features in the layout they are stored in: images [B,C,H,W], contiguous, fp32 or -- `prec="bf16"`
+        """`forward` from the features in the layout they are stored in: images [B,C,H,W], contiguous, fp32, fp16 or -- `prec="bf16"`
         inference only, whose layer 0 then reads nothing but bf16(x) -- bf16.  The ingest kernels (csrc/ingest.cuh) replace
         the NHWC permute.  Inference (keep = 1, no save_for_backward): `mac_ingest_nchw` writes the bf16 stem's layer-0 patch
         matrix directly, for the other precisions the fp32 NHWC tensor their own patch passes read.  Training (a dropout or
         save_for_backward): the bf16 and bf16x3 stems run `mac_ingest_nchw_train`, which writes the undropped fp32 NHWC tensor
         (saved as layer 0's input) and layer 0's dropped-out bf16 or split patch matrix from one read; the fp32 stem runs the
         NHWC ingest and its usual pass.  Returns -- and saves, and differentiates -- what
-        `forward(images.permute(0, 2, 3, 1).contiguous(), keep, step, save_for_backward)` does, bit for bit.  C must be a
-        multiple of 64.  Raises before any launch."""
+        `forward(images.permute(0, 2, 3, 1).contiguous(), keep, step, save_for_backward)` does, bit for bit.  fp16 images
+        (every precision, inference and training) run the `_f16` entry points, which widen on the device: the result, the
+        saved tensors and the gradients are those of `forward_nchw(images.float(), ...)` bit for bit.  C must be a multiple
+        of 64.  Raises before any launch."""
         if images.dim() != 4 or not images.is_contiguous():
             raise ValueError("images must be a contiguous [B, C, H, W] tensor")
-        if images.dtype not in (torch.float32, torch.bfloat16):
-            raise ValueError("images must be float32 or bfloat16, got %s" % images.dtype)
+        if images.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+            raise ValueError("images must be float32, float16 or bfloat16, got %s" % images.dtype)
         x_bf16 = int(images.dtype == torch.bfloat16)
+        f16 = images.dtype == torch.float16
         train = save_for_backward or float(keep) != 1.0
         if x_bf16 and (self.prec != "bf16" or train):
             raise ValueError("bf16 images are for the bf16 stem's inference only: prec=%r%s reads the fp32 features"
@@ -200,21 +203,27 @@ class Stem(object):
             split = self.prec == "bf16x3"
             x = torch.empty((B, H, Wd, C), dtype=torch.float32, device=self.device)
             cols = torch.empty((B * H * Wd, 9 * C * (2 if split else 1)), dtype=torch.bfloat16, device=self.device)
-            check(self.lib.mac_ingest_nchw_train(ptr(images), ptr(x), ptr(cols), INGEST_COLS_SPLIT if split else INGEST_COLS_BF16,
-                                                 float(keep), self.seed, SITE_STEM, int(step), B, C, H, Wd, stream_ptr()),
-                  "mac_ingest_nchw_train")
+            name = "mac_ingest_nchw_train_f16" if f16 else "mac_ingest_nchw_train"
+            check(getattr(self.lib, name)(ptr(images), ptr(x), ptr(cols), INGEST_COLS_SPLIT if split else INGEST_COLS_BF16,
+                                          float(keep), self.seed, SITE_STEM, int(step), B, C, H, Wd, stream_ptr()), name)
             return self.forward(x, keep, step, save_for_backward, _cols0=cols)
         if self.prec != "bf16":
             if self.prec == "fp8":
                 self._check_fp8(C, 1.0)
             x = torch.empty((B, H, Wd, C), dtype=torch.float32, device=self.device)
-            check(self.lib.mac_ingest_nchw(ptr(images), x_bf16, ptr(x), INGEST_NHWC_F32, B, C, H, Wd, stream_ptr()),
-                  "mac_ingest_nchw")
+            self._ingest(images, x_bf16, x, INGEST_NHWC_F32)
             return self.forward(x, keep, step, save_for_backward)
         cols = torch.empty((B * H * Wd, 9 * C), dtype=torch.bfloat16, device=self.device)
-        check(self.lib.mac_ingest_nchw(ptr(images), x_bf16, ptr(cols), INGEST_PATCH_BF16, B, C, H, Wd, stream_ptr()),
-              "mac_ingest_nchw")
+        self._ingest(images, x_bf16, cols, INGEST_PATCH_BF16)
         return self.forward(images.permute(0, 2, 3, 1), _cols0=cols)     # a view: layer 0 reads `cols`, not the image
+
+    def _ingest(self, images, x_bf16, out, mode):
+        """`mac_ingest_nchw` of fp32 or bf16 images, `mac_ingest_nchw_f16` of fp16 ones."""
+        B, C, H, Wd = images.shape
+        if images.dtype == torch.float16:
+            check(self.lib.mac_ingest_nchw_f16(ptr(images), ptr(out), mode, B, C, H, Wd, stream_ptr()), "mac_ingest_nchw_f16")
+        else:
+            check(self.lib.mac_ingest_nchw(ptr(images), x_bf16, ptr(out), mode, B, C, H, Wd, stream_ptr()), "mac_ingest_nchw")
 
     def backward(self, d_kb, grads, need_d_images=False):
         """Backward of `forward(save_for_backward=True)` (the reference differentiates the graph with TF autodiff,
