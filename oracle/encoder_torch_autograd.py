@@ -7,11 +7,13 @@ import torch
 ENC = "encoder/birnnLayer/bidirectional_rnn/"
 
 
-def run(params_np, qIndices, lengths, keep_input=1.0, keep_question=1.0, uniforms=None, d_cntx=None, d_vecq=None,
-        forget_bias=1.0):
-    """Returns (cntx, vecq, grads: name -> d(sum(cntx*d_cntx) + sum(vecq*d_vecq))/d param)."""
-    t64 = lambda a: torch.tensor(a, dtype=torch.float64)
-    p = {k: t64(v).requires_grad_(True) for k, v in params_np.items()}
+def graph(p, qIndices, lengths, keep_input=1.0, keep_question=1.0, uniforms=None, forget_bias=1.0):
+    """The encoder as a differentiable graph: `p` maps variable names to fp64 tensors on one device, `qIndices` [B, S]
+    and `lengths` [B] are long tensors there.  Returns (questionWords, questionCntxWords, vecQuestions) tensors;
+    questionWords is the embedding lookup before the input dropout.  `uniforms`: the draws in the reference's call order
+    (an iterator is consumed as far as the dropouts need)."""
+    dev = p["qEmbeddings/emb"].device
+    t64 = lambda a: torch.as_tensor(a, dtype=torch.float64).to(dev)
     us = iter(uniforms or [])
 
     def dropout(x, keep):
@@ -19,22 +21,22 @@ def run(params_np, qIndices, lengths, keep_input=1.0, keep_question=1.0, uniform
             return x
         return x / keep * torch.floor(keep + t64(next(us)))
 
-    idx = torch.as_tensor(qIndices).long()
-    lens = torch.as_tensor(lengths).long()
+    idx, lens = qIndices, lengths
     B, S = idx.shape
     emb = p["qEmbeddings/emb"]
-    table = torch.cat([torch.zeros(1, emb.shape[1], dtype=torch.float64), emb], 0)
-    x = dropout(table[idx], keep_input)
+    table = torch.cat([torch.zeros(1, emb.shape[1], dtype=torch.float64, device=dev), emb], 0)
+    words = table[idx]
+    x = dropout(words, keep_input)
     outs, finals = [], []
-    ar = torch.arange(B)
+    ar = torch.arange(B, device=dev)
     uni = "encoder/rnnLayer/rnn/basic_lstm_cell/kernel" in p
     for name, reverse in ((("", False),) if uni else (("fw", False), ("bw", True))):
         sc = "encoder/rnnLayer/rnn/" if uni else ENC + name + "/"
         K, bias = p[sc + "basic_lstm_cell/kernel"], p[sc + "basic_lstm_cell/bias"]
         hd = K.shape[1] // 4
-        c = torch.zeros(B, hd, dtype=torch.float64)
-        h = torch.zeros(B, hd, dtype=torch.float64)
-        out = torch.zeros(B, S, hd, dtype=torch.float64)
+        c = torch.zeros(B, hd, dtype=torch.float64, device=dev)
+        h = torch.zeros(B, hd, dtype=torch.float64, device=dev)
+        out = torch.zeros(B, S, hd, dtype=torch.float64, device=dev)
         for s in range(S):
             live = (s < lens)
             t = torch.where(live, (lens - 1 - s) if reverse else torch.full_like(lens, s), torch.zeros_like(lens))
@@ -45,7 +47,7 @@ def run(params_np, qIndices, lengths, keep_input=1.0, keep_question=1.0, uniform
             lv = live.unsqueeze(1)
             c = torch.where(lv, cn, c)
             h = torch.where(lv, hn, h)
-            upd = torch.zeros(B, S, hd, dtype=torch.float64)
+            upd = torch.zeros(B, S, hd, dtype=torch.float64, device=dev)
             upd[ar, t] = torch.where(lv, hn, torch.zeros_like(hn))
             out = out + upd
         outs.append(out)
@@ -55,6 +57,16 @@ def run(params_np, qIndices, lengths, keep_input=1.0, keep_question=1.0, uniform
     if "encoder/linearLayerprojCW/weights/weight" in p:
         cntx = cntx @ p["encoder/linearLayerprojCW/weights/weight"] + p["encoder/linearLayerprojCW/biases/bias"]
         vecq = vecq @ p["encoder/linearLayerprojQ/weights/weight"] + p["encoder/linearLayerprojQ/biases/bias"]
+    return words, cntx, vecq
+
+
+def run(params_np, qIndices, lengths, keep_input=1.0, keep_question=1.0, uniforms=None, d_cntx=None, d_vecq=None,
+        forget_bias=1.0):
+    """Returns (cntx, vecq, grads: name -> d(sum(cntx*d_cntx) + sum(vecq*d_vecq))/d param)."""
+    t64 = lambda a: torch.tensor(a, dtype=torch.float64)
+    p = {k: t64(v).requires_grad_(True) for k, v in params_np.items()}
+    _, cntx, vecq = graph(p, torch.as_tensor(qIndices).long(), torch.as_tensor(lengths).long(), keep_input, keep_question,
+                          uniforms, forget_bias)
     grads = {}
     if d_cntx is not None:
         loss = (cntx * t64(d_cntx)).sum() + (vecq * t64(d_vecq)).sum()

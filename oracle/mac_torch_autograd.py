@@ -270,6 +270,22 @@ class _Cell(object):
         return new_control, new_memory, info
 
 
+def graph(cfg, p, x, lengths, L, dropouts=(1.0, 1.0, 1.0), uniforms=None, train=False, trace=None):
+    """The cell's L steps as a differentiable graph: `p` maps full variable names to fp64 tensors, `x` holds the fp64
+    "vecQuestions", "questionWords", "questionCntxWords" and "knowledgeBase", `lengths` the question lengths (long), all on
+    one device.  Returns (control_L, memory_L) tensors; every uniform of `uniforms` must be consumed."""
+    cell = _Cell(cfg, p, uniforms, dropouts, train, x["knowledgeBase"].device)
+    control, memory = cell.zero_state(x["vecQuestions"], x["questionWords"], x["questionCntxWords"], lengths,
+                                      x["knowledgeBase"])
+    for i in range(L):
+        control, memory, info = cell.step(i, control, memory)
+        if trace is not None:
+            trace.append({k: v.detach().cpu().numpy() for k, v in (("control", control), ("memory", memory),
+                                                                    ("info", info))})
+    assert next(cell.uniforms, None) is None, "uniform draws left over: the dropout calls differ from the reference's"
+    return control, memory
+
+
 def run(cfg, params_np, inputs_np, L, dropouts=(1.0, 1.0, 1.0), uniforms=None, d_control=None, d_memory=None,
         train=False, device="cpu", trace=None):
     """Returns (control_L, memory_L, grads) as numpy arrays, with grads keyed like the product's `mac_backward` output:
@@ -284,15 +300,7 @@ def run(cfg, params_np, inputs_np, L, dropouts=(1.0, 1.0, 1.0), uniforms=None, d
     for k in ("vecQuestions", words_key, "knowledgeBase"):
         x[k].requires_grad_(True)
     lengths = torch.as_tensor(inputs_np["questionLengths"]).long().to(dev)
-    cell = _Cell(cfg, p, uniforms, dropouts, train, dev)
-    control, memory = cell.zero_state(x["vecQuestions"], x["questionWords"], x["questionCntxWords"], lengths,
-                                      x["knowledgeBase"])
-    for i in range(L):
-        control, memory, info = cell.step(i, control, memory)
-        if trace is not None:
-            trace.append({k: v.detach().cpu().numpy() for k, v in (("control", control), ("memory", memory),
-                                                                    ("info", info))})
-    assert next(cell.uniforms, None) is None, "uniform draws left over: the dropout calls differ from the reference's"
+    control, memory = graph(cfg, p, x, lengths, L, dropouts, uniforms, train, trace)
     grads = {}
     if d_control is not None or d_memory is not None:
         loss = 0.0

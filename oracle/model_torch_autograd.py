@@ -1,0 +1,125 @@
+"""ORACLE (test infrastructure only): the reference's whole training loss (`MACnet.build`, model.py:774-821) as one
+differentiable fp64 PyTorch graph, used to check the trainer's hand-written backward element by element against
+`torch.autograd` (the reference uses TF autodiff, model.py:626-636):
+
+    embeddings + bi-LSTM (`encoder_torch_autograd.graph`) -> image stem (`stem_graph`) -> optional gather of each question's
+    knowledge base by `imageIndex` -> netLength MAC steps (`mac_torch_autograd.graph`) -> output unit and classifier
+    (`output_graph`) -> sum of the per-sample softmax cross-entropies / global_batch.
+
+Each unit consumes its own list of uniforms in the reference's call order, with tf.nn.dropout's x / keep * floor(keep + U).
+The forward is pinned to the chain of numpy oracles (each pinned to the reference's own code on the TF1 shim) and the
+gradient to central differences of this graph in tests/test_model_autograd_oracle.py."""
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+from oracle import encoder_torch_autograd, mac_torch_autograd
+
+UNITS = ("encoder", "stem", "cell", "output")
+
+
+def _dropout(x, keep, us):
+    if float(keep) == 1.0:
+        return x
+    return x / float(keep) * torch.floor(float(keep) + torch.as_tensor(next(us), dtype=torch.float64).to(x.device))
+
+
+def _act(relu, x):
+    """ops.py:161-187: the "RELU" activation of the stem and the classifier under `config.relu`."""
+    return F.elu(x) if relu == "ELU" else torch.relu(x)
+
+
+def mask_uniforms(mask):
+    """Uniforms whose tf.nn.dropout mask floor(keep + U) is exactly `mask` (0 / 1) for any keep in (2^-30, 1)."""
+    return torch.as_tensor(mask, dtype=torch.float64) * (1.0 - 2.0 ** -30)
+
+
+def stem_graph(relu, p, images, keep=1.0, uniforms=None):
+    """ops.CNNLayer (ops.py:380-438): per layer, dropout on the input, 3x3 stride-1 SAME conv2d with the HWIO kernel, bias,
+    activation.  `images` fp64 NHWC [B, H, W, C]; returns the knowledge base [B, H*W, d]."""
+    us = iter(uniforms or [])
+    cur = images
+    n = len([k for k in p if k.startswith("stem/") and k.endswith("kernels/kernel")])
+    for i in range(n):
+        cur = _dropout(cur, keep, us)
+        K = p["stem/cnnLayercnn_%d/kernels/kernel" % i]                       # HWIO -> OIHW
+        y = F.conv2d(cur.permute(0, 3, 1, 2), K.permute(3, 2, 0, 1), padding=K.shape[0] // 2).permute(0, 2, 3, 1)
+        cur = _act(relu, y + p["stem/cnnLayercnn_%d/biases/bias" % i])
+    return cur.reshape(cur.shape[0], -1, cur.shape[-1])
+
+
+def output_graph(relu, p, memory, vecQuestions, answers, keep=1.0, uniforms=None):
+    """outputOp + classifier + the per-sample sparse softmax cross-entropy (model.py:512-596): returns (logits, losses)."""
+    us = iter(uniforms or [])
+    eq = vecQuestions @ p["outputUnit/linearLayeroutQuestion/weights/weight"] + p["outputUnit/linearLayeroutQuestion/biases/bias"]
+    x = torch.cat([memory, eq], -1)
+    nfc = len([k for k in p if k.startswith("classifier/linearLayerfc_") and k.endswith("weights/weight")])
+    for i in range(nfc):
+        sc = "classifier/linearLayerfc_%d/" % i
+        x = _dropout(x, keep, us) @ p[sc + "weights/weight"] + p[sc + "biases/bias"]
+        if i < nfc - 1:
+            x = _act(relu, x)
+    losses = torch.logsumexp(x, -1) - x.gather(1, answers.view(-1, 1)).squeeze(1)
+    return x, losses
+
+
+def stem_grads(relu, params, images, keep, uniforms, d_kb):
+    """The stem's fp64 forward and its gradients for the upstream gradient `d_kb`: (kb, {name: grad}, d_images), on the
+    device and in the array kind (numpy or torch) of `images`."""
+    as_np = isinstance(images, np.ndarray)
+    dev = torch.device("cpu") if as_np else images.device
+    t64 = lambda a: torch.as_tensor(np.asarray(a) if isinstance(a, np.ndarray) else a, dtype=torch.float64).to(dev)
+    p = {k: t64(v).requires_grad_(True) for k, v in params.items()}
+    x = t64(images).requires_grad_(True)
+    kb = stem_graph(relu, p, x, keep, uniforms)
+    (kb * t64(d_kb)).sum().backward()
+    out = lambda t: t.detach().cpu().numpy() if as_np else t.detach()
+    return out(kb), {k: out(v.grad) for k, v in p.items()}, out(x.grad)
+
+
+def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="cpu", grad=True):
+    """The training loss of one shard.
+
+    `values`: every variable by its TF name (numpy or torch); `data`: "questions" [B, S] (0 = padding),
+    "questionLengths" [B], "answers" [B], the images as exactly one of "images" (NHWC [k, H, W, C]) and "images_nchw"
+    ([k, C, H, W], permuted here), and optionally "imageIndex" [B] (question b asks about image imageIndex[b]; without it
+    k = B).  `keeps`: {"encoder": (input, question), "stem": keep, "cell": (memory, read, write), "output": keep}.
+    `uniforms`: {unit: list of draws in the reference's call order} for the units in UNITS; each list must be consumed
+    exactly.  `global_batch`: the loss is sum(losses) / global_batch (default B).
+
+    Returns {"logits", "losses", "loss"} and, with `grad`, "grads" (every variable's gradient, zeros for the stored
+    batch-norm statistics) and "d_images" (in the layout of the images given), all fp64 tensors on `device`."""
+    dev = torch.device(device)
+    t64 = lambda a: torch.as_tensor(np.asarray(a) if isinstance(a, np.ndarray) else a).to(dev, torch.float64)
+    p = {k: t64(v).requires_grad_(grad and "/BatchNorm/moving_" not in k) for k, v in values.items()}
+    lng = lambda a: torch.as_tensor(np.asarray(a) if isinstance(a, np.ndarray) else a).to(dev, torch.long)
+    uniforms = uniforms or {}
+    assert set(uniforms) <= set(UNITS), sorted(uniforms)
+    its = {u: iter(uniforms.get(u, [])) for u in UNITS}
+    if ("images" in data) == ("images_nchw" in data):
+        raise ValueError("data needs exactly one of images and images_nchw")
+    nchw = "images_nchw" in data
+    x_img = t64(data["images_nchw" if nchw else "images"]).requires_grad_(grad)
+    questions, lengths, answers = lng(data["questions"]), lng(data["questionLengths"]), lng(data["answers"])
+    B = questions.shape[0]
+    words, cntx, vecq = encoder_torch_autograd.graph(p, questions, lengths, keeps["encoder"][0], keeps["encoder"][1],
+                                                     its["encoder"])
+    kb = stem_graph(cfg.relu, p, x_img.permute(0, 2, 3, 1) if nchw else x_img, keeps["stem"], its["stem"])
+    if data.get("imageIndex") is not None:
+        kb = kb[lng(data["imageIndex"])]
+    assert kb.shape[0] == B, (kb.shape, B)
+    x = {"vecQuestions": vecq, "questionWords": words, "questionCntxWords": cntx, "knowledgeBase": kb}
+    _, memory = mac_torch_autograd.graph(cfg, p, x, lengths, L, keeps["cell"], its["cell"], train=True)
+    # the cell's vecQuestions is the encoder's output: the output unit reads the same tensor (model.py:512-528)
+    logits, losses = output_graph(cfg.relu, p, memory, vecq, answers, keeps["output"], its["output"])
+    for u in UNITS:
+        assert next(its[u], None) is None, "%s: uniform draws left over: the dropout calls differ from the reference's" % u
+    loss = losses.sum() / float(B if global_batch is None else global_batch)
+    out = {"logits": logits.detach(), "losses": losses.detach(), "loss": loss.detach()}
+    if grad:
+        names = [k for k, v in p.items() if v.requires_grad]
+        got = torch.autograd.grad(loss, [p[k] for k in names] + [x_img], allow_unused=True)
+        g = dict(zip(names, got[:-1]))
+        out["grads"] = {k: (g[k] if g.get(k) is not None else torch.zeros_like(v)).detach() for k, v in p.items()}
+        out["d_images"] = (got[-1] if got[-1] is not None else torch.zeros_like(x_img)).detach()
+    return out

@@ -2,26 +2,39 @@
 netLength MAC steps -> output unit -> classifier -> mean softmax-CE, and its hand-written backward.
 
 Forward: against the chain of fp64 numpy oracles (each pinned to the reference's own code on the TF1 shim).
-Backward: the flat gradient bucket against central differences of that fp64 oracle chain along random directions
-restricted to each sub-model's variables (a check that needs no autograd restatement of the chained model)."""
+Backward: the flat gradient bucket element by element against torch.autograd on the fp64 graph of the same loss
+(oracle/model_torch_autograd.py, pinned to that oracle chain and to central differences in
+tests/test_model_autograd_oracle.py)."""
 import numpy as np
 import pytest
 
 from tests._util import max_rel
 
 
-def _oracle_loss(cfg, L, values, data):
+def _oracle_loss(cfg, L, values, data, keeps=None, uniforms=None):
+    """The chain of numpy oracles on `data` (NHWC "images", optionally "imageIndex").  `keeps` and `uniforms` as
+    `oracle.model_torch_autograd.run` takes them: every dropout with its uniforms, the cell in training mode; by default
+    every dropout off."""
     from oracle.encoder_oracle import encoder_forward
     from oracle.stem_oracle import stem_forward
     from oracle.output_oracle import output_forward
     from oracle.mac_oracle import MACOracle
+    keeps = keeps or {"encoder": (1.0, 1.0), "stem": 1.0, "cell": (1.0, 1.0, 1.0), "output": 1.0}
+    us = uniforms or {}
     v = {k: np.asarray(a, np.float64) for k, a in values.items()}
-    eo = encoder_forward(v, data["questions"], data["questionLengths"])
-    kb = stem_forward(cfg.relu, {k: a for k, a in v.items() if k.startswith("stem/")}, data["images"].astype(np.float64))
-    ref = MACOracle(cfg, v, dtype=np.float64).run(L, eo["vecQuestions"], eo["questionWords"], eo["questionCntxWords"],
-                                                  data["questionLengths"], kb)
+    eo = encoder_forward(v, data["questions"], data["questionLengths"], keeps["encoder"][0], keeps["encoder"][1],
+                         us.get("encoder"))
+    kb = stem_forward(cfg.relu, {k: a for k, a in v.items() if k.startswith("stem/")}, data["images"].astype(np.float64),
+                      keeps["stem"], us.get("stem"))
+    if data.get("imageIndex") is not None:
+        kb = kb[np.asarray(data["imageIndex"])]
+    cell = MACOracle(cfg, v, dtype=np.float64)
+    cell.train = uniforms is not None
+    dm, dr, dw = keeps["cell"]
+    ref = cell.run(L, eo["vecQuestions"], eo["questionWords"], eo["questionCntxWords"], data["questionLengths"], kb,
+                   memoryDropout=dm, readDropout=dr, writeDropout=dw, uniforms=us.get("cell"))
     out = output_forward(cfg.relu, {k: a for k, a in v.items() if k.startswith(("outputUnit/", "classifier/"))},
-                         ref.memory, eo["vecQuestions"], data["answers"])
+                         ref.memory, eo["vecQuestions"], data["answers"], keep=keeps["output"], uniforms=us.get("output"))
     return out
 
 
@@ -64,34 +77,38 @@ def test_full_model_forward_and_gradient(flags):
     ref = _oracle_loss(cfg, L, values, data)
     assert max_rel(logits.cpu().numpy(), ref["logits"]) < 1e-4
     assert max_rel(losses.cpu().numpy(), ref["losses"]) < 1e-4
-    check_directional_derivatives(cfg, L, values, data, tr, flags)
+    check_bucket_against_fp64(cfg, L, values, data, tr, flags)
 
 
-def check_directional_derivatives(cfg, L, values, data, tr, tag):
-    """The trainer's gradient bucket (of the loss at `values` on `data`) along one random direction per sub-model's
-    variables against central differences of the fp64 oracle chain."""
-    bucket = tr.bucket.cpu().numpy().astype(np.float64)
-    offs, specs = tr.params.offsets, tr.params.specs
-    groups = {"encoder": ("encoder/", "qEmbeddings/"), "stem": ("stem/",), "cell": ("MACnetwork/",),
-              "output": ("outputUnit/", "classifier/")}
-    for gname, prefixes in groups.items():
-        names = [n for n in specs if n.startswith(prefixes)]
-        assert names, gname
-        drng = np.random.RandomState(100 + sorted(groups).index(gname))
-        direction = {n: drng.standard_normal(values[n].shape) for n in names}
-        analytic = 0.0
-        for n in names:
-            k = max(1, int(np.prod(specs[n][0])) if specs[n][0] else 1)
-            analytic += float(np.dot(bucket[offs[n]:offs[n] + k], direction[n].reshape(-1)))
-        eps = 1e-5
-        lo = dict(values)
-        hi = dict(values)
-        for n in names:
-            hi[n] = values[n].astype(np.float64) + eps * direction[n]
-            lo[n] = values[n].astype(np.float64) - eps * direction[n]
-        numeric = (_oracle_loss(cfg, L, hi, data)["loss"] - _oracle_loss(cfg, L, lo, data)["loss"]) / (2 * eps)
-        print("%s %-8s directional derivative: analytic %.6e numeric %.6e" % (tag, gname, analytic, numeric))
-        assert abs(analytic - numeric) <= 2e-3 * max(abs(numeric), 1e-3), (gname, analytic, numeric)
+# fp32 trainer against the fp64 graph, every dropout off (H100 80GB HBM3, 700 W power limit):           measured worst
+BAR_GRAD = 1e-5             # at the initial weights with perturbed biases, and at weights moved by four steps   2.8e-6
+BAR_NULL = 1e-7             # a softmax logit bias, of the model's largest gradient                               2.5e-8
+
+
+def check_bucket_against_fp64(cfg, L, values, data, tr, tag, bar=BAR_GRAD, null_bar=BAR_NULL):
+    """The trainer's gradient bucket of the loss at `values` on `data` (every dropout off) against torch.autograd on the
+    fp64 graph (oracle/model_torch_autograd.py), element by element: max |got - ref| / max |ref| of each tensor; a softmax
+    logit bias (true gradient 0) against the model's largest gradient.  Returns the worst errors."""
+    import torch
+    from oracle import model_torch_autograd as MA
+    from tests.test_gpu_tc32_training import NULL_GRADIENTS
+    keeps = {"encoder": (1.0, 1.0), "stem": 1.0, "cell": (1.0, 1.0, 1.0), "output": 1.0}
+    ref = MA.run(cfg, L, values, data, keeps, device="cuda")["grads"]
+    p = tr.params
+    gmax = max(float(g.abs().max()) for g in ref.values())
+    errs, null = {}, {}
+    for n, g in ref.items():
+        got = tr.bucket[p.offsets[n]:p.offsets[n] + g.numel()].double()
+        if n.endswith(NULL_GRADIENTS):
+            null[n] = float(got.abs().max()) / gmax
+        elif "/BatchNorm/moving_" not in n:
+            errs[n] = float((got - g.reshape(-1)).abs().max()) / float(g.abs().max())
+    top = sorted(errs.items(), key=lambda kv: -kv[1])[:3]
+    print("%s gradients against fp64: worst %s; null %.1e" % (tag, ["%s %.2e" % kv for kv in top], max(null.values())))
+    bad = {n: e for n, e in errs.items() if not e < bar}
+    bad.update({n: e for n, e in null.items() if not e < null_bar})
+    assert not bad, (tag, bad)
+    return errs
 
 
 @pytest.mark.gpu

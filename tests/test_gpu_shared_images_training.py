@@ -16,7 +16,8 @@ import pytest
 import torch
 
 from mac_network_b200 import _lib as L_
-from tests.test_gpu_stem_bf16x3 import BAR_FWD, BAR_GRAD, _mr, _stem_autograd_fp64
+from oracle.model_torch_autograd import mask_uniforms, stem_grads
+from tests.test_gpu_stem_bf16x3 import BAR_FWD, BAR_GRAD, _mr
 from tests.test_stem_tc_training import TOL_STEM_BF16, _uniform_mask
 
 pytestmark = pytest.mark.gpu
@@ -139,9 +140,9 @@ def test_stem_through_gather_and_sum_against_fp64_autograd(prec, k):
     assert torch.equal(kb, kb_u[index.long()])
     # the fp64 model: the per-image masks (the Philox numbering over the k-row tensor), each image's gradient summed over its
     # questions in fp64
-    masks = [_uniform_mask(lib, seed, SITE_STEM + i, step, (k, H, W, c), keep).double() for i, c in ((0, cin), (1, cout))]
+    us = [mask_uniforms(_uniform_mask(lib, seed, SITE_STEM + i, step, (k, H, W, c), keep)) for i, c in ((0, cin), (1, cout))]
     d_ref = torch.zeros(k, N, cout, dtype=torch.float64, device="cuda").index_add_(0, index.long(), d_kb.double())
-    kb_ref, gref, _ = _stem_autograd_fp64(params, images.permute(0, 2, 3, 1), keep, masks, d_ref)
+    kb_ref, gref, _ = stem_grads("ELU", params, images.permute(0, 2, 3, 1), keep, us, d_ref)
     errs = {"kb": _mr(kb, kb_ref[index.long()])}
     errs.update({n: _mr(grads[n], gref[n]) for n in gref})
     print("%s stem, %d images for %d questions: %s" % (prec, k, B, ", ".join(

@@ -13,6 +13,7 @@ import pytest
 import torch
 
 from mac_network_b200 import _lib as L_
+from oracle.model_torch_autograd import mask_uniforms, stem_grads
 from tests.test_gpu_wgmma import excess, pack3, split_hi_lo
 from tests.test_stem_tc_training import _col2im, _patches, _uniform_mask
 
@@ -153,23 +154,6 @@ def test_conv3x3_bwd_tc32_against_fp64(shape, keep, with_dx):
 
 
 # ------------------------------------------------------------------------------------------------ the stem
-def _stem_autograd_fp64(params, images, keep, masks, d_kb):
-    """torch.autograd on the fp64 restatement of the fp32 stem (patch matrix @ kernel + bias, ELU), on the GPU."""
-    p = {k: v.double().requires_grad_(True) for k, v in params.items()}
-    x = images.double().requires_grad_(True)
-    B, H, W, _ = x.shape
-    cur = x
-    for i in range(len(params) // 2):
-        if keep < 1.0:
-            cur = cur / keep * masks[i]
-        K = p["stem/cnnLayercnn_%d/kernels/kernel" % i]
-        y = _patches(cur) @ K.reshape(-1, K.shape[3]) + p["stem/cnnLayercnn_%d/biases/bias" % i]
-        cur = torch.nn.functional.elu(y).reshape(B, H, W, -1)
-    kb = cur.reshape(B, H * W, -1)
-    (kb * d_kb.double()).sum().backward()
-    return kb.detach(), {k: v.grad for k, v in p.items()}, x.grad
-
-
 @pytest.mark.parametrize("keep,shape", [(0.82, (2, 5, 7, 128, 128)), (1.0, (4, 14, 14, 256, 256)),
                                         (0.82, (64, 14, 14, 1024, 512))])
 def test_stem_bf16x3_training_against_fp64_autograd(keep, shape):
@@ -187,9 +171,9 @@ def test_stem_bf16x3_training_against_fp64_autograd(keep, shape):
     kb_inf = st.forward(images, keep=keep, step=4)                               # the inference form: the same products
     torch.cuda.synchronize()
     assert torch.equal(kb_inf, kb)
-    masks = [_uniform_mask(lib, 13, SITE_STEM + i, 4, (B, H, W, c), keep).double() for i, c in ((0, cin), (1, cout))] \
+    us = [mask_uniforms(_uniform_mask(lib, 13, SITE_STEM + i, 4, (B, H, W, c), keep)) for i, c in ((0, cin), (1, cout))] \
         if keep < 1.0 else None
-    kb_ref, gref, dimg_ref = _stem_autograd_fp64(params, images, keep, masks, d_kb)
+    kb_ref, gref, dimg_ref = stem_grads("ELU", params, images, keep, us, d_kb)
     errs = {"kb": _mr(kb, kb_ref), "d_images": _mr(d_img, dimg_ref)}
     errs.update({k: _mr(grads[k], gref[k]) for k in gref})
     print("bf16x3 stem keep=%s %s: %s" % (keep, shape, ", ".join("%s %.2e" % (k.split("/")[1] + "/" + k.split("/")[-1]

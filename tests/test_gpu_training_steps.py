@@ -9,7 +9,8 @@ evaluation, and the graphs `serving.HostPipeline` captures.
     trainer's steps reuse cached cells, rebuild an evicted one and reuse that again; the twin builds every cell.  Each optimizer
     step element by element against `dp.adam_reference`, which a twin that shares a wrongly plumbed step counter or
     hyperparameter would not catch.
-(b) The fp32 trainer at weights that have moved (biases no longer 0) against the fp64 oracle chain, and its tc32 twin there.
+(b) The fp32 trainer at weights that have moved (biases no longer 0) against the fp64 oracle chain and the fp64 autograd graph,
+    and its tc32 twin there.
 (c) Resume from `save_training_state` equals the uninterrupted run bit for bit.
 (d) `MACnet.runBatch` evaluation between training steps equals a fresh model's, and does not disturb the training run.
 (e) `HostPipeline` after a weight update equals a direct cell on the new weights."""
@@ -19,7 +20,7 @@ import torch
 
 from mac_network_b200.config import MACConfig
 from tests._util import load_golden, max_rel
-from tests.test_full_model import _make, _oracle_loss, check_directional_derivatives
+from tests.test_full_model import _make, _oracle_loss, check_bucket_against_fp64
 from tests.test_gpu_backward_kernels import same_bits
 
 pytestmark = pytest.mark.gpu
@@ -164,7 +165,7 @@ def test_long_lived_trainer_equals_a_fresh_twin_at_every_step(case):
 # ================================================================================================ (b) fp64 at moved weights
 def test_fp32_trainer_matches_fp64_at_moved_weights_and_so_does_its_tc32_twin():
     """fp32 `args`, every dropout 1.0, lr = 3e-3: logits and losses against the fp64 oracle chain at every step's weights;
-    at step K the per-group directional derivatives, then a tc32 / bf16x3-stem twin's bucket and loss against the fp32 ones
+    at step K every gradient tensor element by element against the fp64 graph, then a tc32 / bf16x3-stem twin's bucket and loss against the fp32 ones
     at the bars of test_gpu_tc32_training.py's bench-shape twin test (measured there at initialised weights only)."""
     from mac_network_b200.dp import DPTrainer
     from tests.test_gpu_tc32_training import NULL_GRADIENTS
@@ -186,7 +187,7 @@ def test_fp32_trainer_matches_fp64_at_moved_weights_and_so_does_its_tc32_twin():
             tr.apply()
     still = [n for n, v in values.items() if n.endswith("bias") and v.size > 1 and not np.max(np.abs(v)) > 1e-3]
     assert not still, still             # every bias vector has moved off TF's zero initialisation
-    check_directional_derivatives(cfg, L, values, data, tr, "step %d" % K)
+    check_bucket_against_fp64(cfg, L, values, data, tr, "step %d" % K)
     g32, l32 = tr.bucket.double(), float(losses.double().mean())
     tw = DPTrainer(cfg, L, prec="tc32", bwd_tc=True, stem_prec="bf16x3", **kw)
     tw.params.flat.copy_(tr.params.flat)

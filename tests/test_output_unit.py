@@ -6,6 +6,7 @@ import os
 import numpy as np
 import pytest
 
+from oracle.model_torch_autograd import output_graph
 from oracle.output_oracle import output_forward
 from mac_network_b200.output_unit import output_specs, init_output_params
 from tests._util import GOLDEN_DIR, max_rel
@@ -60,18 +61,12 @@ def test_output_unit_gpu_forward_backward(keep):
     ref = output_forward("ELU", pv, memory, vecq, answers, keep=keep, uniforms=us)
     assert max_rel(logits.cpu().numpy(), ref["logits"]) < 1e-4
     assert max_rel(losses.cpu().numpy(), ref["losses"]) < 1e-4
-    # gradients vs torch.autograd on an fp64 restatement with the same masks
+    # gradients vs torch.autograd on the fp64 restatement with the same masks
     t = lambda a: torch.tensor(a, dtype=torch.float64, requires_grad=True)
     P = {k: t(v) for k, v in pv.items()}
     M_, Q_ = t(memory), t(vecq)
-    it = iter(us)
-    drop = (lambda x: x / keep * torch.floor(keep + torch.tensor(next(it)))) if keep < 1.0 else (lambda x: x)
-    eq = Q_ @ P["outputUnit/linearLayeroutQuestion/weights/weight"] + P["outputUnit/linearLayeroutQuestion/biases/bias"]
-    h = torch.nn.functional.elu(drop(torch.cat([M_, eq], 1)) @ P["classifier/linearLayerfc_0/weights/weight"]
-                                + P["classifier/linearLayerfc_0/biases/bias"])
-    lg = drop(h) @ P["classifier/linearLayerfc_1/weights/weight"] + P["classifier/linearLayerfc_1/biases/bias"]
-    loss = torch.nn.functional.cross_entropy(lg, torch.from_numpy(answers).long())
-    loss.backward()
+    _, ls = output_graph("ELU", P, M_, Q_, torch.from_numpy(answers).long(), keep=keep, uniforms=us)
+    ls.mean().backward()
     assert max_rel(dmem.cpu().numpy(), M_.grad.numpy()) < 2e-4
     assert max_rel(dq.cpu().numpy(), Q_.grad.numpy()) < 2e-4
     for k in pv:

@@ -6,6 +6,7 @@ import os
 import numpy as np
 import pytest
 
+from oracle.model_torch_autograd import stem_grads
 from oracle.stem_oracle import stem_forward
 from mac_network_b200.stem import stem_specs, init_stem_params
 from tests._util import GOLDEN_DIR, max_rel
@@ -57,33 +58,12 @@ def test_stem_gpu(prec, keep, shape):
     assert err < (1e-4 if prec == "fp32" else 2e-2)
 
 
-def _torch_stem_grads(pv, images, keep, us, d_kb):
-    """fp64 torch.autograd restatement of the stem (conv2d = the published TF SAME/stride-1 semantics) -> gradients."""
-    import torch
-    import torch.nn.functional as F
-    t64 = lambda a: torch.tensor(np.asarray(a), dtype=torch.float64)
-    p = {k: t64(v).requires_grad_(True) for k, v in pv.items()}
-    x = t64(images).requires_grad_(True)
-    cur, it = x, iter(us)
-    n = len([k for k in pv if k.endswith("kernels/kernel")])
-    for i in range(n):
-        if keep < 1.0:
-            cur = cur / keep * torch.floor(keep + t64(next(it)))
-        K = p["stem/cnnLayercnn_%d/kernels/kernel" % i]                       # HWIO -> OIHW
-        y = F.conv2d(cur.permute(0, 3, 1, 2), K.permute(3, 2, 0, 1), padding=1).permute(0, 2, 3, 1)
-        cur = F.elu(y + p["stem/cnnLayercnn_%d/biases/bias" % i])
-    kb = cur.reshape(cur.shape[0], -1, cur.shape[-1])
-    (kb * t64(d_kb)).sum().backward()
-    g = {k: v.grad.numpy() for k, v in p.items()}
-    return kb.detach().numpy(), g, x.grad.numpy()
-
-
 def test_torch_stem_restatement_matches_oracle():
     meta, g = _load("stem_train")
     B, H, W, cin, cout = meta["shape"]
     pv = init_stem_params(stem_specs(cin, cout, meta["layers"], meta["ksize"]), seed=meta["param_seed"], dtype=np.float64)
     us = [g["uniform_%03d" % i] for i in range(meta["n_uniform"])]
-    kb, _, _ = _torch_stem_grads(pv, g["images"], meta["keep"], us, np.zeros_like(g["kb"]))
+    kb, _, _ = stem_grads(meta["relu"], pv, g["images"], meta["keep"], us, np.zeros_like(g["kb"]))
     assert np.max(np.abs(kb - g["kb"])) < 1e-12
 
 
@@ -112,7 +92,7 @@ def test_stem_backward_gpu(keep, shape):
             u = torch.empty(B * H * W * c, device="cuda")
             L.check(lib.mac_dropout_uniform(13, SITE_STEM + layer, 4, L.ptr(u), u.numel(), L.stream_ptr()))
             us.append(u.cpu().numpy().astype(np.float64).reshape(B, H, W, c))
-    kb_ref, gref, dimg_ref = _torch_stem_grads(pv, images, keep, us, d_kb)
+    kb_ref, gref, dimg_ref = stem_grads("ELU", pv, images, keep, us, d_kb)
     assert max_rel(kb.cpu().numpy(), kb_ref) < 1e-4
     for k in gref:
         err = max_rel(grads[k].cpu().numpy(), gref[k])

@@ -281,7 +281,7 @@ def test_stem_bf16_training_against_fp64_autograd(keep, shape):
     """Stem(prec="bf16") forward(save) + backward against torch.autograd on the fp64 restatement of the fp32 model."""
     from mac_network_b200.stem import Stem, SITE_STEM, stem_specs, init_stem_params
     from tests._util import max_rel
-    from tests.test_stem import _torch_stem_grads
+    from oracle.model_torch_autograd import stem_grads
     lib = L_.load()
     B, H, W, cin, cout = shape
     pv = init_stem_params(stem_specs(cin, cout), seed=8, dtype=np.float64)
@@ -299,7 +299,7 @@ def test_stem_bf16_training_against_fp64_autograd(keep, shape):
             u = torch.empty(B * H * W * c, device="cuda")
             L_.check(lib.mac_dropout_uniform(13, SITE_STEM + layer, 4, L_.ptr(u), u.numel(), L_.stream_ptr()))
             us.append(u.cpu().numpy().astype(np.float64).reshape(B, H, W, c))
-    kb_ref, gref, dimg_ref = _torch_stem_grads(pv, images, keep, us, d_kb)
+    kb_ref, gref, dimg_ref = stem_grads("ELU", pv, images, keep, us, d_kb)
     errs = {"kb": max_rel(kb.cpu().numpy(), kb_ref), "d_images": max_rel(d_img.cpu().numpy(), dimg_ref)}
     for k in gref:
         errs[k] = max_rel(grads[k].cpu().numpy(), gref[k])
