@@ -57,6 +57,7 @@ struct TcGemmParams {
   long long split_stride;  //   its fp32 partial to outf + slice * split_stride; 0 / 1 = off
   float bias_const;        // TC_EPI_F32: added to every pre-activation (ops.linear's bias_const, mac_linear_fwd)
   int accum;               // TC_EPI_F32: outf (+)= act(...) -- the data gradients of mac_linear_bwd_tc with dx_accum
+  int promote;             // TC_EPI_F32: two-level accumulation (tc_gemm_kernel's PROMOTE form); 0 = one accumulator
 };
 
 // ------------------------------------------------------------------ wgmma PTX wrappers
@@ -162,9 +163,17 @@ __device__ __forceinline__ uint32_t pack_bf16_lo(float a, float b, uint32_t hw) 
   return pack_bf16(a - __uint_as_float(hw << 16), b - __uint_as_float(hw & 0xffff0000u));
 }
 
+// Two-level accumulation (PROMOTE): every TC_PROMOTE_KB k-blocks go into a fresh register accumulator, which the CUDA
+// cores then add into the fp32 master accumulator.  Hopper's bf16 wgmma adds its products into an accumulator with fewer
+// mantissa bits than an fp32 add: with one accumulator over the image stem's K = 9 C (9216 at C = 1024, tripled by the
+// split's three terms) the loss grows with the accumulator's magnitude, and the split-bf16 stem's output left the fp32
+// parity bar once composed with the cell.  Bounding each wgmma sum to 128 products keeps mac_linear_tc32_fwd near an fp32
+// dot product (tests/test_gpu_stem_bf16x3.py).  The group's last k-block waits for all of its MMAs before the add.
+constexpr int TC_PROMOTE_KB = 2;
+
 // SAVE (TC_EPI_ACT_SPLIT / TC_EPI_LOGITS with outf != NULL): a separate instantiation, so the inference form's kernels
-// (outf == NULL) are compiled exactly as without the fp32 store
-template <int EPI, int ACT, bool SAVE = false>
+// (outf == NULL) are compiled exactly as without the fp32 store; PROMOTE (TC_EPI_F32 only) likewise
+template <int EPI, int ACT, bool SAVE = false, bool PROMOTE = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
                const __grid_constant__ CUtensorMap map_b, const TcGemmParams p) {
@@ -219,7 +228,36 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
   float acc[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-  {
+  if constexpr (PROMOTE) {
+    float blk[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) blk[i] = 0.f;
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < kblocks; ++kb) {
+      const int kg = kb % TC_PROMOTE_KB;                    // place in the current group: 0 starts a fresh accumulator
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(tiles + stage * TC_STAGE_BYTES);
+      const uint64_t adesc = make_sw128_kmajor_desc(sa + g * (64 * 128));
+      const uint64_t bdesc = make_sw128_kmajor_desc(sa + TC_A_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k) wgmma_bf16_n128(blk, adesc + 2 * k, bdesc + 2 * k, (kg | k) ? 1u : 0u);
+      wgmma_commit();
+      if (kg == TC_PROMOTE_KB - 1 || kb == kblocks - 1) {
+        wgmma_wait<0>();                                    // the group's products have retired
+        wgmma_hold(blk);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] += blk[i];
+      } else {
+        wgmma_wait<1>();                                    // the previous k-block's products have retired
+        wgmma_hold(blk);
+      }
+      if (kb > 0 && lane == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
+    }
+  } else {
     int stage = 0, prev = 0;
     uint32_t phase = 0;
     for (int kb = 0; kb < kblocks; ++kb) {
@@ -334,10 +372,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
 // ------------------------------------------------------------------ host side
 inline int tc_num_sms() { return mac_num_sms(); }
 
-template <int EPI, int ACT, bool SAVE = false>
+template <int EPI, int ACT, bool SAVE = false, bool PROMOTE = false>
 inline int tc_gemm_launch_t(const CUtensorMap& ma0, const CUtensorMap& ma1, const CUtensorMap& mb,
                             const TcGemmParams& p, cudaStream_t stream) {
-  auto kern = tc_gemm_kernel<EPI, ACT, SAVE>;
+  auto kern = tc_gemm_kernel<EPI, ACT, SAVE, PROMOTE>;
   // the shared-memory opt-in belongs to the current device's context: set it on every launch
   MAC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
   const dim3 grid(p.N / TC_BN, (p.M + TC_BM - 1) / TC_BM, p.ksplit > 1 ? p.ksplit : 1);
@@ -348,6 +386,15 @@ inline int tc_gemm_launch_t(const CUtensorMap& ma0, const CUtensorMap& ma1, cons
 
 inline int tc_gemm_dispatch(const CUtensorMap& ma0, const CUtensorMap& ma1, const CUtensorMap& mb,
                             const TcGemmParams& p, cudaStream_t stream) {
+  if (p.promote) {
+    if (p.epi != TC_EPI_F32) return MAC_ERR_UNSUPPORTED;
+    switch (p.act) {
+      case MAC_ACT_NON: return tc_gemm_launch_t<TC_EPI_F32, MAC_ACT_NON, false, true>(ma0, ma1, mb, p, stream);
+      case MAC_ACT_ELU: return tc_gemm_launch_t<TC_EPI_F32, MAC_ACT_ELU, false, true>(ma0, ma1, mb, p, stream);
+      case MAC_ACT_RELU: return tc_gemm_launch_t<TC_EPI_F32, MAC_ACT_RELU, false, true>(ma0, ma1, mb, p, stream);
+    }
+    return MAC_ERR_UNSUPPORTED;
+  }
   switch (p.epi) {
     case TC_EPI_P: return tc_gemm_launch_t<TC_EPI_P, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
     case TC_EPI_ADDACT:

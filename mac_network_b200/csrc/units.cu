@@ -312,6 +312,7 @@ extern "C" int mac_linear_tc32_fwd(const void* a_split, const void* wt3, const f
   TcGemmParams p{};
   p.M = M; p.N = n_out; p.act = act; p.bias = b; p.ldo = n_out; p.rows_per_batch = 1;
   p.epi = TC_EPI_F32; p.outf = y;
+  p.promote = 1;            // the stem's K = 9 C: two-level accumulation keeps the long contraction at fp32 accuracy
   return tc3_gemm(a_split, K, wt3, p, reinterpret_cast<cudaStream_t>(stream_));
 }
 

@@ -155,6 +155,7 @@ class _Cell(object):
             dim = c.ctrlDim
         logits = self.linear(inter, sc + "inter2logits/", "logits", dim, 1)
         att = torch.softmax(logits + self.mask, dim=-1)
+        self.att_question = att
         new_control = (att.unsqueeze(-1) * outWords).sum(-2)
         if c.controlContinuous:
             new_control = new_cont
@@ -191,6 +192,7 @@ class _Cell(object):
                 dim += added_dim
             inter = self.act(c.readCtrlAct, inter)
         att = self.inter2att(inter, sc, dim, dropout=self.dropouts["read"])
+        self.att_kb = att
         if c.readSmryKBProj:
             knowledgeBase = projectedKB
         return (att.unsqueeze(-1) * knowledgeBase).sum(-2)
@@ -273,7 +275,9 @@ class _Cell(object):
 def graph(cfg, p, x, lengths, L, dropouts=(1.0, 1.0, 1.0), uniforms=None, train=False, trace=None):
     """The cell's L steps as a differentiable graph: `p` maps full variable names to fp64 tensors, `x` holds the fp64
     "vecQuestions", "questionWords", "questionCntxWords" and "knowledgeBase", `lengths` the question lengths (long), all on
-    one device.  Returns (control_L, memory_L) tensors; every uniform of `uniforms` must be consumed."""
+    one device.  Returns (control_L, memory_L) tensors; every uniform of `uniforms` must be consumed.  `trace`: a list that
+    receives, per step, numpy copies of the control, memory and retrieved info and of the question and knowledge-base
+    attention maps ("att_question" [B, S], "att_kb" [B, N])."""
     cell = _Cell(cfg, p, uniforms, dropouts, train, x["knowledgeBase"].device)
     control, memory = cell.zero_state(x["vecQuestions"], x["questionWords"], x["questionCntxWords"], lengths,
                                       x["knowledgeBase"])
@@ -281,7 +285,8 @@ def graph(cfg, p, x, lengths, L, dropouts=(1.0, 1.0, 1.0), uniforms=None, train=
         control, memory, info = cell.step(i, control, memory)
         if trace is not None:
             trace.append({k: v.detach().cpu().numpy() for k, v in (("control", control), ("memory", memory),
-                                                                    ("info", info))})
+                                                                    ("info", info), ("att_question", cell.att_question),
+                                                                    ("att_kb", cell.att_kb))})
     assert next(cell.uniforms, None) is None, "uniform draws left over: the dropout calls differ from the reference's"
     return control, memory
 
@@ -291,7 +296,8 @@ def run(cfg, params_np, inputs_np, L, dropouts=(1.0, 1.0, 1.0), uniforms=None, d
     """Returns (control_L, memory_L, grads) as numpy arrays, with grads keyed like the product's `mac_backward` output:
     every parameter (zeros for the stored batch-norm statistics), "knowledgeBase", the words key ("questionCntxWords" with
     controlContextual, else "questionWords") and "vecQuestions".  `train`: the cell's train argument (memoryBN only);
-    `device`: where the fp64 arithmetic runs; `trace`: a list that receives each step's control, memory and info."""
+    `device`: where the fp64 arithmetic runs; `trace`: a list that receives each step's control, memory, info and attention
+    maps (see `graph`)."""
     dev = torch.device(device)
     t64 = lambda a: torch.as_tensor(a, dtype=torch.float64).to(dev)
     p = {k: t64(v).requires_grad_("/BatchNorm/moving_" not in k) for k, v in params_np.items()}

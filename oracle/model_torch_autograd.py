@@ -77,7 +77,7 @@ def stem_grads(relu, params, images, keep, uniforms, d_kb):
     return out(kb), {k: out(v.grad) for k, v in p.items()}, out(x.grad)
 
 
-def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="cpu", grad=True):
+def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="cpu", grad=True, trace=None):
     """The training loss of one shard.
 
     `values`: every variable by its TF name (numpy or torch); `data`: "questions" [B, S] (0 = padding),
@@ -88,7 +88,12 @@ def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="c
     exactly.  `global_batch`: the loss is sum(losses) / global_batch (default B).
 
     Returns {"logits", "losses", "loss"} and, with `grad`, "grads" (every variable's gradient, zeros for the stored
-    batch-norm statistics) and "d_images" (in the layout of the images given), all fp64 tensors on `device`."""
+    batch-norm statistics) and "d_images" (in the layout of the images given), all fp64 tensors on `device`.
+
+    `trace`: a list that receives the cell's per-step control, memory, info, "att_question" and "att_kb" (numpy, see
+    `mac_torch_autograd.graph`); with it the result also holds the units' outputs the cell reads: "knowledgeBase" (the
+    stem's, one per image [k, H*W, d], before the imageIndex gather), "vecQuestions", "questionWords" and
+    "questionCntxWords".  It changes nothing else."""
     dev = torch.device(device)
     t64 = lambda a: torch.as_tensor(np.asarray(a) if isinstance(a, np.ndarray) else a).to(dev, torch.float64)
     p = {k: t64(v).requires_grad_(grad and "/BatchNorm/moving_" not in k) for k, v in values.items()}
@@ -104,18 +109,21 @@ def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="c
     B = questions.shape[0]
     words, cntx, vecq = encoder_torch_autograd.graph(p, questions, lengths, keeps["encoder"][0], keeps["encoder"][1],
                                                      its["encoder"])
-    kb = stem_graph(cfg.relu, p, x_img.permute(0, 2, 3, 1) if nchw else x_img, keeps["stem"], its["stem"])
+    kb = stem_kb = stem_graph(cfg.relu, p, x_img.permute(0, 2, 3, 1) if nchw else x_img, keeps["stem"], its["stem"])
     if data.get("imageIndex") is not None:
         kb = kb[lng(data["imageIndex"])]
     assert kb.shape[0] == B, (kb.shape, B)
     x = {"vecQuestions": vecq, "questionWords": words, "questionCntxWords": cntx, "knowledgeBase": kb}
-    _, memory = mac_torch_autograd.graph(cfg, p, x, lengths, L, keeps["cell"], its["cell"], train=True)
+    _, memory = mac_torch_autograd.graph(cfg, p, x, lengths, L, keeps["cell"], its["cell"], train=True, trace=trace)
     # the cell's vecQuestions is the encoder's output: the output unit reads the same tensor (model.py:512-528)
     logits, losses = output_graph(cfg.relu, p, memory, vecq, answers, keeps["output"], its["output"])
     for u in UNITS:
         assert next(its[u], None) is None, "%s: uniform draws left over: the dropout calls differ from the reference's" % u
     loss = losses.sum() / float(B if global_batch is None else global_batch)
     out = {"logits": logits.detach(), "losses": losses.detach(), "loss": loss.detach()}
+    if trace is not None:
+        out.update({"knowledgeBase": stem_kb.detach(), "vecQuestions": vecq.detach(), "questionWords": words.detach(),
+                    "questionCntxWords": cntx.detach()})
     if grad:
         names = [k for k, v in p.items() if v.requires_grad]
         got = torch.autograd.grad(loss, [p[k] for k in names] + [x_img], allow_unused=True)

@@ -21,21 +21,26 @@ pytestmark = pytest.mark.gpu
 
 ACT_ELU = L_.ACT["ELU"]
 # fraction of the absolute-value reference                                                        measured
-TOL_LINEAR = 1.5e-5         # mac_linear_tc32_fwd: 2.6e-6 at K = 1152, 3.9e-6 at K = 4608               4.9e-6 at K = 9216
+# mac_linear_tc32_fwd, worst over M = 49, 245, 12 544.  One fp32 wgmma accumulator over the whole K measured 2.6e-6, 3.9e-6
+# and 4.9e-6 at K = 1152, 4608 and 9216: from K = 4608 on these bars reject it.                     measured
+TOL_LINEAR = {1152: 4.5e-6,                                                                  # 1.5e-6
+              4608: 2.1e-6,                                                                  # 7.0e-7
+              9216: 1.6e-6,                                                                  # 5.3e-7
+              18432: 1.1e-6}                                                                 # 3.6e-7
 TOL_CONV = {"dkernel": 3.6e-5,      # 8.8e-6 over Mp = 12 544; over M = 49 single terms show: the dropped lo*lo product is
                                     # up to 2^-16 of a term and does not average out                1.2e-5
             "dbias": 2.5e-7,                                                                 # 8.1e-8
             "dx": 3.5e-6}           # contraction over Cout, then nine fp32 adds                    1.2e-6
 # Stem(prec="bf16x3") against the fp64 restatement: the fp32 stem's own bars (tests/test_stem.py), not looser.  Measured at
-# B=64, 14x14, 1024 -> 512 -> 512, keep 0.82: kb 5.6e-5, layer 1's kernel gradient 1.2e-4, layer 0's 7.3e-5, d_images 1.9e-5
+# B=64, 14x14, 1024 -> 512 -> 512, keep 0.82: kb 7.1e-6, layer 0's kernel gradient 7.6e-5, layer 1's 7.4e-5, d_images 6.8e-6
 BAR_FWD, BAR_GRAD = 1e-4, 2e-4
 # whole-model trainer, stem_prec="bf16x3" against "fp32" under the tc32 cell, two steps (the tc32 cell against the fp32
 # cell: 1.8e-5, DESIGN.md section 9 item 5)
 TOL_TRAINER_LOSS = 1e-5             # relative                                                      3.9e-7
 TOL_TRAINER = 1e-4                  # every gradient tensor, of its max: 3.2e-5 (a cell tensor); stem tensors 6.4e-6
 # MACnet(prec="bf16") evaluation, the bf16x3 stem against the fp32 stem (max-norm relative)
-TOL_EVAL = {"kb": 1e-4,             # the forward bar                                               5.9e-5
-            "logits": 2e-4}                                                                  # 6.3e-5
+TOL_EVAL = {"kb": 1e-4,             # the forward bar                                               6.2e-6
+            "logits": 2e-4}                                                                  # 1.3e-5
 
 
 def _mr(a, b):
@@ -63,10 +68,11 @@ def test_im2col3x3_split_equals_the_host_split_bit_for_bit(shape, keep):
 
 
 # ------------------------------------------------------------------------------------------------ mac_linear_tc32_fwd
-@pytest.mark.parametrize("K", [1152, 4608, 9216])
+@pytest.mark.parametrize("K", [1152, 4608, 9216, 18432])
 @pytest.mark.parametrize("M", [49, 245, 12544])
 def test_linear_tc32_fwd_against_fp64(M, K):
-    """y = ELU(A W + b) from [A_hi | A_lo] and [W_hi | W_hi | W_lo]: the whole K in one fp32 wgmma accumulator."""
+    """y = ELU(A W + b) from [A_hi | A_lo] and [W_hi | W_hi | W_lo], two-level accumulation (tc_gemm_kernel's PROMOTE
+    form), up to the stem's K = 9 C at C = 1024 and 2048."""
     lib = L_.load()
     N = 256
     g = torch.Generator(device="cuda").manual_seed(M + K)
@@ -89,7 +95,7 @@ def test_linear_tc32_fwd_against_fp64(M, K):
     # ELU is 1-Lipschitz: the pre-activation's bound carries over; 2e-7 for the epilogue's fp32 exponential
     e = excess(ys[0], torch.where(pre > 0, pre, torch.expm1(pre)), absref, tiny=2e-7)
     print("mac_linear_tc32_fwd M=%d K=%d: %.2e of the absolute-value product" % (M, K, e))
-    assert e <= TOL_LINEAR, e
+    assert e <= TOL_LINEAR[K], e
 
 
 # ------------------------------------------------------------------------------------------------ mac_conv3x3_bwd_tc32

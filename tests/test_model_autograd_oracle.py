@@ -242,3 +242,33 @@ def test_gradient_against_central_differences(flags, nchw, indexed):
     print("%s: %d tensors, worst %s" % (flags, len(worst), ["%s %.1e" % kv for kv in top]))
     bad = {n: e for n, e in worst.items() if not e < 1e-6}
     assert not bad, bad
+
+
+@pytest.mark.parametrize("flags", ["gqa", "p2_memory_bn_train"])
+def test_trace_changes_neither_the_forward_nor_the_gradients(flags):
+    """`trace=` records each step's state and attention maps and returns the tensors the cell reads, and nothing it
+    computes moves: the logits, losses, every gradient and the image gradient equal the untraced run's bit for bit, with
+    the training dropouts and k < B images.  The traced attention maps are distributions, exactly 0 beyond each length."""
+    cfg, cell_dp = model_config(flags, 8, L)
+    values = model_values(cfg, L, V, E, C, A, HIDDEN, seed=13)
+    keeps = training_keeps(cell_dp)
+    index = np.array([1, 0, 2, 1, 1])
+    data = make_data(B, S, V, 3, H, W, C, A, seed=14, index=index)
+    us = random_uniforms(dropout_plan(cfg, L, values, keeps, B, S, 3, H, W, step=0), seed=15)
+    want = MA.run(cfg, L, values, data, keeps, us)
+    trace = []
+    got = MA.run(cfg, L, values, data, keeps, us, trace=trace)
+    for k in ("logits", "losses", "loss", "d_images"):
+        assert torch.equal(got[k], want[k]), k
+    assert set(got["grads"]) == set(want["grads"])
+    for n, g in want["grads"].items():
+        assert torch.equal(got["grads"][n], g), n
+    assert set(want) == {"logits", "losses", "loss", "grads", "d_images"}
+    assert tuple(got["knowledgeBase"].shape) == (3, H * W, 8) and tuple(got["vecQuestions"].shape) == (B, 8)
+    assert tuple(got["questionWords"].shape) == tuple(got["questionCntxWords"].shape) == (B, S, 8)
+    assert len(trace) == L
+    for step in trace:
+        assert set(step) == {"control", "memory", "info", "att_question", "att_kb"}
+        assert step["att_question"].shape == (B, S) and step["att_kb"].shape == (B, H * W)
+        assert np.abs(step["att_question"].sum(1) - 1).max() < 1e-12 and np.abs(step["att_kb"].sum(1) - 1).max() < 1e-12
+        assert not step["att_question"][np.arange(S)[None, :] >= data["questionLengths"][:, None]].any()
