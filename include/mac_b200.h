@@ -167,6 +167,13 @@ size_t mac_read_workspace_bytes(int B, int N, int d, int prec);
 size_t mac_read_invariant_bytes(int B, int N, int d, int prec);
 int mac_read_invariant(const float* kb, const void* kb_bf16, const mac_read_weights* w, int prec, void* inv,
                        size_t inv_bytes, int B, int N, int d, mac_stream_t stream);
+/* mac_read_invariant's MAC_PREC_BF16 / MAC_PREC_FP8 result from the fp32 knowledge base kb [B*N, d], which it also casts
+ * into kb_bf16 (written: round-to-nearest-even, the bits of mac_cast_bf16).  One launch (csrc/read_inv.cuh) where a cast
+ * followed by mac_read_invariant(kb_bf16) takes two; P, Q, P8, sP and kb_bf16 are bit-identical to that pair.  At d = 512
+ * mac_read_invariant runs the same kernel on kb_bf16.  Needs d == 512 (else MAC_ERR_UNSUPPORTED), kb and kb_bf16
+ * (MAC_ERR_INVALID), and otherwise refuses what mac_read_invariant(kb, kb_bf16, ...) refuses, before any launch. */
+int mac_read_invariant_cast(const float* kb, void* kb_bf16, const mac_read_weights* w, int prec, void* inv,
+                            size_t inv_bytes, int B, int N, int d, mac_stream_t stream);
 int mac_read_fwd_inv(const float* kb, const void* kb_bf16, const void* inv, const float* y_pre,
                      const float* memory_in, const float* control, const mac_read_weights* w, int prec,
                      float* info, float* att, void* workspace, size_t workspace_bytes, int B, int N, int d,

@@ -49,6 +49,8 @@ PROTOTYPES = {
     "mac_read_invariant_bytes": (c_sz, [c_int, c_int, c_int, c_int]),
     "mac_read_invariant": (c_int, [c_fp, c_fp, ctypes.POINTER(ReadWeights), c_int, c_fp, c_sz, c_int, c_int, c_int,
                                    c_fp]),
+    "mac_read_invariant_cast": (c_int, [c_fp, c_fp, ctypes.POINTER(ReadWeights), c_int, c_fp, c_sz, c_int, c_int,
+                                        c_int, c_fp]),
     "mac_read_fwd_inv": (c_int, [c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, ctypes.POINTER(ReadWeights), c_int, c_fp, c_fp,
                                  c_fp, c_sz, c_int, c_int, c_int, c_fp]),
     "mac_read_step_fused": (c_int, [c_fp, c_fp, c_fp, c_fp, ctypes.POINTER(ReadWeights), c_fp, c_fp, c_int, c_int, c_int,

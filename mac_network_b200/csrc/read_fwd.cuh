@@ -1,5 +1,6 @@
 // The read unit's forward (mac_cell.py:209-277, see mac_read_fwd in mac_b200.h) in each of its forms, and the C entry points
-// that pick one: mac_read_fwd, mac_read_fwd_inv, mac_read_invariant, mac_read_step_fused and their size queries.
+// that pick one: mac_read_fwd, mac_read_fwd_inv, mac_read_invariant (and mac_read_invariant_cast), mac_read_step_fused and
+// their size queries.
 //
 //   FP32_TRAIN, BF16_TRAIN, TC32_TRAIN   mac_read_fwd with MAC_PREC_FP32 / BF16 / TC32: P, H, I1 + logits on the FMA pipe,
 //                                        on tc_gemm, or as split-bf16 products (tc3_gemm)
@@ -410,9 +411,12 @@ static int read_fp32_invariant(const float* kb, const mac_read_weights* w, const
   return sgemm_launch(p, nullptr, nullptr, 0, stream, false);
 }
 
-// P and Q in bf16 (MAC_PREC_BF16, and the P and Q that MAC_PREC_FP8 quantises)
-static int read_bf16_invariant(const void* kb_bf16, const mac_read_weights* w, const ReadInv& I, int B, int N, int d,
-                               cudaStream_t stream) {
+// P and Q in bf16 (MAC_PREC_BF16, and the P and Q that MAC_PREC_FP8 quantises).  At d = RS_D one read_invariant_kernel
+// launch (csrc/read_inv.cuh); there kb (fp32) may be given instead, and kb_bf16 is then written as its bf16 cast.  Other
+// widths: two tc_gemm launches from kb_bf16.
+static int read_bf16_invariant(const float* kb, const void* kb_bf16, const mac_read_weights* w, const ReadInv& I, int B,
+                               int N, int d, cudaStream_t stream) {
+  if (d == RS_D) return read_invariant_launch(kb, const_cast<void*>(kb_bf16), w, I.P, I.Q, B * N, stream);
   TcGemmParams p{};
   p.M = B * N; p.N = d; p.rows_per_batch = N; p.ldo = d;
   p.epi = TC_EPI_ACT; p.act = MAC_ACT_NON; p.bias = w->bx; p.out0 = (__nv_bfloat16*)I.P;
@@ -439,9 +443,9 @@ static int read_tc32_invariant(const float* kb, const mac_read_weights* w, const
 }
 
 // P and Q exactly as read_bf16_invariant computes them, then P8 and sP from P
-static int read_fp8_invariant(const void* kb_bf16, const mac_read_weights* w, const ReadInv& I, int B, int N, int d,
-                              cudaStream_t stream) {
-  const int st = read_bf16_invariant(kb_bf16, w, I, B, N, d, stream);
+static int read_fp8_invariant(const float* kb, const void* kb_bf16, const mac_read_weights* w, const ReadInv& I, int B,
+                              int N, int d, cudaStream_t stream) {
+  const int st = read_bf16_invariant(kb, kb_bf16, w, I, B, N, d, stream);
   if (st != MAC_OK) return st;
   const int M = B * N;
   quant_rows_e4m3_kernel<<<(M + 7) / 8, 256, 0, stream>>>((const __nv_bfloat16*)I.P, I.P8, I.sP, M);
@@ -593,11 +597,25 @@ extern "C" int mac_read_invariant(const float* kb, const void* kb_bf16, const ma
   if (st != MAC_OK) return st;
   const ReadInv I = read_inv_layout(prec, inv, B, N, d);
   switch (f) {
-    case RF_BF16_STEP: case RF_BF16_INV: return read_bf16_invariant(kb_bf16, w, I, B, N, d, stream);
+    case RF_BF16_STEP: case RF_BF16_INV: return read_bf16_invariant(nullptr, kb_bf16, w, I, B, N, d, stream);
     case RF_TC32_INV: return read_tc32_invariant(kb, w, I, B, N, d, stream);
-    case RF_FP8_STEP: return read_fp8_invariant(kb_bf16, w, I, B, N, d, stream);
+    case RF_FP8_STEP: return read_fp8_invariant(nullptr, kb_bf16, w, I, B, N, d, stream);
     default: return read_fp32_invariant(kb, w, I, B, N, d, stream);
   }
+}
+
+extern "C" int mac_read_invariant_cast(const float* kb, void* kb_bf16, const mac_read_weights* w, int prec, void* inv,
+                                       size_t inv_bytes, int B, int N, int d, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (prec != MAC_PREC_BF16 && prec != MAC_PREC_FP8) return MAC_ERR_UNSUPPORTED;
+  if (!kb || !kb_bf16) return MAC_ERR_INVALID;
+  const ReadForm f = read_form(prec, true, true, read_step_supported(B, N, d));
+  const int st = read_inv_check(f, kb, kb_bf16, w, prec, inv, inv_bytes, B, N, d);
+  if (st != MAC_OK) return st;
+  if (d != RS_D) return MAC_ERR_UNSUPPORTED;
+  const ReadInv I = read_inv_layout(prec, inv, B, N, d);
+  return f == RF_FP8_STEP ? read_fp8_invariant(kb, kb_bf16, w, I, B, N, d, stream)
+                          : read_bf16_invariant(kb, kb_bf16, w, I, B, N, d, stream);
 }
 
 extern "C" int mac_read_fwd(const float* kb, const void* kb_bf16, const float* memory_in, const float* control,

@@ -4,6 +4,7 @@
 #include "skinny.cuh"
 #include "tc_gemm.cuh"
 #include "read_step.cuh"
+#include "read_inv.cuh"
 #include "read_step_fp8.cuh"
 #include "tc_gemm_fp8.cuh"
 #include "skinny_tc.cuh"
