@@ -573,6 +573,41 @@ int mac_conv3x3_bwd_tc32(const float* x, const float* y, const float* dy, const 
                          int site, int step, float* dkernel, float* dbias, float* dx, void* workspace, size_t workspace_bytes,
                          int B, int H, int W, int C, int Cout, mac_stream_t stream);
 size_t mac_conv3x3_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx);
+/* Stem layers of any kernel size k and stride s (--stemKernelSize(s), --stemStrideSizes, --stemLinear as k = s = 1), with
+ * tf.nn.conv2d's SAME padding: Ho = ceil(H / s), pad_total = max((Ho - 1) s + k - H, 0), pad_top = pad_total / 2 (the odd
+ * row on the bottom); the same for the width.  Output pixel m = (b, ho, wo), M = B*Ho*Wo, reads input pixel
+ * (b, ho s - pad_top + kh, wo s - pad_left + kw) for tap kh k + kw; the GEMM weight is the HWIO kernel viewed as [k^2 C, Cout].
+ * The keep-mask is mac_im2col3x3's, one philox4x32_10(seed, e >> 2, site, step) per channel quad of the SOURCE element's NHWC
+ * flat index e: every copy of a pixel shares one draw, and a pixel no tap reads is never drawn.  keep in (0, 1].
+ * mac_im2col: cols [M, k^2 C], tap-major, channel fastest: fp32 (MAC_COLS_F32), bf16 (MAC_COLS_BF16) or [hi | lo] bf16
+ *   [M, 2 k^2 C] (MAC_COLS_SPLIT); zero for taps outside the image.  At k = 3, s = 1 bit for bit mac_im2col3x3 /
+ *   mac_im2col3x3_split.  C % 4 == 0 (C % 64 == 0 for MAC_COLS_SPLIT).
+ * mac_col2im: dx [B,H,W,C] = keep-mask/keep * the sum over taps in ascending order of the dcols [M, k^2 C] entries that read
+ *   each pixel (gather per input pixel, no atomics: reruns are bit-identical).  C % 4 == 0.
+ * mac_im2col_t: the bf16 patch matrix transposed, colsT [k^2 C, Mp] (split = 0) or [k^2 C, 2 Mp] = [hi | lo] (split = 1),
+ *   Mp = M rounded up to 64; columns M..Mp-1 are written as zeros on every call.  C % 64 == 0.
+ * mac_conv_bwd_tc / _tc32: mac_conv3x3_bwd_tc / _tc32 for any k and s (x [B,H,W,C], y and dy [M, Cout], dkernel
+ *   [k,k,C,Cout]); k = 3, s = 1 runs exactly what mac_conv3x3_bwd_tc / _tc32 run.  Their own workspace queries (0 for a
+ *   refused geometry).
+ * Every entry point: a null pointer, a size, k or s <= 0, keep outside (0, 1] or more than 2^30 input or output pixels ->
+ * MAC_ERR_INVALID; k or s > 16, the channel rules above, k^2 C / 64 > 65535 (mac_im2col_t, mac_conv_bwd_tc / _tc32: one
+ * launch row per 64 patch columns) or an unknown form -> MAC_ERR_UNSUPPORTED; pointers not 16-byte
+ * aligned -> MAC_ERR_ALIGN.  All checks precede any launch. */
+enum { MAC_COLS_F32 = 0, MAC_COLS_BF16 = 1, MAC_COLS_SPLIT = 2 };
+int mac_im2col(const float* x, void* cols, int form, float keep, uint64_t seed, int site, int step, int B, int H, int W, int C,
+               int k, int s, mac_stream_t stream);
+int mac_col2im(const float* dcols, float* dx, float keep, uint64_t seed, int site, int step, int B, int H, int W, int C, int k,
+               int s, mac_stream_t stream);
+int mac_im2col_t(const float* x, void* colsT, int split, float keep, uint64_t seed, int site, int step, int B, int H, int W,
+                 int C, int k, int s, mac_stream_t stream);
+int mac_conv_bwd_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep, uint64_t seed,
+                    int site, int step, float* dkernel, float* dbias, float* dx, void* workspace, size_t workspace_bytes, int B,
+                    int H, int W, int C, int Cout, int k, int s, mac_stream_t stream);
+size_t mac_conv_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int k, int s, int with_dx);
+int mac_conv_bwd_tc32(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep, uint64_t seed,
+                      int site, int step, float* dkernel, float* dbias, float* dx, void* workspace, size_t workspace_bytes,
+                      int B, int H, int W, int C, int Cout, int k, int s, mac_stream_t stream);
+size_t mac_conv_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int k, int s, int with_dx);
 
 /* ------------------------------------------------------------------------------------------------
  * Question input unit ("next" row, model.py:208-220, 279-307; ops.py:859-905): embedding lookup + bi-LSTM encoder.

@@ -140,6 +140,15 @@ PROTOTYPES = {
     "mac_conv3x3_bwd_tc32": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_fp, c_fp, c_sz,
                                      c_int, c_int, c_int, c_int, c_int, c_fp]),
     "mac_conv3x3_bwd_tc32_workspace_bytes": (c_sz, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "mac_im2col": (c_int, [c_fp, c_fp, c_int, c_f, c_u64] + [c_int] * 8 + [c_fp]),
+    "mac_col2im": (c_int, [c_fp, c_fp, c_f, c_u64] + [c_int] * 8 + [c_fp]),
+    "mac_im2col_t": (c_int, [c_fp, c_fp, c_int, c_f, c_u64] + [c_int] * 8 + [c_fp]),
+    "mac_conv_bwd_tc": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_fp, c_fp, c_sz]
+                        + [c_int] * 7 + [c_fp]),
+    "mac_conv_bwd_tc_workspace_bytes": (c_sz, [c_int] * 8),
+    "mac_conv_bwd_tc32": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_fp, c_fp, c_sz]
+                          + [c_int] * 7 + [c_fp]),
+    "mac_conv_bwd_tc32_workspace_bytes": (c_sz, [c_int] * 8),
     "mac_pack_weight_bf16": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_split3": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_fp8": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_fp]),

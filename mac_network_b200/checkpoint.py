@@ -148,8 +148,14 @@ def attention_maps(cell, image_dims=None):
     return out
 
 
-def write_preds(path, cell, predictions=None, image_dims=(14, 14)):
-    """One JSON record per sample with its per-step attention maps (`model.py:693-710`, `preprocess.py:263-272`)."""
+def write_preds(path, cell, predictions=None, image_dims=None):
+    """One JSON record per sample with its per-step attention maps (`model.py:693-710`, `preprocess.py:263-272`).
+    `image_dims`: the knowledge base's grid (`Stem.grid(H, W)`) the `kb` maps are reshaped to; None takes the reference's
+    14 x 14 (`visualization.py:121`) for a 196-cell knowledge base and leaves any other flat."""
+    if image_dims is None:
+        image_dims = (14, 14) if cell.N == 196 else None
+    elif int(image_dims[0]) * int(image_dims[1]) != cell.N:
+        raise ValueError("image_dims %s do not hold the %d knowledge-base cells" % (tuple(image_dims), cell.N))
     att = attention_maps(cell, image_dims)
     B = cell.B
     recs = []

@@ -886,6 +886,169 @@ extern "C" int mac_col2im3x3(const float* dcols, float* dx, float keep, uint64_t
   return MAC_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ stem: any k x k, stride s
+// tf.nn.conv2d's SAME geometry (ops.py:397): Ho = ceil(H / s), pad_total = max((Ho - 1) s + k - H, 0), pad_top =
+// pad_total / 2 (the odd row goes to the bottom), and the same for the width.  Output pixel (ho, wo) reads input
+// (ho s - pad_top + kh, wo s - pad_left + kw) for tap kh k + kw.  At k = 3, s = 1 this is the 3x3 kernels' geometry; those
+// stay (they are fused with the NCHW ingest), and these serve every other layer.
+namespace mac {
+struct ConvGeom {
+  int B, H, W, C, k, s, Ho, Wo, pt, pl;
+};
+inline ConvGeom conv_geom(int B, int H, int W, int C, int k, int s) {
+  ConvGeom g{B, H, W, C, k, s, (H + s - 1) / s, (W + s - 1) / s, 0, 0};
+  g.pt = std::max((g.Ho - 1) * s + k - H, 0) / 2;
+  g.pl = std::max((g.Wo - 1) * s + k - W, 0) / 2;
+  return g;
+}
+constexpr int CONV_MAX_K = 16, CONV_MAX_S = 16;
+
+// The refusals every general stem entry point shares, before any launch: sizes, k, s, keep, and the 2^30-row bound.
+inline int conv_geom_check(int B, int H, int W, int C, int k, int s, float keep) {
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || k <= 0 || s <= 0 || !(keep > 0.f && keep <= 1.f)) return MAC_ERR_INVALID;
+  if (k > CONV_MAX_K || s > CONV_MAX_S) return MAC_ERR_UNSUPPORTED;
+  const ConvGeom g = conv_geom(B, H, W, C, k, s);
+  if ((long long)B * H * W > (1LL << 30) || (long long)B * g.Ho * g.Wo > (1LL << 30)) return MAC_ERR_INVALID;
+  return MAC_OK;
+}
+
+__device__ __forceinline__ void dropout_quad(float4& v, uint64_t seed, long long e, int site, int step, uint32_t thresh,
+                                             float scale) {
+  const Philox4 p = philox4x32_10(seed, (uint64_t)e >> 2, (uint32_t)site, (uint32_t)step);
+  v.x = ((p.x >> 8) >= thresh) ? v.x * scale : 0.f;
+  v.y = ((p.y >> 8) >= thresh) ? v.y * scale : 0.f;
+  v.z = ((p.z >> 8) >= thresh) ? v.z * scale : 0.f;
+  v.w = ((p.w >> 8) >= thresh) ? v.w * scale : 0.f;
+}
+
+// cols[m, tap C + c] (FORM fp32 / bf16) or cols[m, [hi | lo]] (FORM split, each k^2 C wide) of the dropped-out input; the
+// Philox draw is the SOURCE element's quad, so every copy of a pixel shares its mask and a pixel no tap reads is never drawn.
+// V channels per thread: one 16-byte store per thread and half (V = 4 fp32, V = 8 bf16 and split; V = 4 bf16 when C % 8).
+template <int V, int FORM>
+__global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ x, void* __restrict__ cols_, uint32_t thresh,
+                                                     float scale, uint64_t seed, int site, int step, ConvGeom g) {
+  const int cvn = g.C / V, taps = g.k * g.k;
+  const long long total = (long long)g.B * g.Ho * g.Wo * taps * cvn;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int cv = (int)(i % cvn);
+  long long r = i / cvn;
+  const int tap = (int)(r % taps);
+  const long long m = r / taps;
+  const int wo = (int)(m % g.Wo);
+  r = m / g.Wo;
+  const int ho = (int)(r % g.Ho), b = (int)(r / g.Ho);
+  const int hs = ho * g.s - g.pt + tap / g.k, wsrc = wo * g.s - g.pl + tap % g.k;
+  float4 v[V / 4];
+#pragma unroll
+  for (int q = 0; q < V / 4; ++q) v[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (hs >= 0 && hs < g.H && wsrc >= 0 && wsrc < g.W) {
+    const long long e = (((long long)b * g.H + hs) * g.W + wsrc) * g.C + cv * V;
+#pragma unroll
+    for (int q = 0; q < V / 4; ++q) {
+      v[q] = __ldg(reinterpret_cast<const float4*>(x + e) + q);
+      if (thresh) dropout_quad(v[q], seed, e + 4 * q, site, step, thresh, scale);
+    }
+  }
+  const long long K = (long long)taps * g.C;
+  if constexpr (FORM == 0) {
+    *reinterpret_cast<float4*>(reinterpret_cast<float*>(cols_) + m * K + (long long)tap * g.C + cv * V) = v[0];
+  } else if constexpr (FORM == 1) {
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(cols_) + m * K + (long long)tap * g.C + cv * V;
+    if constexpr (V == 8) {
+      *reinterpret_cast<uint4*>(o) = make_uint4(pack_bf16(v[0].x, v[0].y), pack_bf16(v[0].z, v[0].w),
+                                                pack_bf16(v[1].x, v[1].y), pack_bf16(v[1].z, v[1].w));
+    } else {
+      *reinterpret_cast<uint2*>(o) = make_uint2(pack_bf16(v[0].x, v[0].y), pack_bf16(v[0].z, v[0].w));
+    }
+  } else {
+    uint4 hi, lo;
+    hi.x = pack_bf16(v[0].x, v[0].y); hi.y = pack_bf16(v[0].z, v[0].w);
+    hi.z = pack_bf16(v[1].x, v[1].y); hi.w = pack_bf16(v[1].z, v[1].w);
+    lo.x = pack_bf16_lo(v[0].x, v[0].y, hi.x); lo.y = pack_bf16_lo(v[0].z, v[0].w, hi.y);
+    lo.z = pack_bf16_lo(v[1].x, v[1].y, hi.z); lo.w = pack_bf16_lo(v[1].z, v[1].w, hi.w);
+    __nv_bfloat16* row = reinterpret_cast<__nv_bfloat16*>(cols_) + m * 2 * K + (long long)tap * g.C + cv * V;
+    *reinterpret_cast<uint4*>(row) = hi;
+    *reinterpret_cast<uint4*>(row + K) = lo;
+  }
+}
+
+// dx[b,h,w,c] = keep-mask/keep * sum over taps (kh, kw) ascending of dcols[(b, ho, wo), tap C + c] for every output pixel
+// (ho, wo) whose tap read (h, w).  Gather per input pixel in a fixed order: deterministic, no atomics.
+__global__ void __launch_bounds__(256) col2im_kernel(const float* __restrict__ dcols, float* __restrict__ dx, uint32_t thresh,
+                                                     float scale, uint64_t seed, int site, int step, ConvGeom g) {
+  const int c4n = g.C / 4;
+  const long long total = (long long)g.B * g.H * g.W * c4n;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int c4 = (int)(i % c4n);
+  long long r = i / c4n;
+  const int w = (int)(r % g.W);
+  r /= g.W;
+  const int h = (int)(r % g.H), b = (int)(r / g.H);
+  const long long K = (long long)g.k * g.k * g.C;
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int kh = 0; kh < g.k; ++kh) {
+    const int th = h + g.pt - kh;                               // = ho * s for the output row that read (h, w) with this kh
+    if (th < 0 || th % g.s || th / g.s >= g.Ho) continue;
+    for (int kw = 0; kw < g.k; ++kw) {
+      const int tw = w + g.pl - kw;
+      if (tw < 0 || tw % g.s || tw / g.s >= g.Wo) continue;
+      const long long o = (((long long)b * g.Ho + th / g.s) * g.Wo + tw / g.s) * K + (long long)(kh * g.k + kw) * g.C + c4 * 4;
+      const float4 v = __ldg(reinterpret_cast<const float4*>(dcols + o));
+      acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+    }
+  }
+  const long long e = (((long long)b * g.H + h) * g.W + w) * g.C + c4 * 4;
+  if (thresh) dropout_quad(acc, seed, e, site, step, thresh, scale);
+  *reinterpret_cast<float4*>(dx + e) = acc;
+}
+}  // namespace mac
+
+extern "C" int mac_im2col(const float* x, void* cols, int form, float keep, uint64_t seed, int site, int step, int B, int H,
+                          int W, int C, int k, int s, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x || !cols) return MAC_ERR_INVALID;
+  const int st = conv_geom_check(B, H, W, C, k, s, keep);
+  if (st != MAC_OK) return st;
+  if (form != MAC_COLS_F32 && form != MAC_COLS_BF16 && form != MAC_COLS_SPLIT) return MAC_ERR_UNSUPPORTED;
+  if (C % 4 || (form == MAC_COLS_SPLIT && C % TC_BK)) return MAC_ERR_UNSUPPORTED;   // float4 reads; split: whole k-blocks
+  if (!mac_aligned16(x) || !mac_aligned16(cols)) return MAC_ERR_ALIGN;
+  const ConvGeom g = conv_geom(B, H, W, C, k, s);
+  const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
+  const float scale = keep < 1.f ? 1.f / keep : 1.f;
+  const int V = form == MAC_COLS_F32 || (form == MAC_COLS_BF16 && C % 8) ? 4 : 8;
+  const long long total = (long long)B * g.Ho * g.Wo * k * k * (C / V);
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  if (form == MAC_COLS_F32)
+    im2col_kernel<4, 0><<<grid, 256, 0, stream>>>(x, cols, thr, scale, seed, site, step, g);
+  else if (form == MAC_COLS_SPLIT)
+    im2col_kernel<8, 2><<<grid, 256, 0, stream>>>(x, cols, thr, scale, seed, site, step, g);
+  else if (V == 8)
+    im2col_kernel<8, 1><<<grid, 256, 0, stream>>>(x, cols, thr, scale, seed, site, step, g);
+  else
+    im2col_kernel<4, 1><<<grid, 256, 0, stream>>>(x, cols, thr, scale, seed, site, step, g);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+extern "C" int mac_col2im(const float* dcols, float* dx, float keep, uint64_t seed, int site, int step, int B, int H, int W,
+                          int C, int k, int s, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!dcols || !dx) return MAC_ERR_INVALID;
+  const int st = conv_geom_check(B, H, W, C, k, s, keep);
+  if (st != MAC_OK) return st;
+  if (C % 4) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(dcols) || !mac_aligned16(dx)) return MAC_ERR_ALIGN;
+  const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
+  const float scale = keep < 1.f ? 1.f / keep : 1.f;
+  const long long total = (long long)B * H * W * (C / 4);
+  col2im_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(dcols, dx, thr, scale, seed, site, step,
+                                                                      conv_geom(B, H, W, C, k, s));
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ stem: backward on wgmma
 // One 3x3 convolution layer's backward with its two GEMMs on tensor cores (fp32 accumulation, fp32 element-wise work),
 // M = B*H*W rows, Mp = M rounded up to the 64-row k-block of the weight gradient.  mac_conv3x3_bwd_tc (bf16 operands):
@@ -1006,14 +1169,63 @@ __global__ void __launch_bounds__(256) im2col3x3_t_kernel(const float* __restric
   }
 }
 
+// im2col3x3_t_kernel for any ConvGeom: colsT[tap C + c, m] = bf16(dropout(x))[the pixel output m's tap reads, c], zero
+// outside the image and for m >= M (the padding columns are written on every call).  C % 64 == 0.
+template <bool SPLIT>
+__global__ void __launch_bounds__(256) im2col_t_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ colsT,
+                                                       uint32_t thresh, float scale, uint64_t seed, int site, int step,
+                                                       ConvGeom g, int Mp) {
+  __shared__ float tile[64][65];                              // [channel][pixel]
+  const int k0 = blockIdx.y * 64, m0 = blockIdx.x * 64;
+  const int tap = k0 / g.C, c0 = k0 - tap * g.C;
+  const int dh = tap / g.k - g.pt, dw = tap % g.k - g.pl;
+  const int M = g.B * g.Ho * g.Wo;
+  const int tq = threadIdx.x & 15, tr = threadIdx.x >> 4;     // 16 channel quads x 16 pixels per pass
+#pragma unroll
+  for (int p = 0; p < 4; ++p) {
+    const int mm = tr + 16 * p, m = m0 + mm;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (m < M) {
+      const int wo = m % g.Wo, r = m / g.Wo;
+      const int ho = r % g.Ho, b = r / g.Ho;
+      const int hs = ho * g.s + dh, wsrc = wo * g.s + dw;
+      if (hs >= 0 && hs < g.H && wsrc >= 0 && wsrc < g.W) {
+        const long long e = (((long long)b * g.H + hs) * g.W + wsrc) * g.C + c0 + tq * 4;
+        v = __ldg(reinterpret_cast<const float4*>(x + e));
+        if (thresh) dropout_quad(v, seed, e, site, step, thresh, scale);
+      }
+    }
+    tile[tq * 4 + 0][mm] = v.x;
+    tile[tq * 4 + 1][mm] = v.y;
+    tile[tq * 4 + 2][mm] = v.z;
+    tile[tq * 4 + 3][mm] = v.w;
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int r = warp; r < 64; r += 8) {
+    const float a = tile[r][2 * lane], b = tile[r][2 * lane + 1];
+    const uint32_t hw = pack_bf16(a, b);
+    if constexpr (!SPLIT) {
+      *reinterpret_cast<uint32_t*>(colsT + (size_t)(k0 + r) * Mp + m0 + 2 * lane) = hw;
+    } else {
+      __nv_bfloat16* row = colsT + (size_t)(k0 + r) * 2 * Mp + m0 + 2 * lane;
+      *reinterpret_cast<uint32_t*>(row) = hw;
+      *reinterpret_cast<uint32_t*>(row + Mp) = pack_bf16_lo(a, b, hw);
+    }
+  }
+}
+
+// im2col_t_kernel's launch: one 64-row tile (within one tap: C % 64 == 0) per gridDim.y index, at most 65535 of them
+inline bool im2col_t_grid_ok(int k, int C) { return (long long)k * k * C / 64 <= 65535; }
+
 // workspace of mac_conv3x3_bwd_tc / _tc32: 1 KB-aligned slabs behind a 1 KB alignment slack.  `split`: the bf16 operands
 // carry 2 (dz rows, colsT) or 3 (dzT, kernel) segments, and the weight gradient contracts over 3 Mp.
 struct ConvBwdLayout {
   size_t dz, dzT, colsT, bpart, wpart, k16, dcols, total;
 };
-inline ConvBwdLayout conv_bwd_layout(int B, int H, int W, int C, int Cout, bool with_dx, bool split) {
+inline ConvBwdLayout conv_bwd_layout(const ConvGeom& g, int Cout, bool with_dx, bool split) {
   auto al = [](size_t v) { return (v + 1023) & ~(size_t)1023; };
-  const size_t M = (size_t)B * H * W, Mp = (M + 63) & ~(size_t)63, K = (size_t)9 * C;
+  const size_t M = (size_t)g.B * g.Ho * g.Wo, Mp = (M + 63) & ~(size_t)63, K = (size_t)g.k * g.k * g.C;
   const size_t s2 = split ? 2 : 1, s3 = split ? 3 : 1;
   // the split-K partials for the slice count the weight gradient will use on this device (tc_wgrad_splitk / tc3_wgrad_splitk)
   const int S = tc_pick_ksplit((int)(s3 * Mp), (int)(K / TC_BM) * (Cout / TC_BN));
@@ -1033,21 +1245,26 @@ inline ConvBwdLayout conv_bwd_layout(int B, int H, int W, int C, int Cout, bool 
   return l;
 }
 
-static int conv3x3_bwd_wgmma(bool split, const float* x, const float* y, const float* dy, const float* kernel, int act,
-                             float keep, uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
-                      size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
+// k = 3, s = 1 runs the 3x3 kernels (im2col3x3_t_kernel, mac_col2im3x3), every other geometry the general ones.
+static int conv_bwd_wgmma(bool split, const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                          uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
+                          size_t workspace_bytes, int B, int H, int W, int C, int Cout, int k, int s, mac_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x || !y || !dy || !kernel || !dkernel || !dbias || !workspace) return MAC_ERR_INVALID;
-  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0 || !(keep > 0.f && keep <= 1.f)) return MAC_ERR_INVALID;
-  if ((long long)B * H * W > (1LL << 30)) return MAC_ERR_INVALID;
-  if ((C % 128) || (Cout % 128)) return MAC_ERR_UNSUPPORTED;     // wgmma tiles: 9C and Cout are GEMM N / M extents
+  if (Cout <= 0) return MAC_ERR_INVALID;
+  const int gst = conv_geom_check(B, H, W, C, k, s, keep);
+  if (gst != MAC_OK) return gst;
+  if ((C % 128) || (Cout % 128)) return MAC_ERR_UNSUPPORTED;     // wgmma tiles: k^2 C and Cout are GEMM N / M extents
+  if (!im2col_t_grid_ok(k, C)) return MAC_ERR_UNSUPPORTED;
   if (!mac_aligned16(x) || !mac_aligned16(y) || !mac_aligned16(dy) || !mac_aligned16(kernel) || !mac_aligned16(dkernel) ||
       (dx && !mac_aligned16(dx)))
     return MAC_ERR_ALIGN;
-  const ConvBwdLayout l = conv_bwd_layout(B, H, W, C, Cout, dx != nullptr, split);
+  const ConvGeom g = conv_geom(B, H, W, C, k, s);
+  const bool k3s1 = k == 3 && s == 1;
+  const ConvBwdLayout l = conv_bwd_layout(g, Cout, dx != nullptr, split);
   if (workspace_bytes < l.total) return MAC_ERR_WORKSPACE;
   if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
-  const int M = B * H * W, Mp = (M + 63) & ~63, K = 9 * C;
+  const int M = B * g.Ho * g.Wo, Mp = (M + 63) & ~63, K = k * k * C;
   char* base = tc_align1k(workspace);
   __nv_bfloat16* dz = reinterpret_cast<__nv_bfloat16*>(base + l.dz);
   __nv_bfloat16* dzT = reinterpret_cast<__nv_bfloat16*>(base + l.dzT);
@@ -1060,11 +1277,17 @@ static int conv3x3_bwd_wgmma(bool split, const float* x, const float* y, const f
   if (split) {
     conv_dz_pack_kernel<true><<<gz, 256, 0, stream>>>(y, dy, act, dx ? dz : nullptr, dzT, bpart, M, Mp, Cout);
     MAC_LAUNCH_CHECK();
-    im2col3x3_t_kernel<true><<<gc, 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, B, H, W, C, Mp);
+    if (k3s1)
+      im2col3x3_t_kernel<true><<<gc, 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, B, H, W, C, Mp);
+    else
+      im2col_t_kernel<true><<<gc, 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, g, Mp);
   } else {
     conv_dz_pack_kernel<false><<<gz, 256, 0, stream>>>(y, dy, act, dz, dzT, bpart, M, Mp, Cout);
     MAC_LAUNCH_CHECK();
-    im2col3x3_t_kernel<false><<<gc, 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, B, H, W, C, Mp);
+    if (k3s1)
+      im2col3x3_t_kernel<false><<<gc, 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, B, H, W, C, Mp);
+    else
+      im2col_t_kernel<false><<<gc, 256, 0, stream>>>(x, colsT, thr, scale, seed, site, step, g, Mp);
   }
   MAC_LAUNCH_CHECK();
   int st = mac_colsum(bpart, dbias, 1, Mp / 64, Cout, 1, stream_);
@@ -1084,30 +1307,79 @@ static int conv3x3_bwd_wgmma(bool split, const float* x, const float* y, const f
     st = mac_linear_tc_fwd(dz, k16, nullptr, MAC_ACT_NON, dcols, 0, M, Cout, K, stream_);
   }
   if (st != MAC_OK) return st;
-  return mac_col2im3x3(dcols, dx, keep, seed, site, step, B, H, W, C, stream_);
+  return k3s1 ? mac_col2im3x3(dcols, dx, keep, seed, site, step, B, H, W, C, stream_)
+              : mac_col2im(dcols, dx, keep, seed, site, step, B, H, W, C, k, s, stream_);
 }
 }  // namespace mac
 
+extern "C" int mac_im2col_t(const float* x, void* colsT, int split, float keep, uint64_t seed, int site, int step, int B, int H,
+                            int W, int C, int k, int s, mac_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x || !colsT) return MAC_ERR_INVALID;
+  const int st = conv_geom_check(B, H, W, C, k, s, keep);
+  if (st != MAC_OK) return st;
+  if ((split != 0 && split != 1) || C % 64 || !im2col_t_grid_ok(k, C)) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(x) || !mac_aligned16(colsT)) return MAC_ERR_ALIGN;
+  const ConvGeom g = conv_geom(B, H, W, C, k, s);
+  const int M = B * g.Ho * g.Wo, Mp = (M + 63) & ~63;
+  const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
+  const float scale = keep < 1.f ? 1.f / keep : 1.f;
+  const dim3 gc(Mp / 64, k * k * C / 64);
+  if (split)
+    im2col_t_kernel<true><<<gc, 256, 0, stream>>>(x, reinterpret_cast<__nv_bfloat16*>(colsT), thr, scale, seed, site, step, g,
+                                                  Mp);
+  else
+    im2col_t_kernel<false><<<gc, 256, 0, stream>>>(x, reinterpret_cast<__nv_bfloat16*>(colsT), thr, scale, seed, site, step, g,
+                                                   Mp);
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+extern "C" size_t mac_conv_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int k, int s, int with_dx) {
+  if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C)) return 0;
+  return conv_bwd_layout(conv_geom(B, H, W, C, k, s), Cout, with_dx != 0, false).total;
+}
+
+extern "C" int mac_conv_bwd_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                               uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
+                               size_t workspace_bytes, int B, int H, int W, int C, int Cout, int k, int s, mac_stream_t stream_) {
+  return conv_bwd_wgmma(false, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
+                        B, H, W, C, Cout, k, s, stream_);
+}
+
+extern "C" size_t mac_conv_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int k, int s, int with_dx) {
+  if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C)) return 0;
+  return conv_bwd_layout(conv_geom(B, H, W, C, k, s), Cout, with_dx != 0, true).total;
+}
+
+extern "C" int mac_conv_bwd_tc32(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                                 uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
+                                 size_t workspace_bytes, int B, int H, int W, int C, int Cout, int k, int s,
+                                 mac_stream_t stream_) {
+  return conv_bwd_wgmma(true, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
+                        B, H, W, C, Cout, k, s, stream_);
+}
+
 extern "C" size_t mac_conv3x3_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx) {
   if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return 0;
-  return conv_bwd_layout(B, H, W, C, Cout, with_dx != 0, false).total;
+  return conv_bwd_layout(conv_geom(B, H, W, C, 3, 1), Cout, with_dx != 0, false).total;
 }
 
 extern "C" int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
                                   uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
                                   size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
-  return conv3x3_bwd_wgmma(false, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
-                           B, H, W, C, Cout, stream_);
+  return conv_bwd_wgmma(false, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
+                        B, H, W, C, Cout, 3, 1, stream_);
 }
 
 extern "C" size_t mac_conv3x3_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx) {
   if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return 0;
-  return conv_bwd_layout(B, H, W, C, Cout, with_dx != 0, true).total;
+  return conv_bwd_layout(conv_geom(B, H, W, C, 3, 1), Cout, with_dx != 0, true).total;
 }
 
 extern "C" int mac_conv3x3_bwd_tc32(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
                                     uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
                                     size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
-  return conv3x3_bwd_wgmma(true, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
-                           B, H, W, C, Cout, stream_);
+  return conv_bwd_wgmma(true, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
+                        B, H, W, C, Cout, 3, 1, stream_);
 }

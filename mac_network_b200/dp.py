@@ -40,9 +40,11 @@ def check_model_precisions(cfg, encoder, stem, stem_prec, enc_prec):
     if stem_prec != "fp32":
         if stem is None:
             raise ValueError("stem_prec=%r needs stem=" % (stem_prec,))
-        if stem[0] % 128 or cfg.memDim % 128:
-            raise NotImplementedError("stem_prec=%r needs the image channels (%d) and memDim (%d) to be multiples of "
-                                      "128 (the wgmma tiles of mac_conv3x3_bwd_tc)" % (stem_prec, stem[0], cfg.memDim))
+        stem_dim = stem_geometry(stem)["stem_dim"]
+        if stem[0] % 128 or cfg.memDim % 128 or (stem_dim is not None and stem_dim % 128):
+            raise NotImplementedError("stem_prec=%r needs the image channels (%d), memDim (%d) and stem_dim (%s) to be "
+                                      "multiples of 128 (the wgmma tiles of mac_conv3x3_bwd_tc)"
+                                      % (stem_prec, stem[0], cfg.memDim, stem_dim))
     if enc_prec not in ("fp32", "bf16"):
         raise ValueError("enc_prec must be 'fp32' or 'bf16', got %r" % (enc_prec,))
     if enc_prec != "fp32":
@@ -51,6 +53,25 @@ def check_model_precisions(cfg, encoder, stem, stem_prec, enc_prec):
         if cfg.ctrlDim != 512:
             raise NotImplementedError("enc_prec='bf16' needs ctrlDim = 512 (h = 256 per LSTM direction), got %d"
                                       % cfg.ctrlDim)
+
+
+STEM_GEOMETRY = {"ksizes": None, "strides": None, "linear": False, "stem_dim": None}
+
+
+def stem_geometry(stem):
+    """The geometry of `stem=(imageInDim, stemNumLayers[, geometry])`: a dict with the keys of STEM_GEOMETRY --
+    `ksizes` (--stemKernelSizes, one kernel size per layer; None: 3x3), `strides` (--stemStrideSizes; None: 1),
+    `linear` (--stemLinear) and `stem_dim` (--stemDim; None: memDim) -- defaults filled in."""
+    geom = dict(STEM_GEOMETRY)
+    extra = dict(stem[2]) if len(stem) > 2 and stem[2] is not None else {}
+    unknown = sorted(set(extra) - set(geom))
+    if unknown:
+        raise ValueError("unknown stem geometry keys %s (known: %s)" % (unknown, sorted(geom)))
+    geom.update(extra)
+    if geom["linear"] and (geom["ksizes"] is not None or geom["stem_dim"] is not None
+                           or geom["strides"] not in (None, [1], (1,))):
+        raise ValueError("the linear stem is one 1x1 stride-1 layer: it takes no ksizes, strides or stem_dim, got %s" % extra)
+    return geom
 
 
 def model_parameters(cfg, netLength, seed, classifier=None, encoder=None, stem=None, param_values=None):
@@ -71,7 +92,9 @@ def model_parameters(cfg, netLength, seed, classifier=None, encoder=None, stem=N
         from .encoder import encoder_specs, init_encoder_params
         from .stem import stem_specs, init_stem_params
         enc_specs = encoder_specs(encoder[0], encoder[1], cfg.ctrlDim, ctrl_dim=cfg.ctrlDim, bi=True)
-        stem_specs_ = stem_specs(stem[0], cfg.memDim, num_layers=stem[1])
+        geom = stem_geometry(stem)
+        stem_specs_ = stem_specs(stem[0], cfg.memDim, num_layers=stem[1], ksizes=geom["ksizes"], stem_dim=geom["stem_dim"],
+                                 linear=geom["linear"])
         extra_specs = collections.OrderedDict(list(extra_specs.items()) + list(enc_specs.items())
                                               + list(stem_specs_.items()))
         extra_values = dict(extra_values)
@@ -89,7 +112,9 @@ class DPTrainer(object):
                  stem_prec="fp32", enc_prec="fp32"):
         """`classifier=(answerWordsNum, outClassifierDims)` adds the reference's output unit + answer loss
         (model.py:512-528, 547-576, 593-596); `encoder=(vocabulary rows, wrdEmbDim)` the question input unit
-        (model.py:208-220, 279-307) and `stem=(imageInDim, stemNumLayers)` the image stem (model.py:165-204), with the
+        (model.py:208-220, 279-307) and `stem=(imageInDim, stemNumLayers)` the image stem (model.py:165-204) -- or
+        `stem=(imageInDim, stemNumLayers, geometry)` with the stem's kernel sizes, strides, linear form and width
+        (`stem_geometry`) --, with the
         reference's training dropouts (config.py:202-206).  All variables join the same flat buckets, so the one
         all-reduce and the one fused optimizer pass cover the whole model (`train_step_full`).
         `prec="bf16"` runs the read unit's forward projections on tensor cores in training too (activations saved in bf16,
@@ -131,8 +156,9 @@ class DPTrainer(object):
             self.enc = QuestionEncoder({k: self.params.t[k] for k in self._enc_specs}, keep_input=enc_dropouts[0],
                                        keep_question=enc_dropouts[1], seed=seed, prec=enc_prec,
                                        version=lambda: self.params.version)
+            geom = self.stem_geometry = stem_geometry(stem)
             self.stem = Stem({k: self.params.t[k] for k in self._stem_specs}, relu=cfg.relu, prec=stem_prec, seed=seed,
-                             version=lambda: self.params.version)
+                             version=lambda: self.params.version, strides=geom["strides"], linear=geom["linear"])
             self.stem_dropout = float(stem_dropout)
             self._full_bufs = {}
         n = self.params.numel

@@ -429,15 +429,18 @@ def _encoder_fn(mod, grads, seed_step, questions, lengths):
 
 class ImageStem(_KernelModule):
     """The image stem (model.py:165-204): `forward(images=NHWC fp32)` or `forward(images_nchw=NCHW fp32 or fp16)` -> the
-    knowledge base [B, H*W, out_dim].  The gradient w.r.t. the images is computed exactly when they require grad, and
-    comes back in their dtype.  `prec`: "fp32", "bf16" or "bf16x3" (training and inference) or "fp8" (inference)."""
+    knowledge base [B, Ho*Wo, out_dim] on the stem's output grid (`grid`).  The gradient w.r.t. the images is computed
+    exactly when they require grad, and comes back in their dtype.  `prec`: "fp32", "bf16" or "bf16x3" (training and
+    inference) or "fp8" (inference).  `ksizes`, `strides`, `linear`, `stem_dim`: the reference's --stemKernelSizes,
+    --stemStrideSizes, --stemLinear and --stemDim."""
 
-    def __init__(self, in_dim, out_dim, num_layers=2, relu="ELU", prec="fp32", values=None, seed=0, device="cuda"):
+    def __init__(self, in_dim, out_dim, num_layers=2, relu="ELU", prec="fp32", values=None, seed=0, device="cuda",
+                 ksizes=None, strides=None, linear=False, stem_dim=None):
         super(ImageStem, self).__init__()
-        specs = stem_specs(in_dim, out_dim, num_layers=num_layers)
+        specs = stem_specs(in_dim, out_dim, num_layers=num_layers, ksizes=ksizes, linear=linear, stem_dim=stem_dim)
         values = values if values is not None else init_stem_params(specs, seed=seed + 23, bias_scale=0.0)
         self._register(_Params(specs, values, device), seed)
-        self._stem = _stem_unit(self.params, relu, prec)
+        self._stem = _stem_unit(self.params, relu, prec, {"strides": strides, "linear": linear})
         self._stem_names, self.stem_keep = list(specs), STEM_KEEP
 
     def forward(self, images=None, images_nchw=None):
@@ -448,9 +451,9 @@ class ImageStem(_KernelModule):
         return _stem_fn(self, self._grads(), self._next(), x, nchw)
 
 
-def _stem_unit(params, relu, prec):
+def _stem_unit(params, relu, prec, geometry):
     return Stem({k: params.t[k] for k in params.t if k.startswith("stem/")}, relu=relu, prec=prec,
-                version=lambda: params.version)
+                version=lambda: params.version, strides=geometry["strides"], linear=geometry["linear"])
 
 
 def _pick_images(images, images_nchw):
@@ -503,12 +506,12 @@ class MACModel(_KernelModule):
 
     def __init__(self, cfg, netLength, vocab, n_answers, wrd_emb_dim=300, image_in_dim=1024, classifier_dims=(512,),
                  stem_layers=2, prec="fp32", bwd_tc=False, stem_prec="fp32", enc_prec="fp32", eval_prec=None, values=None,
-                 seed=0, device="cuda"):
+                 seed=0, device="cuda", stem_geometry=None):
         super(MACModel, self).__init__()
-        from .dp import check_model_precisions, model_parameters
+        from .dp import check_model_precisions, model_parameters, stem_geometry as stem_geometry_of
         if not cfg.controlContextual:
             raise NotImplementedError("the raw-word control inputs (controlContextual off) need wrdEmbDim == ctrlDim")
-        encoder, stem = (vocab, wrd_emb_dim), (image_in_dim, stem_layers)
+        encoder, stem = (vocab, wrd_emb_dim), (image_in_dim, stem_layers, stem_geometry)
         check_model_precisions(cfg, encoder, stem, stem_prec, enc_prec)
         cell_values, extra_specs, extra_values, enc_specs, stem_specs_ = model_parameters(
             cfg, netLength, seed, (n_answers, list(classifier_dims)), encoder, stem, values)
@@ -521,7 +524,7 @@ class MACModel(_KernelModule):
         self._enc_names, self._stem_names = list(enc_specs), list(stem_specs_)
         self._out_names = [k for k in extra_specs if k.startswith(("outputUnit/", "classifier/"))]
         self._enc = _encoder_units(self.params, enc_prec)
-        self._stem = _stem_unit(self.params, cfg.relu, stem_prec)
+        self._stem = _stem_unit(self.params, cfg.relu, stem_prec, stem_geometry_of(stem))
         self._out = _output_unit(self.params, cfg.relu)
         self.stem_keep = STEM_KEEP
         self.cells = _Cells(cfg, netLength, self.params, prec, bwd_tc, eval_prec,
@@ -536,13 +539,12 @@ class MACModel(_KernelModule):
             raise ValueError("from_trainer needs a trainer built with classifier=, encoder= and stem=")
         specs = t.params.specs
         vocab, E = specs["qEmbeddings/emb"][0]
-        kernels = [k for k in t._stem_specs if k.endswith("kernels/kernel")]
         fcs = [specs[k][0] for k in specs if k.startswith("classifier/") and k.endswith("weights/weight")]
         values = {k: v.reshape(specs[k][0]) for k, v in t.params.numpy().items()}
-        m = cls(t.cfg, t.L, vocab, fcs[-1][1], wrd_emb_dim=E, image_in_dim=specs[kernels[0]][0][2],
-                classifier_dims=[s[1] for s in fcs[:-1]], stem_layers=len(kernels), prec=t.prec, bwd_tc=t.bwd_tc,
+        m = cls(t.cfg, t.L, vocab, fcs[-1][1], wrd_emb_dim=E, image_in_dim=t.stem.in_dim,
+                classifier_dims=[s[1] for s in fcs[:-1]], stem_layers=t.stem.nlayers, prec=t.prec, bwd_tc=t.bwd_tc,
                 stem_prec=t.stem_prec, enc_prec=t.enc_prec, eval_prec=eval_prec, values=values, seed=t.base_seed,
-                device=t.params.device)
+                device=t.params.device, stem_geometry=t.stem_geometry)
         m.step = t.step_id
         m.cells.dropouts = tuple(float(k) for k in t.dropouts)
         m._enc[0].keep_input, m._enc[0].keep_question = t.enc.keep_input, t.enc.keep_question
@@ -565,7 +567,8 @@ class MACModel(_KernelModule):
         x, nchw = _pick_images(images, images_nchw)
         lengths = _int32(questionLengths)
         B, S = questions.shape
-        N = x.shape[2] * x.shape[3] if nchw else x.shape[1] * x.shape[2]
+        Ho, Wo = self._stem.grid(*(x.shape[2:4] if nchw else x.shape[1:3]))
+        N = Ho * Wo
         U = None if imageIndex is None else x.shape[0]
         if not self._trains(x):
             words, cntx, vecq = self._enc[1].forward(questions, lengths)

@@ -385,7 +385,7 @@ class _ModelSlot(object):
         t, cfg = model.trainer, model.cfg
         p = t.params
         self.model, self.B, self.topk, self.use_graph = model, B, topk, use_graph
-        C = p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2]
+        C = model._stem.in_dim
         self.stream = torch.cuda.Stream()
         self.x = {"questions": torch.zeros(B, S, dtype=torch.int32, device=p.device),
                   "questionLengths": torch.full((B,), S, dtype=torch.int32, device=p.device),
@@ -397,7 +397,8 @@ class _ModelSlot(object):
         version = lambda: p.version
         self.enc = QuestionEncoder({k: p.t[k] for k in t._enc_specs}, keep_input=1.0, keep_question=1.0,
                                    prec=model._enc.prec, version=version)
-        self.stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=model._stem.prec, version=version)
+        self.stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=model._stem.prec, version=version,
+                         strides=model._stem.strides, linear=model._stem.linear)
         self.out = OutputUnit({k: p.t[k] for k in p.specs if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu,
                               keep=1.0, version=version)
         self.cell = None
@@ -669,8 +670,8 @@ class ModelPipeline(object):
     path; callers who see the copies keep up should pass `host_cast=False`.
 
     `out`: `answers` int32 [B, topk] (column 0 is the prediction), `probs` [B, topk], `logits` [B, A], `memory` [B, d],
-    `att_kb` [L, B, H*W], `att_question` [L, B, S], and `gate` [L, B, d] / `self` [L, B, L] (step i's i + 1 weights, zero
-    beyond) when the flag set has them.
+    `att_kb` [L, B, Ho*Wo] (the stem's output grid, `Stem.grid`), `att_question` [L, B, S], and `gate` [L, B, d] /
+    `self` [L, B, L] (step i's i + 1 weights, zero beyond) when the flag set has them.
 
     Several questions per image: with `images=U` (1 <= U <= B) a batch carries k <= U distinct images and each question's
     image number,
@@ -685,7 +686,7 @@ class ModelPipeline(object):
 
     Knowledge bases kept on the device across batches: with `cache=C` (C >= B, and `images=U` the number of images one stem
     pass takes) the pipeline keeps the knowledge bases of the last C distinct images it has seen in one device pool
-    [C, H*W, d], shared by all slots, keyed by the caller's integer image ids,
+    [C, Ho*Wo, d], shared by all slots, keyed by the caller's integer image ids,
 
         pipe = ModelPipeline(model, shape=(B, S, H, W), slots=4, images=16, cache=15000)
         t = pipe.submit({"questions": ..., "questionLengths": ..., "imageIds": int [B], "images": load})
@@ -732,7 +733,7 @@ class ModelPipeline(object):
             raise ValueError("host_cast=True casts fp32 features to bf16 on the host: with image_dtype=torch.float16 the "
                              "features cross PCIe as stored and are widened on the device")
         p = model.trainer.params
-        C = int(p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2])
+        C = model._stem.in_dim
         nfc = len([k for k in p.t if k.startswith("classifier/linearLayerfc_") and k.endswith("weights/weight")])
         A = int(p.t["classifier/linearLayerfc_%d/weights/weight" % (nfc - 1)].shape[1])
         if min(B, S, H, W) <= 0 or slots < 1:
@@ -773,7 +774,8 @@ class ModelPipeline(object):
             # _kb_gather_bf16 condition), the stem's fp32 rows for every other form
             cfg = model.cfg
             pool_bf16 = model.prec in ("bf16", "fp8") and cfg.is_fast_path and not cfg.unsharedCells
-            self.pool = torch.zeros(cache, H * W, cfg.memDim, dtype=torch.bfloat16 if pool_bf16 else torch.float32,
+            n_kb = int(np.prod(model._stem.grid(H, W)))             # the stem's output grid
+            self.pool = torch.zeros(cache, n_kb, cfg.memDim, dtype=torch.bfloat16 if pool_bf16 else torch.float32,
                                     device=p.device)
             self._cache = _KBCache(cache, slots)
             self.slots = [_CachedSlot(model, self.shape, self.use_graph, self.topk, images, self.pool, image_dtype)
@@ -1046,7 +1048,7 @@ class TrainPipeline(object):
         if t.stem is None:
             raise ValueError("the model's trainer has no stem: TrainPipeline trains the whole model")
         p = t.params
-        C = int(p.t["stem/cnnLayercnn_0/kernels/kernel"].shape[2])
+        C = model._stem.in_dim
         nfc = len([k for k in p.t if k.startswith("classifier/linearLayerfc_") and k.endswith("weights/weight")])
         self.A = int(p.t["classifier/linearLayerfc_%d/weights/weight" % (nfc - 1)].shape[1])
         if min(B, S, H, W) <= 0 or int(depth) < 1:

@@ -10,7 +10,13 @@ indexed by the SOURCE element, so all nine copies of a pixel share its mask), in
 forward in e4m3: `mac_im2col3x3_fp8` (per-row scales, no dropout) and `mac_linear_fp8_fwd` (csrc/tc_gemm_fp8.cuh).
 `prec="bf16x3"` is the parity arithmetic on tensor cores, for inference and training: every fp32 operand as hi + lo bf16
 halves and three bf16 products per fp32 product (`mac_im2col3x3_split`, `mac_linear_tc32_fwd`, `mac_conv3x3_bwd_tc32`;
-the split-bf16 scheme the cell calls "tc32", DESIGN.md section 9 item 6)."""
+the split-bf16 scheme the cell calls "tc32", DESIGN.md section 9 item 6).
+
+Other geometries (--stemKernelSize(s), --stemStrideSizes, --stemLinear): a layer is (k, s, act, dropout) with TF SAME
+padding (`Ho = ceil(H / s)`, the odd padding row on the bottom / right); the linear stem is the layer (1, 1, NON, no
+dropout) on the `[inDim, outDim]` weight viewed as `[1, 1, inDim, outDim]`.  Layers with k = 3, s = 1 run the 3x3 kernels
+above; every other layer runs the general patch passes (`mac_im2col`, `mac_col2im`, `mac_conv_bwd_tc` / `_tc32`) with the
+same GEMMs.  The e4m3 stem keeps only the 3x3 stride-1 geometry."""
 import collections
 
 import numpy as np
@@ -22,16 +28,43 @@ from ._lib import act_code, check, ptr, segments, stream_ptr
 SITE_STEM = 32            # Philox site base for the stem's input dropouts (site + layer index)
 INGEST_NHWC_F32, INGEST_PATCH_BF16 = 0, 1       # enum MAC_INGEST_* (include/mac_b200.h)
 INGEST_COLS_BF16, INGEST_COLS_SPLIT = 0, 1      # enum MAC_INGEST_COLS_*
+COLS_F32, COLS_BF16, COLS_SPLIT = 0, 1, 2       # enum MAC_COLS_*
+LINEAR_W, LINEAR_B = "stem/linearLayer/weights/weight", "stem/linearLayer/biases/bias"
 
 
-def stem_specs(in_dim, out_dim, num_layers=2, ksize=3, stem_dim=None):
-    stem_dim = out_dim if stem_dim is None else stem_dim
-    dims = [in_dim] + [stem_dim] * (num_layers - 1) + [out_dim]
+def stem_specs(in_dim, out_dim, num_layers=2, ksize=3, stem_dim=None, ksizes=None, linear=False):
+    """The stem's variables as the reference names and shapes them (model.py:165-204): `--stemLinear` one `ops.linear`
+    (`stem/linearLayer/weights/weight` [inDim, outDim] and its bias), else `num_layers` HWIO kernels
+    `stem/cnnLayercnn_i/kernels/kernel` [k_i, k_i, Cin, Cout] of kernel size `ksizes[i]` (--stemKernelSizes) or `ksize`
+    (--stemKernelSize) for every layer."""
     s = collections.OrderedDict()
+    if linear:
+        if ksizes is not None or stem_dim is not None:
+            raise ValueError("the linear stem is one [inDim, outDim] layer: it takes no ksizes or stem_dim")
+        s[LINEAR_W] = ((in_dim, out_dim), "xavier")
+        s[LINEAR_B] = ((out_dim,), "zeros")
+        return s
+    stem_dim = out_dim if stem_dim is None else stem_dim
+    ks = [ksize] * num_layers if ksizes is None else [int(k) for k in ksizes]
+    if len(ks) != num_layers:
+        raise ValueError("ksizes has %d entries for %d stem layers" % (len(ks), num_layers))
+    dims = [in_dim] + [stem_dim] * (num_layers - 1) + [out_dim]
     for i in range(num_layers):
-        s["stem/cnnLayercnn_%d/kernels/kernel" % i] = ((ksize, ksize, dims[i], dims[i + 1]), "xavier")
+        s["stem/cnnLayercnn_%d/kernels/kernel" % i] = ((ks[i], ks[i], dims[i], dims[i + 1]), "xavier")
         s["stem/cnnLayercnn_%d/biases/bias" % i] = ((dims[i + 1],), "zeros")
     return s
+
+
+def conv_out(n, s):
+    """TF SAME output extent of a stride-`s` convolution over `n` pixels: ceil(n / s) whatever the kernel size."""
+    return -(-int(n) // int(s))
+
+
+def stem_grid(H, W, strides):
+    """The knowledge-base grid (Ho, Wo) a stem with per-layer `strides` makes of an H x W feature map."""
+    for s in strides:
+        H, W = conv_out(H, s), conv_out(W, s)
+    return H, W
 
 
 def init_stem_params(specs, seed=0, dtype=np.float32, bias_scale=0.1):
@@ -41,40 +74,86 @@ def init_stem_params(specs, seed=0, dtype=np.float32, bias_scale=0.1):
         if kind == "zeros":
             v = bias_scale * rng.standard_normal(shape)
         else:       # tf.contrib.layers.xavier_initializer on [kh,kw,cin,cout]: fan_in = kh*kw*cin, fan_out = kh*kw*cout
-            rf = shape[0] * shape[1]
-            lim = np.sqrt(6.0 / (rf * shape[2] + rf * shape[3]))
+            rf = shape[0] * shape[1] if len(shape) == 4 else 1
+            lim = np.sqrt(6.0 / (rf * shape[-2] + rf * shape[-1]))
             v = rng.uniform(-lim, lim, size=shape)
         out[name] = np.asarray(v, dtype=dtype)
     return out
 
 
 class Stem(object):
-    def __init__(self, params, relu="ELU", prec="fp32", seed=0, version=None):
-        """`params`: dict TF-name -> CUDA fp32 tensor (HWIO kernels, biases).  `version`: optional callable returning a counter
+    def __init__(self, params, relu="ELU", prec="fp32", seed=0, version=None, strides=None, linear=False):
+        """`params`: dict TF-name -> CUDA fp32 tensor (HWIO kernels, biases; or with `linear=True` the `stem/linearLayer`
+        weight [inDim, outDim] and bias).  Each layer's kernel size is read from its kernel's shape; `strides`
+        (--stemStrideSizes) gives one stride per layer, default 1.  `version`: optional callable returning a counter
         that changes whenever the parameter values do (`MACParams.version`): the packed bf16 / e4m3 kernels are rebuilt when it moves
         (optimizer step, checkpoint restore, EMA swap -- ADVICE r1), whoever changed the values."""
         self.lib = _lib.load()
         self.p = params
         self.relu, self.prec, self.seed = relu, prec, int(seed)
-        self.nlayers = len([k for k in params if k.endswith("kernels/kernel")])
+        self.linear = bool(linear)
+        if self.linear:
+            if set(params) != {LINEAR_W, LINEAR_B}:
+                raise ValueError("a linear stem takes %s and %s, got %s" % (LINEAR_W, LINEAR_B, sorted(params)))
+            self.nlayers, self.ksizes = 1, [1]
+        else:
+            self.nlayers = len([k for k in params if k.endswith("kernels/kernel")])
+            self.ksizes = [int(params["stem/cnnLayercnn_%d/kernels/kernel" % i].shape[0]) for i in range(self.nlayers)]
+        self.strides = [1] * self.nlayers if strides is None else [int(v) for v in strides]
+        if len(self.strides) != self.nlayers or any(v < 1 for v in self.strides) or (self.linear and self.strides != [1]):
+            raise ValueError("strides %s do not fit a %s stem of %d layer(s)" % (strides, "linear" if self.linear else "CNN",
+                                                                                 self.nlayers))
         self._cache = packs.Cache(version)
         dev = next(iter(params.values())).device
         self.device = dev
 
+    @property
+    def in_dim(self):
+        """The image channels the stem reads (layer 0's Cin)."""
+        return int(self.p[self._names(0)[0]].shape[-2])
+
+    def grid(self, H, W):
+        """The knowledge base's grid (Ho, Wo) for H x W features: the knowledge base has Ho * Wo rows."""
+        return stem_grid(H, W, self.strides)
+
+    def _names(self, i):
+        if self.linear:
+            return LINEAR_W, LINEAR_B
+        return "stem/cnnLayercnn_%d/kernels/kernel" % i, "stem/cnnLayercnn_%d/biases/bias" % i
+
+    def _bias(self, i):
+        return self.p[self._names(i)[1]]
+
+    def _k3s1(self, i):
+        return self.ksizes[i] == 3 and self.strides[i] == 1
+
+    def _act(self):
+        return act_code("NON", self.relu) if self.linear else act_code("RELU", self.relu)
+
+    def _keep(self, keep):
+        return 1.0 if self.linear else float(keep)      # ops.linear runs without dropout in the stem (ops.py:298)
+
+    def _cout(self, i):
+        return int(self.p[self._names(i)[0]].shape[-1])
+
     def _weights(self, i):
-        """(W, packed): the fp32 [9*Cin, Cout] view and, for bf16, the bf16 [Cout, 9*Cin] pack; for bf16x3, the split pack
-        [Cout, 3*9*Cin] = [hi | hi | lo]; for fp8, the e4m3 [Cout, 9*Cin] pack and its per-column scales as a pair."""
-        K = self.p["stem/cnnLayercnn_%d/kernels/kernel" % i]
-        W = K.reshape(-1, K.shape[3])                       # [9*Cin, Cout], row-major view of the HWIO kernel
+        """(W, packed): the fp32 [k*k*Cin, Cout] view and, for bf16, the bf16 [Cout, k*k*Cin] pack; for bf16x3, the split pack
+        [Cout, 3*k*k*Cin] = [hi | hi | lo]; for fp8, the e4m3 [Cout, 9*Cin] pack and its per-column scales as a pair."""
+        K = self.p[self._names(i)[0]]
+        W = K.reshape(-1, K.shape[-1])                      # [k*k*Cin, Cout], row-major view of the HWIO kernel
         build = {"bf16": packs.bf16, "bf16x3": packs.split3, "fp8": packs.fp8}.get(self.prec)
         return W, None if build is None else self._cache.pack(build, W, stream=stream_ptr())
 
     def _check_fp8(self, in_dim, keep):
-        """The e4m3 stem is the inference forward only (no dropout) with every channel count a multiple of 128 (whole
-        128-byte k-blocks and 128-column tiles of mac_linear_fp8_fwd).  Raises before any launch."""
+        """The e4m3 stem is the inference forward only (no dropout) of the 3x3 stride-1 geometry with every channel count a
+        multiple of 128 (whole 128-byte k-blocks and 128-column tiles of mac_linear_fp8_fwd).  Raises before any launch."""
+        if self.linear or not all(self._k3s1(i) for i in range(self.nlayers)):
+            raise NotImplementedError("the fp8 stem runs the 3x3 stride-1 geometry only, got %s"
+                                      % ("the linear stem" if self.linear else "kernel sizes %s, strides %s"
+                                         % (self.ksizes, self.strides)))
         if float(keep) != 1.0:
             raise NotImplementedError("the fp8 stem is inference only: keep must be 1.0, got %r" % (keep,))
-        dims = [in_dim] + [int(self.p["stem/cnnLayercnn_%d/kernels/kernel" % i].shape[3]) for i in range(self.nlayers)]
+        dims = [in_dim] + [self._cout(i) for i in range(self.nlayers)]
         if any(c % 128 for c in dims):
             raise NotImplementedError("the fp8 stem needs channel counts that are multiples of 128, got %s" % dims)
 
@@ -83,7 +162,7 @@ class Stem(object):
         M = B * H * Wd
         for i in range(self.nlayers):
             _, (W8, sw) = self._weights(i)
-            b = self.p["stem/cnnLayercnn_%d/biases/bias" % i]
+            b = self._bias(i)
             C, Nout = x.shape[3], W8.shape[0]
             cols = torch.empty((M, 9 * C), dtype=torch.uint8, device=self.device)
             sa = torch.empty(M, dtype=torch.float32, device=self.device)
@@ -98,7 +177,7 @@ class Stem(object):
         return x.view(B, H * Wd, x.shape[3])
 
     def _check_tiles(self, in_dim, what):
-        dims = [in_dim] + [int(self.p["stem/cnnLayercnn_%d/kernels/kernel" % i].shape[3]) for i in range(self.nlayers)]
+        dims = [in_dim] + [self._cout(i) for i in range(self.nlayers)]
         if any(c % 128 for c in dims):
             raise NotImplementedError("%s needs channel counts that are multiples of 128 (the wgmma tiles of "
                                       "mac_conv3x3_bwd_tc), got %s; use prec='fp32' (DESIGN.md section 9)" % (what, dims))
@@ -113,50 +192,56 @@ class Stem(object):
             raise NotImplementedError("stem training runs in fp32, bf16 or bf16x3, not %r (DESIGN.md section 9)" % self.prec)
         self._check_tiles(in_dim, "%s stem training" % self.prec)
 
+    def _patches(self, x, i, form, keep, step):
+        """Layer i's patch matrix of x [B,H,W,C] (form COLS_F32, COLS_BF16 or COLS_SPLIT), dropout fused: the 3x3 stride-1
+        passes for that geometry, `mac_im2col` for every other."""
+        B, H, Wd, C = x.shape
+        k, s = self.ksizes[i], self.strides[i]
+        Ho, Wo = conv_out(H, s), conv_out(Wd, s)
+        K = k * k * C
+        cols = torch.empty((B * Ho * Wo, K * (2 if form == COLS_SPLIT else 1)),
+                           dtype=torch.float32 if form == COLS_F32 else torch.bfloat16, device=self.device)
+        if not self._k3s1(i):
+            check(self.lib.mac_im2col(ptr(x), ptr(cols), form, float(keep), self.seed, SITE_STEM + i, int(step), B, H, Wd, C,
+                                      k, s, stream_ptr()), "mac_im2col")
+        elif form == COLS_SPLIT:
+            check(self.lib.mac_im2col3x3_split(ptr(x), ptr(cols), float(keep), self.seed, SITE_STEM + i, int(step), B, H, Wd,
+                                               C, stream_ptr()), "mac_im2col3x3_split")
+        else:
+            check(self.lib.mac_im2col3x3(ptr(x), ptr(cols), int(form == COLS_BF16), float(keep), self.seed, SITE_STEM + i,
+                                         int(step), B, H, Wd, C, stream_ptr()), "mac_im2col3x3")
+        return cols
+
     def forward(self, images, keep=1.0, step=0, save_for_backward=False, _cols0=None):
         """images: [B,H,W,C] fp32 NHWC (the reference transposes the NCHW h5 features first, model.py:~770).
-        Returns the knowledge base [B, H*W, outDim] fp32.  `_cols0` (`forward_nchw`, bf16 and bf16x3 stems): layer 0's patch
-        matrix, already built with this call's keep and step; `images` is then read only by the backward, if at all."""
+        Returns the knowledge base [B, Ho*Wo, outDim] fp32 (`grid`).  `_cols0` (`forward_nchw`, bf16 and bf16x3 stems): layer
+        0's patch matrix, already built with this call's keep and step; `images` is then read only by the backward, if at all."""
         x = images
         B, H, Wd, C = x.shape
-        act = act_code("RELU", self.relu)
+        act = self._act()
+        keep = self._keep(keep)
         if save_for_backward:
             self._check_trainable(C)
-            self._saved = {"xs": [], "ys": [], "keep": float(keep), "step": int(step), "act": act}
+            self._saved = {"xs": [], "ys": [], "keep": keep, "step": int(step), "act": act}
         if self.prec == "fp8":
             self._check_fp8(C, keep)
             return self._forward_fp8(x, act)
         if self.prec == "bf16x3":
             self._check_tiles(C, "the bf16x3 stem")
+        form = {"bf16": COLS_BF16, "bf16x3": COLS_SPLIT}.get(self.prec, COLS_F32)
         for i in range(self.nlayers):
             if save_for_backward:
                 self._saved["xs"].append(x)
             W, Wt = self._weights(i)
-            b = self.p["stem/cnnLayercnn_%d/biases/bias" % i]
-            C = x.shape[3]
-            M, K, Nout = B * H * Wd, 9 * C, W.shape[1]
-            bf16 = self.prec == "bf16"
+            b = self._bias(i)
+            H, Wd = conv_out(H, self.strides[i]), conv_out(Wd, self.strides[i])
+            M, K, Nout = B * H * Wd, W.shape[0], W.shape[1]
             y = torch.empty((M, Nout), dtype=torch.float32, device=self.device)
-            if self.prec == "bf16x3":
-                if i == 0 and _cols0 is not None:
-                    cols = _cols0
-                else:
-                    cols = torch.empty((M, 2 * K), dtype=torch.bfloat16, device=self.device)          # [hi | lo]
-                    check(self.lib.mac_im2col3x3_split(ptr(x), ptr(cols), float(keep), self.seed, SITE_STEM + i, step, B, H,
-                                                       Wd, C, stream_ptr()), "mac_im2col3x3_split")
+            cols = _cols0 if (i == 0 and _cols0 is not None) else self._patches(x, i, form, keep, step)
+            if form == COLS_SPLIT:
                 check(self.lib.mac_linear_tc32_fwd(ptr(cols), ptr(Wt), ptr(b), act, ptr(y), M, K, Nout, stream_ptr()),
                       "mac_linear_tc32_fwd")
-                if save_for_backward:
-                    self._saved["ys"].append(y)
-                x = y.view(B, H, Wd, Nout)
-                continue
-            if i == 0 and _cols0 is not None:
-                cols = _cols0
-            else:
-                cols = torch.empty((M, K), dtype=torch.bfloat16 if bf16 else torch.float32, device=self.device)
-                check(self.lib.mac_im2col3x3(ptr(x), ptr(cols), 1 if bf16 else 0, float(keep), self.seed, SITE_STEM + i, step,
-                                             B, H, Wd, C, stream_ptr()), "mac_im2col3x3")
-            if bf16:
+            elif form == COLS_BF16:
                 check(self.lib.mac_linear_tc_fwd(ptr(cols), ptr(Wt), ptr(b), act, ptr(y), 0, M, K, Nout, stream_ptr()),
                       "mac_linear_tc_fwd")
             else:
@@ -172,7 +257,8 @@ class Stem(object):
         """`forward` from the features in the layout they are stored in: images [B,C,H,W], contiguous, fp32, fp16 or -- `prec="bf16"`
         inference only, whose layer 0 then reads nothing but bf16(x) -- bf16.  The ingest kernels (csrc/ingest.cuh) replace
         the NHWC permute.  Inference (keep = 1, no save_for_backward): `mac_ingest_nchw` writes the bf16 stem's layer-0 patch
-        matrix directly, for the other precisions the fp32 NHWC tensor their own patch passes read.  Training (a dropout or
+        matrix directly, for the other precisions the fp32 NHWC tensor their own patch passes read.  A layer 0 of any other
+        geometry than 3x3 stride 1 reads the fp32 NHWC tensor in every precision.  Training (a dropout or
         save_for_backward): the bf16 and bf16x3 stems run `mac_ingest_nchw_train`, which writes the undropped fp32 NHWC tensor
         (saved as layer 0's input) and layer 0's dropped-out bf16 or split patch matrix from one read; the fp32 stem runs the
         NHWC ingest and its usual pass.  Returns -- and saves, and differentiates -- what
@@ -186,7 +272,8 @@ class Stem(object):
             raise ValueError("images must be float32, float16 or bfloat16, got %s" % images.dtype)
         x_bf16 = int(images.dtype == torch.bfloat16)
         f16 = images.dtype == torch.float16
-        train = save_for_backward or float(keep) != 1.0
+        keep = self._keep(keep)
+        train = save_for_backward or keep != 1.0
         if x_bf16 and (self.prec != "bf16" or train):
             raise ValueError("bf16 images are for the bf16 stem's inference only: prec=%r%s reads the fp32 features"
                              % (self.prec, " in training" if train else ""))
@@ -199,6 +286,10 @@ class Stem(object):
             self._check_fp8(C, keep)
         if self.prec == "bf16x3":
             self._check_tiles(C, "the bf16x3 stem")
+        if not self._k3s1(0):         # the fused ingests build 3x3 patches: write the NHWC tensor, then the general pass
+            x = torch.empty((B, H, Wd, C), dtype=torch.float32, device=self.device)
+            self._ingest(images, x_bf16, x, INGEST_NHWC_F32)
+            return self.forward(x, keep, step, save_for_backward)
         if train and self.prec in ("bf16", "bf16x3"):
             split = self.prec == "bf16x3"
             x = torch.empty((B, H, Wd, C), dtype=torch.float32, device=self.device)
@@ -227,49 +318,55 @@ class Stem(object):
 
     def backward(self, d_kb, grads, need_d_images=False):
         """Backward of `forward(save_for_backward=True)` (the reference differentiates the graph with TF autodiff,
-        model.py:626-636).  d_kb [B, H*W, outDim]; accumulates (+=) into `grads` (dict TF-name -> tensor shaped like the
+        model.py:626-636).  d_kb [B, Ho*Wo, outDim]; accumulates (+=) into `grads` (dict TF-name -> tensor shaped like the
         parameter).  Per layer, last to first:  dZ = dY * act'(Y);  dKernel += cols^T @ dZ, dBias += colsum(dZ)
         (`mac_linear_bwd` on the re-generated patch matrix);  dcols = dZ @ Kernel^T;  dX = col2im(dcols) * dropout mask.
         The gradient w.r.t. the images (and with it layer 0's largest GEMM) is skipped unless asked for.
-        With prec="bf16" each layer is one `mac_conv3x3_bwd_tc` call: the same steps with both GEMMs on tensor cores; with
-        prec="bf16x3" one `mac_conv3x3_bwd_tc32` call: the same again on split-bf16 operands."""
+        With prec="bf16" each layer is one `mac_conv3x3_bwd_tc` call (`mac_conv_bwd_tc` for other geometries): the same
+        steps with both GEMMs on tensor cores; with prec="bf16x3" one `mac_conv3x3_bwd_tc32` (`mac_conv_bwd_tc32`) call: the
+        same again on split-bf16 operands."""
         sv = getattr(self, "_saved", None)
         if sv is None:
             raise RuntimeError("forward(save_for_backward=True) must run first")
-        B, H, Wd, _ = sv["xs"][0].shape
-        M = B * H * Wd
-        dy = d_kb.contiguous().view(M, -1)
+        dy = d_kb.contiguous().view(-1, d_kb.shape[-1])
         dx = None
         for i in reversed(range(self.nlayers)):
             x, y = sv["xs"][i], sv["ys"][i]
-            C, Nout = x.shape[3], y.shape[1]
-            K = 9 * C
+            B, H, Wd, C = x.shape
+            Nout = y.shape[1]
+            k, s = self.ksizes[i], self.strides[i]
+            wname, bname = self._names(i)
             W, _ = self._weights(i)
+            need_dx = need_d_images or i > 0
             if self.prec in ("bf16", "bf16x3"):
-                name = "mac_conv3x3_bwd_tc" if self.prec == "bf16" else "mac_conv3x3_bwd_tc32"
-                dx = torch.empty_like(x) if (need_d_images or i > 0) else None
-                nbytes = int(getattr(self.lib, name + "_workspace_bytes")(B, H, Wd, C, Nout, int(dx is not None)))
+                dx = torch.empty_like(x) if need_dx else None
+                if self._k3s1(i):
+                    name = "mac_conv3x3_bwd_tc" if self.prec == "bf16" else "mac_conv3x3_bwd_tc32"
+                    geom = ()
+                else:
+                    name = "mac_conv_bwd_tc" if self.prec == "bf16" else "mac_conv_bwd_tc32"
+                    geom = (k, s)
+                nbytes = int(getattr(self.lib, name + "_workspace_bytes")(B, H, Wd, C, Nout, *geom, int(dx is not None)))
                 ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
                 check(getattr(self.lib, name)(ptr(x), ptr(y), ptr(dy), ptr(W), sv["act"], sv["keep"], self.seed,
-                                              SITE_STEM + i, sv["step"], ptr(grads["stem/cnnLayercnn_%d/kernels/kernel" % i]),
-                                              ptr(grads["stem/cnnLayercnn_%d/biases/bias" % i]), ptr(dx), ptr(ws), nbytes,
-                                              B, H, Wd, C, Nout, stream_ptr()), name)
+                                              SITE_STEM + i, sv["step"], ptr(grads[wname].view(W.shape)), ptr(grads[bname]),
+                                              ptr(dx), ptr(ws), nbytes, B, H, Wd, C, Nout, *geom, stream_ptr()), name)
                 if dx is not None:
-                    dy = dx.view(M, C)
+                    dy = dx.view(-1, C)
                 continue
             dz = torch.empty_like(y)
             check(self.lib.mac_activation_bwd(ptr(y), ptr(dy), sv["act"], ptr(dz), dz.numel(), stream_ptr()), "mac_activation_bwd")
-            cols = torch.empty((M, K), dtype=torch.float32, device=self.device)
-            check(self.lib.mac_im2col3x3(ptr(x), ptr(cols), 0, sv["keep"], self.seed, SITE_STEM + i, sv["step"], B, H, Wd, C,
-                                         stream_ptr()), "mac_im2col3x3")
-            need_dx = need_d_images or i > 0
-            dcols = torch.empty((M, K), dtype=torch.float32, device=self.device) if need_dx else None
+            cols = self._patches(x, i, COLS_F32, sv["keep"], sv["step"])
+            dcols = torch.empty_like(cols) if need_dx else None
             Wt = W.t().contiguous() if need_dx else None
-            _lib.linear_bwd([cols], Wt, dz, [dcols], [0], grads["stem/cnnLayercnn_%d/kernels/kernel" % i],
-                            grads["stem/cnnLayercnn_%d/biases/bias" % i], None, 0, stream_ptr())
+            _lib.linear_bwd([cols], Wt, dz, [dcols], [0], grads[wname].view(W.shape), grads[bname], None, 0, stream_ptr())
             if need_dx:
                 dx = torch.empty_like(x)
-                check(self.lib.mac_col2im3x3(ptr(dcols), ptr(dx), sv["keep"], self.seed, SITE_STEM + i, sv["step"], B, H, Wd,
-                                             C, stream_ptr()), "mac_col2im3x3")
-                dy = dx.view(M, C)
+                if self._k3s1(i):
+                    check(self.lib.mac_col2im3x3(ptr(dcols), ptr(dx), sv["keep"], self.seed, SITE_STEM + i, sv["step"], B, H,
+                                                 Wd, C, stream_ptr()), "mac_col2im3x3")
+                else:
+                    check(self.lib.mac_col2im(ptr(dcols), ptr(dx), sv["keep"], self.seed, SITE_STEM + i, sv["step"], B, H, Wd,
+                                              C, k, s, stream_ptr()), "mac_col2im")
+                dy = dx.view(-1, C)
         return dx if need_d_images else None
