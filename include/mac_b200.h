@@ -608,6 +608,45 @@ int mac_conv_bwd_tc32(const float* x, const float* y, const float* dy, const flo
                       int site, int step, float* dkernel, float* dbias, float* dx, void* workspace, size_t workspace_bytes,
                       int B, int H, int W, int C, int Cout, int k, int s, mac_stream_t stream);
 size_t mac_conv_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int k, int s, int with_dx);
+/* Location-aware layer 0 (--locationAware, ops.py:448-559 with mod CNCT): layer 0 reads concat(x, g), g [H, W, l] fp32 the
+ * constant location grid (l = 2 for --locationType L, 4 locationDim for PE).  Its HWIO kernel's rows split into the image rows
+ * W_img [k^2 C, Cout] and the location rows; the location patch matrix Q is a second GEMM operand:
+ *   Kq = mac_loc_cols_width(l, k) = k^2 l rounded up to 128; W_loc [Kq, Cout] is the location rows then zero rows.
+ *   The location dropout is its own Philox stream (`site`): Q[m, tap l + j] of output m = (b, ho, wo) reads g[hs, ws, j] of the
+ *   source pixel (hs, ws) (mac_im2col's SAME geometry, zero outside the image) and keeps it with component e & 3 of
+ *   philox4x32_10(seed, e >> 2, site, step), e = ((b H + hs) W + ws) l + j: every tap copy shares one draw.
+ * mac_loc_cols: Q [M, Kq] fp32 (MAC_COLS_F32), bf16 (MAC_COLS_BF16) or [hi | lo] bf16 [M, 2 Kq] (MAC_COLS_SPLIT);
+ *   columns k^2 l..Kq-1 are written as zeros on every call.
+ * mac_loc_cols_t: Q^T bf16 [Kq, Mp] (split = 0) or [Kq, 2 Mp] = [hi | lo] (split = 1), Mp = M rounded up to 64, zero in the
+ *   padding rows and in columns M..Mp-1 on every call.
+ * mac_linear_tc_fwd_acc / mac_linear_tc32_fwd_acc: y = act(x W + y) in place, fp32 y [M, n_out], act NON, ELU or RELU, with
+ *   the operands of mac_linear_tc_fwd / mac_linear_tc32_fwd (K % 64 == 0, n_out % 128 == 0).  Layer 0's forward is
+ *   y = Q W_loc + b (mac_linear_tc_fwd / _tc32_fwd, act NON, fp32 out), then y = act(P W_img + y) with these.
+ * mac_conv_bwd_loc_tc / _tc32: mac_conv_bwd_tc / _tc32 of the image half (kernel, dkernel: [k^2 C, Cout]), then
+ *   dwloc [Kq, Cout] += Q^T dZ (tc_wgrad_splitk / tc3_wgrad_splitk on the same dZ^T).  The location channels take no data
+ *   gradient.  Their own workspace queries (0 for a refused shape).
+ * Every entry point: a null pointer, a size, l, k or s <= 0, or keep outside (0, 1] -> MAC_ERR_INVALID; an unknown form, l >
+ * 65536 or the image rules of mac_conv_bwd_tc -> MAC_ERR_UNSUPPORTED; pointers not 16-byte aligned -> MAC_ERR_ALIGN.  All
+ * checks precede any launch. */
+int mac_loc_cols_width(int l, int k);
+int mac_loc_cols(const float* grid, void* cols, int form, float keep, uint64_t seed, int site, int step, int B, int H, int W,
+                 int l, int k, int s, mac_stream_t stream);
+int mac_loc_cols_t(const float* grid, void* colsT, int split, float keep, uint64_t seed, int site, int step, int B, int H,
+                   int W, int l, int k, int s, mac_stream_t stream);
+int mac_linear_tc_fwd_acc(const void* x_bf16, const void* wt_bf16, int act, float* y, int M, int K, int n_out,
+                          mac_stream_t stream);
+int mac_linear_tc32_fwd_acc(const void* a_split, const void* wt3, int act, float* y, int M, int K, int n_out,
+                            mac_stream_t stream);
+int mac_conv_bwd_loc_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                        uint64_t seed, int site, int step, const float* grid, int l, int loc_site, float* dkernel, float* dwloc,
+                        float* dbias, float* dx, void* workspace, size_t workspace_bytes, int B, int H, int W, int C, int Cout,
+                        int k, int s, mac_stream_t stream);
+size_t mac_conv_bwd_loc_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int l, int k, int s, int with_dx);
+int mac_conv_bwd_loc_tc32(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                          uint64_t seed, int site, int step, const float* grid, int l, int loc_site, float* dkernel,
+                          float* dwloc, float* dbias, float* dx, void* workspace, size_t workspace_bytes, int B, int H, int W,
+                          int C, int Cout, int k, int s, mac_stream_t stream);
+size_t mac_conv_bwd_loc_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int l, int k, int s, int with_dx);
 
 /* ------------------------------------------------------------------------------------------------
  * Question input unit ("next" row, model.py:208-220, 279-307; ops.py:859-905): embedding lookup + bi-LSTM encoder.

@@ -149,6 +149,17 @@ PROTOTYPES = {
     "mac_conv_bwd_tc32": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_fp, c_fp, c_fp, c_sz]
                           + [c_int] * 7 + [c_fp]),
     "mac_conv_bwd_tc32_workspace_bytes": (c_sz, [c_int] * 8),
+    "mac_loc_cols_width": (c_int, [c_int, c_int]),
+    "mac_loc_cols": (c_int, [c_fp, c_fp, c_int, c_f, c_u64] + [c_int] * 8 + [c_fp]),
+    "mac_loc_cols_t": (c_int, [c_fp, c_fp, c_int, c_f, c_u64] + [c_int] * 8 + [c_fp]),
+    "mac_linear_tc_fwd_acc": (c_int, [c_fp, c_fp, c_int, c_fp, c_int, c_int, c_int, c_fp]),
+    "mac_linear_tc32_fwd_acc": (c_int, [c_fp, c_fp, c_int, c_fp, c_int, c_int, c_int, c_fp]),
+    "mac_conv_bwd_loc_tc": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_int, c_int, c_fp, c_fp,
+                                    c_fp, c_fp, c_fp, c_sz] + [c_int] * 7 + [c_fp]),
+    "mac_conv_bwd_loc_tc_workspace_bytes": (c_sz, [c_int] * 9),
+    "mac_conv_bwd_loc_tc32": (c_int, [c_fp, c_fp, c_fp, c_fp, c_int, c_f, c_u64, c_int, c_int, c_fp, c_int, c_int, c_fp, c_fp,
+                                      c_fp, c_fp, c_fp, c_sz] + [c_int] * 7 + [c_fp]),
+    "mac_conv_bwd_loc_tc32_workspace_bytes": (c_sz, [c_int] * 9),
     "mac_pack_weight_bf16": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_split3": (c_int, [c_fp, c_fp, c_int, c_int, c_fp]),
     "mac_pack_weight_fp8": (c_int, [c_fp, c_fp, c_fp, c_int, c_int, c_fp]),

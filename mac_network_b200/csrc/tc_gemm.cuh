@@ -23,6 +23,8 @@
 //   TC_EPI_ACT_SPLIT  x = act(acc + b + addf[m,n]) (addf fp32, optional) -> bf16 hi at out0[m, n] and bf16 lo = x - hi at
 //                     out0[m, N + n] (ldo = 2N): the A operand of the next split-bf16 ("tc32") product; outf != NULL also
 //                     stores x in fp32 at outf[m * N + n] (the tc32 training forward's saved H, exactly as computed here)
+//   TC_EPI_F32_ADD act(acc + b + addf[m,n]) -> fp32 at outf, addf fp32 [M, ldaf] and possibly outf itself; no split-K
+//                  (the location-aware stem's layer 0: the image product added to the location product, stem.py)
 #pragma once
 #include "common.cuh"
 #include "tmap.cuh"
@@ -30,7 +32,8 @@
 
 namespace mac {
 
-enum { TC_EPI_P = 0, TC_EPI_ACT = 1, TC_EPI_LOGITS = 2, TC_EPI_F32 = 3, TC_EPI_ADDACT = 4, TC_EPI_ACT_SPLIT = 5 };
+enum { TC_EPI_P = 0, TC_EPI_ACT = 1, TC_EPI_LOGITS = 2, TC_EPI_F32 = 3, TC_EPI_ADDACT = 4, TC_EPI_ACT_SPLIT = 5,
+       TC_EPI_F32_ADD = 6 };
 
 struct TcGemmParams {
   int M, N, K;
@@ -41,7 +44,7 @@ struct TcGemmParams {
   __nv_bfloat16* out1;     // bf16 output 1 (P*y)
   float* outf;             // fp32 output (TC_EPI_F32)
   const __nv_bfloat16* add;   // TC_EPI_ADDACT: pre-activation addend [M, ldo]
-  const float* addf;          // TC_EPI_ACT_SPLIT: optional fp32 pre-activation addend [M, ldaf]
+  const float* addf;          // TC_EPI_ACT_SPLIT (optional), TC_EPI_F32_ADD: fp32 pre-activation addend [M, ldaf]
   int ldaf;
   int ldo;
   const float* y;          // [B, N] row scale for TC_EPI_P
@@ -341,6 +344,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
           }
           *reinterpret_cast<float2*>(outf_t + o) = v;
         }
+      } else if constexpr (EPI == TC_EPI_F32_ADD) {
+        if (row_ok) {                                       // addf may be outf itself: each element is read, then written
+          const float2 a = *reinterpret_cast<const float2*>(p.addf + (size_t)row * p.ldaf + n);
+          *reinterpret_cast<float2*>(p.outf + o) = make_float2(act_ct<ACT>(x0 + a.x), act_ct<ACT>(x1 + a.y));
+        }
       } else {  // TC_EPI_LOGITS
         const float2 cc = __ldg(reinterpret_cast<const float2*>(p.ctrl + (size_t)bidx * p.N + n));
         const float2 ww = make_float2(__ldg(p.wr + n), __ldg(p.wr + n + 1));
@@ -386,6 +394,14 @@ inline int tc_gemm_launch_t(const CUtensorMap& ma0, const CUtensorMap& ma1, cons
 
 inline int tc_gemm_dispatch(const CUtensorMap& ma0, const CUtensorMap& ma1, const CUtensorMap& mb,
                             const TcGemmParams& p, cudaStream_t stream) {
+  if (p.promote && p.epi == TC_EPI_F32_ADD) {
+    switch (p.act) {
+      case MAC_ACT_NON: return tc_gemm_launch_t<TC_EPI_F32_ADD, MAC_ACT_NON, false, true>(ma0, ma1, mb, p, stream);
+      case MAC_ACT_ELU: return tc_gemm_launch_t<TC_EPI_F32_ADD, MAC_ACT_ELU, false, true>(ma0, ma1, mb, p, stream);
+      case MAC_ACT_RELU: return tc_gemm_launch_t<TC_EPI_F32_ADD, MAC_ACT_RELU, false, true>(ma0, ma1, mb, p, stream);
+    }
+    return MAC_ERR_UNSUPPORTED;
+  }
   if (p.promote) {
     if (p.epi != TC_EPI_F32) return MAC_ERR_UNSUPPORTED;
     switch (p.act) {
@@ -414,6 +430,14 @@ inline int tc_gemm_dispatch(const CUtensorMap& ma0, const CUtensorMap& ma1, cons
     case TC_EPI_ACT:
       if (p.act == MAC_ACT_ELU) return tc_gemm_launch_t<TC_EPI_ACT, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
       if (p.act == MAC_ACT_NON) return tc_gemm_launch_t<TC_EPI_ACT, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
+      return MAC_ERR_UNSUPPORTED;
+    case TC_EPI_F32_ADD:
+      if (p.ksplit > 1) return MAC_ERR_UNSUPPORTED;
+      switch (p.act) {
+        case MAC_ACT_NON: return tc_gemm_launch_t<TC_EPI_F32_ADD, MAC_ACT_NON>(ma0, ma1, mb, p, stream);
+        case MAC_ACT_ELU: return tc_gemm_launch_t<TC_EPI_F32_ADD, MAC_ACT_ELU>(ma0, ma1, mb, p, stream);
+        case MAC_ACT_RELU: return tc_gemm_launch_t<TC_EPI_F32_ADD, MAC_ACT_RELU>(ma0, ma1, mb, p, stream);
+      }
       return MAC_ERR_UNSUPPORTED;
     case TC_EPI_F32:
       switch (p.act) {

@@ -352,6 +352,37 @@ extern "C" int mac_linear_tc_fwd(const void* x_bf16, const void* wt_bf16, const 
   return tc_gemm_launch(x_bf16, K, nullptr, 0, wt_bf16, p, stream);
 }
 
+// y = act(x @ W + y) in place (TC_EPI_F32_ADD): the second product of a sum of two GEMMs, the first written by
+// mac_linear_tc_fwd / mac_linear_tc32_fwd with act NON and fp32 out
+extern "C" int mac_linear_tc_fwd_acc(const void* x_bf16, const void* wt_bf16, int act, float* y, int M, int K, int n_out,
+                                     mac_stream_t stream_) {
+  if (!x_bf16 || !wt_bf16 || !y || M <= 0 || K <= 0 || n_out <= 0) return MAC_ERR_INVALID;
+  if ((K % TC_BK) || (n_out % TC_BN) || (act != MAC_ACT_NON && act != MAC_ACT_ELU && act != MAC_ACT_RELU))
+    return MAC_ERR_UNSUPPORTED;
+  if ((M + TC_BM - 1) / TC_BM > 65535) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(x_bf16) || !mac_aligned16(wt_bf16) || !mac_aligned16(y)) return MAC_ERR_ALIGN;
+  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
+  TcGemmParams p{};
+  p.M = M; p.N = n_out; p.act = act; p.ldo = n_out; p.rows_per_batch = 1;
+  p.epi = TC_EPI_F32_ADD; p.outf = y; p.addf = y; p.ldaf = n_out;
+  return tc_gemm_launch(x_bf16, K, nullptr, 0, wt_bf16, p, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int mac_linear_tc32_fwd_acc(const void* a_split, const void* wt3, int act, float* y, int M, int K, int n_out,
+                                       mac_stream_t stream_) {
+  if (!a_split || !wt3 || !y || M <= 0 || K <= 0 || n_out <= 0) return MAC_ERR_INVALID;
+  if ((K % TC_BK) || (n_out % TC_BN) || (act != MAC_ACT_NON && act != MAC_ACT_ELU && act != MAC_ACT_RELU))
+    return MAC_ERR_UNSUPPORTED;
+  if ((M + TC_BM - 1) / TC_BM > 65535) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(a_split) || !mac_aligned16(wt3) || !mac_aligned16(y)) return MAC_ERR_ALIGN;
+  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
+  TcGemmParams p{};
+  p.M = M; p.N = n_out; p.act = act; p.ldo = n_out; p.rows_per_batch = 1;
+  p.epi = TC_EPI_F32_ADD; p.outf = y; p.addf = y; p.ldaf = n_out;
+  p.promote = 1;            // as mac_linear_tc32_fwd
+  return tc3_gemm(a_split, K, wt3, p, reinterpret_cast<cudaStream_t>(stream_));
+}
+
 extern "C" int mac_pack_weight_bf16_split(const float* W, void* hi_bf16, void* lo_bf16, int K, int N, mac_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!W || !hi_bf16 || !lo_bf16 || K <= 0 || N <= 0) return MAC_ERR_INVALID;
@@ -1049,6 +1080,126 @@ extern "C" int mac_col2im(const float* dcols, float* dx, float keep, uint64_t se
   return MAC_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ stem: location features
+// --locationAware (ops.py:448-559, mod CNCT): layer 0 reads concat(x, g) with the constant grid g [H, W, l].  Its patch matrix
+// splits into the image patches P (mac_im2col / mac_im2col3x3, unchanged) and the location patches Q [M, Kq], tap-major and
+// channel fastest as P, Kq = k^2 l rounded up to 128 (one wgmma tile of tc_wgrad_splitk), the columns k^2 l..Kq-1 zero.  The
+// dropout of the location channels is a Philox stream of its own (site): the draw of Q[m, tap l + j] is component e & 3
+// of philox4x32_10(seed, e >> 2, site, step) with e = ((b H + hs) W + ws) l + j the NHWC flat index of the [B, H, W, l]
+// location tensor at the source pixel (hs, ws), so every tap copy of an element shares its draw.
+namespace mac {
+inline int loc_width(int l, int k) { return (k * k * l + 127) / 128 * 128; }
+
+__device__ __forceinline__ float loc_value(const float* __restrict__ grid, const ConvGeom& g, int Kl, long long m, int col,
+                                           uint32_t thresh, float scale, uint64_t seed, int site, int step) {
+  if (m >= (long long)g.B * g.Ho * g.Wo || col >= Kl) return 0.f;
+  const int tap = col / g.C, j = col - tap * g.C;
+  const int wo = (int)(m % g.Wo);
+  const long long r = m / g.Wo;
+  const int ho = (int)(r % g.Ho), b = (int)(r / g.Ho);
+  const int hs = ho * g.s - g.pt + tap / g.k, ws = wo * g.s - g.pl + tap % g.k;
+  if (hs < 0 || hs >= g.H || ws < 0 || ws >= g.W) return 0.f;
+  float v = __ldg(grid + ((long long)hs * g.W + ws) * g.C + j);
+  if (thresh) {
+    const long long e = (((long long)b * g.H + hs) * g.W + ws) * g.C + j;
+    const Philox4 p = philox4x32_10(seed, (uint64_t)e >> 2, (uint32_t)site, (uint32_t)step);
+    const uint32_t u = (e & 3) == 0 ? p.x : (e & 3) == 1 ? p.y : (e & 3) == 2 ? p.z : p.w;
+    v = (u >> 8) >= thresh ? v * scale : 0.f;
+  }
+  return v;
+}
+
+// One element per thread (Q is small: k^2 l columns against the image's k^2 C).  TRANS = false: Q [M, Kq] in fp32 (FORM 0),
+// bf16 (1) or [hi | lo] [M, 2 Kq] (2).  TRANS = true: Q^T [Kq, Mp] (FORM 1) or [Kq, 2 Mp] = [hi | lo] (FORM 2), the weight
+// gradient's operand, zero in columns M..Mp-1.  g.C is l.
+template <int FORM, bool TRANS>
+__global__ void __launch_bounds__(256) loc_cols_kernel(const float* __restrict__ grid, void* __restrict__ out, uint32_t thresh,
+                                                       float scale, uint64_t seed, int site, int step, ConvGeom g, int Kq,
+                                                       int Mp) {
+  const long long rows = TRANS ? (long long)Kq : (long long)g.B * g.Ho * g.Wo, cols = TRANS ? (long long)Mp : (long long)Kq;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * cols) return;
+  const long long r = i / cols, c = i - r * cols;
+  const long long m = TRANS ? c : r;
+  const int col = (int)(TRANS ? r : c);
+  const float v = loc_value(grid, g, g.k * g.k * g.C, m, col, thresh, scale, seed, site, step);
+  if constexpr (FORM == 0) {
+    reinterpret_cast<float*>(out)[i] = v;
+  } else {
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+    if constexpr (FORM == 1) {
+      o[i] = hi;
+    } else {
+      const long long at = r * 2 * cols + c;
+      o[at] = hi;
+      o[at + cols] = __float2bfloat16_rn(v - __bfloat162float(hi));
+    }
+  }
+}
+
+// The refusals of every location entry point after its own pointer checks: l, B, H, W, k, s, keep and the row bounds.
+inline int loc_check(int B, int H, int W, int l, int k, int s, float keep) {
+  if (l <= 0) return MAC_ERR_INVALID;
+  const int st = conv_geom_check(B, H, W, l, k, s, keep);
+  if (st != MAC_OK) return st;
+  if (l > 65536) return MAC_ERR_UNSUPPORTED;
+  const ConvGeom g = conv_geom(B, H, W, l, k, s);
+  const long long Mp = ((long long)B * g.Ho * g.Wo + 63) & ~63LL;
+  if (Mp * loc_width(l, k) >= (1LL << 39)) return MAC_ERR_UNSUPPORTED;     // one thread per element, 256 per block
+  return MAC_OK;
+}
+
+inline void loc_cols_launch(const float* grid, void* out, int form, bool trans, float keep, uint64_t seed, int site, int step,
+                            const ConvGeom& g, cudaStream_t stream) {
+  const int Kq = loc_width(g.C, g.k);
+  const long long M = (long long)g.B * g.Ho * g.Wo;
+  const int Mp = (int)((M + 63) & ~63LL);
+  const uint32_t thr = keep < 1.f ? keep_threshold(keep) : 0u;
+  const float scale = keep < 1.f ? 1.f / keep : 1.f;
+  const long long n = (trans ? (long long)Mp : M) * Kq;
+  const unsigned blocks = (unsigned)((n + 255) / 256);
+  if (trans && form == MAC_COLS_SPLIT)
+    loc_cols_kernel<2, true><<<blocks, 256, 0, stream>>>(grid, out, thr, scale, seed, site, step, g, Kq, Mp);
+  else if (trans)
+    loc_cols_kernel<1, true><<<blocks, 256, 0, stream>>>(grid, out, thr, scale, seed, site, step, g, Kq, Mp);
+  else if (form == MAC_COLS_F32)
+    loc_cols_kernel<0, false><<<blocks, 256, 0, stream>>>(grid, out, thr, scale, seed, site, step, g, Kq, Mp);
+  else if (form == MAC_COLS_BF16)
+    loc_cols_kernel<1, false><<<blocks, 256, 0, stream>>>(grid, out, thr, scale, seed, site, step, g, Kq, Mp);
+  else
+    loc_cols_kernel<2, false><<<blocks, 256, 0, stream>>>(grid, out, thr, scale, seed, site, step, g, Kq, Mp);
+}
+}  // namespace mac
+
+extern "C" int mac_loc_cols_width(int l, int k) { return l <= 0 || k <= 0 || k > CONV_MAX_K ? 0 : loc_width(l, k); }
+
+extern "C" int mac_loc_cols(const float* grid, void* cols, int form, float keep, uint64_t seed, int site, int step, int B, int H,
+                            int W, int l, int k, int s, mac_stream_t stream_) {
+  if (!grid || !cols) return MAC_ERR_INVALID;
+  const int st = loc_check(B, H, W, l, k, s, keep);
+  if (st != MAC_OK) return st;
+  if (form != MAC_COLS_F32 && form != MAC_COLS_BF16 && form != MAC_COLS_SPLIT) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(grid) || !mac_aligned16(cols)) return MAC_ERR_ALIGN;
+  loc_cols_launch(grid, cols, form, false, keep, seed, site, step, conv_geom(B, H, W, l, k, s),
+                  reinterpret_cast<cudaStream_t>(stream_));
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
+extern "C" int mac_loc_cols_t(const float* grid, void* colsT, int split, float keep, uint64_t seed, int site, int step, int B,
+                              int H, int W, int l, int k, int s, mac_stream_t stream_) {
+  if (!grid || !colsT) return MAC_ERR_INVALID;
+  const int st = loc_check(B, H, W, l, k, s, keep);
+  if (st != MAC_OK) return st;
+  if (split != 0 && split != 1) return MAC_ERR_UNSUPPORTED;
+  if (!mac_aligned16(grid) || !mac_aligned16(colsT)) return MAC_ERR_ALIGN;
+  loc_cols_launch(grid, colsT, split ? MAC_COLS_SPLIT : MAC_COLS_BF16, true, keep, seed, site, step,
+                  conv_geom(B, H, W, l, k, s), reinterpret_cast<cudaStream_t>(stream_));
+  MAC_LAUNCH_CHECK();
+  return MAC_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ stem: backward on wgmma
 // One 3x3 convolution layer's backward with its two GEMMs on tensor cores (fp32 accumulation, fp32 element-wise work),
 // M = B*H*W rows, Mp = M rounded up to the 64-row k-block of the weight gradient.  mac_conv3x3_bwd_tc (bf16 operands):
@@ -1221,9 +1372,11 @@ inline bool im2col_t_grid_ok(int k, int C) { return (long long)k * k * C / 64 <=
 // workspace of mac_conv3x3_bwd_tc / _tc32: 1 KB-aligned slabs behind a 1 KB alignment slack.  `split`: the bf16 operands
 // carry 2 (dz rows, colsT) or 3 (dzT, kernel) segments, and the weight gradient contracts over 3 Mp.
 struct ConvBwdLayout {
-  size_t dz, dzT, colsT, bpart, wpart, k16, dcols, total;
+  size_t dz, dzT, colsT, bpart, wpart, k16, dcols, qT, qpart, total;
 };
-inline ConvBwdLayout conv_bwd_layout(const ConvGeom& g, int Cout, bool with_dx, bool split) {
+// `l` > 0: the location-aware layer 0 (mac_conv_bwd_loc_tc / _tc32) also holds Q^T [Kq, Mp] (split: [Kq, 2 Mp]) and the
+// split-K partials of dW_loc, after every slab of the location-free layout
+inline ConvBwdLayout conv_bwd_layout(const ConvGeom& g, int Cout, bool with_dx, bool split, int l_ = 0) {
   auto al = [](size_t v) { return (v + 1023) & ~(size_t)1023; };
   const size_t M = (size_t)g.B * g.Ho * g.Wo, Mp = (M + 63) & ~(size_t)63, K = (size_t)g.k * g.k * g.C;
   const size_t s2 = split ? 2 : 1, s3 = split ? 3 : 1;
@@ -1241,27 +1394,48 @@ inline ConvBwdLayout conv_bwd_layout(const ConvGeom& g, int Cout, bool with_dx, 
     o += al(K * Cout * 2 * s3);
     l.dcols = o; o += al(M * K * 4);
   }
+  l.qT = l.qpart = o;
+  if (l_ > 0) {
+    const size_t Kq = (size_t)loc_width(l_, g.k);
+    const int Sq = tc_pick_ksplit((int)(s3 * Mp), (int)(Kq / TC_BM) * (Cout / TC_BN));
+    o += al(Kq * Mp * 2 * s2);
+    l.qpart = o; o += al((size_t)Sq * Kq * Cout * 4);
+  }
   l.total = o + 1024;
   return l;
 }
 
-// k = 3, s = 1 runs the 3x3 kernels (im2col3x3_t_kernel, mac_col2im3x3), every other geometry the general ones.
+// The location half of a location-aware layer 0: grid [H, W, l], its dropout site, and dW_loc [Kq, Cout] (+=).
+struct ConvBwdLoc {
+  const float* grid;
+  int l, site;
+  float* dwloc;
+};
+
+// k = 3, s = 1 runs the 3x3 kernels (im2col3x3_t_kernel, mac_col2im3x3), every other geometry the general ones.  With `loc`,
+// the same schedule then adds dW_loc += Q^T dZ from the same dZ^T.
 static int conv_bwd_wgmma(bool split, const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
                           uint64_t seed, int site, int step, float* dkernel, float* dbias, float* dx, void* workspace,
-                          size_t workspace_bytes, int B, int H, int W, int C, int Cout, int k, int s, mac_stream_t stream_) {
+                          size_t workspace_bytes, int B, int H, int W, int C, int Cout, int k, int s, mac_stream_t stream_,
+                          const ConvBwdLoc* loc = nullptr) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x || !y || !dy || !kernel || !dkernel || !dbias || !workspace) return MAC_ERR_INVALID;
+  if (loc && (!loc->grid || !loc->dwloc)) return MAC_ERR_INVALID;
   if (Cout <= 0) return MAC_ERR_INVALID;
   const int gst = conv_geom_check(B, H, W, C, k, s, keep);
   if (gst != MAC_OK) return gst;
+  if (loc) {
+    const int lst = loc_check(B, H, W, loc->l, k, s, keep);
+    if (lst != MAC_OK) return lst;
+  }
   if ((C % 128) || (Cout % 128)) return MAC_ERR_UNSUPPORTED;     // wgmma tiles: k^2 C and Cout are GEMM N / M extents
   if (!im2col_t_grid_ok(k, C)) return MAC_ERR_UNSUPPORTED;
   if (!mac_aligned16(x) || !mac_aligned16(y) || !mac_aligned16(dy) || !mac_aligned16(kernel) || !mac_aligned16(dkernel) ||
-      (dx && !mac_aligned16(dx)))
+      (dx && !mac_aligned16(dx)) || (loc && (!mac_aligned16(loc->grid) || !mac_aligned16(loc->dwloc))))
     return MAC_ERR_ALIGN;
   const ConvGeom g = conv_geom(B, H, W, C, k, s);
   const bool k3s1 = k == 3 && s == 1;
-  const ConvBwdLayout l = conv_bwd_layout(g, Cout, dx != nullptr, split);
+  const ConvBwdLayout l = conv_bwd_layout(g, Cout, dx != nullptr, split, loc ? loc->l : 0);
   if (workspace_bytes < l.total) return MAC_ERR_WORKSPACE;
   if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
   const int M = B * g.Ho * g.Wo, Mp = (M + 63) & ~63, K = k * k * C;
@@ -1294,7 +1468,19 @@ static int conv_bwd_wgmma(bool split, const float* x, const float* y, const floa
   if (st != MAC_OK) return st;
   st = split ? tc3_wgrad_splitk(colsT, dzT, dkernel, wpart, K, Cout, Mp, stream)
              : tc_wgrad_splitk(colsT, dzT, dkernel, wpart, K, Cout, Mp, stream);
-  if (st != MAC_OK || !dx) return st;
+  if (st != MAC_OK) return st;
+  if (loc) {                                                    // dW_loc += Q^T dZ on the same dZ^T
+    void* qT = base + l.qT;
+    float* qpart = reinterpret_cast<float*>(base + l.qpart);
+    const int Kq = loc_width(loc->l, k);
+    loc_cols_launch(loc->grid, qT, split ? MAC_COLS_SPLIT : MAC_COLS_BF16, true, keep, seed, loc->site, step,
+                    conv_geom(B, H, W, loc->l, k, s), stream);
+    MAC_LAUNCH_CHECK();
+    st = split ? tc3_wgrad_splitk(qT, dzT, loc->dwloc, qpart, Kq, Cout, Mp, stream)
+               : tc_wgrad_splitk(qT, dzT, loc->dwloc, qpart, Kq, Cout, Mp, stream);
+    if (st != MAC_OK) return st;
+  }
+  if (!dx) return MAC_OK;
   void* k16 = base + l.k16;                                     // the kernel in its own [9C, Cout] layout: K-major B operand
   float* dcols = reinterpret_cast<float*>(base + l.dcols);
   if (split) {
@@ -1382,4 +1568,39 @@ extern "C" int mac_conv3x3_bwd_tc32(const float* x, const float* y, const float*
                                     size_t workspace_bytes, int B, int H, int W, int C, int Cout, mac_stream_t stream_) {
   return conv_bwd_wgmma(true, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
                         B, H, W, C, Cout, 3, 1, stream_);
+}
+
+// The location-aware layer 0 (--locationAware): mac_conv_bwd_tc / _tc32 of the image half (kernel and dkernel are the image
+// rows [k^2 C, Cout]), then dW_loc [Kq, Cout] += Q^T dZ.  The location channels take no data gradient.
+extern "C" size_t mac_conv_bwd_loc_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int l, int k, int s, int with_dx) {
+  if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C) ||
+      loc_check(B, H, W, l, k, s, 1.f) != MAC_OK)
+    return 0;
+  return conv_bwd_layout(conv_geom(B, H, W, C, k, s), Cout, with_dx != 0, false, l).total;
+}
+
+extern "C" int mac_conv_bwd_loc_tc(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                                   uint64_t seed, int site, int step, const float* grid, int l, int loc_site, float* dkernel,
+                                   float* dwloc, float* dbias, float* dx, void* workspace, size_t workspace_bytes, int B,
+                                   int H, int W, int C, int Cout, int k, int s, mac_stream_t stream_) {
+  const ConvBwdLoc loc{grid, l, loc_site, dwloc};
+  return conv_bwd_wgmma(false, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
+                        B, H, W, C, Cout, k, s, stream_, &loc);
+}
+
+extern "C" size_t mac_conv_bwd_loc_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int l, int k, int s,
+                                                        int with_dx) {
+  if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C) ||
+      loc_check(B, H, W, l, k, s, 1.f) != MAC_OK)
+    return 0;
+  return conv_bwd_layout(conv_geom(B, H, W, C, k, s), Cout, with_dx != 0, true, l).total;
+}
+
+extern "C" int mac_conv_bwd_loc_tc32(const float* x, const float* y, const float* dy, const float* kernel, int act, float keep,
+                                     uint64_t seed, int site, int step, const float* grid, int l, int loc_site, float* dkernel,
+                                     float* dwloc, float* dbias, float* dx, void* workspace, size_t workspace_bytes, int B,
+                                     int H, int W, int C, int Cout, int k, int s, mac_stream_t stream_) {
+  const ConvBwdLoc loc{grid, l, loc_site, dwloc};
+  return conv_bwd_wgmma(true, x, y, dy, kernel, act, keep, seed, site, step, dkernel, dbias, dx, workspace, workspace_bytes,
+                        B, H, W, C, Cout, k, s, stream_, &loc);
 }

@@ -55,13 +55,16 @@ def check_model_precisions(cfg, encoder, stem, stem_prec, enc_prec):
                                       % cfg.ctrlDim)
 
 
-STEM_GEOMETRY = {"ksizes": None, "strides": None, "linear": False, "stem_dim": None}
+STEM_GEOMETRY = {"ksizes": None, "strides": None, "linear": False, "stem_dim": None, "location": None, "location_bias": 1.0,
+                 "location_dim": 32}
 
 
 def stem_geometry(stem):
     """The geometry of `stem=(imageInDim, stemNumLayers[, geometry])`: a dict with the keys of STEM_GEOMETRY --
     `ksizes` (--stemKernelSizes, one kernel size per layer; None: 3x3), `strides` (--stemStrideSizes; None: 1),
-    `linear` (--stemLinear) and `stem_dim` (--stemDim; None: memDim) -- defaults filled in."""
+    `linear` (--stemLinear), `stem_dim` (--stemDim; None: memDim) and `location`, `location_bias`, `location_dim`
+    (--locationAware with --locationType "L" or "PE", --locationBias, --locationDim; None: off) -- defaults filled in.
+    Location features with the linear stem, an unknown type, a dim < 1 or a non-finite bias raise ValueError."""
     geom = dict(STEM_GEOMETRY)
     extra = dict(stem[2]) if len(stem) > 2 and stem[2] is not None else {}
     unknown = sorted(set(extra) - set(geom))
@@ -71,7 +74,18 @@ def stem_geometry(stem):
     if geom["linear"] and (geom["ksizes"] is not None or geom["stem_dim"] is not None
                            or geom["strides"] not in (None, [1], (1,))):
         raise ValueError("the linear stem is one 1x1 stride-1 layer: it takes no ksizes, strides or stem_dim, got %s" % extra)
+    if geom["location"] is not None and geom["linear"]:
+        raise ValueError("the linear stem takes no location features (the reference adds them in the CNN stem only)")
+    stem_location(geom)
     return geom
+
+
+def stem_location(geom):
+    """The `Stem(location=)` of a filled-in geometry: None or the checked (type, bias, dim)."""
+    from .stem import location_spec
+    if geom["location"] is None:
+        return None
+    return location_spec((geom["location"], geom["location_bias"], geom["location_dim"]))
 
 
 def model_parameters(cfg, netLength, seed, classifier=None, encoder=None, stem=None, param_values=None):
@@ -94,7 +108,7 @@ def model_parameters(cfg, netLength, seed, classifier=None, encoder=None, stem=N
         enc_specs = encoder_specs(encoder[0], encoder[1], cfg.ctrlDim, ctrl_dim=cfg.ctrlDim, bi=True)
         geom = stem_geometry(stem)
         stem_specs_ = stem_specs(stem[0], cfg.memDim, num_layers=stem[1], ksizes=geom["ksizes"], stem_dim=geom["stem_dim"],
-                                 linear=geom["linear"])
+                                 linear=geom["linear"], location=stem_location(geom))
         extra_specs = collections.OrderedDict(list(extra_specs.items()) + list(enc_specs.items())
                                               + list(stem_specs_.items()))
         extra_values = dict(extra_values)
@@ -158,7 +172,8 @@ class DPTrainer(object):
                                        version=lambda: self.params.version)
             geom = self.stem_geometry = stem_geometry(stem)
             self.stem = Stem({k: self.params.t[k] for k in self._stem_specs}, relu=cfg.relu, prec=stem_prec, seed=seed,
-                             version=lambda: self.params.version, strides=geom["strides"], linear=geom["linear"])
+                             version=lambda: self.params.version, strides=geom["strides"], linear=geom["linear"],
+                             location=stem_location(geom))
             self.stem_dropout = float(stem_dropout)
             self._full_bufs = {}
         n = self.params.numel

@@ -35,7 +35,8 @@ class MACnet(object):
     def __init__(self, cfg, netLength, vocab, n_answers, wrd_emb_dim=300, image_in_dim=1024, classifier_dims=(512,),
                  stem_layers=2, seed=0, rank=0, world=1, lr=1e-4, prec="bf16", use_ema=False, answer_decoder=None,
                  device="cuda", eval_stem_prec=None, eval_enc_prec=None, train_prec="fp32", stem_kernel_sizes=None,
-                 stem_strides=None, stem_linear=False, stem_dim=None, **trainer_kw):
+                 stem_strides=None, stem_linear=False, stem_dim=None, stem_location=None, stem_location_bias=1.0,
+                 stem_location_dim=32, **trainer_kw):
         """`vocab`: rows of the question-embedding variable (ids 1..vocab; 0 is padding); `answer_decoder`: optional
         id -> answer string (`answerDict.decodeId`, model.py:699).  `prec`: arithmetic of the evaluation forward; with
         "fp8" the cell's read step runs on e4m3 and the image stem in bf16.  `eval_stem_prec="fp8"` runs the evaluation
@@ -46,13 +47,16 @@ class MACnet(object):
         "bf16" or "tc32"); the other training precisions pass through as `DPTrainer` keywords (`bwd_tc`, `stem_prec`,
         `enc_prec`).  `stem_kernel_sizes`, `stem_strides`, `stem_linear` and `stem_dim` are the reference's
         --stemKernelSizes, --stemStrideSizes, --stemLinear and --stemDim (`dp.stem_geometry`); the knowledge base then has
-        the stem's output grid (`Stem.grid`)."""
+        the stem's output grid (`Stem.grid`).  `stem_location` ("L" or "PE"; None: off), `stem_location_bias` and
+        `stem_location_dim` are --locationAware with --locationType, --locationBias and --locationDim."""
         if eval_stem_prec not in (None, "fp8", "bf16x3"):
             raise ValueError("eval_stem_prec must be None, 'fp8' or 'bf16x3', got %r" % (eval_stem_prec,))
         if eval_enc_prec not in (None, "bf16"):
             raise ValueError("eval_enc_prec must be None or 'bf16', got %r" % (eval_enc_prec,))
         default_geometry = not stem_linear and all(int(k) == 3 for k in (stem_kernel_sizes or [3])) and \
             all(int(s) == 1 for s in (stem_strides or [1]))
+        if eval_stem_prec == "fp8" and stem_location is not None:
+            raise NotImplementedError("the fp8 stem does not run location features; use eval_stem_prec=None or 'bf16x3'")
         if eval_stem_prec == "fp8" and not default_geometry:
             raise NotImplementedError("the fp8 stem runs the 3x3 stride-1 geometry only, got kernel sizes %s, strides %s%s"
                                       % (stem_kernel_sizes, stem_strides, ", linear" if stem_linear else ""))
@@ -61,7 +65,10 @@ class MACnet(object):
         self.trainer = DPTrainer(cfg, netLength, seed=seed, rank=rank, world=world, lr=lr, device=device,
                                  classifier=(n_answers, list(classifier_dims)), encoder=(vocab, wrd_emb_dim),
                                  stem=(image_in_dim, stem_layers, {"ksizes": stem_kernel_sizes, "strides": stem_strides,
-                                                                   "linear": stem_linear, "stem_dim": stem_dim}),
+                                                                   "linear": stem_linear, "stem_dim": stem_dim,
+                                                                   "location": stem_location,
+                                                                   "location_bias": stem_location_bias,
+                                                                   "location_dim": stem_location_dim}),
                                  prec=train_prec, **trainer_kw)
         p = self.trainer.params
         t = self.trainer
@@ -70,7 +77,7 @@ class MACnet(object):
                                     prec=eval_enc_prec or "fp32", version=lambda: p.version)
         stem_prec = eval_stem_prec or ("bf16" if prec == "fp8" else prec)
         self._stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=stem_prec, version=lambda: p.version,
-                          strides=t.stem.strides, linear=t.stem.linear)
+                          strides=t.stem.strides, linear=t.stem.linear, location=t.stem.location)
         self._out = OutputUnit({k: p.t[k] for k in p.specs if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu,
                                keep=1.0, version=lambda: p.version)
         self.device = p.device

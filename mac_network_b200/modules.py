@@ -432,15 +432,16 @@ class ImageStem(_KernelModule):
     knowledge base [B, Ho*Wo, out_dim] on the stem's output grid (`grid`).  The gradient w.r.t. the images is computed
     exactly when they require grad, and comes back in their dtype.  `prec`: "fp32", "bf16" or "bf16x3" (training and
     inference) or "fp8" (inference).  `ksizes`, `strides`, `linear`, `stem_dim`: the reference's --stemKernelSizes,
-    --stemStrideSizes, --stemLinear and --stemDim."""
+    --stemStrideSizes, --stemLinear and --stemDim; `location`: --locationAware as `Stem(location=)` takes it."""
 
     def __init__(self, in_dim, out_dim, num_layers=2, relu="ELU", prec="fp32", values=None, seed=0, device="cuda",
-                 ksizes=None, strides=None, linear=False, stem_dim=None):
+                 ksizes=None, strides=None, linear=False, stem_dim=None, location=None):
         super(ImageStem, self).__init__()
-        specs = stem_specs(in_dim, out_dim, num_layers=num_layers, ksizes=ksizes, linear=linear, stem_dim=stem_dim)
+        specs = stem_specs(in_dim, out_dim, num_layers=num_layers, ksizes=ksizes, linear=linear, stem_dim=stem_dim,
+                           location=location)
         values = values if values is not None else init_stem_params(specs, seed=seed + 23, bias_scale=0.0)
         self._register(_Params(specs, values, device), seed)
-        self._stem = _stem_unit(self.params, relu, prec, {"strides": strides, "linear": linear})
+        self._stem = _stem_unit(self.params, relu, prec, {"strides": strides, "linear": linear, "location": location})
         self._stem_names, self.stem_keep = list(specs), STEM_KEEP
 
     def forward(self, images=None, images_nchw=None):
@@ -453,7 +454,8 @@ class ImageStem(_KernelModule):
 
 def _stem_unit(params, relu, prec, geometry):
     return Stem({k: params.t[k] for k in params.t if k.startswith("stem/")}, relu=relu, prec=prec,
-                version=lambda: params.version, strides=geometry["strides"], linear=geometry["linear"])
+                version=lambda: params.version, strides=geometry["strides"], linear=geometry["linear"],
+                location=geometry["location"])
 
 
 def _pick_images(images, images_nchw):
@@ -508,7 +510,7 @@ class MACModel(_KernelModule):
                  stem_layers=2, prec="fp32", bwd_tc=False, stem_prec="fp32", enc_prec="fp32", eval_prec=None, values=None,
                  seed=0, device="cuda", stem_geometry=None):
         super(MACModel, self).__init__()
-        from .dp import check_model_precisions, model_parameters, stem_geometry as stem_geometry_of
+        from .dp import check_model_precisions, model_parameters, stem_geometry as stem_geometry_of, stem_location
         if not cfg.controlContextual:
             raise NotImplementedError("the raw-word control inputs (controlContextual off) need wrdEmbDim == ctrlDim")
         encoder, stem = (vocab, wrd_emb_dim), (image_in_dim, stem_layers, stem_geometry)
@@ -524,7 +526,8 @@ class MACModel(_KernelModule):
         self._enc_names, self._stem_names = list(enc_specs), list(stem_specs_)
         self._out_names = [k for k in extra_specs if k.startswith(("outputUnit/", "classifier/"))]
         self._enc = _encoder_units(self.params, enc_prec)
-        self._stem = _stem_unit(self.params, cfg.relu, stem_prec, stem_geometry_of(stem))
+        geom = stem_geometry_of(stem)
+        self._stem = _stem_unit(self.params, cfg.relu, stem_prec, dict(geom, location=stem_location(geom)))
         self._out = _output_unit(self.params, cfg.relu)
         self.stem_keep = STEM_KEEP
         self.cells = _Cells(cfg, netLength, self.params, prec, bwd_tc, eval_prec,

@@ -398,7 +398,7 @@ class _ModelSlot(object):
         self.enc = QuestionEncoder({k: p.t[k] for k in t._enc_specs}, keep_input=1.0, keep_question=1.0,
                                    prec=model._enc.prec, version=version)
         self.stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=model._stem.prec, version=version,
-                         strides=model._stem.strides, linear=model._stem.linear)
+                         strides=model._stem.strides, linear=model._stem.linear, location=model._stem.location)
         self.out = OutputUnit({k: p.t[k] for k in p.specs if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu,
                               keep=1.0, version=version)
         self.cell = None

@@ -16,7 +16,12 @@ Other geometries (--stemKernelSize(s), --stemStrideSizes, --stemLinear): a layer
 padding (`Ho = ceil(H / s)`, the odd padding row on the bottom / right); the linear stem is the layer (1, 1, NON, no
 dropout) on the `[inDim, outDim]` weight viewed as `[1, 1, inDim, outDim]`.  Layers with k = 3, s = 1 run the 3x3 kernels
 above; every other layer runs the general patch passes (`mac_im2col`, `mac_col2im`, `mac_conv_bwd_tc` / `_tc32`) with the
-same GEMMs.  The e4m3 stem keeps only the 3x3 stride-1 geometry."""
+same GEMMs.  The e4m3 stem keeps only the 3x3 stride-1 geometry.
+
+Location features (--locationAware, DESIGN.md "Location-aware stem"): layer 0 reads concat(x, g) with the constant grid
+g [H, W, l] (`location_grid`), as conv(x, K_img) + conv(g, K_loc).  The image half is the layer-0 path above, unchanged; the
+location half is the patch matrix Q [M, Kq] of g (`mac_loc_cols`, its own dropout site SITE_LOCATION) against W_loc, the
+kernel's location rows padded with zero rows to Kq = k^2 l rounded up to 128."""
 import collections
 
 import numpy as np
@@ -30,15 +35,61 @@ INGEST_NHWC_F32, INGEST_PATCH_BF16 = 0, 1       # enum MAC_INGEST_* (include/mac
 INGEST_COLS_BF16, INGEST_COLS_SPLIT = 0, 1      # enum MAC_INGEST_COLS_*
 COLS_F32, COLS_BF16, COLS_SPLIT = 0, 1, 2       # enum MAC_COLS_*
 LINEAR_W, LINEAR_B = "stem/linearLayer/weights/weight", "stem/linearLayer/biases/bias"
+SITE_LOCATION = 50        # Philox site of layer 0's location channels' dropout
 
 
-def stem_specs(in_dim, out_dim, num_layers=2, ksize=3, stem_dim=None, ksizes=None, linear=False):
+def location_spec(location):
+    """`location`: None, or (type, bias, dim) -- --locationType ("L" or "PE"), --locationBias, --locationDim -- or a bare
+    type with the reference's defaults (bias 1.0, dim 32).  Returns None or the checked (type, bias, dim)."""
+    if location is None:
+        return None
+    if isinstance(location, str):
+        location = (location, 1.0, 32)
+    kind, bias, dim = location
+    if kind not in ("L", "PE"):
+        raise ValueError("location type must be 'L' or 'PE', got %r" % (kind,))
+    if not np.isfinite(float(bias)):
+        raise ValueError("location bias must be finite, got %r" % (bias,))
+    if int(dim) != dim or int(dim) < 1:
+        raise ValueError("location dim must be a positive integer, got %r" % (dim,))
+    return kind, float(bias), int(dim)
+
+
+def location_channels(location):
+    """l, the location channels layer 0 reads after the image's: 2 for L, 4 dim for PE (ops.py:448-488)."""
+    loc = location_spec(location)
+    return 0 if loc is None else (2 if loc[0] == "L" else 4 * loc[2])
+
+
+def location_grid(location, H, W):
+    """The location grid [H, W, l] in fp64 (ops.py:448-488, addLocation's CNCT mode): x = linspace(-bias, bias, W)[w], y =
+    linspace(-bias, bias, H)[h] (TF's linspace of one point is [-bias]); L is [x, y]; PE is
+    [sin x_i | cos x_i | sin y_i | cos y_i] with x_i = x / 10000^(i / dim), i = 0 .. dim - 1."""
+    kind, bias, dim = location_spec(location)
+    lin = lambda n: np.linspace(-bias, bias, n) if n > 1 else np.array([-bias])
+    x = np.broadcast_to(lin(W)[None, :, None], (H, W, 1))
+    y = np.broadcast_to(lin(H)[:, None, None], (H, W, 1))
+    if kind == "L":
+        return np.concatenate([x, y], axis=-1)
+    f = np.power(10000.0, np.arange(dim) / float(dim))
+    return np.concatenate([np.sin(x / f), np.cos(x / f), np.sin(y / f), np.cos(y / f)], axis=-1)
+
+
+def location_width(l, k):
+    """Kq: the location patch matrix's width, k^2 l rounded up to the 128-wide wgmma tile (mac_loc_cols_width)."""
+    return -(-k * k * l // 128) * 128
+
+
+def stem_specs(in_dim, out_dim, num_layers=2, ksize=3, stem_dim=None, ksizes=None, linear=False, location=None):
     """The stem's variables as the reference names and shapes them (model.py:165-204): `--stemLinear` one `ops.linear`
     (`stem/linearLayer/weights/weight` [inDim, outDim] and its bias), else `num_layers` HWIO kernels
     `stem/cnnLayercnn_i/kernels/kernel` [k_i, k_i, Cin, Cout] of kernel size `ksizes[i]` (--stemKernelSizes) or `ksize`
-    (--stemKernelSize) for every layer."""
+    (--stemKernelSize) for every layer.  `location` (--locationAware, `location_spec`) gives layer 0 Cin = inDim + l and
+    creates no variable."""
     s = collections.OrderedDict()
     if linear:
+        if location is not None:
+            raise ValueError("the linear stem takes no location features (the reference adds them in the CNN stem only)")
         if ksizes is not None or stem_dim is not None:
             raise ValueError("the linear stem is one [inDim, outDim] layer: it takes no ksizes or stem_dim")
         s[LINEAR_W] = ((in_dim, out_dim), "xavier")
@@ -48,7 +99,7 @@ def stem_specs(in_dim, out_dim, num_layers=2, ksize=3, stem_dim=None, ksizes=Non
     ks = [ksize] * num_layers if ksizes is None else [int(k) for k in ksizes]
     if len(ks) != num_layers:
         raise ValueError("ksizes has %d entries for %d stem layers" % (len(ks), num_layers))
-    dims = [in_dim] + [stem_dim] * (num_layers - 1) + [out_dim]
+    dims = [in_dim + location_channels(location)] + [stem_dim] * (num_layers - 1) + [out_dim]
     for i in range(num_layers):
         s["stem/cnnLayercnn_%d/kernels/kernel" % i] = ((ks[i], ks[i], dims[i], dims[i + 1]), "xavier")
         s["stem/cnnLayercnn_%d/biases/bias" % i] = ((dims[i + 1],), "zeros")
@@ -82,12 +133,21 @@ def init_stem_params(specs, seed=0, dtype=np.float32, bias_scale=0.1):
 
 
 class Stem(object):
-    def __init__(self, params, relu="ELU", prec="fp32", seed=0, version=None, strides=None, linear=False):
+    def __init__(self, params, relu="ELU", prec="fp32", seed=0, version=None, strides=None, linear=False, location=None):
         """`params`: dict TF-name -> CUDA fp32 tensor (HWIO kernels, biases; or with `linear=True` the `stem/linearLayer`
         weight [inDim, outDim] and bias).  Each layer's kernel size is read from its kernel's shape; `strides`
         (--stemStrideSizes) gives one stride per layer, default 1.  `version`: optional callable returning a counter
         that changes whenever the parameter values do (`MACParams.version`): the packed bf16 / e4m3 kernels are rebuilt when it moves
-        (optimizer step, checkpoint restore, EMA swap -- ADVICE r1), whoever changed the values."""
+        (optimizer step, checkpoint restore, EMA swap -- ADVICE r1), whoever changed the values.  `location`
+        (--locationAware, `location_spec`): layer 0's kernel holds inDim + l input channels, the last l of them the location
+        grid's; not with the linear stem (ValueError) or prec="fp8" (NotImplementedError)."""
+        self.location = location_spec(location)
+        if self.location is not None and linear:
+            raise ValueError("the linear stem takes no location features (the reference adds them in the CNN stem only)")
+        if self.location is not None and prec == "fp8":
+            raise NotImplementedError("the fp8 stem does not run location features; use prec='bf16'")
+        self.nloc = location_channels(self.location)
+        self._grids = {}
         self.lib = _lib.load()
         self.p = params
         self.relu, self.prec, self.seed = relu, prec, int(seed)
@@ -110,7 +170,7 @@ class Stem(object):
     @property
     def in_dim(self):
         """The image channels the stem reads (layer 0's Cin)."""
-        return int(self.p[self._names(0)[0]].shape[-2])
+        return int(self.p[self._names(0)[0]].shape[-2]) - self.nloc
 
     def grid(self, H, W):
         """The knowledge base's grid (Ho, Wo) for H x W features: the knowledge base has Ho * Wo rows."""
@@ -143,6 +203,67 @@ class Stem(object):
         W = K.reshape(-1, K.shape[-1])                      # [k*k*Cin, Cout], row-major view of the HWIO kernel
         build = {"bf16": packs.bf16, "bf16x3": packs.split3, "fp8": packs.fp8}.get(self.prec)
         return W, None if build is None else self._cache.pack(build, W, stream=stream_ptr())
+
+    def location_grid(self, H, W):
+        """The fp32 location grid [H, W, l] on the device, built once per (H, W) (a captured graph reads this tensor)."""
+        if (H, W) not in self._grids:
+            g = np.ascontiguousarray(location_grid(self.location, H, W), dtype=np.float32)
+            self._grids[(H, W)] = torch.from_numpy(g).to(self.device)
+        return self._grids[(H, W)]
+
+    def _loc_weights(self):
+        """(W_img [k^2 C, Cout], W_loc [Kq, Cout]): fp32 contiguous views of one [W_img; W_loc] gathered from layer 0's
+        interleaved [k^2 (C + l), Cout] rows (W_loc's rows k^2 l..Kq-1 zero), rebuilt when the parameters move."""
+        K = self.p[self._names(0)[0]]
+        k, Cout, l = int(K.shape[0]), int(K.shape[-1]), self.nloc
+        C = int(K.shape[2]) - l
+        n_img = k * k * C
+
+        def build():
+            Kv = K.detach().reshape(k * k, C + l, Cout)
+            cat = torch.zeros((n_img + location_width(l, k), Cout), dtype=torch.float32, device=K.device)
+            cat[:n_img].view(k * k, C, Cout).copy_(Kv[:, :C])
+            cat[n_img:n_img + k * k * l].view(k * k, l, Cout).copy_(Kv[:, C:])
+            return cat
+        cat = self._cache.get(("location", K.data_ptr()), build)
+        return cat, cat[:n_img], cat[n_img:]
+
+    def _loc_cols(self, B, H, Wd, form, keep, step):
+        """Q [M, Kq] (or [M, 2 Kq] split) of layer 0's location channels on the H x W input grid, dropout fused."""
+        k, s = self.ksizes[0], self.strides[0]
+        M = B * conv_out(H, s) * conv_out(Wd, s)
+        Kq = location_width(self.nloc, k)
+        q = torch.empty((M, Kq * (2 if form == COLS_SPLIT else 1)),
+                        dtype=torch.float32 if form == COLS_F32 else torch.bfloat16, device=self.device)
+        check(self.lib.mac_loc_cols(ptr(self.location_grid(H, Wd)), ptr(q), form, float(keep), self.seed, SITE_LOCATION,
+                                    int(step), B, H, Wd, self.nloc, k, s, stream_ptr()), "mac_loc_cols")
+        return q
+
+    def _loc_scatter(self, grads, dk_img, dw_loc):
+        """Adds dK_img [k^2 C, Cout] and dW_loc[:k^2 l] into layer 0's interleaved kernel gradient [k, k, C + l, Cout]."""
+        G = grads[self._names(0)[0]]
+        k, l, Cout = int(G.shape[0]), self.nloc, int(G.shape[-1])
+        Gv = G.view(k * k, -1, Cout)
+        C = Gv.shape[1] - l
+        Gv[:, :C] += dk_img.view(k * k, C, Cout)
+        Gv[:, C:] += dw_loc[:k * k * l].view(k * k, l, Cout)
+
+    def _backward_loc0_tc(self, x, y, dy, W_img, dx, grads):
+        """Layer 0's tensor-core backward with location features (`mac_conv_bwd_loc_tc` / `_tc32`): the image half as
+        `mac_conv_bwd_tc`, and dW_loc += Q^T dZ from the same dZ^T; both scattered into the interleaved kernel gradient."""
+        sv = self._saved
+        B, H, Wd, C = x.shape
+        Nout, k, s, l = y.shape[1], self.ksizes[0], self.strides[0], self.nloc
+        name = "mac_conv_bwd_loc_tc" if self.prec == "bf16" else "mac_conv_bwd_loc_tc32"
+        nbytes = int(getattr(self.lib, name + "_workspace_bytes")(B, H, Wd, C, Nout, l, k, s, int(dx is not None)))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        dk = torch.zeros_like(W_img)
+        dwl = torch.zeros((location_width(l, k), Nout), dtype=torch.float32, device=self.device)
+        check(getattr(self.lib, name)(ptr(x), ptr(y), ptr(dy), ptr(W_img), sv["act"], sv["keep"], self.seed, SITE_STEM,
+                                      sv["step"], ptr(self.location_grid(H, Wd)), l, SITE_LOCATION, ptr(dk), ptr(dwl),
+                                      ptr(grads[self._names(0)[1]]), ptr(dx), ptr(ws), nbytes, B, H, Wd, C, Nout, k, s,
+                                      stream_ptr()), name)
+        self._loc_scatter(grads, dk, dwl)
 
     def _check_fp8(self, in_dim, keep):
         """The e4m3 stem is the inference forward only (no dropout) of the 3x3 stride-1 geometry with every channel count a
@@ -232,13 +353,17 @@ class Stem(object):
         for i in range(self.nlayers):
             if save_for_backward:
                 self._saved["xs"].append(x)
-            W, Wt = self._weights(i)
+            loc0 = i == 0 and self.location is not None
+            W, Wt = (self._loc_weights()[1], None) if loc0 else self._weights(i)
             b = self._bias(i)
+            Hin, Win = H, Wd
             H, Wd = conv_out(H, self.strides[i]), conv_out(Wd, self.strides[i])
             M, K, Nout = B * H * Wd, W.shape[0], W.shape[1]
             y = torch.empty((M, Nout), dtype=torch.float32, device=self.device)
             cols = _cols0 if (i == 0 and _cols0 is not None) else self._patches(x, i, form, keep, step)
-            if form == COLS_SPLIT:
+            if loc0:
+                self._forward_loc0(cols, self._loc_cols(B, Hin, Win, form, keep, step), form, b, act, y)
+            elif form == COLS_SPLIT:
                 check(self.lib.mac_linear_tc32_fwd(ptr(cols), ptr(Wt), ptr(b), act, ptr(y), M, K, Nout, stream_ptr()),
                       "mac_linear_tc32_fwd")
             elif form == COLS_BF16:
@@ -252,6 +377,28 @@ class Stem(object):
                 self._saved["ys"].append(y)
             x = y.view(B, H, Wd, Nout)
         return x.view(B, H * Wd, x.shape[3])
+
+    def _forward_loc0(self, cols, q, form, b, act, y):
+        """Layer 0 with location features: y = act(P W_img + (Q W_loc + b)) -- one fp32 GEMM over the segments [P, Q], or on
+        tensor cores Q W_loc + b into y, then the image GEMM adding y before its activation (mac_linear_tc(32)_fwd_acc)."""
+        cat, W_img, W_loc = self._loc_weights()
+        M, Nout = y.shape
+        if form == COLS_F32:
+            arr_p, arr_k, arr_ld = segments([cols, q])
+            check(self.lib.mac_linear_fwd(arr_p, arr_k, arr_ld, 2, ptr(cat), ptr(b), 0.0, act, ptr(y), Nout, M, Nout, None, 0,
+                                          stream_ptr()), "mac_linear_fwd")
+            return
+        K, Kq = W_img.shape[0], W_loc.shape[0]
+        if form == COLS_SPLIT:
+            check(self.lib.mac_linear_tc32_fwd(ptr(q), ptr(self._cache.pack(packs.split3, W_loc, stream=stream_ptr())), ptr(b),
+                                               _lib.ACT["NON"], ptr(y), M, Kq, Nout, stream_ptr()), "mac_linear_tc32_fwd")
+            check(self.lib.mac_linear_tc32_fwd_acc(ptr(cols), ptr(self._cache.pack(packs.split3, W_img, stream=stream_ptr())),
+                                                   act, ptr(y), M, K, Nout, stream_ptr()), "mac_linear_tc32_fwd_acc")
+        else:
+            check(self.lib.mac_linear_tc_fwd(ptr(q), ptr(self._cache.pack(packs.bf16, W_loc, stream=stream_ptr())), ptr(b),
+                                             _lib.ACT["NON"], ptr(y), 0, M, Kq, Nout, stream_ptr()), "mac_linear_tc_fwd")
+            check(self.lib.mac_linear_tc_fwd_acc(ptr(cols), ptr(self._cache.pack(packs.bf16, W_img, stream=stream_ptr())), act,
+                                                 ptr(y), M, K, Nout, stream_ptr()), "mac_linear_tc_fwd_acc")
 
     def forward_nchw(self, images, keep=1.0, step=0, save_for_backward=False):
         """`forward` from the features in the layout they are stored in: images [B,C,H,W], contiguous, fp32, fp16 or -- `prec="bf16"`
@@ -336,8 +483,13 @@ class Stem(object):
             Nout = y.shape[1]
             k, s = self.ksizes[i], self.strides[i]
             wname, bname = self._names(i)
-            W, _ = self._weights(i)
+            loc0 = i == 0 and self.location is not None
+            W = self._loc_weights()[1] if loc0 else self._weights(i)[0]
             need_dx = need_d_images or i > 0
+            if self.prec in ("bf16", "bf16x3") and loc0:
+                dx = torch.empty_like(x) if need_dx else None
+                self._backward_loc0_tc(x, y, dy, W, dx, grads)
+                continue
             if self.prec in ("bf16", "bf16x3"):
                 dx = torch.empty_like(x) if need_dx else None
                 if self._k3s1(i):
@@ -358,8 +510,16 @@ class Stem(object):
             check(self.lib.mac_activation_bwd(ptr(y), ptr(dy), sv["act"], ptr(dz), dz.numel(), stream_ptr()), "mac_activation_bwd")
             cols = self._patches(x, i, COLS_F32, sv["keep"], sv["step"])
             dcols = torch.empty_like(cols) if need_dx else None
-            Wt = W.t().contiguous() if need_dx else None
-            _lib.linear_bwd([cols], Wt, dz, [dcols], [0], grads[wname].view(W.shape), grads[bname], None, 0, stream_ptr())
+            if loc0:                    # segments [P, Q] against [W_img; W_loc]; only P takes a data gradient
+                cat = self._loc_weights()[0]
+                q = self._loc_cols(B, H, Wd, COLS_F32, sv["keep"], sv["step"])
+                dcat = torch.zeros_like(cat)
+                _lib.linear_bwd([cols, q], cat.t().contiguous() if need_dx else None, dz, [dcols, None], [0, 0], dcat,
+                                grads[bname], None, 0, stream_ptr())
+                self._loc_scatter(grads, dcat[:W.shape[0]], dcat[W.shape[0]:])
+            else:
+                Wt = W.t().contiguous() if need_dx else None
+                _lib.linear_bwd([cols], Wt, dz, [dcols], [0], grads[wname].view(W.shape), grads[bname], None, 0, stream_ptr())
             if need_dx:
                 dx = torch.empty_like(x)
                 if self._k3s1(i):
