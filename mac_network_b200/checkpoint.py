@@ -23,6 +23,13 @@ MODEL_SCOPE = "macModel/"          # model.py:774
 EMA_SUFFIX = "/ExponentialMovingAverage"
 
 
+def _untracked(name):
+    """Variables the reference's optimizer and EMA never see (`ema.apply(tf.trainable_variables())`, model.py:658-667):
+    the output unit's stored batch-norm statistics.  No EMA shadow or Adam slot is written or expected for them."""
+    from .output_unit import is_moving_stat
+    return is_moving_stat(name)
+
+
 def save_checkpoint(path, params, ema_flat=None):
     """Write parameters (and optionally the EMA shadow buffer laid out like `params.flat`) under TF variable names."""
     out = collections.OrderedDict()
@@ -32,6 +39,8 @@ def save_checkpoint(path, params, ema_flat=None):
     if ema_flat is not None:
         ema = ema_flat.detach().cpu().numpy()
         for name, (shape, _) in params.specs.items():
+            if _untracked(name):
+                continue
             n = int(np.prod(shape)) if shape else 1
             o = params.offsets[name]
             out[MODEL_SCOPE + name + EMA_SUFFIX] = ema[o:o + n].reshape(shape)
@@ -42,12 +51,14 @@ def save_checkpoint(path, params, ema_flat=None):
 def save_tf_checkpoint(prefix, values, ema_values=None, extra=None):
     """Write {variable name without the model scope: array} (+ EMA shadows, + extra entries such as global_step) as a real
     TensorFlow checkpoint `<prefix>.index` / `<prefix>.data-00000-of-00001`, plus the `checkpoint` state file
-    `tf.train.latest_checkpoint` reads (`main.py:171-178`)."""
+    `tf.train.latest_checkpoint` reads (`main.py:171-178`).  `ema_values` entries of the output unit's stored batch-norm
+    statistics are skipped: the reference keeps no shadow of them."""
     import os
     from .tf_bundle import write_tensor_bundle
     out = {MODEL_SCOPE + k: np.asarray(v, dtype=np.float32) for k, v in values.items()}
     if ema_values is not None:
-        out.update({MODEL_SCOPE + k + EMA_SUFFIX: np.asarray(v, dtype=np.float32) for k, v in ema_values.items()})
+        out.update({MODEL_SCOPE + k + EMA_SUFFIX: np.asarray(v, dtype=np.float32) for k, v in ema_values.items()
+                    if not _untracked(k)})
     if extra:
         out.update(extra)
     names = write_tensor_bundle(prefix, out)
@@ -85,6 +96,8 @@ def save_training_state(path, trainer):
         n = int(np.prod(shape)) if shape else 1
         o = p.offsets[name]
         for suffix, buf in host.items():
+            if suffix and _untracked(name):
+                continue
             out[MODEL_SCOPE + name + suffix] = buf[o:o + n].reshape(shape)
     step = int(trainer.step_id)
     out["beta1_power"] = np.float32(trainer.hp["b1"] ** step)
@@ -106,6 +119,8 @@ def load_training_state(path, trainer):
     for suffix, dst in flats.items():
         host = np.zeros(p.numel, dtype=np.float32)
         for name, (shape, _) in p.specs.items():
+            if suffix and _untracked(name):
+                continue
             key = MODEL_SCOPE + name + suffix
             if key not in z.files:
                 raise KeyError("checkpoint %s has no %s" % (path, key))

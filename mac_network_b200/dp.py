@@ -32,6 +32,29 @@ def allreduce_sum_(bucket, group=None):
     return bucket
 
 
+def allreduce_sum_with_stats_(bucket, flat, start, group=None):
+    """The step's one exchange when the flat layout ends in stored batch-norm statistics (elements `start:` of `flat`,
+    `DPTrainer.n_train`), which each rank has just moved with its own batch: the bucket's tail, which holds no gradient,
+    carries each rank's statistics / world, so the SUM leaves the mean over ranks, copied back into `flat`.  Every rank
+    then holds the same statistics, moved by the mean over ranks of the per-rank batch statistics (the update is linear in
+    them).  The gradient norm, clipping, Adam and the EMA read elements `:start` only.  At world = 1 nothing is touched."""
+    import torch.distributed as dist
+    world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+    tail = world > 1 and start < flat.numel()
+    if tail:
+        torch.mul(flat[start:], 1.0 / world, out=bucket[start:])
+    allreduce_sum_(bucket, group)
+    if tail:
+        flat[start:].copy_(bucket[start:])
+    return bucket
+
+
+def classifier_options(classifier):
+    """The output unit options of `classifier=(answerWordsNum, outClassifierDims[, options])` (`output_options`)."""
+    from .output_unit import output_options
+    return output_options(classifier[2] if len(classifier) > 2 else None)
+
+
 def check_model_precisions(cfg, encoder, stem, stem_prec, enc_prec):
     """The stem's and the encoder's training precisions against the model's shapes (DPTrainer, modules.MACModel): raises
     before anything is allocated or launched."""
@@ -96,7 +119,8 @@ def model_parameters(cfg, netLength, seed, classifier=None, encoder=None, stem=N
     extra_specs = extra_values = None
     if classifier is not None:
         from .output_unit import output_specs, init_output_params
-        extra_specs = output_specs(cfg.ctrlDim, cfg.memDim, list(classifier[1]), classifier[0])
+        extra_specs = output_specs(cfg.ctrlDim, cfg.memDim, list(classifier[1]), classifier[0],
+                                   **classifier_options(classifier))
         extra_values = init_output_params(extra_specs, seed=seed + 17, bias_scale=0.0)
     enc_specs = stem_specs_ = None
     if encoder is not None or stem is not None:
@@ -114,6 +138,12 @@ def model_parameters(cfg, netLength, seed, classifier=None, encoder=None, stem=N
         extra_values = dict(extra_values)
         extra_values.update(init_encoder_params(enc_specs, seed=seed + 19, bias_scale=0.0))   # TF: zero biases
         extra_values.update(init_stem_params(stem_specs_, seed=seed + 23, bias_scale=0.0))
+    if extra_specs is not None:
+        from .output_unit import is_moving_stat
+        # the classifier's stored batch-norm statistics last: the optimizer and the EMA run over the flat buffer before them
+        import collections
+        extra_specs = collections.OrderedDict([kv for kv in extra_specs.items() if not is_moving_stat(kv[0])]
+                                              + [kv for kv in extra_specs.items() if is_moving_stat(kv[0])])
     if extra_specs is not None and param_values is None:
         param_values = init_params(cfg, netLength, seed=seed)
     return param_values, extra_specs, extra_values, enc_specs, stem_specs_
@@ -125,7 +155,11 @@ class DPTrainer(object):
                  encoder=None, stem=None, enc_dropouts=(0.85, 0.92), stem_dropout=0.82, prec="fp32", bwd_tc=False,
                  stem_prec="fp32", enc_prec="fp32"):
         """`classifier=(answerWordsNum, outClassifierDims)` adds the reference's output unit + answer loss
-        (model.py:512-528, 547-576, 593-596); `encoder=(vocabulary rows, wrdEmbDim)` the question input unit
+        (model.py:512-528, 547-576, 593-596), and `classifier=(answerWordsNum, outClassifierDims, options)` the one of
+        the options {"question", "mul", "bn"} (--outQuestion, --outQuestionMul, --outputBN; `output_unit.output_options`,
+        unknown keys raise ValueError).  With "bn" the stored statistics sit at the end of the flat buffer, from `n_train`:
+        they get no gradient, clipping, Adam update or EMA shadow, and after each step every rank holds their mean over
+        ranks (`allreduce_sum_with_stats_`); `encoder=(vocabulary rows, wrdEmbDim)` the question input unit
         (model.py:208-220, 279-307) and `stem=(imageInDim, stemNumLayers)` the image stem (model.py:165-204) -- or
         `stem=(imageInDim, stemNumLayers, geometry)` with the stem's kernel sizes, strides, linear form and width
         (`stem_geometry`) --, with the
@@ -157,12 +191,16 @@ class DPTrainer(object):
         self.params = MACParams(cfg, netLength, values=param_values, seed=seed, device=device, extra_specs=extra_specs,
                                 extra_values=extra_values)   # replicated
         self.out = None
+        self.n_train = self.params.numel      # the optimizer's and the EMA's elements of the flat buffer
         if classifier is not None:
-            from .output_unit import OutputUnit
+            from .output_unit import OutputUnit, is_moving_stat
             self.out = OutputUnit({k: self.params.t[k] for k in extra_specs
                                    if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu, keep=output_dropout,
-                                  seed=seed, version=lambda: self.params.version)
+                                  seed=seed, version=lambda: self.params.version, bn_decay=cfg.bnDecay,
+                                  **classifier_options(classifier))
             self._views_of = views_of
+            tail = [self.params.offsets[k] for k in extra_specs if is_moving_stat(k)]
+            self.n_train = min(tail) if tail else self.params.numel
         self.enc = self.stem = None
         if self._enc_specs is not None:
             from .encoder import QuestionEncoder
@@ -245,11 +283,11 @@ class DPTrainer(object):
 
     def apply(self):
         """all-reduce the bucket, then clip + Adam + EMA (model.py:645-667) in one fused pass; refresh derived weights."""
-        allreduce_sum_(self.bucket)
+        allreduce_sum_with_stats_(self.bucket, self.params.flat, self.n_train)
         self.step_id += 1
         h = self.hp
         check(self.lib.mac_clip_adam_ema_step(ptr(self.params.flat), ptr(self.bucket), ptr(self.adam_m), ptr(self.adam_v),
-                                              ptr(self.ema), self.params.numel, 1.0, h["clip"], h["lr"], h["b1"], h["b2"],
+                                              ptr(self.ema), self.n_train, 1.0, h["clip"], h["lr"], h["b1"], h["b2"],
                                               h["eps"], self.step_id, h["ema"], ptr(self.norm), ptr(self.ows),
                                               self.ows_bytes, stream_ptr()), "mac_clip_adam_ema_step")
         self.params.touch()

@@ -36,7 +36,7 @@ class MACnet(object):
                  stem_layers=2, seed=0, rank=0, world=1, lr=1e-4, prec="bf16", use_ema=False, answer_decoder=None,
                  device="cuda", eval_stem_prec=None, eval_enc_prec=None, train_prec="fp32", stem_kernel_sizes=None,
                  stem_strides=None, stem_linear=False, stem_dim=None, stem_location=None, stem_location_bias=1.0,
-                 stem_location_dim=32, **trainer_kw):
+                 stem_location_dim=32, out_question=True, out_question_mul=False, output_bn=False, **trainer_kw):
         """`vocab`: rows of the question-embedding variable (ids 1..vocab; 0 is padding); `answer_decoder`: optional
         id -> answer string (`answerDict.decodeId`, model.py:699).  `prec`: arithmetic of the evaluation forward; with
         "fp8" the cell's read step runs on e4m3 and the image stem in bf16.  `eval_stem_prec="fp8"` runs the evaluation
@@ -48,7 +48,14 @@ class MACnet(object):
         `enc_prec`).  `stem_kernel_sizes`, `stem_strides`, `stem_linear` and `stem_dim` are the reference's
         --stemKernelSizes, --stemStrideSizes, --stemLinear and --stemDim (`dp.stem_geometry`); the knowledge base then has
         the stem's output grid (`Stem.grid`).  `stem_location` ("L" or "PE"; None: off), `stem_location_bias` and
-        `stem_location_dim` are --locationAware with --locationType, --locationBias and --locationDim."""
+        `stem_location_dim` are --locationAware with --locationType, --locationBias and --locationDim.
+        `out_question`, `out_question_mul` and `output_bn` are the output unit's --outQuestion, --outQuestionMul and
+        --outputBN (`DPTrainer(classifier=)`).  The default keeps the shipped flag files' output unit; note that the
+        reference's own default for --outQuestion is off (a model trained without the flag files needs
+        out_question=False), and that --outQuestionMul does nothing without --outQuestion.  With output_bn, evaluation
+        (`runBatch(train=False)`) normalises with the stored statistics, which are not trainable: `use_ema=True` swaps the
+        trained weights only, so evaluation reads the live statistics, as the reference's EMA (trainable variables only,
+        model.py:658-667) does."""
         if eval_stem_prec not in (None, "fp8", "bf16x3"):
             raise ValueError("eval_stem_prec must be None, 'fp8' or 'bf16x3', got %r" % (eval_stem_prec,))
         if eval_enc_prec not in (None, "bf16"):
@@ -63,7 +70,9 @@ class MACnet(object):
         self.cfg, self.L, self.prec, self.use_ema = cfg, netLength, prec, bool(use_ema)
         self.decode = answer_decoder
         self.trainer = DPTrainer(cfg, netLength, seed=seed, rank=rank, world=world, lr=lr, device=device,
-                                 classifier=(n_answers, list(classifier_dims)), encoder=(vocab, wrd_emb_dim),
+                                 classifier=(n_answers, list(classifier_dims),
+                                             {"question": out_question, "mul": out_question_mul, "bn": output_bn}),
+                                 encoder=(vocab, wrd_emb_dim),
                                  stem=(image_in_dim, stem_layers, {"ksizes": stem_kernel_sizes, "strides": stem_strides,
                                                                    "linear": stem_linear, "stem_dim": stem_dim,
                                                                    "location": stem_location,
@@ -79,7 +88,7 @@ class MACnet(object):
         self._stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=stem_prec, version=lambda: p.version,
                           strides=t.stem.strides, linear=t.stem.linear, location=t.stem.location)
         self._out = OutputUnit({k: p.t[k] for k in p.specs if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu,
-                               keep=1.0, version=lambda: p.version)
+                               keep=1.0, version=lambda: p.version, bn_decay=cfg.bnDecay, **t.out.options)
         self.device = p.device
         self.macCell = None                      # the cell of the last batch (model.py:740 reads macCell.attentions)
 
@@ -135,11 +144,13 @@ class MACnet(object):
         return dev
 
     def _swap_ema(self):
-        """Evaluate on the EMA shadows (main.py:717-719): swap them with the live weights (and back)."""
+        """Evaluate on the EMA shadows (main.py:717-719): swap them with the live weights (and back).  The EMA covers the
+        trainable variables (`DPTrainer.n_train`), so the classifier's stored batch-norm statistics stay the live ones."""
         t = self.trainer
-        tmp = t.params.flat.clone()
-        t.params.flat.copy_(t.ema)
-        t.ema.copy_(tmp)
+        n = t.n_train
+        tmp = t.params.flat[:n].clone()
+        t.params.flat[:n].copy_(t.ema[:n])
+        t.ema[:n].copy_(tmp)
         t.params.touch()
 
     # ------------------------------------------------------------------ model.py:732-760
@@ -168,7 +179,7 @@ class MACnet(object):
                 cell = MACCell(vecq, words, cntx, dev["questionLengths"], kb, 1.0, 1.0, 1.0, B, False, config=self.cfg,
                                params=t.params, prec=self.prec, kbIndex=kbIndex)
                 _, memory = mac_network(cell, self.L)
-                logits, losses, _ = self._out.forward(memory, vecq, dev["answers"])
+                logits, losses, _ = self._out.forward(memory, vecq, dev["answers"], train=False)
                 self.macCell = cell
             finally:
                 if self.use_ema:

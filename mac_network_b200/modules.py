@@ -32,7 +32,7 @@ from ._lib import check, ptr, stream_ptr
 from .autograd import check_backward, mac_backward
 from .encoder import QuestionEncoder as _Encoder, encoder_specs, init_encoder_params
 from .mac_cell import MACCell, MACParams, flat_layout, mac_network, views_of
-from .output_unit import OutputUnit as _Output, init_output_params, output_specs
+from .output_unit import OutputUnit as _Output, init_output_params, is_moving_stat, output_specs
 from .params import param_specs
 from .stem import Stem, init_stem_params, stem_specs
 
@@ -321,7 +321,10 @@ class _KernelModule(nn.Module):
     def _register(self, params, seed):
         self.params = params
         for name, view in params.t.items():     # scalars as the reference's 0-d variables (the kernels' views are [1])
-            self.register_parameter(name, nn.Parameter(view.view(params.specs[name][0])))
+            if is_moving_stat(name):            # the classifier's stored batch-norm statistics: state, not parameters
+                self.register_buffer(name, view.view(params.specs[name][0]))
+            else:
+                self.register_parameter(name, nn.Parameter(view.view(params.specs[name][0])))
         self._seen = params.flat._version
         self.seed, self.step = int(seed), 0
 
@@ -471,27 +474,32 @@ def _stem_fn(mod, grads, seed_step, x, nchw):
 
 class OutputUnit(_KernelModule):
     """The output unit and classifier (model.py:512-528, 547-576): `forward(memory, vecQuestions)` -> logits [B, A]; the
-    loss is `answer_loss`."""
+    loss is `answer_loss`.  `question`, `mul`, `bn`: --outQuestion, --outQuestionMul, --outputBN (`output_specs`); with
+    `bn` the stored statistics are buffers (`moving_mean`, `moving_variance` under the reference's names), the batch
+    normalisation follows `training` -- batch statistics and an in-place update of the stored ones in train mode, the
+    stored statistics in eval mode -- and `bn_decay` is --bnDecay."""
 
-    def __init__(self, ctrl_dim, mem_dim, hidden, n_answers, relu="ELU", values=None, seed=0, device="cuda"):
+    def __init__(self, ctrl_dim, mem_dim, hidden, n_answers, relu="ELU", values=None, seed=0, device="cuda",
+                 question=True, mul=False, bn=False, bn_decay=0.999):
         super(OutputUnit, self).__init__()
-        specs = output_specs(ctrl_dim, mem_dim, list(hidden), n_answers)
+        opts = {"question": question, "mul": mul, "bn": bn}
+        specs = output_specs(ctrl_dim, mem_dim, list(hidden), n_answers, **opts)
         values = values if values is not None else init_output_params(specs, seed=seed + 17, bias_scale=0.0)
         self._register(_Params(specs, values, device), seed)
-        self._out = _output_unit(self.params, relu)
-        self._out_names = list(specs)
+        self._out = _output_unit(self.params, relu, opts=opts, bn_decay=bn_decay)
+        self._out_names = [k for k in specs if not is_moving_stat(k)]
 
     def forward(self, memory, vecQuestions):
         self._refresh()
         memory, vecq = memory.contiguous(), vecQuestions.contiguous()
         if not self._trains(memory, vecq):
-            return self._out.logits(memory, vecq)
+            return self._out.logits(memory, vecq, train=self.training)
         return _output_fn(self, self._grads(), self._next(), memory, vecq)
 
 
-def _output_unit(params, relu, keep=OUTPUT_KEEP):
+def _output_unit(params, relu, keep=OUTPUT_KEEP, opts=None, bn_decay=0.999):
     return _Output({k: params.t[k] for k in params.t if k.startswith(("outputUnit/", "classifier/"))}, relu=relu,
-                   keep=keep, version=lambda: params.version)
+                   keep=keep, version=lambda: params.version, bn_decay=bn_decay, **(opts or {}))
 
 
 def _output_fn(mod, grads, seed_step, memory, vecq):
@@ -508,15 +516,16 @@ class MACModel(_KernelModule):
 
     def __init__(self, cfg, netLength, vocab, n_answers, wrd_emb_dim=300, image_in_dim=1024, classifier_dims=(512,),
                  stem_layers=2, prec="fp32", bwd_tc=False, stem_prec="fp32", enc_prec="fp32", eval_prec=None, values=None,
-                 seed=0, device="cuda", stem_geometry=None):
+                 seed=0, device="cuda", stem_geometry=None, out_question=True, out_question_mul=False, output_bn=False):
         super(MACModel, self).__init__()
         from .dp import check_model_precisions, model_parameters, stem_geometry as stem_geometry_of, stem_location
         if not cfg.controlContextual:
             raise NotImplementedError("the raw-word control inputs (controlContextual off) need wrdEmbDim == ctrlDim")
         encoder, stem = (vocab, wrd_emb_dim), (image_in_dim, stem_layers, stem_geometry)
+        opts = {"question": out_question, "mul": out_question_mul, "bn": output_bn}
         check_model_precisions(cfg, encoder, stem, stem_prec, enc_prec)
         cell_values, extra_specs, extra_values, enc_specs, stem_specs_ = model_parameters(
-            cfg, netLength, seed, (n_answers, list(classifier_dims)), encoder, stem, values)
+            cfg, netLength, seed, (n_answers, list(classifier_dims), opts), encoder, stem, values)
         if values is not None:
             extra_values = {k: values[k] for k in extra_specs}
         self.cfg, self.L = cfg, netLength
@@ -524,11 +533,11 @@ class MACModel(_KernelModule):
                                  extra_values=extra_values), seed)
         self._cell_names = list(param_specs(cfg, netLength))
         self._enc_names, self._stem_names = list(enc_specs), list(stem_specs_)
-        self._out_names = [k for k in extra_specs if k.startswith(("outputUnit/", "classifier/"))]
+        self._out_names = [k for k in extra_specs if k.startswith(("outputUnit/", "classifier/")) and not is_moving_stat(k)]
         self._enc = _encoder_units(self.params, enc_prec)
         geom = stem_geometry_of(stem)
         self._stem = _stem_unit(self.params, cfg.relu, stem_prec, dict(geom, location=stem_location(geom)))
-        self._out = _output_unit(self.params, cfg.relu)
+        self._out = _output_unit(self.params, cfg.relu, opts=opts, bn_decay=cfg.bnDecay)
         self.stem_keep = STEM_KEEP
         self.cells = _Cells(cfg, netLength, self.params, prec, bwd_tc, eval_prec,
                             (cfg.memoryDropout, cfg.readDropout, cfg.writeDropout))
@@ -547,7 +556,8 @@ class MACModel(_KernelModule):
         m = cls(t.cfg, t.L, vocab, fcs[-1][1], wrd_emb_dim=E, image_in_dim=t.stem.in_dim,
                 classifier_dims=[s[1] for s in fcs[:-1]], stem_layers=t.stem.nlayers, prec=t.prec, bwd_tc=t.bwd_tc,
                 stem_prec=t.stem_prec, enc_prec=t.enc_prec, eval_prec=eval_prec, values=values, seed=t.base_seed,
-                device=t.params.device, stem_geometry=t.stem_geometry)
+                device=t.params.device, stem_geometry=t.stem_geometry, out_question=t.out.options["question"],
+                out_question_mul=t.out.options["mul"], output_bn=t.out.options["bn"])
         m.step = t.step_id
         m.cells.dropouts = tuple(float(k) for k in t.dropouts)
         m._enc[0].keep_input, m._enc[0].keep_question = t.enc.keep_input, t.enc.keep_question
@@ -577,7 +587,7 @@ class MACModel(_KernelModule):
             words, cntx, vecq = self._enc[1].forward(questions, lengths)
             kb = self._stem.forward_nchw(x) if nchw else self._stem.forward(x)
             _, memory = self.cells.infer(vecq, words, cntx, lengths, kb, imageIndex)
-            return self._out.logits(memory, vecq), memory
+            return self._out.logits(memory, vecq, train=self.training), memory
         # the training cell first: every refusal of the configuration comes before the first launch
         key, cell = self.cells.acquire(True, B, S, self._enc[0].E, N, U)
         if imageIndex is not None:

@@ -400,7 +400,7 @@ class _ModelSlot(object):
         self.stem = Stem({k: p.t[k] for k in t._stem_specs}, relu=cfg.relu, prec=model._stem.prec, version=version,
                          strides=model._stem.strides, linear=model._stem.linear, location=model._stem.location)
         self.out = OutputUnit({k: p.t[k] for k in p.specs if k.startswith(("outputUnit/", "classifier/"))}, relu=cfg.relu,
-                              keep=1.0, version=version)
+                              keep=1.0, version=version, bn_decay=cfg.bnDecay, **t.out.options)
         self.cell = None
         self.graph = None
         self.outs_host = None
