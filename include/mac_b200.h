@@ -591,8 +591,9 @@ size_t mac_conv3x3_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout
  *   refused geometry).
  * Every entry point: a null pointer, a size, k or s <= 0, keep outside (0, 1] or more than 2^30 input or output pixels ->
  * MAC_ERR_INVALID; k or s > 16, the channel rules above, k^2 C / 64 > 65535 (mac_im2col_t, mac_conv_bwd_tc / _tc32: one
- * launch row per 64 patch columns) or an unknown form -> MAC_ERR_UNSUPPORTED; pointers not 16-byte
- * aligned -> MAC_ERR_ALIGN.  All checks precede any launch. */
+ * launch row per 64 patch columns), Mp / 64 > 65535 (every conv backward, mac_conv3x3_bwd_tc / _tc32 included: one launch row
+ * per 64 output pixels, so M <= 4 194 240; their workspace queries return 0) or an unknown form -> MAC_ERR_UNSUPPORTED;
+ * pointers not 16-byte aligned -> MAC_ERR_ALIGN.  All checks precede any launch. */
 enum { MAC_COLS_F32 = 0, MAC_COLS_BF16 = 1, MAC_COLS_SPLIT = 2 };
 int mac_im2col(const float* x, void* cols, int form, float keep, uint64_t seed, int site, int step, int B, int H, int W, int C,
                int k, int s, mac_stream_t stream);

@@ -1368,6 +1368,8 @@ __global__ void __launch_bounds__(256) im2col_t_kernel(const float* __restrict__
 
 // im2col_t_kernel's launch: one 64-row tile (within one tap: C % 64 == 0) per gridDim.y index, at most 65535 of them
 inline bool im2col_t_grid_ok(int k, int C) { return (long long)k * k * C / 64 <= 65535; }
+// conv_dz_pack_kernel's launch: one 64-row block of dZ per gridDim.y index, Mp / 64 <= 65535 (M <= 4 194 240)
+inline bool conv_dz_grid_ok(const ConvGeom& g) { return ((long long)g.B * g.Ho * g.Wo + 63) / 64 <= 65535; }
 
 // workspace of mac_conv3x3_bwd_tc / _tc32: 1 KB-aligned slabs behind a 1 KB alignment slack.  `split`: the bf16 operands
 // carry 2 (dz rows, colsT) or 3 (dzT, kernel) segments, and the weight gradient contracts over 3 Mp.
@@ -1429,11 +1431,11 @@ static int conv_bwd_wgmma(bool split, const float* x, const float* y, const floa
     if (lst != MAC_OK) return lst;
   }
   if ((C % 128) || (Cout % 128)) return MAC_ERR_UNSUPPORTED;     // wgmma tiles: k^2 C and Cout are GEMM N / M extents
-  if (!im2col_t_grid_ok(k, C)) return MAC_ERR_UNSUPPORTED;
+  const ConvGeom g = conv_geom(B, H, W, C, k, s);
+  if (!im2col_t_grid_ok(k, C) || !conv_dz_grid_ok(g)) return MAC_ERR_UNSUPPORTED;
   if (!mac_aligned16(x) || !mac_aligned16(y) || !mac_aligned16(dy) || !mac_aligned16(kernel) || !mac_aligned16(dkernel) ||
       (dx && !mac_aligned16(dx)) || (loc && (!mac_aligned16(loc->grid) || !mac_aligned16(loc->dwloc))))
     return MAC_ERR_ALIGN;
-  const ConvGeom g = conv_geom(B, H, W, C, k, s);
   const bool k3s1 = k == 3 && s == 1;
   const ConvBwdLayout l = conv_bwd_layout(g, Cout, dx != nullptr, split, loc ? loc->l : 0);
   if (workspace_bytes < l.total) return MAC_ERR_WORKSPACE;
@@ -1522,7 +1524,9 @@ extern "C" int mac_im2col_t(const float* x, void* colsT, int split, float keep, 
 }
 
 extern "C" size_t mac_conv_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int k, int s, int with_dx) {
-  if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C)) return 0;
+  if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C) ||
+      !conv_dz_grid_ok(conv_geom(B, H, W, C, k, s)))
+    return 0;
   return conv_bwd_layout(conv_geom(B, H, W, C, k, s), Cout, with_dx != 0, false).total;
 }
 
@@ -1534,7 +1538,9 @@ extern "C" int mac_conv_bwd_tc(const float* x, const float* y, const float* dy, 
 }
 
 extern "C" size_t mac_conv_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int k, int s, int with_dx) {
-  if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C)) return 0;
+  if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C) ||
+      !conv_dz_grid_ok(conv_geom(B, H, W, C, k, s)))
+    return 0;
   return conv_bwd_layout(conv_geom(B, H, W, C, k, s), Cout, with_dx != 0, true).total;
 }
 
@@ -1547,7 +1553,7 @@ extern "C" int mac_conv_bwd_tc32(const float* x, const float* y, const float* dy
 }
 
 extern "C" size_t mac_conv3x3_bwd_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx) {
-  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return 0;
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0 || !conv_dz_grid_ok(conv_geom(B, H, W, C, 3, 1))) return 0;
   return conv_bwd_layout(conv_geom(B, H, W, C, 3, 1), Cout, with_dx != 0, false).total;
 }
 
@@ -1559,7 +1565,7 @@ extern "C" int mac_conv3x3_bwd_tc(const float* x, const float* y, const float* d
 }
 
 extern "C" size_t mac_conv3x3_bwd_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int with_dx) {
-  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0) return 0;
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0 || !conv_dz_grid_ok(conv_geom(B, H, W, C, 3, 1))) return 0;
   return conv_bwd_layout(conv_geom(B, H, W, C, 3, 1), Cout, with_dx != 0, true).total;
 }
 
@@ -1574,6 +1580,7 @@ extern "C" int mac_conv3x3_bwd_tc32(const float* x, const float* y, const float*
 // rows [k^2 C, Cout]), then dW_loc [Kq, Cout] += Q^T dZ.  The location channels take no data gradient.
 extern "C" size_t mac_conv_bwd_loc_tc_workspace_bytes(int B, int H, int W, int C, int Cout, int l, int k, int s, int with_dx) {
   if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C) ||
+      !conv_dz_grid_ok(conv_geom(B, H, W, C, k, s)) ||
       loc_check(B, H, W, l, k, s, 1.f) != MAC_OK)
     return 0;
   return conv_bwd_layout(conv_geom(B, H, W, C, k, s), Cout, with_dx != 0, false, l).total;
@@ -1591,6 +1598,7 @@ extern "C" int mac_conv_bwd_loc_tc(const float* x, const float* y, const float* 
 extern "C" size_t mac_conv_bwd_loc_tc32_workspace_bytes(int B, int H, int W, int C, int Cout, int l, int k, int s,
                                                         int with_dx) {
   if (Cout <= 0 || conv_geom_check(B, H, W, C, k, s, 1.f) != MAC_OK || !im2col_t_grid_ok(k, C) ||
+      !conv_dz_grid_ok(conv_geom(B, H, W, C, k, s)) ||
       loc_check(B, H, W, l, k, s, 1.f) != MAC_OK)
     return 0;
   return conv_bwd_layout(conv_geom(B, H, W, C, k, s), Cout, with_dx != 0, true, l).total;
