@@ -299,7 +299,10 @@ int mac_linear_tc_fwd(const void* x_bf16, const void* wt_bf16, const float* b, i
  * does not pass through bf16.  wt_lo == NULL: one plain bf16 pass.
  * Epilogue: act in MAC_ACT_*; y2 != NULL sends columns >= n_split to y2[m, n - n_split] (the folded write unit, see
  * mac_write_fwd_next_y); gate_new != NULL selects the write gate z = sigmoid(t), y = gate_new*z + gate_old*(1-z), z stored
- * to gate_z when given (mac_cell.py:358-367).  Needs k_segs[i] % 64 == 0, n_out % 32 == 0, else MAC_ERR_UNSUPPORTED. */
+ * to gate_z when given (mac_cell.py:358-367).  Needs k_segs[i] % 64 == 0, n_out % 32 == 0, else MAC_ERR_UNSUPPORTED;
+ * the gate and y2 together are MAC_ERR_UNSUPPORTED.  MAC_ERR_INVALID, before any CUDA call: ldx[i] < k_segs[i], gate_z
+ * without the gate, ldy < n_out without y2, and with y2 n_split outside (0, n_out) or ldy < max(n_split, n_out - n_split).
+ * y, y2, the gate operands and both packs must be 16-byte aligned (MAC_ERR_ALIGN). */
 int mac_pack_weight_bf16_split(const float* W, void* hi_bf16, void* lo_bf16, int K, int n_out, mac_stream_t stream);
 int mac_linear_tc_small_fwd(const float* const* x_segs, const int* k_segs, const int* ldx, int nseg,
                             const void* wt_hi, const void* wt_lo, const float* b, float bias_const, int act,

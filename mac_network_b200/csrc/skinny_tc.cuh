@@ -246,17 +246,35 @@ skinny_tc_kernel(const __grid_constant__ SkinnyTcMaps maps, const SkinnyTcParams
   }
 }
 
-// wt_hi / wt_lo: bf16 [N, K] (K-major) halves of the fp32 weight (mac_pack_weight_bf16_split); wt_lo == NULL: single pass
-inline int skinny_tc_launch(SkinnyTcParams p, const void* wt_hi, const void* wt_lo, cudaStream_t stream) {
+// The arguments skinny_tc_launch cannot serve, checked on the host alone (no CUDA call, so mac_linear_tc_small_fwd runs it
+// before its device check): what the tiles do not take (UNSUPPORTED), a missing operand, an output region its stride
+// cannot hold or a segment wider than its row stride (INVALID), misalignment (ALIGN).
+// The epilogue writes rows [0, M) of y at stride ldy: columns [0, N), or [0, n_split) and y2's [0, N - n_split); the write
+// gate reads gnew / gold and writes gate_z over y's columns.  The gate and the column split are one epilogue each.
+inline int skinny_tc_check(const SkinnyTcParams& p, const void* wt_hi, const void* wt_lo) {
   if (p.M <= 0 || p.M > 128 || p.N <= 0 || p.K <= 0 || p.nseg < 1 || p.nseg > 4) return MAC_ERR_INVALID;
   if ((p.N % 32) || (p.K % TC_BK) || (p.ldy & 3) || (p.Y2 && (p.n_split % 32))) return MAC_ERR_UNSUPPORTED;
+  if (p.Y2 && p.gnew) return MAC_ERR_UNSUPPORTED;
+  if (p.gate_z && !p.gnew) return MAC_ERR_INVALID;
+  if (p.Y2 ? (p.n_split <= 0 || p.n_split >= p.N || p.ldy < p.n_split || p.ldy < p.N - p.n_split) : p.ldy < p.N)
+    return MAC_ERR_INVALID;
   int ksum = 0;
   for (int i = 0; i < p.nseg; ++i) {
     if (!p.a[i] || p.ak[i] <= 0 || (p.ak[i] % TC_BK) || (p.lda[i] & 3)) return MAC_ERR_UNSUPPORTED;
+    if (p.lda[i] < p.ak[i]) return MAC_ERR_INVALID;
     if (!mac_aligned16(p.a[i])) return MAC_ERR_ALIGN;
     ksum += p.ak[i];
   }
   if (ksum != p.K || !wt_hi || !p.Y || !mac_aligned16(p.Y) || !mac_aligned16(wt_hi)) return MAC_ERR_INVALID;
+  if ((wt_lo && !mac_aligned16(wt_lo)) || (p.Y2 && !mac_aligned16(p.Y2)) || (p.gnew && !mac_aligned16(p.gnew)) ||
+      (p.gold && !mac_aligned16(p.gold)) || (p.gate_z && !mac_aligned16(p.gate_z)))
+    return MAC_ERR_ALIGN;
+  return MAC_OK;
+}
+
+// wt_hi / wt_lo: bf16 [N, K] (K-major) halves of the fp32 weight (mac_pack_weight_bf16_split); wt_lo == NULL: single pass.
+// p has passed skinny_tc_check.
+inline int skinny_tc_launch(SkinnyTcParams p, const void* wt_hi, const void* wt_lo, cudaStream_t stream) {
   p.split = wt_lo ? 1 : 0;
   const int BN = (p.N % 64 == 0 && p.N >= 1024) ? 64 : 32;
   const bool cols = p.M <= 64;

@@ -400,7 +400,6 @@ extern "C" int mac_linear_tc_small_fwd(const float* const* x_segs, const int* k_
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x_segs || !k_segs || !ldx || nseg < 1 || nseg > 4 || !wt_hi || !y || M <= 0 || n_out <= 0) return MAC_ERR_INVALID;
   if ((gate_new != nullptr) != (gate_old != nullptr)) return MAC_ERR_INVALID;
-  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
   SkinnyTcParams p{};
   p.nseg = nseg;
   for (int i = 0; i < nseg; ++i) {
@@ -412,6 +411,9 @@ extern "C" int mac_linear_tc_small_fwd(const float* const* x_segs, const int* k_
   p.M = M; p.N = n_out; p.bias = b; p.bias_const = bias_const; p.act = act;
   p.Y = y; p.ldy = ldy; p.Y2 = y2; p.n_split = n_split;
   p.gnew = gate_new; p.gold = gate_old; p.gate_z = gate_z;
+  const int st = skinny_tc_check(p, wt_hi, wt_lo);
+  if (st != MAC_OK) return st;
+  if (!mac_b200_device_ok()) return MAC_ERR_ARCH;
   return skinny_tc_launch(p, wt_hi, wt_lo, stream);
 }
 

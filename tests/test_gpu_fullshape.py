@@ -205,21 +205,29 @@ def test_bf16_small_tc_form_matches_oracle(variant):
     """The throughput form of the bf16 cell (MACCell(small_tc=True): projY, write unit, gate and ctrlProj
     as three-pass split-bf16 wgmma products, write unit folded with the next projY) against the fp64 oracle at the
     headline and GQA shapes: same bounds as the default form (the split keeps these projections at fp32-class accuracy)."""
-    if variant == "args":
-        cfg, inputs, params, ref = headline_case()
-        L = SHAPES["headline"][4]
-    else:
-        shape = SHAPES["gqa"]
-        cfg, inputs, params, ref = headline_case("gqa", shape, seeds=(41, 42, 43))
-        L = shape[4]
+    check_small_tc_form(variant, SHAPES["headline"] if variant == "args" else SHAPES["gqa"])
+
+
+@pytest.mark.parametrize("B", [1, 100, 128])
+@pytest.mark.parametrize("variant", ["args", "gqa"])
+def test_bf16_small_tc_row_form_matches_oracle(variant, B):
+    """The throughput form at batches where skinny_tc_kernel's two warpgroups split the rows (B = 100, 128) and at a single
+    row (B = 1), N = 49, L = 4: the bounds of test_bf16_small_tc_form_matches_oracle."""
+    check_small_tc_form(variant, (B, 20, 49, 512, 4))
+
+
+def check_small_tc_form(variant, shape):
+    cfg, inputs, params, ref = headline_case(variant, shape, seeds=(1234, 100, 101) if variant == "args" else (41, 42, 43))
+    L = shape[4]
     got, cell = run_gpu(cfg, params, inputs, L, prec="bf16", small_tc=True)
     assert cell._small_tc
     errs = {k: max(max_rel(got[k][i], ref[k][i]) for i in range(L)) for k in PER_STEP}
-    print("bf16 throughput form (%s) worst per-step max-rel:" % variant, errs)
+    print("bf16 throughput form (%s, %s) worst per-step max-rel:" % (variant, shape), errs)
     assert errs["control"] < 1e-4
     assert errs["memory"] < 1.5e-3 and errs["info"] < 4e-3 and errs["att_kb"] < 3e-3, errs
     if variant == "gqa":
         g = max(max_rel(got["att_gate"][i], ref["att_gate"][i]) for i in range(L))
+        print("bf16 throughput form (%s, %s) worst att_gate max-rel: %.2e" % (variant, shape, g))
         assert g < 1.5e-3, g
 
 
