@@ -14,6 +14,10 @@ against (tests/test_gpu_read_step_fp8.py); the model-level error of the scheme i
     att = softmax_n(logits);  info = sum_n att * bf16(KB)
 
 An all-zero row or column has scale 0 and quantises to zeros.
+
+quant_rows_f32, pack_weight_f32 and a8_f32 restate the three quantisers with the kernels' own fp32 operations instead, so
+the library's bytes and scales are checked against them bit for bit (tests/test_gpu_read_step_fp8.py,
+tests/test_gpu_fp8_kernels.py); the fp64 functions above them stay the model of the scheme.
 """
 import torch
 
@@ -45,6 +49,41 @@ def pack_weight(W):
     """Per-output-column scaling of W [K, n_out] ([in, out], the reference's layout): (W8 [K, n_out], s [1, n_out]).
     The library stores W8 transposed ([out, in], K-major); the values are the same."""
     return _quantise(W, W.abs().amax(0, keepdim=True))
+
+
+# ---- fp32 restatements of the quantisers: the kernels' own fp32 operations, so their bytes and scales compare bit for bit.
+# Every division runs on full tensors (torch divides by a 0-d tensor as a product with its reciprocal).
+def _quantise_f32(X, amax):
+    """(e4m3(X / fp32(amax / 448)), fp32 amax / 448) with IEEE fp32 division, amax broadcast against X; zeros where
+    amax == 0 (quant_rows_e4m3_kernel, pack_weight_fp8_kernel)."""
+    s = amax / torch.full_like(amax, E4M3_MAX)
+    sx, nz = s.expand_as(X).contiguous(), (amax > 0).expand_as(X)
+    return e4m3(torch.where(nz, X / torch.where(nz, sx, torch.ones_like(sx)), torch.zeros_like(X))), s
+
+
+def quant_rows_f32(X):
+    """P8 and sP as mac_read_invariant computes them from the bf16 P (fp32 X [M, K]): (X8 [M, K] fp64, s [M] fp32)."""
+    X = torch.as_tensor(X).float()
+    X8, s = _quantise_f32(X, X.abs().amax(1, keepdim=True))
+    return X8, s.reshape(-1)
+
+
+def pack_weight_f32(W):
+    """mac_pack_weight_fp8 of fp32 W [K, n_out] ([in, out]): (W8 [K, n_out] fp64 e4m3 values, sW [n_out] fp32)."""
+    W = torch.as_tensor(W).float()
+    W8, s = _quantise_f32(W, W.abs().amax(0, keepdim=True))
+    return W8, s.reshape(-1)
+
+
+def a8_f32(P8, y, N):
+    """The read step's GEMM 1 operand, A8 = e4m3(P8 * fp32(y_b * fp32(1 / ay_b))), ay_b = max|y_b| (1 / ay_b = 0 for an
+    all-zero y_b), from the e4m3 values P8 [B*N, d] and fp32 y [B, d]: fp64 [B*N, d]."""
+    y = torch.as_tensor(y).float()
+    ay = y.abs().amax(1, keepdim=True)
+    nz = ay > 0
+    iay = torch.where(nz, torch.ones_like(ay) / torch.where(nz, ay, torch.ones_like(ay)), torch.zeros_like(ay))
+    ys = (y * iay.expand_as(y).contiguous()).repeat_interleave(N, 0)
+    return e4m3(torch.as_tensor(P8).float() * ys)
 
 
 def invariant(KB, Wx, bx, Wm, bm):

@@ -13,7 +13,7 @@ A window that is all zero has sA = 0, zero bytes and y = act(b).
 import numpy as np
 import torch
 
-from oracle.fp8_read_oracle import E4M3_MAX, e4m3
+from oracle.fp8_read_oracle import E4M3_MAX, e4m3, pack_weight_f32
 
 
 def im2col3x3(x):
@@ -46,11 +46,7 @@ def quant_patches(x):
 
 def pack_weight(W):
     """(W8 [K, n_out] fp64 e4m3 values, sW [n_out] fp32) as mac_pack_weight_fp8 computes them from fp32 W [K, n_out]."""
-    W = torch.as_tensor(W, dtype=torch.float32)
-    am = W.abs().amax(0)
-    s = am / torch.full_like(am, E4M3_MAX)
-    q = torch.where(am > 0, W / torch.where(am > 0, s, torch.ones_like(s)), torch.zeros_like(W))
-    return e4m3(q), s
+    return pack_weight_f32(W)
 
 
 def _act(y, relu):
