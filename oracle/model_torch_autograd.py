@@ -77,7 +77,30 @@ def stem_grads(relu, params, images, keep, uniforms, d_kb):
     return out(kb), {k: out(v.grad) for k, v in p.items()}, out(x.grad)
 
 
-def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="cpu", grad=True, trace=None):
+def stem_graph_for(geometry):
+    """The stem `run` calls for a model with the stem options `geometry`, with the signature of `stem_graph`: a dict as
+    `DPTrainer(stem=(C, layers, geometry))` takes it, of which "strides", "linear" and "location" (with "location_bias"
+    and "location_dim", defaulting as the library's do) select the graph; the kernel sizes are the kernels' own.  The
+    stem's uniforms are the reference's: with location features the first draw covers layer 0's whole input
+    [k, H, W, C + l] (`oracle/stem_geometry.py`, `oracle/stem_location.py`)."""
+    # imported here: oracle/output_options.py imports this module, and these two are only needed with the options
+    from oracle.stem_geometry import stem_torch
+    from oracle.stem_location import stem_loc_torch
+    strides, linear = geometry.get("strides"), bool(geometry.get("linear", False))
+    location = geometry.get("location")
+    if location is not None:
+        location = (location, geometry.get("location_bias", 1.0), geometry.get("location_dim", 32))
+
+    def graph(relu, p, images, keep=1.0, uniforms=None):
+        ps = {k: v for k, v in p.items() if k.startswith("stem/")}
+        if location is not None:
+            return stem_loc_torch(relu, ps, images, location, keep, uniforms, strides)
+        return stem_torch(relu, ps, images, keep, uniforms, strides, linear)
+    return graph
+
+
+def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="cpu", grad=True, trace=None, stem=None,
+        output=None, train=True, moving=None):
     """The training loss of one shard.
 
     `values`: every variable by its TF name (numpy or torch); `data`: "questions" [B, S] (0 = padding),
@@ -93,7 +116,13 @@ def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="c
     `trace`: a list that receives the cell's per-step control, memory, info, "att_question" and "att_kb" (numpy, see
     `mac_torch_autograd.graph`); with it the result also holds the units' outputs the cell reads: "knowledgeBase" (the
     stem's, one per image [k, H*W, d], before the imageIndex gather), "vecQuestions", "questionWords" and
-    "questionCntxWords".  It changes nothing else."""
+    "questionCntxWords".  It changes nothing else.
+
+    `stem`: the stem options (see `stem_graph_for`; None: `stem_graph`, the shipped 3x3 stride-1 stem).  `output`: the
+    output unit's options {"question", "mul", "bn"} (`oracle/output_options.output_graph`; None: `output_graph`, the
+    shipped layout).  `train`: the batch norms' form, of the cell's memoryBN and the output unit's: batch statistics (True)
+    or the stored ones (False, the reference's evaluation).  `moving`: a dict that receives the output unit's stored
+    statistics after a training forward."""
     dev = torch.device(device)
     t64 = lambda a: torch.as_tensor(np.asarray(a) if isinstance(a, np.ndarray) else a).to(dev, torch.float64)
     p = {k: t64(v).requires_grad_(grad and "/BatchNorm/moving_" not in k) for k, v in values.items()}
@@ -109,14 +138,20 @@ def run(cfg, L, values, data, keeps, uniforms=None, global_batch=None, device="c
     B = questions.shape[0]
     words, cntx, vecq = encoder_torch_autograd.graph(p, questions, lengths, keeps["encoder"][0], keeps["encoder"][1],
                                                      its["encoder"])
-    kb = stem_kb = stem_graph(cfg.relu, p, x_img.permute(0, 2, 3, 1) if nchw else x_img, keeps["stem"], its["stem"])
+    stem_fn = stem_graph if stem is None else stem_graph_for(stem)
+    kb = stem_kb = stem_fn(cfg.relu, p, x_img.permute(0, 2, 3, 1) if nchw else x_img, keeps["stem"], its["stem"])
     if data.get("imageIndex") is not None:
         kb = kb[lng(data["imageIndex"])]
     assert kb.shape[0] == B, (kb.shape, B)
     x = {"vecQuestions": vecq, "questionWords": words, "questionCntxWords": cntx, "knowledgeBase": kb}
-    _, memory = mac_torch_autograd.graph(cfg, p, x, lengths, L, keeps["cell"], its["cell"], train=True, trace=trace)
+    _, memory = mac_torch_autograd.graph(cfg, p, x, lengths, L, keeps["cell"], its["cell"], train=train, trace=trace)
     # the cell's vecQuestions is the encoder's output: the output unit reads the same tensor (model.py:512-528)
-    logits, losses = output_graph(cfg.relu, p, memory, vecq, answers, keeps["output"], its["output"])
+    if output is None:
+        logits, losses = output_graph(cfg.relu, p, memory, vecq, answers, keeps["output"], its["output"])
+    else:
+        from oracle.output_options import output_graph as options_graph
+        logits, losses = options_graph(cfg.relu, p, memory, vecq, answers, keeps["output"], its["output"], train=train,
+                                       decay=cfg.bnDecay, moving=moving, **output)
     for u in UNITS:
         assert next(its[u], None) is None, "%s: uniform draws left over: the dropout calls differ from the reference's" % u
     loss = losses.sum() / float(B if global_batch is None else global_batch)
